@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- CacheGen encode+decode throughput of the B200 hot path (BASELINE.json metric).
+"""bench.py -- CacheGen encode+decode throughput of the H100 hot path (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            (driver launches N>1 under torchrun)
   python bench.py --impl reference ...                     CPU arm: the oracle port of the reference's path
@@ -19,7 +19,10 @@ Printed JSON line (rank 0):
                (host->device || decode); the KV starts on the GPU, as it does in vLLM.  All copies are inside the timed
                region.  e2e.raw_upload_variant adds an upload of the raw KV from page-locked host memory before every
                store (the round-1 definition), reported separately because that copy is not part of store().
-  roofline     algorithmic HBM bytes of the dominant kernel / its live event-timed duration vs MEASURED_PEAKS.json.
+  roofline     algorithmic HBM bytes of the dominant kernel / its live event-timed duration vs MEASURED_PEAKS.json, or
+               the H100 SXM data sheet's 3.35 TB/s where that file is absent.
+  --dump-outputs DIR  after the timed steps, what the last one computed: a fixed, seeded sample of the decoded KV and
+               the containers of the last wave, as .npy files in DIR.
   cpu_baseline the CPU oracle (port of the reference path, OpenMP, threads pinned) on a bounded sample of the workload.
   config.entropy_sweep   the same step on data of higher entropy (up to ~4.1 bits/symbol), beside the headline.
 """
@@ -62,6 +65,7 @@ def parse_args():
                     help="container: rans_compact = v3 (default: rANS + symbol counts), rans = v2 (rANS + CDF rows), ac = v1")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed to DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -201,7 +205,7 @@ def run_reference_arm(args):
     if rank != 0:
         return
     n = args.cpu_chunks
-    steps, warmup = max(3, min(args.steps, 5)), max(2, min(args.warmup, 3))
+    steps, warmup = args.steps, args.warmup
     gbs, (med, best), cores = cpu_codec_sample(n, args.chunk, steps, warmup)
     n_all = args.tokens // args.chunk
     sample = (f"{n} of {n_all} chunks ([{L},2,{args.chunk},{H},{D}] bf16 each) per step; median of {steps} steps after "
@@ -497,7 +501,7 @@ def main():
     parity = parity_spot_check(kv, out, cs)
     status_words = codec.decode_status()
 
-    # ---- timed: K steps, device-resident inputs (4 GiB >> 126 MB L2: no reuse between iterations)
+    # ---- timed: K steps, device-resident inputs (4 GiB >> 50 MB L2: no reuse between iterations)
     sampler = ClockSampler(local) if rank == 0 else None
     barrier()
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -508,6 +512,9 @@ def main():
     barrier()
     ms_total = ev0.elapsed_time(ev1)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        n_waves = sum(1 for _ in waves())
+        dump_outputs(args.dump_outputs, out, stagings[(n_waves - 1) % len(stagings)], stride, list(waves())[-1][1], N)
     from lmcache_b200.dist_util import aggregate_gbps, max_over_ranks
     ms_step = max_over_ranks(ms_total, dev) / args.steps          # device time, max over ranks
     value = aggregate_gbps(raw_bytes, ms_step, world)              # weak scaling: every rank codes its own block
@@ -518,8 +525,8 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except OSError:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 GB/s (of fallback)"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "H100 SXM data sheet, 3.35 TB/s (not measured)"
     alg = {  # algorithmic HBM bytes per step (DESIGN.md section 4): read 2 B/elem + write w, and the reverse
         "absmax": raw_bytes,
         "encode": raw_bytes + container_bytes,
@@ -529,32 +536,12 @@ def main():
                   "achieved_GBps": round(alg[k] / (kern_ms[k] * 1e-3) / 1e9, 1),
                   "frac": round(alg[k] / (kern_ms[k] * 1e-3) / 1e9 / peak, 4)} for k in alg if k in kern_ms}
     dom = max((k for k in ("encode", "decode") if k in kern_ms), key=lambda k: kern_ms[k])
-    # DRAM traffic and instruction counts of one launch come from the COMMITTED ncu --set full capture of this workload
-    # (profiles/r2_traffic.json, made by profiles/traffic.py from the .ncu-rep); they are not measured in this run
-    traffic, traffic_src = None, None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json")))
-        if tj["workload"] == {"tokens": T, "chunk": cs, "data": args.data, "coder": args.coder}:
-            traffic_src = "profiles/r2_traffic.json (committed ncu capture, not measured in this run)"
-            sm_mhz = float((clocks or {}).get("sm_mhz") or peaks.get("sm_max_mhz") or 1965.0)
-            n_smsp = torch.cuda.get_device_properties(dev).multi_processor_count * 4
-            for k in alg:
-                e = tj.get(f"{k}_kernel")
-                if k in rl_all and e:
-                    rl_all[k]["ncu_dram_bytes"] = e["dram_read_bytes"] + e["dram_write_bytes"]
-                    if e.get("warp_inst_executed"):
-                        slots = kern_ms[k] * 1e-3 * sm_mhz * 1e6 * n_smsp
-                        rl_all[k]["issue"] = {"warp_inst": e["warp_inst_executed"], "issue_slots": round(slots),
-                                              "frac": round(e["warp_inst_executed"] / slots, 4),
-                                              "ncu_alu_pipe_pct": e.get("ncu_alu_pipe_pct")}
-            traffic = rl_all[dom].get("ncu_dram_bytes")
-    except (OSError, KeyError, ValueError):
-        pass
+    traffic, traffic_src = None, "not measured"
     roofline = {"kernel": f"{dom}_kernel", "bound": "hbm", "achieved": rl_all[dom]["achieved_GBps"], "peak": peak,
                 "unit": "GB/s", "frac": rl_all[dom]["frac"], "traffic": traffic, "traffic_source": traffic_src,
                 "peak_source": peak_src,
                 "note": "integer coder kernels bound by instruction issue / ALU and shared-memory wavefronts (DESIGN.md "
-                        "section 5), DRAM below 20 % of peak; achieved = algorithmic bytes of a step / summed live "
+                        "section 5); achieved = algorithmic bytes of a step / summed live "
                         "event-timed duration of the kernel's launches in that step",
                 "kernels": rl_all, "other_kernels_ms": {k: round(v, 4) for k, v in kern_ms.items() if k not in alg}}
 
@@ -616,7 +603,7 @@ def main():
                                    "they may sum to slightly more than ms_per_step") if pipelined else "1",
                        "device_scratch_bytes": {"staging": staging_bytes(stride, W, N) * (2 if pipelined else 1), "encode_workspace": int(ws_enc),
                                                                   "decode_workspace": int(ws_dec)},
-                       "l2": "inputs (4 GiB) exceed the 126 MB L2; no flush needed", "parity_spot_check": parity,
+                       "l2": "inputs (4 GiB) exceed the 50 MB L2; no flush needed", "parity_spot_check": parity,
                        "decode_status_words_nonzero": sum(1 for w in status_words if w),
                        "entropy_sweep": sweep},
             "encode_GBps": round(raw_bytes / (sum(kern_ms.get(k, 0) for k in ("absmax", "cdf", "encode", "compact")) * 1e-3) / 1e9, 1),
@@ -627,6 +614,28 @@ def main():
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(path, out, buf, stride, k, N):
+    """What the last timed step computed, as a caller of encode and decode receives it: the decoded KV block and the
+    containers of the step's last wave (the k containers at buf + j * stride).  Fixed, seeded samples keep the files
+    under 64 MB: 8 Mi elements of the decoded KV (float32), 256 Ki bytes of every container (float32, positions drawn
+    over the container's own extent), and every container's size in bytes (float64)."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    g = torch.Generator(device=out.device).manual_seed(20240611)
+    flat = out.view(-1)
+    idx = torch.randint(0, flat.numel(), (8 << 20,), device=out.device, generator=g)
+    np.save(os.path.join(path, "decoded_kv_sample.npy"), flat[idx].float().cpu().numpy())
+    heads = buf[:k * stride].view(k, stride)[:, :N.HEADER_BYTES].cpu().numpy()
+    sizes = [N.Header.from_buffer_copy(heads[j].tobytes()).total_bytes for j in range(k)]
+    sample = []
+    for j, n in enumerate(sizes):
+        pos = torch.randint(0, n, (256 << 10,), device=buf.device, generator=g) + j * stride
+        sample.append(buf[pos].float().cpu().numpy())
+    np.save(os.path.join(path, "container_sizes.npy"), np.asarray(sizes, np.float64))
+    np.save(os.path.join(path, "container_bytes_sample.npy"), np.stack(sample))
 
 
 def staging_bytes(stride, W, N):
@@ -681,7 +690,7 @@ def run_e2e(args, kv, dev, world, rank, barrier):
     host_bytes = backend.host_bytes()
     cont_bytes = sum(e.nbytes for e in backend.dict.values() if e.blk is not None)
     barrier()
-    steps = max(2, min(args.steps, 3))
+    steps = args.steps
     t0 = time.perf_counter()
     parts = [one_step() for _ in range(steps)]
     barrier()

@@ -15,8 +15,8 @@ outside the GIL), which speaks the reference's wire protocol (lmcache/protocol.p
 
 One JSON line on rank 0: aggregate store / retrieve GB/s of raw bf16 KV, per-sequence retrieve latency percentiles, the wire
 bytes, and ttft_saved_ms_p50 = t_prefill - t_retrieve(p50), with t_prefill a STATED model constant (no LLM is run,
-SURVEY.md 8d): 2 * 6.74e9 FLOPs per token for the 7B weights plus causal attention, at 60 % of the measured sustained bf16
-peak of this GPU pool (MEASURED_PEAKS.json)."""
+SURVEY.md 8d): 2 * 6.74e9 FLOPs per token for the 7B weights plus causal attention, at 60 % of the sustained bf16 peak in
+MEASURED_PEAKS.json, or of the H100 SXM data sheet's dense bf16 rate (989 TFLOP/s) where that file is absent."""
 import ctypes
 import json
 import os
@@ -35,7 +35,7 @@ def prefill_ms(tokens: int) -> float:
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except OSError:
         pass
-    tflops = 0.6 * float(peaks.get("bf16_tflops_sustained", 1400.0))
+    tflops = 0.6 * float(peaks.get("bf16_tflops_sustained", 989.0))
     flops = 2.0 * 6.74e9 * tokens + 2.0 * L * tokens * tokens * C        # weights + causal QK^T/PV (4 L T^2 C / 2)
     return flops / (tflops * 1e12) * 1e3
 

@@ -1,5 +1,5 @@
 /*
- * b200kv.h -- C ABI of libb200kv.so, the B200 (sm_100a) KV-cache store/load hot path.
+ * b200kv.h -- C ABI of libb200kv.so, the H100 (sm_90a) KV-cache store/load hot path.
  *
  * This is the drop-in boundary for ONE path of LMCache v0.1.2 (paths below are relative to the
  * reference tree): CacheGen encode / decode, the chunked token-id SHA-256 prefix hash, and the
@@ -42,8 +42,8 @@ extern "C" {
                                      * headline entropy), the int32 stream length by one byte */
 #define B200KV_CONTAINER_VERSION(coder) ((coder) + 1) /* "B2KV" wire container version (b200kv_header.version) */
 #define B200KV_ENCODE_HINT_HIGH_ENTROPY 0x100 /* OR into `coder` of b200kv_encode_chunks: the caller expects more than ~2.7
-                                               * payload bits per symbol (e.g. the previous call's sizes said so); selects the
-                                               * TMA-staged encode kernel whose time does not grow with entropy.  Output bytes
+                                               * payload bits per symbol (e.g. the previous call's sizes said so); the
+                                               * compaction kernel then keeps its full-size shared-memory stage.  Output bytes
                                                * are identical either way. */
 #define B200KV_ENCODE_HINT_MID_ENTROPY 0x200  /* likewise: more than ~1.2 payload bits per symbol expected -- the compaction
                                                * kernel then keeps its full-size shared-memory stage (tiles of 10+ KB) */
@@ -185,7 +185,7 @@ int b200kv_sha256_chain(const void* tokens, int32_t elem_size, const int64_t* se
                         int32_t chunk_size, void* digests, void* stream);
 /* Same, and digest k is announced as soon as it exists: ready[k] (DEVICE-visible uint32 array, one word per digest slot,
  * normally mapped host memory like `digests`; or NULL) is set to `epoch` after digest k has been made visible system-wide.
- * A chain is serial -- 38 us per 256-token chunk -- so a host thread that polls ready[] can look up and move the first
+ * A chain is serial -- one 256-token chunk after another -- so a host thread that polls ready[] can look up and move the first
  * chunks while the later ones are still being hashed (LMCacheEngine.store / retrieve do).  The digests must be 4-byte
  * aligned. */
 int b200kv_sha256_chain_ready(const void* tokens, int32_t elem_size, const int64_t* seq_offsets, int32_t n_seq,

@@ -162,7 +162,7 @@ def require_cuda() -> None:
         _cuda_ok = n > 0
         if not _cuda_ok:
             _cuda_ok = None
-            raise RuntimeError(f"lmcache_b200 needs a CUDA device (sm_100a); none usable: {last_error() or 'count=0'}. "
+            raise RuntimeError(f"lmcache_b200 needs a CUDA device (sm_90a); none usable: {last_error() or 'count=0'}. "
                                f"There is no CPU fallback.")
 
 

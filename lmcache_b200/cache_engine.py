@@ -31,7 +31,7 @@ logger = init_logger(__name__)
 
 class LazySeq:
     """A read-only sequence whose items are computed on access: fn(base[i]).  Slices stay lazy.  The engine passes its
-    chunk keys around in this form: item i only exists once the hash chain has reached chunk i (38 us per chunk), and a
+    chunk keys around in this form: item i only exists once the hash chain has reached chunk i (one chunk after another), and a
     consumer that walks the sequence front to back -- look up / fetch / encode wave by wave -- overlaps with the chain
     instead of waiting for its end."""
 
@@ -136,7 +136,7 @@ class _HashRun:
 
 def sha256_prefix_chain_lazy(tokens: torch.Tensor, chunk_size: int, seq_offsets: Optional[List[int]] = None) -> LazySeq:
     """sha256_prefix_chain without waiting for the end of the chain: returns at once with a lazy sequence of hex digests;
-    digest i becomes available ~38 us x (i + 1) after the launch (one 256-token chunk of int64 ids)."""
+    digest i becomes available once the chain has hashed chunks 0..i."""
     N.require_cuda()
     if tokens.dim() != 1:
         raise ValueError(f"Invalid shape of tokens: {tokens.shape}")
@@ -277,7 +277,7 @@ class LMCacheEngine:
             view = KvView.from_tuple(kv_cuda, fmt)
             self._geom = (view.L, view.H, view.D, view.dtype)
             if self._fast_path():
-                # B200-native path: the backend consumes the caller's 2L tensors directly (batched encode / one gather)
+                # native path: the backend consumes the caller's 2L tensors directly (batched encode / one gather)
                 end_make_chunks = time.perf_counter()
                 n_chunks = self.engine_.put_kv_chunks(keys, view, start_chunk_idx * self.chunk_size, self.chunk_size,
                                                       blocking=blocking)
@@ -432,7 +432,7 @@ class LMCacheEngine:
             ret_mask[got:] = False
         return ret_mask
 
-    # ------------------------------------------------------------------ B200-native fast paths
+    # ------------------------------------------------------------------ native fast paths
     def _fast_path(self) -> bool:
         f = getattr(self.engine_, "supports_kv_view", None)
         return bool(f and f())

@@ -1,4 +1,4 @@
-// codec.cu -- CacheGen encode / decode kernels for sm_100a and their C-ABI entry points.
+// codec.cu -- CacheGen encode / decode kernels for sm_90a and their C-ABI entry points.
 //
 // Replaces (reference paths relative to the LMCache v0.1.2 tree):
 //   encode: lmcache/storage_backend/serde/cachegen_encoder.py:266-325 (encode_function) incl. the three
@@ -140,8 +140,8 @@ __device__ __forceinline__ int64_t tok_row(const int64_t* slot_map, int64_t tok)
 // (cachegen_encoder.py:54-55).  |x| ordering == integer ordering of (bits & 0x7fff); a NaN in the row
 // wins (pattern above inf), like torch.amax.  One warp per row, 128-bit loads when alignment allows.
 // Round 2 tried to hide this kernel -- the only HBM-bound one of the path -- under the instruction-bound coding kernels of
-// the previous wave (second stream, 128-thread blocks with <= 32 registers so that a block fits next to them): no gain
-// (8.31 -> 8.28 ms per step).  Both coder kernels fill the SM's shared memory with their own CTAs (7 x 32.5 KB, 12 x 18.6
+// the previous wave (second stream, 128-thread blocks with <= 32 registers so that a block fits next to them): no gain.
+// Both coder kernels fill the SM's shared memory with their own CTAs (7 x 32.5 KB, 12 x 18.6
 // KB incl. the 1 KB the system reserves per CTA), so not even a block without shared memory finds room; the kernels only
 // overlap at their tails.  Measured, rejected.
 template <bool VEC, bool PAGED>
@@ -414,8 +414,8 @@ __global__ void __launch_bounds__(CT, FUSED ? 7 : 4) encode_kernel(EncParams P) 
                 } else {
                     // token tk + k is one row further than token tk + k - 1: ONE IMAD.WIDE.U32 per address (row
                     // pitch x 2, the 2 from a register ptxas cannot fold, added to the previous address) instead of the
-                    // 64-bit add chains the compiler builds from the pointer arithmetic (4.6 -> 2 instructions per load,
-                    // ncu round 2).  The chain of twelve is off the critical path: the batch is a prefetch.
+                    // 64-bit add chains the compiler builds from the pointer arithmetic (fewer than
+                    // half the instructions per load).  The chain of twelve is off the critical path: the batch is a prefetch.
                     const uint16_t* q = src + (int64_t)tk * s1;
                     if (tk + BT <= gt) {
 #pragma unroll
@@ -753,7 +753,7 @@ __global__ void __launch_bounds__(CT, 7) encode_tma_kernel(EncParams P) {
 #pragma unroll
         for (int i = 0; i < 32; ++i) mask |= (cnt[i] != 0u ? 1u : 0u) << i;
         // this kernel is picked for high-entropy data, where every symbol is in use somewhere in the warp: no skipping
-        // of unused symbols here (the tests cost more than they save: 5.23 -> 5.48 ms at 4.1 bits per symbol, measured)
+        // of unused symbols here (the tests cost more than they save at 4.1 bits per symbol, measured)
         const uint32_t wany = 0xffffffffu;
         if (P.compact) {
             uint32_t w0, w1;
@@ -1422,8 +1422,8 @@ __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
             // streams themselves are short and neighbours share cache lines) each count is one byte load at a position
             // that depends on the mask alone -- branch-free; when a quarter of the lanes or more have long headers, the
             // header is pulled into registers with aligned word loads, only as many as it is long, and consumed a byte
-            // at a time (scattered byte loads would cost a cache-line access each).  Measured, whole kernel: 3.29 / 4.64
-            // ms (byte loads only) vs 3.40 / 3.95 ms (registers only) at 0.6 / 4.1 payload bits per symbol.
+            // at a time (scattered byte loads would cost a cache-line access each): byte loads alone are slower at high
+            // entropy, registers alone at low entropy (measured, whole kernel, at 0.6 / 4.1 payload bits per symbol).
             const int nb = 2 * ((int)cq + 1);
             const uint32_t mbytes = (uint32_t)hdr_mask_bytes(nb);
             const uint8_t* sp = dc.base + my_off;
@@ -1794,12 +1794,11 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
         else { if (paged) B2_LAUNCH_ENC(FUSED, 1, true, SMEM); else B2_LAUNCH_ENC(FUSED, 1, false, SMEM); } \
     } while (0)
     // TMA-staged kernel (encode_tma_kernel): rANS, fused mode, tiles of exactly CT channels that are contiguous in every
-    // token row and 16-byte aligned.  B200KV_ENCODE_PATH=legacy forces the kernel above (A/B measurements).
-    // Measured (profiles/r2_encode_variants.json): the TMA-staged kernel is flat in the data's entropy (4.4 .. 5.2 ms per
-    // 8192-token block), the register-staged one is faster below ~2.7 payload bits per symbol (3.75 ms at 0.6) and slower
-    // above (6.2 ms at 4.1): the caller says which regime it expects (B200KV_ENCODE_HINT_HIGH_ENTROPY, e.g. from the
-    // sizes of the previous call).  B200KV_ENCODE_PATH=legacy|tma overrides (A/B measurements).
-    bool tma = hint_tma;
+    // token row and 16-byte aligned; the output bytes are the same.  Measured on an H100 SXM (700 W), 8192-token block:
+    // the register-staged kernel above is as fast at 0.6 payload bits per symbol and faster above it (10.3 vs 11.0 ms at
+    // 3.2 coder bits per symbol, 13.0 vs 13.6 ms at 4.1), so no entropy hint selects this kernel here.
+    // B200KV_ENCODE_PATH=tma selects it (A/B measurements).
+    bool tma = false;
     if (const char* e = getenv("B200KV_ENCODE_PATH")) tma = e[0] == 't';
     tma = tma && fused && coder == CODER_RANS && P.C % CT == 0 && (kv->sH == kv->D || kv->D % CT == 0) &&
           kv->sT % 8 == 0 && kv->sH % 8 == 0;
@@ -1846,7 +1845,7 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
         // a few dozen bytes long -- oversized tiles take the direct path inside the kernel
         P.stage_bytes = coder == CODER_RANS ? CT * (TEMPW_FUSED_RANS * 4 + 4) + 32 : CT * TEMPW_FUSED * 4 + 32;
         // The kernel waits on sparse row reads: more resident CTAs hide more of that latency.  Without an entropy hint a
-        // tile's streams total a few KB, so a 12 KB stage (12 CTAs per SM instead of 9: 0.41 -> 0.31 ms per block) covers
+        // tile's streams total a few KB, so a 12 KB stage (12 CTAs per SM instead of 9: measured faster) covers
         // them; the rare larger tile takes the kernel's direct path.  B200KV_COMPACT_STAGE=<bytes> overrides (knob).
         if (coder == CODER_RANS && !hint_tma && !hint_mid) P.stage_bytes = 12 * 1024;
         if (const char* e = getenv("B200KV_COMPACT_STAGE")) {
@@ -1899,7 +1898,7 @@ int b200kv_decode_chunks(const void* containers, int64_t containers_bytes, const
     const int64_t tiles_max = Gmax * 2 * P.L * P.tpp;
     B2_REQUIRE(tiles_max < (1ll << 31) && n_chunks <= 65535, "too many tiles / chunks in one call");
     // table layout of the rANS decoder: the conflict-free (transposed) one pays off above ~3.6 payload bits per symbol
-    // (measured: 3.28 / 3.60 ms at 0.6 bits, 4.04 / 3.72 ms at 4.1 bits, row-major / transposed); the containers say how
+    // (measured: row-major is faster at 0.6 bits, transposed at 4.1 bits); the containers say how
     // many bits they hold.  B200KV_DECODE_TABLE=rows|transposed overrides (measurement knob).
     bool transposed = false;
     {

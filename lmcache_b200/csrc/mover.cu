@@ -90,7 +90,10 @@ static int launch_pack(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, i
     const int V = vec ? 8 : 1;
     const int64_t total = ((int64_t)(n_chunks - 1) * chunk_tokens + last_chunk_tokens) * 2 * kv->L * kv->H * (kv->D / V);
     int64_t blocks = (total + 255) / 256;
-    const int64_t cap = 148ll * 8 * 4;   // a few waves of 148 SMs x 8 CTAs; grid-stride covers the rest
+    int dev = 0, sms = 0;
+    B2_CHECK_CUDA(cudaGetDevice(&dev));
+    B2_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const int64_t cap = (int64_t)sms * 8 * 4;   // a few waves of SMs x 8 CTAs; grid-stride covers the rest
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
     if (pack) {

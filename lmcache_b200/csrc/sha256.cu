@@ -120,12 +120,12 @@ __global__ void __launch_bounds__(128) sha256_expand_kernel(ShaParams P) {
 //   FMA_ADDS = false (default): the additions are IADD3s on the same pipe (4 more): pipe floor 28 cycles per round.
 //   FMA_ADDS = true : every addition is x * 1 + y with a multiplier the compiler cannot see through (IMAD, FMA pipe, one
 //                     warp instruction per cycle): 20 cycles of ALU pipe + 6 of FMA pipe, overlappable on paper.
-// The recurrence e -> Sigma1 -> t1 -> e' is SHF -> LOP3 -> add -> add, ~18 cycles of latency.  Measured (round 2, 8192
-// tokens = 1057 blocks in one chain): 1.225 ms with IADD3s (37 cycles per round), 1.345 ms with IMADs -- six two-input
+// The recurrence e -> Sigma1 -> t1 -> e' is SHF -> LOP3 -> add -> add, ~18 cycles of latency.  Measured (8192 tokens =
+// 1057 blocks in one chain): IADD3s are faster than IMADs -- six two-input
 // IMADs form a longer dependency chain than two three-input IADD3s, and one warp is bound by that chain, not by pipe
 // throughput.  The same lesson as the attempt to move half of the ROTATIONS to the FMA pipe (x * 2^(32-n) as a 64-bit
-// product, halves summed): 1.74 ms.  A third variant moves only h + (W + K) -- known three rounds ahead, off every chain --
-// to the FMA pipe (13 ALU instructions per round instead of 14): 1.231 ms, no gain either.
+// product, halves summed): slower still.  A third variant moves only h + (W + K) -- known three rounds ahead, off every chain --
+// to the FMA pipe (13 ALU instructions per round instead of 14): no gain either.
 // B200KV_SHA_ADDS=alu|hwk|fma picks the variant (measurement knob, default alu).
 template <bool FMA_ADDS>
 __device__ __forceinline__ uint32_t sha_add(uint32_t x, uint32_t y, uint32_t one) {
@@ -206,8 +206,8 @@ constexpr int kShaStages = 3;
 
 // One thread per sequence (chain).  The precomputed (W + K) blocks of a chunk are streamed through a three-stage ring in
 // shared memory with per-thread cp.async groups: block k + 2 is in flight while block k is consumed, so the chain never
-// waits for L2 / DRAM (round 1 kept the next block in registers; the compiler sank those loads to the point where the
-// registers became free, 70 % into the loop body, and a sixth of the cycles went to waiting for them -- ncu, round 2).
+// waits for L2 / DRAM (an earlier version kept the next block in registers; the compiler sank those loads to the point where
+// the registers became free, late in the loop body, and the chain waited for them).
 // The ring is lane-interleaved at 16-byte granularity: a warp's LDS.128 of "its" i-th group is one conflict-free request.
 template <int FMA_ADDS>
 __global__ void __launch_bounds__(32) sha256_chain_kernel(ShaParams P) {
@@ -344,8 +344,8 @@ extern "C" int b200kv_sha256_chain_ready(const void* tokens, int32_t elem_size, 
     const size_t tab_pad = (tab_bytes + 255) & ~(size_t)255;
     // Scratch comes from a grow-only per-device buffer owned by the library, not from cudaMallocAsync: the default memory
     // pool hands its memory back to the driver at every synchronisation point (release threshold 0), so a per-call pool
-    // allocation turned into a real allocation -- 3 to 90 ms once the process has gigabytes of mapped page-locked memory
-    // (measured, round 2) -- on the critical path of every store() and retrieve().  Calls are ordered through an event, so
+    // allocation turned into a real allocation -- milliseconds or more once the process has gigabytes of mapped page-locked
+    // memory -- on the critical path of every store() and retrieve().  Calls are ordered through an event, so
     // two streams can share the buffer.
     static std::mutex mu;
     static uint8_t* g_buf[64] = {nullptr};

@@ -1,7 +1,7 @@
 """Connector factory (lmcache/storage_backend/connector/__init__.py:28-102).  Only the transport the
 north-star deployment uses is provided here: `lm://host:port` (one lmcache.server over host sockets).  Both clients speak
 the same wire protocol and both send from / receive into page-locked slabs without copies: `lm://` is the Python-socket
-client (measured faster per connection on the B200 host, profiles/r1_extra_measurements.json), `lmn://` the client of the
+client, `lmn://` the client of the
 native library (csrc/lmnet.cu).
 `redis://` needs the external redis client and is outside the rebuilt hot path."""
 import re

@@ -355,7 +355,7 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         self._retired = keep
 
     def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True) -> int:
-        # `keys` may be lazy (the engine's hash chain produces key i ~38 us x (i + 1) after its launch): the encode waves
+        # `keys` may be lazy (the engine's hash chain produces key i after keys 0..i-1): the encode waves
         # need no keys, so they are enqueued first; the entries are published as their keys arrive.  Readers wait on `ready`.
         entries = [_CEntry() for _ in range(len(keys))]
         job = self._pipe.submit(view, tok_begin, chunk_size, entries)

@@ -9,7 +9,7 @@ Engine fast paths (CacheGen serde + a connector with get_into), both pipelined a
   get   the containers of all requested chunks are fetched by k connections into the slab while the main thread uploads
         and decodes the waves that are already complete (network || H2D || decode: what remote_backend.py:183-275 does
         with a network thread and a deserialize thread, here also on the engine's one-blob path).
-LMCACHE_B200_REMOTE_CONNS sets k (default 4; one TCP stream tops out at 2-4 GB/s)."""
+LMCACHE_B200_REMOTE_CONNS sets k (default 4; one TCP stream is slower than the GPU side)."""
 import os
 import queue
 import threading

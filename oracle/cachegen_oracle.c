@@ -5,14 +5,14 @@
  * file; only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl
  * reference legs use it, and only as the checker / the timed CPU baseline.
  *
- * Each function cites the reference file:line (relative to /root/reference) it follows.
+ * Each function cites the reference file:line (relative to the reference tree) it follows.
  *
  * Parity status
  *   quantise / dequantise / CDF / SHA-256 chain : PINNED against golden vectors generated
  *       from the reference's own functions (tests/golden/make_golden.py).
  *   arithmetic-coder bitstream                  : "parity unpinned" -- the coder lives in
  *       the un-vendored PyPI wheel `torchac_cuda >= 0.2.5` (setup.py:19), absent from
- *       /root/reference.  This file restates the published torchac-lineage algorithm
+ *       the reference tree.  This file restates the published torchac-lineage algorithm
  *       (32-bit low/high, 16-bit CDF precision, E1/E2/E3 renormalisation with pending
  *       bits, MSB-first packing; SURVEY.md Appendix A.3/A.4) and anchors it on the
  *       reference call sites cachegen_encoder.py:241-262,301-316 and

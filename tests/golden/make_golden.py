@@ -1,13 +1,13 @@
 """Generate golden vectors by importing the *reference's own* functions (CPU, this container).
 
-Run once in the build container (needs /root/reference; the GPU box never runs this):
+Run once on a CPU machine with a checkout of the reference (GPU test runs only read the outputs):
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py <path of an LMCache v0.1.2 tree>
 
 Outputs (committed): tests/golden/golden_codec.npz, tests/golden/golden_hash.json,
 tests/golden/golden_engine.json.
 
-What is pinned, and by which reference code (paths relative to /root/reference):
+What is pinned, and by which reference code (paths relative to the reference tree):
   * quantise           lmcache/storage_backend/serde/cachegen_encoder.py:40-61  torch_quant_vectorized
                        + _split_kv :76-91 and the K/V concat :284-285
   * dequantise + cast  lmcache/storage_backend/serde/cachegen_decoder.py:24-35 do_dequantize
@@ -25,7 +25,7 @@ import os
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path[:0] = [os.path.join(HERE, "..", "_refstubs"), "/root/reference"]
+sys.path[:0] = [os.path.join(HERE, "..", "_refstubs"), sys.argv[1]]
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402

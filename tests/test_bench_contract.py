@@ -40,7 +40,7 @@ def test_reference_arm_other_ranks_are_silent():
 
 
 def test_committed_gpu_line_has_the_contract_objects():
-    d = json.loads(open(os.path.join(ROOT, "profiles", "r2_final_bench.json")).read().strip().splitlines()[-1])
+    d = json.loads(open(os.path.join(ROOT, "profiles", "h100_bench.json")).read().strip().splitlines()[-1])
     assert REQUIRED <= set(d) and {"roofline", "clocks", "gpu_launches"} <= set(d)
     rl = d["roofline"]
     assert {"bound", "achieved", "peak", "unit", "frac", "traffic"} <= set(rl) and rl["bound"] == "hbm"

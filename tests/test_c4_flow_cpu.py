@@ -2,13 +2,15 @@
 process -- at the level that needs no GPU: token ids -> SHA-256 chain -> engine key strings -> B2KV containers over the
 wire -> header checks -> decode, with the CPU oracle standing in for the kernels on both sides;
 (2) wire interoperability with the REFERENCE's own server and client (lmcache/server/__main__.py:29-104,
-lmcache/storage_backend/connector/lm_connector.py:15-84), run from /root/reference with the import stubs of
-tests/_refstubs -- skipped where the reference tree is absent (the GPU box)."""
+lmcache/storage_backend/connector/lm_connector.py:15-84), through the byte exchange of a session between the two
+recorded by tests/golden/make_lm_wire.py (tests/golden/golden_lm_wire.npz)."""
 import ctypes
+import json
 import os
 import socket
 import subprocess
 import sys
+import threading
 import time
 
 import numpy as np
@@ -16,7 +18,6 @@ import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = "/root/reference"
 
 
 def _free_port():
@@ -116,74 +117,105 @@ def test_c4_flow_two_processes_one_server(coder, server_kind, tmp_path):
         srv.wait()
 
 
-needs_ref = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "lmcache")), reason="reference tree not present (GPU box)")
+def _recv_exact(s, n):
+    buf = bytearray()
+    while len(buf) < n:
+        d = s.recv(min(n - len(buf), 1 << 20))
+        if not d:
+            break
+        buf.extend(d)
+    return bytes(buf)
 
 
-@needs_ref
+def _wire():
+    """the recorded session: calls (op, key, value or expected answer) and per call (client bytes, server bytes)"""
+    z = np.load(os.path.join(HERE, "golden", "golden_lm_wire.npz"))
+    calls = json.loads(z["calls"].tobytes().decode())
+    return calls, [(z[f"c2s_{i}"].tobytes(), z[f"s2c_{i}"].tobytes()) for i in range(len(calls))]
+
+
+class _RecordedServer:
+    """plays the reference server's side of the recorded session to one connection: reads each request, which must be
+    the reference client's bytes, and answers with the reference server's bytes"""
+
+    def __init__(self, segs):
+        self.sock = socket.create_server(("127.0.0.1", 0))
+        self.port = self.sock.getsockname()[1]
+        self.segs, self.done, self.errors = segs, 0, []
+        self.thread = threading.Thread(target=self._run, daemon=True)
+        self.thread.start()
+
+    def _run(self):
+        conn, _ = self.sock.accept()
+        with conn:
+            for i, (c2s, s2c) in enumerate(self.segs):
+                got = _recv_exact(conn, len(c2s))
+                if got != c2s:
+                    self.errors.append(f"call {i}: request differs from the reference client's ({len(got)} B, first "
+                                       f"difference at {next((k for k, (a, b) in enumerate(zip(got, c2s)) if a != b), min(len(got), len(c2s)))})")
+                    return
+                conn.sendall(s2c)
+                self.done += 1
+
+    def close(self):
+        self.thread.join(timeout=30)
+        self.sock.close()
+
+
 @pytest.mark.parametrize("scheme", ["lm", "lmn"])
 def test_our_clients_against_the_reference_server(scheme):
-    """python -m lmcache.server from /root/reference, driven by this package's two lm:// clients"""
+    """this package's two lm:// clients in the recorded session against the reference server's recorded answers: every
+    request byte-identical to the reference client's, every answer read as the reference client read it"""
     from lmcache_b200.storage_backend.connector import CreateConnector
-    port = _free_port()
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([os.path.join(HERE, "_refstubs"), REF]))
-    srv = subprocess.Popen([sys.executable, "-m", "lmcache.server", "127.0.0.1", str(port)], env=env, cwd="/tmp",
-                           stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
+    calls, segs = _wire()
+    srv = _RecordedServer(segs)
     try:
-        assert _wait_port(port, srv), "reference server did not start"
-        c = CreateConnector(f"{scheme}://127.0.0.1:{port}")
-        rng = np.random.default_rng(5)
-        blobs = {f"vllm@lmsys/longchat-7b-16k@2@0@{i:064x}": rng.integers(0, 256, n, dtype=np.uint8).tobytes()
-                 for i, n in enumerate([1, 157, 65536, 2 * 1024 * 1024 + 3])}
-        for k, v in blobs.items():
-            c.set(k, v)
-        for k, v in blobs.items():
-            for _ in range(400):
-                if c.exists(k):
-                    break
-                time.sleep(0.005)
-            assert c.exists(k)
-            assert bytes(c.get(k)) == v
-            buf = np.zeros(len(v) + 64, np.uint8)
-            assert c.get_into(k, buf.ctypes.data, buf.size) == len(v) and buf[:len(v)].tobytes() == v
-        assert not c.exists("vllm@m@1@0@" + "f" * 64) and c.get("vllm@m@1@0@" + "f" * 64) is None
-        assert sorted(c.list()) == sorted(blobs)
+        c = CreateConnector(f"{scheme}://127.0.0.1:{srv.port}")
+        seen = set()
+        for call in calls:
+            op, k = call["op"], call["key"]
+            if op == "set":
+                c.set(k, bytes([call["byte"]]) * call["size"])
+            elif op == "exists":
+                assert c.exists(k) == call["want"]
+            elif op == "get":
+                want = None if call["want"] is None else bytes([call["want"]["byte"]]) * call["want"]["size"]
+                if want is None or k in seen:          # the second GET of a key goes through get_into
+                    got = c.get(k)
+                    assert (got is None) if want is None else bytes(got) == want
+                else:
+                    buf = np.zeros(len(want) + 64, np.uint8)
+                    assert c.get_into(k, buf.ctypes.data, buf.size) == len(want) and buf[:len(want)].tobytes() == want
+                    seen.add(k)
+            else:
+                assert sorted(c.list()) == sorted(call["want"])
         c.close()
     finally:
-        srv.terminate()
-        srv.wait()
+        srv.close()
+    assert not srv.errors, srv.errors
+    assert srv.done == len(segs)
 
 
-@needs_ref
 def test_reference_client_against_our_native_server():
-    """the reference's LMCServerConnector (imported from /root/reference in a subprocess) against csrc/lmnet.cu's server"""
+    """the reference client's recorded requests sent to csrc/lmnet.cu's server: every answer byte-identical to the
+    reference server's (LIST: the same keys, in any order)"""
     import __graft_entry__ as ge
     ge.build_cuda()
     from lmcache_b200 import _native as N
+    calls, segs = _wire()
     lib = N.lib()
     h = ctypes.c_void_p()
     N.check(lib.b200kv_lm_server_start(b"127.0.0.1", 0, ctypes.byref(h)))
-    port = lib.b200kv_lm_server_port(h)
-    code = f'''
-import sys, time
-sys.path[:0] = [{os.path.join(HERE, "_refstubs")!r}, {REF!r}]
-from lmcache.storage_backend.connector.lm_connector import LMCServerConnector
-c = LMCServerConnector("127.0.0.1", {port})
-blobs = {{"vllm@a/b@1@0@" + "%064x" % i: bytes([i]) * n for i, n in enumerate([1, 158, 70000, 1 << 21])}}
-for k, v in blobs.items():
-    c.set(k, v)
-for k, v in blobs.items():
-    for _ in range(400):
-        if c.exists(k): break
-        time.sleep(0.005)
-    assert c.exists(k) and bytes(c.get(k)) == v, k
-assert not c.exists("nope@x@1@0@00") and c.get("nope@x@1@0@00") is None
-assert sorted(c.list()) == sorted(blobs)
-c.close()
-print("ok")
-'''
     try:
-        r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=120, cwd="/tmp")
-        assert r.returncode == 0 and r.stdout.strip().endswith("ok"), r.stderr[-3000:]
+        s = socket.create_connection(("127.0.0.1", lib.b200kv_lm_server_port(h)))
+        for i, (call, (c2s, s2c)) in enumerate(zip(calls, segs)):
+            s.sendall(c2s)
+            got = _recv_exact(s, len(s2c))
+            if call["op"] == "list":
+                assert got[:8] == s2c[:8] and sorted(got[8:].split(b"\n")) == sorted(s2c[8:].split(b"\n")), i
+            else:
+                assert got == s2c, (i, call["op"])
+        s.close()
         assert lib.b200kv_lm_server_num_keys(h) == 4
     finally:
         N.check(lib.b200kv_lm_server_stop(h))

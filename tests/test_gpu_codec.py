@@ -21,7 +21,7 @@ def _tensor_bits(t: torch.Tensor) -> np.ndarray:
 
 
 def _eq_nan(a: np.ndarray, b: np.ndarray, dt: int) -> bool:
-    """bit equality, except that any NaN matches any NaN (payloads differ between x86 and sm_100)."""
+    """bit equality, except that any NaN matches any NaN (payloads differ between x86 and the GPU)."""
     if np.array_equal(a, b):
         return True
     f = (lambda u: (u.astype(np.uint32) << 16).view(np.float32)) if dt == 0 else (lambda u: u.view(np.float16))

@@ -179,7 +179,7 @@ def test_retrieve_device(backend, src_device, autorelease):
 
 @pytest.fixture(params=["fast", "generic"])
 def engine_path(request, monkeypatch):
-    """Run engine tests through both code paths: the B200-native fast path (backend consumes the caller's KV tensors /
+    """Run engine tests through both code paths: the native fast path (backend consumes the caller's KV tensors /
     fills one blob) and the generic per-chunk plugin path every third-party backend would take."""
     if request.param == "generic":
         from lmcache_b200.storage_backend.local_backend import LMCLocalBackend
