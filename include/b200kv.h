@@ -41,12 +41,10 @@ extern "C" {
                                      * is a function of, carried sparsely in front of the stream's rANS bytes (~5 B at the
                                      * headline entropy), the int32 stream length by one byte */
 #define B200KV_CONTAINER_VERSION(coder) ((coder) + 1) /* "B2KV" wire container version (b200kv_header.version) */
-#define B200KV_ENCODE_HINT_HIGH_ENTROPY 0x100 /* OR into `coder` of b200kv_encode_chunks: the caller expects more than ~2.7
+#define B200KV_ENCODE_HINT_MID_ENTROPY 0x200  /* OR into `coder` of b200kv_encode_chunks: the caller expects more than ~1.2
                                                * payload bits per symbol (e.g. the previous call's sizes said so); the
-                                               * compaction kernel then keeps its full-size shared-memory stage.  Output bytes
-                                               * are identical either way. */
-#define B200KV_ENCODE_HINT_MID_ENTROPY 0x200  /* likewise: more than ~1.2 payload bits per symbol expected -- the compaction
-                                               * kernel then keeps its full-size shared-memory stage (tiles of 10+ KB) */
+                                               * compaction kernel then keeps its full-size shared-memory stage (tiles of
+                                               * 10+ KB).  Output bytes are identical either way. */
 #define B200KV_LP 33            /* CDF entries per stream (cachegen_encoder.py:287-289: int(bins.max()) + 1) */
 #define B200KV_GROUP_TOKENS 256 /* CACHEGEN_GPU_MAX_TOKENS_PER_CHUNK (cachegen_basics.py:13) */
 #define B200KV_MAX_PLANES 128   /* 2 * nlayers upper bound */

@@ -22,7 +22,6 @@ CODER_RANS_COMPACT = 2   # container version 3: rANS streams that carry their ow
 ENCODE_HINT_MID_ENTROPY = 0x200    # B200KV_ENCODE_HINT_MID_ENTROPY
 HDR_MAX = 36             # longest version-3 stream header (4 mask bytes + 31 counts + 1 pad)
 CODERS = {"ac": CODER_AC, "rans": CODER_RANS, "rans_compact": CODER_RANS_COMPACT}
-ENCODE_HINT_HIGH_ENTROPY = 0x100   # B200KV_ENCODE_HINT_HIGH_ENTROPY
 LP = 33
 GROUP_TOKENS = 256
 MAX_PLANES = 128

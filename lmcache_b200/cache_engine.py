@@ -12,7 +12,6 @@ miss ends the match, everything after the first missing chunk is (re)stored (:18
 from __future__ import annotations
 
 import ctypes
-import os
 import threading
 import time
 from typing import Dict, Iterable, List, Optional, Tuple, Union
@@ -186,10 +185,7 @@ class LMCacheEngine:
     def _prefix_hash(self, tokens: torch.Tensor, num_skip_chunk: Optional[int] = 0):
         """All chunk digests of `tokens` (the whole chain is hashed, then the first num_skip_chunk digests are
         dropped, like cache_engine.py:86-96).  A lazy sequence: digest i is there once the chain has reached chunk i."""
-        hashes = sha256_prefix_chain_lazy(tokens, self.chunk_size)[num_skip_chunk or 0:]
-        if os.environ.get("LMCACHE_B200_EAGER_KEYS") == "1":      # measurement knob: wait for the whole chain first
-            return list(hashes)
-        return hashes
+        return sha256_prefix_chain_lazy(tokens, self.chunk_size)[num_skip_chunk or 0:]
 
     def _keys_of(self, chunk_hashes, fmt: str) -> LazySeq:
         return LazySeq(lambda h: self._make_key(h, fmt), chunk_hashes)

@@ -411,10 +411,10 @@ class CacheGenCodec:
             elif sizes.nbytes < 8 * n_chunks:
                 raise ValueError("sizes buffer too small")
             # KV statistics of one model are stable from call to call: the previous call's measured entropy picks the
-            # encode kernel variant for this one (byte-identical output either way)
-            # (the thresholds are in coder bits per symbol; a version-3 payload also holds ~0.4 bits of stream headers)
+            # compaction kernel's shared-memory stage size for this one (byte-identical output either way)
+            # (the threshold is in coder bits per symbol; a version-3 payload also holds ~0.4 bits of stream headers)
             b = self._last_bits_per_symbol - (0.4 if coder == N.CODER_RANS_COMPACT else 0.0)
-            flags = coder | (N.ENCODE_HINT_HIGH_ENTROPY if b > 2.7 else 0) | (N.ENCODE_HINT_MID_ENTROPY if b > 1.2 else 0)
+            flags = coder | (N.ENCODE_HINT_MID_ENTROPY if b > 1.2 else 0)
             N.check(lib.b200kv_encode_chunks(ctypes.byref(view.desc), tok_begin, n_chunks, chunk_size, last,
                                              self._kb, self._vb, flags, out.data_ptr(), stride, sizes.dev_ptr,
                                              self._enc_ws.data_ptr(), self._enc_ws.numel(), tstream.cuda_stream),

@@ -21,7 +21,7 @@
 //     low (pending bits = carry resolution), so every shift of any kind is one funnel shift with one
 //     count k = n + m, emission needs no pending counter, and the decoder finds the symbol with an
 //     approximate reciprocal + a fixed-depth branch-free search that the exact interval products verify
-//     (DESIGN.md sections 3.2 and 3.3).
+//     (DESIGN.md sections 3.2 and 3.4).
 #pragma once
 #include <stdint.h>
 

@@ -334,7 +334,8 @@ __device__ __forceinline__ void rans_put(uint32_t& x, int32_t& nk, const uint16_
 // reference) is done by scan_kernel + compact_kernel afterwards, so no CTA ever waits on another one.
 template <bool FUSED, int DT, bool PAGED, int CODER>
 __global__ void __launch_bounds__(CT, FUSED ? 7 : 4) encode_kernel(EncParams P) {
-    extern __shared__ __align__(16) uint32_t smem[];
+    // 128-byte aligned base (also in cdf_kernel and decode_kernel): the shared-memory layout the kernels were measured with
+    extern __shared__ __align__(128) uint32_t smem[];
     // FUSED : symbol rows u32[CT][SYMW] | cdf rows u16[CT][33] (also the histogram) | fac[256] (later fl32(n/t)[257])
     // !FUSED: pair rows u32[CT][33]                                                 | fac[256]
     constexpr int ROWS_W = FUSED ? CT * SYMW : 0;
@@ -600,236 +601,10 @@ __global__ void __launch_bounds__(CT, FUSED ? 7 : 4) encode_kernel(EncParams P) 
     if (tid == 0) P.tile_tot[(int64_t)j * P.tiles_full + id.tile_in_chunk] = tile_total;
 }
 
-// ------------------------------------------------------------------------------------------ encode, TMA-staged
-// The fused rANS encoder again, rebuilt around three facts the profiles of the kernel above showed (profiles/r2b_*):
-// it is bound by instruction issue (85 % at 0.6 bits/symbol) and, at high entropy, by shared-memory bank conflicts (9.9
-// extra wavefronts per warp-symbol at 4.1 bits); its per-thread LDG.U16 loads with their address arithmetic cost 4.4
-// instructions per symbol; and packing symbols into shared-memory rows only to unpack them again costs another 4.
-//   * Input tiles arrive through the TMA unit: `cp.async.bulk` copies of the tile's token rows (128 channels = 256
-//     contiguous bytes each; any row pitch, paged slots included) into a 3-stage ring of 16-token boxes, completion on
-//     mbarriers.  A symbol's load is then one LDS.U16 at an immediate offset.
-//   * No symbol rows: pass 2 streams the tile through the ring a second time (last box first: rANS codes a stream back
-//     to front) and re-quantises -- 4 instructions, fewer than store + load + unpack, and 22 KB of shared memory less.
-//     The second read is served by L2 or DRAM; the kernel sits at a fifth of the HBM roofline, the bytes are there.
-//   * One TRANSPOSED table [32 entries][128 streams] of 32-bit words serves as histogram (pass 1: one red.shared.add
-//     per symbol) and then as the coder's (start | freq << 16) table (pass 2: one LDS per symbol): a lane never leaves
-//     its own bank, so neither pass has bank conflicts at any entropy; the columns are thread-private, so the passes
-//     need no CTA-wide barrier between them.
-// Eligibility (host side): rANS, chunk <= 256 tokens, tiles of exactly 128 channels that are contiguous in every
-// token row, 16-byte aligned rows.  Everything else takes encode_kernel above.
-constexpr int BOXT = 16;                 // tokens per ring box: 16 x 256 B = 4 KB
-constexpr int RSTAGES = 3;
-constexpr int kEncTmaSmem = 32 * CT * 4 + (kGroup + 16) * 4 + (kGroup + 8) * 4 + RSTAGES * BOXT * CT * 2 + 64;
-
-__device__ __forceinline__ void mbar_init(uint32_t a, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t a, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(a), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t a) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(a) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t a, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tLAB_WAIT:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n\t"
-        "@p bra LAB_DONE;\n\tbra LAB_WAIT;\n\tLAB_DONE:\n\t}" ::"r"(a), "r"(parity), "r"(20000u) : "memory");
-}
-// one row of a box: global -> shared through the TMA unit, completion (bytes) on the stage's mbarrier
-__device__ __forceinline__ void bulk_row_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t mbar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(dst), "l"(src), "r"(bytes), "r"(mbar) : "memory");
-}
-
-template <int DT, bool PAGED>
-__global__ void __launch_bounds__(CT, 7) encode_tma_kernel(EncParams P) {
-    extern __shared__ __align__(128) uint8_t smem8[];
-    uint32_t* tbl = reinterpret_cast<uint32_t*>(smem8);                                   // [32][CT]: counts, then (start | freq << 16)
-    float* fac = reinterpret_cast<float*>(smem8 + 32 * CT * 4);                          // [kGroup + 16]
-    float* ntab = fac + (kGroup + 16);                                                    // fl32(n / t), n = 0..t
-    uint8_t* ring = smem8 + 32 * CT * 4 + (kGroup + 16) * 4 + (kGroup + 8) * 4;          // RSTAGES boxes of BOXT x 256 B
-    const uint32_t ring_a = (uint32_t)__cvta_generic_to_shared(ring);
-    const uint32_t bar_a = ring_a + RSTAGES * BOXT * CT * 2;                              // full[RSTAGES], empty[RSTAGES]
-    __shared__ uint32_t s_warp[CT / 32];
-
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    TileId id;
-    if (!decode_tile(P, blockIdx.x, &id)) return;
-    const int NL = 2 * P.L;
-    const int j = id.j, nl = id.nl, ct = id.ct, t = id.t, gt = id.gt;
-    const int c = ct * CT + tid;
-    uint8_t* cont = P.out + (int64_t)j * P.out_stride;
-    const Layout lo = layout_of(P, t);
-    const uint16_t* maxes = reinterpret_cast<const uint16_t*>(cont + lo.off_maxes) + (int64_t)nl * t + id.tok0;
-    const float maxq = P.pt.maxq[nl];
-    const int64_t tokabs = P.tok_begin + (int64_t)j * P.chunk_tokens + id.tok0;
-    // channel 0 of this tile in row 0 of the plane; the tile's 128 channels are contiguous in every row (host checked)
-    const uint16_t* tile0 = P.pt.p[nl] + (int64_t)((ct * CT) / P.D) * P.sH + ((ct * CT) % P.D);
-    const int NB = (gt + BOXT - 1) / BOXT;               // boxes per pass
-    const int NQ = 2 * NB;                               // pass 1 forwards, pass 2 backwards
-
-    // ---- prologue: factors, n/t table, zeroed counters, barriers
-    for (int i = tid; i < kGroup + 16; i += CT)
-        fac[i] = i < gt ? quant_factor_safe(maxq, half_to_float(maxes[i], DT)) : 0.0f;
-    {
-        const float tf = (float)t;
-        for (int n = tid; n <= t; n += CT) ntab[n] = fdiv((float)n, tf);
-    }
-#pragma unroll
-    for (int i = 0; i < 32; ++i) tbl[i * CT + tid] = 0u;
-    if (tid == 0) {
-        for (int s = 0; s < RSTAGES; ++s) {
-            mbar_init(bar_a + 8 * s, 1);                          // full: the producer's expect_tx arrival (+ the bytes)
-            mbar_init(bar_a + 8 * (RSTAGES + s), CT / 32);        // empty: one arrival per warp
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-
-    // box q of the 2 NB box sequence: pass 1 walks boxes 0..NB-1, pass 2 walks NB-1..0
-    auto issue = [&](int q) {                                      // warp 0, all lanes
-        const int b = q < NB ? q : NQ - 1 - q;
-        const int rows = min(BOXT, gt - b * BOXT);
-        const int stage = q % RSTAGES;
-        const uint32_t full = bar_a + 8 * stage;
-        if (lane == 0) mbar_expect_tx(full, (uint32_t)rows * CT * 2);
-        __syncwarp();
-        if (lane < rows) {
-            const int64_t row = tok_row<PAGED>(P.slot_map, tokabs + b * BOXT + lane);
-            bulk_row_g2s(ring_a + (uint32_t)(stage * BOXT + lane) * CT * 2, tile0 + row * P.sT, CT * 2, full);
-        }
-    };
-    if (warp == 0)
-        for (int q = 0; q < min(RSTAGES, NQ); ++q) issue(q);
-
-    uint32_t* const mycol = tbl + tid;
-    const uint32_t mycol_a = (uint32_t)__cvta_generic_to_shared(mycol);
-    auto consume_done = [&](int q) {                               // every thread, after its last read of box q
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_a + 8 * (RSTAGES + q % RSTAGES));
-        if (warp == 0 && q + RSTAGES < NQ) {                       // the stage is free once all four warps have arrived
-            mbar_wait(bar_a + 8 * (RSTAGES + q % RSTAGES), (uint32_t)(q / RSTAGES) & 1u);
-            issue(q + RSTAGES);
-        }
-    };
-    auto load_box = [&](int q, uint16_t (&x)[BOXT]) {
-        const int stage = q % RSTAGES;
-        mbar_wait(bar_a + 8 * stage, (uint32_t)(q / RSTAGES) & 1u);
-        const uint16_t* colp = reinterpret_cast<const uint16_t*>(ring) + stage * (BOXT * CT) + tid;
-#pragma unroll
-        for (int k = 0; k < BOXT; ++k) x[k] = colp[k * CT];        // LDS.U16 at immediate offsets
-    };
-
-    // ---- pass 1: histogram (one shared-memory reduction per symbol, conflict-free by layout)
-    auto count = [&](uint16_t xv, float f) {
-        const uint32_t sym = quant_symbol_nc(half_to_float(xv, DT), f, maxq);
-        asm volatile("red.shared.add.u32 [%0], 1;" ::"r"(mycol_a + sym * (CT * 4)) : "memory");
-    };
-    for (int q = 0; q < NB; ++q) {
-        uint16_t x[BOXT];
-        load_box(q, x);
-        const int tk0 = q * BOXT;
-        const int rows = min(BOXT, gt - tk0);
-        if (rows == BOXT) {                                         // all boxes but (at most) the last: no per-token test
-#pragma unroll
-            for (int k = 0; k < BOXT; ++k) count(x[k], fac[tk0 + k]);
-        } else {
-#pragma unroll
-            for (int k = 0; k < BOXT; ++k)
-                if (k < rows) count(x[k], fac[tk0 + k]);
-        }
-        consume_done(q);
-    }
-
-    // ---- CDF from the thread's own column, written back as (start | freq << 16) over the counts
-    uint32_t c32, hlen = 0u;
-    uint32_t* trow = P.temp + ((int64_t)blockIdx.x * CT + tid) * P.tempw;
-    {
-        uint32_t cnt[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) cnt[i] = mycol[i * CT];
-        uint32_t mask = 0u;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) mask |= (cnt[i] != 0u ? 1u : 0u) << i;
-        // this kernel is picked for high-entropy data, where every symbol is in use somewhere in the warp: no skipping
-        // of unused symbols here (the tests cost more than they save at 4.1 bits per symbol, measured)
-        const uint32_t wany = 0xffffffffu;
-        if (P.compact) {
-            uint32_t w0, w1;
-            hlen = build_stream_header(cnt, mask, wany, 2 * ((int)maxq + 1), trow, w0, w1);
-            reinterpret_cast<uint2*>(P.rstate)[((int64_t)blockIdx.x * CT + tid) * 2] = make_uint2(w0, w1);
-        }
-        CdfAccum2 acc;
-        acc.init();
-        uint32_t c0 = 0u;
-#pragma unroll
-        for (uint32_t i = 0; i < 31u; ++i) {
-            if ((wany >> i) & 1u) acc.absorb(ntab[cnt[i]]);
-            const uint32_t c1 = acc.value(i + 1u);
-            mycol[i * CT] = c0 | ((c1 - c0) << 16);                 // symbols are <= 30: entry 31 is never coded
-            c0 = c1;
-        }
-        if ((wany >> 31) & 1u) acc.absorb(ntab[cnt[31]]);
-        c32 = acc.value(32u);
-        mycol[31 * CT] = c0 | (c32 << 16);                          // keeps cdf[31] and cdf[32] for the container's CDF row
-    }
-
-    // ---- pass 2: rANS, last token first
-    uint32_t x_state = kRansLow;
-    const uint16_t* const wend = reinterpret_cast<const uint16_t*>(trow) + 2 * P.tempw;             // the row's end
-    int32_t nk = 0;
-    auto code = [&](uint16_t xv, float f) {
-        // the same symbol as pass 1 without the XU pipe (F2I there, reciprocal + F2I in rans_put here): adding
-        // 1.5 * 2^23 rounds v to an integer half-to-even exactly like F2I.RN and leaves it in the low mantissa bits;
-        // fmaxf turns the NaN of a "safe factor" row into the bias itself, i.e. symbol 0, as F2I does
-        const float v = fadd(fmul(half_to_float(xv, DT), f), maxq);
-        const uint32_t sym = __float_as_uint(fmaxf(__fadd_rn(v, 12582912.0f), 12582912.0f)) & 31u;
-        uint32_t pk;
-        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(pk) : "r"(mycol_a + sym * (CT * 4)));
-        rans_put(x_state, nk, wend, pk & 0xffffu, pk >> 16);
-    };
-    for (int q = NB; q < NQ; ++q) {
-        uint16_t x[BOXT];
-        load_box(q, x);
-        const int b = NQ - 1 - q;
-        const int tk0 = b * BOXT;
-        const int rows = min(BOXT, gt - tk0);
-        if (rows == BOXT) {
-#pragma unroll
-            for (int k = BOXT - 1; k >= 0; --k) code(x[k], fac[tk0 + k]);
-        } else {
-#pragma unroll
-            for (int k = BOXT - 1; k >= 0; --k)
-                if (k < rows) code(x[k], fac[tk0 + k]);
-        }
-        consume_done(q);
-    }
-    if (P.compact) reinterpret_cast<uint2*>(P.rstate)[((int64_t)blockIdx.x * CT + tid) * 2 + 1] = make_uint2(x_state, hlen);
-    else P.rstate[(int64_t)blockIdx.x * CT + tid] = x_state;
-    const uint32_t len = hlen + 4u - 2u * (uint32_t)nk;
-
-    // ---- stream lengths, tile total, CDF rows (staged through the now idle ring: stream-major u16[33] rows,
-    //      contiguous in the container -> one coalesced copy)
-    store_len(cont + lo.off_lengths, ((int64_t)id.g * NL + nl) * P.C + c, len, P.compact != 0);
-    uint32_t tile_total;
-    (void)block_excl_scan(len, s_warp, &tile_total);               // has a __syncthreads: every thread is done with the ring
-    if (tid == 0) P.tile_tot[(int64_t)j * P.tiles_full + id.tile_in_chunk] = tile_total;
-    if (id.g == 0 && !P.compact) {                                  // the CDF belongs to the chunk; its first group writes it
-        uint16_t* stg = reinterpret_cast<uint16_t*>(ring);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) stg[tid * kLp + i] = (uint16_t)mycol[i * CT];
-        stg[tid * kLp + 32] = (uint16_t)c32;
-        __syncthreads();
-        uint16_t* dstc = reinterpret_cast<uint16_t*>(cont + lo.off_cdf) + ((int64_t)nl * P.C + ct * CT) * kLp;
-        for (int e = tid; e < CT * kLp; e += CT) dstc[e] = stg[e];
-    }
-}
-
 // ------------------------------------------------------------------------------------------ cdf (chunks > 256 tokens)
 template <int DT, bool PAGED>
 __global__ void __launch_bounds__(CT) cdf_kernel(EncParams P) {
-    extern __shared__ __align__(16) uint32_t smem[];
+    extern __shared__ __align__(128) uint32_t smem[];
     uint32_t* cnts = smem;                                        // CT * PAIRW counters
     float* fac = reinterpret_cast<float*>(cnts + CT * PAIRW);     // kGroup
     const int tid = threadIdx.x;
@@ -1369,7 +1144,7 @@ __device__ __forceinline__ uint32_t rans_decode_stream(const uint8_t* cont, uint
 // intermediates in HBM).  CODER selects the payload format (container version 1: arithmetic coder, 2: rANS).
 template <int OUT_DT, bool PAGED, int CODER, bool TR>
 __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
-    extern __shared__ __align__(16) uint32_t smem[];
+    extern __shared__ __align__(128) uint32_t smem[];
     uint32_t* tab = smem;                                                            // CT * 33 words (rows of 33, odd)
     float* mx = reinterpret_cast<float*>(smem + CT * kLp);                           // kGroup
     float* lut = mx + kGroup;                                                        // 32
@@ -1711,7 +1486,6 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     EncParams P;
     B2_REQUIRE(key_bins && value_bins, "bins are NULL");
-    const bool hint_tma = (coder & B200KV_ENCODE_HINT_HIGH_ENTROPY) != 0;
     const bool hint_mid = (coder & B200KV_ENCODE_HINT_MID_ENTROPY) != 0;
     coder &= 0xff;
     B2_REQUIRE(coder >= CODER_AC && coder <= CODER_RANS_COMPACT, "coder must be one of B200KV_CODER_*");
@@ -1793,28 +1567,7 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
         if (P.dtype == B200KV_DT_BF16) { if (paged) B2_LAUNCH_ENC(FUSED, 0, true, SMEM); else B2_LAUNCH_ENC(FUSED, 0, false, SMEM); } \
         else { if (paged) B2_LAUNCH_ENC(FUSED, 1, true, SMEM); else B2_LAUNCH_ENC(FUSED, 1, false, SMEM); } \
     } while (0)
-    // TMA-staged kernel (encode_tma_kernel): rANS, fused mode, tiles of exactly CT channels that are contiguous in every
-    // token row and 16-byte aligned; the output bytes are the same.  Measured on an H100 SXM (700 W), 8192-token block:
-    // the register-staged kernel above is as fast at 0.6 payload bits per symbol and faster above it (10.3 vs 11.0 ms at
-    // 3.2 coder bits per symbol, 13.0 vs 13.6 ms at 4.1), so no entropy hint selects this kernel here.
-    // B200KV_ENCODE_PATH=tma selects it (A/B measurements).
-    bool tma = false;
-    if (const char* e = getenv("B200KV_ENCODE_PATH")) tma = e[0] == 't';
-    tma = tma && fused && coder == CODER_RANS && P.C % CT == 0 && (kv->sH == kv->D || kv->D % CT == 0) &&
-          kv->sT % 8 == 0 && kv->sH % 8 == 0;
-    for (int nl = 0; nl < 2 * P.L && tma; ++nl) tma = (reinterpret_cast<uintptr_t>(P.pt.p[nl]) & 15) == 0;
-    if (tma) {
-        ProfScope prof(kProfEncode, stream);
-#define B2_LAUNCH_TMA(DT, PAGED)                                                                                       \
-    do {                                                                                                               \
-        B2_CHECK_CUDA(cudaFuncSetAttribute(encode_tma_kernel<DT, PAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
-                                           kEncTmaSmem));                                                              \
-        encode_tma_kernel<DT, PAGED><<<(unsigned)n_tiles, CT, kEncTmaSmem, stream>>>(P);                               \
-    } while (0)
-        if (P.dtype == B200KV_DT_BF16) { if (paged) B2_LAUNCH_TMA(0, true); else B2_LAUNCH_TMA(0, false); }
-        else { if (paged) B2_LAUNCH_TMA(1, true); else B2_LAUNCH_TMA(1, false); }
-#undef B2_LAUNCH_TMA
-    } else if (fused) {
+    if (fused) {
         ProfScope prof(kProfEncode, stream);
         B2_LAUNCH_ENC2(true, smem_fused);
     } else {
@@ -1846,12 +1599,8 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
         P.stage_bytes = coder == CODER_RANS ? CT * (TEMPW_FUSED_RANS * 4 + 4) + 32 : CT * TEMPW_FUSED * 4 + 32;
         // The kernel waits on sparse row reads: more resident CTAs hide more of that latency.  Without an entropy hint a
         // tile's streams total a few KB, so a 12 KB stage (12 CTAs per SM instead of 9: measured faster) covers
-        // them; the rare larger tile takes the kernel's direct path.  B200KV_COMPACT_STAGE=<bytes> overrides (knob).
-        if (coder == CODER_RANS && !hint_tma && !hint_mid) P.stage_bytes = 12 * 1024;
-        if (const char* e = getenv("B200KV_COMPACT_STAGE")) {
-            const int v = atoi(e);
-            if (v >= 1024 && v <= P.stage_bytes + 16 * 1024) P.stage_bytes = v & ~15;
-        }
+        // them; the rare larger tile takes the kernel's direct path.
+        if (coder == CODER_RANS && !hint_mid) P.stage_bytes = 12 * 1024;
         B2_CHECK_CUDA(cudaFuncSetAttribute(compact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, P.stage_bytes));
         enc_scan_kernel<<<(unsigned)n_chunks, 1024, 0, stream>>>(P);
         compact_kernel<<<(unsigned)n_tiles, CT, (size_t)P.stage_bytes, stream>>>(P);

@@ -115,58 +115,22 @@ __global__ void __launch_bounds__(128) sha256_expand_kernel(ShaParams P) {
 }
 
 // 64 rounds over precomputed (W + K); state in registers, variables renamed instead of rotated.
-// One chain is one thread.  Per round: three funnel shifts + one LOP3 per Sigma, one LOP3 each for Ch and Maj -- ten
-// integer-ALU-pipe instructions (one warp instruction per 2 cycles per SM sub-partition) -- and the additions.
-//   FMA_ADDS = false (default): the additions are IADD3s on the same pipe (4 more): pipe floor 28 cycles per round.
-//   FMA_ADDS = true : every addition is x * 1 + y with a multiplier the compiler cannot see through (IMAD, FMA pipe, one
-//                     warp instruction per cycle): 20 cycles of ALU pipe + 6 of FMA pipe, overlappable on paper.
-// The recurrence e -> Sigma1 -> t1 -> e' is SHF -> LOP3 -> add -> add, ~18 cycles of latency.  Measured (8192 tokens =
-// 1057 blocks in one chain): IADD3s are faster than IMADs -- six two-input
-// IMADs form a longer dependency chain than two three-input IADD3s, and one warp is bound by that chain, not by pipe
-// throughput.  The same lesson as the attempt to move half of the ROTATIONS to the FMA pipe (x * 2^(32-n) as a 64-bit
-// product, halves summed): slower still.  A third variant moves only h + (W + K) -- known three rounds ahead, off every chain --
-// to the FMA pipe (13 ALU instructions per round instead of 14): no gain either.
-// B200KV_SHA_ADDS=alu|hwk|fma picks the variant (measurement knob, default alu).
-template <bool FMA_ADDS>
-__device__ __forceinline__ uint32_t sha_add(uint32_t x, uint32_t y, uint32_t one) {
-    if constexpr (FMA_ADDS) {
-        uint32_t r;
-        asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(r) : "r"(x), "r"(one), "r"(y));
-        return r;
-    } else {
-        return x + y;
-    }
-}
-
+// One chain is one thread, so the chain is bound by the latency of e -> Sigma1 -> t1 -> e', not by pipe throughput: all
+// of it stays on the integer ALU pipe (three-input IADD3s).  Moving additions or rotations to the FMA pipe (IMADs)
+// lengthened that dependency chain and was slower (DESIGN.md 3.5).
 #define B2_SHA_ROUND(a, b, c, d, e, f, g, h, wk)                                                          \
     {                                                                                                      \
         const uint32_t s1_ = rotr(e, 6) ^ rotr(e, 11) ^ rotr(e, 25);                                       \
         const uint32_t ch_ = ((e) & (f)) ^ (~(e) & (g));                                                   \
         const uint32_t s0_ = rotr(a, 2) ^ rotr(a, 13) ^ rotr(a, 22);                                       \
         const uint32_t mj_ = ((a) & (b)) ^ ((a) & (c)) ^ ((b) & (c));                                      \
-        if constexpr (FMA_ADDS == 1) {                                                                     \
-            uint32_t t1_ = sha_add<true>(h, wk, one);          /* off the critical path */                 \
-            t1_ = sha_add<true>(t1_, ch_, one);                                                            \
-            t1_ = sha_add<true>(t1_, s1_, one);                                                            \
-            const uint32_t t2_ = sha_add<true>(s0_, mj_, one);                                             \
-            (d) = sha_add<true>(d, t1_, one);                                                              \
-            (h) = sha_add<true>(t1_, t2_, one);                                                            \
-        } else if constexpr (FMA_ADDS == 2) {                                                              \
-            /* only h + (W + K) -- known three rounds ahead, off every dependency chain -- leaves the ALU pipe */ \
-            const uint32_t hwk_ = sha_add<true>(h, wk, one);                                               \
-            const uint32_t t1_ = hwk_ + s1_ + ch_;                                                         \
-            (d) += t1_;                                                                                    \
-            (h) = t1_ + s0_ + mj_;                                                                         \
-        } else {                                                                                           \
-            const uint32_t t1_ = (h) + s1_ + ch_ + (wk);                                                   \
-            (d) += t1_;                                                                                    \
-            (h) = t1_ + s0_ + mj_;                                                                         \
-        }                                                                                                  \
+        const uint32_t t1_ = (h) + s1_ + ch_ + (wk);                                                       \
+        (d) += t1_;                                                                                        \
+        (h) = t1_ + s0_ + mj_;                                                                             \
     }
 
 // 64 rounds over a block's (W + K) held in registers
-template <int FMA_ADDS>
-__device__ __forceinline__ void compress_regs(uint32_t (&st)[8], const uint4 (&q)[16], uint32_t one) {
+__device__ __forceinline__ void compress_regs(uint32_t (&st)[8], const uint4 (&q)[16]) {
     uint32_t a = st[0], b = st[1], c = st[2], d = st[3], e = st[4], f = st[5], g = st[6], h = st[7];
 #pragma unroll
     for (int i = 0; i < 16; i += 2) {
@@ -184,8 +148,7 @@ __device__ __forceinline__ void compress_regs(uint32_t (&st)[8], const uint4 (&q
 }
 
 // ... and over a block staged in shared memory: slot[i * 32] is this lane's i-th 16-byte group
-template <int FMA_ADDS>
-__device__ __forceinline__ void compress_smem(uint32_t (&st)[8], const uint4* slot, uint32_t one) {
+__device__ __forceinline__ void compress_smem(uint32_t (&st)[8], const uint4* slot) {
     uint32_t a = st[0], b = st[1], c = st[2], d = st[3], e = st[4], f = st[5], g = st[6], h = st[7];
 #pragma unroll
     for (int i = 0; i < 16; i += 2) {
@@ -209,13 +172,11 @@ constexpr int kShaStages = 3;
 // waits for L2 / DRAM (an earlier version kept the next block in registers; the compiler sank those loads to the point where
 // the registers became free, late in the loop body, and the chain waited for them).
 // The ring is lane-interleaved at 16-byte granularity: a warp's LDS.128 of "its" i-th group is one conflict-free request.
-template <int FMA_ADDS>
 __global__ void __launch_bounds__(32) sha256_chain_kernel(ShaParams P) {
     __shared__ __align__(16) uint4 ring[kShaStages][16][32];
     const int lane = threadIdx.x;
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= P.n_seq) return;
-    const uint32_t one = P.n_seq > 0 ? 1u : 0u;          // 1, but not a constant ptxas can fold
     const int64_t t0 = P.seq_offsets[s], t1 = P.seq_offsets[s + 1];
     int64_t slot = P.seq_chunk0[s];
     int64_t gb = P.seq_block0[s];
@@ -271,13 +232,13 @@ __global__ void __launch_bounds__(32) sha256_chain_kernel(ShaParams P) {
             for (int i = 0; i < 16; ++i)
                 q[i] = make_uint4(w[4 * i] + kK[4 * i], w[4 * i + 1] + kK[4 * i + 1], w[4 * i + 2] + kK[4 * i + 2],
                                   w[4 * i + 3] + kK[4 * i + 3]);
-            compress_regs<FMA_ADDS>(st, q, one);
+            compress_regs(st, q);
         }
 #pragma unroll 1
         for (uint32_t k = 0; k < ntail; ++k) {
             asm volatile("cp.async.wait_group 1;" ::: "memory");          // all but the newest group: block k has landed
             issue(k + 2);                                                  // into the stage block k - 1 has just left
-            compress_smem<FMA_ADDS>(st, &ring[k % kShaStages][0][lane], one);
+            compress_smem(st, &ring[k % kShaStages][0][lane]);
         }
         asm volatile("cp.async.wait_group 0;" ::: "memory");
         gb += P.blocks_per_full_chunk;      // scratch blocks are laid out at a fixed stride per chunk
@@ -391,13 +352,7 @@ extern "C" int b200kv_sha256_chain_ready(const void* tokens, int32_t elem_size, 
     sha256_expand_kernel<<<(unsigned)((n_blocks + 127) / 128), 128, 0, stream>>>(P);
     e = cudaGetLastError();
     if (e == cudaSuccess) {
-        static const int adds = [] {
-            const char* v = getenv("B200KV_SHA_ADDS");
-            return v == nullptr ? 0 : v[0] == 'f' ? 1 : v[0] == 'h' ? 2 : 0;
-        }();
-        if (adds == 1) sha256_chain_kernel<1><<<(unsigned)((n_seq + 31) / 32), 32, 0, stream>>>(P);
-        else if (adds == 2) sha256_chain_kernel<2><<<(unsigned)((n_seq + 31) / 32), 32, 0, stream>>>(P);
-        else sha256_chain_kernel<0><<<(unsigned)((n_seq + 31) / 32), 32, 0, stream>>>(P);
+        sha256_chain_kernel<<<(unsigned)((n_seq + 31) / 32), 32, 0, stream>>>(P);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaEventRecord(g_ev[devi], stream);
