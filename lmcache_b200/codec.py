@@ -186,8 +186,10 @@ class KvView:
         return KvView(d, (keep, ptrs), slot_mapping.numel(), ref.device, ref.dtype, "vllm")
 
 
-def parse_header(buf) -> N.Header:
-    """Validate and return the 64-byte header of a B2KV container (bytes / bytearray / memoryview)."""
+def parse_header(buf, total: Optional[int] = None) -> N.Header:
+    """Validate and return the 64-byte header of a B2KV container (bytes / bytearray / memoryview).  `buf` is the whole
+    container, or -- when `total`, the size of the whole container, is given -- a prefix of it that holds the header
+    and, for version 3, the nb map after it."""
     mv = memoryview(buf)
     if mv.nbytes < N.HEADER_BYTES:
         raise ValueError("buffer too small for a B2KV container")
@@ -196,7 +198,7 @@ def parse_header(buf) -> N.Header:
         raise ValueError("not a B2KV container (bad magic)")
     if hd.version not in (1, 2, 3):
         raise ValueError(f"unsupported B2KV version {hd.version}")
-    if hd.total_bytes > mv.nbytes:
+    if hd.total_bytes > (mv.nbytes if total is None else total):
         raise ValueError("truncated B2KV container")
     if hd.status != 0:
         raise ValueError(f"B2KV container carries encoder error status {hd.status}")
@@ -568,11 +570,7 @@ class CacheGenCodec:
         heads = []
         for c in containers:
             if isinstance(c, torch.Tensor):
-                hb = c[:N.HEADER_BYTES + N.MAX_PLANES].cpu().numpy().tobytes()
-                hd = N.Header.from_buffer_copy(hb[:N.HEADER_BYTES])
-                if hd.magic != N.MAGIC or hd.version not in (1, 2, 3) or hd.status != 0 or hd.total_bytes > c.numel():
-                    raise ValueError("bad B2KV container tensor")
-                check_header(hd, list(hb[N.HEADER_BYTES:N.HEADER_BYTES + 2 * hd.L]) if hd.version == 3 else None)
+                hd = parse_header(c[:N.HEADER_BYTES + N.MAX_PLANES].cpu().numpy().tobytes(), c.numel())
             else:
                 hd = parse_header(c)
             if not self.accepts(hd):

@@ -4,25 +4,33 @@ decode on the way in (SURVEY.md section 7 step 7, BASELINE configs[2]).
 A store is cut into waves of a few chunks.  Each wave owns a *slot*: a device staging area for its containers and a
 page-locked array for their sizes.  The caller's thread only enqueues kernels (CacheGenCodec.encode_async on the
 caller's stream: the KV is consumed in stream order, nothing is synchronised) and hands the slot to a worker thread;
-the worker waits for the wave's event, learns the container sizes, and moves exactly those bytes to the tier (device ->
-page-locked slab on a copy stream, or a socket).  While it does, the next wave is already encoding.  Scratch is bounded
-by slots x wave size instead of the whole block (round 1 staged every chunk of a store at once: ~4 GB of device scratch
-for a 4 GiB block).
+the worker waits for the wave's event, learns the container sizes, and hands the wave to the tier's sink, which `land`s
+exactly those bytes in a page-locked slab (and keeps them, writes them to files or sends them over sockets).  While it
+does, the next wave is already encoding.  Scratch is bounded by slots x wave size instead of the whole block (round 1
+staged every chunk of a store at once: ~4 GB of device scratch for a 4 GiB block).
+
+On the way in, every tier hands `upload_decode` its containers in chunk order as `HostContainer` records -- the ones it
+keeps, or disk reads / GETs still in flight (`fetched_in_order`) -- and `DeferredFree` releases transient blocks once
+their uploads are done.
 
 The reference does none of this: LMCLocalBackend.put_nonblocking hands whole chunk tensors to a queue and its worker
 calls tensor.to("cpu") + torch.cuda.synchronize() per chunk (lmcache/storage_backend/local_backend.py:82-117).
 """
 from __future__ import annotations
 
+import collections
+import ctypes
+import functools
 import os
 import queue
 import threading
-from typing import Callable, List, Optional, Sequence
+from concurrent.futures import Future
+from typing import Callable, Iterable, Iterator, List, Optional, Sequence
 
 import torch
 
 from lmcache_b200 import _native as N
-from lmcache_b200.codec import CacheGenCodec, EncodeTicket, KvView, PinnedBuffer
+from lmcache_b200.codec import CacheGenCodec, EncodeTicket, KvView, PinnedBuffer, parse_header
 
 
 def wave_chunks_default() -> int:
@@ -224,75 +232,167 @@ class UploadRing:
         self._busy[i] = ev
 
 
-def fetch_decode(codec: CacheGenCodec, upload: UploadRing, futures: Sequence, dst: KvView, dst_tok0: int, chunk_size: int,
-                 inflight: list, on_more: Optional[Callable[[int], None]] = None, wave: Optional[int] = None) -> int:
-    """Consume container fetches IN ORDER -- futures[i].result() is (slab block, nbytes) or None for a miss; an entry may
-    also be such a tuple directly -- and, wave by wave, upload the containers on the copy stream and decode them into
-    `dst` on the current stream (chunk i lands at token dst_tok0 + i * chunk_size).  Fetches of later chunks keep running
-    in their pool while earlier waves upload and decode: network / disk || H2D || decode.  Stops at the first miss or
-    damaged / mismatching container; everything fetched past that point is released.  Blocks of uploaded waves are
-    appended to `inflight` as (event, [blocks]) for the caller to free once the event has completed.
-    `on_more(i)` is called before chunk i is awaited (lets the caller keep a window of fetches in flight)."""
-    import ctypes
+class HostContainer:
+    """One CacheGen container in a page-locked slab block, with the header fields its upload and decode need."""
+    __slots__ = ("blk", "nbytes", "ntokens", "L", "H", "D", "max_dtype", "coder", "last_read")
 
-    from lmcache_b200.codec import parse_header
-    W = wave or wave_chunks_default()
+    def __init__(self, blk, nbytes: int, hd: "N.Header"):
+        self.blk = blk                       # None once the tier no longer keeps the bytes (the disk tier's index)
+        self.nbytes = int(nbytes)
+        self.ntokens = int(hd.ntokens)
+        self.L, self.H, self.D = int(hd.L), int(hd.H), int(hd.D)
+        self.max_dtype = int(hd.max_dtype)
+        self.coder = int(hd.version) - 1
+        self.last_read: Optional[torch.cuda.Event] = None   # most recent upload out of the block
+
+
+@functools.lru_cache(maxsize=None)
+def _d2h_stream(device: torch.device) -> torch.cuda.Stream:
+    return torch.cuda.Stream(device=device)
+
+
+def land(slab, slot: WaveSlot, batch) -> List[HostContainer]:
+    """Store-pipeline sink side: copy a finished wave's containers out of slot.dev into fresh blocks of `slab` (exactly
+    their bytes, on the device's copy stream), wait for the copies, and parse every header.  Raises -- with every block
+    freed -- when a copy fails or a container carries an encoder error."""
+    dev = slot.dev.device
+    cs = _d2h_stream(dev)
+    blocks = [slab.alloc(size) for size in batch.sizes]
+    try:
+        with torch.cuda.device(dev):
+            try:
+                for j, (blk, size) in enumerate(zip(blocks, batch.sizes)):
+                    N.check(N.lib().b200kv_copy_async(ctypes.c_void_p(blk.host_ptr),
+                                                      ctypes.c_void_p(slot.dev.data_ptr() + j * batch.stride), size,
+                                                      cs.cuda_stream), "copy_async")
+            finally:
+                cs.synchronize()             # no block leaves this function while a copy may still write it
+        return [HostContainer(blk, blk.nbytes, parse_header(blk.view())) for blk in blocks]
+    except BaseException:
+        for blk in blocks:
+            blk.free()
+        raise
+
+
+def read_container(codec: CacheGenCodec, blk, nbytes: int) -> Optional[HostContainer]:
+    """The record of a container a disk read or a GET put into the first `nbytes` of `blk`, or None -- with the block
+    freed -- when it is damaged or was written with another model's bins (a miss, not an error)."""
+    try:
+        hd = parse_header(blk.view()[:nbytes])
+        if codec.accepts(hd):
+            return HostContainer(blk, nbytes, hd)
+    except ValueError:
+        pass
+    blk.free()
+    return None
+
+
+class DeferredFree:
+    """Slab blocks that host->device copies may still be reading: each group is freed once the event recorded after
+    those copies has completed (an event of None: nothing reads them)."""
+
+    def __init__(self):
+        self._held: list = []              # (event, [blocks])
+        self._lock = threading.Lock()
+
+    def add(self, event: Optional[torch.cuda.Event], blocks: list) -> None:
+        with self._lock:
+            self._held.append((event, blocks))
+
+    def sweep(self, wait: bool = False) -> None:
+        """Free every group whose event has completed (wait=True: wait for all of them first)."""
+        with self._lock:
+            keep = []
+            for ev, blocks in self._held:
+                if wait and ev is not None:
+                    ev.synchronize()
+                if ev is None or ev.query():
+                    for b in blocks:
+                        b.free()
+                else:
+                    keep.append((ev, blocks))
+            self._held = keep
+
+    def drain(self) -> None:
+        """Blocking: free everything once its copies are done (a tier's close())."""
+        self.sweep(wait=True)
+
+
+def fetched_in_order(futures: Iterable[Future], window: Optional[int] = None) -> Iterator[Optional[HostContainer]]:
+    """Results of container fetches (futures of a HostContainer, None for a miss) in the order given, with at most
+    `window` of them taken from `futures` ahead of the consumer (None: all of them) -- `futures` may submit each fetch
+    as it is taken.  When the consumer stops early, the fetches already issued run to completion and their blocks are
+    freed."""
+    pending: "collections.deque[Future]" = collections.deque()
+    try:
+        for f in futures:
+            pending.append(f)
+            if window is not None and len(pending) >= window:
+                yield pending.popleft().result()
+        while pending:
+            yield pending.popleft().result()
+    finally:
+        for f in pending:
+            rec = f.result()
+            if rec is not None:
+                rec.blk.free()
+
+
+def upload_decode(codec: CacheGenCodec, upload: UploadRing, records: Iterable[Optional[HostContainer]], dst: KvView,
+                  dst_tok0: int, chunk_size: int, release: Optional[DeferredFree] = None) -> int:
+    """Upload + decode consecutive chunks straight into `dst`: records[i] (None: a miss) is chunk i and lands at token
+    dst_tok0 + i * chunk_size.  Wave by wave the containers are copied into an UploadRing slot on its copy stream and
+    decoded on the current stream; nothing is synchronised, and the records are consumed as the caller produces them
+    (later fetches / hash-chain keys overlap earlier waves).  Every uploaded record's `last_read` is set to its wave's
+    upload event.  Returns the number of chunks decoded: the match stops at the first miss, at the first container whose
+    geometry differs from `dst` or that does not fit it, and at the first whose (max_dtype, coder) differs from the
+    first container's.  With `release`, the records' blocks are transient: each wave's go to `release` with its upload
+    event, and the block of the record the match stopped at is freed."""
+    W = wave_chunks_default()
     lib = N.lib()
-    n_done = 0
-    wave_items: list = []                  # (block, nbytes, header, chunk index)
+    wave: List[HostContainer] = []
+    n = 0
+    first = None
     with torch.cuda.device(dst.device):
         cur = torch.cuda.current_stream()
 
         def flush():
-            if not wave_items:
+            if not wave:
                 return
             offs, o = [], 0
-            for _, n, _, _ in wave_items:
+            for r in wave:
                 offs.append(o)
-                o += (n + 15) & ~15
+                o += (r.nbytes + 15) & ~15
             slot, buf = upload.next_slot(o)
-            for (blk, n, _, _), off in zip(wave_items, offs):
-                N.check(lib.b200kv_copy_async(ctypes.c_void_p(buf.data_ptr() + off), ctypes.c_void_p(blk.host_ptr), n,
-                                              upload.copy_stream.cuda_stream), "copy_async")
+            for r, off in zip(wave, offs):
+                N.check(lib.b200kv_copy_async(ctypes.c_void_p(buf.data_ptr() + off), ctypes.c_void_p(r.blk.host_ptr),
+                                              r.nbytes, upload.copy_stream.cuda_stream), "copy_async")
             ev = torch.cuda.Event()
             ev.record(upload.copy_stream)
-            inflight.append((ev, [w[0] for w in wave_items]))
+            for r in wave:
+                r.last_read = ev
+            if release is not None:
+                release.add(ev, [r.blk for r in wave])
             cur.wait_event(ev)
-            h0 = wave_items[0][2]
-            codec.decode_raw(buf.data_ptr(), buf.numel(), offs, [w[1] for w in wave_items],
-                             [int(w[2].ntokens) for w in wave_items], dst,
-                             [dst_tok0 + w[3] * chunk_size for w in wave_items], int(h0.max_dtype), int(h0.version) - 1, cur)
+            w0 = n - len(wave)
+            codec.decode_raw(buf.data_ptr(), buf.numel(), offs, [r.nbytes for r in wave], [r.ntokens for r in wave], dst,
+                             [dst_tok0 + (w0 + j) * chunk_size for j in range(len(wave))], wave[0].max_dtype,
+                             wave[0].coder, cur)
             upload.mark_read(slot, cur)
-            wave_items.clear()
+            wave.clear()
 
-        stop_at = len(futures)
-        for i in range(len(futures)):
-            if on_more is not None:
-                on_more(i)
-            f = futures[i]
-            got = f.result() if hasattr(f, "result") else f
-            if got is None:
-                stop_at = i
+        for r in records:
+            if r is None:
                 break
-            blk, n = got
-            try:
-                hd = parse_header(blk.view()[:n])
-                ok = codec.accepts(hd) and (hd.L, hd.H, hd.D) == (dst.L, dst.H, dst.D) and \
-                    dst_tok0 + i * chunk_size + hd.ntokens <= dst.ntokens and \
-                    (not wave_items or (hd.max_dtype, hd.version) == (wave_items[0][2].max_dtype, wave_items[0][2].version))
-            except ValueError:
-                ok = False                      # damaged container: a miss, not an error
-            if not ok:
-                blk.free()
-                stop_at = i
+            if (r.L, r.H, r.D) != (dst.L, dst.H, dst.D) or dst_tok0 + n * chunk_size + r.ntokens > dst.ntokens or \
+                    (first is not None and (r.max_dtype, r.coder) != (first.max_dtype, first.coder)):
+                if release is not None:
+                    r.blk.free()
                 break
-            wave_items.append((blk, n, hd, i))
-            n_done += 1
-            if len(wave_items) == W:
+            first = first or r
+            wave.append(r)
+            n += 1
+            if len(wave) == W:
                 flush()
         flush()
-    for f in futures[stop_at + 1:]:              # fetches past the first miss: let them finish, drop their blocks
-        r = f.result() if hasattr(f, "result") else f
-        if r is not None:
-            r[0].free()
-    return n_done
+    return n

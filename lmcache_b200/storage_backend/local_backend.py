@@ -252,20 +252,23 @@ class LMCLocalBackend(LMCBackendInterface):
 
 # ---------------------------------------------------------------------------------------------- compressed host tier
 class _CEntry:
-    """One CacheGen container in the page-locked slab."""
-    __slots__ = ("blk", "path", "nbytes", "ntokens", "L", "H", "D", "max_dtype", "coder", "ready", "error", "last_read")
+    """One stored chunk: its container's record (pipeline.HostContainer) plus the tier's bookkeeping."""
+    __slots__ = ("rec", "path", "ready", "error")
 
     def __init__(self):
-        self.blk = None
-        self.path = None                     # disk tier: the container's file (then blk is None)
-        self.nbytes = 0
-        self.ntokens = 0
-        self.L = self.H = self.D = 0
-        self.max_dtype = 0
-        self.coder = 0
+        self.rec = None                      # None until the container has landed (and again once it is retired)
+        self.path = None                     # disk tier: the container's file (then rec.blk is None)
         self.ready = threading.Event()       # set by the store worker once the container is in host memory
         self.error: Optional[BaseException] = None
-        self.last_read: Optional[torch.cuda.Event] = None   # most recent upload out of the block
+
+    # read by reports (bench.py's e2e counts the container bytes a retrieve uploads)
+    @property
+    def blk(self):
+        return None if self.rec is None else self.rec.blk
+
+    @property
+    def nbytes(self) -> int:
+        return 0 if self.rec is None else self.rec.nbytes
 
 
 class LMCLocalCompressedBackend(LMCBackendInterface):
@@ -283,7 +286,7 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
     def __init__(self, config: LMCacheEngineConfig, metadata):
         super().__init__()
         from lmcache_b200.codec import CacheGenCodec
-        from lmcache_b200.pipeline import EncodePipeline, UploadRing
+        from lmcache_b200.pipeline import DeferredFree, EncodePipeline, UploadRing
         from lmcache_b200.slab import PinnedSlab
         N.require_cuda()
         self.chunk_size = config.chunk_size
@@ -294,65 +297,30 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         self.slab = PinnedSlab()
         self.dict: Dict[CacheEngineKey, _CEntry] = {}
         self.update_lock = threading.Lock()
-        self._copy_stream: Optional[torch.cuda.Stream] = None
         self._pipe = EncodePipeline(self.codec, self._sink)
         self._upload: Optional[UploadRing] = None
-        self._retired = []                                    # (event, block): overwritten entries still being read
+        self._release = DeferredFree()        # blocks uploads may still read: retired entries, the disk tier's file reads
         self._closed = False
 
     # ------------------------------------------------------------------ store
-    def _land(self, slot, batch, entries) -> None:
-        """worker thread: the wave's containers -> slab blocks (one async copy each, exactly `size` bytes); fills the
-        entries from the container headers.  Raises (after marking the entries) when anything is wrong."""
-        dev = slot.dev.device
-        with torch.cuda.device(dev):
-            if self._copy_stream is None or self._copy_stream.device != dev:
-                self._copy_stream = torch.cuda.Stream(device=dev)
-            cs = self._copy_stream
-            try:
-                blocks = []
-                for j, size in enumerate(batch.sizes):
-                    blk = self.slab.alloc(size)
-                    blocks.append(blk)
-                    N.check(N.lib().b200kv_copy_async(ctypes.c_void_p(blk.host_ptr),
-                                                      ctypes.c_void_p(slot.dev.data_ptr() + j * batch.stride), size,
-                                                      cs.cuda_stream), "copy_async")
-                cs.synchronize()
-                from lmcache_b200.codec import parse_header
-                for e, blk in zip(entries, blocks):
-                    hd = parse_header(blk.view())              # raises on a nonzero encoder status
-                    e.blk, e.nbytes, e.ntokens = blk, blk.nbytes, int(hd.ntokens)
-                    e.L, e.H, e.D, e.max_dtype, e.coder = int(hd.L), int(hd.H), int(hd.D), int(hd.max_dtype), int(hd.version) - 1
-            except BaseException as err:     # noqa: BLE001
-                for e in entries:
-                    e.error = err
-                raise
-
     def _sink(self, slot, batch, c0, entries) -> None:
         """store pipeline sink: land the wave in host memory, then publish the entries (readers wait on `ready`)"""
+        from lmcache_b200.pipeline import land
         try:
-            self._land(slot, batch, entries)
+            for e, rec in zip(entries, land(self.slab, slot, batch)):
+                e.rec = rec
+        except BaseException as err:     # noqa: BLE001 -- the entries become misses; the job reports the error
+            for e in entries:
+                e.error = err
+            raise
         finally:
             for e in entries:
                 e.ready.set()
 
     def _retire(self, e: _CEntry) -> None:
-        if e.blk is None:
-            return
-        if e.last_read is not None and not e.last_read.query():
-            self._retired.append((e.last_read, e.blk))
-        else:
-            e.blk.free()
-        e.blk = None
-
-    def _sweep(self) -> None:
-        keep = []
-        for ev, blk in self._retired:
-            if ev.query():
-                blk.free()
-            else:
-                keep.append((ev, blk))
-        self._retired = keep
+        rec, e.rec = e.rec, None
+        if rec is not None:
+            self._release.add(rec.last_read, [rec.blk])
 
     def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True) -> int:
         # `keys` may be lazy (the engine's hash chain produces key i after keys 0..i-1): the encode waves
@@ -369,7 +337,7 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         for prev in old:                            # an overwritten container leaves once nobody reads it any more
             prev.ready.wait()
             self._retire(prev)
-        self._sweep()
+        self._release.sweep()
         if blocking:
             job.wait()
         return len(keys)
@@ -383,25 +351,24 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         self.put_kv_chunks([key], view, 0, view.ntokens, blocking=blocking)
 
     # ------------------------------------------------------------------ lookup
+    def _lookup(self, key: CacheEngineKey) -> Optional[_CEntry]:
+        return self.dict.get(key)
+
     def contains(self, key: CacheEngineKey) -> bool:
-        e = self.dict.get(key)
-        if e is None:
-            return False
-        if e.ready.is_set() and e.error is not None:
-            return False
-        return True
+        e = self._lookup(key)
+        return e is not None and not (e.ready.is_set() and e.error is not None)
 
     def _ready_entry(self, key) -> Optional[_CEntry]:
-        e = self.dict.get(key)
+        e = self._lookup(key)
         if e is None:
             return None
         e.ready.wait()
-        return None if e.error is not None or e.blk is None else e
+        return None if e.error is not None or e.rec is None else e
 
     def peek_geometry(self, key, fmt: str = "vllm"):
         """(L, H, D, output dtype) of the stored chunks, read from a container header (no decode)."""
         e = self._ready_entry(key)
-        return None if e is None else (e.L, e.H, e.D, self.out_dtype())
+        return None if e is None else (e.rec.L, e.rec.H, e.rec.D, self.out_dtype())
 
     def out_dtype(self) -> torch.dtype:
         # the reference's decoder casts by format, ignoring metadata.dtype (cachegen_decoder.py:189-200)
@@ -414,57 +381,17 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
     def get_kv_into(self, keys, dst, dst_tok0: int, chunk_size: int) -> int:
         """Upload + decode consecutive chunks (until the first miss) straight into `dst`; chunk i lands at token
         dst_tok0 + i * chunk_size.  Everything is enqueued: copies on the copy stream, decodes on the current stream."""
-        from lmcache_b200.pipeline import UploadRing, wave_chunks_default
-        W = wave_chunks_default()
-        lib = N.lib()
-        n_hits = 0
-        first = None
-        with torch.cuda.device(dst.device):
-            if self._upload is None or self._upload.device != dst.device:
-                self._upload = UploadRing(dst.device)
-            up = self._upload
-            cur = torch.cuda.current_stream()
+        from lmcache_b200.pipeline import upload_decode
+        # keys may be lazy (the hash chain is still running): every full wave is uploaded and decoded as soon as its
+        # keys exist, while the chain works on the later chunks.  The records were checked when they landed.
+        recs = (None if e is None else e.rec for e in map(self._ready_entry, keys))
+        return upload_decode(self.codec, self._upload_ring(dst.device), recs, dst, dst_tok0, chunk_size)
 
-            def flush(wave, w0):
-                offs, o = [], 0
-                for e in wave:
-                    offs.append(o)
-                    o += (e.nbytes + 15) & ~15
-                slot, buf = up.next_slot(o)
-                for e, off in zip(wave, offs):
-                    N.check(lib.b200kv_copy_async(ctypes.c_void_p(buf.data_ptr() + off), ctypes.c_void_p(e.blk.host_ptr),
-                                                  e.nbytes, up.copy_stream.cuda_stream), "copy_async")
-                ev = torch.cuda.Event()
-                ev.record(up.copy_stream)
-                for e in wave:
-                    e.last_read = ev
-                cur.wait_event(ev)
-                self.codec.decode_raw(buf.data_ptr(), buf.numel(), offs, [e.nbytes for e in wave],
-                                      [e.ntokens for e in wave], dst,
-                                      [dst_tok0 + (w0 + j) * chunk_size for j in range(len(wave))],
-                                      wave[0].max_dtype, wave[0].coder, cur)
-                up.mark_read(slot, cur)
-
-            # keys may be lazy (the hash chain is still running): every full wave is uploaded and decoded as soon as its
-            # keys exist, while the chain works on the later chunks
-            wave = []
-            for i, key in enumerate(keys):
-                e = self._ready_entry(key)
-                if e is None or (e.L, e.H, e.D) != (dst.L, dst.H, dst.D):
-                    break
-                if dst_tok0 + i * chunk_size + e.ntokens > dst.ntokens:
-                    break
-                if first is not None and (e.max_dtype, e.coder) != (first.max_dtype, first.coder):
-                    break
-                first = first or e
-                wave.append(e)
-                n_hits += 1
-                if len(wave) == W:
-                    flush(wave, n_hits - W)
-                    wave = []
-            if wave:
-                flush(wave, n_hits - len(wave))
-        return n_hits
+    def _upload_ring(self, device):
+        from lmcache_b200.pipeline import UploadRing
+        if self._upload is None or self._upload.device != device:
+            self._upload = UploadRing(device)
+        return self._upload
 
     @_lmcache_nvtx_annotate
     def get(self, key: CacheEngineKey) -> Optional[torch.Tensor]:
@@ -472,9 +399,10 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         e = self._ready_entry(key)
         if e is None:
             return None
-        shape = (e.L, 2, e.ntokens, e.H, e.D) if self.fmt == "vllm" else (e.L, 2, e.H, e.ntokens, e.D)
+        r = e.rec
+        shape = (r.L, 2, r.ntokens, r.H, r.D) if self.fmt == "vllm" else (r.L, 2, r.H, r.ntokens, r.D)
         out = torch.empty(shape, dtype=self.out_dtype(), device=torch.device("cuda", torch.cuda.current_device()))
-        if self.get_kv_into([key], KvView.from_blob(out, self.fmt), 0, e.ntokens) != 1:
+        if self.get_kv_into([key], KvView.from_blob(out, self.fmt), 0, r.ntokens) != 1:
             return None
         return out
 
@@ -517,7 +445,7 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
       * the index (key -> file, size, geometry) is rebuilt from the directory when the backend starts: headers are read
         and checked, damaged or foreign files are ignored -- a restart keeps the cache;
       * retrieve reads the files of the requested chunks with a small thread pool straight into page-locked blocks while
-        earlier waves upload and decode (disk || H2D || decode, lmcache_b200/pipeline.py fetch_decode)."""
+        earlier waves upload and decode (disk || H2D || decode, lmcache_b200/pipeline.py upload_decode)."""
 
     SUFFIX = ".b2kv"
 
@@ -531,7 +459,6 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
         super().__init__(config, metadata)
         self._io = ThreadPoolExecutor(max_workers=max(1, int(os.environ.get("LMCACHE_B200_DISK_THREADS", "4"))),
                                       thread_name_prefix="b200kv-disk")
-        self._inflight_reads = []               # (event, [blocks]) of uploads out of transient read blocks
         self._rebuild_index()
 
     # ---- index
@@ -541,7 +468,8 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
     def _rebuild_index(self) -> int:
         import os
 
-        from lmcache_b200.codec import check_header
+        from lmcache_b200.codec import parse_header
+        from lmcache_b200.pipeline import HostContainer
         n = 0
         for name in os.listdir(self.path):
             if not name.endswith(self.SUFFIX):
@@ -549,20 +477,15 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
             full = self.path + name
             try:
                 size = os.path.getsize(full)
-                if size < N.HEADER_BYTES:
-                    continue
                 with open(full, "rb") as f:
-                    head = f.read(N.HEADER_BYTES + N.MAX_PLANES)
-                hd = N.Header.from_buffer_copy(head[:N.HEADER_BYTES])
-                if hd.magic != N.MAGIC or hd.version not in (1, 2, 3) or hd.status != 0 or int(hd.total_bytes) != size:
+                    hd = parse_header(f.read(N.HEADER_BYTES + N.MAX_PLANES), size)
+                if int(hd.total_bytes) != size:
                     continue
-                check_header(hd, list(head[N.HEADER_BYTES:N.HEADER_BYTES + 2 * hd.L]) if hd.version == 3 else None)
             except (OSError, ValueError):
                 continue                         # damaged / foreign file: not part of the cache
             # "/" in a model name was written as "-": the key of a lookup goes through the same rule, so index by path
             e = _CEntry()
-            e.path, e.nbytes, e.ntokens = full, size, int(hd.ntokens)
-            e.L, e.H, e.D, e.max_dtype, e.coder = int(hd.L), int(hd.H), int(hd.D), int(hd.max_dtype), int(hd.version) - 1
+            e.path, e.rec = full, HostContainer(None, size, hd)
             e.ready.set()
             self._by_path[full] = e
             n += 1
@@ -576,35 +499,33 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
     def _lookup(self, key: CacheEngineKey):
         return self.dict.get(self._key_to_path(key))
 
-    def contains(self, key: CacheEngineKey) -> bool:
-        e = self._lookup(key)
-        return e is not None and not (e.ready.is_set() and e.error is not None)
-
-    def _ready_entry(self, key):
-        e = self._lookup(key)
-        if e is None:
-            return None
-        e.ready.wait()
-        return None if e.error is not None or e.path is None else e
-
     # ---- store: the pipeline's sink writes files instead of keeping blocks
     def _sink(self, slot, batch, c0, entries) -> None:
         import os
+
+        from lmcache_b200.pipeline import land
+        recs = []
         try:
-            self._land(slot, batch, entries)             # containers -> page-locked blocks, headers parsed
+            recs = land(self.slab, slot, batch)          # containers -> page-locked blocks, headers parsed
+        except BaseException as err:     # noqa: BLE001
             for e in entries:
+                e.error = err
+            raise
+        else:
+            for e, rec in zip(entries, recs):
+                e.rec = rec
                 tmp = e.path + ".tmp"
                 try:
                     with open(tmp, "wb") as f:
-                        f.write(e.blk.view())
+                        f.write(rec.blk.view())
                     os.replace(tmp, e.path)               # a file that exists is complete
                 except OSError as err:
                     e.error = err
         finally:
+            for rec in recs:
+                rec.blk.free()
+                rec.blk = None
             for e in entries:
-                if e.blk is not None:
-                    e.blk.free()
-                    e.blk = None
                 e.ready.set()                             # readers see the entry only once its file is in place
 
     def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True) -> int:
@@ -623,60 +544,43 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
 
     # ---- retrieve
     def _read_file(self, e: _CEntry):
-        blk = self.slab.alloc(e.nbytes)
+        """reader pool: the container file -> a fresh slab block -> its record, or None (a miss)"""
+        from lmcache_b200.pipeline import read_container
+        nbytes = e.rec.nbytes
+        blk = self.slab.alloc(nbytes)
         try:
             with open(e.path, "rb", buffering=0) as f:
                 got = f.readinto(blk.view())
-                while got is not None and 0 < got < e.nbytes:
+                while got is not None and 0 < got < nbytes:
                     more = f.readinto(blk.view()[got:])
                     if not more:
                         break
                     got += more
-            if got != e.nbytes:
+            if got != nbytes:
                 raise OSError("short read")
-            return blk, e.nbytes
         except OSError:
             blk.free()
             return None
+        return read_container(self.codec, blk, nbytes)
 
     def get_kv_into(self, keys, dst, dst_tok0: int, chunk_size: int) -> int:
-        from lmcache_b200.pipeline import UploadRing, fetch_decode
-        keep = []
-        for ev, blocks in self._inflight_reads:          # transient read blocks of earlier calls
-            if ev.query():
-                for b in blocks:
-                    b.free()
-            else:
-                keep.append((ev, blocks))
-        self._inflight_reads = keep
-        futs = []
+        import contextlib
+
+        from lmcache_b200.pipeline import fetched_in_order, upload_decode
+        self._release.sweep()                            # transient read blocks of earlier calls
+        reads = []
         for key in keys:
             e = self._ready_entry(key)
             if e is None:
                 break
-            futs.append(self._io.submit(self._read_file, e))
-        if not futs:
-            return 0
-        with torch.cuda.device(dst.device):
-            if self._upload is None or self._upload.device != dst.device:
-                self._upload = UploadRing(dst.device)
-        return fetch_decode(self.codec, self._upload, futs, dst, dst_tok0, chunk_size, self._inflight_reads)
+            reads.append(self._io.submit(self._read_file, e))
+        with contextlib.closing(fetched_in_order(reads)) as recs:
+            return upload_decode(self.codec, self._upload_ring(dst.device), recs, dst, dst_tok0, chunk_size,
+                                 self._release)
 
     def host_bytes(self) -> int:
-        return sum(e.nbytes for e in self.dict.values() if e.path is not None)
+        return sum(e.rec.nbytes for e in self.dict.values() if e.rec is not None)
 
     def close(self):
-        if self._closed:
-            return
-        self._pipe.close()
         self._io.shutdown(wait=True)
-        try:
-            torch.cuda.synchronize()
-        except Exception:       # noqa: BLE001
-            pass
-        for _, blocks in self._inflight_reads:
-            for b in blocks:
-                b.free()
-        self._inflight_reads = []
-        self._closed = True
-        self.slab.close()
+        super().close()              # the slab, transient read blocks included, goes after a device synchronise

@@ -20,6 +20,7 @@ import torch
 
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.logging import init_logger
+from lmcache_b200.pipeline import DeferredFree
 from lmcache_b200.storage_backend.abstract_backend import LMCBackendInterface
 from lmcache_b200.storage_backend.connector import CreateConnector
 from lmcache_b200.storage_backend.serde import CreateSerde
@@ -30,21 +31,6 @@ logger = init_logger(__name__)
 
 class RemoteBackendEndSignal:
     pass
-
-
-class _LazyFutures:
-    """list view over futures that are submitted on demand: entries past `issued` do not exist yet"""
-
-    def __init__(self, futs, issued):
-        self.futs, self.issued = futs, issued
-
-    def __len__(self):
-        return len(self.futs)
-
-    def __getitem__(self, i):
-        if isinstance(i, slice):
-            return [f for f in self.futs[i] if f is not None]
-        return self.futs[i]
 
 
 class LMCRemoteBackend(LMCBackendInterface):
@@ -74,9 +60,8 @@ class LMCRemoteBackend(LMCBackendInterface):
         self._slab = None
         self._pipe = None
         self._upload = None
-        self._copy_stream = None
-        self._inflight = []          # (event, [slab blocks]) of uploads still reading host memory
-        self._peek = None            # (key, block, nbytes): the container peek_geometry fetched, reused by get_kv_into
+        self._release = DeferredFree()   # fetched blocks that uploads may still read
+        self._peek = None            # (key, HostContainer): the container peek_geometry fetched, reused by get_kv_into
 
     @_lmcache_nvtx_annotate
     def put_worker(self):
@@ -168,51 +153,21 @@ class LMCRemoteBackend(LMCBackendInterface):
             self._slab = PinnedSlab()
         return self._slab
 
-    def _sweep(self, wait: bool = False) -> None:
-        keep = []
-        for ev, blocks in self._inflight:
-            if wait:
-                ev.synchronize()
-            if wait or ev.query():
-                for b in blocks:
-                    b.free()
-            else:
-                keep.append((ev, blocks))
-        self._inflight = keep
-
     # ---- put
     def _sink(self, slot, batch, c0, keys) -> None:
-        """store worker: one wave's containers -> page-locked slab (async copies on a copy stream), then k-way send"""
-        import ctypes
-
-        import torch as _t
-
-        from lmcache_b200 import _native as N
-        from lmcache_b200.codec import parse_header
-        dev = slot.dev.device
-        slab = self._host_slab()
-        with _t.cuda.device(dev):
-            if self._copy_stream is None or self._copy_stream.device != dev:
-                self._copy_stream = _t.cuda.Stream(device=dev)
-            cs = self._copy_stream
-            blocks = [slab.alloc(sz) for sz in batch.sizes]
-            try:
-                for j, (blk, sz) in enumerate(zip(blocks, batch.sizes)):
-                    N.check(N.lib().b200kv_copy_async(ctypes.c_void_p(blk.host_ptr),
-                                                      ctypes.c_void_p(slot.dev.data_ptr() + j * batch.stride), sz,
-                                                      cs.cuda_stream), "copy_async")
-                cs.synchronize()
-                for blk in blocks:
-                    parse_header(blk.view())          # raises on a nonzero encoder status: nothing corrupt leaves the host
-
-                def send(key, blk):
-                    self._conn().set(self._combine_key(key), blk.view())
-                    return key
-                for key in self._executor().map(send, keys, blocks):
-                    self.existing_keys.add(key)
-            finally:
-                for blk in blocks:
-                    blk.free()
+        """store worker: one wave's containers -> page-locked slab (land() raises on a nonzero encoder status: nothing
+        corrupt leaves the host), then k-way send"""
+        from lmcache_b200.pipeline import land
+        blocks = [rec.blk for rec in land(self._host_slab(), slot, batch)]
+        try:
+            def send(key, blk):
+                self._conn().set(self._combine_key(key), blk.view())
+                return key
+            for key in self._executor().map(send, keys, blocks):
+                self.existing_keys.add(key)
+        finally:
+            for blk in blocks:
+                blk.free()
 
     def _put_view_blocking(self, keys, view, tok_begin: int, chunk_size: int) -> None:
         n_tokens = view.ntokens - tok_begin
@@ -272,40 +227,33 @@ class LMCRemoteBackend(LMCBackendInterface):
         self.flush()
 
     # ---- get
-    def _fetch(self, key: CacheEngineKey, bound: int):
-        """pool thread: one GET into a fresh slab block -> (block, nbytes) or None on a miss"""
+    def _fetch(self, key: CacheEngineKey, bound: int, conn=None):
+        """one GET into a fresh slab block (on a pool thread: over that thread's connection) -> its HostContainer, or
+        None on a miss or a damaged / foreign container"""
+        from lmcache_b200.pipeline import read_container
         blk = self._host_slab().alloc(bound)
         try:
-            n = self._conn().get_into(self._combine_key(key), blk.host_ptr, bound)
+            n = (conn or self._conn()).get_into(self._combine_key(key), blk.host_ptr, bound)
         except Exception:      # noqa: BLE001 -- a broken connection is a miss
             n = None
         if not n:
             blk.free()
             return None
         blk.shrink(int(n))                      # the bound covers the largest container version; a v3 one is a tenth of it
-        return blk, int(n)
+        return read_container(self.deserializer.codec, blk, int(n))
 
     def peek_geometry(self, key: CacheEngineKey, fmt: str = "vllm"):
         """(L, H, D, output dtype) from the header of the first chunk's container.  The fetched container is kept for the
         get_kv_into call that follows, so a retrieve-only replica neither decodes nor fetches chunk 0 twice."""
         if not (self._striped() and hasattr(self.deserializer, "out_dtype")):
             return None
-        from lmcache_b200.codec import parse_header
-        blk = self._host_slab().alloc(256 << 20)          # the geometry is what we are asking for: be generous
-        try:
-            n = self.connection.get_into(self._combine_key(key), blk.host_ptr, blk.cap)
-            hd = parse_header(blk.view()[:n]) if n else None
-            if n:
-                blk.shrink(int(n))
-        except Exception:       # noqa: BLE001 -- broken connection / damaged container: a miss
-            hd = None
-        if hd is None:
-            blk.free()
+        rec = self._fetch(key, 256 << 20, self.connection)       # the geometry is what we are asking for: be generous
+        if rec is None:
             return None
         if self._peek is not None:
-            self._peek[1].free()
-        self._peek = (key, blk, int(n))
-        return (int(hd.L), int(hd.H), int(hd.D), self.deserializer.out_dtype())
+            self._peek[1].blk.free()
+        self._peek = (key, rec)
+        return (rec.L, rec.H, rec.D, self.deserializer.out_dtype())
 
     def get_kv_into(self, keys: List[CacheEngineKey], dst, dst_tok0: int, chunk_size: int) -> int:
         """Fetch consecutive chunks until the first miss and decode them straight into `dst` (chunk i lands at token
@@ -325,35 +273,31 @@ class LMCRemoteBackend(LMCBackendInterface):
         return len(blobs)
 
     def _get_striped(self, keys, dst, dst_tok0: int, chunk_size: int) -> int:
-        import torch as _t
+        import contextlib
+        from concurrent.futures import Future
 
-        from lmcache_b200.pipeline import UploadRing, fetch_decode, wave_chunks_default
-        self._sweep()
+        from lmcache_b200.pipeline import UploadRing, fetched_in_order, upload_decode, wave_chunks_default
+        self._release.sweep()
         bound = (self.deserializer.container_bound(dst.L, dst.H, dst.D, chunk_size) + 255) & ~255
         ex = self._executor()
-        window = max(2 * self._nconn, 2 * wave_chunks_default())       # fetches in flight ahead of the consumer
         peek, self._peek = self._peek, None
-        futs: list = [None] * len(keys)
-        issued = [0]
-
-        def on_more(i):
-            while issued[0] < min(len(keys), i + window):
-                k = issued[0]
-                if peek is not None and k == 0 and peek[0] == keys[0]:
-                    futs[0] = (peek[1], peek[2])                       # already in host memory (peek_geometry)
-                else:
-                    futs[k] = ex.submit(self._fetch, keys[k], bound)
-                issued[0] += 1
-        on_more(0)
         if peek is not None and not (keys and peek[0] == keys[0]):
-            peek[1].free()
-        with _t.cuda.device(dst.device):
-            if self._upload is None or self._upload.device != dst.device:
-                self._upload = UploadRing(dst.device)
-        # only what has been submitted can be awaited: hand fetch_decode the live list, it asks for more as it goes
-        n = fetch_decode(self.deserializer.codec, self._upload, _LazyFutures(futs, issued), dst, dst_tok0, chunk_size,
-                         self._inflight, on_more)
-        return n
+            peek[1].blk.free()
+            peek = None
+
+        def gets():
+            for i, key in enumerate(keys):
+                if i == 0 and peek is not None:
+                    f = Future()
+                    f.set_result(peek[1])                               # already in host memory (peek_geometry)
+                    yield f
+                else:
+                    yield ex.submit(self._fetch, key, bound)
+        if self._upload is None or self._upload.device != dst.device:
+            self._upload = UploadRing(dst.device)
+        window = max(2 * self._nconn, 2 * wave_chunks_default())       # fetches in flight ahead of the consumer
+        with contextlib.closing(fetched_in_order(gets(), window)) as recs:
+            return upload_decode(self.deserializer.codec, self._upload, recs, dst, dst_tok0, chunk_size, self._release)
 
     def close(self):
         if self.put_thread is not None and self.put_thread.is_alive():
@@ -365,10 +309,10 @@ class LMCRemoteBackend(LMCBackendInterface):
         if getattr(self, "_pool", None) is not None:
             self._pool.shutdown(wait=True)
             self._pool = None
-        if getattr(self, "_inflight", None):
-            self._sweep(wait=True)
+        if getattr(self, "_release", None) is not None:
+            self._release.drain()
         if getattr(self, "_peek", None) is not None:
-            self._peek[1].free()
+            self._peek[1].blk.free()
             self._peek = None
         for c in getattr(self, "_conns", []):
             try:

@@ -504,6 +504,37 @@ def test_hybrid_backend_write_through_and_fall_through(serde, lmserver, autorele
         assert torch.equal(got.view(torch.int16), want.view(torch.int16))
 
 
+@pytest.mark.parametrize("backend", ["cpu-cachegen", "disk", "lm-cachegen"])
+def test_kv_dtype_change_ends_the_match(backend, lmserver, tmp_path, autorelease):
+    """Chunks 0-3 stored from fp16 KV, chunks 4-7 from bf16 KV: every CacheGen tier returns exactly chunks 0-3, decoded
+    as the reference decodes them.  A retrieve ends at the first container whose KV dtype differs from chunk 0's, also
+    when the change falls on a wave boundary (waves of 4 chunks by default)."""
+    import ref_torch
+    from lmcache_b200.cache_engine import LMCacheEngine
+    from lmcache_b200.config import LMCacheEngineConfig
+    model = "mistralai/Mistral-7B-Instruct-v0.2"
+    cs, T = 256, 8 * 256
+    if backend == "cpu-cachegen":
+        cfg = LMCacheEngineConfig.from_legacy(chunk_size=cs, backend="cpu", local_serde="cachegen")
+    elif backend == "disk":
+        cfg = LMCacheEngineConfig.from_legacy(chunk_size=cs, backend="file://" + str(tmp_path / "kvdisk") + "/")
+    else:
+        cfg = LMCacheEngineConfig(cs, None, lmserver, "cachegen", False, False)
+    tokens = generate_tokens(T, "cuda")
+    kv = generate_kv_cache(T, "vllm", "cuda", 8, 2, 128)                # bf16
+    kv16 = tuple((k[:4 * cs].half(), v[:4 * cs].half()) for k, v in kv)
+    engine = autorelease(LMCacheEngine(cfg, dumb_metadata("vllm", model)))
+    engine.store(tokens[:4 * cs], kv16)
+    engine.store(tokens, kv, skip_existing=True)                         # chunks 4-7 are bf16 containers
+    r, m = engine.retrieve(tokens)
+    assert int(m.sum()) == 4 * cs and r[0][0].shape[0] == 4 * cs
+    kb, vb = (torch.tensor(b) for b in O.make_bins(model))
+    blob = torch.stack((torch.stack([k for k, _ in kv16]), torch.stack([v for _, v in kv16]))).permute(1, 0, 2, 3, 4)
+    want = torch.cat([ref_torch.roundtrip(c.contiguous(), kb, vb, "vllm") for c in torch.split(blob, cs, dim=2)], dim=2)
+    got = torch.stack([torch.stack(p) for p in r])
+    assert got.dtype == want.dtype and torch.equal(got.view(torch.int16), want.view(torch.int16))
+
+
 @pytest.mark.parametrize("backend", ["cuda", "cpu"])
 def test_fp32_kv_takes_the_generic_path(backend, autorelease):
     """the reference's local tiers accept any dtype (local_backend.py:95-100); the 16-bit kernels do not, so such KV goes
