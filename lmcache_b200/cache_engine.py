@@ -258,6 +258,7 @@ class LMCacheEngine:
                     start_chunk_idx = i
                     break
         n_chunks = 0
+        self._touch(chunk_hashes[:start_chunk_idx], fmt)
         if start_chunk_idx < len(chunk_hashes):
             keys = self._keys_of(chunk_hashes[start_chunk_idx:], fmt)
             kv_cuda = self._as_cuda_kv(kv_tensors_raw)
@@ -267,6 +268,7 @@ class LMCacheEngine:
                 chunks = self._pack_chunks_torch(kv_cuda, start_chunk_idx * self.chunk_size, fmt)
                 end_make_chunks = time.perf_counter()
                 n_chunks = self.engine_.batched_put(zip(keys, chunks), blocking=blocking)
+                self._touch(chunk_hashes, fmt)
                 logger.info(f"Stored/updated {n_chunks} chunks, total time {time.perf_counter() - start_time:.2f}s, "
                             f"make chunks time {end_make_chunks - start_time:.2f}s")
                 return
@@ -283,6 +285,8 @@ class LMCacheEngine:
                 n_chunks = self.engine_.batched_put(zip(keys, chunks), blocking=blocking)
         else:
             end_make_chunks = time.perf_counter()
+        if start_chunk_idx < len(chunk_hashes):
+            self._touch(chunk_hashes, fmt)
         end_time = time.perf_counter()
         logger.info(f"Stored/updated {n_chunks} chunks, total time {end_time - start_time:.2f}s, "
                     f"make chunks time {end_make_chunks - start_time:.2f}s")
@@ -305,10 +309,12 @@ class LMCacheEngine:
         fmt = self.metadata.fmt
         if fmt not in ("vllm", "huggingface"):
             raise ValueError(f"Invalid format: {fmt}")
-        chunk_hashes = self._prefix_hash(tokens, num_skip_chunk)
+        full_chain = self._prefix_hash(tokens)
+        chunk_hashes = full_chain[num_skip_chunk:]
         if self._fast_path() and len(chunk_hashes) > 0 and not getattr(self, "_wide_dtype", False):
             try:
-                return self._retrieve_into_blob(tokens, chunk_hashes, num_skip_tok, num_skip_chunk, ret_mask, fmt, st)
+                return self._retrieve_into_blob(tokens, chunk_hashes, num_skip_tok, num_skip_chunk, ret_mask, fmt, st,
+                                                full_chain)
             except TypeError:
                 self._wide_dtype = True      # chunks of a dtype the kernels do not move: per-chunk path from now on
         retrieved: List[torch.Tensor] = []
@@ -316,6 +322,7 @@ class LMCacheEngine:
             if chunk is None:
                 break
             retrieved.append(chunk)
+        self._touch(full_chain[:num_skip_chunk + len(retrieved)], fmt)
         if len(retrieved) == 0:
             logger.info("Retrieved 0 chunks")
             ret_mask[:] = False
@@ -370,11 +377,13 @@ class LMCacheEngine:
                 if not self.engine_.contains(self._make_key(h, fmt)):
                     start_chunk_idx = i
                     break
+        self._touch(chunk_hashes[:start_chunk_idx], fmt)
         if start_chunk_idx < len(chunk_hashes):
             view = KvView.from_paged(kv_caches, slot_mapping.cuda())
             self._geom = (view.L, view.H, view.D, view.dtype)
             keys = self._keys_of(chunk_hashes[start_chunk_idx:], fmt)
             self.engine_.put_kv_chunks(keys, view, start_chunk_idx * self.chunk_size, self.chunk_size, blocking=blocking)
+            self._touch(chunk_hashes, fmt)
 
     @_lmcache_nvtx_annotate
     @torch.no_grad()
@@ -403,7 +412,8 @@ class LMCacheEngine:
         extra = num_skip_tok - num_skip_chunk * cs
         ret_mask = torch.ones_like(tokens, dtype=torch.bool)
         ret_mask[:num_skip_tok] = False
-        keys = self._keys_of(self._prefix_hash(tokens, num_skip_chunk), "vllm")
+        full_chain = self._prefix_hash(tokens)
+        keys = self._keys_of(full_chain[num_skip_chunk:], "vllm")
         base = num_skip_chunk * cs
         view = KvView.from_paged(kv_caches, slots[base:])
         got_chunks, first = 0, 0
@@ -412,6 +422,7 @@ class LMCacheEngine:
             t0 = min(cs, len(tokens) - base)
             tmp = torch.empty((view.L, 2, t0, view.H, view.D), dtype=view.dtype, device=dev)
             if self.engine_.get_kv_into(keys[:1], KvView.from_blob(tmp, "vllm"), 0, cs) == 0:
+                self._touch(full_chain[:num_skip_chunk], "vllm")
                 ret_mask[:] = False
                 return ret_mask
             idx = slots[base + extra: base + t0]
@@ -421,12 +432,23 @@ class LMCacheEngine:
             got_chunks, first = 1, 1
         if len(keys) > first:
             got_chunks += self.engine_.get_kv_into(keys[first:], view, first * cs, cs)
+        self._touch(full_chain[:num_skip_chunk + got_chunks], "vllm")
         got = min(base + got_chunks * cs, len(tokens))
         if got <= num_skip_tok:
             ret_mask[:] = False
         else:
             ret_mask[got:] = False
         return ret_mask
+
+    def _touch(self, chunk_hashes, fmt: str) -> None:
+        """Recency update for a bounded local tier (lmcache_b200/eviction.py): one call with the keys of a chain prefix,
+        chunk 0 first -- every key of a stored sequence, the skipped and hit keys of a retrieve.  Touching a chunk only
+        together with all of its predecessors is what keeps a tier's eviction from cutting a chain in the middle.  A store
+        touches the prefix its scan matched (possibly none) right before it stores the rest: the tier protects what was
+        touched since then while that store lands."""
+        f = getattr(self.engine_, "touch", None)
+        if f is not None:
+            f(self._keys_of(chunk_hashes, fmt))
 
     # ------------------------------------------------------------------ native fast paths
     def _fast_path(self) -> bool:
@@ -437,7 +459,7 @@ class LMCacheEngine:
         """(L, H, D, dtype) of this engine's chunks, learnt from the first store / a probe get."""
         return getattr(self, "_geom", None)
 
-    def _retrieve_into_blob(self, tokens, chunk_hashes, num_skip_tok, num_skip_chunk, ret_mask, fmt, st):
+    def _retrieve_into_blob(self, tokens, chunk_hashes, num_skip_tok, num_skip_chunk, ret_mask, fmt, st, full_chain):
         """retrieve() without per-chunk tensors or torch.cat: the backend decodes / uploads every hit chunk straight
         into one preallocated blob; the suffix-mask trim of the first chunk is a view offset, not a copy."""
         keys = self._keys_of(chunk_hashes, fmt)
@@ -455,6 +477,7 @@ class LMCacheEngine:
                     geom = ((first.shape[0], first.shape[3], first.shape[4]) if fmt == "vllm" else
                             (first.shape[0], first.shape[2], first.shape[4])) + (first.dtype,)
             if geom is None:
+                self._touch(full_chain[:num_skip_chunk], fmt)
                 logger.info("Retrieved 0 chunks")
                 ret_mask[:] = False
                 return (), ret_mask
@@ -468,6 +491,7 @@ class LMCacheEngine:
         device = torch.device("cuda", torch.cuda.current_device())
         blob = torch.empty(shape, dtype=dtype, device=device)
         n = self.engine_.get_kv_into(keys, KvView.from_blob(blob, fmt), 0, self.chunk_size)
+        self._touch(full_chain[:num_skip_chunk + n], fmt)
         if n == 0:
             logger.info("Retrieved 0 chunks")
             ret_mask[:] = False

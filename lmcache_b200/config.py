@@ -33,6 +33,10 @@ class LMCacheEngineConfig:
     # (local_backend.py:95-100); "cachegen" = CacheGen containers in page-locked memory (LMCLocalCompressedBackend).
     # The environment variable LMCACHE_B200_LOCAL_SERDE sets the default for configurations that do not name it.
     local_serde: Optional[str] = None
+    # not in the reference: the most bytes the local CacheGen tier keeps (slab blocks of the host tier, .b2kv files of the
+    # disk tier); beyond it chunks are evicted from the tail of the coldest chain (lmcache_b200/eviction.py).  None = no
+    # bound.  Only the two CacheGen tiers honour it (CreateStorageBackend rejects it elsewhere).
+    local_capacity_bytes: Optional[int] = None
 
     def __post_init__(self):
         if self.local_serde is None:
@@ -40,19 +44,24 @@ class LMCacheEngineConfig:
             self.local_serde = os.environ.get("LMCACHE_B200_LOCAL_SERDE") or None
         if self.local_serde not in (None, "cachegen"):
             raise ValueError(f"Invalid local serde: {self.local_serde}")
+        c = self.local_capacity_bytes
+        if c is not None and (isinstance(c, bool) or not isinstance(c, int) or c <= 0):
+            raise ValueError(f"Invalid local capacity: {c!r} (a positive number of bytes, or None)")
 
     @staticmethod
     def from_defaults(chunk_size: int = 256, local_device: str = "cuda",
                       remote_url: str = "redis://localhost:6379", remote_serde: str = "torch",
                       pipelined_backend: bool = False, save_decode_cache: bool = False,
-                      local_serde: Optional[str] = None) -> "LMCacheEngineConfig":
+                      local_serde: Optional[str] = None,
+                      local_capacity_bytes: Optional[int] = None) -> "LMCacheEngineConfig":
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
-                                   save_decode_cache, local_serde)
+                                   save_decode_cache, local_serde, local_capacity_bytes)
 
     @staticmethod
     def from_legacy(chunk_size: int = 256, backend: str = "cuda", persist_path: Optional[str] = None,
                     remote_serde: Optional[str] = "torch", pipelined_backend: bool = False,
-                    save_decode_cache: bool = False, local_serde: Optional[str] = None) -> "LMCacheEngineConfig":
+                    save_decode_cache: bool = False, local_serde: Optional[str] = None,
+                    local_capacity_bytes: Optional[int] = None) -> "LMCacheEngineConfig":
         """backend: "cpu" | "cuda" | "file://<dir>/" | "<scheme>://<host>:<port>" (config.py:51-82)."""
         local_device: Optional[str] = None
         remote_url: Optional[str] = None
@@ -63,7 +72,7 @@ class LMCacheEngineConfig:
         elif _URL_RE.match(backend):
             remote_url = backend
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
-                                   save_decode_cache, local_serde)
+                                   save_decode_cache, local_serde, local_capacity_bytes)
 
     @staticmethod
     def from_file(file_path: str) -> "LMCacheEngineConfig":
@@ -77,6 +86,7 @@ class LMCacheEngineConfig:
         pipelined_backend = cfg.get("pipelined_backend", False)
         save_decode_cache = cfg.get("save_decode_cache", False)
         local_serde = cfg.get("local_serde", None)
+        local_capacity_bytes = cfg.get("local_capacity_bytes", None)
 
         if local_device in ("cpu", "cuda", None):
             pass
@@ -89,7 +99,7 @@ class LMCacheEngineConfig:
             raise ValueError(f"Invalid remote storage url: {remote_url}")
 
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
-                                   save_decode_cache, local_serde)
+                                   save_decode_cache, local_serde, local_capacity_bytes)
 
 
 class GlobalConfig:

@@ -251,13 +251,15 @@ def _d2h_stream(device: torch.device) -> torch.cuda.Stream:
     return torch.cuda.Stream(device=device)
 
 
-def land(slab, slot: WaveSlot, batch) -> List[HostContainer]:
+def land(slab, slot: WaveSlot, batch, blocks: Optional[list] = None) -> List[HostContainer]:
     """Store-pipeline sink side: copy a finished wave's containers out of slot.dev into fresh blocks of `slab` (exactly
     their bytes, on the device's copy stream), wait for the copies, and parse every header.  Raises -- with every block
-    freed -- when a copy fails or a container carries an encoder error."""
+    freed -- when a copy fails or a container carries an encoder error.  `blocks`: blocks the caller allocated for the
+    first len(blocks) containers (a bounded tier); only those are landed."""
     dev = slot.dev.device
     cs = _d2h_stream(dev)
-    blocks = [slab.alloc(size) for size in batch.sizes]
+    if blocks is None:
+        blocks = [slab.alloc(size) for size in batch.sizes]
     try:
         with torch.cuda.device(dev):
             try:
@@ -312,6 +314,11 @@ class DeferredFree:
                 else:
                     keep.append((ev, blocks))
             self._held = keep
+
+    def pending(self) -> int:
+        """groups still held"""
+        with self._lock:
+            return len(self._held)
 
     def drain(self) -> None:
         """Blocking: free everything once its copies are done (a tier's close())."""

@@ -24,6 +24,11 @@ def _default_segment_bytes() -> int:
     return int(os.environ.get("LMCACHE_B200_SLAB_SEGMENT_MB", "1024")) << 20
 
 
+def block_bytes(nbytes: int) -> int:
+    """slab bytes a block of nbytes takes (its `cap`)"""
+    return max(ALIGN, (int(nbytes) + ALIGN - 1) // ALIGN * ALIGN)
+
+
 class SlabBlock:
     """One allocation: `nbytes` at `offset` of segment `seg`; host_ptr / dev_ptr are absolute addresses."""
     __slots__ = ("slab", "seg", "offset", "nbytes", "cap")
@@ -85,12 +90,19 @@ class _FreeList:
         return sum(self.lens)
 
 
+class SlabFull(MemoryError):
+    """No free extent fits the request and the slab may not reserve another segment."""
+
+
 class PinnedSlab:
 
-    def __init__(self, segment_bytes: Optional[int] = None, alloc_fn=None):
+    def __init__(self, segment_bytes: Optional[int] = None, alloc_fn=None, max_segments: Optional[int] = None):
         """alloc_fn(nbytes) -> object with host_ptr / dev_ptr / view(offset, nbytes) / close(); defaults to the
-        library's page-locked allocator (lmcache_b200.codec.PinnedBuffer).  Tests pass a plain-memory stand-in."""
+        library's page-locked allocator (lmcache_b200.codec.PinnedBuffer).  Tests pass a plain-memory stand-in.
+        max_segments: the slab's byte budget in segments (None: unbounded); beyond it `alloc` raises SlabFull instead of
+        page-locking more memory, and requests larger than a segment always do."""
         self.segment_bytes = int(segment_bytes or _default_segment_bytes())
+        self.max_segments = max_segments
         self._alloc_fn = alloc_fn
         self._segs: list = []
         self._free: List[_FreeList] = []
@@ -109,18 +121,20 @@ class PinnedSlab:
         """Make sure at least nbytes are available without a further cudaHostAlloc (start-up warm-up)."""
         with self._lock:
             have = sum(f.free_bytes() for f in self._free)
-            while have < nbytes:
+            while have < nbytes and (self.max_segments is None or len(self._segs) < self.max_segments):
                 self._new_segment(self.segment_bytes)
                 have += self.segment_bytes
 
     def alloc(self, nbytes: int) -> SlabBlock:
-        cap = max(ALIGN, (int(nbytes) + ALIGN - 1) // ALIGN * ALIGN)
+        cap = block_bytes(nbytes)
         with self._lock:
             for s, fl in enumerate(self._free):
                 off = fl.take(cap)
                 if off is not None:
                     self.bytes_in_use += cap
                     return SlabBlock(self, s, off, int(nbytes), cap)
+            if self.max_segments is not None and (len(self._segs) >= self.max_segments or cap > self.segment_bytes):
+                raise SlabFull(f"no free extent of {cap} bytes within {self.max_segments} segments")
             s = self._new_segment(max(self.segment_bytes, cap))       # oversized requests get their own segment
             off = self._free[s].take(cap)
             self.bytes_in_use += cap

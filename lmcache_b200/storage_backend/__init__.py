@@ -5,6 +5,14 @@ from lmcache_b200.storage_backend.abstract_backend import LMCBackendInterface
 
 def CreateStorageBackend(config: LMCacheEngineConfig, metadata: LMCacheEngineMetadata) -> LMCBackendInterface:
     local, remote = config.local_device, config.remote_url
+    if config.local_capacity_bytes is not None:
+        # only the CacheGen tiers evict: the raw tiers keep views of one shared buffer per store, so evicting one view
+        # would free nothing; a remote-only configuration has no local tier
+        if local is None:
+            raise ValueError("local_capacity_bytes needs a local tier; a remote-only configuration has none")
+        if local in ("cpu", "cuda") and not (local == "cpu" and config.local_serde == "cachegen"):
+            raise ValueError(f"local_capacity_bytes is honoured by the CacheGen tiers only (local_device='cpu' with "
+                             f"local_serde='cachegen', or a directory), not by local_device={local!r}")
     if local is None and isinstance(remote, str):
         from lmcache_b200.storage_backend.remote_backend import LMCPipelinedRemoteBackend, LMCRemoteBackend
         return (LMCPipelinedRemoteBackend if config.pipelined_backend else LMCRemoteBackend)(config, metadata)

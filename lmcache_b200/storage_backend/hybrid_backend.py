@@ -20,8 +20,9 @@ class LMCHybridBackend(LMCBackendInterface):
     def __init__(self, config: LMCacheEngineConfig, metadata: LMCacheEngineMetadata):
         super().__init__()
         from lmcache_b200.storage_backend import CreateStorageBackend
+        # a capacity bounds the local tier (one of the CacheGen tiers); chunks it evicts are still served by the remote one
         local_cfg = LMCacheEngineConfig(config.chunk_size, config.local_device, None, None, False, config.save_decode_cache,
-                                        config.local_serde)
+                                        config.local_serde, config.local_capacity_bytes)
         remote_cfg = LMCacheEngineConfig(config.chunk_size, None, config.remote_url, config.remote_serde,
                                          config.pipelined_backend, config.save_decode_cache, None)
         self.local_store = CreateStorageBackend(local_cfg, metadata)
@@ -63,6 +64,11 @@ class LMCHybridBackend(LMCBackendInterface):
         if n < len(keys):
             n += self.remote_store.get_kv_into(keys[n:], dst, dst_tok0 + n * chunk_size, chunk_size)
         return n
+
+    def touch(self, keys) -> None:
+        f = getattr(self.local_store, "touch", None)
+        if f is not None:
+            f(keys)
 
     def peek_geometry(self, key: CacheEngineKey, fmt: str = "vllm"):
         for store in (self.local_store, self.remote_store):

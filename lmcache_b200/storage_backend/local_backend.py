@@ -251,15 +251,30 @@ class LMCLocalBackend(LMCBackendInterface):
 
 
 # ---------------------------------------------------------------------------------------------- compressed host tier
+class _Store:
+    """One put_kv_chunks call.  A bounded tier never evicts a call's entries to make room for its later chunks, nor an
+    entry touched since `since` -- the latest touch on the calling thread, which for LMCacheEngine is the prefix its
+    skip_existing scan matched: evicting that prefix would make the chunks being stored unreachable.  Once one of its
+    containers does not fit, the rest are dropped as well: behind a gap they could never be hit."""
+    __slots__ = ("dropped", "since")
+
+    def __init__(self, since: Optional[int] = None):
+        self.dropped = False
+        self.since = since
+
+
 class _CEntry:
     """One stored chunk: its container's record (pipeline.HostContainer) plus the tier's bookkeeping."""
-    __slots__ = ("rec", "path", "ready", "error")
+    __slots__ = ("rec", "path", "ready", "error", "store", "pins", "retired")
 
-    def __init__(self):
+    def __init__(self, store: Optional[_Store] = None):
         self.rec = None                      # None until the container has landed (and again once it is retired)
         self.path = None                     # disk tier: the container's file (then rec.blk is None)
         self.ready = threading.Event()       # set by the store worker once the container is in host memory
         self.error: Optional[BaseException] = None
+        self.store = store                   # the put_kv_chunks call that made it (None: found on disk at start-up)
+        self.pins = 0                        # retrieves between lookup and upload: the block is neither evicted nor freed
+        self.retired = False                 # retired while pinned: the last unpin hands the block to DeferredFree
 
     # read by reports (bench.py's e2e counts the container bytes a retrieve uploads)
     @property
@@ -281,20 +296,27 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
                 previous wave's containers -- exactly their bytes -- into the page-locked slab on a copy stream;
       retrieve  the containers of wave i+1 are uploaded on a copy stream while wave i is decoded straight into the
                 destination; slot reuse is ordered by events, the host never waits.
-    Every container lives in one PinnedSlab (one cudaHostAlloc per GiB, not one per put)."""
+    Every container lives in one PinnedSlab (one cudaHostAlloc per GiB, not one per put).
+
+    With config.local_capacity_bytes the slab never holds more than that many bytes: the store worker evicts chunks in
+    the order of lmcache_b200.eviction.PrefixLRU before it lands a wave, and drops what does not fit even then."""
 
     def __init__(self, config: LMCacheEngineConfig, metadata):
         super().__init__()
         from lmcache_b200.codec import CacheGenCodec
+        from lmcache_b200.eviction import PrefixLRU
         from lmcache_b200.pipeline import DeferredFree, EncodePipeline, UploadRing
-        from lmcache_b200.slab import PinnedSlab
         N.require_cuda()
         self.chunk_size = config.chunk_size
         self.fmt = metadata.fmt
         if self.fmt not in ("vllm", "huggingface"):
             raise ValueError(f"Invalid format: {self.fmt}")
         self.codec = CacheGenCodec(metadata.model_name)      # ValueError for models outside the bin table
-        self.slab = PinnedSlab()
+        self.capacity: Optional[int] = config.local_capacity_bytes
+        self.slab = self._new_slab()
+        self._order = PrefixLRU()             # eviction order of a bounded tier, keyed like self.dict
+        self._touched = threading.local()     # .tick: the order's tick after this thread's latest touch
+        self.evicted = 0                      # chunks evicted so far (reports)
         self.dict: Dict[CacheEngineKey, _CEntry] = {}
         self.update_lock = threading.Lock()
         self._pipe = EncodePipeline(self.codec, self._sink)
@@ -302,12 +324,22 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         self._release = DeferredFree()        # blocks uploads may still read: retired entries, the disk tier's file reads
         self._closed = False
 
+    def _new_slab(self):
+        """bounded: segments of min(LMCACHE_B200_SLAB_SEGMENT_MB, capacity), at most ceil(capacity / segment) of them"""
+        from lmcache_b200.slab import PinnedSlab, _default_segment_bytes
+        if self.capacity is None:
+            return PinnedSlab()
+        seg = min(_default_segment_bytes(), self.capacity)
+        return PinnedSlab(seg, max_segments=-(-self.capacity // seg))
+
     # ------------------------------------------------------------------ store
     def _sink(self, slot, batch, c0, entries) -> None:
         """store pipeline sink: land the wave in host memory, then publish the entries (readers wait on `ready`)"""
         from lmcache_b200.pipeline import land
         try:
-            for e, rec in zip(entries, land(self.slab, slot, batch)):
+            blocks = None if self.capacity is None else self._make_room(batch.sizes, entries)
+            recs = land(self.slab, slot, batch, blocks) if blocks is None or blocks else []
+            for e, rec in zip(entries, recs):
                 e.rec = rec
         except BaseException as err:     # noqa: BLE001 -- the entries become misses; the job reports the error
             for e in entries:
@@ -317,15 +349,88 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
             for e in entries:
                 e.ready.set()
 
+    def _make_room(self, sizes, entries) -> list:
+        """Bounded tier, on the store worker: a slab block for each container of the wave, in chunk order, while the
+        slab's bytes in use stay within the capacity; chunks are evicted until each one fits.  The first container that
+        does not fit even then is dropped with every later chunk of its store: their entries become misses."""
+        from lmcache_b200.slab import SlabFull, block_bytes
+        store = entries[0].store
+        blocks = []
+        for size in sizes:
+            blk = None
+            while not store.dropped:
+                if self.slab.bytes_in_use + block_bytes(size) <= self.capacity:
+                    try:
+                        blk = self.slab.alloc(size)
+                        break
+                    except SlabFull:             # first-fit fragmentation: free more, never open another segment
+                        pass
+                if self._release.pending():
+                    self._release.sweep(wait=True)    # victims an upload may still read: wait here, off the caller's thread
+                elif not self._evict_one(store):
+                    store.dropped = True
+            if blk is None:
+                break
+            blocks.append(blk)
+        for e in entries[len(blocks):]:
+            e.error = MemoryError(f"chunk does not fit within local_capacity_bytes={self.capacity}")
+        return blocks
+
+    def _evictable(self, k, store: Optional[_Store]) -> bool:
+        e = self.dict.get(k)
+        if e is None:
+            return True
+        if not e.ready.is_set() or e.pins:
+            return False
+        return store is None or (e.store is not store and (store.since is None or self._order.stamp(k)[0] < store.since))
+
+    def _evict_one(self, store: Optional[_Store]) -> bool:
+        """Evict the eligible entry with the smallest stamp (never one of `store`'s, a pinned one or one that has not
+        landed).  False: there is none."""
+        with self.update_lock:
+            k = self._order.victim(lambda k: self._evictable(k, store))
+            if k is None:
+                return False
+            self._order.discard(k)
+            e = self.dict.pop(k, None)
+            if e is not None:
+                self.evicted += 1
+        if e is not None:
+            self._drop(e)
+        return True
+
+    def _drop(self, e: _CEntry) -> None:
+        """an evicted entry's bytes leave the tier"""
+        self._retire(e)
+
     def _retire(self, e: _CEntry) -> None:
-        rec, e.rec = e.rec, None
-        if rec is not None:
+        with self.update_lock:
+            if e.pins:
+                e.retired = True                 # a retrieve still holds it: the last unpin frees the block
+                return
+            rec, e.rec = e.rec, None
+        if rec is not None and rec.blk is not None:
             self._release.add(rec.last_read, [rec.blk])
+
+    def touch(self, keys) -> None:
+        """Recency update of one call: `keys` in chain order, chunk 0 first (LMCacheEngine passes every key of a stored
+        sequence and every key of a retrieved prefix, lmcache_b200/eviction.py).  Keys the tier does not hold are
+        skipped.  No-op on an unbounded tier."""
+        if self.capacity is None:
+            return
+        dks = [self._dict_key(k) for k in keys]
+        with self.update_lock:
+            self._order.touch([k for k in dks if k in self.dict])
+            self._touched.tick = self._order.tick
+
+    def _new_store(self) -> _Store:
+        return _Store(getattr(self._touched, "tick", None) if self.capacity is not None else None)
 
     def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True) -> int:
         # `keys` may be lazy (the engine's hash chain produces key i after keys 0..i-1): the encode waves
         # need no keys, so they are enqueued first; the entries are published as their keys arrive.  Readers wait on `ready`.
-        entries = [_CEntry() for _ in range(len(keys))]
+        store = self._new_store()
+        entries = [_CEntry(store) for _ in range(len(keys))]
         job = self._pipe.submit(view, tok_begin, chunk_size, entries)
         old = []
         for k, e in zip(keys, entries):
@@ -334,6 +439,7 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
                 if prev is not None:
                     old.append(prev)
                 self.dict[k] = e
+        self.touch(keys)                            # one call, positions relative to tok_begin; the engine's touch follows
         for prev in old:                            # an overwritten container leaves once nobody reads it any more
             prev.ready.wait()
             self._retire(prev)
@@ -351,8 +457,11 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         self.put_kv_chunks([key], view, 0, view.ntokens, blocking=blocking)
 
     # ------------------------------------------------------------------ lookup
+    def _dict_key(self, key: CacheEngineKey):
+        return key
+
     def _lookup(self, key: CacheEngineKey) -> Optional[_CEntry]:
-        return self.dict.get(key)
+        return self.dict.get(self._dict_key(key))
 
     def contains(self, key: CacheEngineKey) -> bool:
         e = self._lookup(key)
@@ -384,8 +493,39 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         from lmcache_b200.pipeline import upload_decode
         # keys may be lazy (the hash chain is still running): every full wave is uploaded and decoded as soon as its
         # keys exist, while the chain works on the later chunks.  The records were checked when they landed.
-        recs = (None if e is None else e.rec for e in map(self._ready_entry, keys))
-        return upload_decode(self.codec, self._upload_ring(dst.device), recs, dst, dst_tok0, chunk_size)
+        pinned = []
+        try:
+            return upload_decode(self.codec, self._upload_ring(dst.device), self._pinned_records(keys, pinned), dst,
+                                 dst_tok0, chunk_size)
+        finally:
+            self._unpin(pinned)             # every wave's upload event is recorded in its records' last_read by now
+
+    def _pinned_records(self, keys, pinned: list):
+        """the records of `keys` in order (None: a miss), each entry pinned from its lookup on: neither eviction nor an
+        overwrite frees its block before the upload that reads it is enqueued and recorded"""
+        for key in keys:
+            dk = self._dict_key(key)
+            with self.update_lock:
+                e = self.dict.get(dk)
+                if e is not None:
+                    e.pins += 1
+                    pinned.append(e)
+            if e is None:
+                yield None
+                return
+            e.ready.wait()
+            yield None if e.error is not None else e.rec
+
+    def _unpin(self, pinned: list) -> None:
+        free = []
+        with self.update_lock:
+            for e in pinned:
+                e.pins -= 1
+                if e.pins == 0 and e.retired and e.rec is not None:
+                    free.append(e.rec)
+                    e.rec = None
+        for rec in free:
+            self._release.add(rec.last_read, [rec.blk])
 
     def _upload_ring(self, device):
         from lmcache_b200.pipeline import UploadRing
@@ -404,12 +544,13 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         out = torch.empty(shape, dtype=self.out_dtype(), device=torch.device("cuda", torch.cuda.current_device()))
         if self.get_kv_into([key], KvView.from_blob(out, self.fmt), 0, r.ntokens) != 1:
             return None
+        self.touch([key])
         return out
 
     def reserve_host(self, nbytes: int) -> None:
         """Page-lock at least nbytes of slab up front (a cudaHostAlloc of 1 GiB takes ~0.3 s: better at start-up than
-        inside a store)."""
-        self.slab.reserve(int(nbytes))
+        inside a store).  A bounded tier reserves at most its capacity."""
+        self.slab.reserve(int(nbytes) if self.capacity is None else min(int(nbytes), self.capacity))
 
     def host_bytes(self) -> int:
         """bytes of containers currently held (for reports)"""
@@ -445,7 +586,11 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
       * the index (key -> file, size, geometry) is rebuilt from the directory when the backend starts: headers are read
         and checked, damaged or foreign files are ignored -- a restart keeps the cache;
       * retrieve reads the files of the requested chunks with a small thread pool straight into page-locked blocks while
-        earlier waves upload and decode (disk || H2D || decode, lmcache_b200/pipeline.py upload_decode)."""
+        earlier waves upload and decode (disk || H2D || decode, lmcache_b200/pipeline.py upload_decode);
+      * with config.local_capacity_bytes the .b2kv files total at most that many bytes: the store worker removes files in
+        the order of lmcache_b200.eviction.PrefixLRU before it writes one.  A reader that loses the race to a removal gets
+        an OSError or a short read, which is a miss.  At start-up the order is seeded oldest file (mtime) first, and a
+        directory over the capacity is evicted down to it; the prefix guarantee holds within one process only."""
 
     SUFFIX = ".b2kv"
 
@@ -456,10 +601,16 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
         assert path is not None, "Need to specify local path if when using LMCLocalDiskBackend"
         self.path = path if path.endswith("/") else path + "/"
         os.makedirs(self.path, exist_ok=True)
+        self._file_bytes: Dict[str, int] = {}        # bounded tier: size of every indexed file
+        self._disk_bytes = 0                         # ... and their total
         super().__init__(config, metadata)
         self._io = ThreadPoolExecutor(max_workers=max(1, int(os.environ.get("LMCACHE_B200_DISK_THREADS", "4"))),
                                       thread_name_prefix="b200kv-disk")
         self._rebuild_index()
+
+    def _new_slab(self):
+        from lmcache_b200.slab import PinnedSlab
+        return PinnedSlab()                  # transient blocks only: the capacity bounds the files
 
     # ---- index
     def _key_to_path(self, key: CacheEngineKey) -> str:
@@ -470,13 +621,14 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
 
         from lmcache_b200.codec import parse_header
         from lmcache_b200.pipeline import HostContainer
-        n = 0
+        found = []
         for name in os.listdir(self.path):
             if not name.endswith(self.SUFFIX):
                 continue
             full = self.path + name
             try:
-                size = os.path.getsize(full)
+                st = os.stat(full)
+                size = st.st_size
                 with open(full, "rb") as f:
                     hd = parse_header(f.read(N.HEADER_BYTES + N.MAX_PLANES), size)
                 if int(hd.total_bytes) != size:
@@ -487,17 +639,43 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
             e = _CEntry()
             e.path, e.rec = full, HostContainer(None, size, hd)
             e.ready.set()
+            found.append((st.st_mtime_ns, full, e))
+        found.sort(key=lambda f: f[:2])                  # oldest first: the eviction order of a bounded tier
+        for _, full, e in found:
             self._by_path[full] = e
-            n += 1
-        return n
+            if self.capacity is not None:
+                self._order.touch([full])
+                self._file_bytes[full] = e.rec.nbytes
+                self._disk_bytes += e.rec.nbytes
+        while self.capacity is not None and self._disk_bytes > self.capacity and self._evict_one(None):
+            pass
+        return len(self.dict)
 
     # the dict is keyed by file path: CacheEngineKey -> path is many-to-one ("/" and "-"), exactly as in the reference
     @property
     def _by_path(self):
         return self.dict
 
-    def _lookup(self, key: CacheEngineKey):
-        return self.dict.get(self._key_to_path(key))
+    def _dict_key(self, key: CacheEngineKey) -> str:
+        return self._key_to_path(key)
+
+    def _drop(self, e: _CEntry) -> None:
+        """evicted: the file goes (on the store worker, or at start-up)"""
+        import os
+        try:
+            os.remove(e.path)
+        except OSError:
+            pass
+        self._disk_bytes -= self._file_bytes.pop(e.path, 0)
+
+    def _make_file_room(self, e: _CEntry, nbytes: int) -> bool:
+        """bounded tier: evict until the file of `e` (replacing any file at its path) fits within the capacity"""
+        while not e.store.dropped:
+            if self._disk_bytes - self._file_bytes.get(e.path, 0) + nbytes <= self.capacity:
+                return True
+            if not self._evict_one(e.store):
+                e.store.dropped = True
+        return False
 
     # ---- store: the pipeline's sink writes files instead of keeping blocks
     def _sink(self, slot, batch, c0, entries) -> None:
@@ -514,6 +692,9 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
         else:
             for e, rec in zip(entries, recs):
                 e.rec = rec
+                if self.capacity is not None and not self._make_file_room(e, rec.nbytes):
+                    e.error = OSError(f"chunk does not fit within local_capacity_bytes={self.capacity}")
+                    continue
                 tmp = e.path + ".tmp"
                 try:
                     with open(tmp, "wb") as f:
@@ -521,6 +702,10 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
                     os.replace(tmp, e.path)               # a file that exists is complete
                 except OSError as err:
                     e.error = err
+                    continue
+                if self.capacity is not None:
+                    self._disk_bytes += rec.nbytes - self._file_bytes.get(e.path, 0)
+                    self._file_bytes[e.path] = rec.nbytes
         finally:
             for rec in recs:
                 rec.blk.free()
@@ -529,7 +714,8 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
                 e.ready.set()                             # readers see the entry only once its file is in place
 
     def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True) -> int:
-        entries = [_CEntry() for _ in keys]
+        store = self._new_store()
+        entries = [_CEntry(store) for _ in keys]
         for k, e in zip(keys, entries):
             e.path = self._key_to_path(k)
             e.ready.clear()
@@ -538,6 +724,7 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
                 self.dict[e.path] = e                     # an overwritten chunk's file is replaced atomically by the rename
         # the parent's sink sets `ready` before the file exists: keep readers out until the file is written
         job = self._pipe.submit(view, tok_begin, chunk_size, entries)
+        self.touch(keys)
         if blocking:
             job.wait()
         return len(keys)
