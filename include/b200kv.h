@@ -33,7 +33,10 @@ extern "C" {
 
 #define B200KV_VERSION 4           /* ABI version; 2: b200kv_kv_desc.slot_map; 3: coder selection, decode status, total_bytes;
                                     * 4: compact container (B200KV_CODER_RANS_COMPACT), b200kv_container_layout_v,
-                                    *    b200kv_sha256_chain_ready */
+                                    *    b200kv_sha256_chain_ready.  Added since without changing anything that
+                                    *    existed (the number stays 4; a caller that needs them looks the symbols up,
+                                    *    e.g. dlsym): b200kv_decode_plan / b200kv_decode_layers, b200kv_plane_offsets,
+                                    *    b200kv_plane_offsets_device, b200kv_copy_batch_async */
 #define B200KV_CODER_AC 0          /* payload = torchac-lineage arithmetic coder; container version 1 */
 #define B200KV_CODER_RANS 1        /* payload = rANS, 32-bit state / 16-bit renormalisation; container version 2 */
 #define B200KV_CODER_RANS_COMPACT 2 /* rANS as in version 2, compact side information; container version 3 (chunks of
@@ -115,6 +118,16 @@ int b200kv_container_layout(int32_t L, int32_t H, int32_t D, int32_t ntokens, b2
 /* Same for the container `coder` produces (B200KV_CODER_RANS_COMPACT: off_cdf is the nb map, there is no CDF section). */
 int b200kv_container_layout_v(int32_t L, int32_t H, int32_t D, int32_t ntokens, int32_t coder, b200kv_layout* out);
 
+/* Host side: where each plane's streams lie in a version-3 container in host memory (its fixed sections are read, nothing
+ * else): out[0..2L], plane p (keys of layer p, then values of layer p - L) is bytes [out[p], out[p+1]) of the container,
+ * out[0] = layout.off_payload.  Returns 0, 1 when the half-lengths do not add up to header.total_bytes (damaged), <0 for
+ * anything that is not a version-3 container. */
+int b200kv_plane_offsets(const void* container, int64_t nbytes, int64_t* out, int32_t n_out);
+/* Same for n containers in DEVICE memory, container j at containers + j*stride (the encoder's output, before it leaves the
+ * device): row j of out (DEVICE or mapped-host int64[n][B200KV_MAX_PLANES + 1]) gets the 2L + 1 offsets, or -1 in its
+ * entry 0 for a container that is not version 3 or whose half-lengths do not add up.  Asynchronous on `stream`. */
+int b200kv_plane_offsets_device(const void* containers, int64_t stride, int32_t n, int64_t* out, void* stream);
+
 /* Bytes of device scratch b200kv_encode_chunks / b200kv_decode_chunks need for a call. */
 int64_t b200kv_encode_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t chunk_tokens, int32_t n_chunks,
                                       int32_t coder);
@@ -172,6 +185,36 @@ int b200kv_decode_chunks(const void* containers, int64_t containers_bytes, const
                          uint32_t* status_out, void* workspace, int64_t workspace_bytes, void* stream);
 
 /*
+ * The same decode in two steps, so that a caller can decode a layer as soon as its bytes have arrived (vLLM's
+ * per-layer KV loading: wait_for_layer_load before each attention layer).  b200kv_decode_chunks == plan + layers(0, L).
+ *
+ * b200kv_decode_plan takes b200kv_decode_chunks' arguments and makes all of its checks, zeroes status_out, writes the
+ * chunk descriptors into `workspace` and enqueues the stream-offset kernels (tile sums, tile scan).  Those read the
+ * FIXED sections of every container only (header, nb map / CDF rows, maxes, lengths: [0, layout.off_payload)), so the
+ * payload may still be on its way.  It records its decisions (the table layout among them) in *plan, caller-owned host
+ * memory; the workspace, containers buffer, destination and status_out must stay valid until the last layers call
+ * has run on the device.
+ *
+ * b200kv_decode_layers enqueues the decode of layers [layer_begin, layer_end): planes layer_begin.. (keys) and
+ * L + layer_begin.. (values), 0 <= layer_begin < layer_end <= L, and ORs into the plan's status_out.  Any set of
+ * calls that covers every layer once writes what b200kv_decode_chunks writes.  A call reads the fixed sections and
+ * the payload bytes of its planes' streams; in a version 2 or 3 container nothing past a stream's own bytes reaches
+ * an output or a status bit, so the bytes of later planes may be unwritten (codec.cu explains why).  In a version 3
+ * container (one group) the streams of plane p are the contiguous range that the half-lengths of planes < p and <= p
+ * delimit; containers of several groups (versions 1 / 2 with more than 256 tokens) spread a plane over every group.
+ */
+typedef struct b200kv_decode_plan_t {
+    uint64_t opaque[256];
+} b200kv_decode_plan_t;
+
+int b200kv_decode_plan(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                       const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,
+                       int32_t max_dtype, int32_t coder, const b200kv_kv_desc* dst, const float* key_bins,
+                       const float* value_bins, uint32_t* status_out, void* workspace, int64_t workspace_bytes,
+                       b200kv_decode_plan_t* plan, void* stream);
+int b200kv_decode_layers(const b200kv_decode_plan_t* plan, int32_t layer_begin, int32_t layer_end, void* stream);
+
+/*
  * Token-id prefix hash.  Replaces LMCacheEngine._chunk_tokens/_hash/_prefix_hash
  * (cache_engine.py:58-96): h_i = sha256(ascii_hex(h_{i-1}) || bytes(tokens[i*cs:(i+1)*cs])), h_{-1} = "".
  * n_seq independent sequences are hashed concurrently (one chain each).  tokens: DEVICE pointer to the
@@ -216,6 +259,9 @@ int b200kv_copy_async(void* dst, const void* src, int64_t bytes, void* stream); 
 /* strided 2-D copy: `rows` rows of `row_bytes`, pitches in bytes (chunk slice of a [L,2,T,H,D] blob) */
 int b200kv_copy2d_async(void* dst, int64_t dst_pitch, const void* src, int64_t src_pitch, int64_t row_bytes,
                         int64_t rows, void* stream);
+/* n copies of sizes[i] bytes from srcs[i] to dsts[i] (HOST pointer arrays), in stream order as a batch: the copies of one
+ * call may run in any order among themselves.  One cudaMemcpyBatchAsync where the driver has it (CUDA >= 12.8). */
+int b200kv_copy_batch_async(void* const* dsts, const void* const* srcs, const int64_t* sizes, int64_t n, void* stream);
 int b200kv_stream_create(void** stream);                       /* non-blocking side stream */
 int b200kv_stream_destroy(void* stream);
 int b200kv_stream_sync(void* stream);

@@ -66,6 +66,11 @@ class Layout(ctypes.Structure):
                 ("fixed_bytes", c_i64), ("max_total_bytes", c_i64)]
 
 
+class DecodePlan(ctypes.Structure):
+    """struct b200kv_decode_plan_t (opaque, filled by b200kv_decode_plan)"""
+    _fields_ = [("opaque", ctypes.c_uint64 * 256)]
+
+
 assert ctypes.sizeof(Header) == HEADER_BYTES
 
 # name -> (restype, argtypes); every symbol include/b200kv.h declares
@@ -75,12 +80,17 @@ SIGNATURES = {
     "b200kv_device_count": (c_i32, []),
     "b200kv_container_layout": (c_i32, [c_i32, c_i32, c_i32, c_i32, ctypes.POINTER(Layout)]),
     "b200kv_container_layout_v": (c_i32, [c_i32, c_i32, c_i32, c_i32, c_i32, ctypes.POINTER(Layout)]),
+    "b200kv_plane_offsets": (c_i32, [c_vp, c_i64, c_vp, c_i32]),
+    "b200kv_plane_offsets_device": (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp]),
     "b200kv_encode_workspace_bytes": (c_i64, [c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
     "b200kv_decode_workspace_bytes": (c_i64, [c_i32, c_i32, c_i32, c_i32, c_i32]),
     "b200kv_encode_chunks": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp, c_i64,
                                       c_vp, c_vp, c_i64, c_vp]),
     "b200kv_decode_chunks": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, ctypes.POINTER(KvDesc),
                                       c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    "b200kv_decode_plan": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, ctypes.POINTER(KvDesc),
+                                    c_vp, c_vp, c_vp, c_vp, c_i64, ctypes.POINTER(DecodePlan), c_vp]),
+    "b200kv_decode_layers": (c_i32, [ctypes.POINTER(DecodePlan), c_i32, c_i32, c_vp]),
     "b200kv_sha256_chain": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp]),
     "b200kv_sha256_chain_ready": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, ctypes.c_uint32, c_vp]),
     "b200kv_pack_chunks": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp]),
@@ -90,6 +100,7 @@ SIGNATURES = {
     "b200kv_host_device_ptr": (c_i32, [c_vp, ctypes.POINTER(c_vp)]),
     "b200kv_copy_async": (c_i32, [c_vp, c_vp, c_i64, c_vp]),
     "b200kv_copy2d_async": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_i64, c_i64, c_vp]),
+    "b200kv_copy_batch_async": (c_i32, [c_vp, c_vp, c_vp, c_i64, c_vp]),
     "b200kv_stream_create": (c_i32, [ctypes.POINTER(c_vp)]),
     "b200kv_stream_destroy": (c_i32, [c_vp]),
     "b200kv_stream_sync": (c_i32, [c_vp]),
@@ -137,6 +148,26 @@ def lib() -> ctypes.CDLL:
                     fn.argtypes = args
                 _lib = L
     return _lib
+
+
+_pylib: Optional[ctypes.PyDLL] = None
+
+
+def pylib() -> ctypes.PyDLL:
+    """The library through ctypes.PyDLL, for b200kv_plane_offsets_device alone: the call keeps the GIL.  It is one
+    kernel launch on the store worker; giving the GIL up and taking it back there costs the store more than the launch
+    whenever the caller's thread is busy in Python (it spins on the hash chain's ready words while a store runs)."""
+    global _pylib
+    if _pylib is None:
+        lib()
+        with _lock:
+            if _pylib is None:
+                L = ctypes.PyDLL(LIB_PATH)
+                res, args = SIGNATURES["b200kv_plane_offsets_device"]
+                L.b200kv_plane_offsets_device.restype = res
+                L.b200kv_plane_offsets_device.argtypes = args
+                _pylib = L
+    return _pylib
 
 
 def last_error() -> str:

@@ -23,6 +23,7 @@ from lmcache_b200.codec import KvView, PinnedBuffer
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.logging import init_logger
 from lmcache_b200.storage_backend import CreateStorageBackend
+from lmcache_b200.pipeline import LayerwiseUpload
 from lmcache_b200.utils import CacheEngineKey, KVCache, _lmcache_nvtx_annotate
 
 logger = init_logger(__name__)
@@ -155,6 +156,31 @@ def sha256_prefix_chain(tokens: torch.Tensor, chunk_size: int, seq_offsets: Opti
     are the tensor's native little-endian dtype, as in the reference.  seq_offsets: token boundaries of
     independent sequences (default: one sequence)."""
     return list(sha256_prefix_chain_lazy(tokens, chunk_size, seq_offsets))
+
+
+class LayerwiseRetrieval:
+    """What retrieve_layerwise / retrieve_paged_layerwise return: the hit is known (`ret_mask`, and for the blob form the
+    per-layer (K, V) views `kv`), the KV arrives layer by layer.  Layer l may be read on a stream once wait_layer(l,
+    stream) has been called -- what vLLM's KV connector does in wait_for_layer_load before attention layer l."""
+
+    def __init__(self, ret_mask: torch.Tensor, kv: Optional[KVCache], num_layers: int, upload):
+        self.ret_mask = ret_mask
+        self.kv = kv                        # None for the paged form
+        self.num_layers = num_layers
+        self._upload = upload               # pipeline.LayerwiseUpload
+
+    def wait_layer(self, layer: int, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Make `stream` (default: the current one) wait for layer `layer`.  Blocks the host only until the layer's
+        decode has been enqueued, never until it has run.  A no-op when num_layers is 0: a total miss before the engine
+        knew the model's geometry retrieved nothing, so there is no layer to wait for."""
+        if self.num_layers == 0:
+            return
+        (stream or torch.cuda.current_stream()).wait_event(self._upload.ready(layer))
+
+    def synchronize(self) -> None:
+        """Block the host until every layer is in place."""
+        if self.num_layers > 0:
+            self._upload.ready(self.num_layers - 1).synchronize()     # the layers are decoded in order on one stream
 
 
 class LMCacheEngine:
@@ -392,6 +418,11 @@ class LMCacheEngine:
         """retrieve() straight into a paged KV cache: the longest cached prefix of `tokens` (optionally only the
         suffix selected by `mask`) is written to rows slot_mapping[i]; returns ret_mask as retrieve() does.  Rows of
         tokens that are not retrieved -- misses and the masked-off prefix -- are left untouched."""
+        return self._retrieve_paged(tokens, kv_caches, slot_mapping, mask)
+
+    def _retrieve_paged(self, tokens, kv_caches, slot_mapping, mask, get_kv=None) -> torch.Tensor:
+        """retrieve_paged; get_kv(keys, view, tok0, chunk_size) -> chunks decoded, for every chunk but a first one that
+        straddles the mask (default: the backend's get_kv_into)"""
         if self.metadata.fmt != "vllm":
             raise ValueError(f"paged KV caches use the vllm layout, engine fmt is {self.metadata.fmt}")
         assert len(tokens) == slot_mapping.numel(), "Number of slots does not match the input tokens"
@@ -431,7 +462,7 @@ class LMCacheEngine:
                 vc[idx] = tmp[l, 1, extra:]
             got_chunks, first = 1, 1
         if len(keys) > first:
-            got_chunks += self.engine_.get_kv_into(keys[first:], view, first * cs, cs)
+            got_chunks += (get_kv or self.engine_.get_kv_into)(keys[first:], view, first * cs, cs)
         self._touch(full_chain[:num_skip_chunk + got_chunks], "vllm")
         got = min(base + got_chunks * cs, len(tokens))
         if got <= num_skip_tok:
@@ -459,9 +490,11 @@ class LMCacheEngine:
         """(L, H, D, dtype) of this engine's chunks, learnt from the first store / a probe get."""
         return getattr(self, "_geom", None)
 
-    def _retrieve_into_blob(self, tokens, chunk_hashes, num_skip_tok, num_skip_chunk, ret_mask, fmt, st, full_chain):
+    def _retrieve_into_blob(self, tokens, chunk_hashes, num_skip_tok, num_skip_chunk, ret_mask, fmt, st, full_chain,
+                            get_kv=None):
         """retrieve() without per-chunk tensors or torch.cat: the backend decodes / uploads every hit chunk straight
-        into one preallocated blob; the suffix-mask trim of the first chunk is a view offset, not a copy."""
+        into one preallocated blob; the suffix-mask trim of the first chunk is a view offset, not a copy.  get_kv: as
+        in _retrieve_paged."""
         keys = self._keys_of(chunk_hashes, fmt)
         geom = self._kv_geometry()
         if geom is None:
@@ -490,7 +523,7 @@ class LMCacheEngine:
         shape = (L, 2, n_tok_max, H, D) if fmt == "vllm" else (L, 2, H, n_tok_max, D)
         device = torch.device("cuda", torch.cuda.current_device())
         blob = torch.empty(shape, dtype=dtype, device=device)
-        n = self.engine_.get_kv_into(keys, KvView.from_blob(blob, fmt), 0, self.chunk_size)
+        n = (get_kv or self.engine_.get_kv_into)(keys, KvView.from_blob(blob, fmt), 0, self.chunk_size)
         self._touch(full_chain[:num_skip_chunk + n], fmt)
         if n == 0:
             logger.info("Retrieved 0 chunks")
@@ -505,6 +538,73 @@ class LMCacheEngine:
                     f"elapsed time {time.perf_counter() - st}")
         ret_mask[num_skip_tok + retrieved_token_count:] = False
         return ret, ret_mask
+
+    # ------------------------------------------------------------------ layer-wise retrieve
+    def _layerwise_get(self):
+        """(get_kv for the helpers above, list that receives the LayerwiseUpload), or None: the backend has no
+        layer-major path (raw, remote and hybrid tiers) or its containers hold several groups (chunk_size > 256)"""
+        f = getattr(self.engine_, "get_kv_layerwise", None)
+        if f is None or not self._fast_path() or self.chunk_size > N.GROUP_TOKENS:
+            return None
+        uploads: List[LayerwiseUpload] = []
+
+        def get_kv(keys, view, tok0, cs):
+            uploads.append(f(keys, view, tok0, cs))
+            return uploads[-1].n
+        return get_kv, uploads
+
+    @staticmethod
+    def _layerwise_result(ret_mask, kv, num_layers: int, uploads) -> LayerwiseRetrieval:
+        if uploads:
+            return LayerwiseRetrieval(ret_mask, kv, num_layers, uploads[0])
+        # nothing went layer-major: everything this call enqueued is before one event
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream())
+        return LayerwiseRetrieval(ret_mask, kv, num_layers, LayerwiseUpload.completed(0, num_layers, ev))
+
+    @torch.no_grad()
+    def retrieve_layerwise(self, tokens: torch.Tensor, mask: Optional[torch.Tensor] = None) -> LayerwiseRetrieval:
+        """retrieve(), with the KV made available one layer at a time: returns once the hit is known; ret_mask and the
+        KV after synchronize() are those of retrieve().  On the compressed host and disk tiers the containers are
+        uploaded and decoded layer-major, so layer 0 is ready after about 1/L of the bytes; on every other tier (and
+        for chunks of more than 256 tokens) this is retrieve() followed by one event that stands for every layer."""
+        lw = self._layerwise_get()
+        geom = self._kv_geometry()
+        if lw is None or getattr(self, "_wide_dtype", False):
+            kv, ret_mask = self.retrieve(tokens, mask)
+            return self._layerwise_result(ret_mask, kv, len(kv) if len(kv) else (geom[0] if geom else 0), [])
+        get_kv, uploads = lw
+        num_skip_tok = 0
+        ret_mask = torch.ones_like(tokens, dtype=torch.bool)
+        if mask is not None:
+            num_skip_tok = int(len(mask) - torch.sum(mask))
+        num_skip_chunk = num_skip_tok // self.chunk_size
+        ret_mask[:num_skip_tok] = False
+        fmt = self.metadata.fmt
+        if fmt not in ("vllm", "huggingface"):
+            raise ValueError(f"Invalid format: {fmt}")
+        full_chain = self._prefix_hash(tokens)
+        chunk_hashes = full_chain[num_skip_chunk:]
+        if len(chunk_hashes) == 0:
+            kv, ret_mask = self.retrieve(tokens, mask)
+            return self._layerwise_result(ret_mask, kv, geom[0] if geom else 0, [])
+        kv, ret_mask = self._retrieve_into_blob(tokens, chunk_hashes, num_skip_tok, num_skip_chunk, ret_mask, fmt,
+                                                time.perf_counter(), full_chain, get_kv)
+        geom = self._kv_geometry()
+        return self._layerwise_result(ret_mask, kv, geom[0] if geom else 0, uploads)
+
+    @torch.no_grad()
+    def retrieve_paged_layerwise(self, tokens: torch.Tensor, kv_caches, slot_mapping: torch.Tensor,
+                                 mask: Optional[torch.Tensor] = None) -> LayerwiseRetrieval:
+        """retrieve_paged(), with the KV made available one layer at a time (see retrieve_layerwise).  A first chunk
+        that straddles the mask is decoded and scattered whole before layer 0's wait; `kv` is None."""
+        lw = self._layerwise_get()
+        if lw is None:
+            ret_mask = self.retrieve_paged(tokens, kv_caches, slot_mapping, mask)
+            return self._layerwise_result(ret_mask, None, len(kv_caches), [])
+        get_kv, uploads = lw
+        ret_mask = self._retrieve_paged(tokens, kv_caches, slot_mapping, mask, get_kv)
+        return self._layerwise_result(ret_mask, None, len(kv_caches), uploads)
 
     def close(self):
         self.engine_.close()

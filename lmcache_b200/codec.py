@@ -78,6 +78,17 @@ class KvView:
     @property
     def D(self): return self.desc.D
 
+    def record_stream(self, stream: torch.cuda.Stream) -> None:
+        """Mark every tensor behind the view as used by work on `stream`: the caching allocator reuses none of them
+        before that work has run, even if the caller lets go of them first."""
+        todo = [self._keep]
+        while todo:
+            x = todo.pop()
+            if isinstance(x, torch.Tensor):
+                x.record_stream(stream)
+            elif isinstance(x, (list, tuple)):
+                todo.extend(x)
+
     @staticmethod
     def _code(dtype: torch.dtype) -> int:
         if dtype not in _DTYPE_CODE:
@@ -209,6 +220,20 @@ def parse_header(buf, total: Optional[int] = None) -> N.Header:
         nb = list(bytes(mv[N.HEADER_BYTES:N.HEADER_BYTES + 2 * hd.L]))
     check_header(hd, nb)
     return hd
+
+
+def plane_offsets(buf) -> Optional[np.ndarray]:
+    """Boundaries of the planes' streams in a version-3 container (`buf`: at least its fixed sections), from its
+    half-lengths section: int64[2L + 1], plane p (keys of layer p, then values of layer p - L) is bytes [o[p], o[p + 1])
+    of the container; o[0] is the start of the payload and o[2L] == total_bytes.  None for versions 1 and 2, and when the
+    lengths do not add up to the header's payload (a damaged container: it is only ever uploaded whole)."""
+    src = np.frombuffer(buf, dtype=np.uint8)
+    version, L = (int(v) for v in src[4:12].view(np.uint32))
+    if version != 3:
+        return None
+    o = np.empty(2 * L + 1, dtype=np.int64)
+    rc = N.check(N.lib().b200kv_plane_offsets(src.ctypes.data, src.size, o.ctypes.data, o.size), "plane_offsets")
+    return o if rc == 0 else None
 
 
 def container_layout_of(hd: "N.Header") -> "N.Layout":
@@ -542,6 +567,33 @@ class CacheGenCodec:
         else:
             with self._dec_lock, torch.cuda.device(dst.device):
                 run()
+
+    def decode_plan(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
+                    ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
+                    stream: torch.cuda.Stream, status_ptr: int = 0) -> Tuple["N.DecodePlan", torch.Tensor]:
+        """First half of decode_raw (b200kv_decode_plan): enqueue on `stream` the kernels that read the containers'
+        fixed sections and return (plan, workspace).  The payloads may still be uploading; decode_layers decodes a range
+        of layers once its bytes are there.  The workspace is the caller's (not the codec's shared one), so plans of
+        concurrent retrieves do not order after each other; it must be released only after the plan's last
+        decode_layers (it is recorded on `stream`: run those on the same stream)."""
+        n = len(offsets)
+        lib = N.lib()
+        ws = torch.empty(lib.b200kv_decode_workspace_bytes(dst.L, dst.H, dst.D, max(ntokens), n), dtype=torch.uint8,
+                         device=dst.device)
+        ws.record_stream(stream)
+        plan = N.DecodePlan()
+        N.check(lib.b200kv_decode_plan(base_ptr, int(buf_bytes), N.i64_array(list(offsets)), N.i64_array(list(totals)),
+                                       N.i32_array(list(ntokens)), N.i64_array(list(dst_tok)), n, int(max_dtype),
+                                       int(coder), ctypes.byref(dst.desc), self._kb, self._vb, status_ptr or None,
+                                       ws.data_ptr(), ws.numel(), ctypes.byref(plan), stream.cuda_stream),
+                "decode_plan")
+        return plan, ws
+
+    @staticmethod
+    def decode_layers(plan: "N.DecodePlan", layer_begin: int, layer_end: int, stream: torch.cuda.Stream) -> None:
+        """Second half of decode_raw (b200kv_decode_layers): enqueue the decode of layers [layer_begin, layer_end)."""
+        N.check(N.lib().b200kv_decode_layers(ctypes.byref(plan), int(layer_begin), int(layer_end), stream.cuda_stream),
+                "decode_layers")
 
     def decode_status(self) -> List[int]:
         """Wait for the most recent decode call and return its per-chunk status words (0 = clean; bit 0: a rANS stream

@@ -21,6 +21,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
+#include <string.h>
 
 #include "ac_core.cuh"
 #include "common.cuh"
@@ -887,6 +888,7 @@ struct DecParams {
     const int64_t* slot_map;     // paged destination: token i lives in row slot_map[i]; NULL = row i
     int32_t L, H, D, C, out_dtype, max_dtype, n_chunks, tpp, tiles_max;
     int32_t compact;             // containers are version 3
+    int32_t lb, nlay;            // decode_kernel: this launch decodes layers [lb, lb + nlay), i.e. planes lb.. and L + lb..
     const DecChunk* chunks;      // device
     unsigned long long* tile_base;   // [n_chunks][tiles_max]: tile sums, then exclusive prefix
     uint32_t* status;            // [n_chunks] or NULL: bit 0 = a rANS stream did not return to its initial state,
@@ -948,6 +950,59 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(DecParams P) {
     }
 }
 
+// Plane boundaries of version-3 containers in device memory (b200kv_plane_offsets_device): one CTA of 32 warps per
+// container, one warp per plane at a time, 16-byte loads (the sum is a handful of independent loads per lane, not a chain
+// of byte loads: it runs on the store worker's copy stream, in front of the wave's device->host copies).  out row j:
+// [off_payload, end of plane 0, ..., end of plane 2L-1 = total_bytes], or -1 in entry 0 when the container is not
+// version 3 or its half-lengths do not add up to total_bytes.
+__global__ void __launch_bounds__(1024) plane_offsets_kernel(const uint8_t* base, int64_t stride, int64_t* out) {
+    __shared__ uint32_t s_sum[B200KV_MAX_PLANES];
+    const uint8_t* c = base + (int64_t)blockIdx.x * stride;
+    int64_t* o = out + (int64_t)blockIdx.x * (B200KV_MAX_PLANES + 1);
+    const uint32_t* hw = reinterpret_cast<const uint32_t*>(c);
+    const uint32_t version = hw[1], L = hw[2], H = hw[3], D = hw[4], t = hw[5];
+    const uint64_t total = *reinterpret_cast<const uint64_t*>(c + 40);
+    if (hw[0] != B200KV_MAGIC || version != 3u || L == 0u || 2u * L > (uint32_t)B200KV_MAX_PLANES || H == 0u || D == 0u ||
+        t == 0u || t > (uint32_t)kGroup) {
+        if (threadIdx.x == 0) o[0] = -1;
+        return;
+    }
+    const int NL = 2 * (int)L;
+    const int64_t C = (int64_t)H * D;
+    const Layout lo = make_layout((int)L, (int)C, (int)t, 1);
+    const uint8_t* half = c + lo.off_lengths;                  // 16-byte aligned (container and section)
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int p = warp; p < NL; p += blockDim.x >> 5) {
+        const uint8_t* row = half + p * C;
+        uint32_t sum = 0;
+        if ((C & 15) == 0) {
+            const uint4* v = reinterpret_cast<const uint4*>(row);
+#pragma unroll 4
+            for (int64_t i = lane; i < C / 16; i += 32) {
+                const uint4 q = v[i];
+                sum = __dp4a(q.x, 0x01010101u, sum);
+                sum = __dp4a(q.y, 0x01010101u, sum);
+                sum = __dp4a(q.z, 0x01010101u, sum);
+                sum = __dp4a(q.w, 0x01010101u, sum);
+            }
+        } else {
+            for (int64_t i = lane; i < C; i += 32) sum += row[i];
+        }
+        sum = __reduce_add_sync(0xffffffffu, sum);
+        if (lane == 0) s_sum[p] = sum;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int64_t off = lo.off_payload;
+        o[0] = off;
+        for (int p = 0; p < NL; ++p) {
+            off += 2 * (int64_t)s_sum[p];
+            o[p + 1] = off;
+        }
+        if (off != (int64_t)total) o[0] = -1;
+    }
+}
+
 // Aligned big-endian word reader over the stream's bytes in global memory with a one-word look-ahead: the
 // load for word i+1 is issued when word i is consumed, so its L2/L1 latency overlaps ~8+ symbols of decoding.
 // Each lane walks its own stream; a 32-byte sector serves 8 consecutive refills from L1.
@@ -967,6 +1022,20 @@ struct WordSrc {
 // halfword (rANS) per symbol, whatever the bytes say): at most B200KV_READ_SLACK bytes past the stream's start, which
 // b200kv_decode_chunks checks against the size of the caller's buffer.  A corrupt lengths section therefore cannot make
 // a kernel read outside that buffer: stream starts are clamped to the payload, reads are bounded from there.
+//
+// Bytes read past the end of a stream never reach an output or a status bit (version 2 / 3 streams, rANS), so the
+// bytes of the next plane need not have arrived when a plane is decoded (a layer-major upload, b200kv_decode_layers):
+//   - rANS loop (rans_decode_stream): the init loads 3 words and every window move one more, but a halfword enters the
+//     state only through the PRMT of a renormalisation, and the decoder renormalises exactly where the encoder pushed
+//     (same state sequence), i.e. it consumes exactly the stream's halfwords.  Look-ahead words are loaded, never used.
+//   - v3 header, byte reader (all_short): the load at cb + popc(mask below i) happens for every symbol the warp uses,
+//     but the value is kept only for a set, non-last bit of the lane's own mask: an index < the number of stored
+//     counts, inside the header.  The mask itself is cut to hdr_mask_bytes(nb) bytes.
+//   - v3 header, register reader: words are loaded while 4k < header length; next_byte() hands out the count bytes
+//     only, all of them inside the header (the funnel shift may carry later bytes in the same register, unread).
+//   - status: bit 1 comes from the lengths section (fixed sections) and payload_bytes, bit 0 from the final state.
+// Version 1 (arithmetic coder) is not covered by this argument (its decoder shifts bits past the end of its stream into
+// its window); the layer-major upload of lmcache_b200/pipeline.py splits version-3 containers only.
 
 // rANS: aligned little-endian words off a running pointer; the look-ahead lives in the decoder state (RansDec::nxt)
 struct LeWordSrc {
@@ -1155,9 +1224,13 @@ __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
     const DecChunk dc = P.chunks[j];
     const int NL = 2 * P.L;
     const int per_group = NL * P.tpp;
-    const int tile = blockIdx.x;
-    const int g = tile / per_group;
+    // blockIdx.x walks the launch's tiles of each group: K planes lb.., then V planes L + lb..; `tile` is the tile's
+    // index among all of the chunk's tiles (tile_base)
+    const int launch_group = 2 * P.nlay * P.tpp;
+    const int g = blockIdx.x / launch_group;
     if (g >= dc.ngroups) return;
+    const int kt = blockIdx.x - g * launch_group;
+    const int tile = g * per_group + kt + (kt < P.nlay * P.tpp ? P.lb : P.L - P.nlay + P.lb) * P.tpp;
     const int rem = tile - g * per_group;
     const int nl = rem / P.tpp;
     const int ct = rem - nl * P.tpp;
@@ -1428,6 +1501,18 @@ static size_t dec_ws_layout(int64_t tiles_max, int n_chunks, size_t* off_tb) {
     return (o + 255) & ~(size_t)255;
 }
 
+// What b200kv_decode_plan decided, kept in the caller's b200kv_decode_plan_t: the decode kernel's parameter block (its
+// chunk descriptors and tile bases live in the workspace) and the kernel variant.
+constexpr uint32_t kPlanMagic = 0x4e4c5044u;   // "DPLN"
+struct DecPlan {
+    uint32_t magic;
+    int32_t coder;           // CODER_AC | CODER_RANS
+    int32_t transposed;      // rANS table layout
+    int32_t gmax;            // groups of the longest chunk
+    DecParams P;
+};
+static_assert(sizeof(DecPlan) <= sizeof(b200kv_decode_plan_t), "b200kv_decode_plan_t too small");
+
 }  // namespace b200kv
 
 using namespace b200kv;
@@ -1454,6 +1539,39 @@ int b200kv_container_layout_v(int32_t L, int32_t H, int32_t D, int32_t ntokens, 
     const int64_t streams = 2 * (int64_t)L * H * D;
     out->max_total_bytes = align16(lo.off_payload + streams * (2 * (int64_t)ntokens + 4 * (int64_t)lo.ngroups +
                                                               (compact ? kHdrMax : 0)) + 16);
+    return 0;
+}
+
+int b200kv_plane_offsets(const void* container, int64_t nbytes, int64_t* out, int32_t n_out) {
+    B2_REQUIRE(container != nullptr && out != nullptr && nbytes >= (int64_t)sizeof(b200kv_header), "bad arguments");
+    b200kv_header hd;
+    memcpy(&hd, container, sizeof(hd));
+    B2_REQUIRE(hd.magic == B200KV_MAGIC && hd.version == 3, "not a version-3 container");
+    B2_REQUIRE(hd.L > 0 && 2 * (int64_t)hd.L <= B200KV_MAX_PLANES && hd.H > 0 && hd.D > 0 && hd.ntokens > 0 &&
+               hd.ntokens <= (uint32_t)kGroup, "impossible shape");
+    const int NL = 2 * (int)hd.L;
+    const int64_t C = (int64_t)hd.H * hd.D;
+    B2_REQUIRE(n_out >= NL + 1, "out must hold 2L + 1 offsets");
+    const Layout lo = make_layout((int)hd.L, (int)C, (int)hd.ntokens, 1);
+    B2_REQUIRE(nbytes >= lo.off_payload, "buffer shorter than the fixed sections");
+    const uint8_t* half = static_cast<const uint8_t*>(container) + lo.off_lengths;
+    int64_t o = lo.off_payload;
+    out[0] = o;
+    for (int p = 0; p < NL; ++p) {
+        uint32_t sum = 0;                          // <= 4096 * 255 per plane at the largest shapes: no overflow
+        for (int64_t c = 0; c < C; ++c) sum += half[p * C + c];
+        o += 2 * (int64_t)sum;
+        out[p + 1] = o;
+    }
+    return o == (int64_t)hd.total_bytes ? 0 : 1;
+}
+
+int b200kv_plane_offsets_device(const void* containers, int64_t stride, int32_t n, int64_t* out, void* stream) {
+    B2_REQUIRE(containers != nullptr && out != nullptr && n > 0 && stride >= (int64_t)sizeof(b200kv_header) &&
+               (stride & 15) == 0 && (reinterpret_cast<uintptr_t>(containers) & 15) == 0, "bad arguments");
+    plane_offsets_kernel<<<(unsigned)n, 1024, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const uint8_t*>(containers),
+                                                                                      stride, out);
+    B2_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
@@ -1610,13 +1728,16 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
     return 0;
 }
 
-int b200kv_decode_chunks(const void* containers, int64_t containers_bytes, const int64_t* offsets,
-                         const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,
-                         int32_t max_dtype,
-                         int32_t coder, const b200kv_kv_desc* dst, const float* key_bins, const float* value_bins,
-                         uint32_t* status_out, void* workspace, int64_t workspace_bytes, void* stream_) {
+int b200kv_decode_plan(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                       const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,
+                       int32_t max_dtype, int32_t coder, const b200kv_kv_desc* dst, const float* key_bins,
+                       const float* value_bins, uint32_t* status_out, void* workspace, int64_t workspace_bytes,
+                       b200kv_decode_plan_t* plan_out, void* stream_) {
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    DecParams P;
+    B2_REQUIRE(plan_out != nullptr, "plan is NULL");
+    DecPlan* plan = reinterpret_cast<DecPlan*>(plan_out);
+    plan->magic = 0u;
+    DecParams& P = plan->P;
     B2_REQUIRE(key_bins && value_bins, "bins are NULL");
     B2_REQUIRE(coder >= CODER_AC && coder <= CODER_RANS_COMPACT, "coder must be one of B200KV_CODER_*");
     P.compact = coder == CODER_RANS_COMPACT ? 1 : 0;
@@ -1630,6 +1751,7 @@ int b200kv_decode_chunks(const void* containers, int64_t containers_bytes, const
     P.L = dst->L; P.H = dst->H; P.D = dst->D; P.C = dst->H * dst->D;
     P.out_dtype = dst->dtype; P.max_dtype = max_dtype; P.n_chunks = n_chunks;
     P.tpp = tiles_per_plane(P.C);
+    P.lb = 0; P.nlay = P.L;
     int tmax = 0;
     for (int j = 0; j < n_chunks; ++j) {
         B2_REQUIRE(ntokens[j] > 0, "ntokens must be positive");
@@ -1699,9 +1821,26 @@ int b200kv_decode_chunks(const void* containers, int64_t containers_bytes, const
         tile_scan_kernel<<<(unsigned)n_chunks, 1024, 0, stream>>>(P);
     }
     B2_CHECK_CUDA(cudaGetLastError());
+    plan->coder = coder;
+    plan->transposed = transposed ? 1 : 0;
+    plan->gmax = (int32_t)Gmax;
+    plan->magic = kPlanMagic;
+    return 0;
+}
 
+int b200kv_decode_layers(const b200kv_decode_plan_t* plan_in, int32_t layer_begin, int32_t layer_end, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B2_REQUIRE(plan_in != nullptr, "plan is NULL");
+    const DecPlan* plan = reinterpret_cast<const DecPlan*>(plan_in);
+    B2_REQUIRE(plan->magic == kPlanMagic, "not a plan made by b200kv_decode_plan");
+    DecParams P = plan->P;
+    B2_REQUIRE(layer_begin >= 0 && layer_begin < layer_end && layer_end <= P.L, "layer range out of range");
+    P.lb = layer_begin;
+    P.nlay = layer_end - layer_begin;
+    const int coder = plan->coder;
+    const bool transposed = plan->transposed != 0;
     const size_t smem = (size_t)(CT * kLp + kGroup + 32) * 4;
-    dim3 grid((unsigned)tiles_max, (unsigned)n_chunks);
+    dim3 grid((unsigned)((int64_t)plan->gmax * 2 * P.nlay * P.tpp), (unsigned)P.n_chunks);
     ProfScope prof(kProfDecode, stream);
 #define B2_LAUNCH_DEC1(DT, PAGED, CODER, TR)                                                                           \
     do {                                                                                                               \
@@ -1721,6 +1860,19 @@ int b200kv_decode_chunks(const void* containers, int64_t containers_bytes, const
 #undef B2_LAUNCH_DEC1
     B2_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+int b200kv_decode_chunks(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                         const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,
+                         int32_t max_dtype,
+                         int32_t coder, const b200kv_kv_desc* dst, const float* key_bins, const float* value_bins,
+                         uint32_t* status_out, void* workspace, int64_t workspace_bytes, void* stream) {
+    b200kv_decode_plan_t plan;
+    if (int rc = b200kv_decode_plan(containers, containers_bytes, offsets, total_bytes, ntokens, dst_tok, n_chunks,
+                                    max_dtype, coder, dst, key_bins, value_bins, status_out, workspace, workspace_bytes,
+                                    &plan, stream))
+        return rc;
+    return b200kv_decode_layers(&plan, 0, dst->L, stream);
 }
 
 int b200kv_profile_enable(int32_t on) {

@@ -14,6 +14,8 @@
 
 #include <type_traits>
 
+#include <vector>
+
 #include "common.cuh"
 
 namespace b200kv {
@@ -157,6 +159,37 @@ int b200kv_copy2d_async(void* dst, int64_t dst_pitch, const void* src, int64_t s
     if (row_bytes == 0 || rows == 0) return 0;
     B2_CHECK_CUDA(cudaMemcpy2DAsync(dst, (size_t)dst_pitch, src, (size_t)src_pitch, (size_t)row_bytes, (size_t)rows,
                                     cudaMemcpyDefault, static_cast<cudaStream_t>(stream)));
+    return 0;
+}
+
+int b200kv_copy_batch_async(void* const* dsts, const void* const* srcs, const int64_t* sizes, int64_t n, void* stream) {
+    B2_REQUIRE(n >= 0 && (n == 0 || (dsts != nullptr && srcs != nullptr && sizes != nullptr)), "bad batch copy arguments");
+    std::vector<void*> d, s;
+    std::vector<size_t> z;
+    for (int64_t i = 0; i < n; ++i) {
+        B2_REQUIRE(dsts[i] != nullptr && srcs[i] != nullptr && sizes[i] >= 0, "bad batch copy arguments");
+        if (sizes[i] == 0) continue;
+        d.push_back(dsts[i]);
+        s.push_back(const_cast<void*>(srcs[i]));
+        z.push_back((size_t)sizes[i]);
+    }
+    if (d.empty()) return 0;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    // one driver call for the whole batch: per-copy submission costs ~2 us of host time per copy, which is the copy
+    // engine's time for a few hundred KB -- a layer of a layer-major upload is many copies of that size
+    cudaMemcpyAttributes attr = {};
+    attr.srcAccessOrder = cudaMemcpySrcAccessOrderStream;
+    attr.flags = cudaMemcpyFlagPreferOverlapWithCompute;
+    size_t attr_idx = 0, fail_idx = 0;
+    const cudaError_t e = cudaMemcpyBatchAsync(d.data(), s.data(), z.data(), d.size(), &attr, &attr_idx, 1, &fail_idx, st);
+    // a driver older than the runtime (CUDA < 12.8) answers cudaErrorCallRequiresNewerDriver, a device or stream that
+    // cannot take the batch cudaErrorNotSupported: then the same copies, one call each
+    if (e != cudaErrorNotSupported && e != cudaErrorCallRequiresNewerDriver) {
+        B2_CHECK_CUDA(e);
+        return 0;
+    }
+    (void)cudaGetLastError();
+    for (size_t i = 0; i < d.size(); ++i) B2_CHECK_CUDA(cudaMemcpyAsync(d[i], s[i], z[i], cudaMemcpyDefault, st));
     return 0;
 }
 

@@ -24,13 +24,15 @@ import functools
 import os
 import queue
 import threading
+import time
 from concurrent.futures import Future
 from typing import Callable, Iterable, Iterator, List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from lmcache_b200 import _native as N
-from lmcache_b200.codec import CacheGenCodec, EncodeTicket, KvView, PinnedBuffer, parse_header
+from lmcache_b200.codec import CacheGenCodec, EncodeTicket, KvView, PinnedBuffer, parse_header, plane_offsets
 
 
 def wave_chunks_default() -> int:
@@ -47,10 +49,12 @@ class WaveSlot:
     def __init__(self, nbytes: int, wave: int, device):
         self.dev = torch.empty(nbytes + N.READ_SLACK, dtype=torch.uint8, device=device)
         self.sizes = PinnedBuffer(max(64, 8 * wave))
+        self.planes = PinnedBuffer(8 * (N.MAX_PLANES + 1) * wave)      # b200kv_plane_offsets_device rows, one per chunk
         self.ticket: Optional[EncodeTicket] = None
 
     def close(self):
         self.sizes.close()
+        self.planes.close()
         self.dev = None
 
 
@@ -234,9 +238,9 @@ class UploadRing:
 
 class HostContainer:
     """One CacheGen container in a page-locked slab block, with the header fields its upload and decode need."""
-    __slots__ = ("blk", "nbytes", "ntokens", "L", "H", "D", "max_dtype", "coder", "last_read")
+    __slots__ = ("blk", "nbytes", "ntokens", "L", "H", "D", "max_dtype", "coder", "last_read", "planes")
 
-    def __init__(self, blk, nbytes: int, hd: "N.Header"):
+    def __init__(self, blk, nbytes: int, hd: "N.Header", planes: Optional[np.ndarray] = None):
         self.blk = blk                       # None once the tier no longer keeps the bytes (the disk tier's index)
         self.nbytes = int(nbytes)
         self.ntokens = int(hd.ntokens)
@@ -244,6 +248,9 @@ class HostContainer:
         self.max_dtype = int(hd.max_dtype)
         self.coder = int(hd.version) - 1
         self.last_read: Optional[torch.cuda.Event] = None   # most recent upload out of the block
+        # codec.plane_offsets: where each plane's streams lie, for a layer-major upload; None: upload it whole.  Made by
+        # whoever makes the record (land, read_container), never on the thread of a retrieve.
+        self.planes = planes
 
 
 @functools.lru_cache(maxsize=None)
@@ -263,13 +270,24 @@ def land(slab, slot: WaveSlot, batch, blocks: Optional[list] = None) -> List[Hos
     try:
         with torch.cuda.device(dev):
             try:
+                # plane offsets of the wave, read on the device before the bytes leave it: no host pass over the
+                # lengths sections (on the store worker such a pass made every e2e store ~2 ms slower, measured)
+                N.check(N.pylib().b200kv_plane_offsets_device(ctypes.c_void_p(slot.dev.data_ptr()), batch.stride,
+                                                            len(blocks), ctypes.c_void_p(slot.planes.dev_ptr),
+                                                            cs.cuda_stream), "plane_offsets_device")
                 for j, (blk, size) in enumerate(zip(blocks, batch.sizes)):
                     N.check(N.lib().b200kv_copy_async(ctypes.c_void_p(blk.host_ptr),
                                                       ctypes.c_void_p(slot.dev.data_ptr() + j * batch.stride), size,
                                                       cs.cuda_stream), "copy_async")
             finally:
                 cs.synchronize()             # no block leaves this function while a copy may still write it
-        return [HostContainer(blk, blk.nbytes, parse_header(blk.view())) for blk in blocks]
+        po = np.frombuffer(slot.planes.view(), dtype=np.int64, count=len(blocks) * (N.MAX_PLANES + 1))
+        po = po.reshape(len(blocks), N.MAX_PLANES + 1)
+        recs = []
+        for j, blk in enumerate(blocks):
+            hd = parse_header(blk.view())
+            recs.append(HostContainer(blk, blk.nbytes, hd, po[j, :2 * hd.L + 1].copy() if po[j, 0] >= 0 else None))
+        return recs
     except BaseException:
         for blk in blocks:
             blk.free()
@@ -282,7 +300,7 @@ def read_container(codec: CacheGenCodec, blk, nbytes: int) -> Optional[HostConta
     try:
         hd = parse_header(blk.view()[:nbytes])
         if codec.accepts(hd):
-            return HostContainer(blk, nbytes, hd)
+            return HostContainer(blk, nbytes, hd, plane_offsets(blk.view()[:nbytes]))   # on the reader's thread
     except ValueError:
         pass
     blk.free()
@@ -345,6 +363,12 @@ def fetched_in_order(futures: Iterable[Future], window: Optional[int] = None) ->
                 rec.blk.free()
 
 
+def _continues_match(r: HostContainer, first: Optional[HostContainer], dst: KvView, tok: int) -> bool:
+    """May container `r`, landing at token `tok` of `dst`, extend a match that began with `first` (None: r is first)?"""
+    return (r.L, r.H, r.D) == (dst.L, dst.H, dst.D) and tok + r.ntokens <= dst.ntokens and \
+        (first is None or (r.max_dtype, r.coder) == (first.max_dtype, first.coder))
+
+
 def upload_decode(codec: CacheGenCodec, upload: UploadRing, records: Iterable[Optional[HostContainer]], dst: KvView,
                   dst_tok0: int, chunk_size: int, release: Optional[DeferredFree] = None) -> int:
     """Upload + decode consecutive chunks straight into `dst`: records[i] (None: a miss) is chunk i and lands at token
@@ -391,8 +415,7 @@ def upload_decode(codec: CacheGenCodec, upload: UploadRing, records: Iterable[Op
         for r in records:
             if r is None:
                 break
-            if (r.L, r.H, r.D) != (dst.L, dst.H, dst.D) or dst_tok0 + n * chunk_size + r.ntokens > dst.ntokens or \
-                    (first is not None and (r.max_dtype, r.coder) != (first.max_dtype, first.coder)):
+            if not _continues_match(r, first, dst, dst_tok0 + n * chunk_size):
                 if release is not None:
                     r.blk.free()
                 break
@@ -403,3 +426,205 @@ def upload_decode(codec: CacheGenCodec, upload: UploadRing, records: Iterable[Op
                 flush()
         flush()
     return n
+
+
+class LayerwiseUpload:
+    """One layer-major upload + decode in flight (upload_decode_layerwise): `n` chunks matched, and per layer the event
+    recorded after that layer's decode.  A worker thread records the events one layer after another; `ready(l)` blocks
+    the calling host thread until event l has been recorded -- not until it has completed."""
+
+    def __init__(self, n: int, num_layers: int):
+        self.n = n
+        self.num_layers = num_layers
+        self.enqueue_s: List[float] = []    # host seconds the worker spent enqueueing: fixed sections + plan, then per layer
+        self._ready: List[torch.cuda.Event] = []
+        self._error: Optional[BaseException] = None
+        self._cv = threading.Condition()
+
+    @classmethod
+    def completed(cls, n: int, num_layers: int, event: torch.cuda.Event) -> "LayerwiseUpload":
+        """a handle whose every layer is ready with `event` (a retrieve that was not layer-major)"""
+        u = cls(n, num_layers)
+        u._ready = [event] * num_layers
+        return u
+
+    def _publish(self, event: torch.cuda.Event) -> None:
+        with self._cv:
+            self._ready.append(event)
+            self._cv.notify_all()
+
+    def _fail(self, err: BaseException) -> None:
+        with self._cv:
+            self._error = err
+            self._cv.notify_all()
+
+    def ready(self, layer: int) -> torch.cuda.Event:
+        if not 0 <= layer < self.num_layers:
+            raise IndexError(f"layer {layer} out of range [0, {self.num_layers})")
+        with self._cv:
+            while len(self._ready) <= layer and self._error is None:
+                self._cv.wait()
+            if len(self._ready) <= layer:
+                raise self._error
+            return self._ready[layer]
+
+
+class LayerwiseUploader:
+    """A copy stream, a decode stream and the worker thread that enqueues layer-major uploads on them (one per tier and
+    device).  Jobs run one after another in submission order."""
+
+    def __init__(self, device):
+        self.device = torch.device(device)
+        self.copy_stream = torch.cuda.Stream(device=self.device)
+        self.decode_stream = torch.cuda.Stream(device=self.device)
+        self._q: "queue.Queue" = queue.Queue()
+        self._thread = threading.Thread(target=self._worker, name="b200kv-layerwise", daemon=True)
+        self._thread.start()
+
+    def _worker(self) -> None:
+        torch.cuda.set_device(self.device)
+        while True:
+            job = self._q.get()
+            if job is None:
+                return
+            job()
+
+    def submit(self, job: Callable[[], None]) -> None:
+        self._q.put(job)
+
+    def close(self) -> None:
+        """wait for every submitted job to be enqueued, then stop the worker"""
+        if self._thread is not None:
+            self._q.put(None)
+            self._thread.join()
+            self._thread = None
+
+
+def _batch_copy(dsts: np.ndarray, srcs: np.ndarray, sizes: np.ndarray, stream: torch.cuda.Stream) -> None:
+    """one b200kv_copy_batch_async for contiguous uint64 / uint64 / int64 arrays of equal length"""
+    N.check(N.lib().b200kv_copy_batch_async(dsts.ctypes.data, srcs.ctypes.data, sizes.ctypes.data, len(sizes),
+                                            stream.cuda_stream), "copy_batch_async")
+
+
+def layer_copy_ranges(plane_offs: Sequence[Optional[np.ndarray]], nbytes: Sequence[int], L: int):
+    """The copies of a layer-major upload of n containers, as offsets into each container: (fixed int64[n],
+    start int64[L, 2n], size int64[L, 2n]).  Container j's first fixed[j] bytes go first (its fixed sections; all of it
+    when it has no plane offsets); row l holds the key ranges (plane l) of containers 0..n-1, then their value ranges
+    (plane L + l).  Together they cover every container exactly once."""
+    n = len(nbytes)
+    po = np.stack([o if o is not None else np.zeros(2 * L + 1, np.int64) for o in plane_offs]).astype(np.int64)
+    split = np.array([o is not None for o in plane_offs])
+    fixed = np.where(split, po[:, 0], np.asarray(nbytes, dtype=np.int64)).astype(np.int64)
+    start = np.ascontiguousarray(np.concatenate([po[:, :L], po[:, L:2 * L]]).T)                   # [L, 2n]
+    size = np.ascontiguousarray(np.concatenate([po[:, 1:L + 1] - po[:, :L], po[:, L + 1:] - po[:, L:2 * L]]).T)
+    assert start.shape == (L, 2 * n)
+    return fixed, start, size
+
+
+def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, records: Iterable[Optional[HostContainer]],
+                            dst: KvView, dst_tok0: int, chunk_size: int, release: Optional[DeferredFree] = None,
+                            on_done: Optional[Callable[[], None]] = None) -> LayerwiseUpload:
+    """upload_decode in layer-major order, so that layer 0 of every chunk is decoded after ~1/L of the bytes.
+
+    The match follows upload_decode's rules and is made on the calling thread, which consumes `records` to its end
+    (n is known when this returns).  A worker then enqueues, on the uploader's streams:
+      1. the fixed sections of every matched container (whole containers without plane offsets) into one device staging
+         buffer, and the decode plan (stream offsets) after them;
+      2. for each layer l: the byte ranges of planes l (keys) and L + l (values) of every container, one batched copy,
+         then the decode of layer l, then the layer's ready event.
+    The decode stream first waits for the calling thread's current stream (the destination may have just been
+    allocated there).  Every record's `last_read` is the last copy's event; `release` (transient blocks) gets the blocks
+    with that event; `on_done` runs once that event is recorded (or when the call fails) -- e.g. to unpin the entries."""
+    matched: List[HostContainer] = []
+    L = dst.L
+    submitted = False
+    try:
+        first = None
+        for r in records:
+            if r is None:
+                break
+            if not _continues_match(r, first, dst, dst_tok0 + len(matched) * chunk_size):
+                if release is not None:
+                    r.blk.free()
+                break
+            first = first or r
+            matched.append(r)
+        n = len(matched)
+        with torch.cuda.device(dst.device):
+            start = torch.cuda.Event()
+            start.record(torch.cuda.current_stream())
+            if n == 0:
+                submitted = True
+                if on_done is not None:
+                    on_done()
+                return LayerwiseUpload.completed(0, L, start)
+            offs, o = [], 0
+            for r in matched:
+                offs.append(o)
+                o += (r.nbytes + 15) & ~15
+            staging = torch.empty(o + N.READ_SLACK, dtype=torch.uint8, device=dst.device)
+            staging.record_stream(uploader.copy_stream)
+            staging.record_stream(uploader.decode_stream)
+            dst.record_stream(uploader.decode_stream)
+
+        base = staging.data_ptr()
+        host = np.array([r.blk.host_ptr for r in matched], dtype=np.uint64)
+        dev = base + np.array(offs, dtype=np.uint64)
+        fixed, lo, sz = layer_copy_ranges([r.planes for r in matched], [r.nbytes for r in matched], L)
+        lay_src = np.ascontiguousarray(np.tile(np.concatenate([host, host]), (L, 1)) + lo.astype(np.uint64))
+        lay_dst = np.ascontiguousarray(np.tile(np.concatenate([dev, dev]), (L, 1)) + lo.astype(np.uint64))
+        upload = LayerwiseUpload(n, L)
+        totals = [r.nbytes for r in matched]
+        ntoks = [r.ntokens for r in matched]
+        dst_tok = [dst_tok0 + j * chunk_size for j in range(n)]
+
+        def job():
+            cs, ds = uploader.copy_stream, uploader.decode_stream
+            last = None
+            try:
+                with torch.cuda.device(uploader.device):
+                    t0 = time.perf_counter()
+                    cs.wait_event(start)
+                    ds.wait_event(start)
+                    _batch_copy(dev, host, fixed, cs)
+                    last = torch.cuda.Event()
+                    last.record(cs)
+                    ds.wait_event(last)
+                    plan, ws = codec.decode_plan(base, staging.numel(), offs, totals, ntoks, dst, dst_tok,
+                                                 first.max_dtype, first.coder, ds)
+                    t1 = time.perf_counter()
+                    upload.enqueue_s.append(t1 - t0)
+                    for layer in range(L):
+                        _batch_copy(lay_dst[layer], lay_src[layer], sz[layer], cs)
+                        last = torch.cuda.Event()
+                        last.record(cs)
+                        ds.wait_event(last)
+                        codec.decode_layers(plan, layer, layer + 1, ds)
+                        ev = torch.cuda.Event(enable_timing=True)     # a caller may time the layers against each other
+                        ev.record(ds)
+                        upload._publish(ev)
+                        t0, t1 = t1, time.perf_counter()
+                        upload.enqueue_s.append(t1 - t0)
+                    del ws                            # recorded on the decode stream: reused only after the decodes
+            except BaseException as e:               # noqa: BLE001 -- the caller sees it in ready()
+                upload._fail(e)
+                cs.synchronize()                      # no block is released while a copy that reads it may be queued
+                last = None
+            finally:
+                for r in matched:
+                    r.last_read = last
+                if release is not None:
+                    release.add(last, [r.blk for r in matched])
+                if on_done is not None:
+                    on_done()
+
+        uploader.submit(job)
+        submitted = True
+        return upload
+    finally:
+        if not submitted:                             # failed before the worker took over: nothing was enqueued
+            if release is not None:
+                for r in matched:
+                    r.blk.free()
+            if on_done is not None:
+                on_done()

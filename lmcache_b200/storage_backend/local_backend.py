@@ -321,6 +321,7 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         self.update_lock = threading.Lock()
         self._pipe = EncodePipeline(self.codec, self._sink)
         self._upload: Optional[UploadRing] = None
+        self._layerwise = None                # pipeline.LayerwiseUploader, made by the first layer-wise retrieve
         self._release = DeferredFree()        # blocks uploads may still read: retired entries, the disk tier's file reads
         self._closed = False
 
@@ -500,6 +501,23 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         finally:
             self._unpin(pinned)             # every wave's upload event is recorded in its records' last_read by now
 
+    def get_kv_layerwise(self, keys, dst, dst_tok0: int, chunk_size: int):
+        """get_kv_into in layer-major order (pipeline.upload_decode_layerwise): returns once the hit count is known, with
+        a pipeline.LayerwiseUpload whose ready(l) is the event after layer l's decode.  The entries stay pinned until
+        the last copy is enqueued."""
+        from lmcache_b200.pipeline import upload_decode_layerwise
+        pinned = []
+        return upload_decode_layerwise(self.codec, self._layerwise_uploader(dst.device), self._pinned_records(keys, pinned),
+                                       dst, dst_tok0, chunk_size, on_done=lambda: self._unpin(pinned))
+
+    def _layerwise_uploader(self, device):
+        from lmcache_b200.pipeline import LayerwiseUploader
+        if self._layerwise is None or self._layerwise.device != device:
+            if self._layerwise is not None:
+                self._layerwise.close()
+            self._layerwise = LayerwiseUploader(device)
+        return self._layerwise
+
     def _pinned_records(self, keys, pinned: list):
         """the records of `keys` in order (None: a miss), each entry pinned from its lookup on: neither eviction nor an
         overwrite frees its block before the upload that reads it is enqueued and recorded"""
@@ -561,6 +579,8 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
             return
         self._closed = True
         self._pipe.close()
+        if self._layerwise is not None:
+            self._layerwise.close()
         try:
             torch.cuda.synchronize()
         except Exception:       # noqa: BLE001 -- interpreter shutdown
@@ -764,6 +784,21 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
         with contextlib.closing(fetched_in_order(reads)) as recs:
             return upload_decode(self.codec, self._upload_ring(dst.device), recs, dst, dst_tok0, chunk_size,
                                  self._release)
+
+    def get_kv_layerwise(self, keys, dst, dst_tok0: int, chunk_size: int):
+        import contextlib
+
+        from lmcache_b200.pipeline import fetched_in_order, upload_decode_layerwise
+        self._release.sweep()
+        reads = []
+        for key in keys:
+            e = self._ready_entry(key)
+            if e is None:
+                break
+            reads.append(self._io.submit(self._read_file, e))
+        with contextlib.closing(fetched_in_order(reads)) as recs:
+            return upload_decode_layerwise(self.codec, self._layerwise_uploader(dst.device), recs, dst, dst_tok0,
+                                           chunk_size, self._release)
 
     def host_bytes(self) -> int:
         return sum(e.rec.nbytes for e in self.dict.values() if e.rec is not None)
