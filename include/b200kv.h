@@ -36,7 +36,9 @@ extern "C" {
                                     *    b200kv_sha256_chain_ready.  Added since without changing anything that
                                     *    existed (the number stays 4; a caller that needs them looks the symbols up,
                                     *    e.g. dlsym): b200kv_decode_plan / b200kv_decode_layers, b200kv_plane_offsets,
-                                    *    b200kv_plane_offsets_device, b200kv_copy_batch_async */
+                                    *    b200kv_plane_offsets_device, b200kv_copy_batch_async,
+                                    *    b200kv_encode_layers_workspace_bytes / b200kv_encode_layers_plan /
+                                    *    b200kv_encode_layers / b200kv_encode_layers_finish */
 #define B200KV_CODER_AC 0          /* payload = torchac-lineage arithmetic coder; container version 1 */
 #define B200KV_CODER_RANS 1        /* payload = rANS, 32-bit state / 16-bit renormalisation; container version 2 */
 #define B200KV_CODER_RANS_COMPACT 2 /* rANS as in version 2, compact side information; container version 3 (chunks of
@@ -213,6 +215,46 @@ int b200kv_decode_plan(const void* containers, int64_t containers_bytes, const i
                        const float* value_bins, uint32_t* status_out, void* workspace, int64_t workspace_bytes,
                        b200kv_decode_plan_t* plan, void* stream);
 int b200kv_decode_layers(const b200kv_decode_plan_t* plan, int32_t layer_begin, int32_t layer_end, void* stream);
+
+/*
+ * The encode of b200kv_encode_chunks in three steps, so that a layer can be encoded as soon as the forward pass has
+ * written it (vLLM's save_kv_layer after each attention layer, wait_for_save at the end).  Version-3 containers only
+ * (coder B200KV_CODER_RANS_COMPACT, chunk_tokens <= 256).
+ *
+ * b200kv_encode_layers_plan takes b200kv_encode_chunks' KV arguments and makes its checks, zeroes the counters in
+ * `workspace` and the n_chunks fixed-section images at fixed_out + j * fixed_stride (fixed_stride >= layout.off_payload),
+ * and records its decisions in *plan (caller-owned host memory).  The KV is not read yet.  max_layers: the most layers
+ * one b200kv_encode_layers call may take (the workspace holds one call's temp rows:
+ * b200kv_encode_layers_workspace_bytes).
+ *
+ * b200kv_encode_layers enqueues, for layers [layer_begin, layer_end) -- planes layer_begin.. and L + layer_begin.. -- of
+ * every chunk: the row maxima and the half-lengths into the chunk's fixed image, the entropy coding, and the compaction
+ * of those planes' streams into the device arena (arena_bytes bytes).  The bytes of chunk j for the call (its K planes,
+ * then its V planes) are placed 16-byte aligned at a device-held cursor, in (call, chunk) order.  A chunk whose bytes do
+ * not fit fails, and so does every later chunk of the plan: the chunks that fit are always a prefix.  Row (j, p) of
+ * seg_sizes_out (DEVICE or mapped-host int64[n_chunks][2L][2]) gets the arena offset (-1: chunk failed) and the size of
+ * plane p of chunk j.  Each layer is encoded once; a layer range that was encoded before is an error.
+ *
+ * b200kv_encode_layers_finish writes each chunk's header into its fixed image and sizes_out[j] (total_bytes, or 0 when
+ * the chunk failed: header.status bit 16 = did not fit the arena), and fails unless every layer was encoded.
+ *
+ * For every chunk that did not fail, fixed image [0, layout.off_payload) || the 2L planes in order (keys of layers
+ * 0..L-1, then values) are byte for byte the container b200kv_encode_chunks writes.  The KV, the arena, the images, the
+ * outputs and the workspace must stay valid until the finish step has run on the device.
+ */
+typedef struct b200kv_encode_plan_t {
+    uint64_t opaque[256];
+} b200kv_encode_plan_t;
+
+int64_t b200kv_encode_layers_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t chunk_tokens, int32_t n_chunks,
+                                             int32_t max_layers);
+int b200kv_encode_layers_plan(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
+                              int32_t last_chunk_tokens, const float* key_bins, const float* value_bins, int32_t coder,
+                              void* arena, int64_t arena_bytes, void* fixed_out, int64_t fixed_stride, int64_t* seg_sizes_out,
+                              uint64_t* sizes_out, int32_t max_layers, void* workspace, int64_t workspace_bytes,
+                              b200kv_encode_plan_t* plan, void* stream);
+int b200kv_encode_layers(b200kv_encode_plan_t* plan, int32_t layer_begin, int32_t layer_end, void* stream);
+int b200kv_encode_layers_finish(const b200kv_encode_plan_t* plan, void* stream);
 
 /*
  * Token-id prefix hash.  Replaces LMCacheEngine._chunk_tokens/_hash/_prefix_hash

@@ -71,6 +71,11 @@ class DecodePlan(ctypes.Structure):
     _fields_ = [("opaque", ctypes.c_uint64 * 256)]
 
 
+class EncodePlan(ctypes.Structure):
+    """struct b200kv_encode_plan_t (opaque, filled by b200kv_encode_layers_plan)"""
+    _fields_ = [("opaque", ctypes.c_uint64 * 256)]
+
+
 assert ctypes.sizeof(Header) == HEADER_BYTES
 
 # name -> (restype, argtypes); every symbol include/b200kv.h declares
@@ -91,6 +96,12 @@ SIGNATURES = {
     "b200kv_decode_plan": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, ctypes.POINTER(KvDesc),
                                     c_vp, c_vp, c_vp, c_vp, c_i64, ctypes.POINTER(DecodePlan), c_vp]),
     "b200kv_decode_layers": (c_i32, [ctypes.POINTER(DecodePlan), c_i32, c_i32, c_vp]),
+    "b200kv_encode_layers_workspace_bytes": (c_i64, [c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
+    "b200kv_encode_layers_plan": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp,
+                                          c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_i64, ctypes.POINTER(EncodePlan),
+                                          c_vp]),
+    "b200kv_encode_layers": (c_i32, [ctypes.POINTER(EncodePlan), c_i32, c_i32, c_vp]),
+    "b200kv_encode_layers_finish": (c_i32, [ctypes.POINTER(EncodePlan), c_vp]),
     "b200kv_sha256_chain": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp]),
     "b200kv_sha256_chain_ready": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, ctypes.c_uint32, c_vp]),
     "b200kv_pack_chunks": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp]),

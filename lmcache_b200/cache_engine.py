@@ -14,7 +14,7 @@ from __future__ import annotations
 import ctypes
 import threading
 import time
-from typing import Dict, Iterable, List, Optional, Tuple, Union
+from typing import Callable, Dict, Iterable, List, Optional, Tuple, Union
 
 import torch
 
@@ -125,7 +125,8 @@ class _HashRun:
             if not self.done.query():
                 self.done.synchronize()                      # the kernel still writes into the buffer
             with _HashRun._pool_lock:
-                if len(_HashRun._pool) < 8:
+                # a buffer the cyclic collector finalised first is closed already: it must not be handed out again
+                if len(_HashRun._pool) < 8 and self.buf.host_ptr:
                     _HashRun._pool.append(self.buf)
                     self.buf = None
             if self.buf is not None:
@@ -181,6 +182,65 @@ class LayerwiseRetrieval:
         """Block the host until every layer is in place."""
         if self.num_layers > 0:
             self._upload.ready(self.num_layers - 1).synchronize()     # the layers are decoded in order on one stream
+
+
+class LayerwiseStore:
+    """What store_layerwise / store_paged_layerwise return: a store whose KV is handed over one layer at a time, as
+    vLLM's KV connector does with save_kv_layer after each attention layer and wait_for_save at the end of the forward
+    pass.  save_layer(l, stream) says that layer l is written in `stream` order; finish(stream) completes the store.
+    Neither waits on the host.  On the compressed host and disk tiers each layer is encoded on a side stream as soon as
+    it is saved (pipeline.LayerwiseEncode); elsewhere save_layer only records the layer and finish() runs the ordinary
+    store.  A handle dropped without finish() stores nothing and gives its device scratch back."""
+
+    def __init__(self, num_layers: int, enc, on_finish: Callable):
+        self.num_layers = num_layers
+        self._enc = enc                     # pipeline.LayerwiseEncode, or None: nothing is encoded layer by layer
+        self._on_finish = on_finish         # on_finish(stream, enc): publish / store, on the calling thread
+        self._saved = [False] * num_layers
+        self._finished = False
+
+    def save_layer(self, layer: int, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Layer `layer` is complete in `stream` order (default: the current stream): its encode is enqueued behind an
+        event on that stream.  ValueError for a layer out of range or saved before, or after finish()."""
+        if self._finished:
+            raise ValueError("save_layer after finish()")
+        if not 0 <= layer < self.num_layers:
+            raise ValueError(f"layer {layer} out of range [0, {self.num_layers})")
+        if self._saved[layer]:
+            raise ValueError(f"layer {layer} was saved before")
+        self._saved[layer] = True
+        if self._enc is not None:
+            self._enc.encode_layer(layer, stream or torch.cuda.current_stream())
+
+    def finish(self, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Complete the store: `stream` (default: the current stream) waits for the encode's last read of the KV, so
+        the caller may overwrite the cache in that stream's order; the containers land on the tier's worker thread, and
+        a later retrieve of these keys waits for them.  ValueError, and nothing is stored, when a layer was never
+        saved."""
+        if self._finished:
+            raise ValueError("finish() was called before")
+        self._finished = True
+        missing = [l for l, s in enumerate(self._saved) if not s]
+        if missing:
+            self.close()
+            raise ValueError(f"finish() before layers {missing} were saved; nothing is stored")
+        stream = stream or torch.cuda.current_stream()
+        enc, self._enc = self._enc, None
+        if enc is not None:
+            stream.wait_event(enc.finish())
+        self._on_finish(stream, enc)
+
+    def close(self) -> None:
+        """drop an unfinished store: its device scratch goes back to the tier's pool"""
+        enc, self._enc = self._enc, None
+        if enc is not None:
+            enc.abandon()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:       # noqa: BLE001 -- interpreter shutdown
+            pass
 
 
 class LMCacheEngine:
@@ -605,6 +665,88 @@ class LMCacheEngine:
         get_kv, uploads = lw
         ret_mask = self._retrieve_paged(tokens, kv_caches, slot_mapping, mask, get_kv)
         return self._layerwise_result(ret_mask, None, len(kv_caches), uploads)
+
+    # ------------------------------------------------------------------ layer-wise store
+    def _layerwise_store_ok(self, dtype: torch.dtype) -> bool:
+        """Can this store be encoded layer by layer?  The compressed host and disk tiers can, for 16-bit KV and chunks of
+        at most 256 tokens (version-3 containers); raw, remote and hybrid tiers cannot."""
+        return (getattr(self.engine_, "begin_layerwise_store", None) is not None and self._fast_path() and
+                self.chunk_size <= N.GROUP_TOKENS and dtype in (torch.bfloat16, torch.float16))
+
+    def _skip_scan(self, chunk_hashes, fmt: str) -> int:
+        """store()'s skip_existing scan: the first chunk whose key the tier does not hold"""
+        for i, h in enumerate(chunk_hashes):
+            if not self.engine_.contains(self._make_key(h, fmt)):
+                return i
+        return len(chunk_hashes)
+
+    def _begin_layerwise(self, tokens, view_fn, fmt: str, num_layers: int, skip_existing: bool,
+                         fallback: Callable) -> LayerwiseStore:
+        """The hash chain and the skip_existing scan run here, on the calling thread: the scan blocks until the chain
+        has produced the digest of the first chunk the tier does not hold (one 256-token SHA-256 step per chunk) plus
+        one dict lookup per chunk.  The plan (no KV read) is enqueued on the tier's encode stream.  finish() makes the
+        touches and the put that store() / store_paged() make, in the same order."""
+        chunk_hashes = self._prefix_hash(tokens)
+        start = self._skip_scan(chunk_hashes, fmt) if skip_existing else 0
+        enc = None
+        if start < len(chunk_hashes):
+            view = view_fn()
+            self._geom = (view.L, view.H, view.D, view.dtype)
+            enc = self.engine_.begin_layerwise_store(view, start * self.chunk_size, self.chunk_size)
+            if enc is None:
+                return LayerwiseStore(num_layers, None, fallback)
+
+        def publish(stream, enc):
+            self._touch(chunk_hashes[:start], fmt)
+            if enc is not None:
+                keys = self._keys_of(chunk_hashes[start:], fmt)
+                self.engine_.put_kv_chunks(keys, None, start * self.chunk_size, self.chunk_size, blocking=False,
+                                           encoded=enc)
+                self._touch(chunk_hashes, fmt)
+        return LayerwiseStore(num_layers, enc, publish)
+
+    @torch.no_grad()
+    def store_paged_layerwise(self, tokens: torch.Tensor, kv_caches, slot_mapping: torch.Tensor,
+                              skip_existing=True) -> LayerwiseStore:
+        """store_paged(), with the KV handed over one layer at a time: the caches may still be unwritten when this is
+        called; call save_layer(l) once layer l is written and finish() after the last layer (LayerwiseStore).  The keys
+        stored, the containers and the eviction touches are those of store_paged(tokens, kv_caches, slot_mapping,
+        skip_existing)."""
+        if self.metadata.fmt != "vllm":
+            raise ValueError(f"paged KV caches use the vllm layout, engine fmt is {self.metadata.fmt}")
+        assert len(tokens.shape) == 1, f"Invalid shape of tokens: {tokens.shape}"
+        assert len(kv_caches) > 0, "Empty kv_caches"
+        assert len(tokens) == slot_mapping.numel(), "Number of slots does not match the input tokens"
+
+        def fallback(stream, enc):
+            with torch.cuda.stream(stream):
+                self.store_paged(tokens, kv_caches, slot_mapping, skip_existing)
+        if not self._layerwise_store_ok(kv_caches[0][0].dtype):
+            return LayerwiseStore(len(kv_caches), None, fallback)
+        return self._begin_layerwise(tokens, lambda: KvView.from_paged(kv_caches, slot_mapping.cuda()), "vllm",
+                                     len(kv_caches), skip_existing, fallback)
+
+    @torch.no_grad()
+    def store_layerwise(self, tokens: torch.Tensor, kv_tensors_raw: KVCache, skip_existing=True) -> LayerwiseStore:
+        """store(), with the KV handed over one layer at a time (see store_paged_layerwise): kv_tensors_raw is store()'s
+        per-layer (K, V) tuple on the GPU, possibly not yet written."""
+        fmt = self.metadata.fmt
+        assert len(tokens.shape) == 1, f"Invalid shape of tokens: {tokens.shape}"
+        assert len(kv_tensors_raw) > 0, "Empty kv_tensors"
+        assert len(tokens) == self._num_tokens_in_kv(kv_tensors_raw, fmt), \
+            "Number of tokens in the kv cache does not match the input tokens"
+
+        def fallback(stream, enc):
+            with torch.cuda.stream(stream):
+                self.store(tokens, kv_tensors_raw, skip_existing)
+        k0 = kv_tensors_raw[0][0]
+        # the kernels must read the caller's tensors in place (KvView.from_tuple would copy tensors of other strides
+        # now, before they are written): anything else takes the ordinary store at finish()
+        in_place = all(t.stride() == k0.stride() and t.stride(2) == 1 for kv in kv_tensors_raw for t in kv)
+        if not k0.is_cuda or not in_place or not self._layerwise_store_ok(k0.dtype):
+            return LayerwiseStore(len(kv_tensors_raw), None, fallback)
+        return self._begin_layerwise(tokens, lambda: KvView.from_tuple(kv_tensors_raw, fmt), fmt, len(kv_tensors_raw),
+                                     skip_existing, fallback)
 
     def close(self):
         self.engine_.close()

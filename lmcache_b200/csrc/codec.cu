@@ -62,7 +62,22 @@ struct EncParams {
     uint32_t* tile_tot;              // [n_chunks][tiles_full] bytes per tile, then exclusive prefix (in place)
     unsigned long long* totals;      // [n_chunks] payload bytes
     unsigned int* err;               // [n_chunks]
+    int32_t lb, nlay;                // this launch codes layers [lb, lb + nlay): planes lb.. and L + lb.. (all: 0, L)
+    // b200kv_encode_layers only (NULL / 0 otherwise): the payload goes to a device arena instead of out + j * out_stride
+    uint8_t* arena;
+    int64_t arena_bytes;
+    unsigned long long* chunk_base;  // [n_chunks] arena offset of chunk j's bytes of this call, ~0 = chunk failed
+    unsigned long long* cursor;      // first free arena byte (device-held across calls)
+    unsigned int* fail_from;         // first failed chunk (n_chunks: none); every later chunk fails too
+    unsigned long long* ptotal;      // [n_chunks] payload bytes of every call so far
+    int64_t* seg;                    // [n_chunks][2L][2] (arena offset, bytes) per plane; mapped host memory
+    int32_t layers_left;             // layers not yet encoded after this call (arena reserve, place_kernel)
 };
+
+// plane of the launch's local plane index: K planes lb.., then V planes L + lb.. (the identity when lb = 0, nlay = L)
+__device__ __forceinline__ int launch_plane(const EncParams& P, int local) {
+    return local + (local < P.nlay ? P.lb : P.L - P.nlay + P.lb);
+}
 
 // section offsets of a container of this call (encode and decode parameter blocks alike)
 template <class Prm>
@@ -149,9 +164,9 @@ template <bool VEC, bool PAGED>
 __global__ void __launch_bounds__(256) absmax_kernel(EncParams P, int64_t total_tokens) {
     const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
-    const int64_t nrows = (int64_t)2 * P.L * total_tokens;
+    const int64_t nrows = (int64_t)2 * P.nlay * total_tokens;
     if (warp >= nrows) return;
-    const int nl = (int)(warp / total_tokens);
+    const int nl = launch_plane(P, (int)(warp / total_tokens));
     const int64_t T = warp % total_tokens;
     const uint16_t* row = P.pt.p[nl] + tok_row<PAGED>(P.slot_map, P.tok_begin + T) * P.sT;
     uint32_t m = 0;
@@ -209,9 +224,11 @@ __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* s_warp
 
 // tile -> (chunk j, group g, plane nl, channel tile ct); tiles of a chunk are ordered (g, nl, ct), which is the
 // order of the streams in the container payload.  Returns false for tiles beyond the (ragged) last chunk.
+// A launch over layers [lb, lb + nlay) has tiles_full = 2 * nlay * tpp tiles per chunk (one group: v3 only); its
+// tile_in_chunk counts the launch's tiles, and the local plane maps to the real one with one select (launch_plane).
 struct TileId { int j, g, nl, ct, t, tok0, gt, tile_in_chunk; };
 __device__ __forceinline__ bool decode_tile(const EncParams& P, uint32_t tile, TileId* id) {
-    const uint32_t per_group = 2u * P.L * P.tpp;
+    const uint32_t per_group = 2u * P.nlay * P.tpp;
     const uint32_t j = tile / (uint32_t)P.tiles_full;
     const uint32_t rem = tile - j * (uint32_t)P.tiles_full;
     id->j = (int)j;
@@ -220,8 +237,9 @@ __device__ __forceinline__ bool decode_tile(const EncParams& P, uint32_t tile, T
     id->g = (int)(rem / per_group);
     if (id->g * kGroup >= id->t) return false;
     const uint32_t rem2 = rem - (uint32_t)id->g * per_group;
-    id->nl = (int)(rem2 / P.tpp);
-    id->ct = (int)(rem2 - (uint32_t)id->nl * P.tpp);
+    const int local = (int)(rem2 / P.tpp);
+    id->ct = (int)(rem2 - (uint32_t)local * P.tpp);
+    id->nl = launch_plane(P, local);
     id->tok0 = id->g * kGroup;
     id->gt = min(kGroup, id->t - id->tok0);
     return true;
@@ -660,7 +678,7 @@ __global__ void __launch_bounds__(1024) enc_scan_kernel(EncParams P) {
     __shared__ unsigned long long s_carry;
     const int j = blockIdx.x;
     const int t = chunk_tokens_of(P, j);
-    const int ntiles = ((t + kGroup - 1) / kGroup) * 2 * P.L * P.tpp;
+    const int ntiles = ((t + kGroup - 1) / kGroup) * 2 * P.nlay * P.tpp;
     uint32_t* tb = P.tile_tot + (int64_t)j * P.tiles_full;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     if (threadIdx.x == 0) s_carry = 0ull;
@@ -786,12 +804,19 @@ __global__ void __launch_bounds__(CT, 12) compact_kernel(EncParams P) {
     uint32_t tile_total;
     const uint32_t my_off = block_excl_scan(len, s_warp, &tile_total);
     const uint64_t base = P.tile_tot[(int64_t)id.j * P.tiles_full + id.tile_in_chunk];
-    const int64_t room = P.out_stride - lo.off_payload;
-    if ((int64_t)(base + tile_total) > room) {          // never write past the slot the caller gave us
-        if (tid == 0) atomicOr(&P.err[id.j], 4u);
-        return;
+    uint8_t* dst;
+    if (P.chunk_base) {                                  // arena: place_kernel gave the chunk room, or marked it failed
+        const unsigned long long cb = P.chunk_base[id.j];
+        if (cb == ~0ull) return;
+        dst = P.arena + cb + base;
+    } else {
+        const int64_t room = P.out_stride - lo.off_payload;
+        if ((int64_t)(base + tile_total) > room) {      // never write past the slot the caller gave us
+            if (tid == 0) atomicOr(&P.err[id.j], 4u);
+            return;
+        }
+        dst = cont + lo.off_payload + base;
     }
-    uint8_t* dst = cont + lo.off_payload + base;
     const uint32_t phase = (uint32_t)(reinterpret_cast<uintptr_t>(dst) & 15u);
     // the image of the tile's byte range must fit the shared-memory stage the launch provided; a tile coded against a
     // foreign CDF may (rarely) exceed it, then every thread writes its own stream straight to the payload
@@ -846,6 +871,79 @@ __global__ void __launch_bounds__(CT, 12) compact_kernel(EncParams P) {
     for (uint32_t i = body0 + 16u * tid; i < body1; i += 16u * CT)
         *reinterpret_cast<uint4*>(dbase + i) = *reinterpret_cast<const uint4*>(stage + i);
     for (uint32_t i = body1 + tid; i < hi_b; i += CT) dbase[i] = stage[i];
+}
+
+// ------------------------------------------------------------------------------------------ arena placement
+// b200kv_encode_layers: after enc_scan_kernel, give each chunk's bytes of this call (its K planes, then its V planes)
+// room in the arena, in chunk order from the device-held cursor, 16-byte aligned.  Chunk j fits iff every chunk before
+// it fits and the arena still holds, after chunks 0..j of this call, the layers still to come for them at this call's
+// size per layer (layers_left / nlay times this call's bytes of chunks 0..j): without that reserve the first calls would
+// fill the arena with every chunk and a later call would find no room even for chunk 0.  The first chunk that does not
+// fit is remembered (fail_from), so the chunks that fit are always a prefix, over this call and every later one.  Then
+// one (offset, bytes) row per plane.  One CTA: a few hundred chunks at most, and it runs once per call.
+__global__ void __launch_bounds__(1024) place_kernel(EncParams P) {
+    __shared__ unsigned long long s_w[32];
+    __shared__ unsigned long long s_carry, s_end;
+    __shared__ unsigned int s_fail;
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    if (tid == 0) {
+        s_carry = s_end = *P.cursor;
+        s_fail = *P.fail_from;
+    }
+    __syncthreads();
+    const unsigned long long start = s_carry;
+    for (int b0 = 0; b0 < P.n_chunks; b0 += 1024) {
+        const int i = b0 + tid;
+        const unsigned long long v = i < P.n_chunks ? (P.totals[i] + 15ull) & ~15ull : 0ull;
+        unsigned long long inc = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long n = __shfl_up_sync(0xffffffffu, inc, o);
+            if (lane >= o) inc += n;
+        }
+        if (lane == 31) s_w[wid] = inc;
+        const unsigned int fail0 = s_fail;
+        const unsigned long long carry = s_carry;
+        __syncthreads();
+        unsigned long long wbase = 0ull;
+        for (int w = 0; w < wid; ++w) wbase += s_w[w];
+        const unsigned long long end = carry + wbase + inc;
+        if (i < P.n_chunks) {
+            const unsigned long long reserve = (end - start) * (unsigned long long)P.layers_left / (unsigned)P.nlay;
+            const bool fits = (unsigned)i < fail0 && end + reserve <= (unsigned long long)P.arena_bytes;
+            P.chunk_base[i] = fits ? end - v : ~0ull;
+            if (fits) {
+                P.ptotal[i] += P.totals[i];
+                atomicMax(&s_end, end);
+            } else {
+                atomicOr(&P.err[i], 16u);
+                atomicMin(&s_fail, (unsigned)i);
+            }
+        }
+        __syncthreads();
+        if (tid == 0) s_carry = s_end;
+        __syncthreads();
+    }
+    if (tid == 0) {
+        *P.cursor = s_carry;
+        *P.fail_from = s_fail;
+    }
+    const int NLc = 2 * P.nlay;
+    for (int k = tid; k < P.n_chunks * NLc; k += 1024) {
+        const int j = k / NLc, pl = k - j * NLc;
+        const uint32_t* tb = P.tile_tot + (int64_t)j * P.tiles_full;
+        const unsigned long long off = tb[pl * P.tpp];
+        const unsigned long long end = pl + 1 < NLc ? (unsigned long long)tb[(pl + 1) * P.tpp] : P.totals[j];
+        const unsigned long long cb = P.chunk_base[j];       // written above by this CTA
+        int64_t* row = P.seg + ((int64_t)j * 2 * P.L + launch_plane(P, pl)) * 2;
+        row[0] = cb == ~0ull ? -1 : (int64_t)(cb + off);
+        row[1] = (int64_t)(end - off);
+    }
+}
+
+__global__ void encl_init_kernel(EncParams P) {
+    *P.cursor = 0ull;
+    *P.fail_from = (unsigned)P.n_chunks;
 }
 
 // ------------------------------------------------------------------------------------------ finalize
@@ -1494,6 +1592,56 @@ static size_t enc_ws_layout(int64_t n_tiles_alloc, int n_chunks, int tempw, int 
     return (o + 255) & ~(size_t)255;
 }
 
+// b200kv_encode_layers_plan's workspace: the state that lives across calls (err, running payload totals, chunk bases,
+// cursor + fail_from), then one call's scratch -- tile totals, payload totals, coder states and temp rows for the tiles
+// of at most max_layers layers.
+struct EnclWs { size_t err, ptotal, cbase, state, tot, totals, rstate, temp, bytes; };
+static EnclWs encl_ws_layout(int n_chunks, int64_t call_tiles) {
+    EnclWs w;
+    size_t o = 0;
+    auto take = [&](size_t* off, size_t n) { *off = o; o = (o + n + 255) & ~(size_t)255; };
+    take(&w.err, (size_t)n_chunks * 4);
+    take(&w.ptotal, (size_t)n_chunks * 8);
+    take(&w.cbase, (size_t)n_chunks * 8);
+    take(&w.state, 16);
+    take(&w.tot, (size_t)call_tiles * 4);
+    take(&w.totals, (size_t)n_chunks * 8);
+    take(&w.rstate, (size_t)call_tiles * CT * 16);
+    take(&w.temp, (size_t)call_tiles * CT * TEMPW_FUSED_RANS_HDR * 4);
+    w.bytes = o;
+    return w;
+}
+
+// What b200kv_encode_layers_plan decided, kept in the caller's b200kv_encode_plan_t: the kernels' parameter block (its
+// counters live in the workspace), the layers encoded so far and the most one call may take.
+constexpr uint32_t kEncPlanMagic = 0x4e4c5045u;   // "EPLN"
+struct EncPlan {
+    uint32_t magic;
+    int32_t max_layers;
+    uint64_t done;           // bit l: layer l has been encoded
+    EncParams P;
+};
+static_assert(sizeof(EncPlan) <= sizeof(b200kv_encode_plan_t), "b200kv_encode_plan_t too small");
+
+constexpr size_t kSmemFused = (size_t)(((CT * SYMW + (CT * kLp * 2 + 3) / 4 + 3) & ~3) + kGroup + 8) * 4;
+constexpr int kStageRans = 12 * 1024;   // compact_kernel's stage without an entropy hint (b200kv_encode_chunks)
+
+// absmax over the rows of the launch's planes (P.lb, P.nlay) and tokens [0, total_tokens) of the call
+static int launch_absmax(const EncParams& P, const b200kv_kv_desc* kv, int64_t total_tokens, cudaStream_t stream) {
+    bool vec = (kv->D % 8 == 0) && (kv->sT % 8 == 0) && (kv->sH % 8 == 0);
+    for (int nl = 0; nl < 2 * P.L && vec; ++nl) vec = (reinterpret_cast<uintptr_t>(P.pt.p[nl]) & 15) == 0;
+    const bool paged = P.slot_map != nullptr;
+    const int64_t rows = 2 * (int64_t)P.nlay * total_tokens;
+    const int64_t blocks = (rows + 7) / 8;
+    B2_REQUIRE(blocks < (1ll << 31), "too many rows in one call");
+    if (vec && !paged) absmax_kernel<true, false><<<(unsigned)blocks, 256, 0, stream>>>(P, total_tokens);
+    else if (vec) absmax_kernel<true, true><<<(unsigned)blocks, 256, 0, stream>>>(P, total_tokens);
+    else if (!paged) absmax_kernel<false, false><<<(unsigned)blocks, 256, 0, stream>>>(P, total_tokens);
+    else absmax_kernel<false, true><<<(unsigned)blocks, 256, 0, stream>>>(P, total_tokens);
+    B2_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
 static size_t dec_ws_layout(int64_t tiles_max, int n_chunks, size_t* off_tb) {
     size_t o = ((size_t)n_chunks * sizeof(DecChunk) + 255) & ~(size_t)255;
     *off_tb = o;
@@ -1626,6 +1774,9 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
     P.out = static_cast<uint8_t*>(out);
     P.out_stride = out_stride;
     P.sizes_out = sizes_out;
+    P.lb = 0; P.nlay = P.L;
+    P.arena = nullptr; P.arena_bytes = 0; P.chunk_base = nullptr; P.cursor = nullptr; P.fail_from = nullptr;
+    P.ptotal = nullptr; P.seg = nullptr; P.layers_left = 0;
     const Layout lo = make_layout(P.L, P.C, chunk_tokens, P.compact);
     B2_REQUIRE(out_stride >= lo.off_payload + 16, "out_stride smaller than the fixed container sections");
 
@@ -1653,20 +1804,11 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
     const int64_t total_tokens = (int64_t)(n_chunks - 1) * chunk_tokens + last_chunk_tokens;
     for (int i = 0; i <= kProfFinalize; ++i) g_prof_have[i] = false;
     {
-        bool vec = (kv->D % 8 == 0) && (kv->sT % 8 == 0) && (kv->sH % 8 == 0);
-        for (int nl = 0; nl < 2 * P.L && vec; ++nl) vec = (reinterpret_cast<uintptr_t>(P.pt.p[nl]) & 15) == 0;
-        const int64_t rows = 2 * (int64_t)P.L * total_tokens;
-        const int64_t blocks = (rows + 7) / 8;
-        B2_REQUIRE(blocks < (1ll << 31), "too many rows in one call");
         ProfScope prof(kProfAbsmax, stream);
-        if (vec && !paged) absmax_kernel<true, false><<<(unsigned)blocks, 256, 0, stream>>>(P, total_tokens);
-        else if (vec) absmax_kernel<true, true><<<(unsigned)blocks, 256, 0, stream>>>(P, total_tokens);
-        else if (!paged) absmax_kernel<false, false><<<(unsigned)blocks, 256, 0, stream>>>(P, total_tokens);
-        else absmax_kernel<false, true><<<(unsigned)blocks, 256, 0, stream>>>(P, total_tokens);
-        B2_CHECK_CUDA(cudaGetLastError());
+        if (int rc = launch_absmax(P, kv, total_tokens, stream)) return rc;
     }
     // 2) encode (streams -> temp rows, lengths, tile totals)
-    const size_t smem_fused = (size_t)(((CT * SYMW + (CT * kLp * 2 + 3) / 4 + 3) & ~3) + kGroup + 8) * 4;
+    const size_t smem_fused = kSmemFused;
     const size_t smem_split = (size_t)(((CT * PAIRW + 3) & ~3) + kGroup + 4) * 4;
     const size_t smem_cdf = (size_t)(CT * PAIRW + kGroup) * 4;
 #define B2_LAUNCH_ENC1(FUSED, DT, PAGED, CODER, SMEM)                                                      \
@@ -1724,6 +1866,130 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
         compact_kernel<<<(unsigned)n_tiles, CT, (size_t)P.stage_bytes, stream>>>(P);
         finalize_kernel<<<(n_chunks + 127) / 128, 128, 0, stream>>>(P);
     }
+    B2_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int64_t b200kv_encode_layers_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t chunk_tokens, int32_t n_chunks,
+                                             int32_t max_layers) {
+    if (L <= 0 || H <= 0 || D <= 0 || chunk_tokens <= 0 || chunk_tokens > kGroup || n_chunks <= 0 || max_layers <= 0 ||
+        max_layers > L)
+        return -2;
+    return (int64_t)encl_ws_layout(n_chunks, (int64_t)n_chunks * 2 * max_layers * tiles_per_plane(H * D)).bytes;
+}
+
+int b200kv_encode_layers_plan(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
+                              int32_t last_chunk_tokens, const float* key_bins, const float* value_bins, int32_t coder,
+                              void* arena, int64_t arena_bytes, void* fixed_out, int64_t fixed_stride, int64_t* seg_sizes_out,
+                              uint64_t* sizes_out, int32_t max_layers, void* workspace, int64_t workspace_bytes,
+                              b200kv_encode_plan_t* plan_out, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B2_REQUIRE(plan_out != nullptr, "plan is NULL");
+    EncPlan* plan = reinterpret_cast<EncPlan*>(plan_out);
+    plan->magic = 0u;
+    EncParams& P = plan->P;
+    B2_REQUIRE(key_bins && value_bins, "bins are NULL");
+    B2_REQUIRE((coder & 0xff) == CODER_RANS_COMPACT,
+               "the layer-wise encode writes compact containers only (B200KV_CODER_RANS_COMPACT)");
+    if (int rc = make_plane_table(kv, key_bins, value_bins, &P.pt)) return rc;
+    B2_REQUIRE(n_chunks > 0 && chunk_tokens > 0, "n_chunks / chunk_tokens must be positive");
+    B2_REQUIRE(chunk_tokens <= kGroup, "the compact container (B200KV_CODER_RANS_COMPACT) holds chunks of at most 256 tokens");
+    B2_REQUIRE(last_chunk_tokens > 0 && last_chunk_tokens <= chunk_tokens, "last_chunk_tokens out of range");
+    B2_REQUIRE(tok_begin >= 0, "tok_begin must be >= 0");
+    B2_REQUIRE(max_layers > 0 && max_layers <= kv->L, "max_layers out of range");
+    B2_REQUIRE(arena != nullptr && arena_bytes >= 0 && seg_sizes_out != nullptr && sizes_out != nullptr, "bad outputs");
+    B2_REQUIRE(fixed_out != nullptr && (reinterpret_cast<uintptr_t>(fixed_out) & 15) == 0 && (fixed_stride & 15) == 0,
+               "fixed_out / fixed_stride must be 16-byte aligned");
+    P.sT = kv->sT; P.sH = kv->sH; P.tok_begin = tok_begin;
+    P.slot_map = kv->slot_map;
+    P.L = kv->L; P.H = kv->H; P.D = kv->D; P.C = kv->H * kv->D; P.dtype = kv->dtype;
+    P.n_chunks = n_chunks; P.chunk_tokens = chunk_tokens; P.last_chunk_tokens = last_chunk_tokens;
+    P.tpp = tiles_per_plane(P.C);
+    P.coder = CODER_RANS;
+    P.compact = 1;
+    P.tempw = TEMPW_FUSED_RANS_HDR;
+    P.stage_bytes = kStageRans;
+    const Layout lo = make_layout(P.L, P.C, chunk_tokens, 1);
+    B2_REQUIRE(fixed_stride >= lo.off_payload, "fixed_stride smaller than the fixed container sections");
+    P.out = static_cast<uint8_t*>(fixed_out);
+    P.out_stride = fixed_stride;
+    P.sizes_out = sizes_out;
+    P.arena = static_cast<uint8_t*>(arena);
+    P.arena_bytes = arena_bytes;
+    P.seg = seg_sizes_out;
+    const int64_t call_tiles = (int64_t)n_chunks * 2 * max_layers * P.tpp;
+    B2_REQUIRE(call_tiles < (1ll << 31), "too many tiles in one call");
+    const EnclWs w = encl_ws_layout(n_chunks, call_tiles);
+    B2_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)w.bytes, "workspace too small");
+    uint8_t* ws = static_cast<uint8_t*>(workspace);
+    P.err = reinterpret_cast<unsigned int*>(ws + w.err);
+    P.ptotal = reinterpret_cast<unsigned long long*>(ws + w.ptotal);
+    P.chunk_base = reinterpret_cast<unsigned long long*>(ws + w.cbase);
+    P.cursor = reinterpret_cast<unsigned long long*>(ws + w.state);
+    P.fail_from = reinterpret_cast<unsigned int*>(ws + w.state + 8);
+    P.tile_tot = reinterpret_cast<uint32_t*>(ws + w.tot);
+    P.totals = reinterpret_cast<unsigned long long*>(ws + w.totals);
+    P.rstate = reinterpret_cast<uint32_t*>(ws + w.rstate);
+    P.temp = reinterpret_cast<uint32_t*>(ws + w.temp);
+    // counters; the fixed images too, so that their padding bytes are zero whatever the buffer held before
+    B2_CHECK_CUDA(cudaMemsetAsync(ws, 0, w.tot, stream));
+    B2_CHECK_CUDA(cudaMemsetAsync(fixed_out, 0, (size_t)fixed_stride * n_chunks, stream));
+    encl_init_kernel<<<1, 1, 0, stream>>>(P);
+    B2_CHECK_CUDA(cudaGetLastError());
+    B2_CHECK_CUDA(cudaFuncSetAttribute(compact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, P.stage_bytes));
+    plan->max_layers = max_layers;
+    plan->done = 0ull;
+    plan->magic = kEncPlanMagic;
+    return 0;
+}
+
+int b200kv_encode_layers(b200kv_encode_plan_t* plan_in, int32_t layer_begin, int32_t layer_end, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B2_REQUIRE(plan_in != nullptr, "plan is NULL");
+    EncPlan* plan = reinterpret_cast<EncPlan*>(plan_in);
+    B2_REQUIRE(plan->magic == kEncPlanMagic, "not a plan made by b200kv_encode_layers_plan");
+    EncParams P = plan->P;
+    B2_REQUIRE(layer_begin >= 0 && layer_begin < layer_end && layer_end <= P.L, "layer range out of range");
+    B2_REQUIRE(layer_end - layer_begin <= plan->max_layers, "more layers than the plan's workspace holds");
+    const uint64_t bits = (layer_end - layer_begin == 64 ? ~0ull : ((1ull << (layer_end - layer_begin)) - 1ull)) << layer_begin;
+    B2_REQUIRE((plan->done & bits) == 0ull, "a layer of the range was encoded before");
+    P.lb = layer_begin;
+    P.nlay = layer_end - layer_begin;
+    P.layers_left = P.L - __builtin_popcountll(plan->done | bits);
+    P.tiles_full = 2 * P.nlay * P.tpp;
+    const int64_t n_tiles = (int64_t)P.n_chunks * P.tiles_full;
+    const int64_t total_tokens = (int64_t)(P.n_chunks - 1) * P.chunk_tokens + P.last_chunk_tokens;
+    b200kv_kv_desc kv{};
+    kv.D = P.D; kv.sT = P.sT; kv.sH = P.sH;
+    if (int rc = launch_absmax(P, &kv, total_tokens, stream)) return rc;
+#define B2_LAUNCH_ENCL(DT, PAGED)                                                                                      \
+    do {                                                                                                               \
+        B2_CHECK_CUDA(cudaFuncSetAttribute(encode_kernel<true, DT, PAGED, CODER_RANS>,                                 \
+                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemFused));             \
+        encode_kernel<true, DT, PAGED, CODER_RANS><<<(unsigned)n_tiles, CT, kSmemFused, stream>>>(P);                  \
+    } while (0)
+    if (P.dtype == B200KV_DT_BF16) { if (P.slot_map) B2_LAUNCH_ENCL(0, true); else B2_LAUNCH_ENCL(0, false); }
+    else { if (P.slot_map) B2_LAUNCH_ENCL(1, true); else B2_LAUNCH_ENCL(1, false); }
+#undef B2_LAUNCH_ENCL
+    B2_CHECK_CUDA(cudaGetLastError());
+    enc_scan_kernel<<<(unsigned)P.n_chunks, 1024, 0, stream>>>(P);
+    place_kernel<<<1, 1024, 0, stream>>>(P);
+    compact_kernel<<<(unsigned)n_tiles, CT, (size_t)P.stage_bytes, stream>>>(P);
+    B2_CHECK_CUDA(cudaGetLastError());
+    plan->done |= bits;
+    return 0;
+}
+
+int b200kv_encode_layers_finish(const b200kv_encode_plan_t* plan_in, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B2_REQUIRE(plan_in != nullptr, "plan is NULL");
+    const EncPlan* plan = reinterpret_cast<const EncPlan*>(plan_in);
+    B2_REQUIRE(plan->magic == kEncPlanMagic, "not a plan made by b200kv_encode_layers_plan");
+    EncParams P = plan->P;
+    const uint64_t all = P.L == 64 ? ~0ull : (1ull << P.L) - 1ull;
+    B2_REQUIRE(plan->done == all, "a layer was never encoded");
+    P.totals = P.ptotal;                   // headers carry the payload of every call
+    finalize_kernel<<<(P.n_chunks + 127) / 128, 128, 0, stream>>>(P);
     B2_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -32,7 +32,7 @@ import numpy as np
 import torch
 
 from lmcache_b200 import _native as N
-from lmcache_b200.codec import CacheGenCodec, EncodeTicket, KvView, PinnedBuffer, parse_header, plane_offsets
+from lmcache_b200.codec import CacheGenCodec, EncodedBatch, EncodeTicket, KvView, PinnedBuffer, parse_header, plane_offsets
 
 
 def wave_chunks_default() -> int:
@@ -151,6 +151,13 @@ class EncodePipeline:
             self.ring = EncodeRing(self.codec, view.L, view.H, view.D, chunk_size, view.device)
         return self.ring
 
+    def submit_encoded(self, enc: "LayerwiseEncode", items: Sequence) -> StoreJob:
+        """Hand a finished layer-wise encode (LayerwiseEncode.finish has been called) to the worker: it lands the
+        containers that fit the arena, as one wave, in submission order with the other stores."""
+        job = StoreJob(1)
+        self._q.put((enc.pool, enc.slot, 0, list(items), job))
+        return job
+
     def submit(self, view: KvView, tok_begin: int, chunk_size: int, items: Sequence,
                stream: Optional[torch.cuda.Stream] = None) -> StoreJob:
         """Enqueue the encode of tokens [tok_begin, T) of `view`, len(items) chunks, in waves.  Returns once every wave
@@ -262,7 +269,10 @@ def land(slab, slot: WaveSlot, batch, blocks: Optional[list] = None) -> List[Hos
     """Store-pipeline sink side: copy a finished wave's containers out of slot.dev into fresh blocks of `slab` (exactly
     their bytes, on the device's copy stream), wait for the copies, and parse every header.  Raises -- with every block
     freed -- when a copy fails or a container carries an encoder error.  `blocks`: blocks the caller allocated for the
-    first len(blocks) containers (a bounded tier); only those are landed."""
+    first len(blocks) containers (a bounded tier); only those are landed.  A layer-wise store's slot (SegmentSlot) lands
+    through land_segments."""
+    if isinstance(slot, SegmentSlot):
+        return land_segments(slab, slot, batch, blocks)
     dev = slot.dev.device
     cs = _d2h_stream(dev)
     if blocks is None:
@@ -288,6 +298,227 @@ def land(slab, slot: WaveSlot, batch, blocks: Optional[list] = None) -> List[Hos
             hd = parse_header(blk.view())
             recs.append(HostContainer(blk, blk.nbytes, hd, po[j, :2 * hd.L + 1].copy() if po[j, 0] >= 0 else None))
         return recs
+    except BaseException:
+        for blk in blocks:
+            blk.free()
+        raise
+
+
+def layerwise_store_budget_default() -> int:
+    """LMCACHE_B200_LAYERWISE_STORE_MB: the most device arena one layer-wise store takes (default 1024 MB, about what
+    the ordinary store's EncodeRing holds)."""
+    return max(1, int(os.environ.get("LMCACHE_B200_LAYERWISE_STORE_MB", "1024"))) << 20
+
+
+def arena_placement(seg_bytes: np.ndarray, arena_bytes: int, layers: Optional[Sequence[int]] = None):
+    """Host statement of the layer-wise store's arena rule (place_kernel in codec.cu), for tests and sizing.
+    seg_bytes[c, j]: payload bytes of chunk j in layer call c (its K planes, then its V planes); layers[c]: the layers
+    of call c (default 1 each).  Calls are placed in order; within a call, chunk j's bytes go 16-byte aligned at the
+    cursor.  Chunk j fits if, after chunks 0..j of the call, the arena still holds the layers still to come at this
+    call's size per layer (a reserve, so that a later call finds room for the chunks an earlier one accepted).  A chunk
+    that does not fit fails, and so does every later chunk, in this call and every later one.  Returns (base
+    int64[calls, n], -1 for the chunks that failed; the number of chunks that fit)."""
+    seg_bytes = np.asarray(seg_bytes, dtype=np.int64)
+    calls, n = seg_bytes.shape
+    layers = list(layers) if layers is not None else [1] * calls
+    base = np.full((calls, n), -1, dtype=np.int64)
+    cursor, fail = 0, n
+    for c in range(calls):
+        left = sum(layers[c + 1:])
+        start = cursor
+        for j in range(min(n, fail)):
+            size = (int(seg_bytes[c, j]) + 15) & ~15
+            if cursor + size + (cursor + size - start) * left // layers[c] > arena_bytes:
+                fail = j
+                break
+            base[c, j] = cursor
+            cursor += size
+    base[:, fail:] = -1                      # a failed chunk's earlier segments stay in the arena, unused
+    return base, fail
+
+
+class SegmentSlot:
+    """Device scratch of one layer-wise store: the payload arena, the chunks' fixed-section images, the encode
+    workspace, and in mapped page-locked memory the container sizes and the (arena offset, bytes) row of every plane."""
+
+    def __init__(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, L: int, device):
+        self.arena = torch.empty(max(16, arena_bytes), dtype=torch.uint8, device=device)
+        self.fixed = torch.empty(max(16, fixed_bytes), dtype=torch.uint8, device=device)
+        self.ws = torch.empty(max(16, ws_bytes), dtype=torch.uint8, device=device)
+        self.sizes = PinnedBuffer(max(64, 8 * n_chunks))
+        self.seg = PinnedBuffer(max(64, 16 * 2 * L * n_chunks))
+        self.arena_bytes = arena_bytes
+        self.ticket = None
+        self.layouts: tuple = ()            # (off_payload of a full chunk, of the last chunk)
+        self.fixed_stride = 0
+        self.n_chunks, self.L = 0, L
+
+    def holds(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, L: int) -> bool:
+        return (self.arena.numel() >= arena_bytes and self.fixed.numel() >= fixed_bytes and self.ws.numel() >= ws_bytes
+                and self.sizes.nbytes >= 8 * n_chunks and self.seg.nbytes >= 32 * L * n_chunks)
+
+    def close(self) -> None:
+        self.sizes.close()
+        self.seg.close()
+        self.arena = self.fixed = self.ws = None
+
+
+class SegmentPool:
+    """Reusable SegmentSlots for the layer-wise stores of one tier and device, and the stream they encode on.  A slot
+    is reused by the next store that fits it; at most `keep` idle slots are kept.  Every kernel that touches a slot runs
+    on `stream` and its tensors are allocated there, so reuse and release are ordered by the stream; the worker hands a
+    slot back only after its device->host copies have completed."""
+
+    def __init__(self, device, keep: int = 2):
+        self.device = torch.device(device)
+        self.stream = torch.cuda.Stream(device=self.device)
+        self.keep = keep
+        self._free: List[SegmentSlot] = []
+        self._lock = threading.Lock()
+
+    def acquire(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, L: int) -> SegmentSlot:
+        with self._lock:
+            for s in self._free:
+                if s.holds(arena_bytes, fixed_bytes, ws_bytes, n_chunks, L):
+                    self._free.remove(s)
+                    return s
+        with torch.cuda.device(self.device), torch.cuda.stream(self.stream):
+            return SegmentSlot(arena_bytes, fixed_bytes, ws_bytes, n_chunks, L, self.device)
+
+    def release(self, slot: SegmentSlot) -> None:
+        slot.ticket = None
+        with self._lock:
+            self._free.append(slot)
+            drop = self._free[:-self.keep] if len(self._free) > self.keep else []
+            self._free = self._free[len(drop):]
+        for s in drop:
+            s.close()
+
+    def close(self) -> None:
+        with self._lock:
+            free, self._free = self._free, []
+        self.stream.synchronize()
+        for s in free:
+            s.close()
+
+
+class _SegmentTicket:
+    """The EncodeTicket of a layer-wise store: wait() blocks the worker until the finish step has run and returns the
+    batch of the containers that fit the arena (a prefix of the chunks)."""
+
+    def __init__(self, slot: SegmentSlot, event: torch.cuda.Event, keep):
+        self.slot, self.event, self.keep = slot, event, keep
+
+    def wait(self) -> EncodedBatch:
+        self.event.synchronize()
+        self.keep = None
+        sizes = list((ctypes.c_uint64 * self.slot.n_chunks).from_address(self.slot.sizes.host_ptr))
+        k = next((j for j, s in enumerate(sizes) if s == 0), len(sizes))
+        return EncodedBatch(self.slot.fixed, self.slot.fixed_stride, [int(s) for s in sizes[:k]], 0,
+                            N.CODER_RANS_COMPACT)
+
+
+class LayerwiseEncode:
+    """One layer-wise store's encode (b200kv_encode_layers_plan / _layers / _finish) on the pool's stream.  The plan is
+    made at once; encode_layer(l, stream) makes the encode stream wait for `stream` and enqueues layer l; finish()
+    enqueues the headers and returns the event after which the KV is no longer read and the containers are complete.
+    The host never waits.  The arena is the airtight bound of the chunks (max_total_bytes - off_payload each, plus the
+    alignment of one segment per layer), capped at `budget`: past the cap the later chunks fail and become misses."""
+
+    def __init__(self, codec: CacheGenCodec, pool: SegmentPool, view: KvView, tok_begin: int, chunk_size: int,
+                 budget: Optional[int] = None):
+        if view.L > codec.nlayers:
+            raise ValueError(f"KV has {view.L} layers but the bin table of this model has {codec.nlayers}")
+        n_tok = view.ntokens - tok_begin
+        n = (n_tok + chunk_size - 1) // chunk_size
+        last = n_tok - (n - 1) * chunk_size
+        L, H, D = view.L, view.H, view.D
+        lo = N.container_layout(L, H, D, chunk_size, N.CODER_RANS_COMPACT)
+        lo_last = N.container_layout(L, H, D, last, N.CODER_RANS_COMPACT)
+        stride = (lo.off_payload + 15) & ~15
+        per_chunk = lo.max_total_bytes - lo.off_payload + 16 * L
+        arena = min(n * per_chunk, budget or layerwise_store_budget_default())
+        lib = N.lib()
+        ws_bytes = N.check(lib.b200kv_encode_layers_workspace_bytes(L, H, D, chunk_size, n, 1), "encode_layers_workspace")
+        self.pool, self.view, self.L, self.n_chunks = pool, view, L, n
+        self.plan = N.EncodePlan()
+        self.slot = pool.acquire(arena, n * stride, ws_bytes, n, L)
+        self.slot.n_chunks, self.slot.L, self.slot.fixed_stride = n, L, stride
+        self.slot.layouts = (int(lo.off_payload), int(lo_last.off_payload))
+        self.done: Optional[torch.cuda.Event] = None
+        s = self.slot
+        try:
+            with torch.cuda.device(pool.device):
+                view.record_stream(pool.stream)          # the caller's KV outlives the encode's last read of it
+                N.check(lib.b200kv_encode_layers_plan(ctypes.byref(view.desc), tok_begin, n, chunk_size, last, codec._kb,
+                                                      codec._vb, N.CODER_RANS_COMPACT, s.arena.data_ptr(), arena,
+                                                      s.fixed.data_ptr(), stride, s.seg.dev_ptr, s.sizes.dev_ptr, 1,
+                                                      s.ws.data_ptr(), s.ws.numel(), ctypes.byref(self.plan),
+                                                      pool.stream.cuda_stream), "encode_layers_plan")
+        except BaseException:
+            self.abandon()
+            raise
+
+    def encode_layer(self, layer: int, stream: torch.cuda.Stream) -> None:
+        with torch.cuda.device(self.pool.device):
+            ev = torch.cuda.Event()
+            ev.record(stream)
+            self.pool.stream.wait_event(ev)
+            N.check(N.lib().b200kv_encode_layers(ctypes.byref(self.plan), layer, layer + 1, self.pool.stream.cuda_stream),
+                    "encode_layers")
+
+    def finish(self) -> torch.cuda.Event:
+        with torch.cuda.device(self.pool.device):
+            N.check(N.lib().b200kv_encode_layers_finish(ctypes.byref(self.plan), self.pool.stream.cuda_stream),
+                    "encode_layers_finish")
+            self.done = torch.cuda.Event()
+            self.done.record(self.pool.stream)
+        self.slot.ticket = _SegmentTicket(self.slot, self.done, self.view)
+        self.view = None
+        return self.done
+
+    def abandon(self) -> None:
+        """give the slot back without landing anything (the kernels already enqueued run on; the pool's stream orders
+        the slot's next user after them)"""
+        if self.slot is not None:
+            slot, self.slot, self.view = self.slot, None, None
+            self.pool.release(slot)
+
+
+def land_segments(slab, slot: SegmentSlot, batch, blocks: Optional[list] = None) -> List[HostContainer]:
+    """land() for a layer-wise store: container j is assembled in a fresh block of `slab` from its fixed-section image
+    and its 2L plane segments in the arena (one batched device->host copy of 1 + 2L ranges per container, all
+    containers in one call), and its plane offsets come from the segment sizes.  Raises -- with every block freed --
+    when a copy fails, the segments do not add up to the container's size, or a header carries an encoder error."""
+    if blocks is None:
+        blocks = [slab.alloc(size) for size in batch.sizes]
+    n, L = len(blocks), slot.L
+    try:
+        if n == 0:
+            return []
+        seg = np.frombuffer(slot.seg.view(), dtype=np.int64, count=slot.n_chunks * 2 * L * 2)
+        seg = seg.reshape(slot.n_chunks, 2 * L, 2)[:n]
+        full, last = slot.layouts
+        fixed = np.array([last if j == slot.n_chunks - 1 else full for j in range(n)], dtype=np.int64)
+        planes = np.concatenate([fixed[:, None], fixed[:, None] + np.cumsum(seg[:, :, 1], axis=1)], axis=1)
+        sizes = np.asarray([b.nbytes for b in blocks], dtype=np.int64)
+        if (seg[:, :, 0] < 0).any() or not np.array_equal(planes[:, -1], np.asarray(batch.sizes[:n], dtype=np.int64)):
+            raise N.NativeError("layer-wise store: plane segments do not add up to the container sizes")
+        host = np.array([b.host_ptr for b in blocks], dtype=np.uint64)
+        dsts = np.concatenate([host[:, None], host[:, None] + planes[:, :-1].astype(np.uint64)], axis=1)
+        fbase = slot.fixed.data_ptr() + np.arange(n, dtype=np.uint64) * np.uint64(slot.fixed_stride)
+        srcs = np.concatenate([fbase[:, None], np.uint64(slot.arena.data_ptr()) + seg[:, :, 0].astype(np.uint64)], axis=1)
+        lens = np.concatenate([fixed[:, None], seg[:, :, 1]], axis=1)
+        assert (lens.sum(axis=1) == sizes).all()
+        dev = slot.arena.device
+        cs = _d2h_stream(dev)
+        with torch.cuda.device(dev):
+            try:
+                _batch_copy(np.ascontiguousarray(dsts.ravel()), np.ascontiguousarray(srcs.ravel()),
+                            np.ascontiguousarray(lens.ravel()), cs)
+            finally:
+                cs.synchronize()             # no block leaves this function while a copy may still write it
+        return [HostContainer(blk, blk.nbytes, parse_header(blk.view()), planes[j].copy()) for j, blk in enumerate(blocks)]
     except BaseException:
         for blk in blocks:
             blk.free()

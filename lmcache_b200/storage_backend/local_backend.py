@@ -263,6 +263,13 @@ class _Store:
         self.since = since
 
 
+def _miss_beyond(entries, batch) -> None:
+    """A layer-wise store's batch holds the prefix of its chunks that fit the device arena: the rest are misses."""
+    for e in entries[len(batch.sizes):]:
+        if e.error is None:
+            e.error = MemoryError("chunk did not fit the layer-wise store's device arena (LMCACHE_B200_LAYERWISE_STORE_MB)")
+
+
 class _CEntry:
     """One stored chunk: its container's record (pipeline.HostContainer) plus the tier's bookkeeping."""
     __slots__ = ("rec", "path", "ready", "error", "store", "pins", "retired")
@@ -322,6 +329,7 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         self._pipe = EncodePipeline(self.codec, self._sink)
         self._upload: Optional[UploadRing] = None
         self._layerwise = None                # pipeline.LayerwiseUploader, made by the first layer-wise retrieve
+        self._segments = None                 # pipeline.SegmentPool, made by the first layer-wise store
         self._release = DeferredFree()        # blocks uploads may still read: retired entries, the disk tier's file reads
         self._closed = False
 
@@ -342,6 +350,7 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
             recs = land(self.slab, slot, batch, blocks) if blocks is None or blocks else []
             for e, rec in zip(entries, recs):
                 e.rec = rec
+            _miss_beyond(entries, batch)
         except BaseException as err:     # noqa: BLE001 -- the entries become misses; the job reports the error
             for e in entries:
                 e.error = err
@@ -427,12 +436,17 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
     def _new_store(self) -> _Store:
         return _Store(getattr(self._touched, "tick", None) if self.capacity is not None else None)
 
-    def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True) -> int:
+    def _submit(self, view, tok_begin: int, chunk_size: int, entries, encoded):
+        return self._pipe.submit(view, tok_begin, chunk_size, entries) if encoded is None else \
+            self._pipe.submit_encoded(encoded, entries)
+
+    def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True, encoded=None) -> int:
         # `keys` may be lazy (the engine's hash chain produces key i after keys 0..i-1): the encode waves
         # need no keys, so they are enqueued first; the entries are published as their keys arrive.  Readers wait on `ready`.
+        # encoded: a finished pipeline.LayerwiseEncode of these chunks (store_layerwise), landed instead of encoding `view`
         store = self._new_store()
         entries = [_CEntry(store) for _ in range(len(keys))]
-        job = self._pipe.submit(view, tok_begin, chunk_size, entries)
+        job = self._submit(view, tok_begin, chunk_size, entries, encoded)
         old = []
         for k, e in zip(keys, entries):
             with self.update_lock:
@@ -510,6 +524,18 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         return upload_decode_layerwise(self.codec, self._layerwise_uploader(dst.device), self._pinned_records(keys, pinned),
                                        dst, dst_tok0, chunk_size, on_done=lambda: self._unpin(pinned))
 
+    def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int):
+        """A pipeline.LayerwiseEncode of tokens [tok_begin, T) of `view` (whose KV may not be written yet), or None
+        when this tier's containers for `chunk_size` are not version 3 (the layer-wise encode writes no other)."""
+        from lmcache_b200.pipeline import LayerwiseEncode, SegmentPool
+        if self.codec.coder_for(chunk_size) != N.CODER_RANS_COMPACT:
+            return None
+        if self._segments is None or self._segments.device != view.device:
+            if self._segments is not None:
+                self._segments.close()
+            self._segments = SegmentPool(view.device)
+        return LayerwiseEncode(self.codec, self._segments, view, tok_begin, chunk_size)
+
     def _layerwise_uploader(self, device):
         from lmcache_b200.pipeline import LayerwiseUploader
         if self._layerwise is None or self._layerwise.device != device:
@@ -579,6 +605,8 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
             return
         self._closed = True
         self._pipe.close()
+        if self._segments is not None:
+            self._segments.close()
         if self._layerwise is not None:
             self._layerwise.close()
         try:
@@ -710,6 +738,7 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
                 e.error = err
             raise
         else:
+            _miss_beyond(entries, batch)
             for e, rec in zip(entries, recs):
                 e.rec = rec
                 if self.capacity is not None and not self._make_file_room(e, rec.nbytes):
@@ -733,7 +762,7 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
             for e in entries:
                 e.ready.set()                             # readers see the entry only once its file is in place
 
-    def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True) -> int:
+    def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True, encoded=None) -> int:
         store = self._new_store()
         entries = [_CEntry(store) for _ in keys]
         for k, e in zip(keys, entries):
@@ -743,7 +772,7 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
             for e in entries:
                 self.dict[e.path] = e                     # an overwritten chunk's file is replaced atomically by the rename
         # the parent's sink sets `ready` before the file exists: keep readers out until the file is written
-        job = self._pipe.submit(view, tok_begin, chunk_size, entries)
+        job = self._submit(view, tok_begin, chunk_size, entries, encoded)
         self.touch(keys)
         if blocking:
             job.wait()
