@@ -37,6 +37,10 @@ class LMCacheEngineConfig:
     # disk tier); beyond it chunks are evicted from the tail of the coldest chain (lmcache_b200/eviction.py).  None = no
     # bound.  Only the two CacheGen tiers honour it (CreateStorageBackend rejects it elsewhere).
     local_capacity_bytes: Optional[int] = None
+    # not in the reference: bytes of device memory that keep copies of the local CacheGen tier's containers, so that a
+    # retrieve of a resident chunk decodes it in place instead of uploading it (lmcache_b200/device_cache.py).  None =
+    # off.  The level is inclusive: every device copy has its tier copy beside it.  Only the two CacheGen tiers take it.
+    device_cache_bytes: Optional[int] = None
 
     def __post_init__(self):
         if self.local_serde is None:
@@ -47,21 +51,26 @@ class LMCacheEngineConfig:
         c = self.local_capacity_bytes
         if c is not None and (isinstance(c, bool) or not isinstance(c, int) or c <= 0):
             raise ValueError(f"Invalid local capacity: {c!r} (a positive number of bytes, or None)")
+        d = self.device_cache_bytes
+        if d is not None and (isinstance(d, bool) or not isinstance(d, int) or d <= 0):
+            raise ValueError(f"Invalid device cache size: {d!r} (a positive number of bytes, or None)")
 
     @staticmethod
     def from_defaults(chunk_size: int = 256, local_device: str = "cuda",
                       remote_url: str = "redis://localhost:6379", remote_serde: str = "torch",
                       pipelined_backend: bool = False, save_decode_cache: bool = False,
                       local_serde: Optional[str] = None,
-                      local_capacity_bytes: Optional[int] = None) -> "LMCacheEngineConfig":
+                      local_capacity_bytes: Optional[int] = None,
+                      device_cache_bytes: Optional[int] = None) -> "LMCacheEngineConfig":
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
-                                   save_decode_cache, local_serde, local_capacity_bytes)
+                                   save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes)
 
     @staticmethod
     def from_legacy(chunk_size: int = 256, backend: str = "cuda", persist_path: Optional[str] = None,
                     remote_serde: Optional[str] = "torch", pipelined_backend: bool = False,
                     save_decode_cache: bool = False, local_serde: Optional[str] = None,
-                    local_capacity_bytes: Optional[int] = None) -> "LMCacheEngineConfig":
+                    local_capacity_bytes: Optional[int] = None,
+                    device_cache_bytes: Optional[int] = None) -> "LMCacheEngineConfig":
         """backend: "cpu" | "cuda" | "file://<dir>/" | "<scheme>://<host>:<port>" (config.py:51-82)."""
         local_device: Optional[str] = None
         remote_url: Optional[str] = None
@@ -72,7 +81,7 @@ class LMCacheEngineConfig:
         elif _URL_RE.match(backend):
             remote_url = backend
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
-                                   save_decode_cache, local_serde, local_capacity_bytes)
+                                   save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes)
 
     @staticmethod
     def from_file(file_path: str) -> "LMCacheEngineConfig":
@@ -87,6 +96,7 @@ class LMCacheEngineConfig:
         save_decode_cache = cfg.get("save_decode_cache", False)
         local_serde = cfg.get("local_serde", None)
         local_capacity_bytes = cfg.get("local_capacity_bytes", None)
+        device_cache_bytes = cfg.get("device_cache_bytes", None)
 
         if local_device in ("cpu", "cuda", None):
             pass
@@ -99,7 +109,7 @@ class LMCacheEngineConfig:
             raise ValueError(f"Invalid remote storage url: {remote_url}")
 
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
-                                   save_decode_cache, local_serde, local_capacity_bytes)
+                                   save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes)
 
 
 class GlobalConfig:

@@ -34,9 +34,17 @@ class PrefixLRU:
 
     def touch(self, keys: Iterable[Hashable]) -> None:
         """One call: keys[i] (chain position i, counted from chunk 0) gets the stamp (T, -i)."""
+        self.touch_at(keys, self.new_tick())
+
+    def new_tick(self) -> int:
+        """a fresh tick for a call whose keys are stamped in several parts (touch_at)"""
         self._tick += 1
+        return self._tick
+
+    def touch_at(self, keys: Iterable[Hashable], tick: int, first: int = 0) -> None:
+        """Part of the call of `tick`: keys[i] is at chain position first + i and gets the stamp (tick, -(first + i))."""
         for i, k in enumerate(keys):
-            s = (self._tick, -i)
+            s = (tick, -(first + i))
             self._stamp[k] = s
             heapq.heappush(self._heap, (s, next(self._seq), k))
         if len(self._heap) > 2 * len(self._stamp) + 64:     # drop stale entries: the heap stays O(live keys)

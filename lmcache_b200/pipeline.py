@@ -245,7 +245,8 @@ class UploadRing:
 
 class HostContainer:
     """One CacheGen container in a page-locked slab block, with the header fields its upload and decode need."""
-    __slots__ = ("blk", "nbytes", "ntokens", "L", "H", "D", "max_dtype", "coder", "last_read", "planes")
+    __slots__ = ("blk", "nbytes", "ntokens", "L", "H", "D", "max_dtype", "coder", "last_read", "planes", "dev",
+                 "dev_ready", "dev_read")
 
     def __init__(self, blk, nbytes: int, hd: "N.Header", planes: Optional[np.ndarray] = None):
         self.blk = blk                       # None once the tier no longer keeps the bytes (the disk tier's index)
@@ -258,6 +259,11 @@ class HostContainer:
         # codec.plane_offsets: where each plane's streams lie, for a layer-major upload; None: upload it whole.  Made by
         # whoever makes the record (land, read_container), never on the thread of a retrieve.
         self.planes = planes
+        # the tier's device level (lmcache_b200/device_cache.py): the container's block in the level's pool, the event
+        # after which that block holds the container (None: it does), and the latest decode that read it
+        self.dev = None
+        self.dev_ready: Optional[torch.cuda.Event] = None
+        self.dev_read: Optional[torch.cuda.Event] = None
 
 
 @functools.lru_cache(maxsize=None)
@@ -265,14 +271,16 @@ def _d2h_stream(device: torch.device) -> torch.cuda.Stream:
     return torch.cuda.Stream(device=device)
 
 
-def land(slab, slot: WaveSlot, batch, blocks: Optional[list] = None) -> List[HostContainer]:
+def land(slab, slot: WaveSlot, batch, blocks: Optional[list] = None,
+         dev_dst: Optional[Sequence[Optional[int]]] = None) -> List[HostContainer]:
     """Store-pipeline sink side: copy a finished wave's containers out of slot.dev into fresh blocks of `slab` (exactly
     their bytes, on the device's copy stream), wait for the copies, and parse every header.  Raises -- with every block
     freed -- when a copy fails or a container carries an encoder error.  `blocks`: blocks the caller allocated for the
-    first len(blocks) containers (a bounded tier); only those are landed.  A layer-wise store's slot (SegmentSlot) lands
-    through land_segments."""
+    first len(blocks) containers (a bounded tier); only those are landed.  `dev_dst`: per container, a device address
+    that gets a copy of it as well (None: none), on the same stream and before the same wait.  A layer-wise store's slot
+    (SegmentSlot) lands through land_segments."""
     if isinstance(slot, SegmentSlot):
-        return land_segments(slab, slot, batch, blocks)
+        return land_segments(slab, slot, batch, blocks, dev_dst)
     dev = slot.dev.device
     cs = _d2h_stream(dev)
     if blocks is None:
@@ -289,6 +297,11 @@ def land(slab, slot: WaveSlot, batch, blocks: Optional[list] = None) -> List[Hos
                     N.check(N.lib().b200kv_copy_async(ctypes.c_void_p(blk.host_ptr),
                                                       ctypes.c_void_p(slot.dev.data_ptr() + j * batch.stride), size,
                                                       cs.cuda_stream), "copy_async")
+                for j, (ptr, size) in enumerate(zip(dev_dst or (), batch.sizes)):
+                    if ptr is not None:
+                        N.check(N.lib().b200kv_copy_async(ctypes.c_void_p(ptr),
+                                                          ctypes.c_void_p(slot.dev.data_ptr() + j * batch.stride), size,
+                                                          cs.cuda_stream), "copy_async")
             finally:
                 cs.synchronize()             # no block leaves this function while a copy may still write it
         po = np.frombuffer(slot.planes.view(), dtype=np.int64, count=len(blocks) * (N.MAX_PLANES + 1))
@@ -485,11 +498,13 @@ class LayerwiseEncode:
             self.pool.release(slot)
 
 
-def land_segments(slab, slot: SegmentSlot, batch, blocks: Optional[list] = None) -> List[HostContainer]:
+def land_segments(slab, slot: SegmentSlot, batch, blocks: Optional[list] = None,
+                  dev_dst: Optional[Sequence[Optional[int]]] = None) -> List[HostContainer]:
     """land() for a layer-wise store: container j is assembled in a fresh block of `slab` from its fixed-section image
     and its 2L plane segments in the arena (one batched device->host copy of 1 + 2L ranges per container, all
-    containers in one call), and its plane offsets come from the segment sizes.  Raises -- with every block freed --
-    when a copy fails, the segments do not add up to the container's size, or a header carries an encoder error."""
+    containers in one call), and its plane offsets come from the segment sizes.  `dev_dst` as in land(): those
+    containers are assembled at their device address too, by the same batched copy.  Raises -- with every block freed
+    -- when a copy fails, the segments do not add up to the container's size, or a header carries an encoder error."""
     if blocks is None:
         blocks = [slab.alloc(size) for size in batch.sizes]
     n, L = len(blocks), slot.L
@@ -510,6 +525,13 @@ def land_segments(slab, slot: SegmentSlot, batch, blocks: Optional[list] = None)
         srcs = np.concatenate([fbase[:, None], np.uint64(slot.arena.data_ptr()) + seg[:, :, 0].astype(np.uint64)], axis=1)
         lens = np.concatenate([fixed[:, None], seg[:, :, 1]], axis=1)
         assert (lens.sum(axis=1) == sizes).all()
+        resident = [j for j, ptr in enumerate(list(dev_dst or ())[:n]) if ptr is not None]
+        if resident:
+            dptr = np.array([dev_dst[j] for j in resident], dtype=np.uint64)
+            ddst = np.concatenate([dptr[:, None], dptr[:, None] + planes[resident, :-1].astype(np.uint64)], axis=1)
+            dsts = np.concatenate([dsts, ddst])
+            srcs = np.concatenate([srcs, srcs[resident]])
+            lens = np.concatenate([lens, lens[resident]])
         dev = slot.arena.device
         cs = _d2h_stream(dev)
         with torch.cuda.device(dev):
@@ -590,7 +612,7 @@ def fetched_in_order(futures: Iterable[Future], window: Optional[int] = None) ->
     finally:
         for f in pending:
             rec = f.result()
-            if rec is not None:
+            if rec is not None and rec.blk is not None:     # a record without a block: a device copy, not a read
                 rec.blk.free()
 
 
@@ -600,8 +622,54 @@ def _continues_match(r: HostContainer, first: Optional[HostContainer], dst: KvVi
         (first is None or (r.max_dtype, r.coder) == (first.max_dtype, first.coder))
 
 
+class DeviceLevel:
+    """What upload_decode and upload_decode_layerwise need from a tier's device level (lmcache_b200/device_cache.py):
+    `cache`, the DeviceCache; resident(r): may record r be decoded from the level (it has a device copy in a pool on the
+    destination's device); promote(i, r, src_ptr, stream): r, chunk i of the call, has just been uploaded to src_ptr --
+    the tier may enqueue a copy of it into the level on `stream` (never waiting) and returns whether it did;
+    mark_read(recs, stream): the decodes just enqueued on `stream` read recs' device copies (mark_dev_read, under the
+    tier's lock); hit(n): n chunks were served from it.
+    The tier keeps every resident record's device copy alive until the call has recorded its decode in `dev_read`."""
+    cache = None
+
+    def resident(self, r: HostContainer) -> bool:
+        raise NotImplementedError
+
+    def promote(self, i: int, r: HostContainer, src_ptr: int, stream: torch.cuda.Stream) -> bool:
+        raise NotImplementedError
+
+    def hit(self, n: int) -> None:
+        raise NotImplementedError
+
+    def mark_read(self, recs: Sequence[HostContainer], stream: torch.cuda.Stream) -> None:
+        raise NotImplementedError
+
+
+def mark_dev_read(recs: Sequence[HostContainer], stream: torch.cuda.Stream) -> None:
+    """Record on `stream` the event after which no decode reads recs' device copies any more.  A copy that another
+    stream may still be decoding keeps that reader too: `stream` waits for the previous `dev_read` before the event, so
+    the one event stands for both.  Call under the tier's lock (concurrent retrieves may read the same copies)."""
+    seen = set()
+    for r in recs:
+        if r.dev_read is not None and id(r.dev_read) not in seen:
+            seen.add(id(r.dev_read))
+            stream.wait_event(r.dev_read)
+    ev = _recorded(stream)
+    for r in recs:
+        r.dev_read = ev
+
+
+def _wait_filled(recs: Sequence[HostContainer], stream: torch.cuda.Stream) -> None:
+    seen = set()
+    for r in recs:
+        if r.dev_ready is not None and id(r.dev_ready) not in seen:
+            seen.add(id(r.dev_ready))
+            stream.wait_event(r.dev_ready)
+
+
 def upload_decode(codec: CacheGenCodec, upload: UploadRing, records: Iterable[Optional[HostContainer]], dst: KvView,
-                  dst_tok0: int, chunk_size: int, release: Optional[DeferredFree] = None) -> int:
+                  dst_tok0: int, chunk_size: int, release: Optional[DeferredFree] = None,
+                  level: Optional[DeviceLevel] = None) -> int:
     """Upload + decode consecutive chunks straight into `dst`: records[i] (None: a miss) is chunk i and lands at token
     dst_tok0 + i * chunk_size.  Wave by wave the containers are copied into an UploadRing slot on its copy stream and
     decoded on the current stream; nothing is synchronised, and the records are consumed as the caller produces them
@@ -609,7 +677,12 @@ def upload_decode(codec: CacheGenCodec, upload: UploadRing, records: Iterable[Op
     upload event.  Returns the number of chunks decoded: the match stops at the first miss, at the first container whose
     geometry differs from `dst` or that does not fit it, and at the first whose (max_dtype, coder) differs from the
     first container's.  With `release`, the records' blocks are transient: each wave's go to `release` with its upload
-    event, and the block of the record the match stopped at is freed."""
+    event, and the block of the record the match stopped at is freed.
+
+    With a device `level`, a wave's resident records are not uploaded: they are decoded where they are, in one call at
+    their pool offsets after their fill events, and the rest of the wave in a second call from the slot.  Their
+    `last_read` is left alone and their `dev_read` becomes that decode's event.  Each uploaded record is offered to the
+    level (level.promote) right after its wave's upload."""
     W = wave_chunks_default()
     lib = N.lib()
     wave: List[HostContainer] = []
@@ -621,33 +694,54 @@ def upload_decode(codec: CacheGenCodec, upload: UploadRing, records: Iterable[Op
         def flush():
             if not wave:
                 return
-            offs, o = [], 0
-            for r in wave:
-                offs.append(o)
-                o += (r.nbytes + 15) & ~15
-            slot, buf = upload.next_slot(o)
-            for r, off in zip(wave, offs):
-                N.check(lib.b200kv_copy_async(ctypes.c_void_p(buf.data_ptr() + off), ctypes.c_void_p(r.blk.host_ptr),
-                                              r.nbytes, upload.copy_stream.cuda_stream), "copy_async")
-            ev = torch.cuda.Event()
-            ev.record(upload.copy_stream)
-            for r in wave:
-                r.last_read = ev
-            if release is not None:
-                release.add(ev, [r.blk for r in wave])
-            cur.wait_event(ev)
             w0 = n - len(wave)
-            codec.decode_raw(buf.data_ptr(), buf.numel(), offs, [r.nbytes for r in wave], [r.ntokens for r in wave], dst,
-                             [dst_tok0 + (w0 + j) * chunk_size for j in range(len(wave))], wave[0].max_dtype,
-                             wave[0].coder, cur)
-            upload.mark_read(slot, cur)
+            res = [j for j, r in enumerate(wave) if level is not None and level.resident(r)]
+            up = [j for j in range(len(wave)) if j not in res] if res else list(range(len(wave)))
+            if res:
+                pool = level.cache.pool
+                recs = [wave[j] for j in res]
+                _wait_filled(recs, cur)
+                codec.decode_raw(pool.dev_ptr, pool.buf.numel(), [r.dev.offset for r in recs], [r.nbytes for r in recs],
+                                 [r.ntokens for r in recs], dst, [dst_tok0 + (w0 + j) * chunk_size for j in res],
+                                 wave[0].max_dtype, wave[0].coder, cur)
+                level.mark_read(recs, cur)
+                level.hit(len(recs))
+            if up:
+                recs = [wave[j] for j in up]
+                offs, o = [], 0
+                for r in recs:
+                    offs.append(o)
+                    o += (r.nbytes + 15) & ~15
+                slot, buf = upload.next_slot(o)
+                for r, off in zip(recs, offs):
+                    N.check(lib.b200kv_copy_async(ctypes.c_void_p(buf.data_ptr() + off), ctypes.c_void_p(r.blk.host_ptr),
+                                                  r.nbytes, upload.copy_stream.cuda_stream), "copy_async")
+                ev = torch.cuda.Event()
+                ev.record(upload.copy_stream)
+                for r in recs:
+                    r.last_read = ev
+                if release is not None:
+                    release.add(ev, [r.blk for r in recs])
+                promoted = None
+                if level is not None:       # after the wave's event: the decode does not wait for these copies
+                    if sum(level.promote(w0 + j, r, buf.data_ptr() + off, upload.copy_stream)
+                           for j, r, off in zip(up, recs, offs)):
+                        promoted = torch.cuda.Event()
+                        promoted.record(upload.copy_stream)
+                cur.wait_event(ev)
+                codec.decode_raw(buf.data_ptr(), buf.numel(), offs, [r.nbytes for r in recs], [r.ntokens for r in recs],
+                                 dst, [dst_tok0 + (w0 + j) * chunk_size for j in up], wave[0].max_dtype,
+                                 wave[0].coder, cur)
+                if promoted is not None:    # the slot's next writer (or its replacement) waits for the promotion's reads
+                    cur.wait_event(promoted)
+                upload.mark_read(slot, cur)
             wave.clear()
 
         for r in records:
             if r is None:
                 break
             if not _continues_match(r, first, dst, dst_tok0 + n * chunk_size):
-                if release is not None:
+                if release is not None and r.blk is not None:
                     r.blk.free()
                 break
             first = first or r
@@ -719,6 +813,7 @@ class LayerwiseUploader:
             if job is None:
                 return
             job()
+            job = None               # a finished job's destination must not live on until the next job arrives
 
     def submit(self, job: Callable[[], None]) -> None:
         self._q.put(job)
@@ -754,7 +849,8 @@ def layer_copy_ranges(plane_offs: Sequence[Optional[np.ndarray]], nbytes: Sequen
 
 def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, records: Iterable[Optional[HostContainer]],
                             dst: KvView, dst_tok0: int, chunk_size: int, release: Optional[DeferredFree] = None,
-                            on_done: Optional[Callable[[], None]] = None) -> LayerwiseUpload:
+                            on_done: Optional[Callable[[], None]] = None,
+                            level: Optional[DeviceLevel] = None) -> LayerwiseUpload:
     """upload_decode in layer-major order, so that layer 0 of every chunk is decoded after ~1/L of the bytes.
 
     The match follows upload_decode's rules and is made on the calling thread, which consumes `records` to its end
@@ -765,7 +861,12 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
          then the decode of layer l, then the layer's ready event.
     The decode stream first waits for the calling thread's current stream (the destination may have just been
     allocated there).  Every record's `last_read` is the last copy's event; `release` (transient blocks) gets the blocks
-    with that event; `on_done` runs once that event is recorded (or when the call fails) -- e.g. to unpin the entries."""
+    with that event; `on_done` runs once that event is recorded (or when the call fails) -- e.g. to unpin the entries.
+
+    With a device `level`, resident records take no copies: they get a plan of their own over the level's pool (after
+    their fill events), and each layer is decoded by both plans before its ready event.  Their `last_read` is left
+    alone and their `dev_read` becomes the last decode's event.  The uploaded records are offered to the level
+    (level.promote) after the last copy."""
     matched: List[HostContainer] = []
     L = dst.L
     submitted = False
@@ -775,12 +876,18 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
             if r is None:
                 break
             if not _continues_match(r, first, dst, dst_tok0 + len(matched) * chunk_size):
-                if release is not None:
+                if release is not None and r.blk is not None:
                     r.blk.free()
                 break
             first = first or r
             matched.append(r)
         n = len(matched)
+        res_j = [j for j, r in enumerate(matched) if level is not None and level.resident(r)]
+        up_j = [j for j in range(n) if j not in res_j] if res_j else list(range(n))
+        res = [matched[j] for j in res_j]
+        up = [matched[j] for j in up_j]
+        if res:
+            level.hit(len(res))
         with torch.cuda.device(dst.device):
             start = torch.cuda.Event()
             start.record(torch.cuda.current_stream())
@@ -790,62 +897,79 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
                     on_done()
                 return LayerwiseUpload.completed(0, L, start)
             offs, o = [], 0
-            for r in matched:
+            for r in up:
                 offs.append(o)
                 o += (r.nbytes + 15) & ~15
-            staging = torch.empty(o + N.READ_SLACK, dtype=torch.uint8, device=dst.device)
-            staging.record_stream(uploader.copy_stream)
-            staging.record_stream(uploader.decode_stream)
+            staging = None
+            if up:
+                staging = torch.empty(o + N.READ_SLACK, dtype=torch.uint8, device=dst.device)
+                staging.record_stream(uploader.copy_stream)
+                staging.record_stream(uploader.decode_stream)
             dst.record_stream(uploader.decode_stream)
 
-        base = staging.data_ptr()
-        host = np.array([r.blk.host_ptr for r in matched], dtype=np.uint64)
-        dev = base + np.array(offs, dtype=np.uint64)
-        fixed, lo, sz = layer_copy_ranges([r.planes for r in matched], [r.nbytes for r in matched], L)
-        lay_src = np.ascontiguousarray(np.tile(np.concatenate([host, host]), (L, 1)) + lo.astype(np.uint64))
-        lay_dst = np.ascontiguousarray(np.tile(np.concatenate([dev, dev]), (L, 1)) + lo.astype(np.uint64))
+        if up:
+            base = staging.data_ptr()
+            host = np.array([r.blk.host_ptr for r in up], dtype=np.uint64)
+            dev = base + np.array(offs, dtype=np.uint64)
+            fixed, lo, sz = layer_copy_ranges([r.planes for r in up], [r.nbytes for r in up], L)
+            lay_src = np.ascontiguousarray(np.tile(np.concatenate([host, host]), (L, 1)) + lo.astype(np.uint64))
+            lay_dst = np.ascontiguousarray(np.tile(np.concatenate([dev, dev]), (L, 1)) + lo.astype(np.uint64))
         upload = LayerwiseUpload(n, L)
-        totals = [r.nbytes for r in matched]
-        ntoks = [r.ntokens for r in matched]
         dst_tok = [dst_tok0 + j * chunk_size for j in range(n)]
 
         def job():
             cs, ds = uploader.copy_stream, uploader.decode_stream
             last = None
+            plans = []
             try:
                 with torch.cuda.device(uploader.device):
                     t0 = time.perf_counter()
                     cs.wait_event(start)
                     ds.wait_event(start)
-                    _batch_copy(dev, host, fixed, cs)
-                    last = torch.cuda.Event()
-                    last.record(cs)
-                    ds.wait_event(last)
-                    plan, ws = codec.decode_plan(base, staging.numel(), offs, totals, ntoks, dst, dst_tok,
-                                                 first.max_dtype, first.coder, ds)
-                    t1 = time.perf_counter()
-                    upload.enqueue_s.append(t1 - t0)
-                    for layer in range(L):
-                        _batch_copy(lay_dst[layer], lay_src[layer], sz[layer], cs)
+                    if res:
+                        pool = level.cache.pool
+                        _wait_filled(res, ds)
+                        plans.append(codec.decode_plan(pool.dev_ptr, pool.buf.numel(), [r.dev.offset for r in res],
+                                                       [r.nbytes for r in res], [r.ntokens for r in res], dst,
+                                                       [dst_tok[j] for j in res_j], first.max_dtype, first.coder, ds))
+                    if up:
+                        _batch_copy(dev, host, fixed, cs)
                         last = torch.cuda.Event()
                         last.record(cs)
                         ds.wait_event(last)
-                        codec.decode_layers(plan, layer, layer + 1, ds)
+                        plans.append(codec.decode_plan(base, staging.numel(), offs, [r.nbytes for r in up],
+                                                       [r.ntokens for r in up], dst, [dst_tok[j] for j in up_j],
+                                                       first.max_dtype, first.coder, ds))
+                    t1 = time.perf_counter()
+                    upload.enqueue_s.append(t1 - t0)
+                    for layer in range(L):
+                        if up:
+                            _batch_copy(lay_dst[layer], lay_src[layer], sz[layer], cs)
+                            last = torch.cuda.Event()
+                            last.record(cs)
+                            ds.wait_event(last)
+                        for plan, _ in plans:
+                            codec.decode_layers(plan, layer, layer + 1, ds)
                         ev = torch.cuda.Event(enable_timing=True)     # a caller may time the layers against each other
                         ev.record(ds)
                         upload._publish(ev)
                         t0, t1 = t1, time.perf_counter()
                         upload.enqueue_s.append(t1 - t0)
-                    del ws                            # recorded on the decode stream: reused only after the decodes
+                    if level is not None:             # staging is recorded on the copy stream: freed after these
+                        for j, r, off in zip(up_j, up, offs):
+                            level.promote(j, r, base + off, cs)
+                    plans.clear()                     # workspaces are recorded on the decode stream
             except BaseException as e:               # noqa: BLE001 -- the caller sees it in ready()
                 upload._fail(e)
                 cs.synchronize()                      # no block is released while a copy that reads it may be queued
                 last = None
             finally:
-                for r in matched:
+                for r in up:
                     r.last_read = last
+                if res:
+                    level.mark_read(res, uploader.decode_stream)
                 if release is not None:
-                    release.add(last, [r.blk for r in matched])
+                    release.add(last, [r.blk for r in up])
                 if on_done is not None:
                     on_done()
 
@@ -856,6 +980,13 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
         if not submitted:                             # failed before the worker took over: nothing was enqueued
             if release is not None:
                 for r in matched:
-                    r.blk.free()
+                    if r.blk is not None:
+                        r.blk.free()
             if on_done is not None:
                 on_done()
+
+
+def _recorded(stream: torch.cuda.Stream) -> torch.cuda.Event:
+    ev = torch.cuda.Event()
+    ev.record(stream)
+    return ev

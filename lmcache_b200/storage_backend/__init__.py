@@ -13,6 +13,13 @@ def CreateStorageBackend(config: LMCacheEngineConfig, metadata: LMCacheEngineMet
         if local in ("cpu", "cuda") and not (local == "cpu" and config.local_serde == "cachegen"):
             raise ValueError(f"local_capacity_bytes is honoured by the CacheGen tiers only (local_device='cpu' with "
                              f"local_serde='cachegen', or a directory), not by local_device={local!r}")
+    if config.device_cache_bytes is not None:
+        # the device level keeps copies of CacheGen containers: only the CacheGen local tiers have any
+        if local is None:
+            raise ValueError("device_cache_bytes needs a local CacheGen tier; a remote-only configuration has none")
+        if local in ("cpu", "cuda") and not (local == "cpu" and config.local_serde == "cachegen"):
+            raise ValueError(f"device_cache_bytes is honoured by the CacheGen tiers only (local_device='cpu' with "
+                             f"local_serde='cachegen', or a directory), not by local_device={local!r}")
     if local is None and isinstance(remote, str):
         from lmcache_b200.storage_backend.remote_backend import LMCPipelinedRemoteBackend, LMCRemoteBackend
         return (LMCPipelinedRemoteBackend if config.pipelined_backend else LMCRemoteBackend)(config, metadata)

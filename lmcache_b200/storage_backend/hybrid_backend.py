@@ -20,9 +20,10 @@ class LMCHybridBackend(LMCBackendInterface):
     def __init__(self, config: LMCacheEngineConfig, metadata: LMCacheEngineMetadata):
         super().__init__()
         from lmcache_b200.storage_backend import CreateStorageBackend
-        # a capacity bounds the local tier (one of the CacheGen tiers); chunks it evicts are still served by the remote one
+        # a capacity bounds the local tier (one of the CacheGen tiers); chunks it evicts are still served by the remote one.
+        # A device level belongs to the local tier as well.
         local_cfg = LMCacheEngineConfig(config.chunk_size, config.local_device, None, None, False, config.save_decode_cache,
-                                        config.local_serde, config.local_capacity_bytes)
+                                        config.local_serde, config.local_capacity_bytes, config.device_cache_bytes)
         remote_cfg = LMCacheEngineConfig(config.chunk_size, None, config.remote_url, config.remote_serde,
                                          config.pipelined_backend, config.save_decode_cache, None)
         self.local_store = CreateStorageBackend(local_cfg, metadata)

@@ -251,16 +251,24 @@ class LMCLocalBackend(LMCBackendInterface):
 
 
 # ---------------------------------------------------------------------------------------------- compressed host tier
+def _copy_ptr(dst: int, src: int, nbytes: int, stream: torch.cuda.Stream) -> None:
+    N.check(N.lib().b200kv_copy_async(ctypes.c_void_p(dst), ctypes.c_void_p(src), nbytes, stream.cuda_stream), "copy_async")
+
+
 class _Store:
     """One put_kv_chunks call.  A bounded tier never evicts a call's entries to make room for its later chunks, nor an
     entry touched since `since` -- the latest touch on the calling thread, which for LMCacheEngine is the prefix its
     skip_existing scan matched: evicting that prefix would make the chunks being stored unreachable.  Once one of its
-    containers does not fit, the rest are dropped as well: behind a gap they could never be hit."""
-    __slots__ = ("dropped", "since")
+    containers does not fit, the rest are dropped as well: behind a gap they could never be hit.  The device level
+    likewise never evicts the call's own copies, stamps them all with one tick (`dtick`) in chain order, and once one
+    of its chunks is not cached it caches none of the later ones (`dgap`): what the level holds of the call is a prefix."""
+    __slots__ = ("dropped", "since", "dtick", "dgap")
 
     def __init__(self, since: Optional[int] = None):
         self.dropped = False
         self.since = since
+        self.dtick: Optional[int] = None
+        self.dgap = False
 
 
 def _miss_beyond(entries, batch) -> None:
@@ -293,6 +301,29 @@ class _CEntry:
         return 0 if self.rec is None else self.rec.nbytes
 
 
+class _Level:
+    """pipeline.DeviceLevel of one retrieve: chunk i of the call is entries[i], pinned by the retrieve"""
+
+    def __init__(self, tier: "LMCLocalCompressedBackend", entries: list, device):
+        self.tier, self.entries, self.cache = tier, entries, tier._dcache
+        self.device = torch.device(device)
+
+    def resident(self, r) -> bool:
+        return r.dev is not None and self.cache.serves(self.device)
+
+    def promote(self, i: int, r, src_ptr: int, stream: torch.cuda.Stream) -> bool:
+        return self.tier._promote(self.entries[i], r, src_ptr, stream)
+
+    def hit(self, n: int) -> None:
+        with self.tier.update_lock:
+            self.cache.hits += n
+
+    def mark_read(self, recs, stream: torch.cuda.Stream) -> None:
+        from lmcache_b200.pipeline import mark_dev_read
+        with self.tier.update_lock:
+            mark_dev_read(recs, stream)
+
+
 class LMCLocalCompressedBackend(LMCBackendInterface):
     """local_device="cpu" + local_serde="cachegen": the host tier keeps CacheGen containers instead of raw blobs.
 
@@ -306,7 +337,12 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
     Every container lives in one PinnedSlab (one cudaHostAlloc per GiB, not one per put).
 
     With config.local_capacity_bytes the slab never holds more than that many bytes: the store worker evicts chunks in
-    the order of lmcache_b200.eviction.PrefixLRU before it lands a wave, and drops what does not fit even then."""
+    the order of lmcache_b200.eviction.PrefixLRU before it lands a wave, and drops what does not fit even then.
+
+    With config.device_cache_bytes the tier has a device level (lmcache_b200/device_cache.py): containers are copied
+    into one device pool as they land and as retrieves upload them, and a retrieve decodes the resident ones in place
+    (pipeline.DeviceLevel).  The level is inclusive -- a device copy leaves with its entry -- and filling it never
+    waits: what does not find room at once is not cached."""
 
     def __init__(self, config: LMCacheEngineConfig, metadata):
         super().__init__()
@@ -331,6 +367,10 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         self._layerwise = None                # pipeline.LayerwiseUploader, made by the first layer-wise retrieve
         self._segments = None                 # pipeline.SegmentPool, made by the first layer-wise store
         self._release = DeferredFree()        # blocks uploads may still read: retired entries, the disk tier's file reads
+        self._dcache = None                   # device_cache.DeviceCache: the device level (config.device_cache_bytes)
+        if config.device_cache_bytes is not None:
+            from lmcache_b200.device_cache import DeviceCache
+            self._dcache = DeviceCache(config.device_cache_bytes)
         self._closed = False
 
     def _new_slab(self):
@@ -345,17 +385,30 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
     def _sink(self, slot, batch, c0, entries) -> None:
         """store pipeline sink: land the wave in host memory, then publish the entries (readers wait on `ready`)"""
         from lmcache_b200.pipeline import land
+        dblocks = None
         try:
             blocks = None if self.capacity is None else self._make_room(batch.sizes, entries)
-            recs = land(self.slab, slot, batch, blocks) if blocks is None or blocks else []
+            if self._dcache is None:
+                recs = land(self.slab, slot, batch, blocks) if blocks is None or blocks else []
+            else:
+                dblocks = self._fill_blocks(batch.sizes[:len(batch.sizes) if blocks is None else len(blocks)], slot,
+                                            entries[0].store)
+                recs = land(self.slab, slot, batch, blocks, self._fill_ptrs(dblocks)) if dblocks else []
             for e, rec in zip(entries, recs):
                 e.rec = rec
+            if dblocks:
+                with self.update_lock:
+                    self._dcache.attach(entries, dblocks, at=self._fill_stamp(entries[0].store, c0))  # landed with the wave
+                dblocks = None
             _miss_beyond(entries, batch)
         except BaseException as err:     # noqa: BLE001 -- the entries become misses; the job reports the error
             for e in entries:
                 e.error = err
             raise
         finally:
+            for blk in dblocks or ():
+                if blk is not None:
+                    blk.free()
             for e in entries:
                 e.ready.set()
 
@@ -418,20 +471,37 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
             if e.pins:
                 e.retired = True                 # a retrieve still holds it: the last unpin frees the block
                 return
-            rec, e.rec = e.rec, None
+            if self._dcache is not None:
+                e.retired = True                 # a promotion must not fill it any more
+            rec = self._detach(e)
+        self._free_rec(rec)
+
+    def _detach(self, e: _CEntry):
+        """under the lock: the record whose bytes retiring `e` frees (and its device copy leaves the level)"""
+        rec, e.rec = e.rec, None
+        if rec is not None and self._dcache is not None:
+            self._dcache.order.discard(e)
+            self._dcache.detach(rec)
+        return rec
+
+    def _free_rec(self, rec) -> None:
         if rec is not None and rec.blk is not None:
             self._release.add(rec.last_read, [rec.blk])
 
     def touch(self, keys) -> None:
         """Recency update of one call: `keys` in chain order, chunk 0 first (LMCacheEngine passes every key of a stored
         sequence and every key of a retrieved prefix, lmcache_b200/eviction.py).  Keys the tier does not hold are
-        skipped.  No-op on an unbounded tier."""
-        if self.capacity is None:
+        skipped.  The device level's order gets the same call, over the entries it holds.  No-op on an unbounded tier
+        without a device level."""
+        if self.capacity is None and self._dcache is None:
             return
         dks = [self._dict_key(k) for k in keys]
         with self.update_lock:
-            self._order.touch([k for k in dks if k in self.dict])
-            self._touched.tick = self._order.tick
+            if self.capacity is not None:
+                self._order.touch([k for k in dks if k in self.dict])
+                self._touched.tick = self._order.tick
+            if self._dcache is not None:
+                self._dcache.touch([self.dict.get(k) for k in dks])
 
     def _new_store(self) -> _Store:
         return _Store(getattr(self._touched, "tick", None) if self.capacity is not None else None)
@@ -511,7 +581,7 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         pinned = []
         try:
             return upload_decode(self.codec, self._upload_ring(dst.device), self._pinned_records(keys, pinned), dst,
-                                 dst_tok0, chunk_size)
+                                 dst_tok0, chunk_size, level=self._level(dst.device, pinned))
         finally:
             self._unpin(pinned)             # every wave's upload event is recorded in its records' last_read by now
 
@@ -522,7 +592,8 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         from lmcache_b200.pipeline import upload_decode_layerwise
         pinned = []
         return upload_decode_layerwise(self.codec, self._layerwise_uploader(dst.device), self._pinned_records(keys, pinned),
-                                       dst, dst_tok0, chunk_size, on_done=lambda: self._unpin(pinned))
+                                       dst, dst_tok0, chunk_size, on_done=lambda: self._unpin(pinned),
+                                       level=self._level(dst.device, pinned))
 
     def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int):
         """A pipeline.LayerwiseEncode of tokens [tok_begin, T) of `view` (whose KV may not be written yet), or None
@@ -566,10 +637,82 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
             for e in pinned:
                 e.pins -= 1
                 if e.pins == 0 and e.retired and e.rec is not None:
-                    free.append(e.rec)
-                    e.rec = None
+                    free.append(self._detach(e))
         for rec in free:
-            self._release.add(rec.last_read, [rec.blk])
+            self._free_rec(rec)
+
+    # ------------------------------------------------------------------ device level
+    def _level(self, device, entries: list):
+        """the pipeline's view of the device level for one retrieve into `device`, whose chunk i is entries[i] (an
+        entry pinned from its lookup on), or None without a level"""
+        return None if self._dcache is None else _Level(self, entries, device)
+
+    def _fill_stamp(self, store: _Store, c0: int):
+        """under the lock: (tick, chain position) of the store's copies from chunk c0 on -- one tick per store"""
+        if store.dtick is None:
+            store.dtick = self._dcache.order.new_tick()
+        return store.dtick, c0
+
+    def _fill_blocks(self, sizes, slot, store: _Store) -> list:
+        """store worker: a device block for each landing container, or None where it is not cached.  The store's own
+        copies are never evicted for its later chunks: a sequence larger than the level keeps its head resident."""
+        from lmcache_b200.pipeline import SegmentSlot
+        device = (slot.arena if isinstance(slot, SegmentSlot) else slot.dev).device
+        c = self._dcache
+        with self.update_lock, torch.cuda.device(device):
+            if c.pool is not None and not c.serves(device):
+                return [None] * len(sizes)
+            out = []
+            for size in sizes:
+                blk = None if store.dgap else c.alloc(size, keep=lambda h: h.store is store)
+                if blk is None:
+                    c.skipped += store.dgap          # alloc counted the first one
+                    store.dgap = True
+                out.append(blk)
+            return out
+
+    def _fill_ptrs(self, dblocks) -> list:
+        base = self._dcache.pool.dev_ptr if any(b is not None for b in dblocks) else 0
+        return [None if b is None else base + b.offset for b in dblocks]
+
+    def _promote(self, e: _CEntry, r, src_ptr: int, stream: torch.cuda.Stream) -> bool:
+        """a retrieve uploaded `r` (entry e's container) to src_ptr: copy it into the level on `stream` when a block is
+        free without waiting.  True: the copy is enqueued."""
+        c = self._dcache
+        with self.update_lock:
+            if e.retired or e.rec is None or e.rec.dev is not None or e.rec.nbytes != r.nbytes:
+                return False
+            if c.pool is not None and not c.serves(stream.device):
+                return False
+            with torch.cuda.device(stream.device):
+                blk = c.alloc(r.nbytes)
+                if blk is None:
+                    return False
+                try:
+                    _copy_ptr(c.pool.dev_ptr + blk.offset, src_ptr, r.nbytes, stream)
+                except BaseException:
+                    blk.free()
+                    raise
+                ev = torch.cuda.Event()
+                ev.record(stream)
+            c.attach([e], [blk], ev)
+            c.promotions += 1
+        return True
+
+    def reserve_device(self) -> None:
+        """Make the device level's pool now, on the current device (the first store makes it otherwise).  No-op without
+        a level."""
+        if self._dcache is not None:
+            with self.update_lock:
+                self._dcache.reserve()
+
+    def device_cache_stats(self) -> Optional[dict]:
+        """bytes_in_use, budget_bytes, hits, promotions, evictions, not_cached (chunks that found no room without
+        waiting) of the device level; None without one"""
+        if self._dcache is None:
+            return None
+        with self.update_lock:
+            return self._dcache.stats()
 
     def _upload_ring(self, device):
         from lmcache_b200.pipeline import UploadRing
@@ -614,6 +757,8 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         except Exception:       # noqa: BLE001 -- interpreter shutdown
             pass
         self.slab.close()
+        if self._dcache is not None:
+            self._dcache.close()
 
     def __del__(self):
         try:
@@ -708,13 +853,22 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
         return self._key_to_path(key)
 
     def _drop(self, e: _CEntry) -> None:
-        """evicted: the file goes (on the store worker, or at start-up)"""
+        """evicted: the file goes (on the store worker, or at start-up), and its device copy with it"""
         import os
         try:
             os.remove(e.path)
         except OSError:
             pass
         self._disk_bytes -= self._file_bytes.pop(e.path, 0)
+        if self._dcache is not None:
+            self._retire(e)
+
+    def _detach(self, e: _CEntry):
+        """the index record stays (readers of the entry may still open its path); only the device copy leaves"""
+        if e.rec is not None and self._dcache is not None:
+            self._dcache.order.discard(e)
+            self._dcache.detach(e.rec)
+        return None
 
     def _make_file_room(self, e: _CEntry, nbytes: int) -> bool:
         """bounded tier: evict until the file of `e` (replacing any file at its path) fits within the capacity"""
@@ -731,15 +885,20 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
 
         from lmcache_b200.pipeline import land
         recs = []
+        dblocks = None
         try:
-            recs = land(self.slab, slot, batch)          # containers -> page-locked blocks, headers parsed
+            if self._dcache is None:
+                recs = land(self.slab, slot, batch)      # containers -> page-locked blocks, headers parsed
+            else:
+                dblocks = self._fill_blocks(batch.sizes, slot, entries[0].store)
+                recs = land(self.slab, slot, batch, None, self._fill_ptrs(dblocks))
         except BaseException as err:     # noqa: BLE001
             for e in entries:
                 e.error = err
             raise
         else:
             _miss_beyond(entries, batch)
-            for e, rec in zip(entries, recs):
+            for j, (e, rec) in enumerate(zip(entries, recs)):
                 e.rec = rec
                 if self.capacity is not None and not self._make_file_room(e, rec.nbytes):
                     e.error = OSError(f"chunk does not fit within local_capacity_bytes={self.capacity}")
@@ -755,7 +914,15 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
                 if self.capacity is not None:
                     self._disk_bytes += rec.nbytes - self._file_bytes.get(e.path, 0)
                     self._file_bytes[e.path] = rec.nbytes
+                if dblocks is not None and dblocks[j] is not None:
+                    with self.update_lock:                # inclusive: only beside a file that is in place
+                        if not e.retired:                 # an overwrite retired it: its copy would never be served
+                            self._dcache.attach([e], [dblocks[j]], at=self._fill_stamp(e.store, c0 + j))
+                            dblocks[j] = None
         finally:
+            for blk in dblocks or ():
+                if blk is not None:
+                    blk.free()
             for rec in recs:
                 rec.blk.free()
                 rec.blk = None
@@ -768,12 +935,17 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
         for k, e in zip(keys, entries):
             e.path = self._key_to_path(k)
             e.ready.clear()
+        old = []
         with self.update_lock:
             for e in entries:
+                if self._dcache is not None and e.path in self.dict:
+                    old.append(self.dict[e.path])
                 self.dict[e.path] = e                     # an overwritten chunk's file is replaced atomically by the rename
         # the parent's sink sets `ready` before the file exists: keep readers out until the file is written
         job = self._submit(view, tok_begin, chunk_size, entries, encoded)
         self.touch(keys)
+        for prev in old:      # an overwritten chunk's device copy is never served again (its sink checks `retired`)
+            self._retire(prev)
         if blocking:
             job.wait()
         return len(keys)
@@ -799,35 +971,59 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
             return None
         return read_container(self.codec, blk, nbytes)
 
+    def _reads(self, keys, level: Optional[_Level]) -> list:
+        """futures of the records of `keys` up to the first miss: file reads, or with a device level the index
+        record of a resident entry (no read).  With a level every entry is pinned into level.entries."""
+        from concurrent.futures import Future
+        reads = []
+        for key in keys:
+            if level is None:
+                e = self._ready_entry(key)
+            else:
+                rec = next(self._pinned_records([key], level.entries))
+                e = level.entries[-1] if rec is not None else None
+            if e is None:
+                break
+            if level is not None and level.resident(e.rec):
+                f = Future()
+                f.set_result(e.rec)
+                reads.append(f)
+            else:
+                reads.append(self._io.submit(self._read_file, e))
+        return reads
+
     def get_kv_into(self, keys, dst, dst_tok0: int, chunk_size: int) -> int:
         import contextlib
 
         from lmcache_b200.pipeline import fetched_in_order, upload_decode
         self._release.sweep()                            # transient read blocks of earlier calls
-        reads = []
-        for key in keys:
-            e = self._ready_entry(key)
-            if e is None:
-                break
-            reads.append(self._io.submit(self._read_file, e))
-        with contextlib.closing(fetched_in_order(reads)) as recs:
-            return upload_decode(self.codec, self._upload_ring(dst.device), recs, dst, dst_tok0, chunk_size,
-                                 self._release)
+        level = self._level(dst.device, [])
+        try:
+            reads = self._reads(keys, level)
+            with contextlib.closing(fetched_in_order(reads)) as recs:
+                return upload_decode(self.codec, self._upload_ring(dst.device), recs, dst, dst_tok0, chunk_size,
+                                     self._release, level)
+        finally:
+            if level is not None:
+                self._unpin(level.entries)
 
     def get_kv_layerwise(self, keys, dst, dst_tok0: int, chunk_size: int):
         import contextlib
 
         from lmcache_b200.pipeline import fetched_in_order, upload_decode_layerwise
         self._release.sweep()
-        reads = []
-        for key in keys:
-            e = self._ready_entry(key)
-            if e is None:
-                break
-            reads.append(self._io.submit(self._read_file, e))
+        level = self._level(dst.device, [])
+        try:
+            reads = self._reads(keys, level)
+        except BaseException:
+            if level is not None:
+                self._unpin(level.entries)
+            raise
         with contextlib.closing(fetched_in_order(reads)) as recs:
             return upload_decode_layerwise(self.codec, self._layerwise_uploader(dst.device), recs, dst, dst_tok0,
-                                           chunk_size, self._release)
+                                           chunk_size, self._release,
+                                           on_done=None if level is None else (lambda: self._unpin(level.entries)),
+                                           level=level)
 
     def host_bytes(self) -> int:
         return sum(e.rec.nbytes for e in self.dict.values() if e.rec is not None)
