@@ -233,7 +233,9 @@ int b200kv_decode_layers(const b200kv_decode_plan_t* plan, int32_t layer_begin, 
  * then its V planes) are placed 16-byte aligned at a device-held cursor, in (call, chunk) order.  A chunk whose bytes do
  * not fit fails, and so does every later chunk of the plan: the chunks that fit are always a prefix.  Row (j, p) of
  * seg_sizes_out (DEVICE or mapped-host int64[n_chunks][2L][2]) gets the arena offset (-1: chunk failed) and the size of
- * plane p of chunk j.  Each layer is encoded once; a layer range that was encoded before is an error.
+ * plane p of chunk j.  A chunk that fails in a later call than its first keeps the rows of the calls that had placed it
+ * (those bytes stay in the arena, unused); the rows of the failing call and of every later one are -1.  Read the rows of
+ * chunks whose sizes_out is nonzero only.  Each layer is encoded once; a layer range that was encoded before is an error.
  *
  * b200kv_encode_layers_finish writes each chunk's header into its fixed image and sizes_out[j] (total_bytes, or 0 when
  * the chunk failed: header.status bit 16 = did not fit the arena), and fails unless every layer was encoded.

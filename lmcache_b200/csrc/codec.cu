@@ -964,6 +964,18 @@ __global__ void finalize_kernel(EncParams P) {
     hd->status = P.err[j];
     hd->reserved[0] = hd->reserved[1] = hd->reserved[2] = 0u;
     if (P.sizes_out) P.sizes_out[j] = hd->status ? 0ull : hd->total_bytes;     // 0 = this chunk failed (see header.status)
+    {
+        // the padding in front of the maxima, the lengths and the payload (< 16 bytes each) is zero, not whatever the
+        // output buffer held before: a container's bytes are a function of the KV alone, and no stale device memory
+        // travels with it to a tier
+        uint8_t* c = reinterpret_cast<uint8_t*>(hd);
+        const int64_t NL = 2 * (int64_t)P.L;
+        const int64_t ends[3] = {lo.off_cdf + (P.compact ? NL : NL * P.C * kLp * 2), lo.off_maxes + NL * t * 2,
+                                 lo.off_lengths + (int64_t)lo.ngroups * NL * P.C * (P.compact ? 1 : 4)};
+        const int64_t starts[3] = {lo.off_maxes, lo.off_lengths, lo.off_payload};
+        for (int k = 0; k < 3; ++k)
+            for (int64_t b = ends[k]; b < starts[k]; ++b) c[b] = 0u;
+    }
     if (P.compact) {                               // counts per stream of every plane: makes the container self-describing
         uint8_t* nbmap = reinterpret_cast<uint8_t*>(hd) + lo.off_cdf;
         const int NL = 2 * P.L;
@@ -1435,9 +1447,13 @@ __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
                 CdfAccum2 acc;
                 acc.init();
                 uint32_t c0 = 0u;
+                // every entry the symbol search can read (0..15 for <= 16 symbols, 0..31 otherwise), not only the nb the
+                // plane uses: a plane of 4..14 or 18..30 symbols would otherwise search uninitialised shared memory.
+                // Entries past nb are the reference's CDF there (no mass, one slot each), as in a version-2 CDF row.
+                const int nsearch = cq <= 7.0f ? 16 : 32;
 #pragma unroll
                 for (int i = 0; i < 32; ++i) {
-                    if (i < nb) {
+                    if (i < nsearch) {
                         if ((wany >> i) & 1u) acc.absorb(pn[count(i)]);          // uniform per warp: symbols nobody uses
                         uint32_t c1 = acc.value((uint32_t)i + 1u);
                         if (i == 31) c1 = 0x10000u;                              // cdf[32] wraps to 0 in 16 bits and means 65536

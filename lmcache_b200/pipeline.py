@@ -330,7 +330,11 @@ def arena_placement(seg_bytes: np.ndarray, arena_bytes: int, layers: Optional[Se
     cursor.  Chunk j fits if, after chunks 0..j of the call, the arena still holds the layers still to come at this
     call's size per layer (a reserve, so that a later call finds room for the chunks an earlier one accepted).  A chunk
     that does not fit fails, and so does every later chunk, in this call and every later one.  Returns (base
-    int64[calls, n], -1 for the chunks that failed; the number of chunks that fit)."""
+    int64[calls, n], -1 in every call for the chunks that failed; the number of chunks that fit).
+    The device's seg_sizes_out rows differ for the failed chunks: the calls before the one in which they failed had
+    placed them, and their rows keep those arena offsets (the bytes stay in the arena, unused); only the rows of the
+    failing call and the later ones are -1.  sizes_out is 0 for every failed chunk, so no reader looks at those rows.
+    Zeroing seg_bytes of the calls after c gives the placement as it stood after call c."""
     seg_bytes = np.asarray(seg_bytes, dtype=np.int64)
     calls, n = seg_bytes.shape
     layers = list(layers) if layers is not None else [1] * calls
