@@ -38,7 +38,7 @@ extern "C" {
                                     *    e.g. dlsym): b200kv_decode_plan / b200kv_decode_layers, b200kv_plane_offsets,
                                     *    b200kv_plane_offsets_device, b200kv_copy_batch_async,
                                     *    b200kv_encode_layers_workspace_bytes / b200kv_encode_layers_plan /
-                                    *    b200kv_encode_layers / b200kv_encode_layers_finish */
+                                    *    b200kv_encode_layers / b200kv_encode_layers_finish, b200kv_decode_plan_heads */
 #define B200KV_CODER_AC 0          /* payload = torchac-lineage arithmetic coder; container version 1 */
 #define B200KV_CODER_RANS 1        /* payload = rANS, 32-bit state / 16-bit renormalisation; container version 2 */
 #define B200KV_CODER_RANS_COMPACT 2 /* rANS as in version 2, compact side information; container version 3 (chunks of
@@ -215,6 +215,27 @@ int b200kv_decode_plan(const void* containers, int64_t containers_bytes, const i
                        const float* value_bins, uint32_t* status_out, void* workspace, int64_t workspace_bytes,
                        b200kv_decode_plan_t* plan, void* stream);
 int b200kv_decode_layers(const b200kv_decode_plan_t* plan, int32_t layer_begin, int32_t layer_end, void* stream);
+
+/*
+ * b200kv_decode_plan for a window of each container's KV heads: decoding the containers of another tensor-parallel
+ * layout into this rank's heads.  Container j holds src_H heads (its header's L and D are dst's, its H is src_H; the
+ * workspace is b200kv_decode_workspace_bytes(L, src_H, D, ...)).  Its heads [src_head0[j], src_head0[j] + n_heads[j])
+ * are decoded into destination heads [dst_head0[j], dst_head0[j] + n_heads[j]) at token dst_tok[j]; every other
+ * destination byte is left as it was.  The three arrays are HOST int32[n_chunks].  Containers may share a dst_tok when
+ * their destination head ranges do not overlap (several source shards into one rank, in one call).  The values are
+ * those of a whole decode: every (plane, channel) stream of a container is independent, and the stream offsets come from
+ * the fixed sections.  Status bits come from the decoded streams only.  b200kv_decode_layers runs the plan as it runs
+ * b200kv_decode_plan's.  Only the tiles of CT = 128 streams that meet a window are launched; a thread whose channel
+ * lies outside the window writes nothing.  Containers of every version are accepted, those of several groups (versions
+ * 1 / 2, more than 256 tokens) included.  Refused, writing nothing: n_heads[j] < 1, a window outside [0, src_H), a
+ * destination range outside [0, dst->H), and overlapping destination ranges at one dst_tok.
+ */
+int b200kv_decode_plan_heads(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                             const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,
+                             int32_t max_dtype, int32_t coder, const b200kv_kv_desc* dst, const float* key_bins,
+                             const float* value_bins, uint32_t* status_out, void* workspace, int64_t workspace_bytes,
+                             b200kv_decode_plan_t* plan, void* stream, int32_t src_H, const int32_t* src_head0,
+                             const int32_t* dst_head0, const int32_t* n_heads);
 
 /*
  * The encode of b200kv_encode_chunks in three steps, so that a layer can be encoded as soon as the forward pass has

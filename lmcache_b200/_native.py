@@ -96,6 +96,9 @@ SIGNATURES = {
     "b200kv_decode_plan": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, ctypes.POINTER(KvDesc),
                                     c_vp, c_vp, c_vp, c_vp, c_i64, ctypes.POINTER(DecodePlan), c_vp]),
     "b200kv_decode_layers": (c_i32, [ctypes.POINTER(DecodePlan), c_i32, c_i32, c_vp]),
+    "b200kv_decode_plan_heads": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, ctypes.POINTER(KvDesc),
+                                          c_vp, c_vp, c_vp, c_vp, c_i64, ctypes.POINTER(DecodePlan), c_vp, c_i32, c_vp,
+                                          c_vp, c_vp]),
     "b200kv_encode_layers_workspace_bytes": (c_i64, [c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
     "b200kv_encode_layers_plan": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp,
                                           c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_i64, ctypes.POINTER(EncodePlan),

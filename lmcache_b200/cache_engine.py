@@ -23,7 +23,8 @@ from lmcache_b200.codec import KvView, PinnedBuffer
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.logging import init_logger
 from lmcache_b200.storage_backend import CreateStorageBackend
-from lmcache_b200.pipeline import LayerwiseUpload
+from lmcache_b200.pipeline import HeadWindow, LayerwiseUpload
+from lmcache_b200.reshard import first_source_rank, source_shards
 from lmcache_b200.utils import CacheEngineKey, KVCache, _lmcache_nvtx_annotate
 
 logger = init_logger(__name__)
@@ -250,7 +251,11 @@ class LMCacheEngine:
         self.metadata = metadata
         self.chunk_size = config.chunk_size
         self.save_decode_cache = config.save_decode_cache
+        if config.reshard_world_sizes is not None and metadata.world_size in config.reshard_world_sizes:
+            raise ValueError(f"reshard_world_sizes {config.reshard_world_sizes} holds this engine's own world size "
+                             f"{metadata.world_size}: its chunks are served by the ordinary retrieve")
         self.engine_ = CreateStorageBackend(config, metadata)
+        self._reshard_counts: Dict[int, Dict[str, int]] = {}
         logger.debug(f"Current storage backend type {type(self.engine_)}")
 
     # ------------------------------------------------------------------ keys / hashes
@@ -507,29 +512,99 @@ class LMCacheEngine:
         keys = self._keys_of(full_chain[num_skip_chunk:], "vllm")
         base = num_skip_chunk * cs
         view = KvView.from_paged(kv_caches, slots[base:])
-        got_chunks, first = 0, 0
+        got_chunks, first, own = 0, 0, 0
+        layout = None            # the other layout that serves the chunks after this engine's own prefix (_reshard_get)
         if extra > 0 and keys:
             # the first chunk straddles the mask: decode it next to the cache and scatter only its unmasked tail
             t0 = min(cs, len(tokens) - base)
             tmp = torch.empty((view.L, 2, t0, view.H, view.D), dtype=view.dtype, device=dev)
-            if self.engine_.get_kv_into(keys[:1], KvView.from_blob(tmp, "vllm"), 0, cs) == 0:
-                self._touch(full_chain[:num_skip_chunk], "vllm")
-                ret_mask[:] = False
-                return ret_mask
+            tmp_view = KvView.from_blob(tmp, "vllm")
+            own = self.engine_.get_kv_into(keys[:1], tmp_view, 0, cs)
+            if own == 0:
+                layout, got = self._reshard_get(full_chain[num_skip_chunk:num_skip_chunk + 1], "vllm", tmp_view, 0)
+                if got == 0:
+                    self._touch(full_chain[:num_skip_chunk], "vllm")
+                    ret_mask[:] = False
+                    return ret_mask
             idx = slots[base + extra: base + t0]
             for l, (kc, vc) in enumerate(flat):
                 kc[idx] = tmp[l, 0, extra:]
                 vc[idx] = tmp[l, 1, extra:]
             got_chunks, first = 1, 1
         if len(keys) > first:
-            got_chunks += (get_kv or self.engine_.get_kv_into)(keys[first:], view, first * cs, cs)
-        self._touch(full_chain[:num_skip_chunk + got_chunks], "vllm")
+            if layout is None:
+                got_chunks += (get_kv or self.engine_.get_kv_into)(keys[first:], view, first * cs, cs)
+                own = got_chunks
+            layout, got = self._reshard_get(full_chain[num_skip_chunk + got_chunks:], "vllm", view, got_chunks * cs,
+                                            layout)
+            got_chunks += got
+        self._touch(full_chain[:num_skip_chunk + own], "vllm")
         got = min(base + got_chunks * cs, len(tokens))
         if got <= num_skip_tok:
             ret_mask[:] = False
         else:
             ret_mask[got:] = False
         return ret_mask
+
+    # ------------------------------------------------------------------ other tensor-parallel layouts
+    def _foreign_key(self, chunk_hash: str, fmt: str, world_size: int, rank: int) -> CacheEngineKey:
+        return CacheEngineKey(fmt, self.metadata.model_name, world_size, rank, chunk_hash)
+
+    def _reshard_layout(self, chunk_hash: str, fmt: str, Hg: int) -> Optional[int]:
+        """The first world size of reshard_world_sizes under which every shard of this rank's heads of the chunk exists."""
+        ws, rank = self.metadata.world_size, self.metadata.worker_id
+        for W in self.config.reshard_world_sizes:
+            shards = source_shards(Hg, W, ws, rank)
+            if shards and all(self.engine_.contains(self._foreign_key(chunk_hash, fmt, W, s.rank)) for s in shards):
+                return W
+        return None
+
+    def _reshard_groups(self, chunk_hashes, fmt: str, W: int, Hg: int) -> LazySeq:
+        """Per chunk, the (key, HeadWindow) of every container of layout W that this rank's heads are made of."""
+        wins = [(s.rank, HeadWindow(Hg // W, s.src_head0, s.n_heads, s.dst_head0))
+                for s in source_shards(Hg, W, self.metadata.world_size, self.metadata.worker_id)]
+        return LazySeq(lambda h: [(self._foreign_key(h, fmt, W, r), w) for r, w in wins], chunk_hashes)
+
+    def _reshard_get(self, chunk_hashes, fmt: str, view: KvView, tok0: int,
+                     layout: Optional[int] = None) -> Tuple[Optional[int], int]:
+        """Continue a retrieve whose own-layout prefix has ended: decode the chunks of `chunk_hashes` (the first at token
+        tok0 of `view`) from another layout's shards, up to the first incomplete chunk.  The layout is `layout`, or the
+        first of reshard_world_sizes that holds every shard of the first chunk.  Returns (layout, chunks served).  Off
+        (no request at all) unless reshard_world_sizes is set."""
+        get = getattr(self.engine_, "get_kv_shards_into", None)
+        if not self.config.reshard_world_sizes or get is None or len(chunk_hashes) == 0:
+            return layout, 0
+        Hg = view.H * self.metadata.world_size
+        if layout is None:
+            layout = self._reshard_layout(chunk_hashes[0], fmt, Hg)
+            if layout is None:
+                return None, 0
+        stats: Dict[str, int] = {}
+        n = get(self._reshard_groups(chunk_hashes, fmt, layout, Hg), view, tok0, self.chunk_size, stats)
+        if n:
+            c = self._reshard_counts.setdefault(layout, {"chunks": 0, "bytes": 0})
+            c["chunks"] += n
+            c["bytes"] += stats.get("bytes", 0)
+        return layout, n
+
+    def _reshard_geometry(self, chunk_hash: str, fmt: str):
+        """(L, H, D, dtype) of this rank's chunks for a replica that knows no geometry and whose own layout misses: read
+        from the header of the first source container of the first layout that has one (Hg = its H * W).  The backend
+        keeps that container for the fetch that follows."""
+        peek = getattr(self.engine_, "peek_geometry", None)
+        if peek is None:
+            return None
+        ws, rank = self.metadata.world_size, self.metadata.worker_id
+        for W in self.config.reshard_world_sizes:
+            g = peek(self._foreign_key(chunk_hash, fmt, W, first_source_rank(W, ws, rank)), fmt)
+            if g is not None and source_shards(g[1] * W, W, ws, rank):
+                return (g[0], g[1] * W // ws) + tuple(g[2:])
+        return None
+
+    def reshard_stats(self) -> Dict[int, Dict[str, int]]:
+        """Chunks served from other tensor-parallel layouts since the engine started, per source world size: {"chunks":
+        whole chunks decoded, "bytes": container bytes fetched for them}."""
+        return {W: dict(c) for W, c in self._reshard_counts.items()}
 
     def _touch(self, chunk_hashes, fmt: str) -> None:
         """Recency update for a bounded local tier (lmcache_b200/eviction.py): one call with the keys of a chain prefix,
@@ -557,6 +632,7 @@ class LMCacheEngine:
         in _retrieve_paged."""
         keys = self._keys_of(chunk_hashes, fmt)
         geom = self._kv_geometry()
+        own_miss = False         # this layout holds not even the first chunk: only another layout can serve it
         if geom is None:
             # shapes unknown (nothing stored through this engine yet -- the normal case for a retrieve-only replica):
             # read them from the first chunk's container header / stored blob; only backends without that door pay
@@ -569,6 +645,9 @@ class LMCacheEngine:
                 if first is not None:
                     geom = ((first.shape[0], first.shape[3], first.shape[4]) if fmt == "vllm" else
                             (first.shape[0], first.shape[2], first.shape[4])) + (first.dtype,)
+            if geom is None and self.config.reshard_world_sizes:
+                geom = self._reshard_geometry(chunk_hashes[0], fmt)
+                own_miss = geom is not None
             if geom is None:
                 self._touch(full_chain[:num_skip_chunk], fmt)
                 logger.info("Retrieved 0 chunks")
@@ -583,8 +662,10 @@ class LMCacheEngine:
         shape = (L, 2, n_tok_max, H, D) if fmt == "vllm" else (L, 2, H, n_tok_max, D)
         device = torch.device("cuda", torch.cuda.current_device())
         blob = torch.empty(shape, dtype=dtype, device=device)
-        n = (get_kv or self.engine_.get_kv_into)(keys, KvView.from_blob(blob, fmt), 0, self.chunk_size)
-        self._touch(full_chain[:num_skip_chunk + n], fmt)
+        view = KvView.from_blob(blob, fmt)
+        own = 0 if own_miss else (get_kv or self.engine_.get_kv_into)(keys, view, 0, self.chunk_size)
+        n = own + self._reshard_get(chunk_hashes[own:], fmt, view, own * self.chunk_size)[1]
+        self._touch(full_chain[:num_skip_chunk + own], fmt)
         if n == 0:
             logger.info("Retrieved 0 chunks")
             ret_mask[:] = False

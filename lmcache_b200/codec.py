@@ -535,6 +535,20 @@ class CacheGenCodec:
         """Decode containers that already sit in device memory at base_ptr + offsets[j] (asynchronous).  `buf_bytes` is
         the size of the buffer behind base_ptr: it must extend N.READ_SLACK bytes past every container (checked by the
         library); totals[j] = header.total_bytes."""
+        self._decode_raw(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, stream, _locked)
+
+    def decode_raw_heads(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
+                         ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
+                         src_H: int, src_head0: Sequence[int], dst_head0: Sequence[int], n_heads: Sequence[int],
+                         stream: Optional[torch.cuda.Stream] = None) -> None:
+        """decode_raw for a window of each container's heads (b200kv_decode_plan_heads): every container holds src_H
+        heads, and its heads [src_head0[j], src_head0[j] + n_heads[j]) land in dst's heads from dst_head0[j] on, at token
+        dst_tok[j].  The rest of dst is left as it was."""
+        self._decode_raw(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, stream, False,
+                         (src_H, src_head0, dst_head0, n_heads))
+
+    def _decode_raw(self, base_ptr, buf_bytes, offsets, totals, ntokens, dst: KvView, dst_tok, max_dtype, coder, stream,
+                    _locked: bool, heads=None) -> None:
         n = len(offsets)
         if n == 0:
             return
@@ -543,7 +557,8 @@ class CacheGenCodec:
 
         def run():
             tstream = stream if stream is not None else torch.cuda.current_stream()
-            ws_bytes = lib.b200kv_decode_workspace_bytes(dst.L, dst.H, dst.D, tmax, n)
+            # a shape the library refuses has no workspace size (< 0): the decode call below says why
+            ws_bytes = max(lib.b200kv_decode_workspace_bytes(dst.L, heads[0] if heads else dst.H, dst.D, tmax, n), 0)
             if not _locked:
                 self._order_decode(tstream, 0, ws_bytes)
             self._dec_ws = self._grow(self._dec_ws, ws_bytes, dst.device)
@@ -552,12 +567,18 @@ class CacheGenCodec:
                     self._dec_sync()
                 self._dec_status = PinnedBuffer(max(4096, 8 * n))
             self._dec_status_n = n
-            N.check(lib.b200kv_decode_chunks(base_ptr, int(buf_bytes), N.i64_array(list(offsets)),
-                                             N.i64_array(list(totals)), N.i32_array(list(ntokens)),
-                                             N.i64_array(list(dst_tok)), n, int(max_dtype), int(coder),
-                                             ctypes.byref(dst.desc), self._kb, self._vb, self._dec_status.dev_ptr,
-                                             self._dec_ws.data_ptr(), self._dec_ws.numel(), tstream.cuda_stream),
-                    "decode_chunks")
+            args = (base_ptr, int(buf_bytes), N.i64_array(list(offsets)), N.i64_array(list(totals)),
+                    N.i32_array(list(ntokens)), N.i64_array(list(dst_tok)), n, int(max_dtype), int(coder),
+                    ctypes.byref(dst.desc), self._kb, self._vb, self._dec_status.dev_ptr, self._dec_ws.data_ptr(),
+                    self._dec_ws.numel())
+            if heads is None:
+                N.check(lib.b200kv_decode_chunks(*args, tstream.cuda_stream), "decode_chunks")
+            else:
+                plan = N.DecodePlan()
+                N.check(lib.b200kv_decode_plan_heads(*args, ctypes.byref(plan), tstream.cuda_stream, int(heads[0]),
+                                                     N.i32_array(list(heads[1])), N.i32_array(list(heads[2])),
+                                                     N.i32_array(list(heads[3]))), "decode_plan_heads")
+                self.decode_layers(plan, 0, dst.L, tstream)
             if self._dec_event is None:
                 self._dec_event = torch.cuda.Event()
             self._dec_event.record(tstream)
@@ -587,6 +608,27 @@ class CacheGenCodec:
                                        int(coder), ctypes.byref(dst.desc), self._kb, self._vb, status_ptr or None,
                                        ws.data_ptr(), ws.numel(), ctypes.byref(plan), stream.cuda_stream),
                 "decode_plan")
+        return plan, ws
+
+    def decode_plan_heads(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
+                          ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
+                          src_H: int, src_head0: Sequence[int], dst_head0: Sequence[int], n_heads: Sequence[int],
+                          stream: torch.cuda.Stream, status_ptr: int = 0) -> Tuple["N.DecodePlan", torch.Tensor]:
+        """decode_plan for head windows (see decode_raw_heads); decode_layers runs the plan."""
+        n = len(offsets)
+        lib = N.lib()
+        ws = torch.empty(max(lib.b200kv_decode_workspace_bytes(dst.L, int(src_H), dst.D, max(ntokens), n), 0),
+                         dtype=torch.uint8, device=dst.device)     # < 0: a shape the plan call refuses, with its reason
+        ws.record_stream(stream)
+        plan = N.DecodePlan()
+        N.check(lib.b200kv_decode_plan_heads(base_ptr, int(buf_bytes), N.i64_array(list(offsets)),
+                                             N.i64_array(list(totals)), N.i32_array(list(ntokens)),
+                                             N.i64_array(list(dst_tok)), n, int(max_dtype), int(coder),
+                                             ctypes.byref(dst.desc), self._kb, self._vb, status_ptr or None,
+                                             ws.data_ptr(), ws.numel(), ctypes.byref(plan), stream.cuda_stream,
+                                             int(src_H), N.i32_array(list(src_head0)), N.i32_array(list(dst_head0)),
+                                             N.i32_array(list(n_heads))),
+                "decode_plan_heads")
         return plan, ws
 
     @staticmethod

@@ -4,7 +4,7 @@ from __future__ import annotations
 
 import re
 from dataclasses import dataclass
-from typing import Optional
+from typing import List, Optional
 
 import yaml
 
@@ -41,6 +41,10 @@ class LMCacheEngineConfig:
     # retrieve of a resident chunk decodes it in place instead of uploading it (lmcache_b200/device_cache.py).  None =
     # off.  The level is inclusive: every device copy has its tier copy beside it.  Only the two CacheGen tiers take it.
     device_cache_bytes: Optional[int] = None
+    # not in the reference: other tensor-parallel world sizes whose stored chunks a retrieve may decode into this rank's
+    # KV heads once its own layout's prefix ends (lmcache_b200/reshard.py), tried in this order.  None = off.  Needs a
+    # remote tier with the CacheGen serde (CreateStorageBackend); must not hold the engine's own world size (LMCacheEngine).
+    reshard_world_sizes: Optional[List[int]] = None
 
     def __post_init__(self):
         if self.local_serde is None:
@@ -54,6 +58,12 @@ class LMCacheEngineConfig:
         d = self.device_cache_bytes
         if d is not None and (isinstance(d, bool) or not isinstance(d, int) or d <= 0):
             raise ValueError(f"Invalid device cache size: {d!r} (a positive number of bytes, or None)")
+        r = self.reshard_world_sizes
+        if r is not None and (not isinstance(r, (list, tuple)) or not r or len(set(r)) != len(r) or
+                              any(isinstance(w, bool) or not isinstance(w, int) or w <= 0 for w in r)):
+            raise ValueError(f"Invalid reshard world sizes: {r!r} (a non-empty list of distinct positive ints, or None)")
+        if r is not None:
+            self.reshard_world_sizes = list(r)
 
     @staticmethod
     def from_defaults(chunk_size: int = 256, local_device: str = "cuda",
@@ -61,16 +71,19 @@ class LMCacheEngineConfig:
                       pipelined_backend: bool = False, save_decode_cache: bool = False,
                       local_serde: Optional[str] = None,
                       local_capacity_bytes: Optional[int] = None,
-                      device_cache_bytes: Optional[int] = None) -> "LMCacheEngineConfig":
+                      device_cache_bytes: Optional[int] = None,
+                      reshard_world_sizes: Optional[List[int]] = None) -> "LMCacheEngineConfig":
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
-                                   save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes)
+                                   save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes,
+                                   reshard_world_sizes)
 
     @staticmethod
     def from_legacy(chunk_size: int = 256, backend: str = "cuda", persist_path: Optional[str] = None,
                     remote_serde: Optional[str] = "torch", pipelined_backend: bool = False,
                     save_decode_cache: bool = False, local_serde: Optional[str] = None,
                     local_capacity_bytes: Optional[int] = None,
-                    device_cache_bytes: Optional[int] = None) -> "LMCacheEngineConfig":
+                    device_cache_bytes: Optional[int] = None,
+                    reshard_world_sizes: Optional[List[int]] = None) -> "LMCacheEngineConfig":
         """backend: "cpu" | "cuda" | "file://<dir>/" | "<scheme>://<host>:<port>" (config.py:51-82)."""
         local_device: Optional[str] = None
         remote_url: Optional[str] = None
@@ -81,7 +94,8 @@ class LMCacheEngineConfig:
         elif _URL_RE.match(backend):
             remote_url = backend
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
-                                   save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes)
+                                   save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes,
+                                   reshard_world_sizes)
 
     @staticmethod
     def from_file(file_path: str) -> "LMCacheEngineConfig":
@@ -97,6 +111,7 @@ class LMCacheEngineConfig:
         local_serde = cfg.get("local_serde", None)
         local_capacity_bytes = cfg.get("local_capacity_bytes", None)
         device_cache_bytes = cfg.get("device_cache_bytes", None)
+        reshard_world_sizes = cfg.get("reshard_world_sizes", None)
 
         if local_device in ("cpu", "cuda", None):
             pass
@@ -109,7 +124,8 @@ class LMCacheEngineConfig:
             raise ValueError(f"Invalid remote storage url: {remote_url}")
 
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
-                                   save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes)
+                                   save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes,
+                                   reshard_world_sizes)
 
 
 class GlobalConfig:

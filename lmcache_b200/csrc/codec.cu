@@ -23,6 +23,9 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
+#include <vector>
+
 #include "ac_core.cuh"
 #include "common.cuh"
 
@@ -989,16 +992,19 @@ struct DecChunk {
     int64_t dst_tok;
     int32_t t, ngroups;
     uint32_t payload_bytes;      // from the (host-validated) header: stream offsets are clamped to it
-    uint32_t pad;
+    // head window (b200kv_decode_plan_heads; the whole container otherwise): container channels [cw0, cw1) are decoded
+    // into destination channel c + dshift; they lie in tiles [ct0, ct0 + ntw) of every plane
+    int32_t ct0, ntw, cw0, cw1, dshift;
 };
 
 struct DecParams {
     PlaneTable pt;               // destination planes; maxq = C_l = bins // 2 - 1
     int64_t sT, sH;
     const int64_t* slot_map;     // paged destination: token i lives in row slot_map[i]; NULL = row i
-    int32_t L, H, D, C, out_dtype, max_dtype, n_chunks, tpp, tiles_max;
+    int32_t L, H, D, C, out_dtype, max_dtype, n_chunks, tpp, tiles_max;   // H, C: the containers' (src_H with windows)
     int32_t compact;             // containers are version 3
     int32_t lb, nlay;            // decode_kernel: this launch decodes layers [lb, lb + nlay), i.e. planes lb.. and L + lb..
+    int32_t wtpp;                // decode_kernel: tiles launched per plane = the largest window's ntw (tpp without windows)
     const DecChunk* chunks;      // device
     unsigned long long* tile_base;   // [n_chunks][tiles_max]: tile sums, then exclusive prefix
     uint32_t* status;            // [n_chunks] or NULL: bit 0 = a rANS stream did not return to its initial state,
@@ -1334,24 +1340,29 @@ __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
     const DecChunk dc = P.chunks[j];
     const int NL = 2 * P.L;
     const int per_group = NL * P.tpp;
-    // blockIdx.x walks the launch's tiles of each group: K planes lb.., then V planes L + lb..; `tile` is the tile's
-    // index among all of the chunk's tiles (tile_base)
-    const int launch_group = 2 * P.nlay * P.tpp;
+    // blockIdx.x walks the launch's tiles of each group: K planes lb.., then V planes L + lb.., and in each plane the
+    // wtpp tiles from the chunk's window tile ct0 on (those past the window's ntw leave); `tile` is the tile's index
+    // among all of the chunk's tiles (tile_base).  Without windows ct0 = 0 and ntw = wtpp = tpp.
+    const int launch_group = 2 * P.nlay * P.wtpp;
     const int g = blockIdx.x / launch_group;
     if (g >= dc.ngroups) return;
     const int kt = blockIdx.x - g * launch_group;
-    const int tile = g * per_group + kt + (kt < P.nlay * P.tpp ? P.lb : P.L - P.nlay + P.lb) * P.tpp;
-    const int rem = tile - g * per_group;
-    const int nl = rem / P.tpp;
-    const int ct = rem - nl * P.tpp;
+    const int kp = kt / P.wtpp;
+    const int wt = kt - kp * P.wtpp;
+    if (wt >= dc.ntw) return;
+    const int nl = kp + (kp < P.nlay ? P.lb : P.L - P.nlay + P.lb);
+    const int ct = dc.ct0 + wt;
+    const int tile = g * per_group + nl * P.tpp + ct;
     const int tok0 = g * kGroup;
     const int gt = min(kGroup, dc.t - tok0);
     const int c = ct * CT + tid;
-    const bool active = c < P.C;
+    // every stream of the tile takes part in the scan of its lengths; only those in the window are decoded
+    const bool in_c = c < P.C;
+    const bool active = c >= dc.cw0 && c < dc.cw1;
     const int ncols = min(CT, P.C - ct * CT);
     const Layout lo = layout_of(P, dc.t);
 
-    const uint32_t len = active ? load_len(dc.base + lo.off_lengths, ((int64_t)g * NL + nl) * P.C + c, P.compact != 0) : 0u;
+    const uint32_t len = in_c ? load_len(dc.base + lo.off_lengths, ((int64_t)g * NL + nl) * P.C + c, P.compact != 0) : 0u;
     uint32_t tile_total;
     const uint32_t my_rel = block_excl_scan(len, s_warp, &tile_total);
     // the stream's byte offset inside the container; a corrupt lengths section cannot push it outside the payload
@@ -1525,9 +1536,10 @@ __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
 
     if (!active) return;
     const uint32_t* erow = tab + tid * kLp;
-    const int h = c / P.D;
+    const int oc = c + dc.dshift;                          // destination channel
+    const int h = oc / P.D;
     uint16_t* dst = const_cast<uint16_t*>(P.pt.p[nl]) + (PAGED ? 0 : (dc.dst_tok + tok0) * P.sT) + (int64_t)h * P.sH +
-                    (c - h * P.D);
+                    (oc - h * P.D);
     const int64_t* slots = PAGED ? P.slot_map + dc.dst_tok + tok0 : nullptr;
     uint32_t bad = beyond ? 2u : 0u;
     if constexpr (CODER == CODER_RANS) {
@@ -2010,12 +2022,13 @@ int b200kv_encode_layers_finish(const b200kv_encode_plan_t* plan_in, void* strea
     return 0;
 }
 
-int b200kv_decode_plan(const void* containers, int64_t containers_bytes, const int64_t* offsets,
-                       const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,
-                       int32_t max_dtype, int32_t coder, const b200kv_kv_desc* dst, const float* key_bins,
-                       const float* value_bins, uint32_t* status_out, void* workspace, int64_t workspace_bytes,
-                       b200kv_decode_plan_t* plan_out, void* stream_) {
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+// b200kv_decode_plan and b200kv_decode_plan_heads: src_head0 == NULL decodes every container whole (src_H = dst->H)
+static int decode_plan_impl(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                            const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,
+                            int32_t max_dtype, int32_t coder, const b200kv_kv_desc* dst, const float* key_bins,
+                            const float* value_bins, uint32_t* status_out, void* workspace, int64_t workspace_bytes,
+                            b200kv_decode_plan_t* plan_out, cudaStream_t stream, int32_t src_H, const int32_t* src_head0,
+                            const int32_t* dst_head0, const int32_t* n_heads) {
     B2_REQUIRE(plan_out != nullptr, "plan is NULL");
     DecPlan* plan = reinterpret_cast<DecPlan*>(plan_out);
     plan->magic = 0u;
@@ -2028,12 +2041,43 @@ int b200kv_decode_plan(const void* containers, int64_t containers_bytes, const i
     B2_REQUIRE(containers && offsets && total_bytes && ntokens && dst_tok && n_chunks > 0, "bad chunk arrays");
     B2_REQUIRE(max_dtype == B200KV_DT_BF16 || max_dtype == B200KV_DT_FP16, "bad max_dtype");
     B2_REQUIRE(dst->sT > 0 && dst->sT < (1ll << 23), "destination token stride out of range");
+    const bool windows = src_head0 != nullptr;
+    if (windows) {
+        B2_REQUIRE(dst_head0 != nullptr && n_heads != nullptr, "head window arrays are NULL");
+        B2_REQUIRE(src_H > 0 && (int64_t)src_H * dst->D < (1ll << 24), "src_H out of range");
+    } else {
+        src_H = dst->H;
+    }
     P.sT = dst->sT; P.sH = dst->sH;
     P.slot_map = dst->slot_map;
-    P.L = dst->L; P.H = dst->H; P.D = dst->D; P.C = dst->H * dst->D;
+    P.L = dst->L; P.H = src_H; P.D = dst->D; P.C = src_H * dst->D;
     P.out_dtype = dst->dtype; P.max_dtype = max_dtype; P.n_chunks = n_chunks;
     P.tpp = tiles_per_plane(P.C);
+    P.wtpp = P.tpp;
     P.lb = 0; P.nlay = P.L;
+    if (windows) {
+        int wt = 1;
+        for (int j = 0; j < n_chunks; ++j) {
+            B2_REQUIRE(n_heads[j] >= 1, "a head window must hold at least one head");
+            B2_REQUIRE(src_head0[j] >= 0 && src_head0[j] <= src_H - n_heads[j], "head window outside the container's heads");
+            B2_REQUIRE(dst_head0[j] >= 0 && dst_head0[j] <= dst->H - n_heads[j],
+                       "head window outside the destination's heads");
+            const int c0 = src_head0[j] * P.D, c1 = (src_head0[j] + n_heads[j]) * P.D;
+            wt = std::max(wt, (c1 - 1) / CT - c0 / CT + 1);
+        }
+        // containers that share a destination token must not share a destination head
+        std::vector<int> ord((size_t)n_chunks);
+        for (int j = 0; j < n_chunks; ++j) ord[(size_t)j] = j;
+        std::sort(ord.begin(), ord.end(), [&](int a, int b) {
+            return dst_tok[a] != dst_tok[b] ? dst_tok[a] < dst_tok[b] : dst_head0[a] < dst_head0[b];
+        });
+        for (size_t k = 1; k < ord.size(); ++k) {
+            const int a = ord[k - 1], b = ord[k];
+            B2_REQUIRE(dst_tok[a] != dst_tok[b] || dst_head0[a] + n_heads[a] <= dst_head0[b],
+                       "head windows overlap at the same destination token");
+        }
+        P.wtpp = wt;
+    }
     int tmax = 0;
     for (int j = 0; j < n_chunks; ++j) {
         B2_REQUIRE(ntokens[j] > 0, "ntokens must be positive");
@@ -2081,7 +2125,11 @@ int b200kv_decode_plan(const void* containers, int64_t containers_bytes, const i
             hc[j].ngroups = (ntokens[j] + kGroup - 1) / kGroup;
             const Layout lj = make_layout(P.L, P.C, ntokens[j], P.compact);
             hc[j].payload_bytes = (uint32_t)(total_bytes[j] - lj.off_payload);
-            hc[j].pad = 0;
+            hc[j].cw0 = windows ? src_head0[j] * P.D : 0;
+            hc[j].cw1 = windows ? (src_head0[j] + n_heads[j]) * P.D : P.C;
+            hc[j].dshift = windows ? (dst_head0[j] - src_head0[j]) * P.D : 0;
+            hc[j].ct0 = hc[j].cw0 / CT;
+            hc[j].ntw = (hc[j].cw1 - 1) / CT - hc[j].ct0 + 1;
         }
         cudaError_t e = cudaMemcpyAsync(ws, hc, sizeof(DecChunk) * (size_t)n_chunks, cudaMemcpyHostToDevice, stream);
         free(hc);
@@ -2110,6 +2158,29 @@ int b200kv_decode_plan(const void* containers, int64_t containers_bytes, const i
     return 0;
 }
 
+int b200kv_decode_plan(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                       const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,
+                       int32_t max_dtype, int32_t coder, const b200kv_kv_desc* dst, const float* key_bins,
+                       const float* value_bins, uint32_t* status_out, void* workspace, int64_t workspace_bytes,
+                       b200kv_decode_plan_t* plan_out, void* stream) {
+    return decode_plan_impl(containers, containers_bytes, offsets, total_bytes, ntokens, dst_tok, n_chunks, max_dtype,
+                            coder, dst, key_bins, value_bins, status_out, workspace, workspace_bytes, plan_out,
+                            static_cast<cudaStream_t>(stream), 0, nullptr, nullptr, nullptr);
+}
+
+int b200kv_decode_plan_heads(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                             const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,
+                             int32_t max_dtype, int32_t coder, const b200kv_kv_desc* dst, const float* key_bins,
+                             const float* value_bins, uint32_t* status_out, void* workspace, int64_t workspace_bytes,
+                             b200kv_decode_plan_t* plan_out, void* stream, int32_t src_H, const int32_t* src_head0,
+                             const int32_t* dst_head0, const int32_t* n_heads) {
+    if (plan_out != nullptr) reinterpret_cast<DecPlan*>(plan_out)->magic = 0u;
+    B2_REQUIRE(src_head0 != nullptr, "head window arrays are NULL");
+    return decode_plan_impl(containers, containers_bytes, offsets, total_bytes, ntokens, dst_tok, n_chunks, max_dtype,
+                            coder, dst, key_bins, value_bins, status_out, workspace, workspace_bytes, plan_out,
+                            static_cast<cudaStream_t>(stream), src_H, src_head0, dst_head0, n_heads);
+}
+
 int b200kv_decode_layers(const b200kv_decode_plan_t* plan_in, int32_t layer_begin, int32_t layer_end, void* stream_) {
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     B2_REQUIRE(plan_in != nullptr, "plan is NULL");
@@ -2122,7 +2193,7 @@ int b200kv_decode_layers(const b200kv_decode_plan_t* plan_in, int32_t layer_begi
     const int coder = plan->coder;
     const bool transposed = plan->transposed != 0;
     const size_t smem = (size_t)(CT * kLp + kGroup + 32) * 4;
-    dim3 grid((unsigned)((int64_t)plan->gmax * 2 * P.nlay * P.tpp), (unsigned)P.n_chunks);
+    dim3 grid((unsigned)((int64_t)plan->gmax * 2 * P.nlay * P.wtpp), (unsigned)P.n_chunks);
     ProfScope prof(kProfDecode, stream);
 #define B2_LAUNCH_DEC1(DT, PAGED, CODER, TR)                                                                           \
     do {                                                                                                               \

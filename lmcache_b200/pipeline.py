@@ -26,7 +26,7 @@ import queue
 import threading
 import time
 from concurrent.futures import Future
-from typing import Callable, Iterable, Iterator, List, Optional, Sequence
+from typing import Callable, Iterable, Iterator, List, NamedTuple, Optional, Sequence
 
 import numpy as np
 import torch
@@ -620,9 +620,20 @@ def fetched_in_order(futures: Iterable[Future], window: Optional[int] = None) ->
                 rec.blk.free()
 
 
-def _continues_match(r: HostContainer, first: Optional[HostContainer], dst: KvView, tok: int) -> bool:
-    """May container `r`, landing at token `tok` of `dst`, extend a match that began with `first` (None: r is first)?"""
-    return (r.L, r.H, r.D) == (dst.L, dst.H, dst.D) and tok + r.ntokens <= dst.ntokens and \
+class HeadWindow(NamedTuple):
+    """What upload_decode takes of a container of src_H heads: heads [src_head0, src_head0 + n_heads), written at the
+    destination's head dst_head0 (lmcache_b200/reshard.py says which)."""
+    src_H: int
+    src_head0: int
+    n_heads: int
+    dst_head0: int
+
+
+def _continues_match(r: HostContainer, first: Optional[HostContainer], dst: KvView, tok: int,
+                     src_H: Optional[int] = None) -> bool:
+    """May container `r`, landing at token `tok` of `dst`, extend a match that began with `first` (None: r is first)?
+    src_H: the heads r must hold when it is decoded through a head window (None: dst's)."""
+    return (r.L, r.H, r.D) == (dst.L, dst.H if src_H is None else src_H, dst.D) and tok + r.ntokens <= dst.ntokens and \
         (first is None or (r.max_dtype, r.coder) == (first.max_dtype, first.coder))
 
 
@@ -673,7 +684,7 @@ def _wait_filled(recs: Sequence[HostContainer], stream: torch.cuda.Stream) -> No
 
 def upload_decode(codec: CacheGenCodec, upload: UploadRing, records: Iterable[Optional[HostContainer]], dst: KvView,
                   dst_tok0: int, chunk_size: int, release: Optional[DeferredFree] = None,
-                  level: Optional[DeviceLevel] = None) -> int:
+                  level: Optional[DeviceLevel] = None, windows: Optional[Sequence[HeadWindow]] = None) -> int:
     """Upload + decode consecutive chunks straight into `dst`: records[i] (None: a miss) is chunk i and lands at token
     dst_tok0 + i * chunk_size.  Wave by wave the containers are copied into an UploadRing slot on its copy stream and
     decoded on the current stream; nothing is synchronised, and the records are consumed as the caller produces them
@@ -686,28 +697,45 @@ def upload_decode(codec: CacheGenCodec, upload: UploadRing, records: Iterable[Op
     With a device `level`, a wave's resident records are not uploaded: they are decoded where they are, in one call at
     their pool offsets after their fill events, and the rest of the wave in a second call from the slot.  Their
     `last_read` is left alone and their `dev_read` becomes that decode's event.  Each uploaded record is offered to the
-    level (level.promote) right after its wave's upload."""
+    level (level.promote) right after its wave's upload.
+
+    With `windows`, chunk i is a group of containers: records[i] is a sequence aligned with `windows` (None: a miss),
+    and container k of the group is decoded through head window windows[k] (CacheGenCodec.decode_raw_heads): the chunk
+    is what another tensor-parallel layout stored for this rank's heads.  A chunk matches only when every container of
+    its group is there, holds windows[k].src_H heads and continues the match; the stopped group's blocks are freed as
+    above.  A wave then counts containers, not chunks."""
     W = wave_chunks_default()
     lib = N.lib()
     wave: List[HostContainer] = []
+    wtok: List[int] = []                  # destination token of each wave entry
+    wwin: List[Optional[HeadWindow]] = []
+    widx: List[int] = []                  # chunk index of each wave entry
     n = 0
     first = None
     with torch.cuda.device(dst.device):
         cur = torch.cuda.current_stream()
 
+        def decode(base_ptr: int, buf_bytes: int, offs: List[int], sel: List[int]) -> None:
+            recs = [wave[j] for j in sel]
+            args = (base_ptr, buf_bytes, offs, [r.nbytes for r in recs], [r.ntokens for r in recs], dst,
+                    [wtok[j] for j in sel], wave[0].max_dtype, wave[0].coder)
+            if windows is None:
+                codec.decode_raw(*args, cur)
+            else:
+                ws = [wwin[j] for j in sel]
+                codec.decode_raw_heads(*args, ws[0].src_H, [w.src_head0 for w in ws], [w.dst_head0 for w in ws],
+                                       [w.n_heads for w in ws], cur)
+
         def flush():
             if not wave:
                 return
-            w0 = n - len(wave)
             res = [j for j, r in enumerate(wave) if level is not None and level.resident(r)]
             up = [j for j in range(len(wave)) if j not in res] if res else list(range(len(wave)))
             if res:
                 pool = level.cache.pool
                 recs = [wave[j] for j in res]
                 _wait_filled(recs, cur)
-                codec.decode_raw(pool.dev_ptr, pool.buf.numel(), [r.dev.offset for r in recs], [r.nbytes for r in recs],
-                                 [r.ntokens for r in recs], dst, [dst_tok0 + (w0 + j) * chunk_size for j in res],
-                                 wave[0].max_dtype, wave[0].coder, cur)
+                decode(pool.dev_ptr, pool.buf.numel(), [r.dev.offset for r in recs], res)
                 level.mark_read(recs, cur)
                 level.hit(len(recs))
             if up:
@@ -728,30 +756,41 @@ def upload_decode(codec: CacheGenCodec, upload: UploadRing, records: Iterable[Op
                     release.add(ev, [r.blk for r in recs])
                 promoted = None
                 if level is not None:       # after the wave's event: the decode does not wait for these copies
-                    if sum(level.promote(w0 + j, r, buf.data_ptr() + off, upload.copy_stream)
+                    if sum(level.promote(widx[j], r, buf.data_ptr() + off, upload.copy_stream)
                            for j, r, off in zip(up, recs, offs)):
                         promoted = torch.cuda.Event()
                         promoted.record(upload.copy_stream)
                 cur.wait_event(ev)
-                codec.decode_raw(buf.data_ptr(), buf.numel(), offs, [r.nbytes for r in recs], [r.ntokens for r in recs],
-                                 dst, [dst_tok0 + (w0 + j) * chunk_size for j in up], wave[0].max_dtype,
-                                 wave[0].coder, cur)
+                decode(buf.data_ptr(), buf.numel(), offs, up)
                 if promoted is not None:    # the slot's next writer (or its replacement) waits for the promotion's reads
                     cur.wait_event(promoted)
                 upload.mark_read(slot, cur)
-            wave.clear()
+            for lst in (wave, wtok, wwin, widx):
+                lst.clear()
 
-        for r in records:
-            if r is None:
+        for item in records:
+            if item is None:
                 break
-            if not _continues_match(r, first, dst, dst_tok0 + n * chunk_size):
-                if release is not None and r.blk is not None:
-                    r.blk.free()
+            group = [item] if windows is None else list(item)
+            wins = [None] if windows is None else list(windows)
+            tok = dst_tok0 + n * chunk_size
+            ok = len(group) == len(wins) and all(r is not None for r in group)
+            ok = ok and all(_continues_match(r, first or group[0], dst, tok, w.src_H if w is not None else None) and
+                            r.ntokens == group[0].ntokens for r, w in zip(group, wins))
+            if not ok:
+                if release is not None:
+                    for r in group:
+                        if r is not None and r.blk is not None:
+                            r.blk.free()
                 break
-            first = first or r
-            wave.append(r)
+            first = first or group[0]
+            for r, w in zip(group, wins):
+                wave.append(r)
+                wtok.append(tok)
+                wwin.append(w)
+                widx.append(n)
             n += 1
-            if len(wave) == W:
+            if len(wave) >= W:
                 flush()
         flush()
     return n

@@ -20,6 +20,12 @@ def CreateStorageBackend(config: LMCacheEngineConfig, metadata: LMCacheEngineMet
         if local in ("cpu", "cuda") and not (local == "cpu" and config.local_serde == "cachegen"):
             raise ValueError(f"device_cache_bytes is honoured by the CacheGen tiers only (local_device='cpu' with "
                              f"local_serde='cachegen', or a directory), not by local_device={local!r}")
+    if config.reshard_world_sizes is not None:
+        # another layout's chunks exist only on a shared remote tier, and only CacheGen containers can be decoded a
+        # window of heads at a time
+        if remote is None or config.remote_serde != "cachegen":
+            raise ValueError("reshard_world_sizes needs a remote tier with remote_serde='cachegen', not "
+                             f"remote_url={remote!r} with remote_serde={config.remote_serde!r}")
     if local is None and isinstance(remote, str):
         from lmcache_b200.storage_backend.remote_backend import LMCPipelinedRemoteBackend, LMCRemoteBackend
         return (LMCPipelinedRemoteBackend if config.pipelined_backend else LMCRemoteBackend)(config, metadata)

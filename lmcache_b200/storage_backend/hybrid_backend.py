@@ -66,6 +66,12 @@ class LMCHybridBackend(LMCBackendInterface):
             n += self.remote_store.get_kv_into(keys[n:], dst, dst_tok0 + n * chunk_size, chunk_size)
         return n
 
+    def get_kv_shards_into(self, groups, dst, dst_tok0: int, chunk_size: int, stats=None) -> int:
+        """Chunks of another tensor-parallel layout come from the remote tier alone: the local tier holds this process's
+        keys only, and the chunks served are not kept in it (they are another layout's quantisation, not this one's)."""
+        f = getattr(self.remote_store, "get_kv_shards_into", None)
+        return f(groups, dst, dst_tok0, chunk_size, stats) if f is not None else 0
+
     def touch(self, keys) -> None:
         f = getattr(self.local_store, "touch", None)
         if f is not None:

@@ -33,6 +33,41 @@ class RemoteBackendEndSignal:
     pass
 
 
+class LazyFlat:
+    """The keys of groups of (key, window), k per group, in order; a group is read when one of its keys is reached."""
+
+    def __init__(self, groups, k: int):
+        self.groups, self.k = groups, k
+
+    def __len__(self) -> int:
+        return len(self.groups) * self.k
+
+    def __getitem__(self, i: int):
+        return self.groups[i // self.k][i % self.k][0]
+
+    def __iter__(self):
+        for g in self.groups:
+            for key, _ in g:
+                yield key
+
+
+def _grouped(recs, k: int, sizes: List[int]):
+    """recs (fetched container records) k at a time; the container bytes of each group yielded go to `sizes`.  Records
+    of a group the consumer never received are freed when it stops."""
+    buf: list = []
+    try:
+        for r in recs:
+            buf.append(r)
+            if len(buf) == k:
+                out, buf = buf, []
+                sizes.append(sum(x.nbytes for x in out if x is not None))
+                yield out
+    finally:
+        for r in buf:
+            if r is not None and r.blk is not None:
+                r.blk.free()
+
+
 class LMCRemoteBackend(LMCBackendInterface):
 
     def __init__(self, config: LMCacheEngineConfig, metadata: LMCacheEngineMetadata):
@@ -273,15 +308,31 @@ class LMCRemoteBackend(LMCBackendInterface):
         return len(blobs)
 
     def _get_striped(self, keys, dst, dst_tok0: int, chunk_size: int) -> int:
+        return self._get_striped_groups(keys, None, dst, dst_tok0, chunk_size)
+
+    def get_kv_shards_into(self, groups, dst, dst_tok0: int, chunk_size: int, stats: Optional[dict] = None) -> int:
+        """Serve chunks that another tensor-parallel layout stored: groups[i] lists (key, HeadWindow) for chunk i -- the
+        source containers and the window of each that makes up this rank's heads (the same windows for every chunk).
+        They are fetched over the striped connections and decoded into `dst` (chunk i at token dst_tok0 + i *
+        chunk_size) up to the first chunk that is incomplete.  Returns the number of whole chunks served; with `stats`,
+        stats["bytes"] grows by the container bytes of those chunks.  CacheGen serde only; nothing is kept."""
+        if not (len(groups) and self._striped()):
+            return 0
+        return self._get_striped_groups(groups, [w for _, w in groups[0]], dst, dst_tok0, chunk_size, stats)
+
+    def _get_striped_groups(self, items, windows, dst, dst_tok0: int, chunk_size: int, stats=None) -> int:
+        """items: keys (windows None), or groups of (key, window) (see get_kv_shards_into)"""
         import contextlib
         from concurrent.futures import Future
 
         from lmcache_b200.pipeline import UploadRing, fetched_in_order, upload_decode, wave_chunks_default
         self._release.sweep()
-        bound = (self.deserializer.container_bound(dst.L, dst.H, dst.D, chunk_size) + 255) & ~255
+        H = dst.H if windows is None else windows[0].src_H
+        bound = (self.deserializer.container_bound(dst.L, H, dst.D, chunk_size) + 255) & ~255
         ex = self._executor()
+        keys = items if windows is None else LazyFlat(items, len(windows))
         peek, self._peek = self._peek, None
-        if peek is not None and not (keys and peek[0] == keys[0]):
+        if peek is not None and not (len(keys) and peek[0] == keys[0]):
             peek[1].blk.free()
             peek = None
 
@@ -297,7 +348,16 @@ class LMCRemoteBackend(LMCBackendInterface):
             self._upload = UploadRing(dst.device)
         window = max(2 * self._nconn, 2 * wave_chunks_default())       # fetches in flight ahead of the consumer
         with contextlib.closing(fetched_in_order(gets(), window)) as recs:
-            return upload_decode(self.deserializer.codec, self._upload, recs, dst, dst_tok0, chunk_size, self._release)
+            if windows is None:
+                return upload_decode(self.deserializer.codec, self._upload, recs, dst, dst_tok0, chunk_size,
+                                     self._release)
+            sizes: List[int] = []
+            with contextlib.closing(_grouped(recs, len(windows), sizes)) as grecs:
+                n = upload_decode(self.deserializer.codec, self._upload, grecs, dst, dst_tok0, chunk_size,
+                                  self._release, windows=windows)
+            if stats is not None:
+                stats["bytes"] = stats.get("bytes", 0) + sum(sizes[:n])
+            return n
 
     def close(self):
         if self.put_thread is not None and self.put_thread.is_alive():
