@@ -38,7 +38,11 @@ extern "C" {
                                     *    e.g. dlsym): b200kv_decode_plan / b200kv_decode_layers, b200kv_plane_offsets,
                                     *    b200kv_plane_offsets_device, b200kv_copy_batch_async,
                                     *    b200kv_encode_layers_workspace_bytes / b200kv_encode_layers_plan /
-                                    *    b200kv_encode_layers / b200kv_encode_layers_finish, b200kv_decode_plan_heads */
+                                    *    b200kv_encode_layers / b200kv_encode_layers_finish, b200kv_decode_plan_heads.
+                                    *    B200KV_MAX_PLANES went from 128 to 256 (models of up to 128 layers): the row
+                                    *    width of b200kv_plane_offsets_device, B200KV_MAX_PLANES + 1, and the size of
+                                    *    b200kv_encode_plan_t, 256 -> 512 words, changed with it; a caller takes them
+                                    *    from this header.  b200kv_decode_plan_t keeps its 256 words. */
 #define B200KV_CODER_AC 0          /* payload = torchac-lineage arithmetic coder; container version 1 */
 #define B200KV_CODER_RANS 1        /* payload = rANS, 32-bit state / 16-bit renormalisation; container version 2 */
 #define B200KV_CODER_RANS_COMPACT 2 /* rANS as in version 2, compact side information; container version 3 (chunks of
@@ -52,7 +56,7 @@ extern "C" {
                                                * 10+ KB).  Output bytes are identical either way. */
 #define B200KV_LP 33            /* CDF entries per stream (cachegen_encoder.py:287-289: int(bins.max()) + 1) */
 #define B200KV_GROUP_TOKENS 256 /* CACHEGEN_GPU_MAX_TOKENS_PER_CHUNK (cachegen_basics.py:13) */
-#define B200KV_MAX_PLANES 128   /* 2 * nlayers upper bound */
+#define B200KV_MAX_PLANES 256   /* 2 * nlayers upper bound: models of up to 128 layers */
 #define B200KV_DT_BF16 0
 #define B200KV_DT_FP16 1
 
@@ -126,8 +130,10 @@ int b200kv_container_layout_v(int32_t L, int32_t H, int32_t D, int32_t ntokens, 
  * anything that is not a version-3 container. */
 int b200kv_plane_offsets(const void* container, int64_t nbytes, int64_t* out, int32_t n_out);
 /* Same for n containers in DEVICE memory, container j at containers + j*stride (the encoder's output, before it leaves the
- * device): row j of out (DEVICE or mapped-host int64[n][B200KV_MAX_PLANES + 1]) gets the 2L + 1 offsets, or -1 in its
- * entry 0 for a container that is not version 3 or whose half-lengths do not add up.  Asynchronous on `stream`. */
+ * device): row j of out (DEVICE or mapped-host int64[n][B200KV_MAX_PLANES + 1]) gets the 2L + 1 offsets and zeros in the
+ * rest of the row, or -1 in its
+ * entry 0 for a container that is not version 3, whose header claims fixed sections longer than its total_bytes or than
+ * `stride` (nothing past the header is read then), or whose half-lengths do not add up.  Asynchronous on `stream`. */
 int b200kv_plane_offsets_device(const void* containers, int64_t stride, int32_t n, int64_t* out, void* stream);
 
 /* Bytes of device scratch b200kv_encode_chunks / b200kv_decode_chunks need for a call. */
@@ -206,7 +212,8 @@ int b200kv_decode_chunks(const void* containers, int64_t containers_bytes, const
  * delimit; containers of several groups (versions 1 / 2 with more than 256 tokens) spread a plane over every group.
  */
 typedef struct b200kv_decode_plan_t {
-    uint64_t opaque[256];
+    uint64_t opaque[256];      /* the decode kernel's parameter block; for more than 64 layers its plane table is kept in
+                                * the plan's workspace (b200kv_decode_workspace_bytes counts it) */
 } b200kv_decode_plan_t;
 
 int b200kv_decode_plan(const void* containers, int64_t containers_bytes, const int64_t* offsets,
@@ -266,7 +273,7 @@ int b200kv_decode_plan_heads(const void* containers, int64_t containers_bytes, c
  * outputs and the workspace must stay valid until the finish step has run on the device.
  */
 typedef struct b200kv_encode_plan_t {
-    uint64_t opaque[256];
+    uint64_t opaque[512];      /* holds the encode kernels' parameter block and a 128-bit set of the layers encoded */
 } b200kv_encode_plan_t;
 
 int64_t b200kv_encode_layers_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t chunk_tokens, int32_t n_chunks,

@@ -24,7 +24,7 @@ HDR_MAX = 36             # longest version-3 stream header (4 mask bytes + 31 co
 CODERS = {"ac": CODER_AC, "rans": CODER_RANS, "rans_compact": CODER_RANS_COMPACT}
 LP = 33
 GROUP_TOKENS = 256
-MAX_PLANES = 128
+MAX_PLANES = 256         # B200KV_MAX_PLANES: 2L for models of up to 128 layers
 MAGIC = 0x564B3242
 HEADER_BYTES = 64
 READ_SLACK = 640     # B200KV_READ_SLACK
@@ -73,7 +73,7 @@ class DecodePlan(ctypes.Structure):
 
 class EncodePlan(ctypes.Structure):
     """struct b200kv_encode_plan_t (opaque, filled by b200kv_encode_layers_plan)"""
-    _fields_ = [("opaque", ctypes.c_uint64 * 256)]
+    _fields_ = [("opaque", ctypes.c_uint64 * 512)]
 
 
 assert ctypes.sizeof(Header) == HEADER_BYTES

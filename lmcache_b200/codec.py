@@ -317,11 +317,17 @@ class CacheGenCodec:
     its buffers and is guarded by its own lock.
     """
 
-    def __init__(self, model_name: str, coder: Optional[str] = None):
+    def __init__(self, model_name: str, coder: Optional[str] = None, cachegen_config=None):
         """coder: "rans_compact" (container version 3, the default: rANS payload + symbol counts instead of CDF rows;
         chunks of more than 256 tokens fall back to version 2), "rans" (version 2) or "ac" (version 1, the
         torchac-lineage arithmetic coder); the environment variable LMCACHE_B200_CODER overrides the default.
-        Decoding accepts all three."""
+        Decoding accepts all three.
+
+        cachegen_config: the nine CacheGenConfig fields (LMCacheEngineConfig.cachegen_config), used instead of the bin
+        table for any model name.  Only version 3 records the bins a container was written with, so such a codec writes
+        and reads version 3 only: another coder is a ValueError here, chunks of more than 256 tokens one in coder_for,
+        and accepts() refuses versions 1 and 2 (their values would be dequantised with a step they were not written
+        with)."""
         import os
         from lmcache_b200.storage_backend.serde.cachegen_basics import CacheGenConfig
         N.require_cuda()
@@ -329,7 +335,11 @@ class CacheGenCodec:
         if name not in N.CODERS:
             raise ValueError(f"unknown coder {name!r} (expected one of {sorted(N.CODERS)})")
         self.coder = N.CODERS[name]
-        self.config = CacheGenConfig.from_model_name(model_name)
+        self.v3_only = cachegen_config is not None
+        if self.v3_only and self.coder != N.CODER_RANS_COMPACT:
+            raise ValueError(f"coder {name!r} writes containers that do not record their bins: with cachegen_config "
+                             f"only 'rans_compact' (container version 3) is possible")
+        self.config = CacheGenConfig.for_engine(model_name, cachegen_config)
         kb, vb = self.config.key_bins_list(), self.config.value_bins_list()
         self.nlayers = len(kb)
         self._kb = N.float_array(kb)
@@ -362,6 +372,9 @@ class CacheGenCodec:
     def coder_for(self, chunk_tokens: int) -> int:
         """The container this codec writes for chunks of `chunk_tokens`: the compact one holds <= 256 tokens."""
         if self.coder == N.CODER_RANS_COMPACT and chunk_tokens > N.GROUP_TOKENS:
+            if self.v3_only:
+                raise ValueError(f"chunks of {chunk_tokens} tokens: with cachegen_config the containers are version 3, "
+                                 f"which holds at most {N.GROUP_TOKENS} tokens")
             return N.CODER_RANS
         return self.coder
 
@@ -369,9 +382,10 @@ class CacheGenCodec:
         return N.container_layout(L, H, D, chunk_tokens, self.coder_for(chunk_tokens))
 
     def accepts(self, hd: "N.Header") -> bool:
-        """Can this codec decode the container?  A compact container must have been written with this model's bins."""
+        """Can this codec decode the container?  A compact container must have been written with this model's bins; a
+        codec made from a cachegen_config reads compact containers only (the others do not say which bins they used)."""
         if hd.version != 3:
-            return True
+            return not self.v3_only
         n = self.nlayers
         return hd.L <= n and hd.nb == self._nb[:hd.L] + self._nb[n:n + hd.L]
 
@@ -668,7 +682,8 @@ class CacheGenCodec:
             else:
                 hd = parse_header(c)
             if not self.accepts(hd):
-                raise ValueError("compact container written with another model's bins")
+                raise ValueError("compact container written with another model's bins" if hd.version == 3 else
+                                 f"a codec made from a cachegen_config reads version 3 only, not version {hd.version}")
             if (hd.L, hd.H, hd.D) != (dst.L, dst.H, dst.D):
                 raise ValueError(f"container shape L/H/D={hd.L}/{hd.H}/{hd.D} does not match destination "
                                  f"{dst.L}/{dst.H}/{dst.D}")
@@ -712,3 +727,14 @@ class CacheGenCodec:
                 o += (nb + 15) & ~15
             self.decode_raw(base_ptr, self._dec_in.numel(), offsets, totals, ntoks, dst, dst_tok, max_dtype, coder, tstream,
                             _locked=True)
+
+
+def engine_codec(config, model_name: str) -> CacheGenCodec:
+    """The codec of an engine's CacheGen tier or serde: the bins of config.cachegen_config when it is set (then the
+    containers are version 3, so chunk_size must be <= 256: a ValueError here, when the tier or serde is made, not at
+    the first store), the model's row of the bin table otherwise (ValueError for a name outside it)."""
+    cg = config.cachegen_config
+    if cg is not None and config.chunk_size > N.GROUP_TOKENS:
+        raise ValueError(f"chunk_size {config.chunk_size}: with cachegen_config the containers are version 3, which "
+                         f"holds at most {N.GROUP_TOKENS} tokens")
+    return CacheGenCodec(model_name, cachegen_config=cg)

@@ -4,7 +4,7 @@ from __future__ import annotations
 
 import re
 from dataclasses import dataclass
-from typing import List, Optional
+from typing import Dict, List, Optional
 
 import yaml
 
@@ -45,6 +45,11 @@ class LMCacheEngineConfig:
     # KV heads once its own layout's prefix ends (lmcache_b200/reshard.py), tried in this order.  None = off.  Needs a
     # remote tier with the CacheGen serde (CreateStorageBackend); must not hold the engine's own world size (LMCacheEngine).
     reshard_world_sizes: Optional[List[int]] = None
+    # not in the reference as a key (it is the reference's nine-field CacheGenConfig): the CacheGen bin layout of a model
+    # outside the five-name table of CacheGenConfig.from_model_name, e.g. a 70B model's 80 layers.  A mapping of exactly
+    # the nine fields; None = the table.  When set, the engine's CacheGen tiers and serdes use it for any model name, and
+    # write and read version-3 containers only -- the one version that records the bins (chunk_size <= 256).
+    cachegen_config: Optional[Dict[str, int]] = None
 
     def __post_init__(self):
         if self.local_serde is None:
@@ -64,6 +69,8 @@ class LMCacheEngineConfig:
             raise ValueError(f"Invalid reshard world sizes: {r!r} (a non-empty list of distinct positive ints, or None)")
         if r is not None:
             self.reshard_world_sizes = list(r)
+        if self.cachegen_config is not None:
+            self.cachegen_config = check_cachegen_config(self.cachegen_config)
 
     @staticmethod
     def from_defaults(chunk_size: int = 256, local_device: str = "cuda",
@@ -72,10 +79,11 @@ class LMCacheEngineConfig:
                       local_serde: Optional[str] = None,
                       local_capacity_bytes: Optional[int] = None,
                       device_cache_bytes: Optional[int] = None,
-                      reshard_world_sizes: Optional[List[int]] = None) -> "LMCacheEngineConfig":
+                      reshard_world_sizes: Optional[List[int]] = None,
+                      cachegen_config: Optional[Dict[str, int]] = None) -> "LMCacheEngineConfig":
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
                                    save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes,
-                                   reshard_world_sizes)
+                                   reshard_world_sizes, cachegen_config)
 
     @staticmethod
     def from_legacy(chunk_size: int = 256, backend: str = "cuda", persist_path: Optional[str] = None,
@@ -83,7 +91,8 @@ class LMCacheEngineConfig:
                     save_decode_cache: bool = False, local_serde: Optional[str] = None,
                     local_capacity_bytes: Optional[int] = None,
                     device_cache_bytes: Optional[int] = None,
-                    reshard_world_sizes: Optional[List[int]] = None) -> "LMCacheEngineConfig":
+                    reshard_world_sizes: Optional[List[int]] = None,
+                    cachegen_config: Optional[Dict[str, int]] = None) -> "LMCacheEngineConfig":
         """backend: "cpu" | "cuda" | "file://<dir>/" | "<scheme>://<host>:<port>" (config.py:51-82)."""
         local_device: Optional[str] = None
         remote_url: Optional[str] = None
@@ -95,7 +104,7 @@ class LMCacheEngineConfig:
             remote_url = backend
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
                                    save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes,
-                                   reshard_world_sizes)
+                                   reshard_world_sizes, cachegen_config)
 
     @staticmethod
     def from_file(file_path: str) -> "LMCacheEngineConfig":
@@ -112,6 +121,7 @@ class LMCacheEngineConfig:
         local_capacity_bytes = cfg.get("local_capacity_bytes", None)
         device_cache_bytes = cfg.get("device_cache_bytes", None)
         reshard_world_sizes = cfg.get("reshard_world_sizes", None)
+        cachegen_config = cfg.get("cachegen_config", None)
 
         if local_device in ("cpu", "cuda", None):
             pass
@@ -125,7 +135,46 @@ class LMCacheEngineConfig:
 
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
                                    save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes,
-                                   reshard_world_sizes)
+                                   reshard_world_sizes, cachegen_config)
+
+
+CACHEGEN_CONFIG_FIELDS = ("key_first_layers", "key_second_layers", "key_third_layers", "key_first_bins",
+                          "key_second_bins", "key_third_bins", "value_first_layers", "value_first_bins",
+                          "value_second_bins")
+MAX_LAYERS = 128        # B200KV_MAX_PLANES / 2
+MIN_BINS, MAX_BINS = 4, 32      # the quantiser range of the kernels: bins // 2 - 1 in [1, 15]
+
+
+def check_cachegen_config(c) -> Dict[str, int]:
+    """The nine CacheGenConfig fields of `c` (a mapping, or a CacheGenConfig) as a plain dict, or ValueError.
+    key_third_layers is the model's layer count (1..128); every bin count that some layer gets lies in [4, 32].
+    Layer i's key bins are key_first_bins for i < key_first_layers, else key_second_bins for i < key_second_layers,
+    else key_third_bins; its value bins value_first_bins for i < value_first_layers, else value_second_bins
+    (make_key_bins / make_value_bins of the reference)."""
+    import dataclasses
+    from collections.abc import Mapping
+    if dataclasses.is_dataclass(c) and not isinstance(c, type):
+        c = dataclasses.asdict(c)
+    if not isinstance(c, Mapping) or set(c) != set(CACHEGEN_CONFIG_FIELDS):
+        raise ValueError(f"Invalid cachegen_config: {c!r} (a mapping of exactly the fields {', '.join(CACHEGEN_CONFIG_FIELDS)})")
+    for k in CACHEGEN_CONFIG_FIELDS:
+        if isinstance(c[k], bool) or not isinstance(c[k], int):
+            raise ValueError(f"Invalid cachegen_config: {k} = {c[k]!r} is not an int")
+    c = {k: int(c[k]) for k in CACHEGEN_CONFIG_FIELDS}
+    L = c["key_third_layers"]
+    if not 1 <= L <= MAX_LAYERS:
+        raise ValueError(f"Invalid cachegen_config: key_third_layers = {L} (the layer count, 1..{MAX_LAYERS})")
+    for k in ("key_first_layers", "key_second_layers", "value_first_layers"):
+        if c[k] < 0:
+            raise ValueError(f"Invalid cachegen_config: {k} = {c[k]} is negative")
+    k1, k2 = min(c["key_first_layers"], L), min(c["key_second_layers"], L)
+    v1 = min(c["value_first_layers"], L)
+    applies = {"key_first_bins": k1 > 0, "key_second_bins": k2 > k1, "key_third_bins": L > max(k1, k2),
+               "value_first_bins": v1 > 0, "value_second_bins": L > v1}
+    for k, used in applies.items():
+        if used and not MIN_BINS <= c[k] <= MAX_BINS:
+            raise ValueError(f"Invalid cachegen_config: {k} = {c[k]} (bins must lie in [{MIN_BINS}, {MAX_BINS}])")
+    return c
 
 
 class GlobalConfig:

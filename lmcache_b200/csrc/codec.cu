@@ -76,6 +76,7 @@ struct EncParams {
     int64_t* seg;                    // [n_chunks][2L][2] (arena offset, bytes) per plane; mapped host memory
     int32_t layers_left;             // layers not yet encoded after this call (arena reserve, place_kernel)
 };
+static_assert(sizeof(EncParams) < kMaxParamBytes, "EncParams must stay under 4 KB of kernel parameters");
 
 // plane of the launch's local plane index: K planes lb.., then V planes L + lb.. (the identity when lb = 0, nlay = L)
 __device__ __forceinline__ int launch_plane(const EncParams& P, int local) {
@@ -997,8 +998,13 @@ struct DecChunk {
     int32_t ct0, ntw, cw0, cw1, dshift;
 };
 
+// The decode's parameter block lives in the caller's b200kv_decode_plan_t (256 words), so it carries the destination's
+// plane table inline only up to kInlinePlanes planes (L <= 64).  A deeper model's full table goes to the plan's
+// workspace and the kernel reads it from there (decode_kernel<..., GT = true>): one uniform load per CTA, per plane.
+constexpr int kInlinePlanes = 128;
 struct DecParams {
-    PlaneTable pt;               // destination planes; maxq = C_l = bins // 2 - 1
+    PlaneTableT<kInlinePlanes> pt;   // destination planes; maxq = C_l = bins // 2 - 1 (2L <= kInlinePlanes)
+    const PlaneTable* gpt;           // device copy of the whole table when 2L > kInlinePlanes; NULL otherwise
     int64_t sT, sH;
     const int64_t* slot_map;     // paged destination: token i lives in row slot_map[i]; NULL = row i
     int32_t L, H, D, C, out_dtype, max_dtype, n_chunks, tpp, tiles_max;   // H, C: the containers' (src_H with windows)
@@ -1010,6 +1016,19 @@ struct DecParams {
     uint32_t* status;            // [n_chunks] or NULL: bit 0 = a rANS stream did not return to its initial state,
                                  //   bit 1 = stream offsets beyond the payload (corrupt lengths section)
 };
+static_assert(sizeof(DecParams) < kMaxParamBytes, "DecParams must stay under 4 KB of kernel parameters");
+
+// plane nl's destination pointer and quantiser constant: inline (GT = false) or from the device copy (GT = true)
+template <bool GT>
+__device__ __forceinline__ const uint16_t* dec_plane(const DecParams& P, int nl) {
+    if constexpr (GT) return P.gpt->p[nl];
+    else return P.pt.p[nl];
+}
+template <bool GT>
+__device__ __forceinline__ float dec_maxq(const DecParams& P, int nl) {
+    if constexpr (GT) return P.gpt->maxq[nl];
+    else return P.pt.maxq[nl];
+}
 
 // tile sums of the stream lengths: one warp per tile
 __global__ void __launch_bounds__(128) tile_sum_kernel(DecParams P) {
@@ -1078,16 +1097,24 @@ __global__ void __launch_bounds__(1024) plane_offsets_kernel(const uint8_t* base
     const uint32_t* hw = reinterpret_cast<const uint32_t*>(c);
     const uint32_t version = hw[1], L = hw[2], H = hw[3], D = hw[4], t = hw[5];
     const uint64_t total = *reinterpret_cast<const uint64_t*>(c + 40);
+    // the header alone decides whether the fixed sections lie inside the container and inside this row: nothing past the
+    // header is read before that is known (the lengths section alone is 2L * C bytes, so C <= stride bounds the layout)
+    const uint64_t C64 = (uint64_t)H * D;
     if (hw[0] != B200KV_MAGIC || version != 3u || L == 0u || 2u * L > (uint32_t)B200KV_MAX_PLANES || H == 0u || D == 0u ||
-        t == 0u || t > (uint32_t)kGroup) {
+        t == 0u || t > (uint32_t)kGroup || C64 > (uint64_t)stride || C64 >= (1ull << 31)) {
         if (threadIdx.x == 0) o[0] = -1;
         return;
     }
     const int NL = 2 * (int)L;
-    const int64_t C = (int64_t)H * D;
+    const int64_t C = (int64_t)C64;
     const Layout lo = make_layout((int)L, (int)C, (int)t, 1);
+    if ((uint64_t)lo.off_payload > total || lo.off_payload > stride) {
+        if (threadIdx.x == 0) o[0] = -1;
+        return;
+    }
     const uint8_t* half = c + lo.off_lengths;                  // 16-byte aligned (container and section)
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int p = NL + 1 + (int)threadIdx.x; p <= B200KV_MAX_PLANES; p += blockDim.x) o[p] = 0;   // the row past 2L + 1
     for (int p = warp; p < NL; p += blockDim.x >> 5) {
         const uint8_t* row = half + p * C;
         uint32_t sum = 0;
@@ -1327,7 +1354,7 @@ __device__ __forceinline__ uint32_t rans_decode_stream(const uint8_t* cont, uint
 // dequantisation LUT live in shared memory (~18 KB per CTA), so many CTAs stay resident and hide the serial latency of
 // each stream's coder.  Symbols are dequantised and stored straight into the destination layout (no uint8 / fp32
 // intermediates in HBM).  CODER selects the payload format (container version 1: arithmetic coder, 2: rANS).
-template <int OUT_DT, bool PAGED, int CODER, bool TR>
+template <int OUT_DT, bool PAGED, int CODER, bool TR, bool GT>
 __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
     extern __shared__ __align__(128) uint32_t smem[];
     uint32_t* tab = smem;                                                            // CT * 33 words (rows of 33, odd)
@@ -1373,7 +1400,7 @@ __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
     // stage the per-stream tables (one contiguous run of ncols * 33 halfwords in the container), row maxima, LUT
     const uint16_t* cdf_src = reinterpret_cast<const uint16_t*>(dc.base + lo.off_cdf) + ((int64_t)nl * P.C + ct * CT) * kLp;
     const uint16_t* maxes = reinterpret_cast<const uint16_t*>(dc.base + lo.off_maxes) + (int64_t)nl * dc.t + tok0;
-    const float cq = P.pt.maxq[nl];
+    const float cq = dec_maxq<GT>(P, nl);
     bool built = false;
     uint32_t hl = 0u;                        // version 3: bytes of stream header in front of the rANS state
     if constexpr (CODER == CODER_RANS) {
@@ -1538,7 +1565,7 @@ __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
     const uint32_t* erow = tab + tid * kLp;
     const int oc = c + dc.dshift;                          // destination channel
     const int h = oc / P.D;
-    uint16_t* dst = const_cast<uint16_t*>(P.pt.p[nl]) + (PAGED ? 0 : (dc.dst_tok + tok0) * P.sT) + (int64_t)h * P.sH +
+    uint16_t* dst = const_cast<uint16_t*>(dec_plane<GT>(P, nl)) + (PAGED ? 0 : (dc.dst_tok + tok0) * P.sT) + (int64_t)h * P.sH +
                     (oc - h * P.D);
     const int64_t* slots = PAGED ? P.slot_map + dc.dst_tok + tok0 : nullptr;
     uint32_t bad = beyond ? 2u : 0u;
@@ -1643,10 +1670,43 @@ static EnclWs encl_ws_layout(int n_chunks, int64_t call_tiles) {
 // What b200kv_encode_layers_plan decided, kept in the caller's b200kv_encode_plan_t: the kernels' parameter block (its
 // counters live in the workspace), the layers encoded so far and the most one call may take.
 constexpr uint32_t kEncPlanMagic = 0x4e4c5045u;   // "EPLN"
+// a set of layers [0, B200KV_MAX_PLANES / 2): bit l % 64 of word l / 64
+struct LayerSet {
+    static constexpr int kWords = B200KV_MAX_PLANES / 2 / 64;
+    uint64_t w[kWords];
+    // layers [a, b), 0 <= a <= b <= kWords * 64
+    static LayerSet range(int a, int b) {
+        LayerSet s;
+        for (int i = 0; i < kWords; ++i) {
+            const int lo = std::max(a - 64 * i, 0), hi = std::min(b - 64 * i, 64);   // the range inside word i
+            s.w[i] = lo >= hi ? 0ull : (hi - lo == 64 ? ~0ull : ((1ull << (hi - lo)) - 1ull) << lo);
+        }
+        return s;
+    }
+    bool intersects(const LayerSet& o) const {
+        uint64_t x = 0ull;
+        for (int i = 0; i < kWords; ++i) x |= w[i] & o.w[i];
+        return x != 0ull;
+    }
+    bool operator==(const LayerSet& o) const {
+        for (int i = 0; i < kWords; ++i)
+            if (w[i] != o.w[i]) return false;
+        return true;
+    }
+    void add(const LayerSet& o) {
+        for (int i = 0; i < kWords; ++i) w[i] |= o.w[i];
+    }
+    int count() const {
+        int n = 0;
+        for (int i = 0; i < kWords; ++i) n += __builtin_popcountll(w[i]);
+        return n;
+    }
+};
+static_assert(LayerSet::kWords * 64 == B200KV_MAX_PLANES / 2, "one bit per layer");
 struct EncPlan {
     uint32_t magic;
     int32_t max_layers;
-    uint64_t done;           // bit l: layer l has been encoded
+    LayerSet done;           // the layers encoded so far
     EncParams P;
 };
 static_assert(sizeof(EncPlan) <= sizeof(b200kv_encode_plan_t), "b200kv_encode_plan_t too small");
@@ -1670,11 +1730,15 @@ static int launch_absmax(const EncParams& P, const b200kv_kv_desc* kv, int64_t t
     return 0;
 }
 
-static size_t dec_ws_layout(int64_t tiles_max, int n_chunks, size_t* off_tb) {
+// chunk descriptors, tile bases, and -- for more than kInlinePlanes planes only -- the device copy of the plane table
+static size_t dec_ws_layout(int64_t tiles_max, int n_chunks, int L, size_t* off_tb, size_t* off_pt) {
     size_t o = ((size_t)n_chunks * sizeof(DecChunk) + 255) & ~(size_t)255;
     *off_tb = o;
     o += (size_t)n_chunks * (size_t)tiles_max * 8;
-    return (o + 255) & ~(size_t)255;
+    o = (o + 255) & ~(size_t)255;
+    *off_pt = o;
+    if (2 * L > kInlinePlanes) o = (o + sizeof(PlaneTable) + 255) & ~(size_t)255;
+    return o;
 }
 
 // What b200kv_decode_plan decided, kept in the caller's b200kv_decode_plan_t: the decode kernel's parameter block (its
@@ -1769,8 +1833,8 @@ int64_t b200kv_decode_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t c
     if (L <= 0 || H <= 0 || D <= 0 || chunk_tokens <= 0 || n_chunks <= 0) return -2;
     const int64_t G = (chunk_tokens + kGroup - 1) / kGroup;
     const int64_t tiles_max = G * 2 * L * tiles_per_plane(H * D);
-    size_t a;
-    return (int64_t)dec_ws_layout(tiles_max, n_chunks, &a);
+    size_t a, b;
+    return (int64_t)dec_ws_layout(tiles_max, n_chunks, L, &a, &b);
 }
 
 int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
@@ -1966,7 +2030,7 @@ int b200kv_encode_layers_plan(const b200kv_kv_desc* kv, int64_t tok_begin, int32
     B2_CHECK_CUDA(cudaGetLastError());
     B2_CHECK_CUDA(cudaFuncSetAttribute(compact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, P.stage_bytes));
     plan->max_layers = max_layers;
-    plan->done = 0ull;
+    plan->done = LayerSet::range(0, 0);
     plan->magic = kEncPlanMagic;
     return 0;
 }
@@ -1979,11 +2043,11 @@ int b200kv_encode_layers(b200kv_encode_plan_t* plan_in, int32_t layer_begin, int
     EncParams P = plan->P;
     B2_REQUIRE(layer_begin >= 0 && layer_begin < layer_end && layer_end <= P.L, "layer range out of range");
     B2_REQUIRE(layer_end - layer_begin <= plan->max_layers, "more layers than the plan's workspace holds");
-    const uint64_t bits = (layer_end - layer_begin == 64 ? ~0ull : ((1ull << (layer_end - layer_begin)) - 1ull)) << layer_begin;
-    B2_REQUIRE((plan->done & bits) == 0ull, "a layer of the range was encoded before");
+    const LayerSet bits = LayerSet::range(layer_begin, layer_end);
+    B2_REQUIRE(!plan->done.intersects(bits), "a layer of the range was encoded before");
     P.lb = layer_begin;
     P.nlay = layer_end - layer_begin;
-    P.layers_left = P.L - __builtin_popcountll(plan->done | bits);
+    P.layers_left = P.L - plan->done.count() - bits.count();
     P.tiles_full = 2 * P.nlay * P.tpp;
     const int64_t n_tiles = (int64_t)P.n_chunks * P.tiles_full;
     const int64_t total_tokens = (int64_t)(P.n_chunks - 1) * P.chunk_tokens + P.last_chunk_tokens;
@@ -2004,7 +2068,7 @@ int b200kv_encode_layers(b200kv_encode_plan_t* plan_in, int32_t layer_begin, int
     place_kernel<<<1, 1024, 0, stream>>>(P);
     compact_kernel<<<(unsigned)n_tiles, CT, (size_t)P.stage_bytes, stream>>>(P);
     B2_CHECK_CUDA(cudaGetLastError());
-    plan->done |= bits;
+    plan->done.add(bits);
     return 0;
 }
 
@@ -2014,8 +2078,7 @@ int b200kv_encode_layers_finish(const b200kv_encode_plan_t* plan_in, void* strea
     const EncPlan* plan = reinterpret_cast<const EncPlan*>(plan_in);
     B2_REQUIRE(plan->magic == kEncPlanMagic, "not a plan made by b200kv_encode_layers_plan");
     EncParams P = plan->P;
-    const uint64_t all = P.L == 64 ? ~0ull : (1ull << P.L) - 1ull;
-    B2_REQUIRE(plan->done == all, "a layer was never encoded");
+    B2_REQUIRE(plan->done == LayerSet::range(0, P.L), "a layer was never encoded");
     P.totals = P.ptotal;                   // headers carry the payload of every call
     finalize_kernel<<<(P.n_chunks + 127) / 128, 128, 0, stream>>>(P);
     B2_CHECK_CUDA(cudaGetLastError());
@@ -2037,7 +2100,13 @@ static int decode_plan_impl(const void* containers, int64_t containers_bytes, co
     B2_REQUIRE(coder >= CODER_AC && coder <= CODER_RANS_COMPACT, "coder must be one of B200KV_CODER_*");
     P.compact = coder == CODER_RANS_COMPACT ? 1 : 0;
     if (P.compact) coder = CODER_RANS;
-    if (int rc = make_plane_table(dst, key_bins, value_bins, &P.pt)) return rc;
+    PlaneTable full;
+    if (int rc = make_plane_table(dst, key_bins, value_bins, &full)) return rc;
+    for (int nl = 0; nl < std::min(2 * dst->L, kInlinePlanes); ++nl) {
+        P.pt.p[nl] = full.p[nl];
+        P.pt.maxq[nl] = full.maxq[nl];
+    }
+    P.gpt = nullptr;                         // set below, once every check has passed, when 2L > kInlinePlanes
     B2_REQUIRE(containers && offsets && total_bytes && ntokens && dst_tok && n_chunks > 0, "bad chunk arrays");
     B2_REQUIRE(max_dtype == B200KV_DT_BF16 || max_dtype == B200KV_DT_FP16, "bad max_dtype");
     B2_REQUIRE(dst->sT > 0 && dst->sT < (1ll << 23), "destination token stride out of range");
@@ -2110,10 +2179,14 @@ static int decode_plan_impl(const void* containers, int64_t containers_bytes, co
         if (const char* e = getenv("B200KV_DECODE_TABLE")) transposed = e[0] == 't';
     }
     P.tiles_max = (int32_t)tiles_max;
-    size_t off_tb;
-    const size_t need = dec_ws_layout(tiles_max, n_chunks, &off_tb);
+    size_t off_tb, off_pt;
+    const size_t need = dec_ws_layout(tiles_max, n_chunks, P.L, &off_tb, &off_pt);
     B2_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)need, "workspace too small");
     uint8_t* ws = static_cast<uint8_t*>(workspace);
+    if (2 * P.L > kInlinePlanes) {           // the whole table, staged from pageable memory before the call returns
+        B2_CHECK_CUDA(cudaMemcpyAsync(ws + off_pt, &full, sizeof(PlaneTable), cudaMemcpyHostToDevice, stream));
+        P.gpt = reinterpret_cast<const PlaneTable*>(ws + off_pt);
+    }
     // chunk descriptors: small pageable -> device copy (staged by the driver before the call returns)
     {
         DecChunk* hc = static_cast<DecChunk*>(malloc(sizeof(DecChunk) * (size_t)n_chunks));
@@ -2195,11 +2268,16 @@ int b200kv_decode_layers(const b200kv_decode_plan_t* plan_in, int32_t layer_begi
     const size_t smem = (size_t)(CT * kLp + kGroup + 32) * 4;
     dim3 grid((unsigned)((int64_t)plan->gmax * 2 * P.nlay * P.wtpp), (unsigned)P.n_chunks);
     ProfScope prof(kProfDecode, stream);
+#define B2_LAUNCH_DEC2(DT, PAGED, CODER, TR, GT)                                                                       \
+    do {                                                                                                               \
+        B2_CHECK_CUDA(cudaFuncSetAttribute(decode_kernel<DT, PAGED, CODER, TR, GT>,                                    \
+                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                   \
+        decode_kernel<DT, PAGED, CODER, TR, GT><<<grid, CT, smem, stream>>>(P);                                        \
+    } while (0)
 #define B2_LAUNCH_DEC1(DT, PAGED, CODER, TR)                                                                           \
     do {                                                                                                               \
-        B2_CHECK_CUDA(cudaFuncSetAttribute(decode_kernel<DT, PAGED, CODER, TR>,                                        \
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                   \
-        decode_kernel<DT, PAGED, CODER, TR><<<grid, CT, smem, stream>>>(P);                                            \
+        if (P.gpt != nullptr) B2_LAUNCH_DEC2(DT, PAGED, CODER, TR, true);                                              \
+        else B2_LAUNCH_DEC2(DT, PAGED, CODER, TR, false);                                                              \
     } while (0)
 #define B2_LAUNCH_DEC(DT, PAGED)                                                                                       \
     do {                                                                                                               \
@@ -2211,6 +2289,7 @@ int b200kv_decode_layers(const b200kv_decode_plan_t* plan_in, int32_t layer_begi
     else { if (P.slot_map) B2_LAUNCH_DEC(1, true); else B2_LAUNCH_DEC(1, false); }
 #undef B2_LAUNCH_DEC
 #undef B2_LAUNCH_DEC1
+#undef B2_LAUNCH_DEC2
     B2_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -30,11 +30,15 @@ void set_error(const std::string& msg);   // thread-local last error (api.cu)
     } while (0)
 
 // Kernel-parameter copy of the per-plane base pointers and quantiser constants
-// (plane nl = kv * L + l).  Lives in the constant bank; indexed dynamically.
-struct PlaneTable {
-    const uint16_t* p[B200KV_MAX_PLANES];
-    float maxq[B200KV_MAX_PLANES];       // bins // 2 - 1
+// (plane nl = kv * L + l).  Lives in the constant bank; indexed dynamically.  3 KB at 256 planes: every parameter block
+// that holds one stays under the classic 4 KB kernel-parameter limit (static_asserts next to each).
+template <int N>
+struct PlaneTableT {
+    const uint16_t* p[N];
+    float maxq[N];                       // bins // 2 - 1
 };
+using PlaneTable = PlaneTableT<B200KV_MAX_PLANES>;
+constexpr size_t kMaxParamBytes = 4096;
 
 // Fill a PlaneTable from a kv_desc + bins; returns 0 or <0 with error set.
 int make_plane_table(const b200kv_kv_desc* kv, const float* key_bins, const float* value_bins, PlaneTable* out);

@@ -28,6 +28,7 @@ struct PackParams {
     uint8_t* chunks;
     int64_t chunk_stride_bytes;
 };
+static_assert(sizeof(PackParams) < kMaxParamBytes, "PackParams must stay under 4 KB of kernel parameters");
 
 // One grid-stride loop over (chunk, plane, token, vector) units; VEC halfs per unit.
 // vllm chunk layout [L,2,t,H,D]; huggingface [L,2,H,t,D].

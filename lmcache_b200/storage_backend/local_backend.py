@@ -346,7 +346,7 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
 
     def __init__(self, config: LMCacheEngineConfig, metadata):
         super().__init__()
-        from lmcache_b200.codec import CacheGenCodec
+        from lmcache_b200.codec import engine_codec
         from lmcache_b200.eviction import PrefixLRU
         from lmcache_b200.pipeline import DeferredFree, EncodePipeline, UploadRing
         N.require_cuda()
@@ -354,7 +354,9 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         self.fmt = metadata.fmt
         if self.fmt not in ("vllm", "huggingface"):
             raise ValueError(f"Invalid format: {self.fmt}")
-        self.codec = CacheGenCodec(metadata.model_name)      # ValueError for models outside the bin table
+        # ValueError for models outside the bin table (without config.cachegen_config), and for settings that
+        # config.cachegen_config rules out
+        self.codec = engine_codec(config, metadata.model_name)
         self.capacity: Optional[int] = config.local_capacity_bytes
         self.slab = self._new_slab()
         self._order = PrefixLRU()             # eviction order of a bounded tier, keyed like self.dict

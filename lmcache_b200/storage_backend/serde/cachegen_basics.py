@@ -1,7 +1,8 @@
 """CacheGen configuration and wire-container views.
 
 Mirrors lmcache/storage_backend/serde/cachegen_basics.py:
-  * CACHEGEN_GPU_MAX_TOKENS_PER_CHUNK (:13), CacheGenConfig.from_model_name (:16-78): identical bin table.
+  * CACHEGEN_GPU_MAX_TOKENS_PER_CHUNK (:13), CacheGenConfig.from_model_name (:16-78): identical bin table;
+    CacheGenConfig.for_engine also takes an operator-supplied layout (LMCacheEngineConfig.cachegen_config).
   * CacheGenGPUBytestream / CacheGenGPUEncoderOutput (:109-142): same field names, but `to_bytes` /
     `from_bytes` speak the flat "B2KV" container (include/b200kv.h) that the encode kernel writes on the
     device, instead of pickling CUDA tensors.  `from_bytes` gives the same object a reference consumer
@@ -52,6 +53,15 @@ class CacheGenConfig:
             key_first_layers=10, key_second_layers=20, key_third_layers=_FAMILY_LAYERS[model_name],
             key_first_bins=32, key_second_bins=16, key_third_bins=16,
             value_first_layers=2, value_first_bins=32, value_second_bins=16)
+
+    @staticmethod
+    def for_engine(model_name: str, cachegen_config=None) -> "CacheGenConfig":
+        """The layout an engine uses: `cachegen_config` (LMCacheEngineConfig.cachegen_config: the nine fields, checked
+        by config.check_cachegen_config) for any model name when it is given, the table of from_model_name otherwise."""
+        if cachegen_config is None:
+            return CacheGenConfig.from_model_name(model_name)
+        from lmcache_b200.config import check_cachegen_config
+        return CacheGenConfig(**check_cachegen_config(cachegen_config))
 
     def key_bins_list(self) -> List[float]:
         """make_key_bins (cachegen_encoder.py:339-344): per-layer fp32 bin counts."""

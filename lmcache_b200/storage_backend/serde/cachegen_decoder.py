@@ -7,7 +7,7 @@ from typing import List, Optional, Sequence
 
 import torch
 
-from lmcache_b200.codec import CacheGenCodec, KvView, parse_header
+from lmcache_b200.codec import KvView, engine_codec, parse_header
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.storage_backend.serde.cachegen_basics import CacheGenConfig
 from lmcache_b200.storage_backend.serde.serde import Deserializer
@@ -17,12 +17,12 @@ from lmcache_b200.utils import _lmcache_nvtx_annotate
 class CacheGenDeserializer(Deserializer):
 
     def __init__(self, config: LMCacheEngineConfig, metadata: LMCacheEngineMetadata):
-        self.cachegen_config = CacheGenConfig.from_model_name(metadata.model_name)
+        self.cachegen_config = CacheGenConfig.for_engine(metadata.model_name, config.cachegen_config)
         self.chunk_size = config.chunk_size
         self.fmt = metadata.fmt
         if self.fmt not in ("vllm", "huggingface"):
             raise RuntimeError("Unknown format %s" % self.fmt)
-        self.codec = CacheGenCodec(metadata.model_name)
+        self.codec = engine_codec(config, metadata.model_name)
 
     def _out_dtype(self) -> torch.dtype:
         # reference casts by format, ignoring metadata.dtype (cachegen_decoder.py:189-200)

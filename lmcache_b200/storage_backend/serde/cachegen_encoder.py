@@ -8,7 +8,7 @@ from typing import List, Optional, Sequence
 
 import torch
 
-from lmcache_b200.codec import CacheGenCodec, KvView
+from lmcache_b200.codec import KvView, engine_codec
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.storage_backend.serde.cachegen_basics import CacheGenConfig
 from lmcache_b200.storage_backend.serde.serde import Serializer
@@ -18,11 +18,12 @@ from lmcache_b200.utils import _lmcache_nvtx_annotate
 class CacheGenSerializer(Serializer):
 
     def __init__(self, config: LMCacheEngineConfig, metadata: LMCacheEngineMetadata):
-        # ValueError for models outside the bin table, like the reference (cachegen_basics.py:77-78)
-        self.cachegen_config = CacheGenConfig.from_model_name(metadata.model_name)
+        # ValueError for models outside the bin table, like the reference (cachegen_basics.py:77-78), unless
+        # config.cachegen_config gives the layout
+        self.cachegen_config = CacheGenConfig.for_engine(metadata.model_name, config.cachegen_config)
         self.chunk_size = config.chunk_size
         self.fmt = metadata.fmt
-        self.codec = CacheGenCodec(metadata.model_name)
+        self.codec = engine_codec(config, metadata.model_name)
         self.key_bins = torch.tensor(self.cachegen_config.key_bins_list())
         self.value_bins = torch.tensor(self.cachegen_config.value_bins_list())
 
