@@ -264,14 +264,9 @@ class LMCacheEngine:
                               chunk_hash)
 
     def _num_tokens_in_kv(self, kv_tensors: Union[KVCache, torch.Tensor], fmt: str) -> int:
-        if fmt == "huggingface":
-            return kv_tensors[0][0].shape[1]
-        elif fmt == "vllm":
-            return kv_tensors[0][0].shape[0]
-        raise ValueError(f"Invalid format: {fmt}")
-
-    def _get_init_hash(self) -> str:
-        return ""
+        if fmt not in ("vllm", "huggingface"):
+            raise ValueError(f"Invalid format: {fmt}")
+        return kv_tensors[0][0].shape[KvView.token_dim(fmt) - 2]         # a layer's K is a blob without its [L, 2] dims
 
     def _prefix_hash(self, tokens: torch.Tensor, num_skip_chunk: Optional[int] = 0):
         """All chunk digests of `tokens` (the whole chain is hashed, then the first num_skip_chunk digests are
@@ -282,37 +277,12 @@ class LMCacheEngine:
         return LazySeq(lambda h: self._make_key(h, fmt), chunk_hashes)
 
     # ------------------------------------------------------------------ blob helpers
-    def _chunk_shape(self, view: KvView, t: int, fmt: str) -> Tuple[int, ...]:
-        return (view.L, 2, t, view.H, view.D) if fmt == "vllm" else (view.L, 2, view.H, t, view.D)
-
-    def _pack_chunks(self, view: KvView, tok_begin: int, fmt: str) -> List[torch.Tensor]:
-        """Gather tokens [tok_begin, T) of the kv tuple into contiguous per-chunk blobs with one kernel."""
-        n_tok = view.ntokens - tok_begin
-        if n_tok <= 0:
-            return []
-        cs = self.chunk_size
-        n_chunks = (n_tok + cs - 1) // cs
-        last = n_tok - (n_chunks - 1) * cs
-        per_tok = 2 * view.L * view.H * view.D          # halfs per token over all planes
-        stride_elems = per_tok * cs
-        buf = torch.empty(n_chunks * stride_elems, dtype=view.dtype, device=view.device)
-        with torch.cuda.device(view.device):
-            N.check(N.lib().b200kv_pack_chunks(ctypes.byref(view.desc), tok_begin, n_chunks, cs, last,
-                                               1 if fmt == "huggingface" else 0, ctypes.c_void_p(buf.data_ptr()),
-                                               stride_elems * buf.element_size(),
-                                               torch.cuda.current_stream().cuda_stream), "pack_chunks")
-        chunks = []
-        for j in range(n_chunks):
-            t = cs if j < n_chunks - 1 else last
-            chunks.append(buf[j * stride_elems: j * stride_elems + per_tok * t].view(self._chunk_shape(view, t, fmt)))
-        return chunks
-
     def _pack_chunks_torch(self, kv: KVCache, tok_begin: int, fmt: str) -> List[torch.Tensor]:
         """_tuple_kv_to_blob + _slice_kv_at with torch ops (cache_engine.py:98-161), for dtypes the kernels do not move"""
         k = torch.stack([x[0] for x in kv])
         v = torch.stack([x[1] for x in kv])
         blob = torch.stack((k, v)).permute(1, 0, 2, 3, 4)
-        tdim = 2 if fmt == "vllm" else 3
+        tdim = KvView.token_dim(fmt)
         blob = blob.narrow(tdim, tok_begin, blob.shape[tdim] - tok_begin)
         return [c.contiguous() for c in torch.split(blob, self.chunk_size, dim=tdim)]
 
@@ -325,7 +295,58 @@ class LMCacheEngine:
     def _blob_to_tuple_kv(self, blob: torch.Tensor) -> KVCache:
         return tuple((layer[0], layer[1]) for layer in torch.unbind(blob, dim=0))
 
+    # ------------------------------------------------------------------ arguments and masks
+    def _check_store_args(self, tokens: torch.Tensor, kv_tensors_raw: KVCache, fmt: str) -> None:
+        assert len(tokens.shape) == 1, f"Invalid shape of tokens: {tokens.shape}"
+        assert len(kv_tensors_raw) > 0, "Empty kv_tensors"
+        assert len(tokens) == self._num_tokens_in_kv(kv_tensors_raw, fmt), \
+            "Number of tokens in the kv cache does not match the input tokens"
+
+    def _check_paged_args(self, tokens: torch.Tensor, slot_mapping: torch.Tensor, kv_caches=None) -> None:
+        """The paged methods' argument checks; the stores pass their kv_caches, which are checked too."""
+        if self.metadata.fmt != "vllm":
+            raise ValueError(f"paged KV caches use the vllm layout, engine fmt is {self.metadata.fmt}")
+        if kv_caches is not None:
+            assert len(tokens.shape) == 1, f"Invalid shape of tokens: {tokens.shape}"
+            assert len(kv_caches) > 0, "Empty kv_caches"
+        assert len(tokens) == slot_mapping.numel(), "Number of slots does not match the input tokens"
+
+    def _split_mask(self, tokens: torch.Tensor, mask: Optional[torch.Tensor]) -> Tuple[torch.Tensor, int, int, int]:
+        """A retrieve's suffix mask (None: every token): (ret_mask with the masked-off tokens cleared, num_skip_tok
+        masked-off tokens, num_skip_chunk whole chunks among them, extra masked-off tokens in the first chunk fetched)"""
+        num_skip_tok = 0 if mask is None else int(len(mask) - torch.sum(mask))
+        num_skip_chunk = num_skip_tok // self.chunk_size
+        ret_mask = torch.ones_like(tokens, dtype=torch.bool)
+        ret_mask[:num_skip_tok] = False
+        return ret_mask, num_skip_tok, num_skip_chunk, num_skip_tok - num_skip_chunk * self.chunk_size
+
+    @staticmethod
+    def _trim_mask(ret_mask: torch.Tensor, num_skip_tok: int, n_tok: int) -> torch.Tensor:
+        """ret_mask of a retrieve that got the n_tok tokens after the masked-off ones (none if n_tok <= 0)"""
+        if n_tok <= 0:
+            ret_mask[:] = False
+        else:
+            ret_mask[num_skip_tok + n_tok:] = False
+        return ret_mask
+
     # ------------------------------------------------------------------ store
+    def _skip_scan(self, chunk_hashes, fmt: str) -> int:
+        """store()'s skip_existing scan: the first chunk whose key the tier does not hold"""
+        for i, h in enumerate(chunk_hashes):
+            if not self.engine_.contains(self._make_key(h, fmt)):
+                return i
+        return len(chunk_hashes)
+
+    def _store_put(self, chunk_hashes, start: int, fmt: str, put: Optional[Callable]) -> int:
+        """Every store after its scan: touch the matched chunks [0, start), put(keys, tok_begin) the rest if there is
+        any (and put is not None), then touch the whole chain.  Returns the number of chunks put."""
+        self._touch(chunk_hashes[:start], fmt)
+        if put is None or start == len(chunk_hashes):
+            return 0
+        n = put(self._keys_of(chunk_hashes[start:], fmt), start * self.chunk_size)
+        self._touch(chunk_hashes, fmt)
+        return n
+
     @_lmcache_nvtx_annotate
     @torch.no_grad()
     def store(self, tokens: torch.Tensor, kv_tensors_raw: KVCache, skip_existing=True, blocking=True) -> None:
@@ -334,53 +355,26 @@ class LMCacheEngine:
         without a batch dimension."""
         start_time = time.perf_counter()
         fmt = self.metadata.fmt
-        assert len(tokens.shape) == 1, f"Invalid shape of tokens: {tokens.shape}"
-        assert len(kv_tensors_raw) > 0, "Empty kv_tensors"
-        assert len(tokens) == self._num_tokens_in_kv(kv_tensors_raw, fmt), \
-            "Number of tokens in the kv cache does not match the input tokens"
-
+        self._check_store_args(tokens, kv_tensors_raw, fmt)
         chunk_hashes = self._prefix_hash(tokens)
-        start_chunk_idx = 0
-        if skip_existing:
-            # prefix match: first chunk whose key is absent; everything from there on is stored
-            start_chunk_idx = len(chunk_hashes)
-            for i, h in enumerate(chunk_hashes):
-                if not self.engine_.contains(self._make_key(h, fmt)):
-                    start_chunk_idx = i
-                    break
-        n_chunks = 0
-        self._touch(chunk_hashes[:start_chunk_idx], fmt)
-        if start_chunk_idx < len(chunk_hashes):
-            keys = self._keys_of(chunk_hashes[start_chunk_idx:], fmt)
+        start = self._skip_scan(chunk_hashes, fmt) if skip_existing else 0
+
+        def put(keys, tok_begin):
             kv_cuda = self._as_cuda_kv(kv_tensors_raw)
             if kv_cuda[0][0].dtype not in (torch.bfloat16, torch.float16):
                 # the native pack / codec kernels move 16-bit KV; any other dtype (the reference's local and torch-serde
                 # paths accept every dtype) takes the reference's own blob ops on the GPU (cache_engine.py:98-161)
-                chunks = self._pack_chunks_torch(kv_cuda, start_chunk_idx * self.chunk_size, fmt)
-                end_make_chunks = time.perf_counter()
-                n_chunks = self.engine_.batched_put(zip(keys, chunks), blocking=blocking)
-                self._touch(chunk_hashes, fmt)
-                logger.info(f"Stored/updated {n_chunks} chunks, total time {time.perf_counter() - start_time:.2f}s, "
-                            f"make chunks time {end_make_chunks - start_time:.2f}s")
-                return
+                chunks = self._pack_chunks_torch(kv_cuda, tok_begin, fmt)
+                return self.engine_.batched_put(zip(keys, chunks), blocking=blocking)
             view = KvView.from_tuple(kv_cuda, fmt)
             self._geom = (view.L, view.H, view.D, view.dtype)
             if self._fast_path():
                 # native path: the backend consumes the caller's 2L tensors directly (batched encode / one gather)
-                end_make_chunks = time.perf_counter()
-                n_chunks = self.engine_.put_kv_chunks(keys, view, start_chunk_idx * self.chunk_size, self.chunk_size,
-                                                      blocking=blocking)
-            else:
-                chunks = self._pack_chunks(view, start_chunk_idx * self.chunk_size, fmt)
-                end_make_chunks = time.perf_counter()
-                n_chunks = self.engine_.batched_put(zip(keys, chunks), blocking=blocking)
-        else:
-            end_make_chunks = time.perf_counter()
-        if start_chunk_idx < len(chunk_hashes):
-            self._touch(chunk_hashes, fmt)
-        end_time = time.perf_counter()
-        logger.info(f"Stored/updated {n_chunks} chunks, total time {end_time - start_time:.2f}s, "
-                    f"make chunks time {end_make_chunks - start_time:.2f}s")
+                return self.engine_.put_kv_chunks(keys, view, tok_begin, self.chunk_size, blocking=blocking)
+            _, chunks = view.pack_chunks(tok_begin, self.chunk_size)
+            return self.engine_.batched_put(zip(keys, chunks), blocking=blocking)
+        n_chunks = self._store_put(chunk_hashes, start, fmt, put)
+        logger.info(f"Stored/updated {n_chunks} chunks, total time {time.perf_counter() - start_time:.2f}s")
 
     # ------------------------------------------------------------------ retrieve
     @_lmcache_nvtx_annotate
@@ -388,24 +382,23 @@ class LMCacheEngine:
     def retrieve(self, tokens: torch.Tensor, mask: Optional[torch.Tensor] = None) -> Tuple[KVCache, torch.Tensor]:
         """Retrieve the longest cached prefix of `tokens` (optionally only the suffix selected by a boolean
         suffix `mask`).  Returns (kv tuple -- empty tuple on a total miss, ret_mask marking retrieved tokens)."""
-        num_skip_chunk = 0
-        num_skip_tok = 0
-        ret_mask = torch.ones_like(tokens, dtype=torch.bool)
-        if mask is not None:
-            num_skip_tok = int(len(mask) - torch.sum(mask))
-            num_skip_chunk = num_skip_tok // self.chunk_size
-        ret_mask[:num_skip_tok] = False
+        return self._retrieve(tokens, mask)
 
+    def _retrieve(self, tokens, mask, get_kv=None) -> Tuple[KVCache, torch.Tensor]:
+        """retrieve(); get_kv(keys, view, tok0, chunk_size) -> chunks decoded fetches this layout's chunks on the native
+        path (default: the backend's get_kv_into).  A get_kv comes from _layerwise_get, which has checked that path."""
+        ret_mask, num_skip_tok, num_skip_chunk, extra = self._split_mask(tokens, mask)
         st = time.perf_counter()
         fmt = self.metadata.fmt
         if fmt not in ("vllm", "huggingface"):
             raise ValueError(f"Invalid format: {fmt}")
         full_chain = self._prefix_hash(tokens)
         chunk_hashes = full_chain[num_skip_chunk:]
-        if self._fast_path() and len(chunk_hashes) > 0 and not getattr(self, "_wide_dtype", False):
+        native = get_kv is not None or self._fast_path()
+        if native and len(chunk_hashes) > 0 and not getattr(self, "_wide_dtype", False):
             try:
-                return self._retrieve_into_blob(tokens, chunk_hashes, num_skip_tok, num_skip_chunk, ret_mask, fmt, st,
-                                                full_chain)
+                return self._retrieve_into_blob(tokens, full_chain, ret_mask, num_skip_tok, num_skip_chunk, extra, fmt,
+                                                st, get_kv)
             except TypeError:
                 self._wide_dtype = True      # chunks of a dtype the kernels do not move: per-chunk path from now on
         retrieved: List[torch.Tensor] = []
@@ -416,12 +409,10 @@ class LMCacheEngine:
         self._touch(full_chain[:num_skip_chunk + len(retrieved)], fmt)
         if len(retrieved) == 0:
             logger.info("Retrieved 0 chunks")
-            ret_mask[:] = False
-            return (), ret_mask
+            return (), self._trim_mask(ret_mask, num_skip_tok, 0)
 
         # assemble into one blob; drop the extra leading tokens of the first chunk (suffix mask)
-        tdim = 2 if fmt == "vllm" else 3
-        extra = num_skip_tok - num_skip_chunk * self.chunk_size
+        tdim = KvView.token_dim(fmt)
         sizes = [c.shape[tdim] for c in retrieved]
         total = sum(sizes) - extra
         first = retrieved[0]
@@ -434,12 +425,9 @@ class LMCacheEngine:
             n = src.shape[tdim]
             blob.narrow(tdim, pos, n).copy_(src)
             pos += n
-        ret = self._blob_to_tuple_kv(blob)
-        retrieved_token_count = total
-        logger.info(f"Retrieved {len(retrieved)} chunks ({retrieved_token_count} tokens in total) -- "
+        logger.info(f"Retrieved {len(retrieved)} chunks ({total} tokens in total) -- "
                     f"elapsed time {time.perf_counter() - st}")
-        ret_mask[num_skip_tok + retrieved_token_count:] = False
-        return ret, ret_mask
+        return self._blob_to_tuple_kv(blob), self._trim_mask(ret_mask, num_skip_tok, total)
 
     # ------------------------------------------------------------------ paged KV caches, in place
     @_lmcache_nvtx_annotate
@@ -450,31 +438,19 @@ class LMCacheEngine:
         (key_cache, value_cache) [num_blocks, block_size, H, D].  What lmcache-vllm's lmcache_store_kv does with a
         torch gather per layer + store() (LLM_Engine.rst:91-99); here the backend's kernels read the cache rows
         directly (cachegen: quantise + code from the rows; local tiers: one gather straight into the chunk blobs)."""
-        if self.metadata.fmt != "vllm":
-            raise ValueError(f"paged KV caches use the vllm layout, engine fmt is {self.metadata.fmt}")
-        assert len(tokens.shape) == 1, f"Invalid shape of tokens: {tokens.shape}"
-        assert len(kv_caches) > 0, "Empty kv_caches"
-        assert len(tokens) == slot_mapping.numel(), "Number of slots does not match the input tokens"
+        self._check_paged_args(tokens, slot_mapping, kv_caches)
         if not self._fast_path():
             flat = [(k.reshape(-1, k.shape[-2], k.shape[-1]), v.reshape(-1, v.shape[-2], v.shape[-1])) for k, v in kv_caches]
             idx = slot_mapping.to(flat[0][0].device)
             return self.store(tokens, tuple((k[idx], v[idx]) for k, v in flat), skip_existing, blocking)
-        fmt = "vllm"
         chunk_hashes = self._prefix_hash(tokens)
-        start_chunk_idx = 0
-        if skip_existing:
-            start_chunk_idx = len(chunk_hashes)
-            for i, h in enumerate(chunk_hashes):
-                if not self.engine_.contains(self._make_key(h, fmt)):
-                    start_chunk_idx = i
-                    break
-        self._touch(chunk_hashes[:start_chunk_idx], fmt)
-        if start_chunk_idx < len(chunk_hashes):
+        start = self._skip_scan(chunk_hashes, "vllm") if skip_existing else 0
+
+        def put(keys, tok_begin):
             view = KvView.from_paged(kv_caches, slot_mapping.cuda())
             self._geom = (view.L, view.H, view.D, view.dtype)
-            keys = self._keys_of(chunk_hashes[start_chunk_idx:], fmt)
-            self.engine_.put_kv_chunks(keys, view, start_chunk_idx * self.chunk_size, self.chunk_size, blocking=blocking)
-            self._touch(chunk_hashes, fmt)
+            return self.engine_.put_kv_chunks(keys, view, tok_begin, self.chunk_size, blocking=blocking)
+        self._store_put(chunk_hashes, start, "vllm", put)
 
     @_lmcache_nvtx_annotate
     @torch.no_grad()
@@ -486,11 +462,8 @@ class LMCacheEngine:
         return self._retrieve_paged(tokens, kv_caches, slot_mapping, mask)
 
     def _retrieve_paged(self, tokens, kv_caches, slot_mapping, mask, get_kv=None) -> torch.Tensor:
-        """retrieve_paged; get_kv(keys, view, tok0, chunk_size) -> chunks decoded, for every chunk but a first one that
-        straddles the mask (default: the backend's get_kv_into)"""
-        if self.metadata.fmt != "vllm":
-            raise ValueError(f"paged KV caches use the vllm layout, engine fmt is {self.metadata.fmt}")
-        assert len(tokens) == slot_mapping.numel(), "Number of slots does not match the input tokens"
+        """retrieve_paged; get_kv as in _retrieve, for every chunk but a first one that straddles the mask"""
+        self._check_paged_args(tokens, slot_mapping)
         flat = [(k.reshape(-1, k.shape[-2], k.shape[-1]), v.reshape(-1, v.shape[-2], v.shape[-1])) for k, v in kv_caches]
         dev = flat[0][0].device
         slots = slot_mapping.to(dev)
@@ -503,48 +476,29 @@ class LMCacheEngine:
                     vc[idx] = v.to(vc.dtype)
             return ret_mask
         cs = self.chunk_size
-        num_skip_tok = int(len(mask) - torch.sum(mask)) if mask is not None else 0
-        num_skip_chunk = num_skip_tok // cs
-        extra = num_skip_tok - num_skip_chunk * cs
-        ret_mask = torch.ones_like(tokens, dtype=torch.bool)
-        ret_mask[:num_skip_tok] = False
+        ret_mask, num_skip_tok, num_skip_chunk, extra = self._split_mask(tokens, mask)
         full_chain = self._prefix_hash(tokens)
-        keys = self._keys_of(full_chain[num_skip_chunk:], "vllm")
+        chunk_hashes = full_chain[num_skip_chunk:]
         base = num_skip_chunk * cs
         view = KvView.from_paged(kv_caches, slots[base:])
-        got_chunks, first, own = 0, 0, 0
-        layout = None            # the other layout that serves the chunks after this engine's own prefix (_reshard_get)
-        if extra > 0 and keys:
+        first = 1 if extra > 0 and len(chunk_hashes) > 0 else 0
+        layout, own, got_chunks = None, 0, 0      # layout: the other one that serves the chunks after this engine's own
+        if first:
             # the first chunk straddles the mask: decode it next to the cache and scatter only its unmasked tail
             t0 = min(cs, len(tokens) - base)
-            tmp = torch.empty((view.L, 2, t0, view.H, view.D), dtype=view.dtype, device=dev)
-            tmp_view = KvView.from_blob(tmp, "vllm")
-            own = self.engine_.get_kv_into(keys[:1], tmp_view, 0, cs)
-            if own == 0:
-                layout, got = self._reshard_get(full_chain[num_skip_chunk:num_skip_chunk + 1], "vllm", tmp_view, 0)
-                if got == 0:
-                    self._touch(full_chain[:num_skip_chunk], "vllm")
-                    ret_mask[:] = False
-                    return ret_mask
-            idx = slots[base + extra: base + t0]
-            for l, (kc, vc) in enumerate(flat):
-                kc[idx] = tmp[l, 0, extra:]
-                vc[idx] = tmp[l, 1, extra:]
-            got_chunks, first = 1, 1
-        if len(keys) > first:
-            if layout is None:
-                got_chunks += (get_kv or self.engine_.get_kv_into)(keys[first:], view, first * cs, cs)
-                own = got_chunks
-            layout, got = self._reshard_get(full_chain[num_skip_chunk + got_chunks:], "vllm", view, got_chunks * cs,
-                                            layout)
-            got_chunks += got
+            tmp = torch.empty(KvView.blob_shape("vllm", view.L, view.H, view.D, t0), dtype=view.dtype, device=dev)
+            layout, own, got_chunks = self._fetch(chunk_hashes[:1], "vllm", KvView.from_blob(tmp, "vllm"), 0)
+            if got_chunks:
+                idx = slots[base + extra: base + t0]
+                for l, (kc, vc) in enumerate(flat):
+                    kc[idx] = tmp[l, 0, extra:]
+                    vc[idx] = tmp[l, 1, extra:]
+        if got_chunks == first and len(chunk_hashes) > first:       # not after a straddling chunk that missed
+            layout, own_rest, n = self._fetch(chunk_hashes[first:], "vllm", view, first * cs, get_kv, layout)
+            own += own_rest
+            got_chunks += n
         self._touch(full_chain[:num_skip_chunk + own], "vllm")
-        got = min(base + got_chunks * cs, len(tokens))
-        if got <= num_skip_tok:
-            ret_mask[:] = False
-        else:
-            ret_mask[got:] = False
-        return ret_mask
+        return self._trim_mask(ret_mask, num_skip_tok, min(base + got_chunks * cs, len(tokens)) - num_skip_tok)
 
     # ------------------------------------------------------------------ other tensor-parallel layouts
     def _foreign_key(self, chunk_hash: str, fmt: str, world_size: int, rank: int) -> CacheEngineKey:
@@ -625,64 +579,64 @@ class LMCacheEngine:
         """(L, H, D, dtype) of this engine's chunks, learnt from the first store / a probe get."""
         return getattr(self, "_geom", None)
 
-    def _retrieve_into_blob(self, tokens, chunk_hashes, num_skip_tok, num_skip_chunk, ret_mask, fmt, st, full_chain,
-                            get_kv=None):
+    def _fetch(self, chunk_hashes, fmt: str, view: KvView, tok0: int, get_kv=None, layout: Optional[int] = None,
+               own_miss: bool = False) -> Tuple[Optional[int], int, int]:
+        """Decode the chunks of `chunk_hashes` into `view`, the first at token tok0, up to the first miss: this layout's
+        through get_kv (default: the backend's get_kv_into) -- unless another `layout` was chosen before or this one is
+        known to miss the first chunk (own_miss) -- then the chunks after them from another layout (_reshard_get).
+        Returns (layout, chunks of this layout, chunks in all)."""
+        own = 0
+        if layout is None and not own_miss:
+            own = (get_kv or self.engine_.get_kv_into)(self._keys_of(chunk_hashes, fmt), view, tok0, self.chunk_size)
+        layout, n = self._reshard_get(chunk_hashes[own:], fmt, view, tok0 + own * self.chunk_size, layout)
+        return layout, own, own + n
+
+    def _retrieve_into_blob(self, tokens, full_chain, ret_mask, num_skip_tok, num_skip_chunk, extra, fmt, st, get_kv):
         """retrieve() without per-chunk tensors or torch.cat: the backend decodes / uploads every hit chunk straight
-        into one preallocated blob; the suffix-mask trim of the first chunk is a view offset, not a copy.  get_kv: as
-        in _retrieve_paged."""
-        keys = self._keys_of(chunk_hashes, fmt)
+        into one preallocated blob; the suffix-mask trim of the first chunk is a view offset, not a copy."""
+        chunk_hashes = full_chain[num_skip_chunk:]
         geom = self._kv_geometry()
         own_miss = False         # this layout holds not even the first chunk: only another layout can serve it
         if geom is None:
             # shapes unknown (nothing stored through this engine yet -- the normal case for a retrieve-only replica):
             # read them from the first chunk's container header / stored blob; only backends without that door pay
             # for a full get of chunk 0
+            key0 = self._make_key(chunk_hashes[0], fmt)
             peek = getattr(self.engine_, "peek_geometry", None)
             if peek is not None:
-                geom = peek(keys[0], fmt)
+                geom = peek(key0, fmt)
             else:
-                first = self.engine_.get(keys[0])
+                first = self.engine_.get(key0)
                 if first is not None:
-                    geom = ((first.shape[0], first.shape[3], first.shape[4]) if fmt == "vllm" else
-                            (first.shape[0], first.shape[2], first.shape[4])) + (first.dtype,)
+                    geom = KvView.blob_geometry(first, fmt)
             if geom is None and self.config.reshard_world_sizes:
                 geom = self._reshard_geometry(chunk_hashes[0], fmt)
                 own_miss = geom is not None
             if geom is None:
                 self._touch(full_chain[:num_skip_chunk], fmt)
                 logger.info("Retrieved 0 chunks")
-                ret_mask[:] = False
-                return (), ret_mask
+                return (), self._trim_mask(ret_mask, num_skip_tok, 0)
             self._geom = geom
         L, H, D, dtype = geom
         od = getattr(self.engine_, "out_dtype", None) or getattr(getattr(self.engine_, "deserializer", None), "out_dtype", None)
         if od is not None and od() is not None:
             dtype = od()
         n_tok_max = len(tokens) - num_skip_chunk * self.chunk_size
-        shape = (L, 2, n_tok_max, H, D) if fmt == "vllm" else (L, 2, H, n_tok_max, D)
-        device = torch.device("cuda", torch.cuda.current_device())
-        blob = torch.empty(shape, dtype=dtype, device=device)
-        view = KvView.from_blob(blob, fmt)
-        own = 0 if own_miss else (get_kv or self.engine_.get_kv_into)(keys, view, 0, self.chunk_size)
-        n = own + self._reshard_get(chunk_hashes[own:], fmt, view, own * self.chunk_size)[1]
+        blob = torch.empty(KvView.blob_shape(fmt, L, H, D, n_tok_max), dtype=dtype,
+                           device=torch.device("cuda", torch.cuda.current_device()))
+        _, own, n = self._fetch(chunk_hashes, fmt, KvView.from_blob(blob, fmt), 0, get_kv, own_miss=own_miss)
         self._touch(full_chain[:num_skip_chunk + own], fmt)
         if n == 0:
             logger.info("Retrieved 0 chunks")
-            ret_mask[:] = False
-            return (), ret_mask
-        tdim = 2 if fmt == "vllm" else 3
-        got = min(n * self.chunk_size, n_tok_max)              # the last hit chunk may be the ragged tail
-        extra = num_skip_tok - num_skip_chunk * self.chunk_size
-        ret = self._blob_to_tuple_kv(blob.narrow(tdim, extra, got - extra))
-        retrieved_token_count = got - extra
-        logger.info(f"Retrieved {n} chunks ({retrieved_token_count} tokens in total) -- "
-                    f"elapsed time {time.perf_counter() - st}")
-        ret_mask[num_skip_tok + retrieved_token_count:] = False
-        return ret, ret_mask
+            return (), self._trim_mask(ret_mask, num_skip_tok, 0)
+        got = min(n * self.chunk_size, n_tok_max) - extra      # the last hit chunk may be the ragged tail
+        logger.info(f"Retrieved {n} chunks ({got} tokens in total) -- elapsed time {time.perf_counter() - st}")
+        kv = self._blob_to_tuple_kv(blob.narrow(KvView.token_dim(fmt), extra, got))
+        return kv, self._trim_mask(ret_mask, num_skip_tok, got)
 
     # ------------------------------------------------------------------ layer-wise retrieve
     def _layerwise_get(self):
-        """(get_kv for the helpers above, list that receives the LayerwiseUpload), or None: the backend has no
+        """(get_kv for _retrieve / _retrieve_paged, list that receives the LayerwiseUpload), or None: the backend has no
         layer-major path (raw, remote and hybrid tiers) or its containers hold several groups (chunk_size > 256)"""
         f = getattr(self.engine_, "get_kv_layerwise", None)
         if f is None or not self._fast_path() or self.chunk_size > N.GROUP_TOKENS:
@@ -709,41 +663,17 @@ class LMCacheEngine:
         KV after synchronize() are those of retrieve().  On the compressed host and disk tiers the containers are
         uploaded and decoded layer-major, so layer 0 is ready after about 1/L of the bytes; on every other tier (and
         for chunks of more than 256 tokens) this is retrieve() followed by one event that stands for every layer."""
-        lw = self._layerwise_get()
+        get_kv, uploads = self._layerwise_get() or (None, [])
+        kv, ret_mask = self._retrieve(tokens, mask, get_kv)
         geom = self._kv_geometry()
-        if lw is None or getattr(self, "_wide_dtype", False):
-            kv, ret_mask = self.retrieve(tokens, mask)
-            return self._layerwise_result(ret_mask, kv, len(kv) if len(kv) else (geom[0] if geom else 0), [])
-        get_kv, uploads = lw
-        num_skip_tok = 0
-        ret_mask = torch.ones_like(tokens, dtype=torch.bool)
-        if mask is not None:
-            num_skip_tok = int(len(mask) - torch.sum(mask))
-        num_skip_chunk = num_skip_tok // self.chunk_size
-        ret_mask[:num_skip_tok] = False
-        fmt = self.metadata.fmt
-        if fmt not in ("vllm", "huggingface"):
-            raise ValueError(f"Invalid format: {fmt}")
-        full_chain = self._prefix_hash(tokens)
-        chunk_hashes = full_chain[num_skip_chunk:]
-        if len(chunk_hashes) == 0:
-            kv, ret_mask = self.retrieve(tokens, mask)
-            return self._layerwise_result(ret_mask, kv, geom[0] if geom else 0, [])
-        kv, ret_mask = self._retrieve_into_blob(tokens, chunk_hashes, num_skip_tok, num_skip_chunk, ret_mask, fmt,
-                                                time.perf_counter(), full_chain, get_kv)
-        geom = self._kv_geometry()
-        return self._layerwise_result(ret_mask, kv, geom[0] if geom else 0, uploads)
+        return self._layerwise_result(ret_mask, kv, len(kv) or (geom[0] if geom else 0), uploads)
 
     @torch.no_grad()
     def retrieve_paged_layerwise(self, tokens: torch.Tensor, kv_caches, slot_mapping: torch.Tensor,
                                  mask: Optional[torch.Tensor] = None) -> LayerwiseRetrieval:
         """retrieve_paged(), with the KV made available one layer at a time (see retrieve_layerwise).  A first chunk
         that straddles the mask is decoded and scattered whole before layer 0's wait; `kv` is None."""
-        lw = self._layerwise_get()
-        if lw is None:
-            ret_mask = self.retrieve_paged(tokens, kv_caches, slot_mapping, mask)
-            return self._layerwise_result(ret_mask, None, len(kv_caches), [])
-        get_kv, uploads = lw
+        get_kv, uploads = self._layerwise_get() or (None, [])
         ret_mask = self._retrieve_paged(tokens, kv_caches, slot_mapping, mask, get_kv)
         return self._layerwise_result(ret_mask, None, len(kv_caches), uploads)
 
@@ -753,13 +683,6 @@ class LMCacheEngine:
         at most 256 tokens (version-3 containers); raw, remote and hybrid tiers cannot."""
         return (getattr(self.engine_, "begin_layerwise_store", None) is not None and self._fast_path() and
                 self.chunk_size <= N.GROUP_TOKENS and dtype in (torch.bfloat16, torch.float16))
-
-    def _skip_scan(self, chunk_hashes, fmt: str) -> int:
-        """store()'s skip_existing scan: the first chunk whose key the tier does not hold"""
-        for i, h in enumerate(chunk_hashes):
-            if not self.engine_.contains(self._make_key(h, fmt)):
-                return i
-        return len(chunk_hashes)
 
     def _begin_layerwise(self, tokens, view_fn, fmt: str, num_layers: int, skip_existing: bool,
                          fallback: Callable) -> LayerwiseStore:
@@ -778,12 +701,10 @@ class LMCacheEngine:
                 return LayerwiseStore(num_layers, None, fallback)
 
         def publish(stream, enc):
-            self._touch(chunk_hashes[:start], fmt)
-            if enc is not None:
-                keys = self._keys_of(chunk_hashes[start:], fmt)
-                self.engine_.put_kv_chunks(keys, None, start * self.chunk_size, self.chunk_size, blocking=False,
-                                           encoded=enc)
-                self._touch(chunk_hashes, fmt)
+            # enc is None when the scan matched every chunk, or when the handle was closed: nothing to put
+            put = None if enc is None else lambda keys, tok_begin: self.engine_.put_kv_chunks(
+                keys, None, tok_begin, self.chunk_size, blocking=False, encoded=enc)
+            self._store_put(chunk_hashes, start, fmt, put)
         return LayerwiseStore(num_layers, enc, publish)
 
     @torch.no_grad()
@@ -793,11 +714,7 @@ class LMCacheEngine:
         called; call save_layer(l) once layer l is written and finish() after the last layer (LayerwiseStore).  The keys
         stored, the containers and the eviction touches are those of store_paged(tokens, kv_caches, slot_mapping,
         skip_existing)."""
-        if self.metadata.fmt != "vllm":
-            raise ValueError(f"paged KV caches use the vllm layout, engine fmt is {self.metadata.fmt}")
-        assert len(tokens.shape) == 1, f"Invalid shape of tokens: {tokens.shape}"
-        assert len(kv_caches) > 0, "Empty kv_caches"
-        assert len(tokens) == slot_mapping.numel(), "Number of slots does not match the input tokens"
+        self._check_paged_args(tokens, slot_mapping, kv_caches)
 
         def fallback(stream, enc):
             with torch.cuda.stream(stream):
@@ -812,10 +729,7 @@ class LMCacheEngine:
         """store(), with the KV handed over one layer at a time (see store_paged_layerwise): kv_tensors_raw is store()'s
         per-layer (K, V) tuple on the GPU, possibly not yet written."""
         fmt = self.metadata.fmt
-        assert len(tokens.shape) == 1, f"Invalid shape of tokens: {tokens.shape}"
-        assert len(kv_tensors_raw) > 0, "Empty kv_tensors"
-        assert len(tokens) == self._num_tokens_in_kv(kv_tensors_raw, fmt), \
-            "Number of tokens in the kv cache does not match the input tokens"
+        self._check_store_args(tokens, kv_tensors_raw, fmt)
 
         def fallback(stream, enc):
             with torch.cuda.stream(stream):

@@ -95,6 +95,17 @@ class KvView:
             raise TypeError(f"KV dtype must be bfloat16 or float16, got {dtype}")
         return _DTYPE_CODE[dtype]
 
+    # A chunk blob holds t tokens of every layer: [L,2,t,H,D] (vllm) or [L,2,H,t,D] (huggingface).  Its token
+    # dimension, its shape, and the (L, H, D, dtype) read back from one:
+    @staticmethod
+    def token_dim(fmt: str) -> int: return 2 if fmt == "vllm" else 3
+    @staticmethod
+    def blob_shape(fmt: str, L: int, H: int, D: int, t: int) -> Tuple[int, ...]:
+        return (L, 2, t, H, D) if fmt == "vllm" else (L, 2, H, t, D)
+    @staticmethod
+    def blob_geometry(blob: torch.Tensor, fmt: str) -> Tuple[int, int, int, torch.dtype]:
+        return blob.shape[0], blob.shape[3 if fmt == "vllm" else 2], blob.shape[4], blob.dtype
+
     @staticmethod
     def from_blob(blob: torch.Tensor, fmt: str) -> "KvView":
         """blob: [L,2,T,H,D] (vllm) or [L,2,H,T,D] (huggingface); any strides with a contiguous last dim."""
@@ -195,6 +206,23 @@ class KvView:
         d.dtype = KvView._code(ref.dtype)
         d.slot_map = slot_mapping.data_ptr()
         return KvView(d, (keep, ptrs), slot_mapping.numel(), ref.device, ref.dtype, "vllm")
+
+    def pack_chunks(self, tok_begin: int, chunk_size: int) -> Tuple[torch.Tensor, List[torch.Tensor]]:
+        """Gather tokens [tok_begin, T), at least one, into blobs of chunk_size tokens (the last may be shorter) with one
+        b200kv_pack_chunks launch on the current stream.  Returns the buffer and the blobs, back to back views of it."""
+        n_tok = self.ntokens - tok_begin
+        n_chunks = (n_tok + chunk_size - 1) // chunk_size
+        per_tok = 2 * self.L * self.H * self.D
+        stride = per_tok * chunk_size
+        buf = torch.empty(n_chunks * stride, dtype=self.dtype, device=self.device)
+        with torch.cuda.device(self.device):
+            N.check(N.lib().b200kv_pack_chunks(ctypes.byref(self.desc), tok_begin, n_chunks, chunk_size,
+                                               n_tok - (n_chunks - 1) * chunk_size, int(self.fmt == "huggingface"),
+                                               ctypes.c_void_p(buf.data_ptr()), stride * buf.element_size(),
+                                               _stream_ptr(None)), "pack_chunks")
+        sizes = [min(chunk_size, n_tok - j * chunk_size) for j in range(n_chunks)]
+        return buf, [buf[j * stride: j * stride + per_tok * t].view(self.blob_shape(self.fmt, self.L, self.H, self.D, t))
+                     for j, t in enumerate(sizes)]
 
 
 def parse_header(buf, total: Optional[int] = None) -> N.Header:

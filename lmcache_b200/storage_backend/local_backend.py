@@ -16,6 +16,7 @@ from typing import Dict, Optional
 import torch
 
 from lmcache_b200 import _native as N
+from lmcache_b200.codec import KvView
 from lmcache_b200.config import LMCacheEngineConfig
 from lmcache_b200.logging import init_logger
 from lmcache_b200.storage_backend.abstract_backend import LMCBackendInterface
@@ -119,45 +120,23 @@ class LMCLocalBackend(LMCBackendInterface):
         if val is None:
             return None
         t = val.host if isinstance(val, _HostEntry) else val
-        if t.dim() != 5:
-            return None
-        return (t.shape[0], t.shape[2], t.shape[4], t.dtype) if fmt == "huggingface" else \
-            (t.shape[0], t.shape[3], t.shape[4], t.dtype)
+        return KvView.blob_geometry(t, fmt) if t.dim() == 5 else None
 
     def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True) -> int:
         """Store tokens [tok_begin, T) of `view` as len(keys) chunk blobs: ONE gather kernel (b200kv_pack_chunks)
         builds every chunk blob; for the host tier ONE device->host DMA moves them all into a page-locked slab."""
-        fmt_hf = getattr(view, "fmt", "vllm") == "huggingface"
-        n_tok = view.ntokens - tok_begin
-        n_chunks = len(keys)
-        assert n_chunks == (n_tok + chunk_size - 1) // chunk_size
-        last = n_tok - (n_chunks - 1) * chunk_size
-        per_tok = 2 * view.L * view.H * view.D
-        stride = per_tok * chunk_size
-        dev = torch.empty(n_chunks * stride, dtype=view.dtype, device=view.device)
         with torch.cuda.device(view.device):
-            cur = torch.cuda.current_stream()
-            N.check(N.lib().b200kv_pack_chunks(ctypes.byref(view.desc), tok_begin, n_chunks, chunk_size, last,
-                                               1 if fmt_hf else 0, ctypes.c_void_p(dev.data_ptr()),
-                                               stride * dev.element_size(), cur.cuda_stream), "pack_chunks")
-
-            def shape(t):
-                return (view.L, 2, view.H, t, view.D) if fmt_hf else (view.L, 2, t, view.H, view.D)
-
-            if self.device == "cuda":
-                vals = [dev[j * stride: j * stride + per_tok * (chunk_size if j < n_chunks - 1 else last)]
-                        .view(shape(chunk_size if j < n_chunks - 1 else last)) for j in range(n_chunks)]
-            else:
-                host = torch.empty(n_chunks * stride, dtype=view.dtype, pin_memory=True)
+            dev, vals = view.pack_chunks(tok_begin, chunk_size)
+            assert len(vals) == len(keys)
+            if self.device != "cuda":
+                host = torch.empty(dev.numel(), dtype=dev.dtype, pin_memory=True)
                 side = self._side_stream(view.device)
-                side.wait_stream(cur)
+                side.wait_stream(torch.cuda.current_stream())
                 _copy_async(host, dev, side)
                 ev = torch.cuda.Event()
                 ev.record(side)
-                vals = []
-                for j in range(n_chunks):
-                    t = chunk_size if j < n_chunks - 1 else last
-                    vals.append(_HostEntry(host[j * stride: j * stride + per_tok * t].view(shape(t)), ev, dev))
+                # each host chunk sits at its device chunk's offset
+                vals = [_HostEntry(host.as_strided(c.shape, c.stride(), c.storage_offset()), ev, dev) for c in vals]
                 if blocking:
                     ev.synchronize()
                     for v in vals:
@@ -165,7 +144,7 @@ class LMCLocalBackend(LMCBackendInterface):
         with self.update_lock:
             for key, v in zip(keys, vals):
                 self.dict[key] = v
-        return n_chunks
+        return len(vals)
 
     def get_kv_into(self, keys, dst, dst_tok0: int, chunk_size: int) -> int:
         """Copy consecutive chunks (until the first miss) straight into the destination blob view `dst` at token
@@ -187,7 +166,7 @@ class LMCLocalBackend(LMCBackendInterface):
                     val.wait()
                 elif not src.is_cuda:
                     src = src.cuda()
-                t = src.shape[3] if fmt_hf else src.shape[2]
+                t = src.shape[KvView.token_dim(dst.fmt)]
                 tok = dst_tok0 + i * chunk_size
                 if tok + t > dst.ntokens or src.dtype != blob.dtype:
                     break
@@ -226,7 +205,7 @@ class LMCLocalBackend(LMCBackendInterface):
                     src = val.host.to(dst.device, non_blocking=True)
                 else:
                     src = val if val.is_cuda else val.cuda()
-                t = src.shape[3] if hf else src.shape[2]
+                t = src.shape[KvView.token_dim(dst.fmt)]
                 tok = dst_tok0 + i * chunk_size
                 if tok + t > dst.ntokens or src.dtype != dst.dtype:
                     break
@@ -537,7 +516,6 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
 
     @_lmcache_nvtx_annotate
     def put(self, key: CacheEngineKey, kv_chunk: torch.Tensor, blocking: bool = True) -> None:
-        from lmcache_b200.codec import KvView
         if not kv_chunk.is_cuda:
             kv_chunk = kv_chunk.cuda()              # reference: tensor.cuda() in the serializer (cachegen_encoder.py:383)
         view = KvView.from_blob(kv_chunk, self.fmt)
@@ -724,13 +702,12 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
 
     @_lmcache_nvtx_annotate
     def get(self, key: CacheEngineKey) -> Optional[torch.Tensor]:
-        from lmcache_b200.codec import KvView
         e = self._ready_entry(key)
         if e is None:
             return None
         r = e.rec
-        shape = (r.L, 2, r.ntokens, r.H, r.D) if self.fmt == "vllm" else (r.L, 2, r.H, r.ntokens, r.D)
-        out = torch.empty(shape, dtype=self.out_dtype(), device=torch.device("cuda", torch.cuda.current_device()))
+        out = torch.empty(KvView.blob_shape(self.fmt, r.L, r.H, r.D, r.ntokens), dtype=self.out_dtype(),
+                          device=torch.device("cuda", torch.cuda.current_device()))
         if self.get_kv_into([key], KvView.from_blob(out, self.fmt), 0, r.ntokens) != 1:
             return None
         self.touch([key])
