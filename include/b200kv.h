@@ -54,6 +54,16 @@ extern "C" {
                                                * payload bits per symbol (e.g. the previous call's sizes said so); the
                                                * compaction kernel then keeps its full-size shared-memory stage (tiles of
                                                * 10+ KB).  Output bytes are identical either way. */
+#define B200KV_KV_LATENT 0x100  /* OR into b200kv_kv_desc.dtype: the KV holds ONE plane per layer (multi-head latent attention,
+                                 * e.g. DeepSeek-V2/V3's [T, 576] latent vector), not a (K, V) pair.  Plane l of layer l is
+                                 * planes[l], or base + (l*sL + tok*sT + h*sH + d) * 2 (sKV unused); it is coded with layer l's
+                                 * KEY bins.  Such a descriptor reads and writes container version 4 = version 3 with L planes
+                                 * instead of 2L (rANS-compact coder only; refused with coders 0 and 1).  OR it into `coder`
+                                 * wherever a coder names a container: b200kv_container_layout_v, b200kv_encode_workspace_bytes
+                                 * and the decode calls (coder B200KV_CODER_RANS_COMPACT | B200KV_KV_LATENT = version 4; a
+                                 * decode whose coder and destination disagree on the flag is refused).  Added without
+                                 * changing anything that existed: every entry point below that names "2L" means L for a latent
+                                 * descriptor, and b200kv_decode_plan_heads refuses a latent destination. */
 #define B200KV_LP 33            /* CDF entries per stream (cachegen_encoder.py:287-289: int(bins.max()) + 1) */
 #define B200KV_GROUP_TOKENS 256 /* CACHEGEN_GPU_MAX_TOKENS_PER_CHUNK (cachegen_basics.py:13) */
 #define B200KV_MAX_PLANES 256   /* 2 * nlayers upper bound: models of up to 128 layers */
@@ -96,7 +106,10 @@ typedef struct b200kv_kv_desc {
  *   [a zero byte if that makes the length even] [the version-2 rANS stream];  half-lengths[c] = bytes of all that / 2.
  * The CDF the reference keeps (cachegen_encoder.py:287-290) is a function of these counts n_s and t = ntokens:
  *   cdf[i] = int16(rint(fl32(sum_{k<i} fl32(n_k / t), accumulated in double) * 65504) + i)      (in-tree spec :95-126)
- * so CacheGenGPUEncoderOutput.from_bytes rebuilds the identical tensor, and the decoder evaluates it on the device. */
+ * so CacheGenGPUEncoderOutput.from_bytes rebuilds the identical tensor, and the decoder evaluates it on the device.
+ * Version 4 (B200KV_KV_LATENT: one plane per layer) is version 3 with P = L planes instead of 2L:
+ *   header | nb u8[L] (pad to 16) | maxes [L, t] | half-lengths u8[L][C] | bytestream (streams in plane order)
+ * header.L is the number of layers (= planes). */
 typedef struct b200kv_header {
     uint32_t magic, version;
     uint32_t L, H, D;
@@ -184,7 +197,10 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
  * coder = header.version - 1 of the containers (one call, one coder).
  * status_out: NULL, or DEVICE / mapped-host uint32[n_chunks], zeroed by the call and then OR-ed with
  *   1 = a rANS stream did not return to its initial state (payload or CDF bytes damaged),
- *   2 = stream offsets beyond the payload (lengths section damaged); valid once the stream has run.
+ *   2 = stream offsets beyond the payload (lengths section damaged); valid once the stream has run,
+ *   4 = the container's header.version is not the one `coder` names (B200KV_CODER_RANS_COMPACT | B200KV_KV_LATENT: 4).
+ *       The call cannot read the headers before it returns, so it trusts `coder`; a container of another version (e.g.
+ *       version 3 into a latent destination) is decoded as if it were one and flagged here: treat it as a miss.
  */
 int b200kv_decode_chunks(const void* containers, int64_t containers_bytes, const int64_t* offsets,
                          const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,

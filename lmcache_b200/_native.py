@@ -20,6 +20,8 @@ CODER_AC = 0       # container version 1: arithmetic coder
 CODER_RANS = 1     # container version 2: rANS
 CODER_RANS_COMPACT = 2   # container version 3: rANS streams that carry their own histogram (no CDF section), one-byte lengths
 ENCODE_HINT_MID_ENTROPY = 0x200    # B200KV_ENCODE_HINT_MID_ENTROPY
+KV_LATENT = 0x100        # B200KV_KV_LATENT: OR-ed into KvDesc.dtype (one plane per layer) and into a coder (container version 4)
+CODER_LATENT = CODER_RANS_COMPACT | KV_LATENT   # the coder argument that names container version 4
 HDR_MAX = 36             # longest version-3 stream header (4 mask bytes + 31 counts + 1 pad)
 CODERS = {"ac": CODER_AC, "rans": CODER_RANS, "rans_compact": CODER_RANS_COMPACT}
 LP = 33
@@ -211,10 +213,20 @@ def require_cuda() -> None:
 
 
 def container_layout(L: int, H: int, D: int, ntokens: int, coder: int = CODER_RANS) -> Layout:
-    """Section offsets of the container `coder` produces (versions 1 and 2 share a layout)."""
+    """Section offsets of the container `coder` produces (versions 1 and 2 share a layout; CODER_LATENT: version 4)."""
     lo = Layout()
     check(lib().b200kv_container_layout_v(L, H, D, ntokens, coder, ctypes.byref(lo)), "container_layout")
     return lo
+
+
+def coder_of_version(version: int) -> int:
+    """The coder argument that names a container version: version - 1 for versions 1 to 3, CODER_LATENT for 4."""
+    return CODER_LATENT if version == 4 else int(version) - 1
+
+
+def planes_of(version: int, L: int) -> int:
+    """Planes of a container: one per layer in version 4 (a latent KV), a (K, V) pair per layer otherwise."""
+    return L if version == 4 else 2 * L
 
 
 def nb_map(key_bins, value_bins, L: int) -> list:

@@ -59,7 +59,12 @@ class PinnedBuffer:
 
 class KvView:
     """A KV source / destination for the native library: either one strided blob tensor or the engine's
-    tuple of 2L per-layer tensors (no stack / permute / contiguous copies).  Keeps the tensors alive."""
+    tuple of 2L per-layer tensors (no stack / permute / contiguous copies).  Keeps the tensors alive.
+
+    A latent KV (multi-head latent attention, e.g. DeepSeek-V2/V3: one [T, 576] vector per token and layer, no V) is
+    one tensor per layer where a (K, V) pair would be: a [L, T, D] blob, a tuple of L [T, D] tensors, or L paged
+    [num_blocks, block_size, D] caches.  Its descriptor carries N.KV_LATENT; its L planes are coded with the key bins
+    into version-4 containers."""
 
     def __init__(self, desc: N.KvDesc, keep, ntokens: int, device: torch.device, dtype: torch.dtype,
                  fmt: str = "vllm", blob: Optional[torch.Tensor] = None):
@@ -77,6 +82,16 @@ class KvView:
     def H(self): return self.desc.H
     @property
     def D(self): return self.desc.D
+    @property
+    def latent(self) -> bool: return bool(self.desc.dtype & N.KV_LATENT)
+    @property
+    def planes(self) -> int:
+        """P: planes of the KV, L for a latent KV, 2L otherwise."""
+        return self.L if self.latent else 2 * self.L
+    @property
+    def dtype_code(self) -> int:
+        """N.DT_* of the elements (the descriptor's dtype without the latent flag)."""
+        return int(self.desc.dtype) & ~N.KV_LATENT
 
     def record_stream(self, stream: torch.cuda.Stream) -> None:
         """Mark every tensor behind the view as used by work on `stream`: the caching allocator reuses none of them
@@ -107,8 +122,30 @@ class KvView:
         return blob.shape[0], blob.shape[3 if fmt == "vllm" else 2], blob.shape[4], blob.dtype
 
     @staticmethod
+    def _latent_desc(L: int, D: int, dtype: torch.dtype) -> N.KvDesc:
+        d = N.KvDesc()
+        d.sKV = 0
+        d.L, d.H, d.D = L, 1, D
+        d.dtype = KvView._code(dtype) | N.KV_LATENT
+        return d
+
+    @staticmethod
     def from_blob(blob: torch.Tensor, fmt: str) -> "KvView":
-        """blob: [L,2,T,H,D] (vllm) or [L,2,H,T,D] (huggingface); any strides with a contiguous last dim."""
+        """blob: [L,2,T,H,D] (vllm) or [L,2,H,T,D] (huggingface); any strides with a contiguous last dim.
+        A latent KV: [L,T,D] (vllm format only)."""
+        if blob.dim() == 3:
+            if fmt != "vllm":
+                raise ValueError("a latent KV blob [L,T,D] has the vllm format only")
+            if not blob.is_cuda:
+                raise RuntimeError("KV blob must live on a CUDA device (no CPU fallback)")
+            if blob.stride(2) != 1:
+                blob = blob.contiguous()
+            L, T, D = blob.shape
+            d = KvView._latent_desc(L, D, blob.dtype)
+            d.base = blob.data_ptr()
+            d.planes = None
+            d.sL, d.sT, d.sH = blob.stride(0), blob.stride(1), D
+            return KvView(d, blob, T, blob.device, blob.dtype, fmt, blob)
         if blob.dim() != 5 or blob.shape[1] != 2:
             raise ValueError(f"expected a [L,2,..] KV blob, got {tuple(blob.shape)}")
         if not blob.is_cuda:
@@ -133,10 +170,13 @@ class KvView:
 
     @staticmethod
     def from_tuple(kv: Sequence[Tuple[torch.Tensor, torch.Tensor]], fmt: str) -> "KvView":
-        """kv: L pairs of [T,H,D] (vllm) / [H,T,D] (huggingface) tensors, as passed to LMCacheEngine.store."""
+        """kv: L pairs of [T,H,D] (vllm) / [H,T,D] (huggingface) tensors, as passed to LMCacheEngine.store; or, for a
+        latent KV, L [T,D] tensors (vllm format only)."""
         L = len(kv)
         if L == 0:
             raise ValueError("Empty kv_tensors")
+        if isinstance(kv[0], torch.Tensor):
+            return KvView._from_latent_tuple(kv, fmt)
         ref = kv[0][0]
         if not ref.is_cuda:
             raise RuntimeError("KV tensors must live on a CUDA device (no CPU fallback)")
@@ -170,19 +210,68 @@ class KvView:
         return KvView(d, (keep, ptrs), T, ref.device, ref.dtype, fmt)
 
     @staticmethod
+    def _from_latent_tuple(kv: Sequence[torch.Tensor], fmt: str) -> "KvView":
+        if fmt != "vllm":
+            raise ValueError("a latent KV has the vllm format only")
+        ref = kv[0]
+        if not ref.is_cuda:
+            raise RuntimeError("KV tensors must live on a CUDA device (no CPU fallback)")
+        if ref.dim() != 2:
+            raise ValueError(f"a latent KV takes one [T,D] tensor per layer, got {tuple(ref.shape)}")
+        if any(t.shape != ref.shape or t.dtype != ref.dtype or t.device != ref.device for t in kv):
+            raise ValueError("all latent tensors must share shape, dtype and device")
+        kv = [t if t.stride(1) == 1 else t.contiguous() for t in kv]
+        if any(t.stride() != kv[0].stride() for t in kv):
+            kv = [t.contiguous() for t in kv]
+        L, (T, D) = len(kv), ref.shape
+        ptrs = (ctypes.c_void_p * L)(*[t.data_ptr() for t in kv])
+        d = KvView._latent_desc(L, D, ref.dtype)
+        d.base = None
+        d.planes = ctypes.cast(ptrs, ctypes.POINTER(ctypes.c_void_p))
+        d.sL = 0
+        d.sT, d.sH = kv[0].stride(0), D
+        return KvView(d, (list(kv), ptrs), T, ref.device, ref.dtype, fmt)
+
+    @staticmethod
+    def _from_latent_paged(kv_caches: Sequence[torch.Tensor], slot_mapping: torch.Tensor) -> "KvView":
+        ref = kv_caches[0]
+        if not ref.is_cuda:
+            raise RuntimeError("KV caches must live on a CUDA device (no CPU fallback)")
+        if ref.dim() not in (2, 3):
+            raise ValueError(f"a latent paged cache is [num_blocks, block_size, D] or [num_slots, D], got "
+                             f"{tuple(ref.shape)}")
+        for t in kv_caches:
+            if t.shape != ref.shape or t.dtype != ref.dtype or t.device != ref.device:
+                raise ValueError("all latent caches must share shape, dtype and device")
+            if not t.is_contiguous():
+                raise ValueError("paged latent caches must be contiguous (they are written in place)")
+        L, D = len(kv_caches), ref.shape[-1]
+        ptrs = (ctypes.c_void_p * L)(*[t.data_ptr() for t in kv_caches])
+        d = KvView._latent_desc(L, D, ref.dtype)
+        d.base = None
+        d.planes = ctypes.cast(ptrs, ctypes.POINTER(ctypes.c_void_p))
+        d.sL = 0
+        d.sT, d.sH = D, D
+        d.slot_map = slot_mapping.data_ptr()
+        return KvView(d, ([slot_mapping] + list(kv_caches), ptrs), slot_mapping.numel(), ref.device, ref.dtype, "vllm")
+
+    @staticmethod
     def from_paged(kv_caches: Sequence[Tuple[torch.Tensor, torch.Tensor]], slot_mapping: torch.Tensor) -> "KvView":
         """vLLM's paged KV cache used in place: `kv_caches` holds, per layer, the (key_cache, value_cache) pair shaped
         [num_blocks, block_size, H, D] (or already flattened [num_slots, H, D]); `slot_mapping` (int64, CUDA) gives the
         cache row of every token of the sequence (block * block_size + offset) -- what lmcache-vllm's
         lmcache_store_kv / lmcache_retrieve_kv gather and scatter with torch indexing (LLM_Engine.rst:91-109).
         The codec kernels read (encode) and write (decode) the rows directly; token i of the view is row
-        slot_mapping[i]."""
+        slot_mapping[i].  A latent KV (vLLM's MLA cache): one [num_blocks, block_size, D] (or [num_slots, D]) tensor per
+        layer instead of a pair."""
         L = len(kv_caches)
         if L == 0:
             raise ValueError("Empty kv_caches")
         if slot_mapping.dtype != torch.int64 or not slot_mapping.is_cuda or slot_mapping.dim() != 1:
             raise ValueError("slot_mapping must be a 1-D int64 CUDA tensor")
         slot_mapping = slot_mapping.contiguous()
+        if isinstance(kv_caches[0], torch.Tensor):
+            return KvView._from_latent_paged(kv_caches, slot_mapping)
         ref = kv_caches[0][0]
         if not ref.is_cuda:
             raise RuntimeError("KV caches must live on a CUDA device (no CPU fallback)")
@@ -212,7 +301,7 @@ class KvView:
         b200kv_pack_chunks launch on the current stream.  Returns the buffer and the blobs, back to back views of it."""
         n_tok = self.ntokens - tok_begin
         n_chunks = (n_tok + chunk_size - 1) // chunk_size
-        per_tok = 2 * self.L * self.H * self.D
+        per_tok = self.planes * self.H * self.D
         stride = per_tok * chunk_size
         buf = torch.empty(n_chunks * stride, dtype=self.dtype, device=self.device)
         with torch.cuda.device(self.device):
@@ -221,76 +310,80 @@ class KvView:
                                                ctypes.c_void_p(buf.data_ptr()), stride * buf.element_size(),
                                                _stream_ptr(None)), "pack_chunks")
         sizes = [min(chunk_size, n_tok - j * chunk_size) for j in range(n_chunks)]
-        return buf, [buf[j * stride: j * stride + per_tok * t].view(self.blob_shape(self.fmt, self.L, self.H, self.D, t))
-                     for j, t in enumerate(sizes)]
+        shape = (lambda t: (self.L, t, self.D)) if self.latent else \
+            (lambda t: self.blob_shape(self.fmt, self.L, self.H, self.D, t))
+        return buf, [buf[j * stride: j * stride + per_tok * t].view(shape(t)) for j, t in enumerate(sizes)]
 
 
 def parse_header(buf, total: Optional[int] = None) -> N.Header:
     """Validate and return the 64-byte header of a B2KV container (bytes / bytearray / memoryview).  `buf` is the whole
     container, or -- when `total`, the size of the whole container, is given -- a prefix of it that holds the header
-    and, for version 3, the nb map after it."""
+    and, for versions 3 and 4, the nb map after it."""
     mv = memoryview(buf)
     if mv.nbytes < N.HEADER_BYTES:
         raise ValueError("buffer too small for a B2KV container")
     hd = N.Header.from_buffer_copy(bytes(mv[:N.HEADER_BYTES]))
     if hd.magic != N.MAGIC:
         raise ValueError("not a B2KV container (bad magic)")
-    if hd.version not in (1, 2, 3):
+    if hd.version not in (1, 2, 3, 4):
         raise ValueError(f"unsupported B2KV version {hd.version}")
     if hd.total_bytes > (mv.nbytes if total is None else total):
         raise ValueError("truncated B2KV container")
     if hd.status != 0:
         raise ValueError(f"B2KV container carries encoder error status {hd.status}")
     nb = None
-    if hd.version == 3:
-        if not 0 < hd.L <= N.MAX_PLANES // 2 or mv.nbytes < N.HEADER_BYTES + 2 * hd.L:
+    if hd.version >= 3:
+        P = N.planes_of(hd.version, hd.L)
+        if not 0 < hd.L <= N.MAX_PLANES // 2 or mv.nbytes < N.HEADER_BYTES + P:
             raise ValueError("B2KV header carries an impossible shape")
-        nb = list(bytes(mv[N.HEADER_BYTES:N.HEADER_BYTES + 2 * hd.L]))
+        nb = list(bytes(mv[N.HEADER_BYTES:N.HEADER_BYTES + P]))
     check_header(hd, nb)
     return hd
 
 
 def plane_offsets(buf) -> Optional[np.ndarray]:
-    """Boundaries of the planes' streams in a version-3 container (`buf`: at least its fixed sections), from its
-    half-lengths section: int64[2L + 1], plane p (keys of layer p, then values of layer p - L) is bytes [o[p], o[p + 1])
-    of the container; o[0] is the start of the payload and o[2L] == total_bytes.  None for versions 1 and 2, and when the
-    lengths do not add up to the header's payload (a damaged container: it is only ever uploaded whole)."""
+    """Boundaries of the planes' streams in a version-3 or version-4 container (`buf`: at least its fixed sections), from
+    its half-lengths section: int64[P + 1] (P = 2L planes, keys of layer p then values of layer p - L; P = L latent
+    planes in version 4), plane p is bytes [o[p], o[p + 1]) of the container; o[0] is the start of the payload and
+    o[P] == total_bytes.  None for versions 1 and 2, and when the lengths do not add up to the header's payload (a
+    damaged container: it is only ever uploaded whole)."""
     src = np.frombuffer(buf, dtype=np.uint8)
     version, L = (int(v) for v in src[4:12].view(np.uint32))
-    if version != 3:
+    if version not in (3, 4):
         return None
-    o = np.empty(2 * L + 1, dtype=np.int64)
+    o = np.empty(N.planes_of(version, L) + 1, dtype=np.int64)
     rc = N.check(N.lib().b200kv_plane_offsets(src.ctypes.data, src.size, o.ctypes.data, o.size), "plane_offsets")
     return o if rc == 0 else None
 
 
 def container_layout_of(hd: "N.Header") -> "N.Layout":
     """Section offsets of a parsed container."""
-    return N.container_layout(hd.L, hd.H, hd.D, hd.ntokens, int(hd.version) - 1)
+    return N.container_layout(hd.L, hd.H, hd.D, hd.ntokens, N.coder_of_version(hd.version))
 
 
 def check_header(hd: "N.Header", nb: Optional[Sequence[int]] = None) -> None:
     """Structural checks that make a damaged blob a miss (ValueError) instead of bad device addresses: the section
     offsets follow from (L, H, D, ntokens, version), so total_bytes must be exactly fixed sections + payload.  A compact
-    container (version 3) also carries its nb map -- the 2L bytes after the header, passed as `nb` and attached to the
-    header as `hd.nb`: the symbols per plane its writer's bin table allowed."""
+    container (version 3, or 4 for a latent KV) also carries its nb map -- the P bytes after the header (P = 2L, or L),
+    passed as `nb` and attached to the header as `hd.nb`: the symbols per plane its writer's bin table allowed."""
     if not (0 < hd.L <= N.MAX_PLANES // 2 and hd.H > 0 and hd.D > 0 and hd.ntokens > 0):
         raise ValueError("B2KV header carries an impossible shape")
     if hd.max_dtype not in (N.DT_BF16, N.DT_FP16):
         raise ValueError("B2KV header carries an unknown max_dtype")
     hd.nb = None
-    if hd.version == 3:
-        if nb is None or len(nb) != 2 * hd.L or any(v < 4 or v > 32 or v % 2 for v in nb):
-            raise ValueError("B2KV v3 header: bad nb map")
+    P = N.planes_of(hd.version, hd.L)
+    if hd.version >= 3:
+        if nb is None or len(nb) != P or any(v < 4 or v > 32 or v % 2 for v in nb):
+            raise ValueError(f"B2KV v{hd.version} header: bad nb map")
         if hd.ntokens > N.GROUP_TOKENS:
-            raise ValueError("B2KV v3 header: more than 256 tokens")
+            raise ValueError(f"B2KV v{hd.version} header: more than 256 tokens")
         hd.nb = [int(v) for v in nb]
     lo = container_layout_of(hd)
     if hd.ngroups != (hd.ntokens + N.GROUP_TOKENS - 1) // N.GROUP_TOKENS:
         raise ValueError("B2KV header: ngroups does not match ntokens")
     if hd.total_bytes != lo.off_payload + hd.payload_bytes:
         raise ValueError("B2KV header: total_bytes != fixed sections + payload_bytes (truncated or corrupt)")
-    nstreams = 2 * hd.L * hd.H * hd.D * hd.ngroups
+    nstreams = P * hd.H * hd.D * hd.ngroups
     per_stream = 1 if hd.version == 1 else 4          # rANS streams are >= 4 bytes, arithmetic-coder streams >= 1
     if hd.payload_bytes < per_stream * nstreams or hd.payload_bytes > lo.max_total_bytes:
         raise ValueError("B2KV header: payload_bytes impossible for this shape")
@@ -397,8 +490,14 @@ class CacheGenCodec:
             t = torch.empty(int(nbytes), dtype=torch.uint8, device=device)
         return t
 
-    def coder_for(self, chunk_tokens: int) -> int:
-        """The container this codec writes for chunks of `chunk_tokens`: the compact one holds <= 256 tokens."""
+    def coder_for(self, chunk_tokens: int, latent: bool = False) -> int:
+        """The container this codec writes for chunks of `chunk_tokens`: the compact one holds <= 256 tokens.  A latent
+        KV is written as version 4 (N.CODER_LATENT), which exists for the compact coder and <= 256 tokens only."""
+        if latent:
+            if self.coder != N.CODER_RANS_COMPACT or chunk_tokens > N.GROUP_TOKENS:
+                raise ValueError(f"a latent KV is coded into version-4 containers: coder 'rans_compact' and chunks of "
+                                 f"at most {N.GROUP_TOKENS} tokens only")
+            return N.CODER_LATENT
         if self.coder == N.CODER_RANS_COMPACT and chunk_tokens > N.GROUP_TOKENS:
             if self.v3_only:
                 raise ValueError(f"chunks of {chunk_tokens} tokens: with cachegen_config the containers are version 3, "
@@ -406,32 +505,42 @@ class CacheGenCodec:
             return N.CODER_RANS
         return self.coder
 
-    def layout(self, L: int, H: int, D: int, chunk_tokens: int) -> "N.Layout":
-        return N.container_layout(L, H, D, chunk_tokens, self.coder_for(chunk_tokens))
+    def layout(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> "N.Layout":
+        return N.container_layout(L, H, D, chunk_tokens, self.coder_for(chunk_tokens, latent))
 
-    def accepts(self, hd: "N.Header") -> bool:
-        """Can this codec decode the container?  A compact container must have been written with this model's bins; a
-        codec made from a cachegen_config reads compact containers only (the others do not say which bins they used)."""
+    def accepts(self, hd: "N.Header", latent: bool = False) -> bool:
+        """Can this codec decode the container into a destination of one plane per layer (`latent`) or of (K, V) pairs?
+        The container's plane layout must be the destination's: version 4 for a latent destination, versions 1 to 3
+        otherwise.  A compact container must have been written with this model's bins (a latent plane with the key
+        bins); a codec made from a cachegen_config reads compact containers only (the others do not say which bins they
+        used)."""
+        if (hd.version == 4) != latent:
+            return False
+        n = self.nlayers
+        if hd.version == 4:
+            return hd.L <= n and hd.nb == self._nb[:hd.L]
         if hd.version != 3:
             return not self.v3_only
-        n = self.nlayers
         return hd.L <= n and hd.nb == self._nb[:hd.L] + self._nb[n:n + hd.L]
 
-    def max_container_bytes(self, L: int, H: int, D: int, chunk_tokens: int) -> int:
+    def max_container_bytes(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> int:
         """Upper bound of a container of ANY version this codec can decode (what a receive slab must reserve when the
-        writer may have been configured differently): version 2's sections are the largest."""
+        writer may have been configured differently): version 2's sections are the largest.  A latent KV (one plane per
+        layer) is read from version 4 only: that container's own bound."""
+        if latent:
+            return self.out_stride(L, H, D, chunk_tokens, latent=True)
         lo = N.container_layout(L, H, D, chunk_tokens)
         if chunk_tokens <= N.GROUP_TOKENS:
             return (lo.fixed_bytes + 2 * L * H * D * (chunk_tokens + 4) + 16 + 15) & ~15
         return lo.max_total_bytes
 
-    def out_stride(self, L: int, H: int, D: int, chunk_tokens: int) -> int:
+    def out_stride(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> int:
         """Bytes reserved per container.  Chunks of <= 256 tokens are coded with their own empirical CDF,
         so a stream costs <= 8 bits/symbol (+ flush); larger chunks may reach 16 bits/symbol."""
-        lo = self.layout(L, H, D, chunk_tokens)
+        lo = self.layout(L, H, D, chunk_tokens, latent)
         if chunk_tokens <= N.GROUP_TOKENS:
-            hdr = N.HDR_MAX if self.coder_for(chunk_tokens) == N.CODER_RANS_COMPACT else 0
-            return (lo.fixed_bytes + 2 * L * H * D * (chunk_tokens + 4 + hdr) + 16 + 15) & ~15
+            hdr = N.HDR_MAX if self.coder_for(chunk_tokens, latent) & 0xff == N.CODER_RANS_COMPACT else 0
+            return (lo.fixed_bytes + (1 if latent else 2) * L * H * D * (chunk_tokens + 4 + hdr) + 16 + 15) & ~15
         return lo.max_total_bytes
 
     # ------------------------------------------------------------------ encode
@@ -450,11 +559,11 @@ class CacheGenCodec:
             raise ValueError(f"KV has {view.L} layers but the bin table of this model has {self.nlayers}")
         n_chunks = (n_tokens + chunk_size - 1) // chunk_size
         last = n_tokens - (n_chunks - 1) * chunk_size
-        stride = self.out_stride(view.L, view.H, view.D, chunk_size)
+        stride = self.out_stride(view.L, view.H, view.D, chunk_size, view.latent)
         lib = N.lib()
         with self._enc_lock, torch.cuda.device(view.device):
             tstream = stream if stream is not None else torch.cuda.current_stream()
-            coder = self.coder_for(chunk_size)
+            coder = self.coder_for(chunk_size, view.latent)
             ws_bytes = lib.b200kv_encode_workspace_bytes(view.L, view.H, view.D, chunk_size, n_chunks, coder)
             own_out, own_sizes = out is None, sizes is None
             need_out = stride * n_chunks + N.READ_SLACK if own_out else 0
@@ -482,8 +591,8 @@ class CacheGenCodec:
             # KV statistics of one model are stable from call to call: the previous call's measured entropy picks the
             # compaction kernel's shared-memory stage size for this one (byte-identical output either way)
             # (the threshold is in coder bits per symbol; a version-3 payload also holds ~0.4 bits of stream headers)
-            b = self._last_bits_per_symbol - (0.4 if coder == N.CODER_RANS_COMPACT else 0.0)
-            flags = coder | (N.ENCODE_HINT_MID_ENTROPY if b > 1.2 else 0)
+            b = self._last_bits_per_symbol - (0.4 if coder & 0xff == N.CODER_RANS_COMPACT else 0.0)
+            flags = (coder & 0xff) | (N.ENCODE_HINT_MID_ENTROPY if b > 1.2 else 0)   # the descriptor says latent
             N.check(lib.b200kv_encode_chunks(ctypes.byref(view.desc), tok_begin, n_chunks, chunk_size, last,
                                              self._kb, self._vb, flags, out.data_ptr(), stride, sizes.dev_ptr,
                                              self._enc_ws.data_ptr(), self._enc_ws.numel(), tstream.cuda_stream),
@@ -491,9 +600,9 @@ class CacheGenCodec:
             ev = torch.cuda.Event()
             ev.record(tstream)
             self._enc_event = ev
-            fixed = self.layout(view.L, view.H, view.D, chunk_size).fixed_bytes
-            return EncodeTicket(out, stride, n_chunks, sizes, ev, int(view.desc.dtype), coder, view, self,
-                                (fixed, 2.0 * view.L * view.H * view.D * n_tokens))
+            fixed = self.layout(view.L, view.H, view.D, chunk_size, view.latent).fixed_bytes
+            return EncodeTicket(out, stride, n_chunks, sizes, ev, view.dtype_code, coder, view, self,
+                                (fixed, float(view.planes) * view.H * view.D * n_tokens))
 
     def encode(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int,
                stream: Optional[torch.cuda.Stream] = None, out: Optional[torch.Tensor] = None) -> EncodedBatch:
@@ -681,8 +790,9 @@ class CacheGenCodec:
 
     def decode_status(self) -> List[int]:
         """Wait for the most recent decode call and return its per-chunk status words (0 = clean; bit 0: a rANS stream
-        did not return to its initial state, bit 1: stream offsets beyond the payload).  A nonzero word means the
-        container's bytes were damaged after its header was written: treat the chunk as a miss."""
+        did not return to its initial state, bit 1: stream offsets beyond the payload, bit 2: the header's version is not
+        the one the call's coder named).  A nonzero word means the container's bytes were damaged after its header was
+        written, or it was handed to the wrong decode: treat the chunk as a miss."""
         with self._dec_lock:
             if self._dec_status is None or self._dec_event is None:
                 return []
@@ -709,8 +819,11 @@ class CacheGenCodec:
                 hd = parse_header(c[:N.HEADER_BYTES + N.MAX_PLANES].cpu().numpy().tobytes(), c.numel())
             else:
                 hd = parse_header(c)
-            if not self.accepts(hd):
-                raise ValueError("compact container written with another model's bins" if hd.version == 3 else
+            if (hd.version == 4) != dst.latent:
+                raise ValueError(f"a version-{hd.version} container does not fit a destination of "
+                                 f"{'one plane' if dst.latent else 'a (K, V) pair'} per layer")
+            if not self.accepts(hd, dst.latent):
+                raise ValueError("compact container written with another model's bins" if hd.version >= 3 else
                                  f"a codec made from a cachegen_config reads version 3 only, not version {hd.version}")
             if (hd.L, hd.H, hd.D) != (dst.L, dst.H, dst.D):
                 raise ValueError(f"container shape L/H/D={hd.L}/{hd.H}/{hd.D} does not match destination "
@@ -719,7 +832,7 @@ class CacheGenCodec:
         max_dtype = heads[0].max_dtype
         if any(h.max_dtype != max_dtype or h.version != heads[0].version for h in heads):
             raise ValueError("containers of one decode call must share max_dtype and container version")
-        coder = int(heads[0].version) - 1
+        coder = N.coder_of_version(heads[0].version)
         totals = [int(h.total_bytes) for h in heads]
         ntoks = [int(h.ntokens) for h in heads]
         tmax = max(ntoks)

@@ -794,9 +794,10 @@ struct Layout {
 // and every stream carries that histogram in front of its rANS bytes (stream header, below); a stream's byte length
 // (even, <= 230) is stored halved in one byte.  nb(plane) = 2 * (bins // 2) is the number of symbols a plane can emit.
 // off_cdf is the first byte after the header in both layouts (the nb map in version 3).
-B2_HD Layout make_layout(int L, int C, int t, int compact = 0) {
+// ppl: planes per layer, 2 (keys, values) or 1 (a latent KV: version 4 is the compact layout with L planes).
+B2_HD Layout make_layout(int L, int C, int t, int compact = 0, int ppl = 2) {
     Layout lo;
-    const int64_t NL = 2 * (int64_t)L;
+    const int64_t NL = (int64_t)ppl * L;
     lo.ngroups = (t + kGroup - 1) / kGroup;
     lo.off_cdf = 64;
     if (compact) {

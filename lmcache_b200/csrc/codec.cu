@@ -56,6 +56,7 @@ struct EncParams {
     int32_t stage_bytes;                                       // compact_kernel: bytes of shared-memory stage per CTA
     int32_t coder;                                             // CODER_AC | CODER_RANS (the payload coder)
     int32_t compact;                                           // 1 = container version 3 (histogram in the stream, u8 half-lengths)
+    int32_t ppl;                                               // planes per layer: 2 (K, V) or 1 (latent KV, version 4)
     uint8_t* out;
     int64_t out_stride;
     uint64_t* sizes_out;
@@ -78,7 +79,8 @@ struct EncParams {
 };
 static_assert(sizeof(EncParams) < kMaxParamBytes, "EncParams must stay under 4 KB of kernel parameters");
 
-// plane of the launch's local plane index: K planes lb.., then V planes L + lb.. (the identity when lb = 0, nlay = L)
+// plane of the launch's local plane index: K planes lb.., then V planes L + lb.. (the identity when lb = 0, nlay = L).
+// A latent KV (ppl = 1) has local < nlay throughout: planes lb..
 __device__ __forceinline__ int launch_plane(const EncParams& P, int local) {
     return local + (local < P.nlay ? P.lb : P.L - P.nlay + P.lb);
 }
@@ -86,7 +88,7 @@ __device__ __forceinline__ int launch_plane(const EncParams& P, int local) {
 // section offsets of a container of this call (encode and decode parameter blocks alike)
 template <class Prm>
 __device__ __forceinline__ Layout layout_of(const Prm& P, int t) {
-    return make_layout(P.L, P.C, t, P.compact);
+    return make_layout(P.L, P.C, t, P.compact, P.ppl);
 }
 
 // stream lengths section: int32 bytes (versions 1, 2) or u8 bytes / 2 (version 3: header + rANS stream, even, <= 230 bytes)
@@ -168,7 +170,7 @@ template <bool VEC, bool PAGED>
 __global__ void __launch_bounds__(256) absmax_kernel(EncParams P, int64_t total_tokens) {
     const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
-    const int64_t nrows = (int64_t)2 * P.nlay * total_tokens;
+    const int64_t nrows = (int64_t)P.ppl * P.nlay * total_tokens;
     if (warp >= nrows) return;
     const int nl = launch_plane(P, (int)(warp / total_tokens));
     const int64_t T = warp % total_tokens;
@@ -228,11 +230,11 @@ __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* s_warp
 
 // tile -> (chunk j, group g, plane nl, channel tile ct); tiles of a chunk are ordered (g, nl, ct), which is the
 // order of the streams in the container payload.  Returns false for tiles beyond the (ragged) last chunk.
-// A launch over layers [lb, lb + nlay) has tiles_full = 2 * nlay * tpp tiles per chunk (one group: v3 only); its
+// A launch over layers [lb, lb + nlay) has tiles_full = ppl * nlay * tpp tiles per chunk (one group: v3 / v4 only); its
 // tile_in_chunk counts the launch's tiles, and the local plane maps to the real one with one select (launch_plane).
 struct TileId { int j, g, nl, ct, t, tok0, gt, tile_in_chunk; };
 __device__ __forceinline__ bool decode_tile(const EncParams& P, uint32_t tile, TileId* id) {
-    const uint32_t per_group = 2u * P.nlay * P.tpp;
+    const uint32_t per_group = (uint32_t)P.ppl * P.nlay * P.tpp;
     const uint32_t j = tile / (uint32_t)P.tiles_full;
     const uint32_t rem = tile - j * (uint32_t)P.tiles_full;
     id->j = (int)j;
@@ -371,7 +373,7 @@ __global__ void __launch_bounds__(CT, FUSED ? 7 : 4) encode_kernel(EncParams P) 
     const int tid = threadIdx.x;
     TileId id;
     if (!decode_tile(P, blockIdx.x, &id)) return;
-    const int NL = 2 * P.L;
+    const int NL = P.ppl * P.L;
     const int j = id.j, nl = id.nl, ct = id.ct, t = id.t, gt = id.gt;
     const int c = ct * CT + tid;
     const bool active = c < P.C;
@@ -631,7 +633,7 @@ __global__ void __launch_bounds__(CT) cdf_kernel(EncParams P) {
     uint32_t* cnts = smem;                                        // CT * PAIRW counters
     float* fac = reinterpret_cast<float*>(cnts + CT * PAIRW);     // kGroup
     const int tid = threadIdx.x;
-    const int NL = 2 * P.L;
+    const int NL = P.ppl * P.L;
     const uint32_t per_chunk = (uint32_t)NL * P.tpp;
     const uint32_t j = blockIdx.x / per_chunk;
     const uint32_t rem = blockIdx.x - j * per_chunk;
@@ -682,7 +684,7 @@ __global__ void __launch_bounds__(1024) enc_scan_kernel(EncParams P) {
     __shared__ unsigned long long s_carry;
     const int j = blockIdx.x;
     const int t = chunk_tokens_of(P, j);
-    const int ntiles = ((t + kGroup - 1) / kGroup) * 2 * P.nlay * P.tpp;
+    const int ntiles = ((t + kGroup - 1) / kGroup) * P.ppl * P.nlay * P.tpp;
     uint32_t* tb = P.tile_tot + (int64_t)j * P.tiles_full;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     if (threadIdx.x == 0) s_carry = 0ull;
@@ -796,7 +798,7 @@ __global__ void __launch_bounds__(CT, 12) compact_kernel(EncParams P) {
     const int tid = threadIdx.x;
     TileId id;
     if (!decode_tile(P, blockIdx.x, &id)) return;
-    const int NL = 2 * P.L;
+    const int NL = P.ppl * P.L;
     const int c = id.ct * CT + tid;
     uint8_t* cont = P.out + (int64_t)id.j * P.out_stride;
     const Layout lo = layout_of(P, id.t);
@@ -932,14 +934,14 @@ __global__ void __launch_bounds__(1024) place_kernel(EncParams P) {
         *P.cursor = s_carry;
         *P.fail_from = s_fail;
     }
-    const int NLc = 2 * P.nlay;
+    const int NLc = P.ppl * P.nlay;
     for (int k = tid; k < P.n_chunks * NLc; k += 1024) {
         const int j = k / NLc, pl = k - j * NLc;
         const uint32_t* tb = P.tile_tot + (int64_t)j * P.tiles_full;
         const unsigned long long off = tb[pl * P.tpp];
         const unsigned long long end = pl + 1 < NLc ? (unsigned long long)tb[(pl + 1) * P.tpp] : P.totals[j];
         const unsigned long long cb = P.chunk_base[j];       // written above by this CTA
-        int64_t* row = P.seg + ((int64_t)j * 2 * P.L + launch_plane(P, pl)) * 2;
+        int64_t* row = P.seg + ((int64_t)j * P.ppl * P.L + launch_plane(P, pl)) * 2;
         row[0] = cb == ~0ull ? -1 : (int64_t)(cb + off);
         row[1] = (int64_t)(end - off);
     }
@@ -958,7 +960,8 @@ __global__ void finalize_kernel(EncParams P) {
     const Layout lo = layout_of(P, t);
     b200kv_header* hd = reinterpret_cast<b200kv_header*>(P.out + (int64_t)j * P.out_stride);
     hd->magic = B200KV_MAGIC;
-    hd->version = P.compact ? 3u : (uint32_t)P.coder + 1u;    // 1: arithmetic coder, 2: rANS, 3: rANS + compact sections
+    // 1: arithmetic coder, 2: rANS, 3: rANS + compact sections, 4: version 3 with one plane per layer (latent KV)
+    hd->version = P.compact ? (P.ppl == 1 ? 4u : 3u) : (uint32_t)P.coder + 1u;
     hd->L = P.L; hd->H = P.H; hd->D = P.D;
     hd->ntokens = t;
     hd->ngroups = lo.ngroups;
@@ -973,7 +976,7 @@ __global__ void finalize_kernel(EncParams P) {
         // output buffer held before: a container's bytes are a function of the KV alone, and no stale device memory
         // travels with it to a tier
         uint8_t* c = reinterpret_cast<uint8_t*>(hd);
-        const int64_t NL = 2 * (int64_t)P.L;
+        const int64_t NL = (int64_t)P.ppl * P.L;
         const int64_t ends[3] = {lo.off_cdf + (P.compact ? NL : NL * P.C * kLp * 2), lo.off_maxes + NL * t * 2,
                                  lo.off_lengths + (int64_t)lo.ngroups * NL * P.C * (P.compact ? 1 : 4)};
         const int64_t starts[3] = {lo.off_maxes, lo.off_lengths, lo.off_payload};
@@ -982,7 +985,7 @@ __global__ void finalize_kernel(EncParams P) {
     }
     if (P.compact) {                               // counts per stream of every plane: makes the container self-describing
         uint8_t* nbmap = reinterpret_cast<uint8_t*>(hd) + lo.off_cdf;
-        const int NL = 2 * P.L;
+        const int NL = P.ppl * P.L;
         for (int nl = 0; nl < (int)align16(NL); ++nl) nbmap[nl] = nl < NL ? (uint8_t)(2 * ((int)P.pt.maxq[nl] + 1)) : (uint8_t)0;
     }
 }
@@ -1008,7 +1011,9 @@ struct DecParams {
     int64_t sT, sH;
     const int64_t* slot_map;     // paged destination: token i lives in row slot_map[i]; NULL = row i
     int32_t L, H, D, C, out_dtype, max_dtype, n_chunks, tpp, tiles_max;   // H, C: the containers' (src_H with windows)
-    int32_t compact;             // containers are version 3
+    int32_t compact;             // containers are version 3 (or 4)
+    int32_t ppl;                 // planes per layer: 2 (K, V) or 1 (latent KV, version 4)
+    int32_t version;             // the header version the coder (and the destination's planes) name: status bit 2 if not
     int32_t lb, nlay;            // decode_kernel: this launch decodes layers [lb, lb + nlay), i.e. planes lb.. and L + lb..
     int32_t wtpp;                // decode_kernel: tiles launched per plane = the largest window's ntw (tpp without windows)
     const DecChunk* chunks;      // device
@@ -1036,7 +1041,12 @@ __global__ void __launch_bounds__(128) tile_sum_kernel(DecParams P) {
     const int tile = blockIdx.x * 4 + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     const DecChunk dc = P.chunks[j];
-    const int NL = 2 * P.L;
+    // the header is part of the fixed sections: a container of another version than the call's coder (e.g. version 3
+    // handed to a latent destination) is flagged, so the caller drops the chunk as a miss
+    if (blockIdx.x == 0 && threadIdx.x == 0 && P.status != nullptr &&
+        reinterpret_cast<const uint32_t*>(dc.base)[1] != (uint32_t)P.version)
+        atomicOr(&P.status[j], 4u);
+    const int NL = P.ppl * P.L;
     const int ntiles = dc.ngroups * NL * P.tpp;
     if (tile >= ntiles) return;
     const int plane_row = tile / P.tpp;          // g * NL + nl
@@ -1055,7 +1065,7 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(DecParams P) {
     __shared__ unsigned long long s_carry;
     const int j = blockIdx.x;
     const DecChunk dc = P.chunks[j];
-    const int ntiles = dc.ngroups * 2 * P.L * P.tpp;
+    const int ntiles = dc.ngroups * P.ppl * P.L * P.tpp;
     unsigned long long* tb = P.tile_base + (int64_t)j * P.tiles_max;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     if (threadIdx.x == 0) s_carry = 0ull;
@@ -1085,11 +1095,11 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(DecParams P) {
     }
 }
 
-// Plane boundaries of version-3 containers in device memory (b200kv_plane_offsets_device): one CTA of 32 warps per
-// container, one warp per plane at a time, 16-byte loads (the sum is a handful of independent loads per lane, not a chain
-// of byte loads: it runs on the store worker's copy stream, in front of the wave's device->host copies).  out row j:
-// [off_payload, end of plane 0, ..., end of plane 2L-1 = total_bytes], or -1 in entry 0 when the container is not
-// version 3 or its half-lengths do not add up to total_bytes.
+// Plane boundaries of version-3 / version-4 containers in device memory (b200kv_plane_offsets_device): one CTA of 32
+// warps per container, one warp per plane at a time, 16-byte loads (the sum is a handful of independent loads per lane,
+// not a chain of byte loads: it runs on the store worker's copy stream, in front of the wave's device->host copies).  out
+// row j: [off_payload, end of plane 0, ..., end of plane P-1 = total_bytes] (P = 2L, or L for version 4), or -1 in entry 0
+// when the container is neither or its half-lengths do not add up to total_bytes.
 __global__ void __launch_bounds__(1024) plane_offsets_kernel(const uint8_t* base, int64_t stride, int64_t* out) {
     __shared__ uint32_t s_sum[B200KV_MAX_PLANES];
     const uint8_t* c = base + (int64_t)blockIdx.x * stride;
@@ -1100,21 +1110,22 @@ __global__ void __launch_bounds__(1024) plane_offsets_kernel(const uint8_t* base
     // the header alone decides whether the fixed sections lie inside the container and inside this row: nothing past the
     // header is read before that is known (the lengths section alone is 2L * C bytes, so C <= stride bounds the layout)
     const uint64_t C64 = (uint64_t)H * D;
-    if (hw[0] != B200KV_MAGIC || version != 3u || L == 0u || 2u * L > (uint32_t)B200KV_MAX_PLANES || H == 0u || D == 0u ||
-        t == 0u || t > (uint32_t)kGroup || C64 > (uint64_t)stride || C64 >= (1ull << 31)) {
+    if (hw[0] != B200KV_MAGIC || (version != 3u && version != 4u) || L == 0u || 2u * L > (uint32_t)B200KV_MAX_PLANES ||
+        H == 0u || D == 0u || t == 0u || t > (uint32_t)kGroup || C64 > (uint64_t)stride || C64 >= (1ull << 31)) {
         if (threadIdx.x == 0) o[0] = -1;
         return;
     }
-    const int NL = 2 * (int)L;
+    const int ppl = version == 4u ? 1 : 2;
+    const int NL = ppl * (int)L;
     const int64_t C = (int64_t)C64;
-    const Layout lo = make_layout((int)L, (int)C, (int)t, 1);
+    const Layout lo = make_layout((int)L, (int)C, (int)t, 1, ppl);
     if ((uint64_t)lo.off_payload > total || lo.off_payload > stride) {
         if (threadIdx.x == 0) o[0] = -1;
         return;
     }
     const uint8_t* half = c + lo.off_lengths;                  // 16-byte aligned (container and section)
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int p = NL + 1 + (int)threadIdx.x; p <= B200KV_MAX_PLANES; p += blockDim.x) o[p] = 0;   // the row past 2L + 1
+    for (int p = NL + 1 + (int)threadIdx.x; p <= B200KV_MAX_PLANES; p += blockDim.x) o[p] = 0;   // the row past P + 1
     for (int p = warp; p < NL; p += blockDim.x >> 5) {
         const uint8_t* row = half + p * C;
         uint32_t sum = 0;
@@ -1365,12 +1376,12 @@ __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
     const int tid = threadIdx.x;
     const int j = blockIdx.y;
     const DecChunk dc = P.chunks[j];
-    const int NL = 2 * P.L;
+    const int NL = P.ppl * P.L;
     const int per_group = NL * P.tpp;
-    // blockIdx.x walks the launch's tiles of each group: K planes lb.., then V planes L + lb.., and in each plane the
-    // wtpp tiles from the chunk's window tile ct0 on (those past the window's ntw leave); `tile` is the tile's index
-    // among all of the chunk's tiles (tile_base).  Without windows ct0 = 0 and ntw = wtpp = tpp.
-    const int launch_group = 2 * P.nlay * P.wtpp;
+    // blockIdx.x walks the launch's tiles of each group: K planes lb.., then V planes L + lb.. (a latent KV: planes lb..
+    // only), and in each plane the wtpp tiles from the chunk's window tile ct0 on (those past the window's ntw leave);
+    // `tile` is the tile's index among all of the chunk's tiles (tile_base).  Without windows ct0 = 0 and ntw = wtpp = tpp.
+    const int launch_group = P.ppl * P.nlay * P.wtpp;
     const int g = blockIdx.x / launch_group;
     if (g >= dc.ngroups) return;
     const int kt = blockIdx.x - g * launch_group;
@@ -1588,9 +1599,9 @@ int make_plane_table(const b200kv_kv_desc* kv, const float* key_bins, const floa
     B2_REQUIRE(kv != nullptr, "kv descriptor is NULL");
     B2_REQUIRE(kv->L > 0 && 2 * kv->L <= B200KV_MAX_PLANES, "L out of range");
     B2_REQUIRE(kv->H > 0 && kv->D > 0, "H/D must be positive");
-    B2_REQUIRE(kv->dtype == B200KV_DT_BF16 || kv->dtype == B200KV_DT_FP16, "dtype must be bf16 or fp16");
+    B2_REQUIRE(kv_dtype(kv) == B200KV_DT_BF16 || kv_dtype(kv) == B200KV_DT_FP16, "dtype must be bf16 or fp16");
     B2_REQUIRE(kv->planes != nullptr || kv->base != nullptr, "no KV pointer");
-    for (int kvi = 0; kvi < 2; ++kvi)
+    for (int kvi = 0; kvi < kv_ppl(kv); ++kvi)
         for (int l = 0; l < kv->L; ++l) {
             const int nl = kvi * kv->L + l;
             const uint16_t* p = kv->planes ? static_cast<const uint16_t*>(kv->planes[nl])
@@ -1717,9 +1728,9 @@ constexpr int kStageRans = 12 * 1024;   // compact_kernel's stage without an ent
 // absmax over the rows of the launch's planes (P.lb, P.nlay) and tokens [0, total_tokens) of the call
 static int launch_absmax(const EncParams& P, const b200kv_kv_desc* kv, int64_t total_tokens, cudaStream_t stream) {
     bool vec = (kv->D % 8 == 0) && (kv->sT % 8 == 0) && (kv->sH % 8 == 0);
-    for (int nl = 0; nl < 2 * P.L && vec; ++nl) vec = (reinterpret_cast<uintptr_t>(P.pt.p[nl]) & 15) == 0;
+    for (int nl = 0; nl < P.ppl * P.L && vec; ++nl) vec = (reinterpret_cast<uintptr_t>(P.pt.p[nl]) & 15) == 0;
     const bool paged = P.slot_map != nullptr;
-    const int64_t rows = 2 * (int64_t)P.nlay * total_tokens;
+    const int64_t rows = (int64_t)P.ppl * P.nlay * total_tokens;
     const int64_t blocks = (rows + 7) / 8;
     B2_REQUIRE(blocks < (1ll << 31), "too many rows in one call");
     if (vec && !paged) absmax_kernel<true, false><<<(unsigned)blocks, 256, 0, stream>>>(P, total_tokens);
@@ -1730,14 +1741,14 @@ static int launch_absmax(const EncParams& P, const b200kv_kv_desc* kv, int64_t t
     return 0;
 }
 
-// chunk descriptors, tile bases, and -- for more than kInlinePlanes planes only -- the device copy of the plane table
-static size_t dec_ws_layout(int64_t tiles_max, int n_chunks, int L, size_t* off_tb, size_t* off_pt) {
+// chunk descriptors, tile bases, and -- for more than kInlinePlanes planes (NP) only -- the device copy of the plane table
+static size_t dec_ws_layout(int64_t tiles_max, int n_chunks, int NP, size_t* off_tb, size_t* off_pt) {
     size_t o = ((size_t)n_chunks * sizeof(DecChunk) + 255) & ~(size_t)255;
     *off_tb = o;
     o += (size_t)n_chunks * (size_t)tiles_max * 8;
     o = (o + 255) & ~(size_t)255;
     *off_pt = o;
-    if (2 * L > kInlinePlanes) o = (o + sizeof(PlaneTable) + 255) & ~(size_t)255;
+    if (NP > kInlinePlanes) o = (o + sizeof(PlaneTable) + 255) & ~(size_t)255;
     return o;
 }
 
@@ -1765,10 +1776,13 @@ int b200kv_container_layout(int32_t L, int32_t H, int32_t D, int32_t ntokens, b2
 
 int b200kv_container_layout_v(int32_t L, int32_t H, int32_t D, int32_t ntokens, int32_t coder, b200kv_layout* out) {
     B2_REQUIRE(out != nullptr && L > 0 && H > 0 && D > 0 && ntokens > 0, "bad shape");
+    const int ppl = (coder & B200KV_KV_LATENT) ? 1 : 2;
+    coder &= ~B200KV_KV_LATENT;
     B2_REQUIRE(coder >= CODER_AC && coder <= CODER_RANS_COMPACT, "unknown coder");
     const int compact = coder == CODER_RANS_COMPACT ? 1 : 0;
+    B2_REQUIRE(ppl == 2 || compact, "a latent KV (container version 4) is coded with B200KV_CODER_RANS_COMPACT only");
     B2_REQUIRE(!compact || ntokens <= kGroup, "the compact container holds chunks of at most 256 tokens");
-    const Layout lo = make_layout(L, H * D, ntokens, compact);
+    const Layout lo = make_layout(L, H * D, ntokens, compact, ppl);
     out->off_cdf = lo.off_cdf;
     out->off_maxes = lo.off_maxes;
     out->off_lengths = lo.off_lengths;
@@ -1776,7 +1790,7 @@ int b200kv_container_layout_v(int32_t L, int32_t H, int32_t D, int32_t ntokens, 
     out->fixed_bytes = lo.off_payload;
     // per stream per group: <= 16 bits per symbol (CDF width >= 1/65536) + termination -- 2 flush bits + pad for the
     // arithmetic coder, the 32-bit final state for rANS
-    const int64_t streams = 2 * (int64_t)L * H * D;
+    const int64_t streams = (int64_t)ppl * L * H * D;
     out->max_total_bytes = align16(lo.off_payload + streams * (2 * (int64_t)ntokens + 4 * (int64_t)lo.ngroups +
                                                               (compact ? kHdrMax : 0)) + 16);
     return 0;
@@ -1786,13 +1800,14 @@ int b200kv_plane_offsets(const void* container, int64_t nbytes, int64_t* out, in
     B2_REQUIRE(container != nullptr && out != nullptr && nbytes >= (int64_t)sizeof(b200kv_header), "bad arguments");
     b200kv_header hd;
     memcpy(&hd, container, sizeof(hd));
-    B2_REQUIRE(hd.magic == B200KV_MAGIC && hd.version == 3, "not a version-3 container");
+    B2_REQUIRE(hd.magic == B200KV_MAGIC && (hd.version == 3 || hd.version == 4), "not a version-3 or version-4 container");
     B2_REQUIRE(hd.L > 0 && 2 * (int64_t)hd.L <= B200KV_MAX_PLANES && hd.H > 0 && hd.D > 0 && hd.ntokens > 0 &&
                hd.ntokens <= (uint32_t)kGroup, "impossible shape");
-    const int NL = 2 * (int)hd.L;
+    const int ppl = hd.version == 4 ? 1 : 2;
+    const int NL = ppl * (int)hd.L;
     const int64_t C = (int64_t)hd.H * hd.D;
-    B2_REQUIRE(n_out >= NL + 1, "out must hold 2L + 1 offsets");
-    const Layout lo = make_layout((int)hd.L, (int)C, (int)hd.ntokens, 1);
+    B2_REQUIRE(n_out >= NL + 1, "out must hold P + 1 offsets (P = 2L, or L for version 4)");
+    const Layout lo = make_layout((int)hd.L, (int)C, (int)hd.ntokens, 1, ppl);
     B2_REQUIRE(nbytes >= lo.off_payload, "buffer shorter than the fixed sections");
     const uint8_t* half = static_cast<const uint8_t*>(container) + lo.off_lengths;
     int64_t o = lo.off_payload;
@@ -1818,13 +1833,15 @@ int b200kv_plane_offsets_device(const void* containers, int64_t stride, int32_t 
 int64_t b200kv_encode_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t chunk_tokens, int32_t n_chunks,
                                       int32_t coder) {
     if (L <= 0 || H <= 0 || D <= 0 || chunk_tokens <= 0 || n_chunks <= 0) return -2;
+    const int ppl = (coder & B200KV_KV_LATENT) ? 1 : 2;
     coder &= 0xff;
     const bool compact = coder == CODER_RANS_COMPACT;          // same kernels; rows hold the stream header too
     if (compact) coder = CODER_RANS;
     if (coder != CODER_AC && coder != CODER_RANS) return -2;
     if (compact && chunk_tokens > kGroup) return -2;
+    if (ppl == 1 && !compact) return -2;
     const int64_t G = (chunk_tokens + kGroup - 1) / kGroup;
-    const int64_t n_tiles = (int64_t)n_chunks * G * 2 * L * tiles_per_plane(H * D);
+    const int64_t n_tiles = (int64_t)n_chunks * G * ppl * L * tiles_per_plane(H * D);
     size_t a, b, c, d, e;
     return (int64_t)enc_ws_layout(n_tiles, n_chunks, enc_tempw(chunk_tokens <= kGroup, coder, compact), coder, compact, &a, &b, &c, &d, &e);
 }
@@ -1832,9 +1849,9 @@ int64_t b200kv_encode_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t c
 int64_t b200kv_decode_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t chunk_tokens, int32_t n_chunks) {
     if (L <= 0 || H <= 0 || D <= 0 || chunk_tokens <= 0 || n_chunks <= 0) return -2;
     const int64_t G = (chunk_tokens + kGroup - 1) / kGroup;
-    const int64_t tiles_max = G * 2 * L * tiles_per_plane(H * D);
+    const int64_t tiles_max = G * 2 * L * tiles_per_plane(H * D);     // 2L planes: also enough for a latent KV's L
     size_t a, b;
-    return (int64_t)dec_ws_layout(tiles_max, n_chunks, L, &a, &b);
+    return (int64_t)dec_ws_layout(tiles_max, n_chunks, 2 * L, &a, &b);
 }
 
 int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
@@ -1851,6 +1868,8 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
     if (P.compact) coder = CODER_RANS;                          // version 3 = rANS payload + compact side information
     P.coder = coder;
     if (int rc = make_plane_table(kv, key_bins, value_bins, &P.pt)) return rc;
+    P.ppl = kv_ppl(kv);
+    B2_REQUIRE(P.ppl == 2 || P.compact, "a latent KV (B200KV_KV_LATENT) is coded with B200KV_CODER_RANS_COMPACT only");
     B2_REQUIRE(n_chunks > 0 && chunk_tokens > 0, "n_chunks / chunk_tokens must be positive");
     B2_REQUIRE(!P.compact || chunk_tokens <= kGroup, "the compact container (B200KV_CODER_RANS_COMPACT) holds chunks of at most 256 tokens");
     B2_REQUIRE(last_chunk_tokens > 0 && last_chunk_tokens <= chunk_tokens, "last_chunk_tokens out of range");
@@ -1860,7 +1879,7 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
     P.sT = kv->sT; P.sH = kv->sH; P.tok_begin = tok_begin;
     P.slot_map = kv->slot_map;
     const bool paged = kv->slot_map != nullptr;
-    P.L = kv->L; P.H = kv->H; P.D = kv->D; P.C = kv->H * kv->D; P.dtype = kv->dtype;
+    P.L = kv->L; P.H = kv->H; P.D = kv->D; P.C = kv->H * kv->D; P.dtype = kv_dtype(kv);
     P.n_chunks = n_chunks; P.chunk_tokens = chunk_tokens; P.last_chunk_tokens = last_chunk_tokens;
     P.tpp = tiles_per_plane(P.C);
     P.out = static_cast<uint8_t*>(out);
@@ -1869,11 +1888,11 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
     P.lb = 0; P.nlay = P.L;
     P.arena = nullptr; P.arena_bytes = 0; P.chunk_base = nullptr; P.cursor = nullptr; P.fail_from = nullptr;
     P.ptotal = nullptr; P.seg = nullptr; P.layers_left = 0;
-    const Layout lo = make_layout(P.L, P.C, chunk_tokens, P.compact);
+    const Layout lo = make_layout(P.L, P.C, chunk_tokens, P.compact, P.ppl);
     B2_REQUIRE(out_stride >= lo.off_payload + 16, "out_stride smaller than the fixed container sections");
 
     const int64_t G = lo.ngroups;
-    const int64_t per_group = 2 * (int64_t)P.L * P.tpp;
+    const int64_t per_group = (int64_t)P.ppl * P.L * P.tpp;
     const int64_t tiles_full = G * per_group;
     const int64_t n_tiles = (int64_t)n_chunks * tiles_full;     // tiles beyond a ragged last chunk exit at once
     const bool fused = chunk_tokens <= kGroup;
@@ -1984,6 +2003,7 @@ int b200kv_encode_layers_plan(const b200kv_kv_desc* kv, int64_t tok_begin, int32
     B2_REQUIRE((coder & 0xff) == CODER_RANS_COMPACT,
                "the layer-wise encode writes compact containers only (B200KV_CODER_RANS_COMPACT)");
     if (int rc = make_plane_table(kv, key_bins, value_bins, &P.pt)) return rc;
+    P.ppl = kv_ppl(kv);
     B2_REQUIRE(n_chunks > 0 && chunk_tokens > 0, "n_chunks / chunk_tokens must be positive");
     B2_REQUIRE(chunk_tokens <= kGroup, "the compact container (B200KV_CODER_RANS_COMPACT) holds chunks of at most 256 tokens");
     B2_REQUIRE(last_chunk_tokens > 0 && last_chunk_tokens <= chunk_tokens, "last_chunk_tokens out of range");
@@ -1994,14 +2014,14 @@ int b200kv_encode_layers_plan(const b200kv_kv_desc* kv, int64_t tok_begin, int32
                "fixed_out / fixed_stride must be 16-byte aligned");
     P.sT = kv->sT; P.sH = kv->sH; P.tok_begin = tok_begin;
     P.slot_map = kv->slot_map;
-    P.L = kv->L; P.H = kv->H; P.D = kv->D; P.C = kv->H * kv->D; P.dtype = kv->dtype;
+    P.L = kv->L; P.H = kv->H; P.D = kv->D; P.C = kv->H * kv->D; P.dtype = kv_dtype(kv);
     P.n_chunks = n_chunks; P.chunk_tokens = chunk_tokens; P.last_chunk_tokens = last_chunk_tokens;
     P.tpp = tiles_per_plane(P.C);
     P.coder = CODER_RANS;
     P.compact = 1;
     P.tempw = TEMPW_FUSED_RANS_HDR;
     P.stage_bytes = kStageRans;
-    const Layout lo = make_layout(P.L, P.C, chunk_tokens, 1);
+    const Layout lo = make_layout(P.L, P.C, chunk_tokens, 1, P.ppl);
     B2_REQUIRE(fixed_stride >= lo.off_payload, "fixed_stride smaller than the fixed container sections");
     P.out = static_cast<uint8_t*>(fixed_out);
     P.out_stride = fixed_stride;
@@ -2009,7 +2029,7 @@ int b200kv_encode_layers_plan(const b200kv_kv_desc* kv, int64_t tok_begin, int32
     P.arena = static_cast<uint8_t*>(arena);
     P.arena_bytes = arena_bytes;
     P.seg = seg_sizes_out;
-    const int64_t call_tiles = (int64_t)n_chunks * 2 * max_layers * P.tpp;
+    const int64_t call_tiles = (int64_t)n_chunks * P.ppl * max_layers * P.tpp;
     B2_REQUIRE(call_tiles < (1ll << 31), "too many tiles in one call");
     const EnclWs w = encl_ws_layout(n_chunks, call_tiles);
     B2_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)w.bytes, "workspace too small");
@@ -2048,7 +2068,7 @@ int b200kv_encode_layers(b200kv_encode_plan_t* plan_in, int32_t layer_begin, int
     P.lb = layer_begin;
     P.nlay = layer_end - layer_begin;
     P.layers_left = P.L - plan->done.count() - bits.count();
-    P.tiles_full = 2 * P.nlay * P.tpp;
+    P.tiles_full = P.ppl * P.nlay * P.tpp;
     const int64_t n_tiles = (int64_t)P.n_chunks * P.tiles_full;
     const int64_t total_tokens = (int64_t)(P.n_chunks - 1) * P.chunk_tokens + P.last_chunk_tokens;
     b200kv_kv_desc kv{};
@@ -2097,20 +2117,31 @@ static int decode_plan_impl(const void* containers, int64_t containers_bytes, co
     plan->magic = 0u;
     DecParams& P = plan->P;
     B2_REQUIRE(key_bins && value_bins, "bins are NULL");
+    B2_REQUIRE(dst != nullptr, "destination descriptor is NULL");
+    const bool latent = (coder & B200KV_KV_LATENT) != 0;
+    coder &= ~B200KV_KV_LATENT;
     B2_REQUIRE(coder >= CODER_AC && coder <= CODER_RANS_COMPACT, "coder must be one of B200KV_CODER_*");
+    B2_REQUIRE(!latent || coder == CODER_RANS_COMPACT, "B200KV_KV_LATENT names container version 4: rANS-compact only");
+    B2_REQUIRE(latent == (kv_ppl(dst) == 1),
+               latent ? "a version-4 (latent) container needs a latent destination (B200KV_KV_LATENT)"
+                      : "a latent destination (B200KV_KV_LATENT) takes version-4 containers only");
     P.compact = coder == CODER_RANS_COMPACT ? 1 : 0;
+    P.version = latent ? 4 : coder + 1;
     if (P.compact) coder = CODER_RANS;
+    P.ppl = kv_ppl(dst);
     PlaneTable full;
     if (int rc = make_plane_table(dst, key_bins, value_bins, &full)) return rc;
-    for (int nl = 0; nl < std::min(2 * dst->L, kInlinePlanes); ++nl) {
+    const int NP = P.ppl * dst->L;
+    for (int nl = 0; nl < std::min(NP, kInlinePlanes); ++nl) {
         P.pt.p[nl] = full.p[nl];
         P.pt.maxq[nl] = full.maxq[nl];
     }
-    P.gpt = nullptr;                         // set below, once every check has passed, when 2L > kInlinePlanes
+    P.gpt = nullptr;                         // set below, once every check has passed, when NP > kInlinePlanes
     B2_REQUIRE(containers && offsets && total_bytes && ntokens && dst_tok && n_chunks > 0, "bad chunk arrays");
     B2_REQUIRE(max_dtype == B200KV_DT_BF16 || max_dtype == B200KV_DT_FP16, "bad max_dtype");
     B2_REQUIRE(dst->sT > 0 && dst->sT < (1ll << 23), "destination token stride out of range");
     const bool windows = src_head0 != nullptr;
+    B2_REQUIRE(!windows || !latent, "head windows need a (K, V) destination: a latent KV has no heads to split");
     if (windows) {
         B2_REQUIRE(dst_head0 != nullptr && n_heads != nullptr, "head window arrays are NULL");
         B2_REQUIRE(src_H > 0 && (int64_t)src_H * dst->D < (1ll << 24), "src_H out of range");
@@ -2120,7 +2151,7 @@ static int decode_plan_impl(const void* containers, int64_t containers_bytes, co
     P.sT = dst->sT; P.sH = dst->sH;
     P.slot_map = dst->slot_map;
     P.L = dst->L; P.H = src_H; P.D = dst->D; P.C = src_H * dst->D;
-    P.out_dtype = dst->dtype; P.max_dtype = max_dtype; P.n_chunks = n_chunks;
+    P.out_dtype = kv_dtype(dst); P.max_dtype = max_dtype; P.n_chunks = n_chunks;
     P.tpp = tiles_per_plane(P.C);
     P.wtpp = P.tpp;
     P.lb = 0; P.nlay = P.L;
@@ -2153,7 +2184,7 @@ static int decode_plan_impl(const void* containers, int64_t containers_bytes, co
         B2_REQUIRE(!P.compact || ntokens[j] <= kGroup, "a compact container holds at most 256 tokens");
         B2_REQUIRE((offsets[j] & 15) == 0, "container offsets must be 16-byte aligned");
         // the fixed sections are addressed from (L, H, D, ntokens); the buffer must hold them in full
-        const Layout lj = make_layout(P.L, P.C, ntokens[j], P.compact);
+        const Layout lj = make_layout(P.L, P.C, ntokens[j], P.compact, P.ppl);
         B2_REQUIRE(total_bytes[j] >= lj.off_payload && total_bytes[j] - lj.off_payload < (1ll << 32),
                    "container shorter than its fixed sections (truncated or corrupt)");
         B2_REQUIRE(offsets[j] >= 0 && offsets[j] + total_bytes[j] + B200KV_READ_SLACK <= containers_bytes,
@@ -2161,7 +2192,7 @@ static int decode_plan_impl(const void* containers, int64_t containers_bytes, co
         tmax = ntokens[j] > tmax ? ntokens[j] : tmax;
     }
     const int64_t Gmax = (tmax + kGroup - 1) / kGroup;
-    const int64_t tiles_max = Gmax * 2 * P.L * P.tpp;
+    const int64_t tiles_max = Gmax * NP * P.tpp;
     B2_REQUIRE(tiles_max < (1ll << 31) && n_chunks <= 65535, "too many tiles / chunks in one call");
     // table layout of the rANS decoder: the conflict-free (transposed) one pays off above ~3.6 payload bits per symbol
     // (measured: row-major is faster at 0.6 bits, transposed at 4.1 bits); the containers say how
@@ -2170,9 +2201,9 @@ static int decode_plan_impl(const void* containers, int64_t containers_bytes, co
     {
         double bits = 0.0, syms = 0.0;
         for (int j = 0; j < n_chunks; ++j) {
-            const Layout lj = make_layout(P.L, P.C, ntokens[j], P.compact);
+            const Layout lj = make_layout(P.L, P.C, ntokens[j], P.compact, P.ppl);
             bits += 8.0 * (double)(total_bytes[j] - lj.off_payload);
-            syms += 2.0 * P.L * (double)P.C * ntokens[j];
+            syms += (double)NP * (double)P.C * ntokens[j];
         }
         // a version-3 payload also carries the stream histograms: ~0.5 bits per symbol at that entropy
         transposed = bits > (P.compact ? 4.1 : 3.6) * syms && bits < 6.0 * syms;   // a slot bound instead of a size says nothing: rows
@@ -2180,10 +2211,10 @@ static int decode_plan_impl(const void* containers, int64_t containers_bytes, co
     }
     P.tiles_max = (int32_t)tiles_max;
     size_t off_tb, off_pt;
-    const size_t need = dec_ws_layout(tiles_max, n_chunks, P.L, &off_tb, &off_pt);
+    const size_t need = dec_ws_layout(tiles_max, n_chunks, NP, &off_tb, &off_pt);
     B2_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)need, "workspace too small");
     uint8_t* ws = static_cast<uint8_t*>(workspace);
-    if (2 * P.L > kInlinePlanes) {           // the whole table, staged from pageable memory before the call returns
+    if (NP > kInlinePlanes) {           // the whole table, staged from pageable memory before the call returns
         B2_CHECK_CUDA(cudaMemcpyAsync(ws + off_pt, &full, sizeof(PlaneTable), cudaMemcpyHostToDevice, stream));
         P.gpt = reinterpret_cast<const PlaneTable*>(ws + off_pt);
     }
@@ -2196,7 +2227,7 @@ static int decode_plan_impl(const void* containers, int64_t containers_bytes, co
             hc[j].dst_tok = dst_tok[j];
             hc[j].t = ntokens[j];
             hc[j].ngroups = (ntokens[j] + kGroup - 1) / kGroup;
-            const Layout lj = make_layout(P.L, P.C, ntokens[j], P.compact);
+            const Layout lj = make_layout(P.L, P.C, ntokens[j], P.compact, P.ppl);
             hc[j].payload_bytes = (uint32_t)(total_bytes[j] - lj.off_payload);
             hc[j].cw0 = windows ? src_head0[j] * P.D : 0;
             hc[j].cw1 = windows ? (src_head0[j] + n_heads[j]) * P.D : P.C;
@@ -2266,7 +2297,7 @@ int b200kv_decode_layers(const b200kv_decode_plan_t* plan_in, int32_t layer_begi
     const int coder = plan->coder;
     const bool transposed = plan->transposed != 0;
     const size_t smem = (size_t)(CT * kLp + kGroup + 32) * 4;
-    dim3 grid((unsigned)((int64_t)plan->gmax * 2 * P.nlay * P.wtpp), (unsigned)P.n_chunks);
+    dim3 grid((unsigned)((int64_t)plan->gmax * P.ppl * P.nlay * P.wtpp), (unsigned)P.n_chunks);
     ProfScope prof(kProfDecode, stream);
 #define B2_LAUNCH_DEC2(DT, PAGED, CODER, TR, GT)                                                                       \
     do {                                                                                                               \

@@ -40,7 +40,12 @@ struct PlaneTableT {
 using PlaneTable = PlaneTableT<B200KV_MAX_PLANES>;
 constexpr size_t kMaxParamBytes = 4096;
 
-// Fill a PlaneTable from a kv_desc + bins; returns 0 or <0 with error set.
+// Planes per layer of a kv_desc (1 for a latent KV, B200KV_KV_LATENT) and its element dtype without the flag.
+inline int kv_ppl(const b200kv_kv_desc* kv) { return (kv->dtype & B200KV_KV_LATENT) ? 1 : 2; }
+inline int kv_dtype(const b200kv_kv_desc* kv) { return kv->dtype & ~B200KV_KV_LATENT; }
+
+// Fill a PlaneTable from a kv_desc + bins (planes kv * L + l; a latent KV's plane l takes key_bins[l]); returns 0 or <0
+// with error set.
 int make_plane_table(const b200kv_kv_desc* kv, const float* key_bins, const float* value_bins, PlaneTable* out);
 
 }  // namespace b200kv

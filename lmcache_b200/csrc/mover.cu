@@ -25,17 +25,18 @@ struct PackParams {
     int64_t sT, sH, tok_begin;
     const int64_t* slot_map;       // paged KV: token i lives in row slot_map[i]; NULL = row i
     int32_t L, H, D, n_chunks, chunk_tokens, last_chunk_tokens, hf_layout;
+    int32_t ppl;                   // planes per layer: 2 (K, V) or 1 (latent KV: chunk blob [L, t, H*D])
     uint8_t* chunks;
     int64_t chunk_stride_bytes;
 };
 static_assert(sizeof(PackParams) < kMaxParamBytes, "PackParams must stay under 4 KB of kernel parameters");
 
 // One grid-stride loop over (chunk, plane, token, vector) units; VEC halfs per unit.
-// vllm chunk layout [L,2,t,H,D]; huggingface [L,2,H,t,D].
+// vllm chunk layout [L,2,t,H,D]; huggingface [L,2,H,t,D]; a latent KV (ppl = 1) [L,t,H,D].
 template <int VEC, bool PACK>
 __global__ void __launch_bounds__(256) pack_kernel(PackParams P) {
     using vec_t = typename std::conditional<VEC == 8, uint4, uint16_t>::type;
-    const int NL = 2 * P.L;
+    const int NL = P.ppl * P.L;
     const int vph = P.D / VEC;                 // vectors per head row
     const int64_t vpt = (int64_t)P.H * vph;    // vectors per token
     const int64_t per_chunk_full = (int64_t)NL * P.chunk_tokens * vpt;
@@ -47,13 +48,13 @@ __global__ void __launch_bounds__(256) pack_kernel(PackParams P) {
         const int t = (j == P.n_chunks - 1) ? P.last_chunk_tokens : P.chunk_tokens;
         // r indexes [l][kv][tok][h][v] of the chunk (vllm order) -- map to plane nl = kv*L + l
         const int64_t per_plane = (int64_t)t * vpt;
-        const int lk = (int)(r / per_plane);       // l*2 + kv
+        const int lk = (int)(r / per_plane);       // l*ppl + kv
         r -= (int64_t)lk * per_plane;
         const int tok = (int)(r / vpt);
         r -= (int64_t)tok * vpt;
         const int h = (int)(r / vph);
         const int v = (int)(r - (int64_t)h * vph);
-        const int l = lk >> 1, kv = lk & 1;
+        const int l = P.ppl == 2 ? lk >> 1 : lk, kv = P.ppl == 2 ? lk & 1 : 0;
         const uint16_t* plane = P.pt.p[kv * P.L + l];
         int64_t row = P.tok_begin + j * P.chunk_tokens + tok;
         if (P.slot_map) row = __ldg(P.slot_map + row);       // consecutive threads share the token: broadcast, L1 hit
@@ -78,7 +79,8 @@ static int launch_pack(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, i
     B2_REQUIRE(n_chunks > 0 && chunk_tokens > 0 && last_chunk_tokens > 0 && last_chunk_tokens <= chunk_tokens,
                "bad chunking");
     B2_REQUIRE(chunks != nullptr, "chunks is NULL");
-    const int64_t chunk_bytes = 2ll * kv->L * 2 * chunk_tokens * kv->H * kv->D;
+    P.ppl = kv_ppl(kv);
+    const int64_t chunk_bytes = 2ll * kv->L * P.ppl * chunk_tokens * kv->H * kv->D;
     B2_REQUIRE(chunk_stride_bytes >= chunk_bytes || n_chunks == 1, "chunk_stride_bytes too small");
     P.sT = kv->sT; P.sH = kv->sH; P.tok_begin = tok_begin;
     P.slot_map = kv->slot_map;
@@ -89,9 +91,9 @@ static int launch_pack(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, i
     P.chunk_stride_bytes = chunk_stride_bytes;
     bool vec = (kv->D % 8 == 0) && (kv->sT % 8 == 0) && (kv->sH % 8 == 0) &&
                ((reinterpret_cast<uintptr_t>(chunks) & 15) == 0) && (chunk_stride_bytes % 16 == 0);
-    for (int nl = 0; nl < 2 * P.L && vec; ++nl) vec = (reinterpret_cast<uintptr_t>(P.pt.p[nl]) & 15) == 0;
+    for (int nl = 0; nl < P.ppl * P.L && vec; ++nl) vec = (reinterpret_cast<uintptr_t>(P.pt.p[nl]) & 15) == 0;
     const int V = vec ? 8 : 1;
-    const int64_t total = ((int64_t)(n_chunks - 1) * chunk_tokens + last_chunk_tokens) * 2 * kv->L * kv->H * (kv->D / V);
+    const int64_t total = ((int64_t)(n_chunks - 1) * chunk_tokens + last_chunk_tokens) * P.ppl * kv->L * kv->H * (kv->D / V);
     int64_t blocks = (total + 255) / 256;
     int dev = 0, sms = 0;
     B2_CHECK_CUDA(cudaGetDevice(&dev));

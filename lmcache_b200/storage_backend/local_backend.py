@@ -803,8 +803,8 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
                 size = st.st_size
                 with open(full, "rb") as f:
                     hd = parse_header(f.read(N.HEADER_BYTES + N.MAX_PLANES), size)
-                if int(hd.total_bytes) != size:
-                    continue
+                if int(hd.total_bytes) != size or hd.version == 4:
+                    continue                     # version 4 (a latent KV) is no container of this tier's (K, V) engine
             except (OSError, ValueError):
                 continue                         # damaged / foreign file: not part of the cache
             # "/" in a model name was written as "-": the key of a lookup goes through the same rule, so index by path

@@ -207,6 +207,8 @@ class CacheGenGPUEncoderOutput:
         from lmcache_b200.codec import parse_header
         from lmcache_b200.codec import container_layout_of
         hd = parse_header(bs)
+        if hd.version == 4:
+            raise ValueError("a version-4 container (one latent plane per layer) has no (key, value) object form")
         L, H, D, t, G = hd.L, hd.H, hd.D, hd.ntokens, hd.ngroups
         C = H * D
         lo = container_layout_of(hd)
