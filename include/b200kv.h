@@ -348,7 +348,8 @@ int b200kv_copy_async(void* dst, const void* src, int64_t bytes, void* stream); 
 int b200kv_copy2d_async(void* dst, int64_t dst_pitch, const void* src, int64_t src_pitch, int64_t row_bytes,
                         int64_t rows, void* stream);
 /* n copies of sizes[i] bytes from srcs[i] to dsts[i] (HOST pointer arrays), in stream order as a batch: the copies of one
- * call may run in any order among themselves.  One cudaMemcpyBatchAsync where the driver has it (CUDA >= 12.8). */
+ * call may run in any order among themselves.  One cudaMemcpyBatchAsync where the driver has it (CUDA >= 12.8) and the
+ * stream is not the legacy default stream (NULL), which that call refuses; one cudaMemcpyAsync per copy otherwise. */
 int b200kv_copy_batch_async(void* const* dsts, const void* const* srcs, const int64_t* sizes, int64_t n, void* stream);
 int b200kv_stream_create(void** stream);                       /* non-blocking side stream */
 int b200kv_stream_destroy(void* stream);

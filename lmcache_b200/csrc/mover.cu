@@ -178,20 +178,25 @@ int b200kv_copy_batch_async(void* const* dsts, const void* const* srcs, const in
     }
     if (d.empty()) return 0;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    // one driver call for the whole batch: per-copy submission costs ~2 us of host time per copy, which is the copy
-    // engine's time for a few hundred KB -- a layer of a layer-major upload is many copies of that size
-    cudaMemcpyAttributes attr = {};
-    attr.srcAccessOrder = cudaMemcpySrcAccessOrderStream;
-    attr.flags = cudaMemcpyFlagPreferOverlapWithCompute;
-    size_t attr_idx = 0, fail_idx = 0;
-    const cudaError_t e = cudaMemcpyBatchAsync(d.data(), s.data(), z.data(), d.size(), &attr, &attr_idx, 1, &fail_idx, st);
-    // a driver older than the runtime (CUDA < 12.8) answers cudaErrorCallRequiresNewerDriver, a device or stream that
-    // cannot take the batch cudaErrorNotSupported: then the same copies, one call each
-    if (e != cudaErrorNotSupported && e != cudaErrorCallRequiresNewerDriver) {
-        B2_CHECK_CUDA(e);
-        return 0;
+    // cudaMemcpyBatchAsync refuses the legacy default stream (NULL, e.g. torch's default stream) with "invalid argument":
+    // there the copies go one call each
+    if (st != nullptr && st != cudaStreamLegacy) {
+        // one driver call for the whole batch: per-copy submission costs ~2 us of host time per copy, which is the copy
+        // engine's time for a few hundred KB -- a layer of a layer-major upload is many copies of that size
+        cudaMemcpyAttributes attr = {};
+        attr.srcAccessOrder = cudaMemcpySrcAccessOrderStream;
+        attr.flags = cudaMemcpyFlagPreferOverlapWithCompute;
+        size_t attr_idx = 0, fail_idx = 0;
+        const cudaError_t e = cudaMemcpyBatchAsync(d.data(), s.data(), z.data(), d.size(), &attr, &attr_idx, 1, &fail_idx,
+                                                   st);
+        // a driver older than the runtime (CUDA < 12.8) answers cudaErrorCallRequiresNewerDriver, a device or stream that
+        // cannot take the batch cudaErrorNotSupported: then the same copies, one call each
+        if (e != cudaErrorNotSupported && e != cudaErrorCallRequiresNewerDriver) {
+            B2_CHECK_CUDA(e);
+            return 0;
+        }
+        (void)cudaGetLastError();
     }
-    (void)cudaGetLastError();
     for (size_t i = 0; i < d.size(); ++i) B2_CHECK_CUDA(cudaMemcpyAsync(d[i], s[i], z[i], cudaMemcpyDefault, st));
     return 0;
 }
