@@ -162,7 +162,7 @@ def sha256_prefix_chain(tokens: torch.Tensor, chunk_size: int, seq_offsets: Opti
 
 class LayerwiseRetrieval:
     """What retrieve_layerwise / retrieve_paged_layerwise return: the hit is known (`ret_mask`, and for the blob form the
-    per-layer (K, V) views `kv`), the KV arrives layer by layer.  Layer l may be read on a stream once wait_layer(l,
+    per-layer (K, V) views `kv`, or an MLA engine's latent views), the KV arrives layer by layer.  Layer l may be read on a stream once wait_layer(l,
     stream) has been called -- what vLLM's KV connector does in wait_for_layer_load before attention layer l."""
 
     def __init__(self, ret_mask: torch.Tensor, kv: Optional[KVCache], num_layers: int, upload):
@@ -254,19 +254,59 @@ class LMCacheEngine:
         if config.reshard_world_sizes is not None and metadata.world_size in config.reshard_world_sizes:
             raise ValueError(f"reshard_world_sizes {config.reshard_world_sizes} holds this engine's own world size "
                              f"{metadata.world_size}: its chunks are served by the ordinary retrieve")
+        self._mla = bool(getattr(metadata, "use_mla", False))
+        if self._mla:
+            self._check_mla_config(config, metadata)
         self.engine_ = CreateStorageBackend(config, metadata)
         self._reshard_counts: Dict[int, Dict[str, int]] = {}
         logger.debug(f"Current storage backend type {type(self.engine_)}")
 
+    @staticmethod
+    def _check_mla_config(config: LMCacheEngineConfig, metadata: LMCacheEngineMetadata) -> None:
+        """the settings a latent KV (use_mla) rules out"""
+        if metadata.fmt != "vllm":
+            raise ValueError(f"use_mla: a latent KV has the vllm layout only, not fmt={metadata.fmt!r}")
+        if config.reshard_world_sizes is not None:
+            raise ValueError("use_mla: the keys of a latent KV are shared by every tensor-parallel size already, "
+                             "reshard_world_sizes must be None")
+        local = config.local_device
+        cachegen_tier = ((local == "cpu" and config.local_serde == "cachegen") or local not in (None, "cpu", "cuda") or
+                         (config.remote_url is not None and config.remote_serde == "cachegen"))
+        if cachegen_tier and config.chunk_size > N.GROUP_TOKENS:
+            raise ValueError(f"use_mla: a CacheGen tier keeps a latent KV in version-4 containers, which hold at most "
+                             f"{N.GROUP_TOKENS} tokens; chunk_size is {config.chunk_size}")
+
     # ------------------------------------------------------------------ keys / hashes
     def _make_key(self, chunk_hash: str, fmt: str) -> CacheEngineKey:
+        if self._mla:
+            # every rank holds the same latent: one key for all of them, that of a one-rank layout
+            return CacheEngineKey(fmt, self.metadata.model_name, 1, 0, chunk_hash)
         return CacheEngineKey(fmt, self.metadata.model_name, self.metadata.world_size, self.metadata.worker_id,
                               chunk_hash)
+
+    def _first(self, kv) -> torch.Tensor:
+        """the first tensor of a store's KV: layer 0's latent, or layer 0's K"""
+        return kv[0] if self._mla else kv[0][0]
+
+    def _tensors(self, kv) -> List[torch.Tensor]:
+        return list(kv) if self._mla else [t for pair in kv for t in pair]
 
     def _num_tokens_in_kv(self, kv_tensors: Union[KVCache, torch.Tensor], fmt: str) -> int:
         if fmt not in ("vllm", "huggingface"):
             raise ValueError(f"Invalid format: {fmt}")
+        if self._mla:
+            return kv_tensors[0].shape[0]                                  # a layer's latent is [T, D]
         return kv_tensors[0][0].shape[KvView.token_dim(fmt) - 2]         # a layer's K is a blob without its [L, 2] dims
+
+    def _check_kind(self, kv, what: str) -> None:
+        """AssertionError unless `kv` holds one tensor per layer (a latent KV) on an MLA engine, a (K, V) pair per
+        layer otherwise"""
+        if self._mla:
+            assert all(isinstance(t, torch.Tensor) for t in kv), \
+                f"an MLA engine (use_mla) takes one latent tensor per layer in {what}, not (K, V) pairs"
+        else:
+            assert not any(isinstance(t, torch.Tensor) for t in kv), \
+                f"a (K, V) engine takes a (K, V) pair per layer in {what}; latent tensors need use_mla"
 
     def _prefix_hash(self, tokens: torch.Tensor, num_skip_chunk: Optional[int] = 0):
         """All chunk digests of `tokens` (the whole chain is hashed, then the first num_skip_chunk digests are
@@ -279,26 +319,39 @@ class LMCacheEngine:
     # ------------------------------------------------------------------ blob helpers
     def _pack_chunks_torch(self, kv: KVCache, tok_begin: int, fmt: str) -> List[torch.Tensor]:
         """_tuple_kv_to_blob + _slice_kv_at with torch ops (cache_engine.py:98-161), for dtypes the kernels do not move"""
-        k = torch.stack([x[0] for x in kv])
-        v = torch.stack([x[1] for x in kv])
-        blob = torch.stack((k, v)).permute(1, 0, 2, 3, 4)
-        tdim = KvView.token_dim(fmt)
+        if self._mla:
+            blob = torch.stack(list(kv))                                   # [L, T, D]
+        else:
+            k = torch.stack([x[0] for x in kv])
+            v = torch.stack([x[1] for x in kv])
+            blob = torch.stack((k, v)).permute(1, 0, 2, 3, 4)
+        tdim = KvView.token_dim(fmt, self._mla)
         blob = blob.narrow(tdim, tok_begin, blob.shape[tdim] - tok_begin)
         return [c.contiguous() for c in torch.split(blob, self.chunk_size, dim=tdim)]
 
-    @staticmethod
-    def _as_cuda_kv(kv_tensors_raw: KVCache) -> KVCache:
-        if kv_tensors_raw[0][0].is_cuda:
+    def _as_cuda_kv(self, kv_tensors_raw: KVCache) -> KVCache:
+        if self._first(kv_tensors_raw).is_cuda:
             return kv_tensors_raw
+        if self._mla:
+            return tuple(x.cuda() for x in kv_tensors_raw)
         return tuple((k.cuda(), v.cuda()) for k, v in kv_tensors_raw)
 
     def _blob_to_tuple_kv(self, blob: torch.Tensor) -> KVCache:
+        if self._mla:
+            return tuple(torch.unbind(blob, dim=0))                        # L views [T, D] of the [L, T, D] blob
         return tuple((layer[0], layer[1]) for layer in torch.unbind(blob, dim=0))
+
+    def _flat_paged(self, kv_caches) -> list:
+        """the paged caches as [num_slots, ...] views: per layer a latent cache, or a (key, value) pair"""
+        if self._mla:
+            return [c.reshape(-1, c.shape[-1]) for c in kv_caches]
+        return [(k.reshape(-1, k.shape[-2], k.shape[-1]), v.reshape(-1, v.shape[-2], v.shape[-1])) for k, v in kv_caches]
 
     # ------------------------------------------------------------------ arguments and masks
     def _check_store_args(self, tokens: torch.Tensor, kv_tensors_raw: KVCache, fmt: str) -> None:
         assert len(tokens.shape) == 1, f"Invalid shape of tokens: {tokens.shape}"
         assert len(kv_tensors_raw) > 0, "Empty kv_tensors"
+        self._check_kind(kv_tensors_raw, "kv_tensors_raw")
         assert len(tokens) == self._num_tokens_in_kv(kv_tensors_raw, fmt), \
             "Number of tokens in the kv cache does not match the input tokens"
 
@@ -309,6 +362,7 @@ class LMCacheEngine:
         if kv_caches is not None:
             assert len(tokens.shape) == 1, f"Invalid shape of tokens: {tokens.shape}"
             assert len(kv_caches) > 0, "Empty kv_caches"
+            self._check_kind(kv_caches, "kv_caches")
         assert len(tokens) == slot_mapping.numel(), "Number of slots does not match the input tokens"
 
     def _split_mask(self, tokens: torch.Tensor, mask: Optional[torch.Tensor]) -> Tuple[torch.Tensor, int, int, int]:
@@ -352,7 +406,7 @@ class LMCacheEngine:
     def store(self, tokens: torch.Tensor, kv_tensors_raw: KVCache, skip_existing=True, blocking=True) -> None:
         """Store the KV cache of `tokens`.  kv_tensors_raw: nested tuple of per-layer (K, V), each
         [num_tokens, num_heads, head_size] (vllm) or [num_heads, num_tokens, head_size] (huggingface),
-        without a batch dimension."""
+        without a batch dimension.  An MLA engine (metadata.use_mla) takes one latent [num_tokens, D] per layer."""
         start_time = time.perf_counter()
         fmt = self.metadata.fmt
         self._check_store_args(tokens, kv_tensors_raw, fmt)
@@ -361,7 +415,7 @@ class LMCacheEngine:
 
         def put(keys, tok_begin):
             kv_cuda = self._as_cuda_kv(kv_tensors_raw)
-            if kv_cuda[0][0].dtype not in (torch.bfloat16, torch.float16):
+            if self._first(kv_cuda).dtype not in (torch.bfloat16, torch.float16):
                 # the native pack / codec kernels move 16-bit KV; any other dtype (the reference's local and torch-serde
                 # paths accept every dtype) takes the reference's own blob ops on the GPU (cache_engine.py:98-161)
                 chunks = self._pack_chunks_torch(kv_cuda, tok_begin, fmt)
@@ -381,7 +435,8 @@ class LMCacheEngine:
     @torch.no_grad()
     def retrieve(self, tokens: torch.Tensor, mask: Optional[torch.Tensor] = None) -> Tuple[KVCache, torch.Tensor]:
         """Retrieve the longest cached prefix of `tokens` (optionally only the suffix selected by a boolean
-        suffix `mask`).  Returns (kv tuple -- empty tuple on a total miss, ret_mask marking retrieved tokens)."""
+        suffix `mask`).  Returns (kv tuple -- empty tuple on a total miss, ret_mask marking retrieved tokens).  An MLA
+        engine returns one latent [T, D] per layer: views of one [L, T, D] blob."""
         return self._retrieve(tokens, mask)
 
     def _retrieve(self, tokens, mask, get_kv=None) -> Tuple[KVCache, torch.Tensor]:
@@ -403,7 +458,8 @@ class LMCacheEngine:
                 self._wide_dtype = True      # chunks of a dtype the kernels do not move: per-chunk path from now on
         retrieved: List[torch.Tensor] = []
         for chunk in self.engine_.batched_get(self._make_key(h, fmt) for h in chunk_hashes):
-            if chunk is None:
+            # a blob of the other kind (a latent [L,t,D] for a (K, V) engine, or the reverse) is a miss
+            if chunk is None or chunk.dim() != (3 if self._mla else 5):
                 break
             retrieved.append(chunk)
         self._touch(full_chain[:num_skip_chunk + len(retrieved)], fmt)
@@ -412,7 +468,7 @@ class LMCacheEngine:
             return (), self._trim_mask(ret_mask, num_skip_tok, 0)
 
         # assemble into one blob; drop the extra leading tokens of the first chunk (suffix mask)
-        tdim = KvView.token_dim(fmt)
+        tdim = KvView.token_dim(fmt, self._mla)
         sizes = [c.shape[tdim] for c in retrieved]
         total = sum(sizes) - extra
         first = retrieved[0]
@@ -437,12 +493,14 @@ class LMCacheEngine:
         """store() for a vLLM paged KV cache: token i's K/V live in row slot_mapping[i] of every layer's
         (key_cache, value_cache) [num_blocks, block_size, H, D].  What lmcache-vllm's lmcache_store_kv does with a
         torch gather per layer + store() (LLM_Engine.rst:91-99); here the backend's kernels read the cache rows
-        directly (cachegen: quantise + code from the rows; local tiers: one gather straight into the chunk blobs)."""
+        directly (cachegen: quantise + code from the rows; local tiers: one gather straight into the chunk blobs).
+        An MLA engine takes one latent cache [num_blocks, block_size, D] (or [num_slots, D]) per layer."""
         self._check_paged_args(tokens, slot_mapping, kv_caches)
         if not self._fast_path():
-            flat = [(k.reshape(-1, k.shape[-2], k.shape[-1]), v.reshape(-1, v.shape[-2], v.shape[-1])) for k, v in kv_caches]
-            idx = slot_mapping.to(flat[0][0].device)
-            return self.store(tokens, tuple((k[idx], v[idx]) for k, v in flat), skip_existing, blocking)
+            flat = self._flat_paged(kv_caches)
+            idx = slot_mapping.to(self._first(flat).device)
+            kv = tuple(c[idx] for c in flat) if self._mla else tuple((k[idx], v[idx]) for k, v in flat)
+            return self.store(tokens, kv, skip_existing, blocking)
         chunk_hashes = self._prefix_hash(tokens)
         start = self._skip_scan(chunk_hashes, "vllm") if skip_existing else 0
 
@@ -464,16 +522,21 @@ class LMCacheEngine:
     def _retrieve_paged(self, tokens, kv_caches, slot_mapping, mask, get_kv=None) -> torch.Tensor:
         """retrieve_paged; get_kv as in _retrieve, for every chunk but a first one that straddles the mask"""
         self._check_paged_args(tokens, slot_mapping)
-        flat = [(k.reshape(-1, k.shape[-2], k.shape[-1]), v.reshape(-1, v.shape[-2], v.shape[-1])) for k, v in kv_caches]
-        dev = flat[0][0].device
+        self._check_kind(kv_caches, "kv_caches")
+        flat = self._flat_paged(kv_caches)
+        dev = self._first(flat).device
         slots = slot_mapping.to(dev)
         if not self._fast_path():
             kv, ret_mask = self.retrieve(tokens, mask)
             if len(kv) > 0:
                 idx = slots[ret_mask.to(dev)]
-                for (kc, vc), (k, v) in zip(flat, kv):
-                    kc[idx] = k.to(kc.dtype)
-                    vc[idx] = v.to(vc.dtype)
+                if self._mla:
+                    for c, x in zip(flat, kv):
+                        c[idx] = x.to(c.dtype)
+                else:
+                    for (kc, vc), (k, v) in zip(flat, kv):
+                        kc[idx] = k.to(kc.dtype)
+                        vc[idx] = v.to(vc.dtype)
             return ret_mask
         cs = self.chunk_size
         ret_mask, num_skip_tok, num_skip_chunk, extra = self._split_mask(tokens, mask)
@@ -486,13 +549,18 @@ class LMCacheEngine:
         if first:
             # the first chunk straddles the mask: decode it next to the cache and scatter only its unmasked tail
             t0 = min(cs, len(tokens) - base)
-            tmp = torch.empty(KvView.blob_shape("vllm", view.L, view.H, view.D, t0), dtype=view.dtype, device=dev)
+            tmp = torch.empty(KvView.blob_shape("vllm", view.L, view.H, view.D, t0, self._mla), dtype=view.dtype,
+                              device=dev)
             layout, own, got_chunks = self._fetch(chunk_hashes[:1], "vllm", KvView.from_blob(tmp, "vllm"), 0)
             if got_chunks:
                 idx = slots[base + extra: base + t0]
-                for l, (kc, vc) in enumerate(flat):
-                    kc[idx] = tmp[l, 0, extra:]
-                    vc[idx] = tmp[l, 1, extra:]
+                if self._mla:
+                    for l, c in enumerate(flat):
+                        c[idx] = tmp[l, extra:]
+                else:
+                    for l, (kc, vc) in enumerate(flat):
+                        kc[idx] = tmp[l, 0, extra:]
+                        vc[idx] = tmp[l, 1, extra:]
         if got_chunks == first and len(chunk_hashes) > first:       # not after a straddling chunk that missed
             layout, own_rest, n = self._fetch(chunk_hashes[first:], "vllm", view, first * cs, get_kv, layout)
             own += own_rest
@@ -607,7 +675,7 @@ class LMCacheEngine:
                 geom = peek(key0, fmt)
             else:
                 first = self.engine_.get(key0)
-                if first is not None:
+                if first is not None and first.dim() == (3 if self._mla else 5):     # the other kind's blob: a miss
                     geom = KvView.blob_geometry(first, fmt)
             if geom is None and self.config.reshard_world_sizes:
                 geom = self._reshard_geometry(chunk_hashes[0], fmt)
@@ -622,7 +690,7 @@ class LMCacheEngine:
         if od is not None and od() is not None:
             dtype = od()
         n_tok_max = len(tokens) - num_skip_chunk * self.chunk_size
-        blob = torch.empty(KvView.blob_shape(fmt, L, H, D, n_tok_max), dtype=dtype,
+        blob = torch.empty(KvView.blob_shape(fmt, L, H, D, n_tok_max, self._mla), dtype=dtype,
                            device=torch.device("cuda", torch.cuda.current_device()))
         _, own, n = self._fetch(chunk_hashes, fmt, KvView.from_blob(blob, fmt), 0, get_kv, own_miss=own_miss)
         self._touch(full_chain[:num_skip_chunk + own], fmt)
@@ -631,7 +699,7 @@ class LMCacheEngine:
             return (), self._trim_mask(ret_mask, num_skip_tok, 0)
         got = min(n * self.chunk_size, n_tok_max) - extra      # the last hit chunk may be the ragged tail
         logger.info(f"Retrieved {n} chunks ({got} tokens in total) -- elapsed time {time.perf_counter() - st}")
-        kv = self._blob_to_tuple_kv(blob.narrow(KvView.token_dim(fmt), extra, got))
+        kv = self._blob_to_tuple_kv(blob.narrow(KvView.token_dim(fmt, self._mla), extra, got))
         return kv, self._trim_mask(ret_mask, num_skip_tok, got)
 
     # ------------------------------------------------------------------ layer-wise retrieve
@@ -719,7 +787,7 @@ class LMCacheEngine:
         def fallback(stream, enc):
             with torch.cuda.stream(stream):
                 self.store_paged(tokens, kv_caches, slot_mapping, skip_existing)
-        if not self._layerwise_store_ok(kv_caches[0][0].dtype):
+        if not self._layerwise_store_ok(self._first(kv_caches).dtype):
             return LayerwiseStore(len(kv_caches), None, fallback)
         return self._begin_layerwise(tokens, lambda: KvView.from_paged(kv_caches, slot_mapping.cuda()), "vllm",
                                      len(kv_caches), skip_existing, fallback)
@@ -727,17 +795,17 @@ class LMCacheEngine:
     @torch.no_grad()
     def store_layerwise(self, tokens: torch.Tensor, kv_tensors_raw: KVCache, skip_existing=True) -> LayerwiseStore:
         """store(), with the KV handed over one layer at a time (see store_paged_layerwise): kv_tensors_raw is store()'s
-        per-layer (K, V) tuple on the GPU, possibly not yet written."""
+        per-layer (K, V) tuple (or an MLA engine's latent per layer) on the GPU, possibly not yet written."""
         fmt = self.metadata.fmt
         self._check_store_args(tokens, kv_tensors_raw, fmt)
 
         def fallback(stream, enc):
             with torch.cuda.stream(stream):
                 self.store(tokens, kv_tensors_raw, skip_existing)
-        k0 = kv_tensors_raw[0][0]
+        k0 = self._first(kv_tensors_raw)
         # the kernels must read the caller's tensors in place (KvView.from_tuple would copy tensors of other strides
         # now, before they are written): anything else takes the ordinary store at finish()
-        in_place = all(t.stride() == k0.stride() and t.stride(2) == 1 for kv in kv_tensors_raw for t in kv)
+        in_place = all(t.stride() == k0.stride() and t.stride(-1) == 1 for t in self._tensors(kv_tensors_raw))
         if not k0.is_cuda or not in_place or not self._layerwise_store_ok(k0.dtype):
             return LayerwiseStore(len(kv_tensors_raw), None, fallback)
         return self._begin_layerwise(tokens, lambda: KvView.from_tuple(kv_tensors_raw, fmt), fmt, len(kv_tensors_raw),

@@ -110,15 +110,20 @@ class KvView:
             raise TypeError(f"KV dtype must be bfloat16 or float16, got {dtype}")
         return _DTYPE_CODE[dtype]
 
-    # A chunk blob holds t tokens of every layer: [L,2,t,H,D] (vllm) or [L,2,H,t,D] (huggingface).  Its token
-    # dimension, its shape, and the (L, H, D, dtype) read back from one:
+    # A chunk blob holds t tokens of every layer: [L,2,t,H,D] (vllm) or [L,2,H,t,D] (huggingface); a latent one [L,t,D]
+    # (vllm only).  Its token dimension, its shape, and the (L, H, D, dtype) read back from one (H = 1 for a latent blob,
+    # as in its descriptor):
     @staticmethod
-    def token_dim(fmt: str) -> int: return 2 if fmt == "vllm" else 3
+    def token_dim(fmt: str, latent: bool = False) -> int: return 1 if latent else 2 if fmt == "vllm" else 3
     @staticmethod
-    def blob_shape(fmt: str, L: int, H: int, D: int, t: int) -> Tuple[int, ...]:
+    def blob_shape(fmt: str, L: int, H: int, D: int, t: int, latent: bool = False) -> Tuple[int, ...]:
+        if latent:
+            return (L, t, D)
         return (L, 2, t, H, D) if fmt == "vllm" else (L, 2, H, t, D)
     @staticmethod
     def blob_geometry(blob: torch.Tensor, fmt: str) -> Tuple[int, int, int, torch.dtype]:
+        if blob.dim() == 3:
+            return blob.shape[0], 1, blob.shape[2], blob.dtype
         return blob.shape[0], blob.shape[3 if fmt == "vllm" else 2], blob.shape[4], blob.dtype
 
     @staticmethod

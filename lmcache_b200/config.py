@@ -19,6 +19,11 @@ class LMCacheEngineMetadata:
     worker_id: int    # tensor-parallel rank (part of the key)
     fmt: str          # "vllm" | "huggingface"
     dtype: str        # dtype of the kv tensors
+    # not in the reference: the model caches one latent vector per token and layer (multi-head latent attention,
+    # DeepSeek-V2/V3) instead of a (K, V) pair.  The engine then takes and returns one [T, D] tensor per layer, its
+    # CacheGen tiers keep version-4 containers, and every tensor-parallel rank uses the keys of rank 0 of a one-rank
+    # layout: the latent is the same on every rank, so one copy serves all of them (LMCacheEngine).
+    use_mla: bool = False
 
 
 @dataclass

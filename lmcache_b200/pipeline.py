@@ -63,11 +63,11 @@ class EncodeRing:
     every slot is still in flight -- the only back-pressure of the store pipeline."""
 
     def __init__(self, codec: CacheGenCodec, L: int, H: int, D: int, chunk_size: int, device, wave: Optional[int] = None,
-                 slots: Optional[int] = None):
+                 slots: Optional[int] = None, latent: bool = False):
         self.codec = codec
-        self.geom = (L, H, D, chunk_size, torch.device(device))
+        self.geom = (L, H, D, chunk_size, torch.device(device), latent)
         self.wave = wave or wave_chunks_default()
-        self.stride = codec.out_stride(L, H, D, chunk_size)
+        self.stride = codec.out_stride(L, H, D, chunk_size, latent)
         n = slots or wave_slots_default()
         self._free: "queue.Queue[WaveSlot]" = queue.Queue()
         self._all: List[WaveSlot] = []
@@ -76,8 +76,8 @@ class EncodeRing:
             self._all.append(s)
             self._free.put(s)
 
-    def matches(self, L, H, D, chunk_size, device) -> bool:
-        return self.geom == (L, H, D, chunk_size, torch.device(device))
+    def matches(self, L, H, D, chunk_size, device, latent: bool = False) -> bool:
+        return self.geom == (L, H, D, chunk_size, torch.device(device), latent)
 
     def scratch_bytes(self) -> int:
         return sum(s.dev.numel() for s in self._all)
@@ -145,10 +145,10 @@ class EncodePipeline:
 
     # ------------------------------------------------------------------ caller side
     def _ring_for(self, view: KvView, chunk_size: int) -> EncodeRing:
-        if self.ring is None or not self.ring.matches(view.L, view.H, view.D, chunk_size, view.device):
+        if self.ring is None or not self.ring.matches(view.L, view.H, view.D, chunk_size, view.device, view.latent):
             if self.ring is not None:
                 self.ring.close()
-            self.ring = EncodeRing(self.codec, view.L, view.H, view.D, chunk_size, view.device)
+            self.ring = EncodeRing(self.codec, view.L, view.H, view.D, chunk_size, view.device, latent=view.latent)
         return self.ring
 
     def submit_encoded(self, enc: "LayerwiseEncode", items: Sequence) -> StoreJob:
@@ -254,7 +254,7 @@ class HostContainer:
         self.ntokens = int(hd.ntokens)
         self.L, self.H, self.D = int(hd.L), int(hd.H), int(hd.D)
         self.max_dtype = int(hd.max_dtype)
-        self.coder = int(hd.version) - 1
+        self.coder = N.coder_of_version(hd.version)          # N.CODER_LATENT for version 4 (one plane per layer)
         self.last_read: Optional[torch.cuda.Event] = None   # most recent upload out of the block
         # codec.plane_offsets: where each plane's streams lie, for a layer-major upload; None: upload it whole.  Made by
         # whoever makes the record (land, read_container), never on the thread of a retrieve.
@@ -309,7 +309,8 @@ def land(slab, slot: WaveSlot, batch, blocks: Optional[list] = None,
         recs = []
         for j, blk in enumerate(blocks):
             hd = parse_header(blk.view())
-            recs.append(HostContainer(blk, blk.nbytes, hd, po[j, :2 * hd.L + 1].copy() if po[j, 0] >= 0 else None))
+            P = N.planes_of(hd.version, hd.L)
+            recs.append(HostContainer(blk, blk.nbytes, hd, po[j, :P + 1].copy() if po[j, 0] >= 0 else None))
         return recs
     except BaseException:
         for blk in blocks:
@@ -356,23 +357,25 @@ def arena_placement(seg_bytes: np.ndarray, arena_bytes: int, layers: Optional[Se
 
 class SegmentSlot:
     """Device scratch of one layer-wise store: the payload arena, the chunks' fixed-section images, the encode
-    workspace, and in mapped page-locked memory the container sizes and the (arena offset, bytes) row of every plane."""
+    workspace, and in mapped page-locked memory the container sizes and the (arena offset, bytes) row of every plane.
+    P: planes per chunk, 2L for (K, V) pairs, L for a latent KV."""
 
-    def __init__(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, L: int, device):
+    def __init__(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, P: int, device):
         self.arena = torch.empty(max(16, arena_bytes), dtype=torch.uint8, device=device)
         self.fixed = torch.empty(max(16, fixed_bytes), dtype=torch.uint8, device=device)
         self.ws = torch.empty(max(16, ws_bytes), dtype=torch.uint8, device=device)
         self.sizes = PinnedBuffer(max(64, 8 * n_chunks))
-        self.seg = PinnedBuffer(max(64, 16 * 2 * L * n_chunks))
+        self.seg = PinnedBuffer(max(64, 16 * P * n_chunks))
         self.arena_bytes = arena_bytes
         self.ticket = None
         self.layouts: tuple = ()            # (off_payload of a full chunk, of the last chunk)
         self.fixed_stride = 0
-        self.n_chunks, self.L = 0, L
+        self.coder = N.CODER_RANS_COMPACT   # the coder that names the containers' version (N.CODER_LATENT: 4)
+        self.n_chunks, self.P = 0, P
 
-    def holds(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, L: int) -> bool:
+    def holds(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, P: int) -> bool:
         return (self.arena.numel() >= arena_bytes and self.fixed.numel() >= fixed_bytes and self.ws.numel() >= ws_bytes
-                and self.sizes.nbytes >= 8 * n_chunks and self.seg.nbytes >= 32 * L * n_chunks)
+                and self.sizes.nbytes >= 8 * n_chunks and self.seg.nbytes >= 16 * P * n_chunks)
 
     def close(self) -> None:
         self.sizes.close()
@@ -393,14 +396,14 @@ class SegmentPool:
         self._free: List[SegmentSlot] = []
         self._lock = threading.Lock()
 
-    def acquire(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, L: int) -> SegmentSlot:
+    def acquire(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, P: int) -> SegmentSlot:
         with self._lock:
             for s in self._free:
-                if s.holds(arena_bytes, fixed_bytes, ws_bytes, n_chunks, L):
+                if s.holds(arena_bytes, fixed_bytes, ws_bytes, n_chunks, P):
                     self._free.remove(s)
                     return s
         with torch.cuda.device(self.device), torch.cuda.stream(self.stream):
-            return SegmentSlot(arena_bytes, fixed_bytes, ws_bytes, n_chunks, L, self.device)
+            return SegmentSlot(arena_bytes, fixed_bytes, ws_bytes, n_chunks, P, self.device)
 
     def release(self, slot: SegmentSlot) -> None:
         slot.ticket = None
@@ -431,8 +434,7 @@ class _SegmentTicket:
         self.keep = None
         sizes = list((ctypes.c_uint64 * self.slot.n_chunks).from_address(self.slot.sizes.host_ptr))
         k = next((j for j, s in enumerate(sizes) if s == 0), len(sizes))
-        return EncodedBatch(self.slot.fixed, self.slot.fixed_stride, [int(s) for s in sizes[:k]], 0,
-                            N.CODER_RANS_COMPACT)
+        return EncodedBatch(self.slot.fixed, self.slot.fixed_stride, [int(s) for s in sizes[:k]], 0, self.slot.coder)
 
 
 class LayerwiseEncode:
@@ -450,8 +452,9 @@ class LayerwiseEncode:
         n = (n_tok + chunk_size - 1) // chunk_size
         last = n_tok - (n - 1) * chunk_size
         L, H, D = view.L, view.H, view.D
-        lo = N.container_layout(L, H, D, chunk_size, N.CODER_RANS_COMPACT)
-        lo_last = N.container_layout(L, H, D, last, N.CODER_RANS_COMPACT)
+        coder = N.CODER_LATENT if view.latent else N.CODER_RANS_COMPACT     # version 4 for a latent KV, else 3
+        lo = N.container_layout(L, H, D, chunk_size, coder)
+        lo_last = N.container_layout(L, H, D, last, coder)
         stride = (lo.off_payload + 15) & ~15
         per_chunk = lo.max_total_bytes - lo.off_payload + 16 * L
         arena = min(n * per_chunk, budget or layerwise_store_budget_default())
@@ -459,8 +462,8 @@ class LayerwiseEncode:
         ws_bytes = N.check(lib.b200kv_encode_layers_workspace_bytes(L, H, D, chunk_size, n, 1), "encode_layers_workspace")
         self.pool, self.view, self.L, self.n_chunks = pool, view, L, n
         self.plan = N.EncodePlan()
-        self.slot = pool.acquire(arena, n * stride, ws_bytes, n, L)
-        self.slot.n_chunks, self.slot.L, self.slot.fixed_stride = n, L, stride
+        self.slot = pool.acquire(arena, n * stride, ws_bytes, n, view.planes)
+        self.slot.n_chunks, self.slot.P, self.slot.fixed_stride, self.slot.coder = n, view.planes, stride, coder
         self.slot.layouts = (int(lo.off_payload), int(lo_last.off_payload))
         self.done: Optional[torch.cuda.Event] = None
         s = self.slot
@@ -511,12 +514,12 @@ def land_segments(slab, slot: SegmentSlot, batch, blocks: Optional[list] = None,
     -- when a copy fails, the segments do not add up to the container's size, or a header carries an encoder error."""
     if blocks is None:
         blocks = [slab.alloc(size) for size in batch.sizes]
-    n, L = len(blocks), slot.L
+    n, P = len(blocks), slot.P        # P plane segments per container: 2L, or L for a latent KV
     try:
         if n == 0:
             return []
-        seg = np.frombuffer(slot.seg.view(), dtype=np.int64, count=slot.n_chunks * 2 * L * 2)
-        seg = seg.reshape(slot.n_chunks, 2 * L, 2)[:n]
+        seg = np.frombuffer(slot.seg.view(), dtype=np.int64, count=slot.n_chunks * P * 2)
+        seg = seg.reshape(slot.n_chunks, P, 2)[:n]
         full, last = slot.layouts
         fixed = np.array([last if j == slot.n_chunks - 1 else full for j in range(n)], dtype=np.int64)
         planes = np.concatenate([fixed[:, None], fixed[:, None] + np.cumsum(seg[:, :, 1], axis=1)], axis=1)
@@ -551,12 +554,13 @@ def land_segments(slab, slot: SegmentSlot, batch, blocks: Optional[list] = None,
         raise
 
 
-def read_container(codec: CacheGenCodec, blk, nbytes: int) -> Optional[HostContainer]:
+def read_container(codec: CacheGenCodec, blk, nbytes: int, latent: bool = False) -> Optional[HostContainer]:
     """The record of a container a disk read or a GET put into the first `nbytes` of `blk`, or None -- with the block
-    freed -- when it is damaged or was written with another model's bins (a miss, not an error)."""
+    freed -- when it is damaged, was written with another model's bins, or holds the other kind of KV than `latent`
+    says (version 4 for a latent engine, versions 1 to 3 otherwise): a miss, not an error."""
     try:
         hd = parse_header(blk.view()[:nbytes])
-        if codec.accepts(hd):
+        if codec.accepts(hd, latent):
             return HostContainer(blk, nbytes, hd, plane_offsets(blk.view()[:nbytes]))   # on the reader's thread
     except ValueError:
         pass
@@ -632,8 +636,10 @@ class HeadWindow(NamedTuple):
 def _continues_match(r: HostContainer, first: Optional[HostContainer], dst: KvView, tok: int,
                      src_H: Optional[int] = None) -> bool:
     """May container `r`, landing at token `tok` of `dst`, extend a match that began with `first` (None: r is first)?
-    src_H: the heads r must hold when it is decoded through a head window (None: dst's)."""
+    src_H: the heads r must hold when it is decoded through a head window (None: dst's).  A version-4 container fits a
+    latent destination only, and every other version a (K, V) one."""
     return (r.L, r.H, r.D) == (dst.L, dst.H if src_H is None else src_H, dst.D) and tok + r.ntokens <= dst.ntokens and \
+        (r.coder == N.CODER_LATENT) == dst.latent and \
         (first is None or (r.max_dtype, r.coder) == (first.max_dtype, first.coder))
 
 
@@ -875,18 +881,21 @@ def _batch_copy(dsts: np.ndarray, srcs: np.ndarray, sizes: np.ndarray, stream: t
                                             stream.cuda_stream), "copy_batch_async")
 
 
-def layer_copy_ranges(plane_offs: Sequence[Optional[np.ndarray]], nbytes: Sequence[int], L: int):
+def layer_copy_ranges(plane_offs: Sequence[Optional[np.ndarray]], nbytes: Sequence[int], L: int, ppl: int = 2):
     """The copies of a layer-major upload of n containers, as offsets into each container: (fixed int64[n],
-    start int64[L, 2n], size int64[L, 2n]).  Container j's first fixed[j] bytes go first (its fixed sections; all of it
-    when it has no plane offsets); row l holds the key ranges (plane l) of containers 0..n-1, then their value ranges
-    (plane L + l).  Together they cover every container exactly once."""
+    start int64[L, ppl * n], size int64[L, ppl * n]).  Container j's first fixed[j] bytes go first (its fixed sections;
+    all of it when it has no plane offsets); row l holds the key ranges (plane l) of containers 0..n-1, then their value
+    ranges (plane L + l).  A latent KV (ppl = 1, version 4: plane l is layer l) has one range per container in row l.
+    Together they cover every container exactly once."""
     n = len(nbytes)
-    po = np.stack([o if o is not None else np.zeros(2 * L + 1, np.int64) for o in plane_offs]).astype(np.int64)
+    P = ppl * L
+    po = np.stack([o if o is not None else np.zeros(P + 1, np.int64) for o in plane_offs]).astype(np.int64)
     split = np.array([o is not None for o in plane_offs])
     fixed = np.where(split, po[:, 0], np.asarray(nbytes, dtype=np.int64)).astype(np.int64)
-    start = np.ascontiguousarray(np.concatenate([po[:, :L], po[:, L:2 * L]]).T)                   # [L, 2n]
-    size = np.ascontiguousarray(np.concatenate([po[:, 1:L + 1] - po[:, :L], po[:, L + 1:] - po[:, L:2 * L]]).T)
-    assert start.shape == (L, 2 * n)
+    start = np.ascontiguousarray(np.concatenate([po[:, k * L:(k + 1) * L] for k in range(ppl)]).T)     # [L, ppl * n]
+    size = np.ascontiguousarray(np.concatenate([po[:, k * L + 1:(k + 1) * L + 1] - po[:, k * L:(k + 1) * L]
+                                                for k in range(ppl)]).T)
+    assert start.shape == (L, ppl * n)
     return fixed, start, size
 
 
@@ -954,9 +963,10 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
             base = staging.data_ptr()
             host = np.array([r.blk.host_ptr for r in up], dtype=np.uint64)
             dev = base + np.array(offs, dtype=np.uint64)
-            fixed, lo, sz = layer_copy_ranges([r.planes for r in up], [r.nbytes for r in up], L)
-            lay_src = np.ascontiguousarray(np.tile(np.concatenate([host, host]), (L, 1)) + lo.astype(np.uint64))
-            lay_dst = np.ascontiguousarray(np.tile(np.concatenate([dev, dev]), (L, 1)) + lo.astype(np.uint64))
+            ppl = dst.planes // L
+            fixed, lo, sz = layer_copy_ranges([r.planes for r in up], [r.nbytes for r in up], L, ppl)
+            lay_src = np.ascontiguousarray(np.tile(np.concatenate([host] * ppl), (L, 1)) + lo.astype(np.uint64))
+            lay_dst = np.ascontiguousarray(np.tile(np.concatenate([dev] * ppl), (L, 1)) + lo.astype(np.uint64))
         upload = LayerwiseUpload(n, L)
         dst_tok = [dst_tok0 + j * chunk_size for j in range(n)]
 

@@ -35,7 +35,7 @@ def CreateStorageBackend(config: LMCacheEngineConfig, metadata: LMCacheEngineMet
             return LMCLocalCompressedBackend(config, metadata)
         if local in ("cpu", "cuda"):
             from lmcache_b200.storage_backend.local_backend import LMCLocalBackend
-            return LMCLocalBackend(config)
+            return LMCLocalBackend(config, metadata)
         # a directory: the disk tier (LMCLocalDiskBackend, local_backend.py:163-310), here with CacheGen containers
         from lmcache_b200.storage_backend.local_backend import LMCLocalDiskBackend
         return LMCLocalDiskBackend(config, metadata)

@@ -21,11 +21,15 @@ class LMCHybridBackend(LMCBackendInterface):
         super().__init__()
         from lmcache_b200.storage_backend import CreateStorageBackend
         # a capacity bounds the local tier (one of the CacheGen tiers); chunks it evicts are still served by the remote one.
-        # A device level belongs to the local tier as well.
+        # A device level belongs to the local tier as well.  Both tiers code with the engine's bin layout.
         local_cfg = LMCacheEngineConfig(config.chunk_size, config.local_device, None, None, False, config.save_decode_cache,
-                                        config.local_serde, config.local_capacity_bytes, config.device_cache_bytes)
+                                        config.local_serde, config.local_capacity_bytes, config.device_cache_bytes,
+                                        cachegen_config=config.cachegen_config)
         remote_cfg = LMCacheEngineConfig(config.chunk_size, None, config.remote_url, config.remote_serde,
-                                         config.pipelined_backend, config.save_decode_cache, None)
+                                         config.pipelined_backend, config.save_decode_cache, None,
+                                         cachegen_config=config.cachegen_config)
+        # an MLA engine's remote tier takes stores from rank 0 only (LMCRemoteBackend); the local tier, which is this
+        # process's own, takes every rank's
         self.local_store = CreateStorageBackend(local_cfg, metadata)
         self.remote_store = CreateStorageBackend(remote_cfg, metadata)
 
@@ -57,8 +61,9 @@ class LMCHybridBackend(LMCBackendInterface):
         return bool(f and f() and g and g())
 
     def put_kv_chunks(self, keys: List[CacheEngineKey], view, tok_begin: int, chunk_size: int, blocking: bool = True) -> int:
-        self.local_store.put_kv_chunks(keys, view, tok_begin, chunk_size, blocking=True)
-        return self.remote_store.put_kv_chunks(keys, view, tok_begin, chunk_size, blocking=blocking)
+        n = self.local_store.put_kv_chunks(keys, view, tok_begin, chunk_size, blocking=True)
+        self.remote_store.put_kv_chunks(keys, view, tok_begin, chunk_size, blocking=blocking)
+        return n
 
     def get_kv_into(self, keys: List[CacheEngineKey], dst, dst_tok0: int, chunk_size: int) -> int:
         n = self.local_store.get_kv_into(keys, dst, dst_tok0, chunk_size)

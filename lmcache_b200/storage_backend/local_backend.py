@@ -47,11 +47,13 @@ def _copy_async(dst: torch.Tensor, src: torch.Tensor, stream: torch.cuda.Stream)
 
 class LMCLocalBackend(LMCBackendInterface):
 
-    def __init__(self, config: LMCacheEngineConfig):
+    def __init__(self, config: LMCacheEngineConfig, metadata=None):
         super().__init__()
         N.require_cuda()
         self.chunk_size = config.chunk_size
         self.config = config
+        # the engine's KV is latent (metadata.use_mla): chunk blobs are [L,t,D], and only those are its chunks
+        self.latent = bool(getattr(metadata, "use_mla", False))
         self.device = config.local_device       # "cpu" | "cuda"
         self.dst_device = "cuda"                # like the reference (:53): gets land on the GPU
         self.dict: Dict[CacheEngineKey, object] = {}
@@ -115,12 +117,13 @@ class LMCLocalBackend(LMCBackendInterface):
         return True
 
     def peek_geometry(self, key, fmt: str = "vllm"):
-        """(L, H, D, dtype) of a stored chunk blob, from its shape (no copy): [L,2,t,H,D] (vllm) / [L,2,H,t,D] (hf)."""
+        """(L, H, D, dtype) of a stored chunk blob, from its shape (no copy): [L,2,t,H,D] (vllm) / [L,2,H,t,D] (hf); for
+        a latent engine [L,t,D] (H = 1).  None for a blob of the other kind."""
         val = self.dict.get(key, None)
         if val is None:
             return None
         t = val.host if isinstance(val, _HostEntry) else val
-        return KvView.blob_geometry(t, fmt) if t.dim() == 5 else None
+        return KvView.blob_geometry(t, fmt) if t.dim() == (3 if self.latent else 5) else None
 
     def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True) -> int:
         """Store tokens [tok_begin, T) of `view` as len(keys) chunk blobs: ONE gather kernel (b200kv_pack_chunks)
@@ -166,12 +169,18 @@ class LMCLocalBackend(LMCBackendInterface):
                     val.wait()
                 elif not src.is_cuda:
                     src = src.cuda()
-                t = src.shape[KvView.token_dim(dst.fmt)]
+                if src.dim() != blob.dim():
+                    break                                   # a chunk of the other kind (latent / (K, V)): a miss
+                t = src.shape[KvView.token_dim(dst.fmt, dst.latent)]
                 tok = dst_tok0 + i * chunk_size
                 if tok + t > dst.ntokens or src.dtype != blob.dtype:
                     break
                 es = blob.element_size()
-                if fmt_hf:      # rows = (l, kv, h): t*D contiguous elements each
+                if dst.latent:  # rows = l: t*D contiguous elements each
+                    rows, row_bytes = blob.shape[0], t * blob.shape[2] * es
+                    dst_pitch = blob.shape[1] * blob.shape[2] * es
+                    dptr = blob.data_ptr() + tok * blob.shape[2] * es
+                elif fmt_hf:    # rows = (l, kv, h): t*D contiguous elements each
                     rows, row_bytes = blob.shape[0] * 2 * blob.shape[2], t * blob.shape[4] * es
                     dst_pitch = blob.shape[3] * blob.shape[4] * es
                     dptr = blob.data_ptr() + tok * blob.shape[4] * es
@@ -205,7 +214,9 @@ class LMCLocalBackend(LMCBackendInterface):
                     src = val.host.to(dst.device, non_blocking=True)
                 else:
                     src = val if val.is_cuda else val.cuda()
-                t = src.shape[KvView.token_dim(dst.fmt)]
+                if src.dim() != (3 if dst.latent else 5):
+                    break                                   # a chunk of the other kind (latent / (K, V)): a miss
+                t = src.shape[KvView.token_dim(dst.fmt, dst.latent)]
                 tok = dst_tok0 + i * chunk_size
                 if tok + t > dst.ntokens or src.dtype != dst.dtype:
                     break
@@ -333,6 +344,8 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         self.fmt = metadata.fmt
         if self.fmt not in ("vllm", "huggingface"):
             raise ValueError(f"Invalid format: {self.fmt}")
+        # the engine's KV is latent (metadata.use_mla): its containers are version 4, and only those are its chunks
+        self.latent = bool(getattr(metadata, "use_mla", False))
         # ValueError for models outside the bin table (without config.cachegen_config), and for settings that
         # config.cachegen_config rules out
         self.codec = engine_codec(config, metadata.model_name)
@@ -540,9 +553,12 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         return None if e.error is not None or e.rec is None else e
 
     def peek_geometry(self, key, fmt: str = "vllm"):
-        """(L, H, D, output dtype) of the stored chunks, read from a container header (no decode)."""
+        """(L, H, D, output dtype) of the stored chunks, read from a container header (no decode).  None for a container
+        of the other kind (version 4 for a (K, V) engine, or the reverse)."""
         e = self._ready_entry(key)
-        return None if e is None else (e.rec.L, e.rec.H, e.rec.D, self.out_dtype())
+        if e is None or (e.rec.coder == N.CODER_LATENT) != self.latent:
+            return None
+        return e.rec.L, e.rec.H, e.rec.D, self.out_dtype()
 
     def out_dtype(self) -> torch.dtype:
         # the reference's decoder casts by format, ignoring metadata.dtype (cachegen_decoder.py:189-200)
@@ -577,9 +593,13 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
 
     def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int):
         """A pipeline.LayerwiseEncode of tokens [tok_begin, T) of `view` (whose KV may not be written yet), or None
-        when this tier's containers for `chunk_size` are not version 3 (the layer-wise encode writes no other)."""
+        when this tier's containers for `chunk_size` are not version 3, or version 4 for a latent KV (the layer-wise
+        encode writes no other)."""
         from lmcache_b200.pipeline import LayerwiseEncode, SegmentPool
-        if self.codec.coder_for(chunk_size) != N.CODER_RANS_COMPACT:
+        try:
+            if self.codec.coder_for(chunk_size, view.latent) not in (N.CODER_RANS_COMPACT, N.CODER_LATENT):
+                return None
+        except ValueError:
             return None
         if self._segments is None or self._segments.device != view.device:
             if self._segments is not None:
@@ -706,7 +726,8 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         if e is None:
             return None
         r = e.rec
-        out = torch.empty(KvView.blob_shape(self.fmt, r.L, r.H, r.D, r.ntokens), dtype=self.out_dtype(),
+        out = torch.empty(KvView.blob_shape(self.fmt, r.L, r.H, r.D, r.ntokens, r.coder == N.CODER_LATENT),
+                          dtype=self.out_dtype(),
                           device=torch.device("cuda", torch.cuda.current_device()))
         if self.get_kv_into([key], KvView.from_blob(out, self.fmt), 0, r.ntokens) != 1:
             return None
@@ -803,8 +824,8 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
                 size = st.st_size
                 with open(full, "rb") as f:
                     hd = parse_header(f.read(N.HEADER_BYTES + N.MAX_PLANES), size)
-                if int(hd.total_bytes) != size or hd.version == 4:
-                    continue                     # version 4 (a latent KV) is no container of this tier's (K, V) engine
+                if int(hd.total_bytes) != size or (hd.version == 4) != self.latent:
+                    continue                     # version 4 holds a latent KV: a container of a latent engine only
             except (OSError, ValueError):
                 continue                         # damaged / foreign file: not part of the cache
             # "/" in a model name was written as "-": the key of a lookup goes through the same rule, so index by path
@@ -948,7 +969,7 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
         except OSError:
             blk.free()
             return None
-        return read_container(self.codec, blk, nbytes)
+        return read_container(self.codec, blk, nbytes, self.latent)
 
     def _reads(self, keys, level: Optional[_Level]) -> list:
         """futures of the records of `keys` up to the first miss: file reads, or with a device level the index

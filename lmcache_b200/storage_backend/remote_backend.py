@@ -79,6 +79,10 @@ class LMCRemoteBackend(LMCBackendInterface):
         assert config.remote_serde is not None, "Need to provide remote_serde when using LMCRemoteBackend"
         self.connection = CreateConnector(config.remote_url)
         self.serializer, self.deserializer = CreateSerde(config.remote_serde, config, metadata)
+        # a latent KV (metadata.use_mla) is the same on every tensor-parallel rank and its keys are shared: rank 0
+        # alone puts it to the shared tier, the other ranks only read
+        self.latent = bool(getattr(metadata, "use_mla", False))
+        self.puts = not (self.latent and metadata.worker_id != 0)
         self.dst_device = "cuda"
         self._device = torch.cuda.current_device() if torch.cuda.is_available() else None
         self.put_queue: "queue.Queue[Union[Tuple[CacheEngineKey, torch.Tensor], RemoteBackendEndSignal]]" = \
@@ -144,6 +148,8 @@ class LMCRemoteBackend(LMCBackendInterface):
         self.existing_keys.add(key)
 
     def put(self, key: CacheEngineKey, kv_chunk: torch.Tensor, blocking: bool = True) -> None:
+        if not self.puts:
+            return
         if blocking:
             self.put_blocking(key, kv_chunk)
         else:
@@ -225,7 +231,10 @@ class LMCRemoteBackend(LMCBackendInterface):
         """Store tokens [tok_begin, T) of `view` as len(keys) chunks.  Striped path: every wave is encoded on the caller's
         stream before this returns (so a non-blocking store has consumed the caller's KV in stream order -- paged caches
         included -- like the reference's materialised chunk list, cache_engine.py:274-275); D2H and the sends happen on
-        the pipeline's worker.  Other serdes: one batched encode, then one set() per chunk."""
+        the pipeline's worker.  Other serdes: one batched encode, then one set() per chunk.  A latent KV's rank other
+        than 0 stores nothing (returns 0)."""
+        if not self.puts:
+            return 0
         if self._striped():
             if self._pipe is None:
                 from lmcache_b200.pipeline import EncodePipeline
@@ -275,7 +284,7 @@ class LMCRemoteBackend(LMCBackendInterface):
             blk.free()
             return None
         blk.shrink(int(n))                      # the bound covers the largest container version; a v3 one is a tenth of it
-        return read_container(self.deserializer.codec, blk, int(n))
+        return read_container(self.deserializer.codec, blk, int(n), self.latent)
 
     def peek_geometry(self, key: CacheEngineKey, fmt: str = "vllm"):
         """(L, H, D, output dtype) from the header of the first chunk's container.  The fetched container is kept for the
@@ -328,7 +337,7 @@ class LMCRemoteBackend(LMCBackendInterface):
         from lmcache_b200.pipeline import UploadRing, fetched_in_order, upload_decode, wave_chunks_default
         self._release.sweep()
         H = dst.H if windows is None else windows[0].src_H
-        bound = (self.deserializer.container_bound(dst.L, H, dst.D, chunk_size) + 255) & ~255
+        bound = (self.deserializer.container_bound(dst.L, H, dst.D, chunk_size, dst.latent) + 255) & ~255
         ex = self._executor()
         keys = items if windows is None else LazyFlat(items, len(windows))
         peek, self._peek = self._peek, None

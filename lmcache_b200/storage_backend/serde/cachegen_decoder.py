@@ -28,14 +28,15 @@ class CacheGenDeserializer(Deserializer):
         # reference casts by format, ignoring metadata.dtype (cachegen_decoder.py:189-200)
         return torch.bfloat16 if self.fmt == "vllm" else torch.float16
 
-    def _alloc(self, L: int, H: int, D: int, t: int, device) -> torch.Tensor:
-        shape = (L, 2, t, H, D) if self.fmt == "vllm" else (L, 2, H, t, D)
-        return torch.empty(shape, dtype=self._out_dtype(), device=device)
+    def _alloc(self, L: int, H: int, D: int, t: int, device, latent: bool = False) -> torch.Tensor:
+        return torch.empty(KvView.blob_shape(self.fmt, L, H, D, t, latent), dtype=self._out_dtype(), device=device)
 
     @_lmcache_nvtx_annotate
     def from_bytes(self, bs) -> torch.Tensor:
+        """one container -> its chunk blob: [L,2,t,H,D] / [L,2,H,t,D], or [L,t,D] for a version-4 (latent) one"""
         hd = parse_header(bs)
-        out = self._alloc(hd.L, hd.H, hd.D, hd.ntokens, torch.device("cuda", torch.cuda.current_device()))
+        out = self._alloc(hd.L, hd.H, hd.D, hd.ntokens, torch.device("cuda", torch.cuda.current_device()),
+                          hd.version == 4)
         self.codec.decode([bs], KvView.from_blob(out, self.fmt), [0])
         return out
 
@@ -47,9 +48,10 @@ class CacheGenDeserializer(Deserializer):
     def out_dtype(self) -> torch.dtype:
         return self._out_dtype()
 
-    def container_bound(self, L: int, H: int, D: int, chunk_tokens: int) -> int:
-        """Upper bound of one container's size (what a receive slab must reserve per chunk)."""
-        return self.codec.max_container_bytes(L, H, D, chunk_tokens)
+    def container_bound(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> int:
+        """Upper bound of one container's size (what a receive slab must reserve per chunk); `latent`: a version-4
+        container of one plane per layer."""
+        return self.codec.max_container_bytes(L, H, D, chunk_tokens, latent)
 
     def pinned_staging(self, nbytes: int):
         return self.codec.pinned_staging(nbytes)

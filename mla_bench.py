@@ -2,15 +2,20 @@
 workaround of coding the latent tensor as both K and V (version 3 of the pair `(latent, latent)`).
 
     python mla_bench.py [--tokens 8192] [--steps 20] [--warmup 3]
+    python mla_bench.py --engine [--engine-tokens 8192,65536] [--steps 5] [--warmup 1]
 
 61 layers, D = 576 (kv_lora_rank 512 + rope 64), bf16, 256-token chunks, bench.py's kv8d distribution.  The two legs
 alternate in one process; per leg: encode and decode GB/s of LATENT bytes (L * T * 576 * 2, the same for both legs;
 CUDA events, medians), container bytes, and (one-plane leg) the reconstruction error against the input, max abs and
-relative RMS per layer.  Prints one JSON line with the card's name and power limit; writes nothing."""
+relative RMS per layer.  Prints one JSON line with the card's name and power limit; writes nothing.
+
+With --engine the same latent goes through LMCacheEngine instead (engine_legs): an MLA engine (use_mla) against the
+pair workaround through a (K, V) engine, on the CacheGen host tier, the raw cpu tier and the layer-wise retrieve."""
 import argparse
 import json
 import statistics
 import subprocess
+import time
 
 import torch
 
@@ -57,13 +62,98 @@ def _timed(fn):
     return a.elapsed_time(b)
 
 
+_CFG = dict(key_first_layers=10, key_second_layers=20, key_third_layers=L, key_first_bins=32, key_second_bins=16,
+            key_third_bins=16, value_first_layers=2, value_first_bins=32, value_second_bins=16)
+
+
+def _engine(tier, mla):
+    from lmcache_b200.cache_engine import LMCacheEngine
+    from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
+    cfg = LMCacheEngineConfig(CHUNK, "cpu", None, None, False, False, "cachegen" if tier == "host_cachegen" else None,
+                              cachegen_config=_CFG)
+    return LMCacheEngine(cfg, LMCacheEngineMetadata("deepseek-ai/DeepSeek-V3", 1, 0, "vllm", "bfloat16", mla))
+
+
+def _held_bytes(eng):
+    """bytes the local tier keeps: CacheGen containers, or the raw tier's page-locked chunk blobs"""
+    f = getattr(eng.engine_, "host_bytes", None)
+    if f is not None:
+        return int(f())
+    return sum(v.host.numel() * v.host.element_size() for v in eng.engine_.dict.values())
+
+
+def _wall(fn):
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    out = fn()
+    torch.cuda.synchronize()
+    return (time.perf_counter() - t0) * 1e3, out
+
+
+def engine_legs(T, steps, warmup):
+    """LMCacheEngine.store / retrieve of one T-token latent: the MLA engine (one plane per layer) against the pair
+    workaround (the latent as K and V through a (K, V) engine), on the CacheGen host tier and the raw cpu tier, plus the
+    layer-wise retrieve on the CacheGen host tier (host ms until layer 0 and until the last layer are ready).  Host wall
+    ms around a device synchronise, medians; both kinds alternate step by step."""
+    x = _synth_latent(T, seed=2)
+    tokens = torch.arange(T, dtype=torch.int64)
+    kvs = {"mla": tuple(x[l] for l in range(L)),
+           "pair_workaround": tuple((x[l].unsqueeze(1), x[l].unsqueeze(1)) for l in range(L))}
+    res = {}
+    for tier in ("host_cachegen", "raw_cpu"):
+        engines = {k: _engine(tier, k == "mla") for k in kvs}
+        ms = {k: {"store": [], "retrieve": [], "layer0": [], "last_layer": []} for k in kvs}
+        for step in range(warmup + steps):
+            for k, eng in engines.items():
+                s, _ = _wall(lambda: eng.store(tokens, kvs[k], skip_existing=False))
+                r, (kv, mask) = _wall(lambda: eng.retrieve(tokens))
+                assert int(mask.sum()) == T
+                del kv
+                if step >= warmup:
+                    ms[k]["store"].append(s)
+                    ms[k]["retrieve"].append(r)
+                if tier != "host_cachegen":
+                    continue
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                lw = eng.retrieve_layerwise(tokens)
+                lw._upload.ready(0).synchronize()
+                t1 = time.perf_counter()
+                lw.synchronize()
+                t2 = time.perf_counter()
+                del lw
+                if step >= warmup:
+                    ms[k]["layer0"].append((t1 - t0) * 1e3)
+                    ms[k]["last_layer"].append((t2 - t0) * 1e3)
+        for k, eng in engines.items():
+            leg = {f"{op}_ms": statistics.median(v) for op, v in ms[k].items() if v}
+            leg["bytes_held"] = _held_bytes(eng)
+            res.setdefault(tier, {})[k] = leg
+            eng.close()
+        del engines
+        torch.cuda.empty_cache()
+    for tier, legs in res.items():
+        legs["ratios_mla_over_pair"] = {k: legs["mla"][k] / legs["pair_workaround"][k] for k in legs["mla"]}
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--tokens", type=int, default=8192)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--engine", action="store_true",
+                    help="run the LMCacheEngine legs instead of the codec legs, at --engine-tokens")
+    ap.add_argument("--engine-tokens", default="8192,65536")
     args = ap.parse_args()
     from lmcache_b200.codec import CacheGenCodec, KvView
+    if args.engine:
+        torch.cuda.set_device(0)
+        props = torch.cuda.get_device_properties(0)
+        legs = {int(t): engine_legs(int(t), args.steps, args.warmup) for t in args.engine_tokens.split(",")}
+        print(json.dumps(dict(metric="mla_latent_engine", card=props.name, power_limit_w=_power_limit_w(), layers=L,
+                              D=D, chunk=CHUNK, dtype="bf16", data="kv8d", steps=args.steps, tokens=legs)))
+        return
     T = args.tokens
     torch.cuda.set_device(0)
     x = _synth_latent(T, seed=1)
