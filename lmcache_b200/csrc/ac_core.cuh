@@ -694,34 +694,59 @@ constexpr uint32_t kRansLow = 1u << 16;
 // (c[i] <= slot  <=>  entry <= key, because freq <= 0xffff), and the winning entry carries start and freq.
 B2_HD uint32_t rans_table_entry(uint32_t c_i, uint32_t c_next) { return (c_i << 16) | ((c_next - c_i) & 0xffffu); }
 
-// x / f and x mod f for x < f << 16, 1 <= f < 2^16.  Device: one reciprocal, biased low so that the estimate is q or
-// q - 1 (never above), then one fix-up; exact whatever the approximation did.  Host: plain division.
-B2_HD uint32_t rans_divmod(uint32_t x, uint32_t f, uint32_t* rem) {
-#if defined(__CUDA_ARCH__)
-    float rc;
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rc) : "f"(__uint2float_rn(f)));
-    // relative error of float(x) (RZ: <= 0), rcp (1 ulp) and the two products is < 2^-21; the factor keeps the
-    // estimate at or below the true quotient, and q < 2^16 bounds the shortfall by 0.06 < 1
-    uint32_t q = __float2uint_rz(__uint2float_rz(x) * (rc * 0.99999952316284179688f));
-    uint32_t r = x - q * f;
-    if (r >= f) { q += 1u; r -= f; }
-    *rem = r;
-    return q;
-#else
+// x / f and x mod f for x < f << 16, 1 <= f < 2^16, by plain division: the host statement of the encoder step, for
+// tests/hostsim only.  No kernel calls it or rans_enc_symbol, so neither has a device branch; the kernels run rans_put
+// below, whose quotient is a biased reciprocal estimate plus one fix-up.
+inline uint32_t rans_divmod(uint32_t x, uint32_t f, uint32_t* rem) {
     *rem = x % f;
     return x / f;
-#endif
 }
 
 // Encoder step on the state alone; `emit(h)` receives the low halfword when the state must shrink first.
 template <class Emit>
-B2_HD void rans_enc_symbol(uint32_t& x, uint32_t start, uint32_t freq, Emit&& emit) {
+inline void rans_enc_symbol(uint32_t& x, uint32_t start, uint32_t freq, Emit&& emit) {
     const uint32_t xh = x >> 16;
     if (xh >= freq) { emit(x & 0xffffu); x = xh; }
     uint32_t r;
     const uint32_t q = rans_divmod(x, freq, &r);
     x = (q << 16) + r + start;
 }
+
+#if defined(__CUDACC__)
+// rANS encoder step as the kernels run it (same arithmetic as rans_enc_symbol, laid out for issue slots):
+//   * the state shrinks by one halfword when it must; halfword number k (counted downwards: nk = -k) lands at
+//     row_end + 2 * nk - 2, so the row's tail holds the halfwords in decode order.  The address is one unpredicated
+//     IMAD.WIDE, only the 16-bit store and the count are predicated;
+//   * q = x / f by one reciprocal biased low and one fix-up.  The estimate is q or q - 1 for EVERY x < f << 16,
+//     1 <= f < 2^16: tests/devsim runs this function on an H100 at both ends of every quotient bucket [q f, q f + f)
+//     (the estimate is monotone in x, the quotient constant on a bucket), 8.6e9 steps, and compares with integer
+//     division: no wrong state; the fix-up is taken at every x = q f and, for f > 1, at no x = q f + f - 1 (NVIDIA H100
+//     80GB HBM3, 700 W limit; tests/test_gpu_rans_edges.py::test_rans_put_exhaustive_sweep);
+//   * x' = (q << 16) + (x - q f) + start  ==  x + start + q * (65536 - f).
+__device__ __forceinline__ void rans_put(uint32_t& x, int32_t& nk, const uint16_t* row_end, uint32_t start, uint32_t freq) {
+    const uint32_t xh = x >> 16;
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t.reg .b64 ad;\n\t"
+        "setp.ge.u32 p, %2, %3;\n\t"
+        "mad.wide.s32 ad, %1, 2, %4;\n\t"
+        "@p st.global.u16 [ad+-2], %0;\n\t"
+        "@p add.s32 %1, %1, -1;\n\t"
+        "selp.b32 %0, %2, %0, p;\n\t"
+        "}"
+        : "+r"(x), "+r"(nk) : "r"(xh), "r"(freq), "l"(row_end) : "memory");
+    float rc;
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rc) : "f"(__uint2float_rn(freq)));
+    const uint32_t q = __float2uint_rz(__uint2float_rz(x) * (rc * 0.99999952316284179688f));   // floor(x / f) or one less
+    // With m = 65536 - f:  a = q m + x;  x - q f = a - (q << 16);  x' = a + start, plus m when the estimate was one short.
+    // Six integer instructions (m, a, r, compare, add, predicated add) where "negate f, r, compare, q + 1, select, x +
+    // start, m, multiply-add" took eight (ncu, round 2).
+    const uint32_t m = 65536u - freq;
+    const uint32_t a = q * m + x;
+    const uint32_t r = a - (q << 16);
+    x = a + start;
+    if (r >= freq) x += m;
+}
+#endif
 
 // Decoder state: x plus a two-word window over the stream's halfwords (aligned 32-bit loads, one word of look-ahead).
 // `sel` is the PRMT selector that builds (x << 16) | next halfword from (x, cur): 0x1054 takes cur's low half,

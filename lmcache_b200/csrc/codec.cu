@@ -317,35 +317,8 @@ __device__ __forceinline__ void for_each_symbol_rev(const uint16_t* cbase, const
     }
 }
 
-// rANS encoder step as the kernels run it (same arithmetic as rans_enc_symbol in ac_core.cuh, laid out for issue slots):
-//   * the state shrinks by one halfword when it must; halfword number k (counted downwards: nk = -k) lands at
-//     row_end + 2 * nk - 2, so the row's tail holds the halfwords in decode order.  The address is one unpredicated
-//     IMAD.WIDE, only the 16-bit store and the count are predicated;
-//   * q = x / f by one reciprocal biased low (estimate is q or q - 1) and one fix-up;
-//   * x' = (q << 16) + (x - q f) + start  ==  x + start + q * (65536 - f).
-__device__ __forceinline__ void rans_put(uint32_t& x, int32_t& nk, const uint16_t* row_end, uint32_t start, uint32_t freq) {
-    const uint32_t xh = x >> 16;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 ad;\n\t"
-        "setp.ge.u32 p, %2, %3;\n\t"
-        "mad.wide.s32 ad, %1, 2, %4;\n\t"
-        "@p st.global.u16 [ad+-2], %0;\n\t"
-        "@p add.s32 %1, %1, -1;\n\t"
-        "selp.b32 %0, %2, %0, p;\n\t"
-        "}"
-        : "+r"(x), "+r"(nk) : "r"(xh), "r"(freq), "l"(row_end) : "memory");
-    float rc;
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rc) : "f"(__uint2float_rn(freq)));
-    const uint32_t q = __float2uint_rz(__uint2float_rz(x) * (rc * 0.99999952316284179688f));   // floor(x / f) or one less
-    // With m = 65536 - f:  a = q m + x;  x - q f = a - (q << 16);  x' = a + start, plus m when the estimate was one short.
-    // Six integer instructions (m, a, r, compare, add, predicated add) where "negate f, r, compare, q + 1, select, x +
-    // start, m, multiply-add" took eight (ncu, round 2).
-    const uint32_t m = 65536u - freq;
-    const uint32_t a = q * m + x;
-    const uint32_t r = a - (q << 16);
-    x = a + start;
-    if (r >= freq) x += m;
-}
+// The rANS encoder step the kernels below run, rans_put, lives in ac_core.cuh, where the test-only device build
+// (tests/devsim) can reach it.
 
 // ------------------------------------------------------------------------------------------ encode
 // One tile = CT consecutive channels of one plane and one <= 256-token group; one thread = one coder stream.
