@@ -66,6 +66,11 @@ struct EncParams {
     uint32_t* tile_tot;              // [n_chunks][tiles_full] bytes per tile, then exclusive prefix (in place)
     unsigned long long* totals;      // [n_chunks] payload bytes
     unsigned int* err;               // [n_chunks]
+    // encode_kernel<FUSED = true> (persistent): the next work item to claim, and per (chunk, launch plane) the number of
+    // absmax items done; both zero at launch
+    unsigned int* ticket;
+    unsigned int* ready;             // [n_chunks][ppl * nlay]
+    int32_t vec;                     // every plane's rows allow 128-bit loads (absmax)
     int32_t lb, nlay;                // this launch codes layers [lb, lb + nlay): planes lb.. and L + lb.. (all: 0, L)
     // b200kv_encode_layers only (NULL / 0 otherwise): the payload goes to a device arena instead of out + j * out_stride
     uint8_t* arena;
@@ -161,11 +166,49 @@ __device__ __forceinline__ int64_t tok_row(const int64_t* slot_map, int64_t tok)
 // max1 = amax(|x|, channels) per (plane, token), kept in the input half dtype
 // (cachegen_encoder.py:54-55).  |x| ordering == integer ordering of (bits & 0x7fff); a NaN in the row
 // wins (pattern above inf), like torch.amax.  One warp per row, 128-bit loads when alignment allows.
-// Round 2 tried to hide this kernel -- the only HBM-bound one of the path -- under the instruction-bound coding kernels of
-// the previous wave (second stream, 128-thread blocks with <= 32 registers so that a block fits next to them): no gain.
-// Both coder kernels fill the SM's shared memory with their own CTAs (7 x 32.5 KB, 12 x 18.6
-// KB incl. the 1 KB the system reserves per CTA), so not even a block without shared memory finds room; the kernels only
-// overlap at their tails.  Measured, rejected.
+// Chunks of <= 256 tokens do not launch absmax_kernel: the persistent encode_kernel<FUSED = true> computes the maxima
+// itself, as work items ordered ahead of the tiles that read them (encode_kernel).  A separate kernel cannot hide this
+// HBM-bound pass under the instruction-bound coder: round 2 tried it on a second stream (128-thread blocks with <= 32
+// registers) with no gain -- both coder kernels fill the SM's shared memory with their own CTAs (7 x 32.5 KB, 12 x 18.6
+// KB incl. the 1 KB the system reserves per CTA), so not even a block without shared memory finds room.  Chunks of more
+// than 256 tokens still launch it: their chunk-wide CDF (cdf_kernel) needs every maximum of the chunk first.
+//
+// The bits of |x| of one row (C channels at row, head pitch sH) reduced to their maximum over the warp.
+template <bool VEC>
+__device__ __forceinline__ uint32_t row_absmax(const EncParams& P, const uint16_t* row, int lane) {
+    uint32_t m = 0;
+    if (VEC) {
+        const int vec_per_head = P.D >> 3;
+        const int nvec = P.H * vec_per_head;
+        // batches of 4 loads per lane, all in flight before the first is used (a slot past the row reads as 0)
+        constexpr int B = 4;
+        for (int v0 = lane; v0 < nvec; v0 += 32 * B) {
+            uint4 q[B];
+#pragma unroll
+            for (int b = 0; b < B; ++b) {
+                const int v = v0 + 32 * b;
+                const int h = v / vec_per_head, dv = v - h * vec_per_head;
+                q[b] = v < nvec ? __ldg(reinterpret_cast<const uint4*>(row + (int64_t)h * P.sH + dv * 8)) : make_uint4(0, 0, 0, 0);
+            }
+#pragma unroll
+            for (int b = 0; b < B; ++b) {
+                const uint32_t w[4] = {q[b].x, q[b].y, q[b].z, q[b].w};
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const uint32_t a = w[k] & 0x7fff7fffu;
+                    m = max(m, max(a & 0xffffu, a >> 16));
+                }
+            }
+        }
+    } else {
+        for (int c = lane; c < P.C; c += 32) {
+            const int h = c / P.D, d = c - h * P.D;
+            m = max(m, (uint32_t)(__ldg(row + (int64_t)h * P.sH + d) & 0x7fffu));
+        }
+    }
+    return __reduce_max_sync(0xffffffffu, m);
+}
+
 template <bool VEC, bool PAGED>
 __global__ void __launch_bounds__(256) absmax_kernel(EncParams P, int64_t total_tokens) {
     const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
@@ -175,27 +218,7 @@ __global__ void __launch_bounds__(256) absmax_kernel(EncParams P, int64_t total_
     const int nl = launch_plane(P, (int)(warp / total_tokens));
     const int64_t T = warp % total_tokens;
     const uint16_t* row = P.pt.p[nl] + tok_row<PAGED>(P.slot_map, P.tok_begin + T) * P.sT;
-    uint32_t m = 0;
-    if (VEC) {
-        const int vec_per_head = P.D >> 3;
-        const int nvec = P.H * vec_per_head;
-        for (int v = lane; v < nvec; v += 32) {
-            const int h = v / vec_per_head, dv = v - h * vec_per_head;
-            const uint4 q = __ldg(reinterpret_cast<const uint4*>(row + (int64_t)h * P.sH + dv * 8));
-            const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const uint32_t a = w[k] & 0x7fff7fffu;
-                m = max(m, max(a & 0xffffu, a >> 16));
-            }
-        }
-    } else {
-        for (int c = lane; c < P.C; c += 32) {
-            const int h = c / P.D, d = c - h * P.D;
-            m = max(m, (uint32_t)(__ldg(row + (int64_t)h * P.sH + d) & 0x7fffu));
-        }
-    }
-    m = __reduce_max_sync(0xffffffffu, m);
+    const uint32_t m = row_absmax<VEC>(P, row, lane);
     if (lane == 0) {
         const int j = (int)(T / P.chunk_tokens);
         const int tj = chunk_tokens_of(P, j);
@@ -323,17 +346,50 @@ __device__ __forceinline__ void for_each_symbol_rev(const uint16_t* cbase, const
 // ------------------------------------------------------------------------------------------ encode
 // One tile = CT consecutive channels of one plane and one <= 256-token group; one thread = one coder stream.
 // FUSED (chunk <= 256 tokens): quantise -> 5-bit symbols in shared memory + thread-private histogram -> CDF (the
-//   33-entry rows are contiguous in smem and in the container: one coalesced copy) -> arithmetic coding.  KV is read
-//   from HBM exactly once here (plus once by absmax).
+//   33-entry rows are contiguous in smem and in the container: one coalesced copy) -> arithmetic coding.  The kernel is
+//   persistent and also computes the maxima the tiles read (absmax_item).
 // !FUSED (chunk > 256 tokens): the chunk-wide CDF was produced by cdf_kernel; one tile codes one group, quantising
 //   on the fly.
 // Coder output goes to the tile's temp rows in global memory (sparse 32-bit stores, merged in L2); stream lengths go to
 // the container; the tile's byte total goes to tile_tot.  Compaction into the contiguous payload (collect_bytes in the
-// reference) is done by scan_kernel + compact_kernel afterwards, so no CTA ever waits on another one.
-template <bool FUSED, int DT, bool PAGED, int CODER>
-__global__ void __launch_bounds__(CT, FUSED ? 7 : 4) encode_kernel(EncParams P) {
-    // 128-byte aligned base (also in cdf_kernel and decode_kernel): the shared-memory layout the kernels were measured with
-    extern __shared__ __align__(128) uint32_t smem[];
+// reference) is done by scan_kernel + compact_kernel afterwards.
+//
+// Persistent schedule (FUSED): a unit is one (chunk j, launch plane); its work is kAbsItems absmax items (kAbsRows token
+// rows each, over all C channels) and tpp tiles.  Tickets are claimed with one atomicAdd each and come in steps of
+// kAbsItems + tpp: step s holds the absmax items of unit s, then the tiles of unit s - kAbsLead.  A tile waits until its
+// unit's ready counter shows every absmax item done.
+// Measured on the H100 (DESIGN.md 3.2): 8 rows and a lead of 8 units beat 16 rows and leads of 2, 8 or 16 units.
+constexpr int kAbsRows = 8;                   // token rows per absmax item: 2 per warp
+constexpr int kAbsItems = kGroup / kAbsRows;  // absmax items per unit (a ragged chunk's unused items only count as done)
+constexpr int kAbsLead = 8;                   // units by which a unit's absmax items run ahead of its tiles
+
+// The maxima of token rows [item * kAbsRows, +kAbsRows) of one unit, written to the container's maxes section exactly as
+// absmax_kernel writes them; then the unit's ready counter goes up by one.  Uses no shared memory.
+template <bool PAGED>
+__device__ __forceinline__ void absmax_item(const EncParams& P, int unit, int item) {
+    const int nloc = P.ppl * P.nlay;
+    const int j = unit / nloc;
+    const int nl = launch_plane(P, unit - j * nloc);
+    const int tj = chunk_tokens_of(P, j);
+    const Layout lo = layout_of(P, tj);
+    uint16_t* maxes = reinterpret_cast<uint16_t*>(P.out + (int64_t)j * P.out_stride + lo.off_maxes) + (int64_t)nl * tj;
+    const int64_t tok0 = P.tok_begin + (int64_t)j * P.chunk_tokens;
+    const int lane = threadIdx.x & 31;
+    const int r0 = item * kAbsRows, r1 = min(tj, (item + 1) * kAbsRows);
+    for (int r = r0 + (threadIdx.x >> 5); r < r1; r += CT / 32) {
+        const uint16_t* row = P.pt.p[nl] + tok_row<PAGED>(P.slot_map, tok0 + r) * P.sT;
+        const uint32_t m = P.vec ? row_absmax<true>(P, row, lane) : row_absmax<false>(P, row, lane);
+        if (lane == 0) {
+            maxes[r] = (uint16_t)m;
+            __threadfence();
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(P.ready + unit) : "memory");
+}
+
+template <bool FUSED, int DT, bool PAGED, int CODER, class TileOf>
+__device__ __forceinline__ void encode_tile(const EncParams& P, TileOf tile_of, uint32_t* smem, uint32_t* s_warp) {
     // FUSED : symbol rows u32[CT][SYMW] | cdf rows u16[CT][33] (also the histogram) | fac[256] (later fl32(n/t)[257])
     // !FUSED: pair rows u32[CT][33]                                                 | fac[256]
     constexpr int ROWS_W = FUSED ? CT * SYMW : 0;
@@ -341,11 +397,11 @@ __global__ void __launch_bounds__(CT, FUSED ? 7 : 4) encode_kernel(EncParams P) 
     uint32_t* rows = smem;
     uint32_t* tab = smem + ROWS_W;
     float* fac = reinterpret_cast<float*>(smem + ((ROWS_W + TAB_W + 3) & ~3));
-    __shared__ uint32_t s_warp[CT / 32];
 
     const int tid = threadIdx.x;
     TileId id;
-    if (!decode_tile(P, blockIdx.x, &id)) return;
+    const uint32_t tile = tile_of();
+    if (!decode_tile(P, tile, &id)) return;
     const int NL = P.ppl * P.L;
     const int j = id.j, nl = id.nl, ct = id.ct, t = id.t, gt = id.gt;
     const int c = ct * CT + tid;
@@ -357,9 +413,31 @@ __global__ void __launch_bounds__(CT, FUSED ? 7 : 4) encode_kernel(EncParams P) 
     const uint16_t* maxes = reinterpret_cast<const uint16_t*>(cont + lo.off_maxes) + (int64_t)nl * t + id.tok0;
     const float maxq = P.pt.maxq[nl];
     const int64_t s1 = P.sT;
-    // FUSED: "safe" factors (an infinite factor becomes NaN: same symbols, and pass 1 can skip the range check)
+    if (FUSED) {
+        // Wait for the unit's kAbsItems absmax items.  Why this wait always ends, whatever order the hardware launches or
+        // schedules CTAs in: tickets are handed out in increasing order, one atomicAdd each, and a CTA claims a ticket
+        // only while it is running and only after finishing its previous item.  The absmax items of this tile's unit
+        // hold smaller tickets (step u against step u + kAbsLead), so each of them was claimed before this tile was, by
+        // a CTA that is resident now or has finished.  An absmax item waits on nothing, so each one completes.  No work
+        // item waits on a later ticket: there is no cycle, and nothing spins on work that is not yet running.
+        if (tid == 0) {
+            const unsigned int* rd = P.ready + tile / (uint32_t)P.tpp;
+            uint32_t ns = 32u;
+            for (;;) {
+                uint32_t v;
+                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(rd) : "memory");
+                if (v >= (uint32_t)kAbsItems) break;
+                __nanosleep(ns);
+                ns = min(2u * ns, 1024u);
+            }
+        }
+        __syncthreads();
+    }
+    // FUSED: "safe" factors (an infinite factor becomes NaN: same symbols, and pass 1 can skip the range check).  The
+    // maxima of this launch are read past L1 (__ldcg): L1 is not coherent with the other SMs' writes.
     for (int i = tid; i < gt; i += CT)
-        fac[i] = FUSED ? quant_factor_safe(maxq, half_to_float(maxes[i], DT)) : quant_factor(maxq, half_to_float(maxes[i], DT));
+        fac[i] = FUSED ? quant_factor_safe(maxq, half_to_float(__ldcg(maxes + i), DT))
+                       : quant_factor(maxq, half_to_float(maxes[i], DT));
     if (FUSED) for (int i = gt + tid; i < kGroup + 8; i += CT) fac[i] = 0.0f;      // padded slots of the last batch
 
     const int h = active ? c / P.D : 0;
@@ -367,7 +445,7 @@ __global__ void __launch_bounds__(CT, FUSED ? 7 : 4) encode_kernel(EncParams P) 
     const int64_t tokabs = P.tok_begin + (int64_t)j * P.chunk_tokens + id.tok0;
     const uint16_t* cbase = P.pt.p[nl] + (int64_t)h * P.sH + (active ? c - h * P.D : 0);
     const uint16_t* src = cbase + (PAGED ? 0 : tokabs * P.sT);          // !PAGED: token tk is at src + tk * sT
-    uint32_t* trow = P.temp + ((int64_t)blockIdx.x * CT + tid) * P.tempw;
+    uint32_t* trow = P.temp + ((int64_t)tile * CT + tid) * P.tempw;
     uint32_t cap = (uint32_t)P.tempw;
     // keep the row pointer and the capacity as plain register values: otherwise every flush re-derives the address
     // from (tile, tid, tempw, base) with six extra instructions
@@ -491,7 +569,7 @@ __global__ void __launch_bounds__(CT, FUSED ? 7 : 4) encode_kernel(EncParams P) 
             if (P.compact) {
                 uint32_t w0, w1;
                 hlen = build_stream_header(cnt, mask, wany, 2 * ((int)maxq + 1), trow, w0, w1);
-                reinterpret_cast<uint2*>(P.rstate)[((int64_t)blockIdx.x * CT + tid) * 2] = make_uint2(w0, w1);
+                reinterpret_cast<uint2*>(P.rstate)[((int64_t)tile_of() * CT + tid) * 2] = make_uint2(w0, w1);
             }
         }
         __syncthreads();
@@ -524,8 +602,8 @@ __global__ void __launch_bounds__(CT, FUSED ? 7 : 4) encode_kernel(EncParams P) 
 #pragma unroll
                 for (int k = SPW - 1; k >= 0; --k) code(word, k);
             }
-            if (P.compact) reinterpret_cast<uint2*>(P.rstate)[((int64_t)blockIdx.x * CT + tid) * 2 + 1] = make_uint2(x, hlen);
-            else P.rstate[(int64_t)blockIdx.x * CT + tid] = x;
+            if (P.compact) reinterpret_cast<uint2*>(P.rstate)[((int64_t)tile_of() * CT + tid) * 2 + 1] = make_uint2(x, hlen);
+            else P.rstate[(int64_t)tile_of() * CT + tid] = x;
             len = hlen + 4u - 2u * (uint32_t)nk;
         } else if (active) {
             EncState2 st;
@@ -577,7 +655,7 @@ __global__ void __launch_bounds__(CT, FUSED ? 7 : 4) encode_kernel(EncParams P) 
                     const uint32_t pr = prow[q];
                     rans_put(x, nk, wend, pr & 0xffffu, pr >> 16);
                 });
-                P.rstate[(int64_t)blockIdx.x * CT + tid] = x;
+                P.rstate[(int64_t)tile_of() * CT + tid] = x;
                 len = 4u - 2u * (uint32_t)nk;
             } else {
                 EncState2 st;
@@ -597,6 +675,48 @@ __global__ void __launch_bounds__(CT, FUSED ? 7 : 4) encode_kernel(EncParams P) 
     uint32_t tile_total;
     (void)block_excl_scan(len, s_warp, &tile_total);
     if (tid == 0) P.tile_tot[(int64_t)j * P.tiles_full + id.tile_in_chunk] = tile_total;
+}
+
+// FUSED: persistent, occupancy x SM count CTAs claiming tickets (see above); !FUSED: one tile per CTA
+template <bool FUSED, int DT, bool PAGED, int CODER>
+__global__ void __launch_bounds__(CT, FUSED ? 7 : 4) encode_kernel(EncParams P) {
+    // 128-byte aligned base (also in cdf_kernel and decode_kernel): the shared-memory layout the kernels were measured with
+    extern __shared__ __align__(128) uint32_t smem[];
+    __shared__ uint32_t s_warp[CT / 32];
+    if constexpr (!FUSED) {
+        encode_tile<false, DT, PAGED, CODER>(P, [] { return (uint32_t)blockIdx.x; }, smem, s_warp);
+    } else {
+        // thread 0 claims the ticket and names the work in s_work: a tile, an absmax item (kWorkAbsmax | unit *
+        // kAbsItems + item), a ticket without work, or the end.  Nothing of the schedule stays live in registers across
+        // an item, and the tile body reads its index back from s_work where it needs it late, so it keeps the registers
+        // it had as a kernel of its own.
+        constexpr uint32_t kWorkDone = 0xffffffffu, kWorkNone = 0xfffffffeu, kWorkAbsmax = 0x80000000u;
+        __shared__ uint32_t s_work;
+        for (;;) {
+            __syncthreads();   // the previous item is done with shared memory and s_work
+            if (threadIdx.x == 0) {
+                const uint32_t units = (uint32_t)P.n_chunks * (uint32_t)(P.ppl * P.nlay);
+                const uint32_t step = (uint32_t)(kAbsItems + P.tpp);
+                const uint32_t k = atomicAdd(P.ticket, 1u);
+                const uint32_t s = k / step, r = k - s * step;
+                uint32_t w = kWorkNone;
+                if (s >= units + kAbsLead) w = kWorkDone;
+                else if (r < (uint32_t)kAbsItems) { if (s < units) w = kWorkAbsmax | (s * kAbsItems + r); }
+                else if (s >= (uint32_t)kAbsLead) w = (s - kAbsLead) * (uint32_t)P.tpp + (r - kAbsItems);
+                s_work = w;
+            }
+            __syncthreads();
+            const uint32_t w = s_work;
+            if (w == kWorkDone) break;
+            if (w == kWorkNone) continue;
+            if (w & kWorkAbsmax) {
+                const uint32_t a = w & ~kWorkAbsmax;
+                absmax_item<PAGED>(P, (int)(a / kAbsItems), (int)(a % kAbsItems));
+            } else {
+                encode_tile<true, DT, PAGED, CODER>(P, [] { return *static_cast<volatile uint32_t*>(&s_work); }, smem, s_warp);
+            }
+        }
+    }
 }
 
 // ------------------------------------------------------------------------------------------ cdf (chunks > 256 tokens)
@@ -1620,12 +1740,16 @@ static int enc_tempw(bool fused, int coder, bool compact = false) {
     return fused ? (coder == CODER_RANS ? TEMPW_FUSED_RANS : TEMPW_FUSED) : TEMPW_SPLIT;
 }
 
-static size_t enc_ws_layout(int64_t n_tiles_alloc, int n_chunks, int tempw, int coder, bool compact, size_t* off_tot,
-                            size_t* off_totals, size_t* off_err, size_t* off_state, size_t* off_temp) {
+// Everything in front of off_state is zeroed by every call.  sync: encode_kernel<FUSED = true>'s ticket counter, then
+// one ready counter per unit (n_units = chunks x planes)
+static size_t enc_ws_layout(int64_t n_tiles_alloc, int n_chunks, int64_t n_units, int tempw, int coder, bool compact,
+                            size_t* off_tot, size_t* off_totals, size_t* off_err, size_t* off_sync, size_t* off_state,
+                            size_t* off_temp) {
     size_t o = 0;
     *off_tot = o;    o += (size_t)n_tiles_alloc * 4;  o = (o + 255) & ~(size_t)255;
     *off_totals = o; o += (size_t)n_chunks * 8;       o = (o + 255) & ~(size_t)255;
     *off_err = o;    o += (size_t)n_chunks * 4;       o = (o + 255) & ~(size_t)255;
+    *off_sync = o;   o += (size_t)(1 + n_units) * 4;  o = (o + 255) & ~(size_t)255;
     *off_state = o;  o += coder == CODER_RANS ? (size_t)n_tiles_alloc * CT * (compact ? 16 : 4) : 0;  o = (o + 255) & ~(size_t)255;
     *off_temp = o;   o += (size_t)n_tiles_alloc * CT * (size_t)tempw * 4;
     return (o + 255) & ~(size_t)255;
@@ -1633,9 +1757,9 @@ static size_t enc_ws_layout(int64_t n_tiles_alloc, int n_chunks, int tempw, int 
 
 // b200kv_encode_layers_plan's workspace: the state that lives across calls (err, running payload totals, chunk bases,
 // cursor + fail_from), then one call's scratch -- tile totals, payload totals, coder states and temp rows for the tiles
-// of at most max_layers layers.
-struct EnclWs { size_t err, ptotal, cbase, state, tot, totals, rstate, temp, bytes; };
-static EnclWs encl_ws_layout(int n_chunks, int64_t call_tiles) {
+// of at most max_layers layers, and encode_kernel's ticket and ready counters for the units (chunks x planes) of such a call.
+struct EnclWs { size_t err, ptotal, cbase, state, tot, totals, sync, rstate, temp, bytes; };
+static EnclWs encl_ws_layout(int n_chunks, int64_t call_tiles, int64_t call_units) {
     EnclWs w;
     size_t o = 0;
     auto take = [&](size_t* off, size_t n) { *off = o; o = (o + n + 255) & ~(size_t)255; };
@@ -1645,6 +1769,7 @@ static EnclWs encl_ws_layout(int n_chunks, int64_t call_tiles) {
     take(&w.state, 16);
     take(&w.tot, (size_t)call_tiles * 4);
     take(&w.totals, (size_t)n_chunks * 8);
+    take(&w.sync, (size_t)(1 + call_units) * 4);
     take(&w.rstate, (size_t)call_tiles * CT * 16);
     take(&w.temp, (size_t)call_tiles * CT * TEMPW_FUSED_RANS_HDR * 4);
     w.bytes = o;
@@ -1698,10 +1823,17 @@ static_assert(sizeof(EncPlan) <= sizeof(b200kv_encode_plan_t), "b200kv_encode_pl
 constexpr size_t kSmemFused = (size_t)(((CT * SYMW + (CT * kLp * 2 + 3) / 4 + 3) & ~3) + kGroup + 8) * 4;
 constexpr int kStageRans = 12 * 1024;   // compact_kernel's stage without an entropy hint (b200kv_encode_chunks)
 
-// absmax over the rows of the launch's planes (P.lb, P.nlay) and tokens [0, total_tokens) of the call
-static int launch_absmax(const EncParams& P, const b200kv_kv_desc* kv, int64_t total_tokens, cudaStream_t stream) {
-    bool vec = (kv->D % 8 == 0) && (kv->sT % 8 == 0) && (kv->sH % 8 == 0);
+// every plane's token rows can be read with 128-bit loads
+static bool rows_vec(const EncParams& P) {
+    bool vec = (P.D % 8 == 0) && (P.sT % 8 == 0) && (P.sH % 8 == 0);
     for (int nl = 0; nl < P.ppl * P.L && vec; ++nl) vec = (reinterpret_cast<uintptr_t>(P.pt.p[nl]) & 15) == 0;
+    return vec;
+}
+
+// absmax over the rows of the launch's planes (P.lb, P.nlay) and tokens [0, total_tokens) of the call (chunks > 256
+// tokens; shorter chunks have encode_kernel compute their maxima)
+static int launch_absmax(const EncParams& P, int64_t total_tokens, cudaStream_t stream) {
+    const bool vec = P.vec != 0;
     const bool paged = P.slot_map != nullptr;
     const int64_t rows = (int64_t)P.ppl * P.nlay * total_tokens;
     const int64_t blocks = (rows + 7) / 8;
@@ -1710,6 +1842,30 @@ static int launch_absmax(const EncParams& P, const b200kv_kv_desc* kv, int64_t t
     else if (vec) absmax_kernel<true, true><<<(unsigned)blocks, 256, 0, stream>>>(P, total_tokens);
     else if (!paged) absmax_kernel<false, false><<<(unsigned)blocks, 256, 0, stream>>>(P, total_tokens);
     else absmax_kernel<false, true><<<(unsigned)blocks, 256, 0, stream>>>(P, total_tokens);
+    B2_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// The persistent encode_kernel<FUSED = true>: as many CTAs as fit on the device at once (the occupancy is asked once per
+// instantiation), never more than there are tickets.  P.ticket and P.ready must be zero.
+template <int DT, bool PAGED, int CODER>
+static int launch_encode_fused(const EncParams& P, cudaStream_t stream) {
+    static int occ = 0;
+    auto kern = encode_kernel<true, DT, PAGED, CODER>;
+    B2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemFused));
+    if (occ == 0) {
+        int n = 0;
+        B2_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, CT, kSmemFused));
+        B2_REQUIRE(n > 0, "encode_kernel does not fit on this device");
+        occ = n;
+    }
+    int dev = 0, sms = 0;
+    B2_CHECK_CUDA(cudaGetDevice(&dev));
+    B2_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const int64_t tickets = ((int64_t)P.n_chunks * P.ppl * P.nlay + kAbsLead) * (kAbsItems + P.tpp);
+    B2_REQUIRE(tickets < (1ll << 31) - 2, "too many work items in one call");
+    const int64_t grid = std::min<int64_t>((int64_t)occ * sms, tickets);
+    kern<<<(unsigned)grid, CT, kSmemFused, stream>>>(P);
     B2_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1815,8 +1971,9 @@ int64_t b200kv_encode_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t c
     if (ppl == 1 && !compact) return -2;
     const int64_t G = (chunk_tokens + kGroup - 1) / kGroup;
     const int64_t n_tiles = (int64_t)n_chunks * G * ppl * L * tiles_per_plane(H * D);
-    size_t a, b, c, d, e;
-    return (int64_t)enc_ws_layout(n_tiles, n_chunks, enc_tempw(chunk_tokens <= kGroup, coder, compact), coder, compact, &a, &b, &c, &d, &e);
+    size_t a, b, c, d, e, f;
+    return (int64_t)enc_ws_layout(n_tiles, n_chunks, (int64_t)n_chunks * ppl * L, enc_tempw(chunk_tokens <= kGroup, coder, compact),
+                                  coder, compact, &a, &b, &c, &d, &e, &f);
 }
 
 int64_t b200kv_decode_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t chunk_tokens, int32_t n_chunks) {
@@ -1871,9 +2028,9 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
     const bool fused = chunk_tokens <= kGroup;
     P.tiles_full = (int32_t)tiles_full;
     P.tempw = enc_tempw(fused, coder, P.compact != 0);
-    size_t off_tot, off_totals, off_err, off_state, off_temp;
-    const size_t need = enc_ws_layout(n_tiles, n_chunks, P.tempw, coder, P.compact != 0, &off_tot, &off_totals, &off_err, &off_state,
-                                      &off_temp);
+    size_t off_tot, off_totals, off_err, off_sync, off_state, off_temp;
+    const size_t need = enc_ws_layout(n_tiles, n_chunks, (int64_t)n_chunks * P.ppl * P.L, P.tempw, coder, P.compact != 0, &off_tot,
+                                      &off_totals, &off_err, &off_sync, &off_state, &off_temp);
     B2_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)need, "workspace too small");
     B2_REQUIRE(n_tiles < (1ll << 31) && tiles_full < (1ll << 31), "too many tiles in one call");
     uint8_t* ws = static_cast<uint8_t*>(workspace);
@@ -1882,17 +2039,20 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
     P.err = reinterpret_cast<unsigned int*>(ws + off_err);
     P.temp = reinterpret_cast<uint32_t*>(ws + off_temp);
     P.rstate = reinterpret_cast<uint32_t*>(ws + off_state);
+    P.ticket = reinterpret_cast<unsigned int*>(ws + off_sync);
+    P.ready = P.ticket + 1;
+    P.vec = rows_vec(P) ? 1 : 0;
     B2_CHECK_CUDA(cudaMemsetAsync(ws, 0, off_state, stream));    // counters only; states and temp rows need no init
 
-    // 1) per-(plane, token) absmax -> maxes sections
+    // 1) per-(plane, token) absmax -> maxes sections: a kernel of its own for chunks > 256 tokens, inside encode_kernel
+    //    for the others
     const int64_t total_tokens = (int64_t)(n_chunks - 1) * chunk_tokens + last_chunk_tokens;
     for (int i = 0; i <= kProfFinalize; ++i) g_prof_have[i] = false;
-    {
+    if (!fused) {
         ProfScope prof(kProfAbsmax, stream);
-        if (int rc = launch_absmax(P, kv, total_tokens, stream)) return rc;
+        if (int rc = launch_absmax(P, total_tokens, stream)) return rc;
     }
     // 2) encode (streams -> temp rows, lengths, tile totals)
-    const size_t smem_fused = kSmemFused;
     const size_t smem_split = (size_t)(((CT * PAIRW + 3) & ~3) + kGroup + 4) * 4;
     const size_t smem_cdf = (size_t)(CT * PAIRW + kGroup) * 4;
 #define B2_LAUNCH_ENC1(FUSED, DT, PAGED, CODER, SMEM)                                                      \
@@ -1913,7 +2073,15 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
     } while (0)
     if (fused) {
         ProfScope prof(kProfEncode, stream);
-        B2_LAUNCH_ENC2(true, smem_fused);
+        int rc;
+        if (P.dtype == B200KV_DT_BF16) {
+            if (paged) rc = coder == CODER_RANS ? launch_encode_fused<0, true, CODER_RANS>(P, stream) : launch_encode_fused<0, true, CODER_AC>(P, stream);
+            else rc = coder == CODER_RANS ? launch_encode_fused<0, false, CODER_RANS>(P, stream) : launch_encode_fused<0, false, CODER_AC>(P, stream);
+        } else {
+            if (paged) rc = coder == CODER_RANS ? launch_encode_fused<1, true, CODER_RANS>(P, stream) : launch_encode_fused<1, true, CODER_AC>(P, stream);
+            else rc = coder == CODER_RANS ? launch_encode_fused<1, false, CODER_RANS>(P, stream) : launch_encode_fused<1, false, CODER_AC>(P, stream);
+        }
+        if (rc) return rc;
     } else {
         const unsigned cdf_blocks = (unsigned)((int64_t)n_chunks * per_group);
         {
@@ -1959,7 +2127,8 @@ int64_t b200kv_encode_layers_workspace_bytes(int32_t L, int32_t H, int32_t D, in
     if (L <= 0 || H <= 0 || D <= 0 || chunk_tokens <= 0 || chunk_tokens > kGroup || n_chunks <= 0 || max_layers <= 0 ||
         max_layers > L)
         return -2;
-    return (int64_t)encl_ws_layout(n_chunks, (int64_t)n_chunks * 2 * max_layers * tiles_per_plane(H * D)).bytes;
+    return (int64_t)encl_ws_layout(n_chunks, (int64_t)n_chunks * 2 * max_layers * tiles_per_plane(H * D),
+                                   (int64_t)n_chunks * 2 * max_layers).bytes;
 }
 
 int b200kv_encode_layers_plan(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
@@ -2004,7 +2173,7 @@ int b200kv_encode_layers_plan(const b200kv_kv_desc* kv, int64_t tok_begin, int32
     P.seg = seg_sizes_out;
     const int64_t call_tiles = (int64_t)n_chunks * P.ppl * max_layers * P.tpp;
     B2_REQUIRE(call_tiles < (1ll << 31), "too many tiles in one call");
-    const EnclWs w = encl_ws_layout(n_chunks, call_tiles);
+    const EnclWs w = encl_ws_layout(n_chunks, call_tiles, (int64_t)n_chunks * P.ppl * max_layers);
     B2_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)w.bytes, "workspace too small");
     uint8_t* ws = static_cast<uint8_t*>(workspace);
     P.err = reinterpret_cast<unsigned int*>(ws + w.err);
@@ -2016,6 +2185,9 @@ int b200kv_encode_layers_plan(const b200kv_kv_desc* kv, int64_t tok_begin, int32
     P.totals = reinterpret_cast<unsigned long long*>(ws + w.totals);
     P.rstate = reinterpret_cast<uint32_t*>(ws + w.rstate);
     P.temp = reinterpret_cast<uint32_t*>(ws + w.temp);
+    P.ticket = reinterpret_cast<unsigned int*>(ws + w.sync);
+    P.ready = P.ticket + 1;
+    P.vec = rows_vec(P) ? 1 : 0;
     // counters; the fixed images too, so that their padding bytes are zero whatever the buffer held before
     B2_CHECK_CUDA(cudaMemsetAsync(ws, 0, w.tot, stream));
     B2_CHECK_CUDA(cudaMemsetAsync(fixed_out, 0, (size_t)fixed_stride * n_chunks, stream));
@@ -2043,20 +2215,12 @@ int b200kv_encode_layers(b200kv_encode_plan_t* plan_in, int32_t layer_begin, int
     P.layers_left = P.L - plan->done.count() - bits.count();
     P.tiles_full = P.ppl * P.nlay * P.tpp;
     const int64_t n_tiles = (int64_t)P.n_chunks * P.tiles_full;
-    const int64_t total_tokens = (int64_t)(P.n_chunks - 1) * P.chunk_tokens + P.last_chunk_tokens;
-    b200kv_kv_desc kv{};
-    kv.D = P.D; kv.sT = P.sT; kv.sH = P.sH;
-    if (int rc = launch_absmax(P, &kv, total_tokens, stream)) return rc;
-#define B2_LAUNCH_ENCL(DT, PAGED)                                                                                      \
-    do {                                                                                                               \
-        B2_CHECK_CUDA(cudaFuncSetAttribute(encode_kernel<true, DT, PAGED, CODER_RANS>,                                 \
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemFused));             \
-        encode_kernel<true, DT, PAGED, CODER_RANS><<<(unsigned)n_tiles, CT, kSmemFused, stream>>>(P);                  \
-    } while (0)
-    if (P.dtype == B200KV_DT_BF16) { if (P.slot_map) B2_LAUNCH_ENCL(0, true); else B2_LAUNCH_ENCL(0, false); }
-    else { if (P.slot_map) B2_LAUNCH_ENCL(1, true); else B2_LAUNCH_ENCL(1, false); }
-#undef B2_LAUNCH_ENCL
-    B2_CHECK_CUDA(cudaGetLastError());
+    // encode_kernel's ticket and ready counters start at zero (the maxima are computed inside it)
+    B2_CHECK_CUDA(cudaMemsetAsync(P.ticket, 0, (size_t)(1 + (int64_t)P.n_chunks * P.ppl * P.nlay) * 4, stream));
+    int rc;
+    if (P.dtype == B200KV_DT_BF16) rc = P.slot_map ? launch_encode_fused<0, true, CODER_RANS>(P, stream) : launch_encode_fused<0, false, CODER_RANS>(P, stream);
+    else rc = P.slot_map ? launch_encode_fused<1, true, CODER_RANS>(P, stream) : launch_encode_fused<1, false, CODER_RANS>(P, stream);
+    if (rc) return rc;
     enc_scan_kernel<<<(unsigned)P.n_chunks, 1024, 0, stream>>>(P);
     place_kernel<<<1, 1024, 0, stream>>>(P);
     compact_kernel<<<(unsigned)n_tiles, CT, (size_t)P.stage_bytes, stream>>>(P);
