@@ -222,7 +222,7 @@ int b200kv_decode_chunks(const void* containers, int64_t containers_bytes, const
  * b200kv_decode_layers enqueues the decode of layers [layer_begin, layer_end): planes layer_begin.. (keys) and
  * L + layer_begin.. (values), 0 <= layer_begin < layer_end <= L, and ORs into the plan's status_out.  Any set of
  * calls that covers every layer once writes what b200kv_decode_chunks writes.  A call reads the fixed sections and
- * the payload bytes of its planes' streams; in a version 2 or 3 container nothing past a stream's own bytes reaches
+ * the payload bytes of its planes' streams; in a version 1, 2 or 3 container nothing past a stream's own bytes reaches
  * an output or a status bit, so the bytes of later planes may be unwritten (codec.cu explains why).  In a version 3
  * container (one group) the streams of plane p are the contiguous range that the half-lengths of planes < p and <= p
  * delimit; containers of several groups (versions 1 / 2 with more than 256 tokens) spread a plane over every group.

@@ -35,8 +35,10 @@ constexpr int CT = 128;            // streams (threads) per tile
 constexpr int SPW = 6;             // 5-bit symbols packed per 32-bit word in shared memory
 constexpr int SYMW = 43;           // words per symbol row: ceil(256 / 6); odd -> conflict-free columns
 constexpr int PAIRW = 33;          // split mode: words per CDF-pair row (32 symbols + cdf[32]); odd
-constexpr int TEMPW_FUSED = 40;    // words per stream in the tile's temp rows: own-CDF streams of <= 256 symbols
-                                   //   cost <= 256*log2(31) + 2 bits = 159 bytes (DESIGN.md 3.2)
+constexpr int TEMPW_FUSED = 40;    // words per stream in the tile's temp rows: an own-CDF stream of <= 256 symbols
+                                   //   costs <= 1267.9 ideal bits under the rounded CDF (width >= n*65504/256 - 0.02)
+                                   //   + < 0.001 bits of truncation + 2 termination bits = 1269.95 bits -> 159 bytes,
+                                   //   40 words (DESIGN.md 3.2; tests/ac_edges.py own_bound_bits)
 constexpr int TEMPW_SPLIT = 132;   // foreign CDF (chunk > 256 tokens): <= 16 bits / symbol + termination; 16-byte rows
 constexpr int TEMPW_FUSED_RANS = 48;   // rANS, own-CDF streams: <= 95 renormalisation halfwords for ANY symbol order
                                        //   (ideal <= 1268.5 bits, < 1 bit of overshoot per step; DESIGN.md 3.7); the 32-bit
@@ -1281,8 +1283,11 @@ struct WordSrc {
 //   - v3 header, register reader: words are loaded while 4k < header length; next_byte() hands out the count bytes
 //     only, all of them inside the header (the funnel shift may carry later bytes in the same register, unread).
 //   - status: bit 1 comes from the lengths section (fixed sections) and payload_bytes, bit 0 from the final state.
-// Version 1 (arithmetic coder) is not covered by this argument (its decoder shifts bits past the end of its stream into
-// its window); the layer-major upload of lmcache_b200/pipeline.py splits version-3 containers only.
+//   - arithmetic coder (version 1): the decoder does shift bits past the end of its stream into `off`, but none of them
+//     can change a symbol: termination emits the final bit and its pending run, which leave every continuation of the
+//     stream inside the final interval, so every decision `plo <= off < phi` holds whatever follows (tests/ac_edges.py,
+//     tests/test_gpu_ac_edges.py decode with 0x00 / 0xFF after the planes).  Status comes from the lengths section only.
+// The layer-major upload of lmcache_b200/pipeline.py splits version-3 containers only.
 
 // rANS: aligned little-endian words off a running pointer; the look-ahead lives in the decoder state (RansDec::nxt)
 struct LeWordSrc {
