@@ -38,7 +38,9 @@ extern "C" {
                                     *    e.g. dlsym): b200kv_decode_plan / b200kv_decode_layers, b200kv_plane_offsets,
                                     *    b200kv_plane_offsets_device, b200kv_copy_batch_async,
                                     *    b200kv_encode_layers_workspace_bytes / b200kv_encode_layers_plan /
-                                    *    b200kv_encode_layers / b200kv_encode_layers_finish, b200kv_decode_plan_heads.
+                                    *    b200kv_encode_layers / b200kv_encode_layers_finish, b200kv_decode_plan_heads,
+                                    *    b200kv_lossless_layout / b200kv_lossless_workspace_bytes / b200kv_lossless_encode /
+                                    *    b200kv_lossless_decode (container versions 5 and 6).
                                     *    B200KV_MAX_PLANES went from 128 to 256 (models of up to 128 layers): the row
                                     *    width of b200kv_plane_offsets_device, B200KV_MAX_PLANES + 1, and the size of
                                     *    b200kv_encode_plan_t, 256 -> 512 words, changed with it; a caller takes them
@@ -301,6 +303,78 @@ int b200kv_encode_layers_plan(const b200kv_kv_desc* kv, int64_t tok_begin, int32
                               b200kv_encode_plan_t* plan, void* stream);
 int b200kv_encode_layers(b200kv_encode_plan_t* plan, int32_t layer_begin, int32_t layer_end, void* stream);
 int b200kv_encode_layers_finish(const b200kv_encode_plan_t* plan, void* stream);
+
+/*
+ * Lossless container ("B2KV" versions 5 and 6).  Added without changing anything that existed: b200kv_version() stays 4,
+ * and neither b200kv_container_layout_v nor the CacheGen decode calls know these versions.
+ *
+ * Version 5 holds a (K, V) KV of P = 2L planes (keys of layers 0..L-1, then values), version 6 a latent KV
+ * (B200KV_KV_LATENT) of P = L planes.  header.max_dtype is the element dtype (bf16 or fp16), ngroups = 1, reserved = 0,
+ * 1 <= ntokens = t <= 4096; C = H * D channels.  Every 16-bit element u is split, for both dtypes alike, as
+ *     v = rotl16(u, 1),  sym = v >> 8,  raw = v & 0xff        (bf16: sym = the 8 exponent bits; fp16: the 5 exponent bits
+ *                                                              and the 3 top mantissa bits), u = rotr16((sym << 8) | raw, 1)
+ * Sections, each starting 16-byte aligned, little-endian:
+ *     header | freq u16[P][256] | lens u16[P][C] | raw u8[P][t][C] | streams
+ * freq[p]: the symbol histogram n_s of plane p (its t * C elements, N = t * C) normalised to M = 4096:
+ *     K = #{s : n_s > 0};  f_s = 0 if n_s = 0, else 1 + floor(n_s * (4096 - K) / N)      (integer arithmetic)
+ *     then the symbol with the largest n_s (the smallest symbol among equals) gets 4096 - sum(f) added.
+ *   This is one pass with no loop: K <= 256 < 4096, every occurring symbol starts at 1, and the floors sum to at most
+ *   4096 - K, so the remainder 4096 - sum(f) is >= 0 and adding it keeps every frequency >= 1; the row sums to 4096.
+ *   start_s = f_0 + ... + f_{s-1}.
+ * raw[p][i][c]: the raw byte of token i, channel c of plane p, stored verbatim.
+ * streams: one rANS stream per (plane, channel) over the t symbols, in (plane, channel) order, back to back; lens[p][c]
+ *   is its byte length, payload_bytes their sum, total_bytes = offset of the streams + payload_bytes.  The coder is the
+ *   project's rANS (32-bit state, 16-bit renormalisation; lmcache_b200/csrc/ac_core.cuh) with 12-bit probabilities:
+ *     encoder   x = 2^16; for i = t-1 .. 0:  s = sym[i]; if (x >> 20) >= f_s: push halfword (x & 0xffff), x >>= 16;
+ *               x = ((x / f_s) << 12) + (x mod f_s) + start_s
+ *     bytes     x as LE32, then the pushed halfwords in REVERSE push order (LE16 each); length = 4 + 2 * pushes, even
+ *     decoder   x = LE32; for i = 0 .. t-1:  slot = x & 4095; s = the symbol with start_s <= slot < start_s + f_s;
+ *               x = f_s * (x >> 12) + slot - start_s; if x < 2^16: x = (x << 16) | next LE16
+ *               after the last symbol x == 2^16 again and every halfword has been read (the integrity check).
+ *   The renormalisation bound is f << 20; it is tested as (x >> 20) >= f because a single-symbol plane has f = 4096 and
+ *   4096 << 20 overflows 32 bits (such a plane's streams are the 4 bytes of x = 2^16 and nothing else).  A stream is at
+ *   most 4 + 2 * ceil(3t / 4) + 2 bytes (12 bits per symbol), which fits u16 for t <= 4096; an encode whose stream
+ *   exceeds it sets header.status bit 0 (sizes_out 0).  tests/lossless_ref.py is the numpy statement of all this.
+ */
+typedef struct b200kv_lossless_layout_t {
+    int64_t off_freq, off_lens, off_raw, off_payload;
+    int64_t fixed_bytes;       /* == off_payload */
+    int64_t max_stream_bytes;  /* 4 + 2 * ceil(3t / 4) + 2 */
+    int64_t max_total_bytes;   /* align16(off_payload + P * C * max_stream_bytes): the out_stride an encode needs */
+} b200kv_lossless_layout_t;
+
+/* Section offsets of a version-5 (latent = 0) or version-6 (latent != 0) container; L <= 128, 1 <= ntokens <= 4096. */
+int b200kv_lossless_layout(int32_t L, int32_t H, int32_t D, int32_t ntokens, int32_t latent, b200kv_lossless_layout_t* out);
+/* Bytes of device scratch one b200kv_lossless_encode (decode = 0) or b200kv_lossless_decode (decode != 0) call needs;
+ * < 0 for a shape the calls refuse.  The encode's is dominated by a worst-case scratch row per stream. */
+int64_t b200kv_lossless_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t chunk_tokens, int32_t n_chunks,
+                                        int32_t latent, int32_t decode);
+/*
+ * Lossless encode: the KV, chunking, out / out_stride / sizes_out and workspace arguments of b200kv_encode_chunks
+ * (out_stride >= max_total_bytes of chunk_tokens; chunk_tokens <= 4096).  Version 6 when kv->dtype carries
+ * B200KV_KV_LATENT, 5 otherwise.  The KV is read twice (histogram, then coding), in stream order.
+ */
+int b200kv_lossless_encode(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
+                           int32_t last_chunk_tokens, void* out, int64_t out_stride, uint64_t* sizes_out,
+                           void* workspace, int64_t workspace_bytes, void* stream);
+/*
+ * Lossless decode: b200kv_decode_chunks' container arguments (DEVICE containers at 16-byte aligned offsets[j],
+ * total_bytes[j] = header.total_bytes, the buffer extending B200KV_READ_SLACK bytes past every container, ntokens[j],
+ * dst_tok[j]) into the destination `dst`.  max_dtype = header.max_dtype, the stored element dtype: dst must have that
+ * dtype (a lossless codec does not cast), else the call is refused.  The version decoded is 6 for a latent destination,
+ * 5 otherwise.  Reads stay inside each container whatever its lengths and frequency rows say, and nothing is written
+ * outside the destination rows of the call's tokens.  status_out: NULL, or DEVICE / mapped-host uint32[n_chunks], zeroed
+ * by the call and then OR-ed with
+ *   1 = a stream did not return to its initial state or did not use exactly its bytes, or a frequency row does not sum
+ *       to 4096 (that plane is not written),
+ *   2 = a stream that lies beyond the payload (lengths section damaged; that stream is not written),
+ *   4 = the header is not the one the call names: another version than the destination's latent-ness says, or another
+ *       L / H / D / ntokens / max_dtype.
+ */
+int b200kv_lossless_decode(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                           const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,
+                           int32_t max_dtype, const b200kv_kv_desc* dst, uint32_t* status_out, void* workspace,
+                           int64_t workspace_bytes, void* stream);
 
 /*
  * Token-id prefix hash.  Replaces LMCacheEngine._chunk_tokens/_hash/_prefix_hash

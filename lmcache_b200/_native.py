@@ -22,7 +22,10 @@ CODER_RANS_COMPACT = 2   # container version 3: rANS streams that carry their ow
 ENCODE_HINT_MID_ENTROPY = 0x200    # B200KV_ENCODE_HINT_MID_ENTROPY
 KV_LATENT = 0x100        # B200KV_KV_LATENT: OR-ed into KvDesc.dtype (one plane per layer) and into a coder (container version 4)
 CODER_LATENT = CODER_RANS_COMPACT | KV_LATENT   # the coder argument that names container version 4
-HDR_MAX = 36             # longest version-3 stream header (4 mask bytes + 31 counts + 1 pad)
+CODER_LOSSLESS = 4       # names container version 5: lossless, (K, V) planes (not a b200kv_encode_chunks coder)
+CODER_LOSSLESS_LATENT = CODER_LOSSLESS | KV_LATENT   # container version 6: lossless, one plane per layer
+LOSSLESS_MAX_TOKENS = 4096   # tokens per lossless container
+HDR_MAX = 36            # longest version-3 stream header (4 mask bytes + 31 counts + 1 pad)
 CODERS = {"ac": CODER_AC, "rans": CODER_RANS, "rans_compact": CODER_RANS_COMPACT}
 LP = 33
 GROUP_TOKENS = 256
@@ -68,6 +71,12 @@ class Layout(ctypes.Structure):
                 ("fixed_bytes", c_i64), ("max_total_bytes", c_i64)]
 
 
+class LosslessLayout(ctypes.Structure):
+    """struct b200kv_lossless_layout_t"""
+    _fields_ = [("off_freq", c_i64), ("off_lens", c_i64), ("off_raw", c_i64), ("off_payload", c_i64),
+                ("fixed_bytes", c_i64), ("max_stream_bytes", c_i64), ("max_total_bytes", c_i64)]
+
+
 class DecodePlan(ctypes.Structure):
     """struct b200kv_decode_plan_t (opaque, filled by b200kv_decode_plan)"""
     _fields_ = [("opaque", ctypes.c_uint64 * 256)]
@@ -107,6 +116,12 @@ SIGNATURES = {
                                           c_vp]),
     "b200kv_encode_layers": (c_i32, [ctypes.POINTER(EncodePlan), c_i32, c_i32, c_vp]),
     "b200kv_encode_layers_finish": (c_i32, [ctypes.POINTER(EncodePlan), c_vp]),
+    "b200kv_lossless_layout": (c_i32, [c_i32, c_i32, c_i32, c_i32, c_i32, ctypes.POINTER(LosslessLayout)]),
+    "b200kv_lossless_workspace_bytes": (c_i64, [c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
+    "b200kv_lossless_encode": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp, c_vp,
+                                        c_i64, c_vp]),
+    "b200kv_lossless_decode": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, ctypes.POINTER(KvDesc), c_vp,
+                                        c_vp, c_i64, c_vp]),
     "b200kv_sha256_chain": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp]),
     "b200kv_sha256_chain_ready": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, ctypes.c_uint32, c_vp]),
     "b200kv_pack_chunks": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp]),
@@ -220,13 +235,25 @@ def container_layout(L: int, H: int, D: int, ntokens: int, coder: int = CODER_RA
 
 
 def coder_of_version(version: int) -> int:
-    """The coder argument that names a container version: version - 1 for versions 1 to 3, CODER_LATENT for 4."""
-    return CODER_LATENT if version == 4 else int(version) - 1
+    """The coder argument that names a container version: version - 1 for versions 1 to 3, CODER_LATENT for 4; the
+    lossless containers: CODER_LOSSLESS for 5, CODER_LOSSLESS_LATENT for 6."""
+    if version == 4:
+        return CODER_LATENT
+    if version == 6:
+        return CODER_LOSSLESS_LATENT
+    return int(version) - 1
 
 
 def planes_of(version: int, L: int) -> int:
-    """Planes of a container: one per layer in version 4 (a latent KV), a (K, V) pair per layer otherwise."""
-    return L if version == 4 else 2 * L
+    """Planes of a container: one per layer in versions 4 and 6 (a latent KV), a (K, V) pair per layer otherwise."""
+    return L if version in (4, 6) else 2 * L
+
+
+def lossless_layout(L: int, H: int, D: int, ntokens: int, latent: bool = False) -> LosslessLayout:
+    """Section offsets of a lossless container (version 5, or 6 for a latent KV)."""
+    lo = LosslessLayout()
+    check(lib().b200kv_lossless_layout(L, H, D, ntokens, int(bool(latent)), ctypes.byref(lo)), "lossless_layout")
+    return lo
 
 
 def nb_map(key_bins, value_bins, L: int) -> list:

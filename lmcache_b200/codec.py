@@ -435,7 +435,131 @@ class EncodeTicket:
         return EncodedBatch(self.buf, self.stride, [int(s) for s in sizes], self.max_dtype, self.coder)
 
 
-class CacheGenCodec:
+class _ContainerIO:
+    """What every codec does the same way around its own encode_async / decode: the blocking and host-copy forms of the
+    encode, the page-locked staging of containers on their way in, and the ordering of decodes that share buffers.  A
+    codec provides encode_async, parse_header (its container check) and the attributes _init_io sets."""
+
+    def _init_io(self) -> None:
+        self._enc_lock = threading.RLock()
+        self._dec_lock = threading.Lock()
+        self._enc_event: Optional[torch.cuda.Event] = None
+        self._enc_ws: Optional[torch.Tensor] = None
+        self._dec_ws: Optional[torch.Tensor] = None
+        self._enc_out: Optional[torch.Tensor] = None
+        self._sizes: Optional[PinnedBuffer] = None
+        self._dec_in: Optional[torch.Tensor] = None
+        self._dec_event: Optional[torch.cuda.Event] = None
+        self._dec_status: Optional[PinnedBuffer] = None   # uint32 per chunk of the last decode call (mapped host memory)
+        self._dec_status_n = 0
+        self._pin_lock = threading.Lock()
+        self._pin_in_lock = threading.Lock()
+        self._pin_out: Optional[PinnedBuffer] = None      # containers on their way out (encode_to_pinned)
+        self._pin_in: Optional[PinnedBuffer] = None       # containers on their way in (pinned_staging)
+
+    @staticmethod
+    def _grow(t: Optional[torch.Tensor], nbytes: int, device) -> torch.Tensor:
+        if t is None or t.numel() < nbytes or t.device != device:
+            t = torch.empty(int(nbytes), dtype=torch.uint8, device=device)
+        return t
+
+    def encode(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int,
+               stream: Optional[torch.cuda.Stream] = None, out: Optional[torch.Tensor] = None) -> EncodedBatch:
+        """encode_async + one event wait: blocks until the containers' sizes are known; payloads stay on the device.
+        With out=None the batch aliases the codec's staging, which the next encode call overwrites."""
+        return self.encode_async(view, tok_begin, n_tokens, chunk_size, stream, out).wait()
+
+    def encode_to_host(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int,
+                       stream: Optional[torch.cuda.Stream] = None) -> List[bytes]:
+        """encode + one device->host copy per container through the codec's page-locked slab, returned as immutable
+        bytes (the Serializer.to_bytes contract, serde.py:12-27).  The encoder lock is held until the copies are done:
+        the staging the batch aliases cannot be overwritten by a concurrent encode."""
+        with self._enc_lock, self.encode_to_pinned(view, tok_begin, n_tokens, chunk_size, stream) as views:
+            return [bytes(v) for v in views]
+
+    @contextlib.contextmanager
+    def encode_to_pinned(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int,
+                         stream: Optional[torch.cuda.Stream] = None):
+        """encode + one device->host copy per container into the codec's page-locked slab (kept across calls, grown on
+        demand); yields one writable memoryview per container.  The views -- e.g. handed to a socket send -- are valid
+        inside the `with` block only: the slab is reused by the next call (serialised by a lock)."""
+        with self._enc_lock, self._pin_lock:
+            batch = self.encode(view, tok_begin, n_tokens, chunk_size, stream)
+            total = sum((s + 15) & ~15 for s in batch.sizes)
+            if self._pin_out is None or self._pin_out.nbytes < total:
+                if self._pin_out is not None:
+                    self._pin_out.close()
+                self._pin_out = PinnedBuffer(max(total, 1) * 5 // 4)
+            pin = self._pin_out
+            lib = N.lib()
+            sp = _stream_ptr(stream)
+            offs, o = [], 0
+            with torch.cuda.device(view.device):
+                for j, s in enumerate(batch.sizes):
+                    N.check(lib.b200kv_copy_async(pin.host_ptr + o, batch.buf.data_ptr() + j * batch.stride, s, sp), "copy")
+                    offs.append(o)
+                    o += (s + 15) & ~15
+                N.check(lib.b200kv_stream_sync(sp), "stream_sync")
+            views = [pin.view(offs[j], batch.sizes[j]) for j in range(len(offs))]
+            for v in views:
+                self.parse_header(v)        # raises on encoder error status
+            try:
+                yield views
+            finally:
+                del views
+
+    @contextlib.contextmanager
+    def pinned_staging(self, nbytes: int):
+        """A page-locked receive slab of at least nbytes (kept across calls): a remote tier reads containers straight
+        into it and decode() uploads from it with true asynchronous copies."""
+        with self._pin_in_lock:
+            if self._pin_in is None or self._pin_in.nbytes < nbytes:
+                if self._pin_in is not None:
+                    self._dec_sync()
+                    self._pin_in.close()
+                self._pin_in = PinnedBuffer(max(nbytes, 1) * 5 // 4)
+            try:
+                yield self._pin_in
+            finally:
+                self._dec_sync()       # the uploads out of the slab must finish before the next user overwrites it
+
+    def _dec_sync(self) -> None:
+        if self._dec_event is not None:
+            self._dec_event.synchronize()
+
+    def _order_decode(self, tstream, need_in: int, need_ws: int) -> None:
+        """staging / workspace are reused across calls: order after the previous decode and never free a
+        buffer a kernel may still be reading."""
+        if self._dec_event is None:
+            return
+        if ((self._dec_in is not None and self._dec_in.numel() < need_in) or
+                (self._dec_ws is not None and self._dec_ws.numel() < need_ws)):
+            self._dec_event.synchronize()
+        else:
+            tstream.wait_event(self._dec_event)
+
+    def _status_buffer(self, n: int) -> PinnedBuffer:
+        """the mapped page-locked status words of a decode call of n containers (grown on demand)"""
+        if self._dec_status is None or self._dec_status.nbytes < 4 * n:
+            if self._dec_status is not None:
+                self._dec_sync()
+            self._dec_status = PinnedBuffer(max(4096, 8 * n))
+        self._dec_status_n = n
+        return self._dec_status
+
+    def decode_status(self) -> List[int]:
+        """Wait for the most recent decode call and return its per-chunk status words (0 = clean; bit 0: a rANS stream
+        did not return to its initial state, bit 1: stream offsets beyond the payload, bit 2: the header's version is not
+        the one the call's coder named).  A nonzero word means the container's bytes were damaged after its header was
+        written, or it was handed to the wrong decode: treat the chunk as a miss."""
+        with self._dec_lock:
+            if self._dec_status is None or self._dec_event is None:
+                return []
+            self._dec_event.synchronize()
+            return list((ctypes.c_uint32 * self._dec_status_n).from_address(self._dec_status.host_ptr))
+
+
+class CacheGenCodec(_ContainerIO):
     """Batched CacheGen encode / decode on the current CUDA device.
 
     Thread model: one encoder and one decoder may run concurrently from different threads (the
@@ -471,29 +595,11 @@ class CacheGenCodec:
         self._kb = N.float_array(kb)
         self._vb = N.float_array(vb)
         self._nb = (N.nb_map(kb, vb, len(kb)))          # keys then values, all layers of the model
-        self._enc_lock = threading.RLock()
-        self._dec_lock = threading.Lock()
-        self._enc_event: Optional[torch.cuda.Event] = None
+        self._init_io()
         self._last_bits_per_symbol = 0.0        # payload bits per symbol of the most recent encode whose sizes were read
-        self._enc_ws: Optional[torch.Tensor] = None
-        self._dec_ws: Optional[torch.Tensor] = None
-        self._enc_out: Optional[torch.Tensor] = None
-        self._sizes: Optional[PinnedBuffer] = None
-        self._dec_in: Optional[torch.Tensor] = None
-        self._dec_event: Optional[torch.cuda.Event] = None
-        self._dec_status: Optional[PinnedBuffer] = None   # uint32 per chunk of the last decode call (mapped host memory)
-        self._dec_status_n = 0
-        self._pin_lock = threading.Lock()
-        self._pin_in_lock = threading.Lock()
-        self._pin_out: Optional[PinnedBuffer] = None      # containers on their way out (encode_to_pinned)
-        self._pin_in: Optional[PinnedBuffer] = None       # containers on their way in (pinned_staging)
 
     # ------------------------------------------------------------------ helpers
-    @staticmethod
-    def _grow(t: Optional[torch.Tensor], nbytes: int, device) -> torch.Tensor:
-        if t is None or t.numel() < nbytes or t.device != device:
-            t = torch.empty(int(nbytes), dtype=torch.uint8, device=device)
-        return t
+    parse_header = staticmethod(parse_header)    # the CacheGen container check (versions 1 to 4)
 
     def coder_for(self, chunk_tokens: int, latent: bool = False) -> int:
         """The container this codec writes for chunks of `chunk_tokens`: the compact one holds <= 256 tokens.  A latent
@@ -609,82 +715,7 @@ class CacheGenCodec:
             return EncodeTicket(out, stride, n_chunks, sizes, ev, view.dtype_code, coder, view, self,
                                 (fixed, float(view.planes) * view.H * view.D * n_tokens))
 
-    def encode(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int,
-               stream: Optional[torch.cuda.Stream] = None, out: Optional[torch.Tensor] = None) -> EncodedBatch:
-        """encode_async + one event wait: blocks until the containers' sizes are known; payloads stay on the device.
-        With out=None the batch aliases the codec's staging, which the next encode call overwrites."""
-        return self.encode_async(view, tok_begin, n_tokens, chunk_size, stream, out).wait()
-
-    def encode_to_host(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int,
-                       stream: Optional[torch.cuda.Stream] = None) -> List[bytes]:
-        """encode + one device->host copy per container through the codec's page-locked slab, returned as immutable
-        bytes (the Serializer.to_bytes contract, serde.py:12-27).  The encoder lock is held until the copies are done:
-        the staging the batch aliases cannot be overwritten by a concurrent encode."""
-        with self._enc_lock, self.encode_to_pinned(view, tok_begin, n_tokens, chunk_size, stream) as views:
-            return [bytes(v) for v in views]
-
-    @contextlib.contextmanager
-    def encode_to_pinned(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int,
-                         stream: Optional[torch.cuda.Stream] = None):
-        """encode + one device->host copy per container into the codec's page-locked slab (kept across calls, grown on
-        demand); yields one writable memoryview per container.  The views -- e.g. handed to a socket send -- are valid
-        inside the `with` block only: the slab is reused by the next call (serialised by a lock)."""
-        with self._enc_lock, self._pin_lock:
-            batch = self.encode(view, tok_begin, n_tokens, chunk_size, stream)
-            total = sum((s + 15) & ~15 for s in batch.sizes)
-            if self._pin_out is None or self._pin_out.nbytes < total:
-                if self._pin_out is not None:
-                    self._pin_out.close()
-                self._pin_out = PinnedBuffer(max(total, 1) * 5 // 4)
-            pin = self._pin_out
-            lib = N.lib()
-            sp = _stream_ptr(stream)
-            offs, o = [], 0
-            with torch.cuda.device(view.device):
-                for j, s in enumerate(batch.sizes):
-                    N.check(lib.b200kv_copy_async(pin.host_ptr + o, batch.buf.data_ptr() + j * batch.stride, s, sp), "copy")
-                    offs.append(o)
-                    o += (s + 15) & ~15
-                N.check(lib.b200kv_stream_sync(sp), "stream_sync")
-            views = [pin.view(offs[j], batch.sizes[j]) for j in range(len(offs))]
-            for v in views:
-                parse_header(v)        # raises on encoder error status
-            try:
-                yield views
-            finally:
-                del views
-
-    @contextlib.contextmanager
-    def pinned_staging(self, nbytes: int):
-        """A page-locked receive slab of at least nbytes (kept across calls): a remote tier reads containers straight
-        into it and decode() uploads from it with true asynchronous copies."""
-        with self._pin_in_lock:
-            if self._pin_in is None or self._pin_in.nbytes < nbytes:
-                if self._pin_in is not None:
-                    self._dec_sync()
-                    self._pin_in.close()
-                self._pin_in = PinnedBuffer(max(nbytes, 1) * 5 // 4)
-            try:
-                yield self._pin_in
-            finally:
-                self._dec_sync()       # the uploads out of the slab must finish before the next user overwrites it
-
-    def _dec_sync(self) -> None:
-        if self._dec_event is not None:
-            self._dec_event.synchronize()
-
     # ------------------------------------------------------------------ decode
-    def _order_decode(self, tstream, need_in: int, need_ws: int) -> None:
-        """staging / workspace are reused across calls: order after the previous decode and never free a
-        buffer a kernel may still be reading."""
-        if self._dec_event is None:
-            return
-        if ((self._dec_in is not None and self._dec_in.numel() < need_in) or
-                (self._dec_ws is not None and self._dec_ws.numel() < need_ws)):
-            self._dec_event.synchronize()
-        else:
-            tstream.wait_event(self._dec_event)
-
     def decode_raw(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
                    ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
                    stream: Optional[torch.cuda.Stream] = None, _locked: bool = False) -> None:
@@ -718,14 +749,9 @@ class CacheGenCodec:
             if not _locked:
                 self._order_decode(tstream, 0, ws_bytes)
             self._dec_ws = self._grow(self._dec_ws, ws_bytes, dst.device)
-            if self._dec_status is None or self._dec_status.nbytes < 4 * n:
-                if self._dec_status is not None:
-                    self._dec_sync()
-                self._dec_status = PinnedBuffer(max(4096, 8 * n))
-            self._dec_status_n = n
             args = (base_ptr, int(buf_bytes), N.i64_array(list(offsets)), N.i64_array(list(totals)),
                     N.i32_array(list(ntokens)), N.i64_array(list(dst_tok)), n, int(max_dtype), int(coder),
-                    ctypes.byref(dst.desc), self._kb, self._vb, self._dec_status.dev_ptr, self._dec_ws.data_ptr(),
+                    ctypes.byref(dst.desc), self._kb, self._vb, self._status_buffer(n).dev_ptr, self._dec_ws.data_ptr(),
                     self._dec_ws.numel())
             if heads is None:
                 N.check(lib.b200kv_decode_chunks(*args, tstream.cuda_stream), "decode_chunks")
@@ -792,17 +818,6 @@ class CacheGenCodec:
         """Second half of decode_raw (b200kv_decode_layers): enqueue the decode of layers [layer_begin, layer_end)."""
         N.check(N.lib().b200kv_decode_layers(ctypes.byref(plan), int(layer_begin), int(layer_end), stream.cuda_stream),
                 "decode_layers")
-
-    def decode_status(self) -> List[int]:
-        """Wait for the most recent decode call and return its per-chunk status words (0 = clean; bit 0: a rANS stream
-        did not return to its initial state, bit 1: stream offsets beyond the payload, bit 2: the header's version is not
-        the one the call's coder named).  A nonzero word means the container's bytes were damaged after its header was
-        written, or it was handed to the wrong decode: treat the chunk as a miss."""
-        with self._dec_lock:
-            if self._dec_status is None or self._dec_event is None:
-                return []
-            self._dec_event.synchronize()
-            return list((ctypes.c_uint32 * self._dec_status_n).from_address(self._dec_status.host_ptr))
 
     def decode_device_batch(self, batch: EncodedBatch, ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int],
                             stream: Optional[torch.cuda.Stream] = None) -> None:
@@ -873,6 +888,230 @@ class CacheGenCodec:
                 o += (nb + 15) & ~15
             self.decode_raw(base_ptr, self._dec_in.numel(), offsets, totals, ntoks, dst, dst_tok, max_dtype, coder, tstream,
                             _locked=True)
+
+
+def dtype_of_code(code: int) -> torch.dtype:
+    """torch dtype of an N.DT_* code"""
+    return _CODE_DTYPE[int(code)]
+
+
+def parse_lossless_header(buf, total: Optional[int] = None) -> N.Header:
+    """Validate and return the 64-byte header of a lossless B2KV container (versions 5 and 6; ValueError for anything
+    else, CacheGen containers included).  `buf` is the whole container, or a prefix of at least the header when `total`,
+    the size of the whole container, is given."""
+    mv = memoryview(buf)
+    if mv.nbytes < N.HEADER_BYTES:
+        raise ValueError("buffer too small for a B2KV container")
+    hd = N.Header.from_buffer_copy(bytes(mv[:N.HEADER_BYTES]))
+    if hd.magic != N.MAGIC:
+        raise ValueError("not a B2KV container (bad magic)")
+    if hd.version not in (5, 6):
+        raise ValueError(f"not a lossless B2KV container (version {hd.version})")
+    if hd.total_bytes > (mv.nbytes if total is None else total):
+        raise ValueError("truncated B2KV container")
+    if hd.status != 0:
+        raise ValueError(f"B2KV container carries encoder error status {hd.status}")
+    check_lossless_header(hd)
+    return hd
+
+
+def check_lossless_header(hd: "N.Header") -> None:
+    """Structural checks of a lossless header: a possible shape (L <= 128 layers, 1..4096 tokens), a 16-bit dtype, one
+    group, and total_bytes = fixed sections + payload_bytes with a payload between 4 bytes per stream and the worst case."""
+    if not (0 < hd.L <= N.MAX_PLANES // 2 and hd.H > 0 and hd.D > 0 and hd.H * hd.D < (1 << 24) and
+            0 < hd.ntokens <= N.LOSSLESS_MAX_TOKENS):
+        raise ValueError("B2KV header carries an impossible shape")
+    if hd.max_dtype not in (N.DT_BF16, N.DT_FP16):
+        raise ValueError("B2KV header carries an unknown element dtype")
+    if hd.ngroups != 1 or any(hd.reserved):
+        raise ValueError("B2KV lossless header: ngroups must be 1 and reserved 0")
+    lo = N.lossless_layout(hd.L, hd.H, hd.D, hd.ntokens, hd.version == 6)
+    if hd.total_bytes != lo.off_payload + hd.payload_bytes:
+        raise ValueError("B2KV header: total_bytes != fixed sections + payload_bytes (truncated or corrupt)")
+    nstreams = N.planes_of(hd.version, hd.L) * hd.H * hd.D
+    if hd.payload_bytes < 4 * nstreams or hd.total_bytes > lo.max_total_bytes:
+        raise ValueError("B2KV header: payload_bytes impossible for this shape")
+
+
+class LosslessCodec(_ContainerIO):
+    """Lossless encode / decode on the current CUDA device (container versions 5 and 6, include/b200kv.h): every
+    element's high byte after a one-bit rotation (bf16: the exponent) is rANS-coded per (plane, channel) against one
+    frequency row per plane, the low byte is kept verbatim, and the decode gives back the same bits.  It presents what the
+    remote tier's pipelines take from CacheGenCodec; it needs no model table, and decodes into the stored dtype only.
+
+    Thread model as CacheGenCodec: one encoder and one decoder may run concurrently from different threads."""
+
+    def __init__(self):
+        N.require_cuda()
+        self._init_io()
+
+    parse_header = staticmethod(parse_lossless_header)
+
+    @staticmethod
+    def coder_for(chunk_tokens: int, latent: bool = False) -> int:
+        """The coder value HostContainer / EncodedBatch carry for this codec's containers (version 6 for a latent KV)."""
+        if not 0 < chunk_tokens <= N.LOSSLESS_MAX_TOKENS:
+            raise ValueError(f"a lossless container holds 1 to {N.LOSSLESS_MAX_TOKENS} tokens, not {chunk_tokens}")
+        return N.CODER_LOSSLESS_LATENT if latent else N.CODER_LOSSLESS
+
+    def accepts(self, hd: "N.Header", latent: bool = False) -> bool:
+        """Does a container that passed parse_lossless_header fit a destination of one plane per layer (`latent`: version
+        6) or of (K, V) pairs (version 5)?"""
+        return hd.version in (5, 6) and (hd.version == 6) == latent
+
+    def layout(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> "N.LosslessLayout":
+        self.coder_for(chunk_tokens, latent)
+        return N.lossless_layout(L, H, D, chunk_tokens, latent)
+
+    def out_stride(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> int:
+        """Bytes reserved per container: the worst case, every stream at 12 bits per symbol."""
+        return int(self.layout(L, H, D, chunk_tokens, latent).max_total_bytes)
+
+    def max_container_bytes(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> int:
+        """Upper bound of a container this codec can decode (there is one lossless layout per shape)."""
+        return self.out_stride(L, H, D, chunk_tokens, latent)
+
+    # ------------------------------------------------------------------ encode
+    def encode_async(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int,
+                     stream: Optional[torch.cuda.Stream] = None, out: Optional[torch.Tensor] = None,
+                     sizes: Optional[PinnedBuffer] = None) -> "EncodeTicket":
+        """CacheGenCodec.encode_async for lossless containers: enqueue on `stream`, no host synchronisation; the KV is
+        read in stream order (twice: histogram, then coding)."""
+        if n_tokens <= 0:
+            raise ValueError("n_tokens must be positive")
+        coder = self.coder_for(chunk_size, view.latent)
+        n_chunks = (n_tokens + chunk_size - 1) // chunk_size
+        last = n_tokens - (n_chunks - 1) * chunk_size
+        stride = self.out_stride(view.L, view.H, view.D, chunk_size, view.latent)
+        lib = N.lib()
+        with self._enc_lock, torch.cuda.device(view.device):
+            tstream = stream if stream is not None else torch.cuda.current_stream()
+            ws_bytes = N.check(lib.b200kv_lossless_workspace_bytes(view.L, view.H, view.D, chunk_size, n_chunks,
+                                                                   int(view.latent), 0), "lossless_workspace_bytes")
+            own_out, own_sizes = out is None, sizes is None
+            need_out = stride * n_chunks + N.READ_SLACK if own_out else 0
+            if self._enc_event is not None:
+                grow = (self._enc_ws is None or self._enc_ws.numel() < ws_bytes or self._enc_ws.device != view.device or
+                        (own_out and (self._enc_out is None or self._enc_out.numel() < need_out)))
+                if grow:
+                    self._enc_event.synchronize()
+                else:
+                    tstream.wait_event(self._enc_event)
+            self._enc_ws = self._grow(self._enc_ws, ws_bytes, view.device)
+            if own_out:
+                self._enc_out = self._grow(self._enc_out, need_out, view.device)
+                out = self._enc_out
+            elif out.numel() < stride * n_chunks:
+                raise ValueError("encode output buffer too small")
+            if own_sizes:
+                if self._sizes is None or self._sizes.nbytes < 8 * n_chunks:
+                    self._sizes = PinnedBuffer(max(4096, 8 * n_chunks))
+                sizes = self._sizes
+            elif sizes.nbytes < 8 * n_chunks:
+                raise ValueError("sizes buffer too small")
+            N.check(lib.b200kv_lossless_encode(ctypes.byref(view.desc), tok_begin, n_chunks, chunk_size, last,
+                                               out.data_ptr(), stride, sizes.dev_ptr, self._enc_ws.data_ptr(),
+                                               self._enc_ws.numel(), tstream.cuda_stream), "lossless_encode")
+            ev = torch.cuda.Event()
+            ev.record(tstream)
+            self._enc_event = ev
+            return EncodeTicket(out, stride, n_chunks, sizes, ev, view.dtype_code, coder, view)
+
+    # ------------------------------------------------------------------ decode
+    def decode_raw(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
+                   ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
+                   stream: Optional[torch.cuda.Stream] = None, _locked: bool = False) -> None:
+        """Decode containers that already sit in device memory at base_ptr + offsets[j] (asynchronous), as
+        CacheGenCodec.decode_raw.  max_dtype is the stored element dtype, which must be dst's; coder names the version
+        (N.CODER_LOSSLESS_LATENT: 6), which must match dst's latent-ness."""
+        n = len(offsets)
+        if n == 0:
+            return
+        if coder not in (N.CODER_LOSSLESS, N.CODER_LOSSLESS_LATENT) or bool(coder & N.KV_LATENT) != dst.latent:
+            raise ValueError(f"coder {coder} does not name the lossless container of this destination")
+        lib = N.lib()
+
+        def run():
+            tstream = stream if stream is not None else torch.cuda.current_stream()
+            ws_bytes = max(lib.b200kv_lossless_workspace_bytes(dst.L, dst.H, dst.D, max(ntokens), n, int(dst.latent), 1),
+                           0)          # < 0: a shape the decode call refuses, with its reason
+            if not _locked:
+                self._order_decode(tstream, 0, ws_bytes)
+            self._dec_ws = self._grow(self._dec_ws, max(ws_bytes, 16), dst.device)
+            N.check(lib.b200kv_lossless_decode(base_ptr, int(buf_bytes), N.i64_array(list(offsets)),
+                                               N.i64_array(list(totals)), N.i32_array(list(ntokens)),
+                                               N.i64_array(list(dst_tok)), n, int(max_dtype), ctypes.byref(dst.desc),
+                                               self._status_buffer(n).dev_ptr, self._dec_ws.data_ptr(),
+                                               self._dec_ws.numel(), tstream.cuda_stream), "lossless_decode")
+            if self._dec_event is None:
+                self._dec_event = torch.cuda.Event()
+            self._dec_event.record(tstream)
+
+        if _locked:
+            run()
+        else:
+            with self._dec_lock, torch.cuda.device(dst.device):
+                run()
+
+    def decode(self, containers: Sequence[Union[bytes, bytearray, memoryview, torch.Tensor]], dst: KvView,
+               dst_tok: Sequence[int], stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Decode lossless containers into `dst` at token offsets `dst_tok` (asynchronous on `stream`).  Host
+        containers are uploaded first; a single 16-byte-aligned device tensor is used in place.  ValueError for a
+        container that is not lossless, whose kind (version 6: latent) or shape is not dst's, or whose dtype is not."""
+        n = len(containers)
+        if n == 0:
+            return
+        heads = []
+        for c in containers:
+            if isinstance(c, torch.Tensor):
+                hd = parse_lossless_header(c[:N.HEADER_BYTES].cpu().numpy().tobytes(), c.numel())
+            else:
+                hd = parse_lossless_header(c)
+            if not self.accepts(hd, dst.latent):
+                raise ValueError(f"a version-{hd.version} container does not fit a destination of "
+                                 f"{'one plane' if dst.latent else 'a (K, V) pair'} per layer")
+            if (hd.L, hd.H, hd.D) != (dst.L, dst.H, dst.D):
+                raise ValueError(f"container shape L/H/D={hd.L}/{hd.H}/{hd.D} does not match destination "
+                                 f"{dst.L}/{dst.H}/{dst.D}")
+            if hd.max_dtype != dst.dtype_code:
+                raise ValueError(f"container holds {dtype_of_code(hd.max_dtype)}, destination is {dst.dtype}: a lossless "
+                                 f"container is decoded into its own dtype")
+            heads.append(hd)
+        totals = [int(h.total_bytes) for h in heads]
+        ntoks = [int(h.ntokens) for h in heads]
+        for tok, nt in zip(dst_tok, ntoks):
+            if tok < 0 or tok + nt > dst.ntokens:
+                raise ValueError(f"container of {nt} tokens at offset {tok} does not fit a {dst.ntokens}-token destination")
+        coder = self.coder_for(max(ntoks), dst.latent)
+        lib = N.lib()
+        with self._dec_lock, torch.cuda.device(dst.device):
+            tstream = stream if stream is not None else torch.cuda.current_stream()
+            sp = tstream.cuda_stream
+            need_in = sum((t + 15) & ~15 for t in totals) + N.READ_SLACK
+            self._order_decode(tstream, need_in, lib.b200kv_lossless_workspace_bytes(dst.L, dst.H, dst.D, max(ntoks), n,
+                                                                                     int(dst.latent), 1))
+            if n == 1 and isinstance(containers[0], torch.Tensor) and containers[0].is_cuda \
+                    and containers[0].data_ptr() % 16 == 0 and containers[0].numel() >= totals[0] + N.READ_SLACK:
+                keep_dev = containers[0]
+                self.decode_raw(keep_dev.data_ptr(), keep_dev.numel(), [0], totals, ntoks, dst, dst_tok,
+                                dst.dtype_code, coder, tstream, _locked=True)
+                return
+            self._dec_in = self._grow(self._dec_in, need_in, dst.device)
+            base_ptr = self._dec_in.data_ptr()
+            offsets, o = [], 0
+            for c, nb in zip(containers, totals):
+                if isinstance(c, torch.Tensor):
+                    keep = c
+                    src_ptr = c.data_ptr()
+                else:
+                    keep = np.frombuffer(c, dtype=np.uint8, count=nb)   # zero-copy view of bytes/bytearray/memoryview
+                    src_ptr = keep.ctypes.data
+                N.check(lib.b200kv_copy_async(base_ptr + o, src_ptr, nb, sp), "copy")
+                del keep
+                offsets.append(o)
+                o += (nb + 15) & ~15
+            self.decode_raw(base_ptr, self._dec_in.numel(), offsets, totals, ntoks, dst, dst_tok, dst.dtype_code, coder,
+                            tstream, _locked=True)
 
 
 def engine_codec(config, model_name: str) -> CacheGenCodec:

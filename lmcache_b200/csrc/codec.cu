@@ -156,14 +156,6 @@ __device__ __forceinline__ int chunk_tokens_of(const EncParams& P, int j) {
     return j == P.n_chunks - 1 ? P.last_chunk_tokens : P.chunk_tokens;
 }
 
-// Row of a token inside its plane.  PAGED: the caller's slot mapping (vLLM's paged KV cache: row = block * block_size
-// + offset); every lane of a warp asks for the same token, so the lookup is one broadcast load that hits L1.
-template <bool PAGED>
-__device__ __forceinline__ int64_t tok_row(const int64_t* slot_map, int64_t tok) {
-    if constexpr (PAGED) return __ldg(slot_map + tok);
-    else return tok;
-}
-
 // ------------------------------------------------------------------------------------------ absmax
 // max1 = amax(|x|, channels) per (plane, token), kept in the input half dtype
 // (cachegen_encoder.py:54-55).  |x| ordering == integer ordering of (bits & 0x7fff); a NaN in the row

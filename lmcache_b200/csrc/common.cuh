@@ -48,4 +48,12 @@ inline int kv_dtype(const b200kv_kv_desc* kv) { return kv->dtype & ~B200KV_KV_LA
 // with error set.
 int make_plane_table(const b200kv_kv_desc* kv, const float* key_bins, const float* value_bins, PlaneTable* out);
 
+// Row of a token inside its plane.  PAGED: the caller's slot mapping (vLLM's paged KV cache: row = block * block_size
+// + offset); every lane of a warp asks for the same token, so the lookup is one broadcast load that hits L1.
+template <bool PAGED>
+__device__ __forceinline__ int64_t tok_row(const int64_t* slot_map, int64_t tok) {
+    if constexpr (PAGED) return __ldg(slot_map + tok);
+    else return tok;
+}
+
 }  // namespace b200kv

@@ -1,0 +1,619 @@
+// lossless.cu -- the lossless KV container (B2KV versions 5 and 6): encode / decode kernels and their C-ABI entry points.
+//
+// Every 16-bit element u is split as v = rotl16(u, 1): sym = v >> 8 (bf16: the 8 exponent bits; fp16: the 5 exponent bits
+// and the top 3 mantissa bits), raw = v & 0xff (sign and the rest of the mantissa).  The raw bytes are stored verbatim; the
+// symbols of each (plane, channel) are rANS-coded (32-bit state, 16-bit renormalisation, 12-bit probabilities) against
+// one frequency row per plane.  include/b200kv.h states the format; tests/lossless_ref.py is its numpy statement.
+//
+// Thread mapping, as in codec.cu: one stream = one (plane, channel) = one thread; a CTA owns CT consecutive channels of
+// one plane of one chunk, so a warp reads 64 contiguous bytes per token and writes 32 contiguous raw bytes.
+//   encode: ll_hist_kernel (per-(chunk, plane) histogram) -> ll_norm_kernel (frequency rows) -> ll_encode_kernel (raw
+//           bytes in place, rANS into a worst-case scratch row) -> ll_scan_kernel (tile offsets, header, sizes_out) ->
+//           ll_compact_kernel (streams into the payload).  The KV is read twice: once for the histogram, once to code.
+//   decode: ll_tile_sum_kernel -> ll_scan_kernel (stream offsets from the lengths section) -> ll_decode_kernel.
+#include <cuda_runtime.h>
+#include <stdint.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include "ac_core.cuh"
+#include "common.cuh"
+
+namespace b200kv {
+namespace {
+
+constexpr int kCT = 128;                 // streams (threads) per CTA
+constexpr int kScale = 12;               // probability precision: M = 4096
+constexpr uint32_t kM = 1u << kScale;
+constexpr int kSyms = 256;
+constexpr int kMaxTokens = 4096;         // tokens per container (u16 stream lengths)
+constexpr int kSlice = 128;              // tokens per histogram CTA
+constexpr int kFreqRowBytes = 2 * kSyms;
+
+// fixed sections of a container of P planes of C channels and t tokens; max_stream: the longest stream the encoder can
+// produce (4 state bytes + <= ceil(3t/4) + 1 renormalisation halfwords), max_total: the worst-case container
+struct LlLayout {
+    int64_t off_freq, off_lens, off_raw, off_payload, max_stream, max_total;
+};
+__host__ __device__ __forceinline__ int64_t ll_max_words(int t) { return (3 * (int64_t)t + 3) / 4 + 1; }
+__host__ __device__ __forceinline__ LlLayout ll_layout(int P, int64_t C, int t) {
+    LlLayout lo;
+    lo.off_freq = B200KV_HEADER_BYTES;
+    lo.off_lens = lo.off_freq + (int64_t)P * kFreqRowBytes;
+    lo.off_raw = align16(lo.off_lens + 2 * (int64_t)P * C);
+    lo.off_payload = align16(lo.off_raw + (int64_t)P * t * C);
+    lo.max_stream = 4 + 2 * ll_max_words(t);
+    lo.max_total = align16(lo.off_payload + (int64_t)P * C * lo.max_stream);
+    return lo;
+}
+
+struct LlEnc {
+    PlaneTable pt;                       // source planes (maxq unused)
+    int64_t sT, sH, tok_begin;
+    const int64_t* slot_map;
+    int32_t L, H, D, C, NP, dtype;       // NP = planes: 2L, or L for a latent KV
+    int32_t n_chunks, chunk_tokens, last_chunk_tokens, tpp, ntiles, rw;   // rw: halfwords per scratch row
+    uint8_t* out;
+    int64_t out_stride;
+    uint64_t* sizes_out;
+    uint32_t* hist;                      // [n][NP][256] symbol counts
+    uint32_t* err;                       // [n] bit 0: a stream outgrew the bound
+    uint32_t* tab;                       // [n][NP][256] (start << 16) | freq
+    unsigned long long* tile;            // [n][ntiles] stream bytes per tile, then exclusive prefix
+    uint32_t* state;                     // [n][NP][C] final coder states
+    uint16_t* scratch;                   // [n][NP][C][rw] renormalisation halfwords, the last one pushed first
+};
+static_assert(sizeof(LlEnc) < kMaxParamBytes, "LlEnc must stay under 4 KB of kernel parameters");
+
+struct LlDecChunk {
+    const uint8_t* base;
+    int64_t dst_tok;
+    int64_t payload_bytes;               // total_bytes - off_payload, from the caller: every stream must lie inside
+    int32_t t, pad;
+};
+
+struct LlDec {
+    PlaneTable pt;                       // destination planes (maxq unused)
+    int64_t sT, sH;
+    const int64_t* slot_map;
+    int32_t L, H, D, C, NP, tpp, ntiles, dtype, version, n_chunks;
+    const LlDecChunk* chunks;
+    unsigned long long* tile;            // [n][ntiles]
+    uint32_t* status;                    // [n] or NULL
+};
+static_assert(sizeof(LlDec) < kMaxParamBytes, "LlDec must stay under 4 KB of kernel parameters");
+
+__device__ __forceinline__ int ll_chunk_t(const LlEnc& P, int j) {
+    return j == P.n_chunks - 1 ? P.last_chunk_tokens : P.chunk_tokens;
+}
+
+__device__ __forceinline__ uint32_t rotl1(uint32_t u) { return ((u << 1) | (u >> 15)) & 0xffffu; }
+__device__ __forceinline__ uint32_t rotr1(uint32_t v) { return ((v >> 1) | (v << 15)) & 0xffffu; }
+
+// exclusive prefix of v over a CTA of NT threads, and the CTA's total (every thread must call it)
+template <int NT, class T>
+__device__ __forceinline__ T cta_excl_scan(T v, T* s_w, T* total) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    T inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const T y = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += y;
+    }
+    if (lane == 31) s_w[w] = inc;
+    __syncthreads();
+    T base = 0, tot = 0;
+#pragma unroll
+    for (int i = 0; i < NT / 32; ++i) {
+        const T x = s_w[i];
+        if (i < w) base += x;
+        tot += x;
+    }
+    __syncthreads();
+    *total = tot;
+    return base + inc - v;
+}
+
+// ------------------------------------------------------------------------------------------ encode
+// 1) symbol histogram of one (chunk, plane, channel tile, slice of kSlice tokens): warp-private bins in shared memory,
+//    lanes with equal symbols aggregated (__match_any_sync), then one global add per nonzero bin
+template <bool PAGED>
+__global__ void __launch_bounds__(kCT) ll_hist_kernel(LlEnc P) {
+    __shared__ uint32_t s_h[kCT / 32][kSyms];
+    const int j = blockIdx.z, p = blockIdx.y;
+    const int tile = blockIdx.x % P.tpp, slice = blockIdx.x / P.tpp;
+    const int t = ll_chunk_t(P, j);
+    const int i0 = slice * kSlice;
+    if (i0 >= t) return;
+    const int i1 = min(t, i0 + kSlice);
+    for (int i = threadIdx.x; i < (kCT / 32) * kSyms; i += kCT) (&s_h[0][0])[i] = 0u;
+    __syncthreads();
+    const int c = tile * kCT + threadIdx.x;
+    const bool on = c < P.C;
+    const int h = on ? c / P.D : 0, d = on ? c - h * P.D : 0;
+    const uint16_t* base = P.pt.p[p] + (int64_t)h * P.sH + d;
+    const int64_t tok0 = P.tok_begin + (int64_t)j * P.chunk_tokens;
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int i = i0; i < i1; i += 4) {
+        uint32_t u[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+            u[k] = on && i + k < i1 ? __ldg(base + tok_row<PAGED>(P.slot_map, tok0 + i + k) * P.sT) : 0u;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint32_t sym = on && i + k < i1 ? rotl1(u[k]) >> 8 : 0x100u;   // 0x100: no symbol
+            const uint32_t peers = __match_any_sync(0xffffffffu, sym);
+            if (sym < 0x100u && lane == __ffs(peers) - 1) atomicAdd(&s_h[w][sym], (uint32_t)__popc(peers));
+        }
+    }
+    __syncthreads();
+    uint32_t* g = P.hist + ((int64_t)j * P.NP + p) * kSyms;
+    for (int s = threadIdx.x; s < kSyms; s += kCT) {
+        uint32_t v = 0u;
+#pragma unroll
+        for (int k = 0; k < kCT / 32; ++k) v += s_h[k][s];
+        if (v) atomicAdd(g + s, v);
+    }
+}
+
+// 2) frequency row of one (chunk, plane), one thread per symbol (the normalisation of include/b200kv.h):
+//    K = symbols that occur, N = C * t;  f_s = n_s ? 1 + floor(n_s * (4096 - K) / N) : 0;  the symbol with the largest
+//    count (the smallest such symbol on ties) gets 4096 - sum(f) more.
+__global__ void __launch_bounds__(kSyms) ll_norm_kernel(LlEnc P) {
+    __shared__ uint32_t s_w[kSyms / 32];
+    __shared__ unsigned long long s_k[kSyms / 32];
+    const int j = blockIdx.y, p = blockIdx.x, s = threadIdx.x;
+    const int t = ll_chunk_t(P, j);
+    const int64_t row = (int64_t)j * P.NP + p;
+    const uint32_t n = P.hist[row * kSyms + s];
+    const uint32_t K = (uint32_t)__syncthreads_count(n != 0u);
+    const uint64_t N = (uint64_t)P.C * (uint64_t)t;
+    uint32_t f = n ? 1u + (uint32_t)(((uint64_t)n * (kM - K)) / N) : 0u;
+    uint32_t F;
+    cta_excl_scan<kSyms>(f, s_w, &F);
+    // argmax of (count, -symbol)
+    unsigned long long key = n ? ((unsigned long long)n << 8) | (unsigned long long)(255 - s) : 0ull;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long y = __shfl_xor_sync(0xffffffffu, key, o);
+        key = y > key ? y : key;
+    }
+    if ((threadIdx.x & 31) == 0) s_k[threadIdx.x >> 5] = key;
+    __syncthreads();
+    unsigned long long best = 0ull;
+#pragma unroll
+    for (int k = 0; k < kSyms / 32; ++k) best = s_k[k] > best ? s_k[k] : best;
+    if (s == 255 - (int)(best & 0xffull)) f += kM - F;
+    uint32_t tot;
+    const uint32_t start = cta_excl_scan<kSyms>(f, s_w, &tot);
+    P.tab[row * kSyms + s] = (start << 16) | f;
+    uint8_t* cont = P.out + (int64_t)j * P.out_stride;
+    reinterpret_cast<uint16_t*>(cont + B200KV_HEADER_BYTES + (int64_t)p * kFreqRowBytes)[s] = (uint16_t)f;
+}
+
+// 3) one thread per (chunk, plane, channel): raw bytes to their place in the container, symbols rANS-coded from the last
+//    token to the first (so that the decoder runs forward) into the stream's scratch row.  Encoder step with M = 4096:
+//      if (x >> 20) >= f: push x & 0xffff, x >>= 16;   x = ((x / f) << 12) + (x mod f) + start
+//    The bound is compared as x >> 20 against f, not x against f << 20: a single-symbol plane has f = 4096, and 4096 << 20
+//    does not fit 32 bits.  With f = 4096 the step leaves x unchanged and pushes nothing.  Plain integer division.
+template <bool PAGED>
+__global__ void __launch_bounds__(kCT) ll_encode_kernel(LlEnc P) {
+    __shared__ uint32_t s_tab[kSyms];
+    __shared__ unsigned long long s_w[kCT / 32];
+    const int j = blockIdx.z, p = blockIdx.y, tile = blockIdx.x;
+    const int t = ll_chunk_t(P, j);
+    const int64_t row = (int64_t)j * P.NP + p;
+    for (int s = threadIdx.x; s < kSyms; s += kCT) s_tab[s] = P.tab[row * kSyms + s];
+    __syncthreads();
+    const int c = tile * kCT + threadIdx.x;
+    const bool on = c < P.C;
+    const LlLayout lo = ll_layout(P.NP, P.C, t);
+    uint8_t* cont = P.out + (int64_t)j * P.out_stride;
+    uint32_t x = kRansLow;
+    int32_t k = 0;
+    if (on) {
+        const int h = c / P.D, d = c - h * P.D;
+        const uint16_t* base = P.pt.p[p] + (int64_t)h * P.sH + d;
+        const int64_t tok0 = P.tok_begin + (int64_t)j * P.chunk_tokens;
+        uint8_t* raw = cont + lo.off_raw + (int64_t)p * t * P.C + c;
+        uint16_t* srow = P.scratch + (row * P.C + c) * P.rw;
+        const int rw = P.rw;
+        uint32_t nxt = __ldg(base + tok_row<PAGED>(P.slot_map, tok0 + t - 1) * P.sT);
+        for (int i = t - 1; i >= 0; --i) {
+            const uint32_t u = nxt;
+            if (i > 0) nxt = __ldg(base + tok_row<PAGED>(P.slot_map, tok0 + i - 1) * P.sT);
+            const uint32_t v = rotl1(u);
+            raw[(int64_t)i * P.C] = (uint8_t)v;
+            const uint32_t e = s_tab[v >> 8];
+            const uint32_t f = e & 0xffffu;
+            if ((x >> 20) >= f) {
+                if (k < rw) srow[rw - 1 - k] = (uint16_t)x;
+                ++k;
+                x >>= 16;
+            }
+            x = ((x / f) << kScale) + (x % f) + (e >> 16);
+        }
+        if (k > ll_max_words(t)) atomicOr(&P.err[j], 1u);
+        reinterpret_cast<uint16_t*>(cont + lo.off_lens)[(int64_t)p * P.C + c] = (uint16_t)min(4 + 2 * k, 0xffff);
+        P.state[row * P.C + c] = x;
+    }
+    unsigned long long tot;
+    cta_excl_scan<kCT, unsigned long long>(on ? 4ull + 2ull * (unsigned long long)k : 0ull, s_w, &tot);
+    if (threadIdx.x == 0) P.tile[(int64_t)j * P.ntiles + (int64_t)p * P.tpp + tile] = tot;
+}
+
+// exclusive prefix of one chunk's tile values in place; returns the chunk's total to thread 0
+__device__ unsigned long long ll_scan_tiles(unsigned long long* v, int n) {
+    __shared__ unsigned long long s_w[32];
+    unsigned long long carry = 0ull;
+    for (int b = 0; b < n; b += blockDim.x) {
+        const int i = b + threadIdx.x;
+        const unsigned long long x = i < n ? v[i] : 0ull;
+        const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+        unsigned long long inc = x;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long y = __shfl_up_sync(0xffffffffu, inc, o);
+            if (lane >= o) inc += y;
+        }
+        if (lane == 31) s_w[w] = inc;
+        __syncthreads();
+        unsigned long long base = 0ull, tot = 0ull;
+        for (int k = 0; k < (int)(blockDim.x >> 5); ++k) {
+            if (k < w) base += s_w[k];
+            tot += s_w[k];
+        }
+        if (i < n) v[i] = carry + base + inc - x;
+        carry += tot;
+        __syncthreads();
+    }
+    return carry;
+}
+
+// 4a) per chunk: tile offsets, then the header and sizes_out[j] (0 when the chunk's status is nonzero)
+__global__ void __launch_bounds__(1024) ll_enc_scan_kernel(LlEnc P) {
+    const int j = blockIdx.x;
+    const unsigned long long payload = ll_scan_tiles(P.tile + (int64_t)j * P.ntiles, P.ntiles);
+    if (threadIdx.x != 0) return;
+    const int t = ll_chunk_t(P, j);
+    const LlLayout lo = ll_layout(P.NP, P.C, t);
+    b200kv_header hd;
+    memset(&hd, 0, sizeof(hd));
+    hd.magic = B200KV_MAGIC;
+    hd.version = P.NP == P.L ? 6u : 5u;
+    hd.L = (uint32_t)P.L; hd.H = (uint32_t)P.H; hd.D = (uint32_t)P.D;
+    hd.ntokens = (uint32_t)t;
+    hd.ngroups = 1u;
+    hd.max_dtype = (uint32_t)P.dtype;
+    hd.payload_bytes = payload;
+    hd.total_bytes = (uint64_t)lo.off_payload + payload;
+    hd.status = P.err[j];
+    if (hd.total_bytes > (uint64_t)P.out_stride) hd.status |= 2u;     // cannot happen within the stream bound
+    *reinterpret_cast<b200kv_header*>(P.out + (int64_t)j * P.out_stride) = hd;
+    P.sizes_out[j] = hd.status ? 0ull : hd.total_bytes;
+}
+
+// 4b) streams into the payload, a warp per 32 streams: [LE32 state][halfwords in decode order]
+__global__ void __launch_bounds__(kCT) ll_compact_kernel(LlEnc P) {
+    __shared__ uint32_t s_w[kCT / 32];
+    const int j = blockIdx.z, p = blockIdx.y, tile = blockIdx.x;
+    if (P.err[j]) return;
+    const int t = ll_chunk_t(P, j);
+    const LlLayout lo = ll_layout(P.NP, P.C, t);
+    uint8_t* cont = P.out + (int64_t)j * P.out_stride;
+    const int64_t row = (int64_t)j * P.NP + p;
+    const int c = tile * kCT + threadIdx.x;
+    const bool on = c < P.C;
+    const uint32_t len = on ? reinterpret_cast<const uint16_t*>(cont + lo.off_lens)[(int64_t)p * P.C + c] : 0u;
+    uint32_t tot;
+    const uint32_t ex = cta_excl_scan<kCT>(len, s_w, &tot);
+    const unsigned long long off = (unsigned long long)lo.off_payload + P.tile[(int64_t)j * P.ntiles + (int64_t)p * P.tpp + tile] + ex;
+    const uint32_t st = on ? P.state[row * P.C + c] : 0u;
+    const int lane = threadIdx.x & 31;
+    const int cw = tile * kCT + (threadIdx.x & ~31);
+    for (int src = 0; src < 32; ++src) {
+        const uint32_t sl = __shfl_sync(0xffffffffu, len, src);
+        const unsigned long long so = __shfl_sync(0xffffffffu, off, src);
+        const uint32_t sx = __shfl_sync(0xffffffffu, st, src);
+        if (sl == 0u) continue;
+        const uint32_t nh = sl >> 1, k = nh - 2;
+        const uint16_t* r = P.scratch + (row * P.C + cw + src) * P.rw + (P.rw - k) - 2;
+        uint16_t* dst = reinterpret_cast<uint16_t*>(cont + so);
+        for (uint32_t q = lane; q < nh; q += 32)
+            dst[q] = q == 0 ? (uint16_t)sx : q == 1 ? (uint16_t)(sx >> 16) : r[q];
+    }
+}
+
+// ------------------------------------------------------------------------------------------ decode
+// stream bytes per tile, from the lengths section: one warp per tile
+__global__ void __launch_bounds__(128) ll_tile_sum_kernel(LlDec P) {
+    const int j = blockIdx.y;
+    const int tl = blockIdx.x * 4 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (tl >= P.ntiles) return;
+    const int p = tl / P.tpp, c0 = (tl - p * P.tpp) * kCT;
+    const uint16_t* lens = reinterpret_cast<const uint16_t*>(P.chunks[j].base + B200KV_HEADER_BYTES +
+                                                             (int64_t)P.NP * kFreqRowBytes) + (int64_t)p * P.C;
+    unsigned long long s = 0ull;
+    for (int c = c0 + lane; c < min(P.C, c0 + kCT); c += 32) s += lens[c];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) P.tile[(int64_t)j * P.ntiles + tl] = s;
+}
+
+__global__ void __launch_bounds__(1024) ll_dec_scan_kernel(LlDec P) {
+    ll_scan_tiles(P.tile + (int64_t)blockIdx.x * P.ntiles, P.ntiles);
+}
+
+// One CTA per (chunk, plane, tile of CT channels): the plane's frequency row becomes a 4096-entry slot -> symbol table and
+// (start, freq) pairs in shared memory; each thread decodes its stream forward, recombines every symbol with its raw
+// byte and stores the element through the destination descriptor.  Decoder step:
+//   slot = x & 4095;  s = sym(slot);  x = f(s) * (x >> 12) + slot - start(s);  if x < 2^16: x = (x << 16) | next LE16
+// and after the last token x == 2^16 with every halfword of the stream consumed.  Reads stay inside the stream's own
+// bytes, and the stream inside the payload, whatever the lengths and frequency rows say.
+template <bool PAGED>
+__global__ void __launch_bounds__(kCT) ll_decode_kernel(LlDec P) {
+    __shared__ uint32_t s_ent[kSyms];
+    __shared__ uint8_t s_sym[kM];
+    __shared__ uint32_t s_w[kCT / 32];
+    const int j = blockIdx.z, p = blockIdx.y, tile = blockIdx.x;
+    const LlDecChunk dc = P.chunks[j];
+    const int t = dc.t;
+    const LlLayout lo = ll_layout(P.NP, P.C, t);
+    uint32_t bad = 0u;
+    if (threadIdx.x == 0) {
+        const b200kv_header* hd = reinterpret_cast<const b200kv_header*>(dc.base);
+        if (hd->magic != B200KV_MAGIC || hd->version != (uint32_t)P.version || hd->L != (uint32_t)P.L ||
+            hd->H != (uint32_t)P.H || hd->D != (uint32_t)P.D || hd->ntokens != (uint32_t)t ||
+            hd->max_dtype != (uint32_t)P.dtype)
+            bad |= 4u;
+    }
+    // frequency row: two symbols per thread
+    const uint16_t* frow = reinterpret_cast<const uint16_t*>(dc.base + B200KV_HEADER_BYTES + (int64_t)p * kFreqRowBytes);
+    const uint32_t f0 = frow[2 * threadIdx.x], f1 = frow[2 * threadIdx.x + 1];
+    uint32_t ftot;
+    const uint32_t st0 = cta_excl_scan<kCT>(f0 + f1, s_w, &ftot);
+    if (ftot != kM) {                                   // damaged frequency row: nothing of this plane is decoded
+        if (threadIdx.x == 0 && P.status != nullptr) atomicOr(&P.status[j], bad | 1u);
+        return;
+    }
+    s_ent[2 * threadIdx.x] = (st0 << 16) | f0;
+    s_ent[2 * threadIdx.x + 1] = ((st0 + f0) << 16) | f1;
+    __syncthreads();
+    for (int slot = threadIdx.x; slot < (int)kM; slot += kCT) {
+        int s = 0;                                      // the last symbol whose start <= slot: it has f >= 1
+#pragma unroll
+        for (int step = kSyms / 2; step > 0; step >>= 1)
+            if ((s_ent[s + step] >> 16) <= (uint32_t)slot) s += step;
+        s_sym[slot] = (uint8_t)s;
+    }
+    __syncthreads();
+    const int c = tile * kCT + threadIdx.x;
+    const bool on = c < P.C;
+    const uint32_t len = on ? reinterpret_cast<const uint16_t*>(dc.base + lo.off_lens)[(int64_t)p * P.C + c] : 0u;
+    uint32_t tot;
+    const uint32_t ex = cta_excl_scan<kCT>(len, s_w, &tot);
+    if (on) {
+        const unsigned long long off = P.tile[(int64_t)j * P.ntiles + (int64_t)p * P.tpp + tile] + ex;
+        if (off + len > (unsigned long long)dc.payload_bytes) {
+            bad |= 2u;
+        } else if (len < 4u || ((len | off) & 1u)) {     // a damaged odd length before this stream makes its start odd
+            bad |= 1u;
+        } else {
+            const uint16_t* sp = reinterpret_cast<const uint16_t*>(dc.base + lo.off_payload + off);
+            uint32_t x = (uint32_t)sp[0] | ((uint32_t)sp[1] << 16);
+            const uint16_t* wp = sp + 2;
+            const uint32_t nw = (len - 4u) >> 1;
+            uint32_t k = 0u;
+            const int h = c / P.D, d = c - h * P.D;
+            uint16_t* dst = const_cast<uint16_t*>(P.pt.p[p]) + (int64_t)h * P.sH + d;
+            const uint8_t* raw = dc.base + lo.off_raw + (int64_t)p * t * P.C + c;
+#pragma unroll 4
+            for (int i = 0; i < t; ++i) {
+                const uint32_t rb = raw[(int64_t)i * P.C];
+                const uint32_t slot = x & (kM - 1u);
+                const uint32_t sym = s_sym[slot];
+                const uint32_t e = s_ent[sym];
+                x = (e & 0xffffu) * (x >> kScale) + slot - (e >> 16);
+                if (x < kRansLow) {
+                    const uint32_t hw = k < nw ? (uint32_t)wp[k] : 0u;
+                    ++k;
+                    x = (x << 16) | hw;
+                }
+                dst[tok_row<PAGED>(P.slot_map, dc.dst_tok + i) * P.sT] = (uint16_t)rotr1((sym << 8) | rb);
+            }
+            if (x != kRansLow || k != nw) bad |= 1u;
+        }
+    }
+    if (bad != 0u && P.status != nullptr) atomicOr(&P.status[j], bad);
+}
+
+// ------------------------------------------------------------------------------------------ host side
+int fill_planes(const b200kv_kv_desc* kv, PlaneTable* pt) {
+    float bins[B200KV_MAX_PLANES];
+    for (int i = 0; i < B200KV_MAX_PLANES; ++i) bins[i] = 32.0f;   // no quantiser here; keeps the table valid
+    return make_plane_table(kv, bins, bins, pt);
+}
+
+struct LlEncWs { size_t hist, err, tab, tile, state, scratch, total; };
+LlEncWs ll_enc_ws(int64_t n, int64_t NP, int64_t C, int chunk_tokens, int64_t* rw_out) {
+    const int64_t tpp = (C + kCT - 1) / kCT;
+    const int64_t rw = (ll_max_words(chunk_tokens) + 1) & ~(int64_t)1;
+    LlEncWs w;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { const size_t at = o; o = (o + bytes + 255) & ~(size_t)255; return at; };
+    w.hist = take(sizeof(uint32_t) * n * NP * kSyms);
+    w.err = take(sizeof(uint32_t) * n);
+    w.tab = take(sizeof(uint32_t) * n * NP * kSyms);
+    w.tile = take(sizeof(unsigned long long) * n * NP * tpp);
+    w.state = take(sizeof(uint32_t) * n * NP * C);
+    w.scratch = take(sizeof(uint16_t) * n * NP * C * rw);
+    w.total = o;
+    if (rw_out) *rw_out = rw;
+    return w;
+}
+
+size_t ll_dec_ws(int64_t n, int64_t NP, int64_t C, size_t* off_tile) {
+    const int64_t tpp = (C + kCT - 1) / kCT;
+    *off_tile = ((size_t)sizeof(LlDecChunk) * n + 255) & ~(size_t)255;
+    return *off_tile + sizeof(unsigned long long) * n * NP * tpp;
+}
+
+bool shape_ok(int32_t L, int32_t H, int32_t D, int32_t t) {
+    return L > 0 && 2 * (int64_t)L <= B200KV_MAX_PLANES && H > 0 && D > 0 && (int64_t)H * D < (1ll << 24) && t > 0 &&
+           t <= kMaxTokens;
+}
+
+}  // namespace
+}  // namespace b200kv
+
+using namespace b200kv;
+
+extern "C" {
+
+int b200kv_lossless_layout(int32_t L, int32_t H, int32_t D, int32_t ntokens, int32_t latent,
+                           b200kv_lossless_layout_t* out) {
+    B2_REQUIRE(out != nullptr, "out is NULL");
+    B2_REQUIRE(shape_ok(L, H, D, ntokens), "bad shape (L <= 128, H * D < 2^24, 1 <= ntokens <= 4096)");
+    const LlLayout lo = ll_layout(latent ? L : 2 * L, (int64_t)H * D, ntokens);
+    out->off_freq = lo.off_freq;
+    out->off_lens = lo.off_lens;
+    out->off_raw = lo.off_raw;
+    out->off_payload = lo.off_payload;
+    out->fixed_bytes = lo.off_payload;
+    out->max_stream_bytes = lo.max_stream;
+    out->max_total_bytes = lo.max_total;
+    return 0;
+}
+
+int64_t b200kv_lossless_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t chunk_tokens, int32_t n_chunks,
+                                        int32_t latent, int32_t decode) {
+    if (!shape_ok(L, H, D, chunk_tokens) || n_chunks <= 0) return -2;
+    const int64_t NP = latent ? L : 2 * (int64_t)L, C = (int64_t)H * D;
+    if (decode) {
+        size_t off;
+        return (int64_t)ll_dec_ws(n_chunks, NP, C, &off);
+    }
+    return (int64_t)ll_enc_ws(n_chunks, NP, C, chunk_tokens, nullptr).total;
+}
+
+int b200kv_lossless_encode(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
+                           int32_t last_chunk_tokens, void* out, int64_t out_stride, uint64_t* sizes_out,
+                           void* workspace, int64_t workspace_bytes, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    LlEnc P;
+    if (int rc = fill_planes(kv, &P.pt)) return rc;
+    B2_REQUIRE(shape_ok(kv->L, kv->H, kv->D, chunk_tokens), "bad shape (H * D < 2^24, 1 <= chunk_tokens <= 4096)");
+    B2_REQUIRE(n_chunks > 0 && n_chunks <= 65535, "n_chunks must be in [1, 65535]");
+    B2_REQUIRE(last_chunk_tokens > 0 && last_chunk_tokens <= chunk_tokens, "last_chunk_tokens out of range");
+    B2_REQUIRE(out != nullptr && (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (out_stride & 15) == 0,
+               "out / out_stride must be 16-byte aligned");
+    B2_REQUIRE(sizes_out != nullptr, "sizes_out is NULL");
+    B2_REQUIRE(tok_begin >= 0, "tok_begin must be >= 0");
+    P.NP = kv_ppl(kv) * kv->L;
+    P.L = kv->L; P.H = kv->H; P.D = kv->D; P.C = kv->H * kv->D; P.dtype = kv_dtype(kv);
+    const LlLayout lo = ll_layout(P.NP, P.C, chunk_tokens);
+    B2_REQUIRE(out_stride >= lo.max_total, "out_stride smaller than the worst-case container (b200kv_lossless_layout)");
+    P.sT = kv->sT; P.sH = kv->sH; P.tok_begin = tok_begin;
+    P.slot_map = kv->slot_map;
+    P.n_chunks = n_chunks; P.chunk_tokens = chunk_tokens; P.last_chunk_tokens = last_chunk_tokens;
+    P.tpp = (P.C + kCT - 1) / kCT;
+    P.ntiles = P.NP * P.tpp;
+    int64_t rw;
+    const LlEncWs w = ll_enc_ws(n_chunks, P.NP, P.C, chunk_tokens, &rw);
+    B2_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)w.total, "workspace too small");
+    P.rw = (int32_t)rw;
+    P.out = static_cast<uint8_t*>(out);
+    P.out_stride = out_stride;
+    P.sizes_out = sizes_out;
+    uint8_t* ws = static_cast<uint8_t*>(workspace);
+    P.hist = reinterpret_cast<uint32_t*>(ws + w.hist);
+    P.err = reinterpret_cast<uint32_t*>(ws + w.err);
+    P.tab = reinterpret_cast<uint32_t*>(ws + w.tab);
+    P.tile = reinterpret_cast<unsigned long long*>(ws + w.tile);
+    P.state = reinterpret_cast<uint32_t*>(ws + w.state);
+    P.scratch = reinterpret_cast<uint16_t*>(ws + w.scratch);
+    B2_CHECK_CUDA(cudaMemsetAsync(ws, 0, w.tab, stream));        // histograms and error words
+    const bool paged = kv->slot_map != nullptr;
+    const unsigned nslices = (unsigned)((chunk_tokens + kSlice - 1) / kSlice);
+    const dim3 ghist((unsigned)P.tpp * nslices, (unsigned)P.NP, (unsigned)n_chunks);
+    const dim3 gtile((unsigned)P.tpp, (unsigned)P.NP, (unsigned)n_chunks);
+    if (paged) ll_hist_kernel<true><<<ghist, kCT, 0, stream>>>(P);
+    else ll_hist_kernel<false><<<ghist, kCT, 0, stream>>>(P);
+    B2_CHECK_CUDA(cudaGetLastError());
+    ll_norm_kernel<<<dim3((unsigned)P.NP, (unsigned)n_chunks), kSyms, 0, stream>>>(P);
+    B2_CHECK_CUDA(cudaGetLastError());
+    if (paged) ll_encode_kernel<true><<<gtile, kCT, 0, stream>>>(P);
+    else ll_encode_kernel<false><<<gtile, kCT, 0, stream>>>(P);
+    B2_CHECK_CUDA(cudaGetLastError());
+    ll_enc_scan_kernel<<<(unsigned)n_chunks, 1024, 0, stream>>>(P);
+    B2_CHECK_CUDA(cudaGetLastError());
+    ll_compact_kernel<<<gtile, kCT, 0, stream>>>(P);
+    B2_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int b200kv_lossless_decode(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                           const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,
+                           int32_t max_dtype, const b200kv_kv_desc* dst, uint32_t* status_out, void* workspace,
+                           int64_t workspace_bytes, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    LlDec P;
+    if (int rc = fill_planes(dst, &P.pt)) return rc;
+    B2_REQUIRE(containers && offsets && total_bytes && ntokens && dst_tok && n_chunks > 0 && n_chunks <= 65535,
+               "bad chunk arrays");
+    B2_REQUIRE(max_dtype == B200KV_DT_BF16 || max_dtype == B200KV_DT_FP16, "bad max_dtype");
+    B2_REQUIRE(kv_dtype(dst) == max_dtype,
+               "the destination's dtype is not the stored one: a lossless container is decoded into its own dtype only");
+    B2_REQUIRE(shape_ok(dst->L, dst->H, dst->D, 1), "bad destination shape");
+    P.NP = kv_ppl(dst) * dst->L;
+    P.L = dst->L; P.H = dst->H; P.D = dst->D; P.C = dst->H * dst->D;
+    P.dtype = max_dtype;
+    P.version = kv_ppl(dst) == 1 ? 6 : 5;
+    P.sT = dst->sT; P.sH = dst->sH;
+    P.slot_map = dst->slot_map;
+    P.n_chunks = n_chunks;
+    P.tpp = (P.C + kCT - 1) / kCT;
+    P.ntiles = P.NP * P.tpp;
+    for (int j = 0; j < n_chunks; ++j) {
+        B2_REQUIRE(ntokens[j] > 0 && ntokens[j] <= kMaxTokens, "ntokens must be in [1, 4096]");
+        B2_REQUIRE((offsets[j] & 15) == 0, "container offsets must be 16-byte aligned");
+        const LlLayout lj = ll_layout(P.NP, P.C, ntokens[j]);
+        B2_REQUIRE(total_bytes[j] >= lj.off_payload, "container shorter than its fixed sections (truncated or corrupt)");
+        B2_REQUIRE(offsets[j] >= 0 && offsets[j] + total_bytes[j] + B200KV_READ_SLACK <= containers_bytes,
+                   "containers buffer must extend B200KV_READ_SLACK bytes past the end of every container");
+    }
+    size_t off_tile;
+    const size_t need = ll_dec_ws(n_chunks, P.NP, P.C, &off_tile);
+    B2_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)need, "workspace too small");
+    uint8_t* ws = static_cast<uint8_t*>(workspace);
+    {   // chunk descriptors: small pageable -> device copy (staged by the driver before the call returns)
+        LlDecChunk* hc = static_cast<LlDecChunk*>(malloc(sizeof(LlDecChunk) * (size_t)n_chunks));
+        B2_REQUIRE(hc != nullptr, "out of host memory");
+        for (int j = 0; j < n_chunks; ++j) {
+            hc[j].base = static_cast<const uint8_t*>(containers) + offsets[j];
+            hc[j].dst_tok = dst_tok[j];
+            hc[j].payload_bytes = total_bytes[j] - ll_layout(P.NP, P.C, ntokens[j]).off_payload;
+            hc[j].t = ntokens[j];
+            hc[j].pad = 0;
+        }
+        cudaError_t e = cudaMemcpyAsync(ws, hc, sizeof(LlDecChunk) * (size_t)n_chunks, cudaMemcpyHostToDevice, stream);
+        free(hc);
+        B2_CHECK_CUDA(e);
+    }
+    P.chunks = reinterpret_cast<const LlDecChunk*>(ws);
+    P.tile = reinterpret_cast<unsigned long long*>(ws + off_tile);
+    P.status = status_out;
+    if (status_out) B2_CHECK_CUDA(cudaMemsetAsync(status_out, 0, sizeof(uint32_t) * (size_t)n_chunks, stream));
+    ll_tile_sum_kernel<<<dim3((unsigned)((P.ntiles + 3) / 4), (unsigned)n_chunks), 128, 0, stream>>>(P);
+    B2_CHECK_CUDA(cudaGetLastError());
+    ll_dec_scan_kernel<<<(unsigned)n_chunks, 1024, 0, stream>>>(P);
+    B2_CHECK_CUDA(cudaGetLastError());
+    const dim3 g((unsigned)P.tpp, (unsigned)P.NP, (unsigned)n_chunks);
+    if (P.slot_map) ll_decode_kernel<true><<<g, kCT, 0, stream>>>(P);
+    else ll_decode_kernel<false><<<g, kCT, 0, stream>>>(P);
+    B2_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+}  // extern "C"

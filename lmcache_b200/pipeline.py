@@ -244,7 +244,8 @@ class UploadRing:
 
 
 class HostContainer:
-    """One CacheGen container in a page-locked slab block, with the header fields its upload and decode need."""
+    """One container (CacheGen, or lossless: versions 5 and 6) in a page-locked slab block, with the header fields its
+    upload and decode need."""
     __slots__ = ("blk", "nbytes", "ntokens", "L", "H", "D", "max_dtype", "coder", "last_read", "planes", "dev",
                  "dev_ready", "dev_read")
 
@@ -272,13 +273,14 @@ def _d2h_stream(device: torch.device) -> torch.cuda.Stream:
 
 
 def land(slab, slot: WaveSlot, batch, blocks: Optional[list] = None,
-         dev_dst: Optional[Sequence[Optional[int]]] = None) -> List[HostContainer]:
+         dev_dst: Optional[Sequence[Optional[int]]] = None, parse: Callable = parse_header) -> List[HostContainer]:
     """Store-pipeline sink side: copy a finished wave's containers out of slot.dev into fresh blocks of `slab` (exactly
     their bytes, on the device's copy stream), wait for the copies, and parse every header.  Raises -- with every block
     freed -- when a copy fails or a container carries an encoder error.  `blocks`: blocks the caller allocated for the
     first len(blocks) containers (a bounded tier); only those are landed.  `dev_dst`: per container, a device address
-    that gets a copy of it as well (None: none), on the same stream and before the same wait.  A layer-wise store's slot
-    (SegmentSlot) lands through land_segments."""
+    that gets a copy of it as well (None: none), on the same stream and before the same wait.  `parse`: the header check
+    of the codec that wrote the wave (a lossless codec's for its containers).  A layer-wise store's slot (SegmentSlot)
+    lands through land_segments."""
     if isinstance(slot, SegmentSlot):
         return land_segments(slab, slot, batch, blocks, dev_dst)
     dev = slot.dev.device
@@ -308,7 +310,7 @@ def land(slab, slot: WaveSlot, batch, blocks: Optional[list] = None,
         po = po.reshape(len(blocks), N.MAX_PLANES + 1)
         recs = []
         for j, blk in enumerate(blocks):
-            hd = parse_header(blk.view())
+            hd = parse(blk.view())
             P = N.planes_of(hd.version, hd.L)
             recs.append(HostContainer(blk, blk.nbytes, hd, po[j, :P + 1].copy() if po[j, 0] >= 0 else None))
         return recs
@@ -557,9 +559,10 @@ def land_segments(slab, slot: SegmentSlot, batch, blocks: Optional[list] = None,
 def read_container(codec: CacheGenCodec, blk, nbytes: int, latent: bool = False) -> Optional[HostContainer]:
     """The record of a container a disk read or a GET put into the first `nbytes` of `blk`, or None -- with the block
     freed -- when it is damaged, was written with another model's bins, or holds the other kind of KV than `latent`
-    says (version 4 for a latent engine, versions 1 to 3 otherwise): a miss, not an error."""
+    says (version 4 for a latent engine, versions 1 to 3 otherwise; versions 6 and 5 for a lossless codec): a miss, not an
+    error.  The header is checked by the codec's own parse_header, so a container of the other codec family is a miss."""
     try:
-        hd = parse_header(blk.view()[:nbytes])
+        hd = codec.parse_header(blk.view()[:nbytes])
         if codec.accepts(hd, latent):
             return HostContainer(blk, nbytes, hd, plane_offsets(blk.view()[:nbytes]))   # on the reader's thread
     except ValueError:
@@ -636,10 +639,12 @@ class HeadWindow(NamedTuple):
 def _continues_match(r: HostContainer, first: Optional[HostContainer], dst: KvView, tok: int,
                      src_H: Optional[int] = None) -> bool:
     """May container `r`, landing at token `tok` of `dst`, extend a match that began with `first` (None: r is first)?
-    src_H: the heads r must hold when it is decoded through a head window (None: dst's).  A version-4 container fits a
-    latent destination only, and every other version a (K, V) one."""
+    src_H: the heads r must hold when it is decoded through a head window (None: dst's).  A version-4 or version-6
+    container fits a latent destination only, and every other version a (K, V) one; a lossless container (versions 5
+    and 6) fits a destination of its own dtype only."""
     return (r.L, r.H, r.D) == (dst.L, dst.H if src_H is None else src_H, dst.D) and tok + r.ntokens <= dst.ntokens and \
-        (r.coder == N.CODER_LATENT) == dst.latent and \
+        bool(r.coder & N.KV_LATENT) == dst.latent and \
+        ((r.coder & 0xff) != N.CODER_LOSSLESS or r.max_dtype == dst.dtype_code) and \
         (first is None or (r.max_dtype, r.coder) == (first.max_dtype, first.coder))
 
 

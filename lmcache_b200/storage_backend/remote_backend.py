@@ -199,7 +199,7 @@ class LMCRemoteBackend(LMCBackendInterface):
         """store worker: one wave's containers -> page-locked slab (land() raises on a nonzero encoder status: nothing
         corrupt leaves the host), then k-way send"""
         from lmcache_b200.pipeline import land
-        blocks = [rec.blk for rec in land(self._host_slab(), slot, batch)]
+        blocks = [rec.blk for rec in land(self._host_slab(), slot, batch, parse=self.serializer.codec.parse_header)]
         try:
             def send(key, blk):
                 self._conn().set(self._combine_key(key), blk.view())
@@ -287,8 +287,9 @@ class LMCRemoteBackend(LMCBackendInterface):
         return read_container(self.deserializer.codec, blk, int(n), self.latent)
 
     def peek_geometry(self, key: CacheEngineKey, fmt: str = "vllm"):
-        """(L, H, D, output dtype) from the header of the first chunk's container.  The fetched container is kept for the
-        get_kv_into call that follows, so a retrieve-only replica neither decodes nor fetches chunk 0 twice."""
+        """(L, H, D, output dtype) from the header of the first chunk's container -- the stored dtype when the serde
+        decodes into it (out_dtype() None: the lossless serde).  The fetched container is kept for the get_kv_into call
+        that follows, so a retrieve-only replica neither decodes nor fetches chunk 0 twice."""
         if not (self._striped() and hasattr(self.deserializer, "out_dtype")):
             return None
         rec = self._fetch(key, 256 << 20, self.connection)       # the geometry is what we are asking for: be generous
@@ -297,7 +298,11 @@ class LMCRemoteBackend(LMCBackendInterface):
         if self._peek is not None:
             self._peek[1].blk.free()
         self._peek = (key, rec)
-        return (rec.L, rec.H, rec.D, self.deserializer.out_dtype())
+        od = self.deserializer.out_dtype()
+        if od is None:
+            from lmcache_b200.codec import dtype_of_code
+            od = dtype_of_code(rec.max_dtype)
+        return (rec.L, rec.H, rec.D, od)
 
     def get_kv_into(self, keys: List[CacheEngineKey], dst, dst_tok0: int, chunk_size: int) -> int:
         """Fetch consecutive chunks until the first miss and decode them straight into `dst` (chunk i lands at token
