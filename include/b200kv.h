@@ -40,7 +40,9 @@ extern "C" {
                                     *    b200kv_encode_layers_workspace_bytes / b200kv_encode_layers_plan /
                                     *    b200kv_encode_layers / b200kv_encode_layers_finish, b200kv_decode_plan_heads,
                                     *    b200kv_lossless_layout / b200kv_lossless_workspace_bytes / b200kv_lossless_encode /
-                                    *    b200kv_lossless_decode (container versions 5 and 6).
+                                    *    b200kv_lossless_decode (container versions 5 and 6), b200kv_lossless_plane_offsets /
+                                    *    b200kv_lossless_plane_offsets_device / b200kv_lossless_decode_plan /
+                                    *    b200kv_lossless_decode_layers (b200kv_lossless_decode_plan_t).
                                     *    B200KV_MAX_PLANES went from 128 to 256 (models of up to 128 layers): the row
                                     *    width of b200kv_plane_offsets_device, B200KV_MAX_PLANES + 1, and the size of
                                     *    b200kv_encode_plan_t, 256 -> 512 words, changed with it; a caller takes them
@@ -375,6 +377,46 @@ int b200kv_lossless_decode(const void* containers, int64_t containers_bytes, con
                            const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,
                            int32_t max_dtype, const b200kv_kv_desc* dst, uint32_t* status_out, void* workspace,
                            int64_t workspace_bytes, void* stream);
+
+/* Host side: where each plane's streams lie in a lossless container in host memory (the header and the lengths section
+ * are read, nothing else; nbytes >= off_raw): out[0..P], the streams of plane p (keys of layer p, then values of layer
+ * p - L; P = L for version 6) are bytes [out[p], out[p+1]) of the container, out[0] = off_payload.  Plane p's raw rows are
+ * bytes [off_raw + p * t * C, off_raw + (p + 1) * t * C): the layout gives them.  Returns 0, 1 when the lengths do not
+ * add up to header.total_bytes (damaged), <0 for anything that is not a lossless container of a possible shape. */
+int b200kv_lossless_plane_offsets(const void* container, int64_t nbytes, int64_t* out, int32_t n_out);
+/* Same for n containers in DEVICE memory at containers + j*stride, as b200kv_plane_offsets_device: row j of out (DEVICE or
+ * mapped-host int64[n][B200KV_MAX_PLANES + 1]) gets the P + 1 offsets and zeros in the rest of the row, or -1 in its entry
+ * 0 for a container that is not lossless, whose fixed sections do not fit its total_bytes or `stride` (nothing past the
+ * header is read then), or whose lengths do not add up.  Asynchronous on `stream`. */
+int b200kv_lossless_plane_offsets_device(const void* containers, int64_t stride, int32_t n, int64_t* out, void* stream);
+
+/*
+ * The lossless decode in two steps, as b200kv_decode_plan / b200kv_decode_layers for the CacheGen containers: a caller
+ * decodes a layer as soon as its bytes have arrived.  b200kv_lossless_decode == plan + layers(0, L).
+ *
+ * b200kv_lossless_decode_plan takes b200kv_lossless_decode's arguments and makes all of its checks, zeroes status_out,
+ * writes the chunk descriptors into `workspace` and enqueues the stream-offset kernels.  Those read [0, off_raw) of every
+ * container only (header, frequency rows, lengths), so the raw rows and the streams may still be on their way.  The
+ * workspace, containers buffer, destination and status_out must stay valid until the last layers call has run.
+ *
+ * b200kv_lossless_decode_layers enqueues the decode of layers [layer_begin, layer_end): planes layer_begin.. (keys) and
+ * L + layer_begin.. (values), or planes layer_begin.. alone for version 6, 0 <= layer_begin < layer_end <= L.  A call
+ * reads the header, its planes' frequency rows, the lengths, its planes' raw rows and its planes' streams; no byte of
+ * another plane reaches an output or a status bit.  It writes the destination rows of its layers only and ORs into the
+ * plan's status_out, so any set of calls that covers every layer once writes what b200kv_lossless_decode writes, status
+ * bits included.
+ */
+typedef struct b200kv_lossless_decode_plan_t {
+    uint64_t opaque[512];      /* the decode kernel's parameter block (its 3 KB plane table included) */
+} b200kv_lossless_decode_plan_t;
+
+int b200kv_lossless_decode_plan(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                                const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok,
+                                int32_t n_chunks, int32_t max_dtype, const b200kv_kv_desc* dst, uint32_t* status_out,
+                                void* workspace, int64_t workspace_bytes, b200kv_lossless_decode_plan_t* plan,
+                                void* stream);
+int b200kv_lossless_decode_layers(const b200kv_lossless_decode_plan_t* plan, int32_t layer_begin, int32_t layer_end,
+                                  void* stream);
 
 /*
  * Token-id prefix hash.  Replaces LMCacheEngine._chunk_tokens/_hash/_prefix_hash

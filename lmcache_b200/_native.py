@@ -87,6 +87,11 @@ class EncodePlan(ctypes.Structure):
     _fields_ = [("opaque", ctypes.c_uint64 * 512)]
 
 
+class LosslessDecodePlan(ctypes.Structure):
+    """struct b200kv_lossless_decode_plan_t (opaque, filled by b200kv_lossless_decode_plan)"""
+    _fields_ = [("opaque", ctypes.c_uint64 * 512)]
+
+
 assert ctypes.sizeof(Header) == HEADER_BYTES
 
 # name -> (restype, argtypes); every symbol include/b200kv.h declares
@@ -122,6 +127,11 @@ SIGNATURES = {
                                         c_i64, c_vp]),
     "b200kv_lossless_decode": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, ctypes.POINTER(KvDesc), c_vp,
                                         c_vp, c_i64, c_vp]),
+    "b200kv_lossless_plane_offsets": (c_i32, [c_vp, c_i64, c_vp, c_i32]),
+    "b200kv_lossless_plane_offsets_device": (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp]),
+    "b200kv_lossless_decode_plan": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, ctypes.POINTER(KvDesc),
+                                             c_vp, c_vp, c_i64, ctypes.POINTER(LosslessDecodePlan), c_vp]),
+    "b200kv_lossless_decode_layers": (c_i32, [ctypes.POINTER(LosslessDecodePlan), c_i32, c_i32, c_vp]),
     "b200kv_sha256_chain": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp]),
     "b200kv_sha256_chain_ready": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, ctypes.c_uint32, c_vp]),
     "b200kv_pack_chunks": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp]),
@@ -185,18 +195,20 @@ _pylib: Optional[ctypes.PyDLL] = None
 
 
 def pylib() -> ctypes.PyDLL:
-    """The library through ctypes.PyDLL, for b200kv_plane_offsets_device alone: the call keeps the GIL.  It is one
-    kernel launch on the store worker; giving the GIL up and taking it back there costs the store more than the launch
-    whenever the caller's thread is busy in Python (it spins on the hash chain's ready words while a store runs)."""
+    """The library through ctypes.PyDLL, for b200kv_plane_offsets_device and b200kv_lossless_plane_offsets_device alone:
+    the call keeps the GIL.  It is one kernel launch on the store worker; giving the GIL up and taking it back there costs
+    the store more than the launch whenever the caller's thread is busy in Python (it spins on the hash chain's ready words
+    while a store runs)."""
     global _pylib
     if _pylib is None:
         lib()
         with _lock:
             if _pylib is None:
                 L = ctypes.PyDLL(LIB_PATH)
-                res, args = SIGNATURES["b200kv_plane_offsets_device"]
-                L.b200kv_plane_offsets_device.restype = res
-                L.b200kv_plane_offsets_device.argtypes = args
+                for name in ("b200kv_plane_offsets_device", "b200kv_lossless_plane_offsets_device"):
+                    res, args = SIGNATURES[name]
+                    getattr(L, name).restype = res
+                    getattr(L, name).argtypes = args
                 _pylib = L
     return _pylib
 

@@ -270,7 +270,9 @@ class LMCacheEngine:
             raise ValueError("use_mla: the keys of a latent KV are shared by every tensor-parallel size already, "
                              "reshard_world_sizes must be None")
         local = config.local_device
-        cachegen_tier = ((local == "cpu" and config.local_serde == "cachegen") or local not in (None, "cpu", "cuda") or
+        # a directory keeps CacheGen containers unless local_serde is "lossless" (version 6 then, up to 4096 tokens)
+        cachegen_tier = ((local == "cpu" and config.local_serde == "cachegen") or
+                         (local not in (None, "cpu", "cuda") and config.local_serde != "lossless") or
                          (config.remote_url is not None and config.remote_serde == "cachegen"))
         if cachegen_tier and config.chunk_size > N.GROUP_TOKENS:
             raise ValueError(f"use_mla: a CacheGen tier keeps a latent KV in version-4 containers, which hold at most "
@@ -705,9 +707,11 @@ class LMCacheEngine:
     # ------------------------------------------------------------------ layer-wise retrieve
     def _layerwise_get(self):
         """(get_kv for _retrieve / _retrieve_paged, list that receives the LayerwiseUpload), or None: the backend has no
-        layer-major path (raw, remote and hybrid tiers) or its containers hold several groups (chunk_size > 256)"""
+        layer-major path (raw, remote and hybrid tiers) or its containers hold several groups (CacheGen containers of
+        more than 256 tokens; a lossless container is always one group)"""
         f = getattr(self.engine_, "get_kv_layerwise", None)
-        if f is None or not self._fast_path() or self.chunk_size > N.GROUP_TOKENS:
+        if f is None or not self._fast_path() or \
+                self.chunk_size > getattr(self.engine_, "layerwise_max_tokens", N.GROUP_TOKENS):
             return None
         uploads: List[LayerwiseUpload] = []
 
@@ -730,7 +734,8 @@ class LMCacheEngine:
         """retrieve(), with the KV made available one layer at a time: returns once the hit is known; ret_mask and the
         KV after synchronize() are those of retrieve().  On the compressed host and disk tiers the containers are
         uploaded and decoded layer-major, so layer 0 is ready after about 1/L of the bytes; on every other tier (and
-        for chunks of more than 256 tokens) this is retrieve() followed by one event that stands for every layer."""
+        for CacheGen chunks of more than 256 tokens) this is retrieve() followed by one event that stands for every
+        layer."""
         get_kv, uploads = self._layerwise_get() or (None, [])
         kv, ret_mask = self._retrieve(tokens, mask, get_kv)
         geom = self._kv_geometry()

@@ -600,6 +600,9 @@ class CacheGenCodec(_ContainerIO):
 
     # ------------------------------------------------------------------ helpers
     parse_header = staticmethod(parse_header)    # the CacheGen container check (versions 1 to 4)
+    plane_offsets = staticmethod(plane_offsets)  # where a version-3 / version-4 container's planes lie
+    plane_offsets_device = "b200kv_plane_offsets_device"     # the same for containers on the device (pipeline.land)
+    layerwise_max_tokens = N.GROUP_TOKENS         # a layer-major retrieve needs one group per container
 
     def coder_for(self, chunk_tokens: int, latent: bool = False) -> int:
         """The container this codec writes for chunks of `chunk_tokens`: the compact one holds <= 256 tokens.  A latent
@@ -933,6 +936,28 @@ def check_lossless_header(hd: "N.Header") -> None:
         raise ValueError("B2KV header: payload_bytes impossible for this shape")
 
 
+def lossless_plane_offsets(buf) -> Optional[np.ndarray]:
+    """Where the streams of each plane lie in a lossless container (`buf`: at least its header, frequency rows and
+    lengths), from its lengths section: int64[P + 1] (P = 2L, or L for version 6), the streams of plane p are bytes
+    [o[p], o[p + 1]) of the container, o[0] is off_payload and o[P] == total_bytes.  None when the lengths do not add up
+    to the header's total (a damaged container: it is only ever uploaded whole).  Plane p's raw rows come from the
+    layout: lossless_raw_rows."""
+    src = np.frombuffer(buf, dtype=np.uint8)
+    version, L = (int(v) for v in src[4:12].view(np.uint32))
+    if version not in (5, 6):
+        return None
+    o = np.empty(N.planes_of(version, L) + 1, dtype=np.int64)
+    rc = N.check(N.lib().b200kv_lossless_plane_offsets(src.ctypes.data, src.size, o.ctypes.data, o.size),
+                 "lossless_plane_offsets")
+    return o if rc == 0 else None
+
+
+def lossless_raw_rows(L: int, H: int, D: int, ntokens: int, latent: bool) -> Tuple[int, int]:
+    """(off_raw, bytes per plane) of a lossless container: plane p's raw rows are bytes
+    [off_raw + p * t * C, off_raw + (p + 1) * t * C)."""
+    return int(N.lossless_layout(L, H, D, ntokens, latent).off_raw), int(ntokens) * H * D
+
+
 class LosslessCodec(_ContainerIO):
     """Lossless encode / decode on the current CUDA device (container versions 5 and 6, include/b200kv.h): every
     element's high byte after a one-bit rotation (bf16: the exponent) is rANS-coded per (plane, channel) against one
@@ -946,6 +971,9 @@ class LosslessCodec(_ContainerIO):
         self._init_io()
 
     parse_header = staticmethod(parse_lossless_header)
+    plane_offsets = staticmethod(lossless_plane_offsets)
+    plane_offsets_device = "b200kv_lossless_plane_offsets_device"
+    layerwise_max_tokens = N.LOSSLESS_MAX_TOKENS   # a lossless container is always one group
 
     @staticmethod
     def coder_for(chunk_tokens: int, latent: bool = False) -> int:
@@ -1052,6 +1080,35 @@ class LosslessCodec(_ContainerIO):
         else:
             with self._dec_lock, torch.cuda.device(dst.device):
                 run()
+
+    def decode_plan(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
+                    ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
+                    stream: torch.cuda.Stream, status_ptr: int = 0) -> Tuple["N.LosslessDecodePlan", torch.Tensor]:
+        """CacheGenCodec.decode_plan for lossless containers (b200kv_lossless_decode_plan): enqueue on `stream` the
+        kernels that read [0, off_raw) of every container and return (plan, workspace); decode_layers decodes a range of
+        layers once its raw rows and streams are there.  The workspace is the caller's, recorded on `stream`."""
+        if coder not in (N.CODER_LOSSLESS, N.CODER_LOSSLESS_LATENT) or bool(coder & N.KV_LATENT) != dst.latent:
+            raise ValueError(f"coder {coder} does not name the lossless container of this destination")
+        n = len(offsets)
+        lib = N.lib()
+        ws = torch.empty(max(lib.b200kv_lossless_workspace_bytes(dst.L, dst.H, dst.D, max(ntokens), n, int(dst.latent),
+                                                                 1), 16),
+                         dtype=torch.uint8, device=dst.device)    # < 0: a shape the plan call refuses, with its reason
+        ws.record_stream(stream)
+        plan = N.LosslessDecodePlan()
+        N.check(lib.b200kv_lossless_decode_plan(base_ptr, int(buf_bytes), N.i64_array(list(offsets)),
+                                                N.i64_array(list(totals)), N.i32_array(list(ntokens)),
+                                                N.i64_array(list(dst_tok)), n, int(max_dtype), ctypes.byref(dst.desc),
+                                                status_ptr or None, ws.data_ptr(), ws.numel(), ctypes.byref(plan),
+                                                stream.cuda_stream), "lossless_decode_plan")
+        return plan, ws
+
+    @staticmethod
+    def decode_layers(plan: "N.LosslessDecodePlan", layer_begin: int, layer_end: int, stream: torch.cuda.Stream) -> None:
+        """Second half of the decode (b200kv_lossless_decode_layers): enqueue the decode of layers [layer_begin,
+        layer_end)."""
+        N.check(N.lib().b200kv_lossless_decode_layers(ctypes.byref(plan), int(layer_begin), int(layer_end),
+                                                      stream.cuda_stream), "lossless_decode_layers")
 
     def decode(self, containers: Sequence[Union[bytes, bytearray, memoryview, torch.Tensor]], dst: KvView,
                dst_tok: Sequence[int], stream: Optional[torch.cuda.Stream] = None) -> None:

@@ -35,16 +35,19 @@ class LMCacheEngineConfig:
     pipelined_backend: bool
     save_decode_cache: bool
     # not in the reference: how the LOCAL host tier keeps chunks.  None = raw blobs, as the reference does
-    # (local_backend.py:95-100); "cachegen" = CacheGen containers in page-locked memory (LMCLocalCompressedBackend).
-    # The environment variable LMCACHE_B200_LOCAL_SERDE sets the default for configurations that do not name it.
+    # (local_backend.py:95-100); "cachegen" = CacheGen containers in page-locked memory (LMCLocalCompressedBackend);
+    # "lossless" = lossless containers (versions 5 and 6), in page-locked memory or, for a directory, in the files of the
+    # disk tier, which are CacheGen containers otherwise.  The environment variable LMCACHE_B200_LOCAL_SERDE sets the
+    # default for configurations that do not name it.
     local_serde: Optional[str] = None
     # not in the reference: the most bytes the local CacheGen tier keeps (slab blocks of the host tier, .b2kv files of the
     # disk tier); beyond it chunks are evicted from the tail of the coldest chain (lmcache_b200/eviction.py).  None = no
-    # bound.  Only the two CacheGen tiers honour it (CreateStorageBackend rejects it elsewhere).
+    # bound.  Only the two CacheGen tiers and their lossless forms honour it (CreateStorageBackend rejects it elsewhere).
     local_capacity_bytes: Optional[int] = None
     # not in the reference: bytes of device memory that keep copies of the local CacheGen tier's containers, so that a
     # retrieve of a resident chunk decodes it in place instead of uploading it (lmcache_b200/device_cache.py).  None =
-    # off.  The level is inclusive: every device copy has its tier copy beside it.  Only the two CacheGen tiers take it.
+    # off.  The level is inclusive: every device copy has its tier copy beside it.  Only the two CacheGen tiers and their
+    # lossless forms take it.
     device_cache_bytes: Optional[int] = None
     # not in the reference: other tensor-parallel world sizes whose stored chunks a retrieve may decode into this rank's
     # KV heads once its own layout's prefix ends (lmcache_b200/reshard.py), tried in this order.  None = off.  Needs a
@@ -60,7 +63,7 @@ class LMCacheEngineConfig:
         if self.local_serde is None:
             import os
             self.local_serde = os.environ.get("LMCACHE_B200_LOCAL_SERDE") or None
-        if self.local_serde not in (None, "cachegen"):
+        if self.local_serde not in (None, "cachegen", "lossless"):
             raise ValueError(f"Invalid local serde: {self.local_serde}")
         c = self.local_capacity_bytes
         if c is not None and (isinstance(c, bool) or not isinstance(c, int) or c <= 0):

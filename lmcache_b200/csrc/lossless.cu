@@ -10,7 +10,8 @@
 //   encode: ll_hist_kernel (per-(chunk, plane) histogram) -> ll_norm_kernel (frequency rows) -> ll_encode_kernel (raw
 //           bytes in place, rANS into a worst-case scratch row) -> ll_scan_kernel (tile offsets, header, sizes_out) ->
 //           ll_compact_kernel (streams into the payload).  The KV is read twice: once for the histogram, once to code.
-//   decode: ll_tile_sum_kernel -> ll_scan_kernel (stream offsets from the lengths section) -> ll_decode_kernel.
+//   decode: ll_tile_sum_kernel -> ll_scan_kernel (stream offsets from the lengths section; the plan) ->
+//           ll_decode_kernel (once for every layer, or once per range of layers: b200kv_lossless_decode_layers).
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -77,11 +78,21 @@ struct LlDec {
     int64_t sT, sH;
     const int64_t* slot_map;
     int32_t L, H, D, C, NP, tpp, ntiles, dtype, version, n_chunks;
+    int32_t lb, nl;                      // the launch decodes layers [lb, lb + nl): blockIdx.y < nl keys, then values
     const LlDecChunk* chunks;
     unsigned long long* tile;            // [n][ntiles]
     uint32_t* status;                    // [n] or NULL
 };
 static_assert(sizeof(LlDec) < kMaxParamBytes, "LlDec must stay under 4 KB of kernel parameters");
+
+// What b200kv_lossless_decode_plan decided, kept in the caller's b200kv_lossless_decode_plan_t: the decode kernel's
+// parameter block (its chunk descriptors and tile offsets live in the workspace).
+constexpr uint32_t kLlPlanMagic = 0x4e4c504cu;   // "LPLN"
+struct LlPlan {
+    uint32_t magic, pad;
+    LlDec P;
+};
+static_assert(sizeof(LlPlan) <= sizeof(b200kv_lossless_decode_plan_t), "b200kv_lossless_decode_plan_t too small");
 
 __device__ __forceinline__ int ll_chunk_t(const LlEnc& P, int j) {
     return j == P.n_chunks - 1 ? P.last_chunk_tokens : P.chunk_tokens;
@@ -351,12 +362,16 @@ __global__ void __launch_bounds__(1024) ll_dec_scan_kernel(LlDec P) {
 //   slot = x & 4095;  s = sym(slot);  x = f(s) * (x >> 12) + slot - start(s);  if x < 2^16: x = (x << 16) | next LE16
 // and after the last token x == 2^16 with every halfword of the stream consumed.  Reads stay inside the stream's own
 // bytes, and the stream inside the payload, whatever the lengths and frequency rows say.
+// A launch covers the planes of layers [lb, lb + nl) only (b200kv_lossless_decode_layers): it reads the header, those
+// planes' frequency rows, the lengths section (through the tile offsets the plan computed from it), those planes' raw
+// rows and those planes' streams, and nothing else of the container.
 template <bool PAGED>
 __global__ void __launch_bounds__(kCT) ll_decode_kernel(LlDec P) {
     __shared__ uint32_t s_ent[kSyms];
     __shared__ uint8_t s_sym[kM];
     __shared__ uint32_t s_w[kCT / 32];
-    const int j = blockIdx.z, p = blockIdx.y, tile = blockIdx.x;
+    const int j = blockIdx.z, tile = blockIdx.x;
+    const int p = (int)blockIdx.y < P.nl ? P.lb + (int)blockIdx.y : P.L + P.lb + ((int)blockIdx.y - P.nl);
     const LlDecChunk dc = P.chunks[j];
     const int t = dc.t;
     const LlLayout lo = ll_layout(P.NP, P.C, t);
@@ -426,6 +441,59 @@ __global__ void __launch_bounds__(kCT) ll_decode_kernel(LlDec P) {
         }
     }
     if (bad != 0u && P.status != nullptr) atomicOr(&P.status[j], bad);
+}
+
+// The header fields a stream-offset computation trusts, checked before anything past the header is read: a lossless
+// version, a shape the calls accept, and -- for the device form -- fixed sections that fit total_bytes and `limit`.
+__host__ __device__ __forceinline__ bool ll_offsets_header_ok(const b200kv_header& hd, int64_t limit, LlLayout* lo,
+                                                              int* NP) {
+    if (hd.magic != B200KV_MAGIC || (hd.version != 5u && hd.version != 6u) || hd.L == 0u ||
+        hd.L > (uint32_t)(B200KV_MAX_PLANES / 2) || hd.H == 0u || hd.D == 0u ||
+        (uint64_t)hd.H * hd.D >= (1ull << 24) || hd.ntokens == 0u || hd.ntokens > (uint32_t)kMaxTokens)
+        return false;
+    *NP = hd.version == 6u ? (int)hd.L : 2 * (int)hd.L;
+    *lo = ll_layout(*NP, (int64_t)hd.H * hd.D, (int)hd.ntokens);
+    return (uint64_t)lo->off_payload <= hd.total_bytes && lo->off_payload <= limit;
+}
+
+// Stream offsets of lossless containers in device memory (b200kv_lossless_plane_offsets_device): one CTA of 32 warps
+// per container, one warp per plane at a time, summing the plane's u16 lengths.  out row j: [off_payload, end of plane
+// 0's streams, ..., end of plane P-1 = total_bytes], zeros after it; or -1 in entry 0 when the header is not that of a
+// lossless container whose fixed sections fit total_bytes and the row stride (nothing past the header is read then), or
+// the lengths do not add up to total_bytes.
+__global__ void __launch_bounds__(1024) ll_plane_offsets_kernel(const uint8_t* base, int64_t stride, int64_t* out) {
+    __shared__ unsigned long long s_sum[B200KV_MAX_PLANES];
+    const uint8_t* c = base + (int64_t)blockIdx.x * stride;
+    int64_t* o = out + (int64_t)blockIdx.x * (B200KV_MAX_PLANES + 1);
+    const b200kv_header hd = *reinterpret_cast<const b200kv_header*>(c);
+    LlLayout lo;
+    int NP;
+    if (!ll_offsets_header_ok(hd, stride, &lo, &NP)) {
+        if (threadIdx.x == 0) o[0] = -1;
+        return;
+    }
+    const int64_t C = (int64_t)hd.H * hd.D;
+    const uint16_t* lens = reinterpret_cast<const uint16_t*>(c + lo.off_lens);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int p = NP + 1 + (int)threadIdx.x; p <= B200KV_MAX_PLANES; p += blockDim.x) o[p] = 0;   // the row past P + 1
+    for (int p = warp; p < NP; p += blockDim.x >> 5) {
+        const uint16_t* row = lens + p * C;
+        unsigned long long sum = 0ull;
+        for (int64_t i = lane; i < C; i += 32) sum += row[i];
+#pragma unroll
+        for (int k = 16; k > 0; k >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, k);
+        if (lane == 0) s_sum[p] = sum;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int64_t off = lo.off_payload;
+        o[0] = off;
+        for (int p = 0; p < NP; ++p) {
+            off += (int64_t)s_sum[p];
+            o[p + 1] = off;
+        }
+        if (off != (int64_t)hd.total_bytes) o[0] = -1;
+    }
 }
 
 // ------------------------------------------------------------------------------------------ host side
@@ -553,12 +621,46 @@ int b200kv_lossless_encode(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t 
     return 0;
 }
 
-int b200kv_lossless_decode(const void* containers, int64_t containers_bytes, const int64_t* offsets,
-                           const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,
-                           int32_t max_dtype, const b200kv_kv_desc* dst, uint32_t* status_out, void* workspace,
-                           int64_t workspace_bytes, void* stream_) {
+int b200kv_lossless_plane_offsets(const void* container, int64_t nbytes, int64_t* out, int32_t n_out) {
+    B2_REQUIRE(container != nullptr && out != nullptr && nbytes >= (int64_t)sizeof(b200kv_header), "bad arguments");
+    b200kv_header hd;
+    memcpy(&hd, container, sizeof(hd));
+    LlLayout lo;
+    int NP;
+    B2_REQUIRE(ll_offsets_header_ok(hd, INT64_MAX, &lo, &NP),
+               "not a version-5 or version-6 container of a possible shape, or total_bytes shorter than its fixed sections");
+    B2_REQUIRE(n_out >= NP + 1, "out must hold P + 1 offsets (P = 2L, or L for version 6)");
+    B2_REQUIRE(nbytes >= lo.off_raw, "buffer shorter than the header, frequency rows and lengths");
+    const int64_t C = (int64_t)hd.H * hd.D;
+    const uint16_t* lens = reinterpret_cast<const uint16_t*>(static_cast<const uint8_t*>(container) + lo.off_lens);
+    int64_t o = lo.off_payload;
+    out[0] = o;
+    for (int p = 0; p < NP; ++p) {
+        for (int64_t c = 0; c < C; ++c) o += lens[p * C + c];
+        out[p + 1] = o;
+    }
+    return o == (int64_t)hd.total_bytes ? 0 : 1;
+}
+
+int b200kv_lossless_plane_offsets_device(const void* containers, int64_t stride, int32_t n, int64_t* out, void* stream) {
+    B2_REQUIRE(containers != nullptr && out != nullptr && n > 0 && stride >= (int64_t)sizeof(b200kv_header) &&
+               (stride & 15) == 0 && (reinterpret_cast<uintptr_t>(containers) & 15) == 0, "bad arguments");
+    ll_plane_offsets_kernel<<<(unsigned)n, 1024, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const uint8_t*>(containers), stride, out);
+    B2_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int b200kv_lossless_decode_plan(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                                const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok,
+                                int32_t n_chunks, int32_t max_dtype, const b200kv_kv_desc* dst, uint32_t* status_out,
+                                void* workspace, int64_t workspace_bytes, b200kv_lossless_decode_plan_t* plan_out,
+                                void* stream_) {
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    LlDec P;
+    B2_REQUIRE(plan_out != nullptr, "plan is NULL");
+    LlPlan* plan = reinterpret_cast<LlPlan*>(plan_out);
+    plan->magic = 0u;
+    LlDec& P = plan->P;
     if (int rc = fill_planes(dst, &P.pt)) return rc;
     B2_REQUIRE(containers && offsets && total_bytes && ntokens && dst_tok && n_chunks > 0 && n_chunks <= 65535,
                "bad chunk arrays");
@@ -609,11 +711,38 @@ int b200kv_lossless_decode(const void* containers, int64_t containers_bytes, con
     B2_CHECK_CUDA(cudaGetLastError());
     ll_dec_scan_kernel<<<(unsigned)n_chunks, 1024, 0, stream>>>(P);
     B2_CHECK_CUDA(cudaGetLastError());
-    const dim3 g((unsigned)P.tpp, (unsigned)P.NP, (unsigned)n_chunks);
+    plan->magic = kLlPlanMagic;
+    return 0;
+}
+
+int b200kv_lossless_decode_layers(const b200kv_lossless_decode_plan_t* plan_in, int32_t layer_begin, int32_t layer_end,
+                                  void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B2_REQUIRE(plan_in != nullptr, "plan is NULL");
+    const LlPlan* plan = reinterpret_cast<const LlPlan*>(plan_in);
+    B2_REQUIRE(plan->magic == kLlPlanMagic, "not a plan made by b200kv_lossless_decode_plan");
+    LlDec P = plan->P;
+    B2_REQUIRE(layer_begin >= 0 && layer_begin < layer_end && layer_end <= P.L, "layer range out of range");
+    P.lb = layer_begin;
+    P.nl = layer_end - layer_begin;
+    const int ppl = P.NP / P.L;
+    const dim3 g((unsigned)P.tpp, (unsigned)(ppl * P.nl), (unsigned)P.n_chunks);
     if (P.slot_map) ll_decode_kernel<true><<<g, kCT, 0, stream>>>(P);
     else ll_decode_kernel<false><<<g, kCT, 0, stream>>>(P);
     B2_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+int b200kv_lossless_decode(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                           const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok, int32_t n_chunks,
+                           int32_t max_dtype, const b200kv_kv_desc* dst, uint32_t* status_out, void* workspace,
+                           int64_t workspace_bytes, void* stream) {
+    b200kv_lossless_decode_plan_t plan;
+    if (int rc = b200kv_lossless_decode_plan(containers, containers_bytes, offsets, total_bytes, ntokens, dst_tok,
+                                             n_chunks, max_dtype, dst, status_out, workspace, workspace_bytes, &plan,
+                                             stream))
+        return rc;
+    return b200kv_lossless_decode_layers(&plan, 0, dst->L, stream);
 }
 
 }  // extern "C"

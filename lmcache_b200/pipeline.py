@@ -32,7 +32,8 @@ import numpy as np
 import torch
 
 from lmcache_b200 import _native as N
-from lmcache_b200.codec import CacheGenCodec, EncodedBatch, EncodeTicket, KvView, PinnedBuffer, parse_header, plane_offsets
+from lmcache_b200.codec import (CacheGenCodec, EncodedBatch, EncodeTicket, KvView, PinnedBuffer, lossless_raw_rows,
+                                parse_header)
 
 
 def wave_chunks_default() -> int:
@@ -273,16 +274,17 @@ def _d2h_stream(device: torch.device) -> torch.cuda.Stream:
 
 
 def land(slab, slot: WaveSlot, batch, blocks: Optional[list] = None,
-         dev_dst: Optional[Sequence[Optional[int]]] = None, parse: Callable = parse_header) -> List[HostContainer]:
+         dev_dst: Optional[Sequence[Optional[int]]] = None, codec=CacheGenCodec) -> List[HostContainer]:
     """Store-pipeline sink side: copy a finished wave's containers out of slot.dev into fresh blocks of `slab` (exactly
     their bytes, on the device's copy stream), wait for the copies, and parse every header.  Raises -- with every block
     freed -- when a copy fails or a container carries an encoder error.  `blocks`: blocks the caller allocated for the
     first len(blocks) containers (a bounded tier); only those are landed.  `dev_dst`: per container, a device address
-    that gets a copy of it as well (None: none), on the same stream and before the same wait.  `parse`: the header check
-    of the codec that wrote the wave (a lossless codec's for its containers).  A layer-wise store's slot (SegmentSlot)
-    lands through land_segments."""
+    that gets a copy of it as well (None: none), on the same stream and before the same wait.  `codec`: the codec (or
+    codec class) that wrote the wave: its header check and its plane-offset kernel (a lossless codec's for its
+    containers).  A layer-wise store's slot (SegmentSlot) lands through land_segments."""
     if isinstance(slot, SegmentSlot):
         return land_segments(slab, slot, batch, blocks, dev_dst)
+    parse = codec.parse_header
     dev = slot.dev.device
     cs = _d2h_stream(dev)
     if blocks is None:
@@ -292,9 +294,9 @@ def land(slab, slot: WaveSlot, batch, blocks: Optional[list] = None,
             try:
                 # plane offsets of the wave, read on the device before the bytes leave it: no host pass over the
                 # lengths sections (on the store worker such a pass made every e2e store ~2 ms slower, measured)
-                N.check(N.pylib().b200kv_plane_offsets_device(ctypes.c_void_p(slot.dev.data_ptr()), batch.stride,
-                                                            len(blocks), ctypes.c_void_p(slot.planes.dev_ptr),
-                                                            cs.cuda_stream), "plane_offsets_device")
+                N.check(getattr(N.pylib(), codec.plane_offsets_device)(
+                    ctypes.c_void_p(slot.dev.data_ptr()), batch.stride, len(blocks), ctypes.c_void_p(slot.planes.dev_ptr),
+                    cs.cuda_stream), codec.plane_offsets_device)
                 for j, (blk, size) in enumerate(zip(blocks, batch.sizes)):
                     N.check(N.lib().b200kv_copy_async(ctypes.c_void_p(blk.host_ptr),
                                                       ctypes.c_void_p(slot.dev.data_ptr() + j * batch.stride), size,
@@ -564,7 +566,7 @@ def read_container(codec: CacheGenCodec, blk, nbytes: int, latent: bool = False)
     try:
         hd = codec.parse_header(blk.view()[:nbytes])
         if codec.accepts(hd, latent):
-            return HostContainer(blk, nbytes, hd, plane_offsets(blk.view()[:nbytes]))   # on the reader's thread
+            return HostContainer(blk, nbytes, hd, codec.plane_offsets(blk.view()[:nbytes]))   # on the reader's thread
     except ValueError:
         pass
     blk.free()
@@ -886,21 +888,39 @@ def _batch_copy(dsts: np.ndarray, srcs: np.ndarray, sizes: np.ndarray, stream: t
                                             stream.cuda_stream), "copy_batch_async")
 
 
-def layer_copy_ranges(plane_offs: Sequence[Optional[np.ndarray]], nbytes: Sequence[int], L: int, ppl: int = 2):
+def layer_copy_ranges(plane_offs: Sequence[Optional[np.ndarray]], nbytes: Sequence[int], L: int, ppl: int = 2,
+                      raw: Optional[Sequence[Tuple[int, int]]] = None):
     """The copies of a layer-major upload of n containers, as offsets into each container: (fixed int64[n],
     start int64[L, ppl * n], size int64[L, ppl * n]).  Container j's first fixed[j] bytes go first (its fixed sections;
     all of it when it has no plane offsets); row l holds the key ranges (plane l) of containers 0..n-1, then their value
     ranges (plane L + l).  A latent KV (ppl = 1, version 4: plane l is layer l) has one range per container in row l.
-    Together they cover every container exactly once."""
+    Lossless containers (versions 5 and 6) pass `raw`, their (off_raw, bytes per plane) (codec.lossless_raw_rows): then
+    fixed[j] is off_raw, the part the decode plan reads, and a plane is two ranges, its raw rows and its streams, so the
+    rows are [L, 2 * ppl * n]: the raw ranges of every plane of the row, then the stream ranges.  Together they cover
+    every container exactly once."""
     n = len(nbytes)
     P = ppl * L
     po = np.stack([o if o is not None else np.zeros(P + 1, np.int64) for o in plane_offs]).astype(np.int64)
     split = np.array([o is not None for o in plane_offs])
-    fixed = np.where(split, po[:, 0], np.asarray(nbytes, dtype=np.int64)).astype(np.int64)
     start = np.ascontiguousarray(np.concatenate([po[:, k * L:(k + 1) * L] for k in range(ppl)]).T)     # [L, ppl * n]
     size = np.ascontiguousarray(np.concatenate([po[:, k * L + 1:(k + 1) * L + 1] - po[:, k * L:(k + 1) * L]
                                                 for k in range(ppl)]).T)
     assert start.shape == (L, ppl * n)
+    if raw is None:
+        fixed = np.where(split, po[:, 0], np.asarray(nbytes, dtype=np.int64)).astype(np.int64)
+        return fixed, start, size
+    off_raw = np.asarray([r[0] for r in raw], dtype=np.int64)
+    row = np.asarray([r[1] for r in raw], dtype=np.int64)
+    fixed = np.where(split, off_raw, np.asarray(nbytes, dtype=np.int64)).astype(np.int64)
+    pad = np.where(split, po[:, 0] - (off_raw + P * row), 0)     # alignment between the raw rows and the streams:
+    start[0, :n] -= pad                                          # copied with plane 0's streams, so that the ranges
+    size[0, :n] += pad                                           # cover the container exactly
+    planes = np.concatenate([np.arange(L)[:, None] + k * L for k in range(ppl)], axis=0)         # [ppl * L, 1]
+    rstart = (off_raw[None, :] + planes * row[None, :]).reshape(ppl, L, n).transpose(1, 0, 2).reshape(L, ppl * n)
+    rsize = np.tile(row, (L, ppl))
+    rsize = np.where(np.tile(split, ppl)[None, :], rsize, 0)
+    start = np.ascontiguousarray(np.concatenate([rstart, start], axis=1))
+    size = np.ascontiguousarray(np.concatenate([rsize, size], axis=1))
     return fixed, start, size
 
 
@@ -969,9 +989,13 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
             host = np.array([r.blk.host_ptr for r in up], dtype=np.uint64)
             dev = base + np.array(offs, dtype=np.uint64)
             ppl = dst.planes // L
-            fixed, lo, sz = layer_copy_ranges([r.planes for r in up], [r.nbytes for r in up], L, ppl)
-            lay_src = np.ascontiguousarray(np.tile(np.concatenate([host] * ppl), (L, 1)) + lo.astype(np.uint64))
-            lay_dst = np.ascontiguousarray(np.tile(np.concatenate([dev] * ppl), (L, 1)) + lo.astype(np.uint64))
+            raw = None
+            if (first.coder & 0xff) == N.CODER_LOSSLESS:      # a plane is its raw rows and its streams
+                raw = [lossless_raw_rows(r.L, r.H, r.D, r.ntokens, dst.latent) for r in up]
+            fixed, lo, sz = layer_copy_ranges([r.planes for r in up], [r.nbytes for r in up], L, ppl, raw)
+            k = lo.shape[1] // len(up)
+            lay_src = np.ascontiguousarray(np.tile(np.concatenate([host] * k), (L, 1)) + lo.astype(np.uint64))
+            lay_dst = np.ascontiguousarray(np.tile(np.concatenate([dev] * k), (L, 1)) + lo.astype(np.uint64))
         upload = LayerwiseUpload(n, L)
         dst_tok = [dst_tok0 + j * chunk_size for j in range(n)]
 

@@ -5,21 +5,29 @@ from lmcache_b200.storage_backend.abstract_backend import LMCBackendInterface
 
 def CreateStorageBackend(config: LMCacheEngineConfig, metadata: LMCacheEngineMetadata) -> LMCBackendInterface:
     local, remote = config.local_device, config.remote_url
+    # the compressed host tier: page-locked containers, CacheGen or lossless; "cuda" keeps raw blobs whatever the serde
+    compressed_host = local == "cpu" and config.local_serde in ("cachegen", "lossless")
     if config.local_capacity_bytes is not None:
-        # only the CacheGen tiers evict: the raw tiers keep views of one shared buffer per store, so evicting one view
+        # only the container tiers evict: the raw tiers keep views of one shared buffer per store, so evicting one view
         # would free nothing; a remote-only configuration has no local tier
         if local is None:
             raise ValueError("local_capacity_bytes needs a local tier; a remote-only configuration has none")
-        if local in ("cpu", "cuda") and not (local == "cpu" and config.local_serde == "cachegen"):
+        if local in ("cpu", "cuda") and not compressed_host:
             raise ValueError(f"local_capacity_bytes is honoured by the CacheGen tiers only (local_device='cpu' with "
-                             f"local_serde='cachegen', or a directory), not by local_device={local!r}")
+                             f"local_serde='cachegen', or a directory), and by their lossless forms "
+                             f"(local_serde='lossless'), not by local_device={local!r}")
     if config.device_cache_bytes is not None:
-        # the device level keeps copies of CacheGen containers: only the CacheGen local tiers have any
+        # the device level keeps copies of containers: only the container local tiers have any
         if local is None:
             raise ValueError("device_cache_bytes needs a local CacheGen tier; a remote-only configuration has none")
-        if local in ("cpu", "cuda") and not (local == "cpu" and config.local_serde == "cachegen"):
+        if local in ("cpu", "cuda") and not compressed_host:
             raise ValueError(f"device_cache_bytes is honoured by the CacheGen tiers only (local_device='cpu' with "
-                             f"local_serde='cachegen', or a directory), not by local_device={local!r}")
+                             f"local_serde='cachegen', or a directory), and by their lossless forms "
+                             f"(local_serde='lossless'), not by local_device={local!r}")
+    if config.local_serde == "lossless" and local not in (None, "cuda"):
+        # the compressed host tier or the disk tier holds lossless containers: one container per chunk
+        from lmcache_b200.storage_backend.serde.lossless import _check_chunk_size
+        _check_chunk_size(config)
     if config.reshard_world_sizes is not None:
         # another layout's chunks exist only on a shared remote tier, and only CacheGen containers can be decoded a
         # window of heads at a time
@@ -30,13 +38,14 @@ def CreateStorageBackend(config: LMCacheEngineConfig, metadata: LMCacheEngineMet
         from lmcache_b200.storage_backend.remote_backend import LMCPipelinedRemoteBackend, LMCRemoteBackend
         return (LMCPipelinedRemoteBackend if config.pipelined_backend else LMCRemoteBackend)(config, metadata)
     if isinstance(local, str) and remote is None:
-        if local == "cpu" and config.local_serde == "cachegen":
+        if compressed_host:
             from lmcache_b200.storage_backend.local_backend import LMCLocalCompressedBackend
             return LMCLocalCompressedBackend(config, metadata)
         if local in ("cpu", "cuda"):
             from lmcache_b200.storage_backend.local_backend import LMCLocalBackend
             return LMCLocalBackend(config, metadata)
-        # a directory: the disk tier (LMCLocalDiskBackend, local_backend.py:163-310), here with CacheGen containers
+        # a directory: the disk tier (LMCLocalDiskBackend, local_backend.py:163-310), here with CacheGen containers, or
+        # lossless ones with local_serde="lossless"
         from lmcache_b200.storage_backend.local_backend import LMCLocalDiskBackend
         return LMCLocalDiskBackend(config, metadata)
     if isinstance(local, str) and isinstance(remote, str):

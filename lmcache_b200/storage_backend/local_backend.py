@@ -332,11 +332,17 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
     With config.device_cache_bytes the tier has a device level (lmcache_b200/device_cache.py): containers are copied
     into one device pool as they land and as retrieves upload them, and a retrieve decodes the resident ones in place
     (pipeline.DeviceLevel).  The level is inclusive -- a device copy leaves with its entry -- and filling it never
-    waits: what does not find room at once is not cached."""
+    waits: what does not find room at once is not cached.
+
+    With config.local_serde="lossless" the containers are lossless ones (versions 5 and 6, codec.LosslessCodec), with
+    every feature above: a retrieve gives back the stored bits in the stored dtype, and a chunk whose dtype or kind
+    differs from the destination's is a miss."""
+
+    lossless = False                          # the tier keeps lossless containers (set from config.local_serde)
 
     def __init__(self, config: LMCacheEngineConfig, metadata):
         super().__init__()
-        from lmcache_b200.codec import engine_codec
+        from lmcache_b200.codec import LosslessCodec, engine_codec
         from lmcache_b200.eviction import PrefixLRU
         from lmcache_b200.pipeline import DeferredFree, EncodePipeline, UploadRing
         N.require_cuda()
@@ -347,8 +353,9 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         # the engine's KV is latent (metadata.use_mla): its containers are version 4, and only those are its chunks
         self.latent = bool(getattr(metadata, "use_mla", False))
         # ValueError for models outside the bin table (without config.cachegen_config), and for settings that
-        # config.cachegen_config rules out
-        self.codec = engine_codec(config, metadata.model_name)
+        # config.cachegen_config rules out.  local_serde="lossless": lossless containers, in the stored dtype
+        self.lossless = config.local_serde == "lossless"
+        self.codec = LosslessCodec() if self.lossless else engine_codec(config, metadata.model_name)
         self.capacity: Optional[int] = config.local_capacity_bytes
         self.slab = self._new_slab()
         self._order = PrefixLRU()             # eviction order of a bounded tier, keyed like self.dict
@@ -383,11 +390,11 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         try:
             blocks = None if self.capacity is None else self._make_room(batch.sizes, entries)
             if self._dcache is None:
-                recs = land(self.slab, slot, batch, blocks) if blocks is None or blocks else []
+                recs = land(self.slab, slot, batch, blocks, codec=self.codec) if blocks is None or blocks else []
             else:
                 dblocks = self._fill_blocks(batch.sizes[:len(batch.sizes) if blocks is None else len(blocks)], slot,
                                             entries[0].store)
-                recs = land(self.slab, slot, batch, blocks, self._fill_ptrs(dblocks)) if dblocks else []
+                recs = land(self.slab, slot, batch, blocks, self._fill_ptrs(dblocks), self.codec) if dblocks else []
             for e, rec in zip(entries, recs):
                 e.rec = rec
             if dblocks:
@@ -556,13 +563,26 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         """(L, H, D, output dtype) of the stored chunks, read from a container header (no decode).  None for a container
         of the other kind (version 4 for a (K, V) engine, or the reverse)."""
         e = self._ready_entry(key)
-        if e is None or (e.rec.coder == N.CODER_LATENT) != self.latent:
+        if e is None or bool(e.rec.coder & N.KV_LATENT) != self.latent:
             return None
-        return e.rec.L, e.rec.H, e.rec.D, self.out_dtype()
+        return e.rec.L, e.rec.H, e.rec.D, self._dtype_of(e.rec)
 
-    def out_dtype(self) -> torch.dtype:
-        # the reference's decoder casts by format, ignoring metadata.dtype (cachegen_decoder.py:189-200)
+    def out_dtype(self) -> Optional[torch.dtype]:
+        """The dtype a retrieve decodes into: by format for CacheGen containers (the reference's decoder casts by format,
+        ignoring metadata.dtype, cachegen_decoder.py:189-200); None for lossless ones, which decode into the dtype they
+        were stored in (peek_geometry says which)."""
+        if self.lossless:
+            return None
         return torch.bfloat16 if self.fmt == "vllm" else torch.float16
+
+    def _dtype_of(self, rec) -> torch.dtype:
+        from lmcache_b200.codec import dtype_of_code
+        return self.out_dtype() or dtype_of_code(rec.max_dtype)
+
+    @property
+    def layerwise_max_tokens(self) -> int:
+        """the largest chunk a layer-major retrieve takes: one group per container"""
+        return self.codec.layerwise_max_tokens
 
     # ------------------------------------------------------------------ retrieve
     def supports_kv_view(self) -> bool:
@@ -726,8 +746,8 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         if e is None:
             return None
         r = e.rec
-        out = torch.empty(KvView.blob_shape(self.fmt, r.L, r.H, r.D, r.ntokens, r.coder == N.CODER_LATENT),
-                          dtype=self.out_dtype(),
+        out = torch.empty(KvView.blob_shape(self.fmt, r.L, r.H, r.D, r.ntokens, bool(r.coder & N.KV_LATENT)),
+                          dtype=self._dtype_of(r),
                           device=torch.device("cuda", torch.cuda.current_device()))
         if self.get_kv_into([key], KvView.from_blob(out, self.fmt), 0, r.ntokens) != 1:
             return None
@@ -812,8 +832,10 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
     def _rebuild_index(self) -> int:
         import os
 
-        from lmcache_b200.codec import parse_header
+        from lmcache_b200.codec import parse_header, parse_lossless_header
         from lmcache_b200.pipeline import HostContainer
+        # the tier's own family only: a CacheGen tier indexes versions 1 to 4, a lossless one 5 and 6
+        parse = parse_lossless_header if self.lossless else parse_header
         found = []
         for name in os.listdir(self.path):
             if not name.endswith(self.SUFFIX):
@@ -823,11 +845,11 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
                 st = os.stat(full)
                 size = st.st_size
                 with open(full, "rb") as f:
-                    hd = parse_header(f.read(N.HEADER_BYTES + N.MAX_PLANES), size)
-                if int(hd.total_bytes) != size or (hd.version == 4) != self.latent:
-                    continue                     # version 4 holds a latent KV: a container of a latent engine only
+                    hd = parse(f.read(N.HEADER_BYTES + N.MAX_PLANES), size)
+                if int(hd.total_bytes) != size or bool(N.coder_of_version(hd.version) & N.KV_LATENT) != self.latent:
+                    continue                     # versions 4 and 6 hold a latent KV: containers of a latent engine only
             except (OSError, ValueError):
-                continue                         # damaged / foreign file: not part of the cache
+                continue                         # damaged / foreign file (the other family's too): left as it is
             # "/" in a model name was written as "-": the key of a lookup goes through the same rule, so index by path
             e = _CEntry()
             e.path, e.rec = full, HostContainer(None, size, hd)
@@ -888,10 +910,10 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
         dblocks = None
         try:
             if self._dcache is None:
-                recs = land(self.slab, slot, batch)      # containers -> page-locked blocks, headers parsed
+                recs = land(self.slab, slot, batch, codec=self.codec)   # containers -> page-locked blocks, headers parsed
             else:
                 dblocks = self._fill_blocks(batch.sizes, slot, entries[0].store)
-                recs = land(self.slab, slot, batch, None, self._fill_ptrs(dblocks))
+                recs = land(self.slab, slot, batch, None, self._fill_ptrs(dblocks), self.codec)
         except BaseException as err:     # noqa: BLE001
             for e in entries:
                 e.error = err

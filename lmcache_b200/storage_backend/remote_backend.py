@@ -199,7 +199,7 @@ class LMCRemoteBackend(LMCBackendInterface):
         """store worker: one wave's containers -> page-locked slab (land() raises on a nonzero encoder status: nothing
         corrupt leaves the host), then k-way send"""
         from lmcache_b200.pipeline import land
-        blocks = [rec.blk for rec in land(self._host_slab(), slot, batch, parse=self.serializer.codec.parse_header)]
+        blocks = [rec.blk for rec in land(self._host_slab(), slot, batch, codec=self.serializer.codec)]
         try:
             def send(key, blk):
                 self._conn().set(self._combine_key(key), blk.view())
