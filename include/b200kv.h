@@ -42,7 +42,10 @@ extern "C" {
                                     *    b200kv_lossless_layout / b200kv_lossless_workspace_bytes / b200kv_lossless_encode /
                                     *    b200kv_lossless_decode (container versions 5 and 6), b200kv_lossless_plane_offsets /
                                     *    b200kv_lossless_plane_offsets_device / b200kv_lossless_decode_plan /
-                                    *    b200kv_lossless_decode_layers (b200kv_lossless_decode_plan_t).
+                                    *    b200kv_lossless_decode_layers (b200kv_lossless_decode_plan_t),
+                                    *    b200kv_lossless_encode_layers_workspace_bytes /
+                                    *    b200kv_lossless_encode_layers_plan / b200kv_lossless_encode_layers /
+                                    *    b200kv_lossless_encode_layers_finish (b200kv_lossless_encode_plan_t).
                                     *    B200KV_MAX_PLANES went from 128 to 256 (models of up to 128 layers): the row
                                     *    width of b200kv_plane_offsets_device, B200KV_MAX_PLANES + 1, and the size of
                                     *    b200kv_encode_plan_t, 256 -> 512 words, changed with it; a caller takes them
@@ -417,6 +420,57 @@ int b200kv_lossless_decode_plan(const void* containers, int64_t containers_bytes
                                 void* stream);
 int b200kv_lossless_decode_layers(const b200kv_lossless_decode_plan_t* plan, int32_t layer_begin, int32_t layer_end,
                                   void* stream);
+
+/*
+ * The lossless encode in three steps, as b200kv_encode_layers_plan / _layers / _finish for the CacheGen containers: a
+ * layer is encoded as soon as the forward pass has written it.  Versions 5 and 6, chunk_tokens <= 4096.
+ *
+ * b200kv_lossless_encode_layers_plan takes b200kv_lossless_encode's KV and chunking arguments and makes its checks,
+ * zeroes the error words, payload totals and the arena cursor in `workspace` and the n_chunks fixed images at
+ * fixed_out + j * fixed_stride, and records its decisions in *plan (caller-owned host memory).  A fixed image is
+ * [0, off_raw) of the container (header, frequency rows, lengths): fixed_stride >= off_raw, 16-byte aligned.  The KV is
+ * not read yet.  max_layers: the most layers one b200kv_lossless_encode_layers call may take (the workspace holds one
+ * call's scratch and raw rows: b200kv_lossless_encode_layers_workspace_bytes).  arena: DEVICE, 16-byte aligned.
+ *
+ * b200kv_lossless_encode_layers enqueues, for layers [layer_begin, layer_end) -- planes layer_begin.. and L +
+ * layer_begin.., or planes layer_begin.. alone for version 6 -- of every chunk: the histograms and frequency rows
+ * (into the fixed image), the coding (lengths into the fixed image), and one segment per chunk in the device arena of
+ * arena_bytes bytes:
+ *     [the call's planes' raw rows, t * C bytes each, in plane order; in the call that holds the last plane followed by
+ *      the container's zero bytes up to off_payload; zeros to a 16-byte boundary] [the call's planes' streams, in order]
+ * Segments are placed by the rule of b200kv_encode_layers (16-byte aligned at a device-held cursor in (call, chunk)
+ * order, with a reserve for the layers still to come; the chunks that fit are always a prefix).  Row (j, p) of
+ * seg_sizes_out (DEVICE or mapped-host int64[n_chunks][P][3], P = 2L or L) gets (arena offset of plane p's raw rows,
+ * arena offset of its streams, its stream bytes); the offsets are -1 for a chunk that failed, and a chunk that fails in a
+ * later call than its first keeps the rows of the calls that had placed it, as in b200kv_encode_layers.  Read the rows of
+ * chunks whose sizes_out is nonzero only.  Each layer is encoded once.
+ *
+ * b200kv_lossless_encode_layers_finish writes each chunk's header into its fixed image from the stream bytes of every
+ * call, and sizes_out[j] (total_bytes, or 0 when header.status is nonzero: bit 16 = did not fit the arena, bit 0 = a
+ * stream outgrew its bound), and fails unless every layer was encoded.
+ *
+ * For every chunk that did not fail, fixed image [0, off_raw) || for p = 0..P-1 the raw bytes at row (j, p)[0]
+ * (t * C of them; for p = P - 1 up to off_payload) || for p = 0..P-1 the row (j, p)[2] stream bytes at row (j, p)[1]
+ * is byte for byte the container b200kv_lossless_encode writes.  Every refusal returns < 0 and enqueues nothing: a layer
+ * range out of bounds or encoded before, finish before every layer was encoded, a plan not made by
+ * b200kv_lossless_encode_layers_plan, a misaligned arena or fixed image, a too small fixed stride or workspace, and the
+ * shapes b200kv_lossless_encode refuses.  The KV, arena, images, outputs and workspace must stay valid until the finish
+ * step has run on the device.
+ */
+typedef struct b200kv_lossless_encode_plan_t {
+    uint64_t opaque[512];      /* the encode kernels' parameter block and a 128-bit set of the layers encoded */
+} b200kv_lossless_encode_plan_t;
+
+int64_t b200kv_lossless_encode_layers_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t chunk_tokens,
+                                                      int32_t n_chunks, int32_t latent, int32_t max_layers);
+int b200kv_lossless_encode_layers_plan(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_chunks,
+                                       int32_t chunk_tokens, int32_t last_chunk_tokens, void* arena, int64_t arena_bytes,
+                                       void* fixed_out, int64_t fixed_stride, int64_t* seg_sizes_out,
+                                       uint64_t* sizes_out, int32_t max_layers, void* workspace, int64_t workspace_bytes,
+                                       b200kv_lossless_encode_plan_t* plan, void* stream);
+int b200kv_lossless_encode_layers(b200kv_lossless_encode_plan_t* plan, int32_t layer_begin, int32_t layer_end,
+                                  void* stream);
+int b200kv_lossless_encode_layers_finish(const b200kv_lossless_encode_plan_t* plan, void* stream);
 
 /*
  * Token-id prefix hash.  Replaces LMCacheEngine._chunk_tokens/_hash/_prefix_hash

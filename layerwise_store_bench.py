@@ -2,6 +2,7 @@
 """layerwise_store_bench.py -- what a layer-by-layer store costs and hides during a prefill step, on one GPU.
 
   python layerwise_store_bench.py [--steps K] [--warmup W] [--tokens 8192,65536] [--ffn F]
+                                  [--local-serde cachegen|lossless] [--dtype bf16|fp16]
 
 Model of a prefill step: L = 32 layers, 32 KV heads x 128 dims, bf16, chunk 256, a paged KV cache (block 16, scrambled
 slot mapping).  Per layer the forward stream runs a stand-in for the layer's compute -- one [T, 4096] x [4096, F] bf16
@@ -19,7 +20,9 @@ Per leg, from CUDA events on the forward stream (start = before layer 0's GEMM):
 A forward without any store is timed too (bare_fwd_ms), so the store's slowdown of the forward is fwd_ms - bare_fwd_ms.
 Containers of both legs are compared through digests of their bytes after the timed steps (same tokens, same KV), over
 the chunks both legs hold; chunks_landed says how many each leg holds (a layer-wise store keeps the prefix of chunks that
-fit its device arena, LMCACHE_B200_LAYERWISE_STORE_MB).  Prints one JSON line.  Writes nothing into the tree.
+fit its device arena, LMCACHE_B200_LAYERWISE_STORE_MB).  --local-serde lossless stores lossless containers (versions 5
+and 6) instead of CacheGen ones, --dtype fp16 keeps an fp16 KV cache; the JSON line names them when they are not the
+defaults.  Prints one JSON line.  Writes nothing into the tree.
 """
 import argparse
 import hashlib
@@ -53,7 +56,7 @@ def _container_digests(engine, keys):
     return out
 
 
-def run(T, steps, warmup, ffn):
+def run(T, steps, warmup, ffn, serde="cachegen", dt="bf16"):
     import torch
 
     import bench
@@ -61,20 +64,21 @@ def run(T, steps, warmup, ffn):
     from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
     L, H, D, cs, bs = 32, 32, 128, 256, 16
     dev = torch.device("cuda", 0)
-    base = bench.synth_kv_torch(min(T, 8192), dev, seed=0)          # SURVEY 8d data, as bench.py's headline
+    dtype = torch.float16 if dt == "fp16" else torch.bfloat16
+    base = bench.synth_kv_torch(min(T, 8192), dev, seed=0).to(dtype)  # SURVEY 8d data, as bench.py's headline
     reps = -(-T // base.shape[2])
     nblk = T // bs + 8
     try:
-        caches = [(torch.zeros((nblk, bs, H, D), dtype=torch.bfloat16, device=dev),
-                   torch.zeros((nblk, bs, H, D), dtype=torch.bfloat16, device=dev)) for _ in range(L)]
+        caches = [(torch.zeros((nblk, bs, H, D), dtype=dtype, device=dev),
+                   torch.zeros((nblk, bs, H, D), dtype=dtype, device=dev)) for _ in range(L)]
         x = torch.randn((T, 4096), dtype=torch.bfloat16, device=dev)
         w = torch.randn((4096, ffn), dtype=torch.bfloat16, device=dev) * 0.01
     except torch.cuda.OutOfMemoryError:
         return {"tokens": T, "skipped": "does not fit on the card"}
     slots = torch.randperm(nblk * bs, device=dev)[:T]
-    meta = LMCacheEngineMetadata("lmsys/longchat-7b-16k", 1, 0, "vllm", "bfloat16")
+    meta = LMCacheEngineMetadata("lmsys/longchat-7b-16k", 1, 0, "vllm", "float16" if dt == "fp16" else "bfloat16")
     # a fresh sequence per step: the tier is bounded (8 GiB), so older sequences are evicted
-    eng = LMCacheEngine(LMCacheEngineConfig.from_legacy(chunk_size=cs, backend="cpu", local_serde="cachegen",
+    eng = LMCacheEngine(LMCacheEngineConfig.from_legacy(chunk_size=cs, backend="cpu", local_serde=serde,
                                                         local_capacity_bytes=8 << 30), meta)
     fwd = torch.cuda.current_stream()
 
@@ -132,7 +136,7 @@ def run(T, steps, warmup, ffn):
     # equality of the legs: the same tokens and KV stored by both, compared by container digests
     digests = []
     for m in ("store_paged", "layerwise"):
-        e2 = LMCacheEngine(LMCacheEngineConfig.from_legacy(chunk_size=cs, backend="cpu", local_serde="cachegen"), meta)
+        e2 = LMCacheEngine(LMCacheEngineConfig.from_legacy(chunk_size=cs, backend="cpu", local_serde=serde), meta)
         eng, keep = e2, eng
         tokens = torch.arange(T, device=dev) + 10 ** 7
         if m == "store_paged":
@@ -165,15 +169,19 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--tokens", default="8192,65536")
     ap.add_argument("--ffn", type=int, default=14336)
+    ap.add_argument("--local-serde", choices=("cachegen", "lossless"), default="cachegen")
+    ap.add_argument("--dtype", choices=("bf16", "fp16"), default="bf16")
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("layerwise_store_bench.py needs a CUDA device")
     torch.cuda.set_device(0)
-    results = [run(int(t), a.steps, a.warmup, a.ffn) for t in a.tokens.split(",")]
-    print(json.dumps({"bench": "layerwise_store", "gpu": _gpu_info(), "ffn": a.ffn,
-                      "arena_budget_mb": int(os.environ.get("LMCACHE_B200_LAYERWISE_STORE_MB", "1024")),
-                      "results": results}))
+    results = [run(int(t), a.steps, a.warmup, a.ffn, a.local_serde, a.dtype) for t in a.tokens.split(",")]
+    out = {"bench": "layerwise_store", "gpu": _gpu_info(), "ffn": a.ffn}
+    if a.local_serde != "cachegen" or a.dtype != "bf16":
+        out.update(local_serde=a.local_serde, dtype=a.dtype)
+    out.update(arena_budget_mb=int(os.environ.get("LMCACHE_B200_LAYERWISE_STORE_MB", "1024")), results=results)
+    print(json.dumps(out))
 
 
 if __name__ == "__main__":

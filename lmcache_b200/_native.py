@@ -92,6 +92,11 @@ class LosslessDecodePlan(ctypes.Structure):
     _fields_ = [("opaque", ctypes.c_uint64 * 512)]
 
 
+class LosslessEncodePlan(ctypes.Structure):
+    """struct b200kv_lossless_encode_plan_t (opaque, filled by b200kv_lossless_encode_layers_plan)"""
+    _fields_ = [("opaque", ctypes.c_uint64 * 512)]
+
+
 assert ctypes.sizeof(Header) == HEADER_BYTES
 
 # name -> (restype, argtypes); every symbol include/b200kv.h declares
@@ -132,6 +137,12 @@ SIGNATURES = {
     "b200kv_lossless_decode_plan": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, ctypes.POINTER(KvDesc),
                                              c_vp, c_vp, c_i64, ctypes.POINTER(LosslessDecodePlan), c_vp]),
     "b200kv_lossless_decode_layers": (c_i32, [ctypes.POINTER(LosslessDecodePlan), c_i32, c_i32, c_vp]),
+    "b200kv_lossless_encode_layers_workspace_bytes": (c_i64, [c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
+    "b200kv_lossless_encode_layers_plan": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp,
+                                                   c_i64, c_vp, c_vp, c_i32, c_vp, c_i64,
+                                                   ctypes.POINTER(LosslessEncodePlan), c_vp]),
+    "b200kv_lossless_encode_layers": (c_i32, [ctypes.POINTER(LosslessEncodePlan), c_i32, c_i32, c_vp]),
+    "b200kv_lossless_encode_layers_finish": (c_i32, [ctypes.POINTER(LosslessEncodePlan), c_vp]),
     "b200kv_sha256_chain": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp]),
     "b200kv_sha256_chain_ready": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, ctypes.c_uint32, c_vp]),
     "b200kv_pack_chunks": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp]),

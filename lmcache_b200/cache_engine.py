@@ -189,9 +189,10 @@ class LayerwiseStore:
     """What store_layerwise / store_paged_layerwise return: a store whose KV is handed over one layer at a time, as
     vLLM's KV connector does with save_kv_layer after each attention layer and wait_for_save at the end of the forward
     pass.  save_layer(l, stream) says that layer l is written in `stream` order; finish(stream) completes the store.
-    Neither waits on the host.  On the compressed host and disk tiers each layer is encoded on a side stream as soon as
-    it is saved (pipeline.LayerwiseEncode); elsewhere save_layer only records the layer and finish() runs the ordinary
-    store.  A handle dropped without finish() stores nothing and gives its device scratch back."""
+    Neither waits on the host, except finish() on a lossless disk tier, which returns once the files are written, as
+    the store() it replaced did (the tier's layerwise_store_blocking).  On the compressed host and disk tiers each layer
+    is encoded on a side stream as soon as it is saved (pipeline.LayerwiseEncode); elsewhere save_layer only records the
+    layer and finish() runs the ordinary store.  A handle dropped without finish() stores nothing and gives its device scratch back."""
 
     def __init__(self, num_layers: int, enc, on_finish: Callable):
         self.num_layers = num_layers
@@ -216,8 +217,8 @@ class LayerwiseStore:
     def finish(self, stream: Optional[torch.cuda.Stream] = None) -> None:
         """Complete the store: `stream` (default: the current stream) waits for the encode's last read of the KV, so
         the caller may overwrite the cache in that stream's order; the containers land on the tier's worker thread, and
-        a later retrieve of these keys waits for them.  ValueError, and nothing is stored, when a layer was never
-        saved."""
+        a later retrieve of these keys waits for them (a lossless disk tier waits here for its files to be written).
+        ValueError, and nothing is stored, when a layer was never saved."""
         if self._finished:
             raise ValueError("finish() was called before")
         self._finished = True
@@ -753,9 +754,10 @@ class LMCacheEngine:
     # ------------------------------------------------------------------ layer-wise store
     def _layerwise_store_ok(self, dtype: torch.dtype) -> bool:
         """Can this store be encoded layer by layer?  The compressed host and disk tiers can, for 16-bit KV and chunks of
-        at most 256 tokens (version-3 containers); raw, remote and hybrid tiers cannot."""
+        at most the tier's layerwise_max_tokens (256 for CacheGen's version-3 containers, 4096 for lossless ones); raw,
+        remote and hybrid tiers cannot."""
         return (getattr(self.engine_, "begin_layerwise_store", None) is not None and self._fast_path() and
-                self.chunk_size <= N.GROUP_TOKENS and dtype in (torch.bfloat16, torch.float16))
+                self.chunk_size <= self.engine_.layerwise_max_tokens and dtype in (torch.bfloat16, torch.float16))
 
     def _begin_layerwise(self, tokens, view_fn, fmt: str, num_layers: int, skip_existing: bool,
                          fallback: Callable) -> LayerwiseStore:
@@ -774,9 +776,11 @@ class LMCacheEngine:
                 return LayerwiseStore(num_layers, None, fallback)
 
         def publish(stream, enc):
-            # enc is None when the scan matched every chunk, or when the handle was closed: nothing to put
+            # enc is None when the scan matched every chunk, or when the handle was closed: nothing to put.  The put
+            # waits for the landing on a tier that asks for it (a lossless disk tier: layerwise_store_blocking)
+            blocking = bool(getattr(self.engine_, "layerwise_store_blocking", False))
             put = None if enc is None else lambda keys, tok_begin: self.engine_.put_kv_chunks(
-                keys, None, tok_begin, self.chunk_size, blocking=False, encoded=enc)
+                keys, None, tok_begin, self.chunk_size, blocking=blocking, encoded=enc)
             self._store_put(chunk_hashes, start, fmt, put)
         return LayerwiseStore(num_layers, enc, publish)
 

@@ -10,7 +10,7 @@ import contextlib
 import ctypes
 import threading
 from dataclasses import dataclass
-from typing import List, Optional, Sequence, Tuple, Union
+from typing import List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -394,6 +394,15 @@ def check_header(hd: "N.Header", nb: Optional[Sequence[int]] = None) -> None:
         raise ValueError("B2KV header: payload_bytes impossible for this shape")
 
 
+class SegmentLayout(NamedTuple):
+    """How a layer-wise store assembles a container of some number of tokens (pipeline.segment_copy_ranges): bytes
+    [0, head) come from the chunk's fixed image, the streams start at `payload`, and -- lossless containers only -- plane
+    p's raw rows lie at head + p * raw_plane, raw_plane bytes each (the last plane's range runs up to `payload`)."""
+    head: int
+    payload: int
+    raw_plane: int = 0
+
+
 @dataclass
 class EncodedBatch:
     """Device-resident result of one encode call: n containers at `stride` in `buf`."""
@@ -656,6 +665,39 @@ class CacheGenCodec(_ContainerIO):
             hdr = N.HDR_MAX if self.coder_for(chunk_tokens, latent) & 0xff == N.CODER_RANS_COMPACT else 0
             return (lo.fixed_bytes + (1 if latent else 2) * L * H * D * (chunk_tokens + 4 + hdr) + 16 + 15) & ~15
         return lo.max_total_bytes
+
+    # ------------------------------------------------------------------ layer-wise encode (pipeline.LayerwiseEncode)
+    # b200kv_encode_layers_plan / _layers / _finish, version-3 (version-4) containers; a segment row per (chunk, plane)
+    # is (arena offset, bytes) of the plane's streams
+    seg_row = 2
+    layer_plan_type = N.EncodePlan
+    encode_layers_fn = "b200kv_encode_layers"
+    encode_layers_finish_fn = "b200kv_encode_layers_finish"
+
+    def segment_layout(self, L: int, H: int, D: int, ntokens: int, latent: bool = False) -> SegmentLayout:
+        lo = N.container_layout(L, H, D, ntokens, N.CODER_LATENT if latent else N.CODER_RANS_COMPACT)
+        return SegmentLayout(int(lo.off_payload), int(lo.off_payload))
+
+    def layerwise_chunk_bound(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> int:
+        """arena bytes a chunk can take: its worst-case payload and the alignment of one segment per layer"""
+        lo = N.container_layout(L, H, D, chunk_tokens, N.CODER_LATENT if latent else N.CODER_RANS_COMPACT)
+        return int(lo.max_total_bytes - lo.off_payload) + 16 * L
+
+    def layerwise_workspace_bytes(self, L: int, H: int, D: int, chunk_tokens: int, n_chunks: int,
+                                  latent: bool = False) -> int:
+        return N.check(N.lib().b200kv_encode_layers_workspace_bytes(L, H, D, chunk_tokens, n_chunks, 1),
+                       "encode_layers_workspace")
+
+    def encode_layers_plan(self, view: KvView, tok_begin: int, n: int, chunk_tokens: int, last: int, slot, plan,
+                           stream: torch.cuda.Stream) -> None:
+        """b200kv_encode_layers_plan into a pipeline.SegmentSlot, one layer per call"""
+        if view.L > self.nlayers:
+            raise ValueError(f"KV has {view.L} layers but the bin table of this model has {self.nlayers}")
+        N.check(N.lib().b200kv_encode_layers_plan(ctypes.byref(view.desc), tok_begin, n, chunk_tokens, last, self._kb,
+                                                  self._vb, N.CODER_RANS_COMPACT, slot.arena.data_ptr(), slot.arena_bytes,
+                                                  slot.fixed.data_ptr(), slot.fixed_stride, slot.seg.dev_ptr,
+                                                  slot.sizes.dev_ptr, 1, slot.ws.data_ptr(), slot.ws.numel(),
+                                                  ctypes.byref(plan), stream.cuda_stream), "encode_layers_plan")
 
     # ------------------------------------------------------------------ encode
     def encode_async(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int,
@@ -998,6 +1040,39 @@ class LosslessCodec(_ContainerIO):
     def max_container_bytes(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> int:
         """Upper bound of a container this codec can decode (there is one lossless layout per shape)."""
         return self.out_stride(L, H, D, chunk_tokens, latent)
+
+    # ------------------------------------------------------------------ layer-wise encode (pipeline.LayerwiseEncode)
+    # b200kv_lossless_encode_layers_plan / _layers / _finish; a segment row per (chunk, plane) is (arena offset of the
+    # plane's raw rows, arena offset of its streams, stream bytes)
+    seg_row = 3
+    layer_plan_type = N.LosslessEncodePlan
+    encode_layers_fn = "b200kv_lossless_encode_layers"
+    encode_layers_finish_fn = "b200kv_lossless_encode_layers_finish"
+
+    def segment_layout(self, L: int, H: int, D: int, ntokens: int, latent: bool = False) -> SegmentLayout:
+        lo = self.layout(L, H, D, ntokens, latent)
+        return SegmentLayout(int(lo.off_raw), int(lo.off_payload), int(ntokens) * H * D)
+
+    def layerwise_chunk_bound(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> int:
+        """arena bytes a chunk can take: everything of its worst case after the fixed image, and per layer the alignment
+        of one segment and of the streams inside it"""
+        lo = self.layout(L, H, D, chunk_tokens, latent)
+        return int(lo.max_total_bytes - lo.off_raw) + 32 * L
+
+    def layerwise_workspace_bytes(self, L: int, H: int, D: int, chunk_tokens: int, n_chunks: int,
+                                  latent: bool = False) -> int:
+        return N.check(N.lib().b200kv_lossless_encode_layers_workspace_bytes(L, H, D, chunk_tokens, n_chunks,
+                                                                             int(latent), 1),
+                       "lossless_encode_layers_workspace")
+
+    def encode_layers_plan(self, view: KvView, tok_begin: int, n: int, chunk_tokens: int, last: int, slot, plan,
+                           stream: torch.cuda.Stream) -> None:
+        """b200kv_lossless_encode_layers_plan into a pipeline.SegmentSlot, one layer per call"""
+        N.check(N.lib().b200kv_lossless_encode_layers_plan(ctypes.byref(view.desc), tok_begin, n, chunk_tokens, last,
+                                                           slot.arena.data_ptr(), slot.arena_bytes, slot.fixed.data_ptr(),
+                                                           slot.fixed_stride, slot.seg.dev_ptr, slot.sizes.dev_ptr, 1,
+                                                           slot.ws.data_ptr(), slot.ws.numel(), ctypes.byref(plan),
+                                                           stream.cuda_stream), "lossless_encode_layers_plan")
 
     # ------------------------------------------------------------------ encode
     def encode_async(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int,

@@ -968,59 +968,13 @@ __global__ void __launch_bounds__(CT, 12) compact_kernel(EncParams P) {
 
 // ------------------------------------------------------------------------------------------ arena placement
 // b200kv_encode_layers: after enc_scan_kernel, give each chunk's bytes of this call (its K planes, then its V planes)
-// room in the arena, in chunk order from the device-held cursor, 16-byte aligned.  Chunk j fits iff every chunk before
-// it fits and the arena still holds, after chunks 0..j of this call, the layers still to come for them at this call's
-// size per layer (layers_left / nlay times this call's bytes of chunks 0..j): without that reserve the first calls would
-// fill the arena with every chunk and a later call would find no room even for chunk 0.  The first chunk that does not
-// fit is remembered (fail_from), so the chunks that fit are always a prefix, over this call and every later one.  Then
-// one (offset, bytes) row per plane.  One CTA: a few hundred chunks at most, and it runs once per call.
+// room in the arena by the arena rule (arena_place, common.cuh), then one (offset, bytes) row per plane.  One CTA: a few
+// hundred chunks at most, and it runs once per call.
 __global__ void __launch_bounds__(1024) place_kernel(EncParams P) {
-    __shared__ unsigned long long s_w[32];
-    __shared__ unsigned long long s_carry, s_end;
-    __shared__ unsigned int s_fail;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    if (tid == 0) {
-        s_carry = s_end = *P.cursor;
-        s_fail = *P.fail_from;
-    }
-    __syncthreads();
-    const unsigned long long start = s_carry;
-    for (int b0 = 0; b0 < P.n_chunks; b0 += 1024) {
-        const int i = b0 + tid;
-        const unsigned long long v = i < P.n_chunks ? (P.totals[i] + 15ull) & ~15ull : 0ull;
-        unsigned long long inc = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned long long n = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc += n;
-        }
-        if (lane == 31) s_w[wid] = inc;
-        const unsigned int fail0 = s_fail;
-        const unsigned long long carry = s_carry;
-        __syncthreads();
-        unsigned long long wbase = 0ull;
-        for (int w = 0; w < wid; ++w) wbase += s_w[w];
-        const unsigned long long end = carry + wbase + inc;
-        if (i < P.n_chunks) {
-            const unsigned long long reserve = (end - start) * (unsigned long long)P.layers_left / (unsigned)P.nlay;
-            const bool fits = (unsigned)i < fail0 && end + reserve <= (unsigned long long)P.arena_bytes;
-            P.chunk_base[i] = fits ? end - v : ~0ull;
-            if (fits) {
-                P.ptotal[i] += P.totals[i];
-                atomicMax(&s_end, end);
-            } else {
-                atomicOr(&P.err[i], 16u);
-                atomicMin(&s_fail, (unsigned)i);
-            }
-        }
-        __syncthreads();
-        if (tid == 0) s_carry = s_end;
-        __syncthreads();
-    }
-    if (tid == 0) {
-        *P.cursor = s_carry;
-        *P.fail_from = s_fail;
-    }
+    const int tid = threadIdx.x;
+    arena_place(P.n_chunks, P.totals, P.layers_left, P.nlay, P.arena_bytes, P.cursor, P.fail_from, P.chunk_base, P.err);
+    for (int i = tid; i < P.n_chunks; i += 1024)
+        if (P.chunk_base[i] != ~0ull) P.ptotal[i] += P.totals[i];
     const int NLc = P.ppl * P.nlay;
     for (int k = tid; k < P.n_chunks * NLc; k += 1024) {
         const int j = k / NLc, pl = k - j * NLc;
@@ -1776,39 +1730,6 @@ static EnclWs encl_ws_layout(int n_chunks, int64_t call_tiles, int64_t call_unit
 // What b200kv_encode_layers_plan decided, kept in the caller's b200kv_encode_plan_t: the kernels' parameter block (its
 // counters live in the workspace), the layers encoded so far and the most one call may take.
 constexpr uint32_t kEncPlanMagic = 0x4e4c5045u;   // "EPLN"
-// a set of layers [0, B200KV_MAX_PLANES / 2): bit l % 64 of word l / 64
-struct LayerSet {
-    static constexpr int kWords = B200KV_MAX_PLANES / 2 / 64;
-    uint64_t w[kWords];
-    // layers [a, b), 0 <= a <= b <= kWords * 64
-    static LayerSet range(int a, int b) {
-        LayerSet s;
-        for (int i = 0; i < kWords; ++i) {
-            const int lo = std::max(a - 64 * i, 0), hi = std::min(b - 64 * i, 64);   // the range inside word i
-            s.w[i] = lo >= hi ? 0ull : (hi - lo == 64 ? ~0ull : ((1ull << (hi - lo)) - 1ull) << lo);
-        }
-        return s;
-    }
-    bool intersects(const LayerSet& o) const {
-        uint64_t x = 0ull;
-        for (int i = 0; i < kWords; ++i) x |= w[i] & o.w[i];
-        return x != 0ull;
-    }
-    bool operator==(const LayerSet& o) const {
-        for (int i = 0; i < kWords; ++i)
-            if (w[i] != o.w[i]) return false;
-        return true;
-    }
-    void add(const LayerSet& o) {
-        for (int i = 0; i < kWords; ++i) w[i] |= o.w[i];
-    }
-    int count() const {
-        int n = 0;
-        for (int i = 0; i < kWords; ++i) n += __builtin_popcountll(w[i]);
-        return n;
-    }
-};
-static_assert(LayerSet::kWords * 64 == B200KV_MAX_PLANES / 2, "one bit per layer");
 struct EncPlan {
     uint32_t magic;
     int32_t max_layers;

@@ -56,4 +56,98 @@ __device__ __forceinline__ int64_t tok_row(const int64_t* slot_map, int64_t tok)
     else return tok;
 }
 
+// A set of layers [0, B200KV_MAX_PLANES / 2): bit l % 64 of word l / 64.  The layer-wise encode plans (CacheGen and
+// lossless) record in one the layers encoded so far.
+struct LayerSet {
+    static constexpr int kWords = B200KV_MAX_PLANES / 2 / 64;
+    uint64_t w[kWords];
+    // layers [a, b), 0 <= a <= b <= kWords * 64
+    static LayerSet range(int a, int b) {
+        LayerSet s;
+        for (int i = 0; i < kWords; ++i) {
+            const int lo = a - 64 * i > 0 ? a - 64 * i : 0, hi = b - 64 * i < 64 ? b - 64 * i : 64;   // inside word i
+            s.w[i] = lo >= hi ? 0ull : (hi - lo == 64 ? ~0ull : ((1ull << (hi - lo)) - 1ull) << lo);
+        }
+        return s;
+    }
+    bool intersects(const LayerSet& o) const {
+        uint64_t x = 0ull;
+        for (int i = 0; i < kWords; ++i) x |= w[i] & o.w[i];
+        return x != 0ull;
+    }
+    bool operator==(const LayerSet& o) const {
+        for (int i = 0; i < kWords; ++i)
+            if (w[i] != o.w[i]) return false;
+        return true;
+    }
+    void add(const LayerSet& o) {
+        for (int i = 0; i < kWords; ++i) w[i] |= o.w[i];
+    }
+    int count() const {
+        int n = 0;
+        for (int i = 0; i < kWords; ++i) n += __builtin_popcountll(w[i]);
+        return n;
+    }
+};
+static_assert(LayerSet::kWords * 64 == B200KV_MAX_PLANES / 2, "one bit per layer");
+
+// The arena rule of the layer-wise stores (place_kernel in codec.cu, ll_place_kernel in lossless.cu; its host
+// statement is pipeline.arena_placement).  After a call's encode, chunk i's bytes of the call, seg_bytes[i], get room
+// in the arena in chunk order from the device-held cursor, 16-byte aligned.  Chunk i fits iff every chunk before it
+// fits and the arena still holds, after chunks 0..i of this call, the layers still to come for them at this call's size
+// per layer (layers_left / nlay times this call's bytes of chunks 0..i): without that reserve the first calls would
+// fill the arena with every chunk and a later call would find no room even for chunk 0.  The first chunk that does not
+// fit is remembered (fail_from), so the chunks that fit are always a prefix, over this call and every later one.
+// chunk_base[i] gets the arena offset, or ~0 with bit 16 OR-ed into err[i].  One CTA of 1024 threads, every thread
+// calls it; on return chunk_base is visible to the whole CTA.
+__device__ __forceinline__ void arena_place(int n_chunks, const unsigned long long* seg_bytes, int layers_left, int nlay,
+                                            int64_t arena_bytes, unsigned long long* cursor, unsigned int* fail_from,
+                                            unsigned long long* chunk_base, unsigned int* err) {
+    __shared__ unsigned long long s_w[32];
+    __shared__ unsigned long long s_carry, s_end;
+    __shared__ unsigned int s_fail;
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    if (tid == 0) {
+        s_carry = s_end = *cursor;
+        s_fail = *fail_from;
+    }
+    __syncthreads();
+    const unsigned long long start = s_carry;
+    for (int b0 = 0; b0 < n_chunks; b0 += 1024) {
+        const int i = b0 + tid;
+        const unsigned long long v = i < n_chunks ? (seg_bytes[i] + 15ull) & ~15ull : 0ull;
+        unsigned long long inc = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long n = __shfl_up_sync(0xffffffffu, inc, o);
+            if (lane >= o) inc += n;
+        }
+        if (lane == 31) s_w[wid] = inc;
+        const unsigned int fail0 = s_fail;
+        const unsigned long long carry = s_carry;
+        __syncthreads();
+        unsigned long long wbase = 0ull;
+        for (int w = 0; w < wid; ++w) wbase += s_w[w];
+        const unsigned long long end = carry + wbase + inc;
+        if (i < n_chunks) {
+            const unsigned long long reserve = (end - start) * (unsigned long long)layers_left / (unsigned)nlay;
+            const bool fits = (unsigned)i < fail0 && end + reserve <= (unsigned long long)arena_bytes;
+            chunk_base[i] = fits ? end - v : ~0ull;
+            if (fits) {
+                atomicMax(&s_end, end);
+            } else {
+                atomicOr(&err[i], 16u);
+                atomicMin(&s_fail, (unsigned)i);
+            }
+        }
+        __syncthreads();
+        if (tid == 0) s_carry = s_end;
+        __syncthreads();
+    }
+    if (tid == 0) {
+        *cursor = s_carry;
+        *fail_from = s_fail;
+    }
+}
+
 }  // namespace b200kv

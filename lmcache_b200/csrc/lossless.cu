@@ -10,12 +10,19 @@
 //   encode: ll_hist_kernel (per-(chunk, plane) histogram) -> ll_norm_kernel (frequency rows) -> ll_encode_kernel (raw
 //           bytes in place, rANS into a worst-case scratch row) -> ll_scan_kernel (tile offsets, header, sizes_out) ->
 //           ll_compact_kernel (streams into the payload).  The KV is read twice: once for the histogram, once to code.
+//   layer-wise encode (b200kv_lossless_encode_layers_plan / _layers / _finish): the same kernels over the planes of a
+//           range of layers (a plane-range remap, the identity for the whole container), with the raw rows staged in
+//           the workspace -> ll_scan_kernel (the call's segment bytes per chunk) -> ll_place_kernel (the arena rule,
+//           segment rows) -> ll_raw_copy_kernel + ll_compact_kernel (raw rows and streams into the arena) ... and at
+//           the end ll_finish_kernel (headers into the fixed images, sizes_out).
 //   decode: ll_tile_sum_kernel -> ll_scan_kernel (stream offsets from the lengths section; the plan) ->
 //           ll_decode_kernel (once for every layer, or once per range of layers: b200kv_lossless_decode_layers).
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
+
+#include <algorithm>
 
 #include "ac_core.cuh"
 #include "common.cuh"
@@ -54,15 +61,30 @@ struct LlEnc {
     const int64_t* slot_map;
     int32_t L, H, D, C, NP, dtype;       // NP = planes: 2L, or L for a latent KV
     int32_t n_chunks, chunk_tokens, last_chunk_tokens, tpp, ntiles, rw;   // rw: halfwords per scratch row
-    uint8_t* out;
+    uint8_t* out;                        // containers (the layer-wise encode: fixed images [0, off_raw))
     int64_t out_stride;
     uint64_t* sizes_out;
-    uint32_t* hist;                      // [n][NP][256] symbol counts
-    uint32_t* err;                       // [n] bit 0: a stream outgrew the bound
-    uint32_t* tab;                       // [n][NP][256] (start << 16) | freq
+    // The launch codes the planes of layers [lb, lb + nl), npc per chunk: local plane pl < nl is plane lb + pl, the
+    // others L + lb + pl - nl (ll_plane; the identity for lb = 0, nl = L).  Scratch rows are indexed by local plane.
+    int32_t lb, nl, npc;
+    int32_t layers_left;                 // layers not yet encoded after this call (arena reserve, ll_place_kernel)
+    uint32_t* hist;                      // [n][npc][256] symbol counts
+    uint32_t* err;                       // [n] bit 0: a stream outgrew the bound; bit 16: the chunk did not fit the arena
+    uint32_t* tab;                       // [n][npc][256] (start << 16) | freq
     unsigned long long* tile;            // [n][ntiles] stream bytes per tile, then exclusive prefix
-    uint32_t* state;                     // [n][NP][C] final coder states
-    uint16_t* scratch;                   // [n][NP][C][rw] renormalisation halfwords, the last one pushed first
+    uint32_t* state;                     // [n][npc][C] final coder states
+    uint16_t* scratch;                   // [n][npc][C][rw] renormalisation halfwords, the last one pushed first
+    uint8_t* raw;                        // raw rows of (chunk j, local plane pl): raw + j * raw_stride + pl * t * C
+    int64_t raw_stride;
+    // b200kv_lossless_encode_layers only (arena NULL otherwise): raw rows and streams go to a device arena
+    uint8_t* arena;
+    int64_t arena_bytes;
+    unsigned long long* chunk_base;      // [n] arena offset of chunk j's segment of this call, ~0 = chunk failed
+    unsigned long long* cursor;          // first free arena byte (device-held across calls)
+    unsigned int* fail_from;             // first failed chunk (n_chunks: none); every later chunk fails too
+    unsigned long long* totals;          // [n] bytes of chunk j's segment of this call
+    unsigned long long* ptotal;          // [n] stream bytes of every call so far (the header's payload_bytes)
+    int64_t* seg;                        // [n][NP][3] segment rows (b200kv_lossless_encode_layers_plan)
 };
 static_assert(sizeof(LlEnc) < kMaxParamBytes, "LlEnc must stay under 4 KB of kernel parameters");
 
@@ -94,8 +116,52 @@ struct LlPlan {
 };
 static_assert(sizeof(LlPlan) <= sizeof(b200kv_lossless_decode_plan_t), "b200kv_lossless_decode_plan_t too small");
 
+// What b200kv_lossless_encode_layers_plan decided, kept in the caller's b200kv_lossless_encode_plan_t: the kernels'
+// parameter block (its counters live in the workspace), the layers encoded so far and the most one call may take.
+constexpr uint32_t kLlEncPlanMagic = 0x4c50454cu;   // "LEPL"
+struct LlEncPlan {
+    uint32_t magic;
+    int32_t max_layers;
+    LayerSet done;
+    LlEnc P;
+};
+static_assert(sizeof(LlEncPlan) <= sizeof(b200kv_lossless_encode_plan_t), "b200kv_lossless_encode_plan_t too small");
+
 __device__ __forceinline__ int ll_chunk_t(const LlEnc& P, int j) {
     return j == P.n_chunks - 1 ? P.last_chunk_tokens : P.chunk_tokens;
+}
+
+// container plane of the launch's local plane (LlEnc.lb / nl)
+__device__ __forceinline__ int ll_plane(const LlEnc& P, int pl) {
+    return pl < P.nl ? P.lb + pl : P.L + P.lb + (pl - P.nl);
+}
+
+// bytes of the raw part of a chunk's segment in the layer-wise encode: the call's raw rows, and -- in the call that
+// holds the last plane -- the container's zero bytes between the raw section and off_payload, then 16-byte aligned
+__device__ __forceinline__ int64_t ll_seg_raw(const LlEnc& P, int t, const LlLayout& lo) {
+    int64_t r = (int64_t)P.npc * t * P.C;
+    if (P.lb + P.nl == P.L) r += lo.off_payload - lo.off_raw - (int64_t)P.NP * t * P.C;
+    return align16(r);
+}
+
+// header of chunk j with `payload` stream bytes
+__device__ __forceinline__ void ll_put_header(const LlEnc& P, int j, unsigned long long payload, uint32_t status) {
+    const int t = ll_chunk_t(P, j);
+    const LlLayout lo = ll_layout(P.NP, P.C, t);
+    b200kv_header hd;
+    memset(&hd, 0, sizeof(hd));
+    hd.magic = B200KV_MAGIC;
+    hd.version = P.NP == P.L ? 6u : 5u;
+    hd.L = (uint32_t)P.L; hd.H = (uint32_t)P.H; hd.D = (uint32_t)P.D;
+    hd.ntokens = (uint32_t)t;
+    hd.ngroups = 1u;
+    hd.max_dtype = (uint32_t)P.dtype;
+    hd.payload_bytes = payload;
+    hd.total_bytes = (uint64_t)lo.off_payload + payload;
+    hd.status = status;
+    if (hd.total_bytes > (uint64_t)P.out_stride && P.arena == nullptr) hd.status |= 2u;   // cannot happen within the bound
+    *reinterpret_cast<b200kv_header*>(P.out + (int64_t)j * P.out_stride) = hd;
+    P.sizes_out[j] = hd.status ? 0ull : hd.total_bytes;
 }
 
 __device__ __forceinline__ uint32_t rotl1(uint32_t u) { return ((u << 1) | (u >> 15)) & 0xffffu; }
@@ -131,7 +197,7 @@ __device__ __forceinline__ T cta_excl_scan(T v, T* s_w, T* total) {
 template <bool PAGED>
 __global__ void __launch_bounds__(kCT) ll_hist_kernel(LlEnc P) {
     __shared__ uint32_t s_h[kCT / 32][kSyms];
-    const int j = blockIdx.z, p = blockIdx.y;
+    const int j = blockIdx.z, pl = blockIdx.y, p = ll_plane(P, pl);
     const int tile = blockIdx.x % P.tpp, slice = blockIdx.x / P.tpp;
     const int t = ll_chunk_t(P, j);
     const int i0 = slice * kSlice;
@@ -158,7 +224,7 @@ __global__ void __launch_bounds__(kCT) ll_hist_kernel(LlEnc P) {
         }
     }
     __syncthreads();
-    uint32_t* g = P.hist + ((int64_t)j * P.NP + p) * kSyms;
+    uint32_t* g = P.hist + ((int64_t)j * P.npc + pl) * kSyms;
     for (int s = threadIdx.x; s < kSyms; s += kCT) {
         uint32_t v = 0u;
 #pragma unroll
@@ -173,9 +239,9 @@ __global__ void __launch_bounds__(kCT) ll_hist_kernel(LlEnc P) {
 __global__ void __launch_bounds__(kSyms) ll_norm_kernel(LlEnc P) {
     __shared__ uint32_t s_w[kSyms / 32];
     __shared__ unsigned long long s_k[kSyms / 32];
-    const int j = blockIdx.y, p = blockIdx.x, s = threadIdx.x;
+    const int j = blockIdx.y, pl = blockIdx.x, p = ll_plane(P, pl), s = threadIdx.x;
     const int t = ll_chunk_t(P, j);
-    const int64_t row = (int64_t)j * P.NP + p;
+    const int64_t row = (int64_t)j * P.npc + pl;
     const uint32_t n = P.hist[row * kSyms + s];
     const uint32_t K = (uint32_t)__syncthreads_count(n != 0u);
     const uint64_t N = (uint64_t)P.C * (uint64_t)t;
@@ -211,9 +277,9 @@ template <bool PAGED>
 __global__ void __launch_bounds__(kCT) ll_encode_kernel(LlEnc P) {
     __shared__ uint32_t s_tab[kSyms];
     __shared__ unsigned long long s_w[kCT / 32];
-    const int j = blockIdx.z, p = blockIdx.y, tile = blockIdx.x;
+    const int j = blockIdx.z, pl = blockIdx.y, p = ll_plane(P, pl), tile = blockIdx.x;
     const int t = ll_chunk_t(P, j);
-    const int64_t row = (int64_t)j * P.NP + p;
+    const int64_t row = (int64_t)j * P.npc + pl;
     for (int s = threadIdx.x; s < kSyms; s += kCT) s_tab[s] = P.tab[row * kSyms + s];
     __syncthreads();
     const int c = tile * kCT + threadIdx.x;
@@ -226,7 +292,7 @@ __global__ void __launch_bounds__(kCT) ll_encode_kernel(LlEnc P) {
         const int h = c / P.D, d = c - h * P.D;
         const uint16_t* base = P.pt.p[p] + (int64_t)h * P.sH + d;
         const int64_t tok0 = P.tok_begin + (int64_t)j * P.chunk_tokens;
-        uint8_t* raw = cont + lo.off_raw + (int64_t)p * t * P.C + c;
+        uint8_t* raw = P.raw + (int64_t)j * P.raw_stride + (int64_t)pl * t * P.C + c;
         uint16_t* srow = P.scratch + (row * P.C + c) * P.rw;
         const int rw = P.rw;
         uint32_t nxt = __ldg(base + tok_row<PAGED>(P.slot_map, tok0 + t - 1) * P.sT);
@@ -250,7 +316,7 @@ __global__ void __launch_bounds__(kCT) ll_encode_kernel(LlEnc P) {
     }
     unsigned long long tot;
     cta_excl_scan<kCT, unsigned long long>(on ? 4ull + 2ull * (unsigned long long)k : 0ull, s_w, &tot);
-    if (threadIdx.x == 0) P.tile[(int64_t)j * P.ntiles + (int64_t)p * P.tpp + tile] = tot;
+    if (threadIdx.x == 0) P.tile[(int64_t)j * P.ntiles + (int64_t)pl * P.tpp + tile] = tot;
 }
 
 // exclusive prefix of one chunk's tile values in place; returns the chunk's total to thread 0
@@ -281,44 +347,42 @@ __device__ unsigned long long ll_scan_tiles(unsigned long long* v, int n) {
     return carry;
 }
 
-// 4a) per chunk: tile offsets, then the header and sizes_out[j] (0 when the chunk's status is nonzero)
+// 4a) per chunk: tile offsets, then the header and sizes_out[j] (0 when the chunk's status is nonzero), and zeros in the
+//     two alignment gaps (after the lengths, after the raw rows) instead of whatever the output buffer held.  In the
+//     layer-wise encode: the bytes of the chunk's segment of this call instead (the raw part, then the streams).
 __global__ void __launch_bounds__(1024) ll_enc_scan_kernel(LlEnc P) {
     const int j = blockIdx.x;
     const unsigned long long payload = ll_scan_tiles(P.tile + (int64_t)j * P.ntiles, P.ntiles);
     if (threadIdx.x != 0) return;
     const int t = ll_chunk_t(P, j);
     const LlLayout lo = ll_layout(P.NP, P.C, t);
-    b200kv_header hd;
-    memset(&hd, 0, sizeof(hd));
-    hd.magic = B200KV_MAGIC;
-    hd.version = P.NP == P.L ? 6u : 5u;
-    hd.L = (uint32_t)P.L; hd.H = (uint32_t)P.H; hd.D = (uint32_t)P.D;
-    hd.ntokens = (uint32_t)t;
-    hd.ngroups = 1u;
-    hd.max_dtype = (uint32_t)P.dtype;
-    hd.payload_bytes = payload;
-    hd.total_bytes = (uint64_t)lo.off_payload + payload;
-    hd.status = P.err[j];
-    if (hd.total_bytes > (uint64_t)P.out_stride) hd.status |= 2u;     // cannot happen within the stream bound
-    *reinterpret_cast<b200kv_header*>(P.out + (int64_t)j * P.out_stride) = hd;
-    P.sizes_out[j] = hd.status ? 0ull : hd.total_bytes;
+    if (P.arena != nullptr) {
+        P.totals[j] = (unsigned long long)ll_seg_raw(P, t, lo) + payload;
+        return;
+    }
+    ll_put_header(P, j, payload, P.err[j]);
+    uint8_t* cont = P.out + (int64_t)j * P.out_stride;
+    for (int64_t b = lo.off_lens + 2 * (int64_t)P.NP * P.C; b < lo.off_raw; ++b) cont[b] = 0u;
+    for (int64_t b = lo.off_raw + (int64_t)P.NP * t * P.C; b < lo.off_payload; ++b) cont[b] = 0u;
 }
 
-// 4b) streams into the payload, a warp per 32 streams: [LE32 state][halfwords in decode order]
+// 4b) streams into the payload (the layer-wise encode: into the chunk's segment, after its raw part), a warp per 32
+//     streams: [LE32 state][halfwords in decode order]
 __global__ void __launch_bounds__(kCT) ll_compact_kernel(LlEnc P) {
     __shared__ uint32_t s_w[kCT / 32];
-    const int j = blockIdx.z, p = blockIdx.y, tile = blockIdx.x;
-    if (P.err[j]) return;
+    const int j = blockIdx.z, pl = blockIdx.y, p = ll_plane(P, pl), tile = blockIdx.x;
+    if (P.err[j]) return;                                // an overflowed stream, or no room in the arena
     const int t = ll_chunk_t(P, j);
     const LlLayout lo = ll_layout(P.NP, P.C, t);
     uint8_t* cont = P.out + (int64_t)j * P.out_stride;
-    const int64_t row = (int64_t)j * P.NP + p;
+    uint8_t* base = P.arena != nullptr ? P.arena + P.chunk_base[j] + ll_seg_raw(P, t, lo) : cont + lo.off_payload;
+    const int64_t row = (int64_t)j * P.npc + pl;
     const int c = tile * kCT + threadIdx.x;
     const bool on = c < P.C;
     const uint32_t len = on ? reinterpret_cast<const uint16_t*>(cont + lo.off_lens)[(int64_t)p * P.C + c] : 0u;
     uint32_t tot;
     const uint32_t ex = cta_excl_scan<kCT>(len, s_w, &tot);
-    const unsigned long long off = (unsigned long long)lo.off_payload + P.tile[(int64_t)j * P.ntiles + (int64_t)p * P.tpp + tile] + ex;
+    const unsigned long long off = P.tile[(int64_t)j * P.ntiles + (int64_t)pl * P.tpp + tile] + ex;
     const uint32_t st = on ? P.state[row * P.C + c] : 0u;
     const int lane = threadIdx.x & 31;
     const int cw = tile * kCT + (threadIdx.x & ~31);
@@ -329,10 +393,71 @@ __global__ void __launch_bounds__(kCT) ll_compact_kernel(LlEnc P) {
         if (sl == 0u) continue;
         const uint32_t nh = sl >> 1, k = nh - 2;
         const uint16_t* r = P.scratch + (row * P.C + cw + src) * P.rw + (P.rw - k) - 2;
-        uint16_t* dst = reinterpret_cast<uint16_t*>(cont + so);
+        uint16_t* dst = reinterpret_cast<uint16_t*>(base + so);
         for (uint32_t q = lane; q < nh; q += 32)
             dst[q] = q == 0 ? (uint16_t)sx : q == 1 ? (uint16_t)(sx >> 16) : r[q];
     }
+}
+
+// ------------------------------------------------------------------------------------------ layer-wise encode
+// After ll_enc_scan_kernel: each chunk's segment of this call gets room in the arena by the arena rule (arena_place,
+// common.cuh), the stream bytes of the chunks placed are added to their payload totals, and every plane of the call gets
+// its segment row (arena offset of its raw rows, arena offset of its streams, stream bytes).  One CTA.
+__global__ void __launch_bounds__(1024) ll_place_kernel(LlEnc P) {
+    const int tid = threadIdx.x;
+    arena_place(P.n_chunks, P.totals, P.layers_left, P.nl, P.arena_bytes, P.cursor, P.fail_from, P.chunk_base, P.err);
+    for (int j = tid; j < P.n_chunks; j += 1024)
+        if (P.chunk_base[j] != ~0ull) {
+            const int t = ll_chunk_t(P, j);
+            P.ptotal[j] += P.totals[j] - (unsigned long long)ll_seg_raw(P, t, ll_layout(P.NP, P.C, t));
+        }
+    for (int k = tid; k < P.n_chunks * P.npc; k += 1024) {
+        const int j = k / P.npc, pl = k - j * P.npc;
+        const int t = ll_chunk_t(P, j);
+        const unsigned long long raw = (unsigned long long)ll_seg_raw(P, t, ll_layout(P.NP, P.C, t));
+        const unsigned long long* tb = P.tile + (int64_t)j * P.ntiles;
+        const unsigned long long off = tb[pl * P.tpp];
+        const unsigned long long end = pl + 1 < P.npc ? tb[(pl + 1) * P.tpp] : P.totals[j] - raw;
+        const unsigned long long cb = P.chunk_base[j];
+        int64_t* row = P.seg + ((int64_t)j * P.NP + ll_plane(P, pl)) * 3;
+        row[0] = cb == ~0ull ? -1 : (int64_t)(cb + (unsigned long long)pl * t * P.C);
+        row[1] = cb == ~0ull ? -1 : (int64_t)(cb + raw + off);
+        row[2] = (int64_t)(end - off);
+    }
+}
+
+// The raw part of each placed chunk's segment: the call's staged raw rows, then zeros up to the segment's streams (the
+// container's gap before off_payload, when the call holds the last plane, and the alignment).  16 bytes per thread.
+__global__ void __launch_bounds__(256) ll_raw_copy_kernel(LlEnc P) {
+    const int j = blockIdx.y;
+    if (P.err[j]) return;
+    const int t = ll_chunk_t(P, j);
+    const int64_t nraw = (int64_t)P.npc * t * P.C, nseg = ll_seg_raw(P, t, ll_layout(P.NP, P.C, t));
+    const uint8_t* src = P.raw + (int64_t)j * P.raw_stride;
+    uint8_t* dst = P.arena + P.chunk_base[j];
+    for (int64_t b = 16 * ((int64_t)blockIdx.x * blockDim.x + threadIdx.x); b < nseg; b += 16 * (int64_t)gridDim.x * blockDim.x) {
+        uint4 v;
+        if (b + 16 <= nraw) {
+            v = __ldg(reinterpret_cast<const uint4*>(src + b));
+        } else {
+            uint8_t x[16];
+#pragma unroll
+            for (int i = 0; i < 16; ++i) x[i] = b + i < nraw ? src[b + i] : (uint8_t)0;
+            memcpy(&v, x, 16);
+        }
+        *reinterpret_cast<uint4*>(dst + b) = v;
+    }
+}
+
+__global__ void ll_encl_init_kernel(LlEnc P) {
+    *P.cursor = 0ull;
+    *P.fail_from = (unsigned)P.n_chunks;
+}
+
+// headers into the fixed images from the payload of every call; sizes_out 0 for a chunk with a nonzero status
+__global__ void ll_finish_kernel(LlEnc P) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < P.n_chunks) ll_put_header(P, j, P.ptotal[j], P.err[j]);
 }
 
 // ------------------------------------------------------------------------------------------ decode
@@ -521,6 +646,32 @@ LlEncWs ll_enc_ws(int64_t n, int64_t NP, int64_t C, int chunk_tokens, int64_t* r
     return w;
 }
 
+// b200kv_lossless_encode_layers_plan's workspace: the state that lives across calls (error words, payload totals,
+// chunk bases, cursor + fail_from, segment bytes), then one call's scratch for npc = planes of at most max_layers
+// layers: histograms, tables, tile totals, coder states, scratch rows, and the call's raw rows, staged.
+struct LlEnclWs { size_t err, ptotal, cbase, state, totals, hist, tab, tile, cstate, scratch, raw, total; int64_t rw, raw_stride; };
+LlEnclWs ll_encl_ws(int64_t n, int64_t npc, int64_t C, int chunk_tokens) {
+    const int64_t tpp = (C + kCT - 1) / kCT;
+    LlEnclWs w;
+    w.rw = (ll_max_words(chunk_tokens) + 1) & ~(int64_t)1;
+    w.raw_stride = align16(npc * chunk_tokens * C);
+    size_t o = 0;
+    auto take = [&](size_t bytes) { const size_t at = o; o = (o + bytes + 255) & ~(size_t)255; return at; };
+    w.err = take(sizeof(uint32_t) * n);
+    w.ptotal = take(sizeof(unsigned long long) * n);
+    w.cbase = take(sizeof(unsigned long long) * n);
+    w.state = take(16);
+    w.totals = take(sizeof(unsigned long long) * n);
+    w.hist = take(sizeof(uint32_t) * n * npc * kSyms);
+    w.tab = take(sizeof(uint32_t) * n * npc * kSyms);
+    w.tile = take(sizeof(unsigned long long) * n * npc * tpp);
+    w.cstate = take(sizeof(uint32_t) * n * npc * C);
+    w.scratch = take(sizeof(uint16_t) * n * npc * C * w.rw);
+    w.raw = take((size_t)(n * w.raw_stride));
+    w.total = o;
+    return w;
+}
+
 size_t ll_dec_ws(int64_t n, int64_t NP, int64_t C, size_t* off_tile) {
     const int64_t tpp = (C + kCT - 1) / kCT;
     *off_tile = ((size_t)sizeof(LlDecChunk) * n + 255) & ~(size_t)255;
@@ -594,6 +745,11 @@ int b200kv_lossless_encode(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t 
     P.out = static_cast<uint8_t*>(out);
     P.out_stride = out_stride;
     P.sizes_out = sizes_out;
+    P.lb = 0; P.nl = P.L; P.npc = P.NP; P.layers_left = 0;        // every plane: the remap is the identity
+    P.raw = P.out + lo.off_raw;                                   // raw rows in place (off_raw does not depend on t)
+    P.raw_stride = out_stride;
+    P.arena = nullptr; P.arena_bytes = 0; P.chunk_base = nullptr; P.cursor = nullptr; P.fail_from = nullptr;
+    P.totals = nullptr; P.ptotal = nullptr; P.seg = nullptr;
     uint8_t* ws = static_cast<uint8_t*>(workspace);
     P.hist = reinterpret_cast<uint32_t*>(ws + w.hist);
     P.err = reinterpret_cast<uint32_t*>(ws + w.err);
@@ -743,6 +899,128 @@ int b200kv_lossless_decode(const void* containers, int64_t containers_bytes, con
                                              stream))
         return rc;
     return b200kv_lossless_decode_layers(&plan, 0, dst->L, stream);
+}
+
+int64_t b200kv_lossless_encode_layers_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t chunk_tokens,
+                                                      int32_t n_chunks, int32_t latent, int32_t max_layers) {
+    if (!shape_ok(L, H, D, chunk_tokens) || n_chunks <= 0 || n_chunks > 65535 || max_layers <= 0 || max_layers > L)
+        return -2;
+    return (int64_t)ll_encl_ws(n_chunks, (latent ? 1 : 2) * (int64_t)max_layers, (int64_t)H * D, chunk_tokens).total;
+}
+
+int b200kv_lossless_encode_layers_plan(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_chunks,
+                                       int32_t chunk_tokens, int32_t last_chunk_tokens, void* arena, int64_t arena_bytes,
+                                       void* fixed_out, int64_t fixed_stride, int64_t* seg_sizes_out,
+                                       uint64_t* sizes_out, int32_t max_layers, void* workspace, int64_t workspace_bytes,
+                                       b200kv_lossless_encode_plan_t* plan_out, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B2_REQUIRE(plan_out != nullptr, "plan is NULL");
+    LlEncPlan* plan = reinterpret_cast<LlEncPlan*>(plan_out);
+    plan->magic = 0u;
+    LlEnc& P = plan->P;
+    if (int rc = fill_planes(kv, &P.pt)) return rc;
+    B2_REQUIRE(shape_ok(kv->L, kv->H, kv->D, chunk_tokens), "bad shape (H * D < 2^24, 1 <= chunk_tokens <= 4096)");
+    B2_REQUIRE(n_chunks > 0 && n_chunks <= 65535, "n_chunks must be in [1, 65535]");
+    B2_REQUIRE(last_chunk_tokens > 0 && last_chunk_tokens <= chunk_tokens, "last_chunk_tokens out of range");
+    B2_REQUIRE(tok_begin >= 0, "tok_begin must be >= 0");
+    B2_REQUIRE(max_layers > 0 && max_layers <= kv->L, "max_layers out of range");
+    B2_REQUIRE(seg_sizes_out != nullptr && sizes_out != nullptr, "seg_sizes_out / sizes_out is NULL");
+    B2_REQUIRE(arena != nullptr && (reinterpret_cast<uintptr_t>(arena) & 15) == 0 && arena_bytes >= 0,
+               "arena must be 16-byte aligned, arena_bytes >= 0");
+    B2_REQUIRE(fixed_out != nullptr && (reinterpret_cast<uintptr_t>(fixed_out) & 15) == 0 && (fixed_stride & 15) == 0,
+               "fixed_out / fixed_stride must be 16-byte aligned");
+    P.NP = kv_ppl(kv) * kv->L;
+    P.L = kv->L; P.H = kv->H; P.D = kv->D; P.C = kv->H * kv->D; P.dtype = kv_dtype(kv);
+    const LlLayout lo = ll_layout(P.NP, P.C, chunk_tokens);
+    B2_REQUIRE(fixed_stride >= lo.off_raw, "fixed_stride smaller than the fixed image [0, off_raw) (b200kv_lossless_layout)");
+    P.sT = kv->sT; P.sH = kv->sH; P.tok_begin = tok_begin;
+    P.slot_map = kv->slot_map;
+    P.n_chunks = n_chunks; P.chunk_tokens = chunk_tokens; P.last_chunk_tokens = last_chunk_tokens;
+    P.tpp = (P.C + kCT - 1) / kCT;
+    const LlEnclWs w = ll_encl_ws(n_chunks, (int64_t)kv_ppl(kv) * max_layers, P.C, chunk_tokens);
+    B2_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)w.total, "workspace too small");
+    uint8_t* ws = static_cast<uint8_t*>(workspace);
+    P.rw = (int32_t)w.rw;
+    P.out = static_cast<uint8_t*>(fixed_out);
+    P.out_stride = fixed_stride;
+    P.sizes_out = sizes_out;
+    P.err = reinterpret_cast<uint32_t*>(ws + w.err);
+    P.ptotal = reinterpret_cast<unsigned long long*>(ws + w.ptotal);
+    P.chunk_base = reinterpret_cast<unsigned long long*>(ws + w.cbase);
+    P.cursor = reinterpret_cast<unsigned long long*>(ws + w.state);
+    P.fail_from = reinterpret_cast<unsigned int*>(ws + w.state + 8);
+    P.totals = reinterpret_cast<unsigned long long*>(ws + w.totals);
+    P.hist = reinterpret_cast<uint32_t*>(ws + w.hist);
+    P.tab = reinterpret_cast<uint32_t*>(ws + w.tab);
+    P.tile = reinterpret_cast<unsigned long long*>(ws + w.tile);
+    P.state = reinterpret_cast<uint32_t*>(ws + w.cstate);
+    P.scratch = reinterpret_cast<uint16_t*>(ws + w.scratch);
+    P.raw = ws + w.raw;
+    P.raw_stride = w.raw_stride;
+    P.arena = static_cast<uint8_t*>(arena);
+    P.arena_bytes = arena_bytes;
+    P.seg = seg_sizes_out;
+    P.lb = 0; P.nl = 0; P.npc = 0; P.ntiles = 0; P.layers_left = 0;    // per call
+    // error words, totals, cursor; the fixed images too, so that their gap before off_raw is zero
+    B2_CHECK_CUDA(cudaMemsetAsync(ws, 0, w.hist, stream));
+    B2_CHECK_CUDA(cudaMemsetAsync(fixed_out, 0, (size_t)fixed_stride * n_chunks, stream));
+    ll_encl_init_kernel<<<1, 1, 0, stream>>>(P);
+    B2_CHECK_CUDA(cudaGetLastError());
+    plan->max_layers = max_layers;
+    plan->done = LayerSet::range(0, 0);
+    plan->magic = kLlEncPlanMagic;
+    return 0;
+}
+
+int b200kv_lossless_encode_layers(b200kv_lossless_encode_plan_t* plan_in, int32_t layer_begin, int32_t layer_end,
+                                  void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B2_REQUIRE(plan_in != nullptr, "plan is NULL");
+    LlEncPlan* plan = reinterpret_cast<LlEncPlan*>(plan_in);
+    B2_REQUIRE(plan->magic == kLlEncPlanMagic, "not a plan made by b200kv_lossless_encode_layers_plan");
+    LlEnc P = plan->P;
+    B2_REQUIRE(layer_begin >= 0 && layer_begin < layer_end && layer_end <= P.L, "layer range out of range");
+    B2_REQUIRE(layer_end - layer_begin <= plan->max_layers, "more layers than the plan's workspace holds");
+    const LayerSet bits = LayerSet::range(layer_begin, layer_end);
+    B2_REQUIRE(!plan->done.intersects(bits), "a layer of the range was encoded before");
+    P.lb = layer_begin;
+    P.nl = layer_end - layer_begin;
+    P.npc = (P.NP / P.L) * P.nl;
+    P.ntiles = P.npc * P.tpp;
+    P.layers_left = P.L - plan->done.count() - bits.count();
+    const int n = P.n_chunks;
+    B2_CHECK_CUDA(cudaMemsetAsync(P.hist, 0, sizeof(uint32_t) * (size_t)n * P.npc * kSyms, stream));
+    const bool paged = P.slot_map != nullptr;
+    const unsigned nslices = (unsigned)((P.chunk_tokens + kSlice - 1) / kSlice);
+    const dim3 ghist((unsigned)P.tpp * nslices, (unsigned)P.npc, (unsigned)n);
+    const dim3 gtile((unsigned)P.tpp, (unsigned)P.npc, (unsigned)n);
+    if (paged) ll_hist_kernel<true><<<ghist, kCT, 0, stream>>>(P);
+    else ll_hist_kernel<false><<<ghist, kCT, 0, stream>>>(P);
+    ll_norm_kernel<<<dim3((unsigned)P.npc, (unsigned)n), kSyms, 0, stream>>>(P);
+    if (paged) ll_encode_kernel<true><<<gtile, kCT, 0, stream>>>(P);
+    else ll_encode_kernel<false><<<gtile, kCT, 0, stream>>>(P);
+    ll_enc_scan_kernel<<<(unsigned)n, 1024, 0, stream>>>(P);
+    ll_place_kernel<<<1, 1024, 0, stream>>>(P);
+    // ~16 KB of raw rows per CTA pass; at most 64 CTAs per chunk
+    const int64_t raw_bytes = align16((int64_t)P.npc * P.chunk_tokens * P.C) + 16;
+    const unsigned rx = (unsigned)std::min<int64_t>(64, (raw_bytes + 16 * 256 * 4 - 1) / (16 * 256 * 4));
+    ll_raw_copy_kernel<<<dim3(rx, (unsigned)n), 256, 0, stream>>>(P);
+    ll_compact_kernel<<<gtile, kCT, 0, stream>>>(P);
+    B2_CHECK_CUDA(cudaGetLastError());
+    plan->done.add(bits);
+    return 0;
+}
+
+int b200kv_lossless_encode_layers_finish(const b200kv_lossless_encode_plan_t* plan_in, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B2_REQUIRE(plan_in != nullptr, "plan is NULL");
+    const LlEncPlan* plan = reinterpret_cast<const LlEncPlan*>(plan_in);
+    B2_REQUIRE(plan->magic == kLlEncPlanMagic, "not a plan made by b200kv_lossless_encode_layers_plan");
+    const LlEnc& P = plan->P;
+    B2_REQUIRE(plan->done == LayerSet::range(0, P.L), "a layer was never encoded");
+    ll_finish_kernel<<<(P.n_chunks + 127) / 128, 128, 0, stream>>>(P);
+    B2_CHECK_CUDA(cudaGetLastError());
+    return 0;
 }
 
 }  // extern "C"

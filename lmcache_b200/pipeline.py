@@ -32,8 +32,8 @@ import numpy as np
 import torch
 
 from lmcache_b200 import _native as N
-from lmcache_b200.codec import (CacheGenCodec, EncodedBatch, EncodeTicket, KvView, PinnedBuffer, lossless_raw_rows,
-                                parse_header)
+from lmcache_b200.codec import (CacheGenCodec, EncodedBatch, EncodeTicket, KvView, PinnedBuffer, SegmentLayout,
+                                lossless_raw_rows)
 
 
 def wave_chunks_default() -> int:
@@ -283,7 +283,7 @@ def land(slab, slot: WaveSlot, batch, blocks: Optional[list] = None,
     codec class) that wrote the wave: its header check and its plane-offset kernel (a lossless codec's for its
     containers).  A layer-wise store's slot (SegmentSlot) lands through land_segments."""
     if isinstance(slot, SegmentSlot):
-        return land_segments(slab, slot, batch, blocks, dev_dst)
+        return land_segments(slab, slot, batch, blocks, dev_dst, codec)
     parse = codec.parse_header
     dev = slot.dev.device
     cs = _d2h_stream(dev)
@@ -329,8 +329,9 @@ def layerwise_store_budget_default() -> int:
 
 
 def arena_placement(seg_bytes: np.ndarray, arena_bytes: int, layers: Optional[Sequence[int]] = None):
-    """Host statement of the layer-wise store's arena rule (place_kernel in codec.cu), for tests and sizing.
-    seg_bytes[c, j]: payload bytes of chunk j in layer call c (its K planes, then its V planes); layers[c]: the layers
+    """Host statement of the layer-wise store's arena rule (arena_place in common.cuh, which both encoders' placement
+    kernels run), for tests and sizing.  seg_bytes[c, j]: bytes of chunk j's segment in layer call c (CacheGen: the
+    payload of its K planes, then its V planes; lossless: its raw part, then those streams); layers[c]: the layers
     of call c (default 1 each).  Calls are placed in order; within a call, chunk j's bytes go 16-byte aligned at the
     cursor.  Chunk j fits if, after chunks 0..j of the call, the arena still holds the layers still to come at this
     call's size per layer (a reserve, so that a later call finds room for the chunks an earlier one accepted).  A chunk
@@ -360,26 +361,26 @@ def arena_placement(seg_bytes: np.ndarray, arena_bytes: int, layers: Optional[Se
 
 
 class SegmentSlot:
-    """Device scratch of one layer-wise store: the payload arena, the chunks' fixed-section images, the encode
-    workspace, and in mapped page-locked memory the container sizes and the (arena offset, bytes) row of every plane.
-    P: planes per chunk, 2L for (K, V) pairs, L for a latent KV."""
+    """Device scratch of one layer-wise store: the arena, the chunks' fixed-section images, the encode workspace, and in
+    mapped page-locked memory the container sizes and the segment row of every (chunk, plane): `row` int64 each (the
+    codec's seg_row: 2 for CacheGen, 3 for lossless).  P: planes per chunk, 2L for (K, V) pairs, L for a latent KV."""
 
-    def __init__(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, P: int, device):
+    def __init__(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, P: int, device, row: int = 2):
         self.arena = torch.empty(max(16, arena_bytes), dtype=torch.uint8, device=device)
         self.fixed = torch.empty(max(16, fixed_bytes), dtype=torch.uint8, device=device)
         self.ws = torch.empty(max(16, ws_bytes), dtype=torch.uint8, device=device)
         self.sizes = PinnedBuffer(max(64, 8 * n_chunks))
-        self.seg = PinnedBuffer(max(64, 16 * P * n_chunks))
+        self.seg = PinnedBuffer(max(64, 8 * row * P * n_chunks))
         self.arena_bytes = arena_bytes
         self.ticket = None
-        self.layouts: tuple = ()            # (off_payload of a full chunk, of the last chunk)
+        self.layouts: tuple = ()            # (SegmentLayout of a full chunk, of the last chunk)
         self.fixed_stride = 0
         self.coder = N.CODER_RANS_COMPACT   # the coder that names the containers' version (N.CODER_LATENT: 4)
-        self.n_chunks, self.P = 0, P
+        self.n_chunks, self.P, self.seg_row = 0, P, row
 
-    def holds(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, P: int) -> bool:
+    def holds(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, P: int, row: int = 2) -> bool:
         return (self.arena.numel() >= arena_bytes and self.fixed.numel() >= fixed_bytes and self.ws.numel() >= ws_bytes
-                and self.sizes.nbytes >= 8 * n_chunks and self.seg.nbytes >= 16 * P * n_chunks)
+                and self.sizes.nbytes >= 8 * n_chunks and self.seg.nbytes >= 8 * row * P * n_chunks)
 
     def close(self) -> None:
         self.sizes.close()
@@ -400,14 +401,15 @@ class SegmentPool:
         self._free: List[SegmentSlot] = []
         self._lock = threading.Lock()
 
-    def acquire(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, P: int) -> SegmentSlot:
+    def acquire(self, arena_bytes: int, fixed_bytes: int, ws_bytes: int, n_chunks: int, P: int,
+                row: int = 2) -> SegmentSlot:
         with self._lock:
             for s in self._free:
-                if s.holds(arena_bytes, fixed_bytes, ws_bytes, n_chunks, P):
+                if s.holds(arena_bytes, fixed_bytes, ws_bytes, n_chunks, P, row):
                     self._free.remove(s)
                     return s
         with torch.cuda.device(self.device), torch.cuda.stream(self.stream):
-            return SegmentSlot(arena_bytes, fixed_bytes, ws_bytes, n_chunks, P, self.device)
+            return SegmentSlot(arena_bytes, fixed_bytes, ws_bytes, n_chunks, P, self.device, row)
 
     def release(self, slot: SegmentSlot) -> None:
         slot.ticket = None
@@ -442,43 +444,36 @@ class _SegmentTicket:
 
 
 class LayerwiseEncode:
-    """One layer-wise store's encode (b200kv_encode_layers_plan / _layers / _finish) on the pool's stream.  The plan is
-    made at once; encode_layer(l, stream) makes the encode stream wait for `stream` and enqueues layer l; finish()
-    enqueues the headers and returns the event after which the KV is no longer read and the containers are complete.
-    The host never waits.  The arena is the airtight bound of the chunks (max_total_bytes - off_payload each, plus the
-    alignment of one segment per layer), capped at `budget`: past the cap the later chunks fail and become misses."""
+    """One layer-wise store's encode on the pool's stream, through the codec's three calls (CacheGen:
+    b200kv_encode_layers_plan / _layers / _finish; lossless: b200kv_lossless_encode_layers_*).  The plan is made at
+    once; encode_layer(l, stream) makes the encode stream wait for `stream` and enqueues layer l; finish() enqueues the
+    headers and returns the event after which the KV is no longer read and the containers are complete.  The host never
+    waits.  The arena is the airtight bound of the chunks (the codec's layerwise_chunk_bound each), capped at `budget`:
+    past the cap the later chunks fail and become misses."""
 
     def __init__(self, codec: CacheGenCodec, pool: SegmentPool, view: KvView, tok_begin: int, chunk_size: int,
                  budget: Optional[int] = None):
-        if view.L > codec.nlayers:
-            raise ValueError(f"KV has {view.L} layers but the bin table of this model has {codec.nlayers}")
         n_tok = view.ntokens - tok_begin
         n = (n_tok + chunk_size - 1) // chunk_size
         last = n_tok - (n - 1) * chunk_size
-        L, H, D = view.L, view.H, view.D
-        coder = N.CODER_LATENT if view.latent else N.CODER_RANS_COMPACT     # version 4 for a latent KV, else 3
-        lo = N.container_layout(L, H, D, chunk_size, coder)
-        lo_last = N.container_layout(L, H, D, last, coder)
-        stride = (lo.off_payload + 15) & ~15
-        per_chunk = lo.max_total_bytes - lo.off_payload + 16 * L
-        arena = min(n * per_chunk, budget or layerwise_store_budget_default())
-        lib = N.lib()
-        ws_bytes = N.check(lib.b200kv_encode_layers_workspace_bytes(L, H, D, chunk_size, n, 1), "encode_layers_workspace")
-        self.pool, self.view, self.L, self.n_chunks = pool, view, L, n
-        self.plan = N.EncodePlan()
-        self.slot = pool.acquire(arena, n * stride, ws_bytes, n, view.planes)
-        self.slot.n_chunks, self.slot.P, self.slot.fixed_stride, self.slot.coder = n, view.planes, stride, coder
-        self.slot.layouts = (int(lo.off_payload), int(lo_last.off_payload))
-        self.done: Optional[torch.cuda.Event] = None
+        L, H, D, latent = view.L, view.H, view.D, view.latent
+        coder = codec.coder_for(chunk_size, latent)
+        layouts = (codec.segment_layout(L, H, D, chunk_size, latent), codec.segment_layout(L, H, D, last, latent))
+        stride = (layouts[0].head + 15) & ~15
+        arena = min(n * codec.layerwise_chunk_bound(L, H, D, chunk_size, latent),
+                    budget or layerwise_store_budget_default())
+        ws_bytes = codec.layerwise_workspace_bytes(L, H, D, chunk_size, n, latent)
+        self.codec, self.pool, self.view, self.L, self.n_chunks = codec, pool, view, L, n
+        self.plan = codec.layer_plan_type()
+        self.slot = pool.acquire(arena, n * stride, ws_bytes, n, view.planes, codec.seg_row)
         s = self.slot
+        s.n_chunks, s.P, s.seg_row, s.fixed_stride, s.coder = n, view.planes, codec.seg_row, stride, coder
+        s.arena_bytes, s.layouts = arena, layouts
+        self.done: Optional[torch.cuda.Event] = None
         try:
             with torch.cuda.device(pool.device):
                 view.record_stream(pool.stream)          # the caller's KV outlives the encode's last read of it
-                N.check(lib.b200kv_encode_layers_plan(ctypes.byref(view.desc), tok_begin, n, chunk_size, last, codec._kb,
-                                                      codec._vb, N.CODER_RANS_COMPACT, s.arena.data_ptr(), arena,
-                                                      s.fixed.data_ptr(), stride, s.seg.dev_ptr, s.sizes.dev_ptr, 1,
-                                                      s.ws.data_ptr(), s.ws.numel(), ctypes.byref(self.plan),
-                                                      pool.stream.cuda_stream), "encode_layers_plan")
+                codec.encode_layers_plan(view, tok_begin, n, chunk_size, last, s, self.plan, pool.stream)
         except BaseException:
             self.abandon()
             raise
@@ -488,12 +483,13 @@ class LayerwiseEncode:
             ev = torch.cuda.Event()
             ev.record(stream)
             self.pool.stream.wait_event(ev)
-            N.check(N.lib().b200kv_encode_layers(ctypes.byref(self.plan), layer, layer + 1, self.pool.stream.cuda_stream),
-                    "encode_layers")
+            N.check(getattr(N.lib(), self.codec.encode_layers_fn)(ctypes.byref(self.plan), layer, layer + 1,
+                                                                  self.pool.stream.cuda_stream), "encode_layers")
 
     def finish(self) -> torch.cuda.Event:
         with torch.cuda.device(self.pool.device):
-            N.check(N.lib().b200kv_encode_layers_finish(ctypes.byref(self.plan), self.pool.stream.cuda_stream),
+            N.check(getattr(N.lib(), self.codec.encode_layers_finish_fn)(ctypes.byref(self.plan),
+                                                                         self.pool.stream.cuda_stream),
                     "encode_layers_finish")
             self.done = torch.cuda.Event()
             self.done.record(self.pool.stream)
@@ -509,49 +505,79 @@ class LayerwiseEncode:
             self.pool.release(slot)
 
 
+def segment_copy_ranges(seg: np.ndarray, layouts: Sequence[SegmentLayout]):
+    """Where the bytes of layer-wise stored containers come from (pure host arithmetic).  seg: int64 [n, P, w], the
+    segment rows of n containers of P planes -- w = 2: (arena offset, bytes) of each plane's streams (CacheGen); w = 3:
+    (arena offset of its raw rows, arena offset of its streams, stream bytes) (lossless).  layouts[j]: container j's
+    SegmentLayout.  Returns (dst, src, nbytes, planes): per container its copy ranges in order -- int64 [n, R] offset in
+    the container, source (-1: offset 0 of the chunk's fixed image; otherwise an arena offset) and length; R = 1 + P
+    (the fixed image, then each plane's streams) or 1 + 2P (the fixed image, each plane's raw rows -- the last plane's
+    running up to the payload --, each plane's streams) -- and int64 [n, P + 1] the plane offsets: payload + the running
+    sum of the stream bytes, what codec.plane_offsets / lossless_plane_offsets return for the same container."""
+    seg = np.asarray(seg, dtype=np.int64)
+    n, P, w = seg.shape
+    head = np.array([lo.head for lo in layouts], dtype=np.int64)[:, None]
+    pay = np.array([lo.payload for lo in layouts], dtype=np.int64)[:, None]
+    sbytes = seg[:, :, w - 1]
+    planes = np.concatenate([pay, pay + np.cumsum(sbytes, axis=1)], axis=1)
+    dst = [np.zeros((n, 1), dtype=np.int64)]
+    src = [np.full((n, 1), -1, dtype=np.int64)]
+    lens = [head]
+    if w == 3:
+        rp = np.array([lo.raw_plane for lo in layouts], dtype=np.int64)[:, None]
+        rlen = np.repeat(rp, P, axis=1)
+        rlen[:, -1:] = pay - head - (P - 1) * rp
+        dst.append(head + np.arange(P, dtype=np.int64)[None, :] * rp)
+        src.append(seg[:, :, 0])
+        lens.append(rlen)
+    dst.append(planes[:, :-1])
+    src.append(seg[:, :, w - 2])
+    lens.append(sbytes)
+    return np.concatenate(dst, axis=1), np.concatenate(src, axis=1), np.concatenate(lens, axis=1), planes
+
+
 def land_segments(slab, slot: SegmentSlot, batch, blocks: Optional[list] = None,
-                  dev_dst: Optional[Sequence[Optional[int]]] = None) -> List[HostContainer]:
+                  dev_dst: Optional[Sequence[Optional[int]]] = None, codec=CacheGenCodec) -> List[HostContainer]:
     """land() for a layer-wise store: container j is assembled in a fresh block of `slab` from its fixed-section image
-    and its 2L plane segments in the arena (one batched device->host copy of 1 + 2L ranges per container, all
-    containers in one call), and its plane offsets come from the segment sizes.  `dev_dst` as in land(): those
-    containers are assembled at their device address too, by the same batched copy.  Raises -- with every block freed
-    -- when a copy fails, the segments do not add up to the container's size, or a header carries an encoder error."""
+    and its segments in the arena (one batched device->host copy of the ranges segment_copy_ranges gives, all
+    containers in one call), its plane offsets come from the segment rows, and its header is checked by `codec`'s
+    parse_header.  `dev_dst` as in land(): those containers are assembled at their device address too, by the same
+    batched copy.  Raises -- with every block freed -- when a copy fails, the segments do not add up to the container's
+    size, or a header carries an encoder error."""
     if blocks is None:
         blocks = [slab.alloc(size) for size in batch.sizes]
-    n, P = len(blocks), slot.P        # P plane segments per container: 2L, or L for a latent KV
+    n, P, w = len(blocks), slot.P, slot.seg_row     # P planes per container: 2L, or L for a latent KV
     try:
         if n == 0:
             return []
-        seg = np.frombuffer(slot.seg.view(), dtype=np.int64, count=slot.n_chunks * P * 2)
-        seg = seg.reshape(slot.n_chunks, P, 2)[:n]
+        seg = np.frombuffer(slot.seg.view(), dtype=np.int64, count=slot.n_chunks * P * w)
+        seg = seg.reshape(slot.n_chunks, P, w)[:n]
         full, last = slot.layouts
-        fixed = np.array([last if j == slot.n_chunks - 1 else full for j in range(n)], dtype=np.int64)
-        planes = np.concatenate([fixed[:, None], fixed[:, None] + np.cumsum(seg[:, :, 1], axis=1)], axis=1)
+        dst, src, lens, planes = segment_copy_ranges(seg, [last if j == slot.n_chunks - 1 else full for j in range(n)])
         sizes = np.asarray([b.nbytes for b in blocks], dtype=np.int64)
-        if (seg[:, :, 0] < 0).any() or not np.array_equal(planes[:, -1], np.asarray(batch.sizes[:n], dtype=np.int64)):
+        if (src[:, 1:] < 0).any() or not np.array_equal(planes[:, -1], np.asarray(batch.sizes[:n], dtype=np.int64)):
             raise N.NativeError("layer-wise store: plane segments do not add up to the container sizes")
-        host = np.array([b.host_ptr for b in blocks], dtype=np.uint64)
-        dsts = np.concatenate([host[:, None], host[:, None] + planes[:, :-1].astype(np.uint64)], axis=1)
-        fbase = slot.fixed.data_ptr() + np.arange(n, dtype=np.uint64) * np.uint64(slot.fixed_stride)
-        srcs = np.concatenate([fbase[:, None], np.uint64(slot.arena.data_ptr()) + seg[:, :, 0].astype(np.uint64)], axis=1)
-        lens = np.concatenate([fixed[:, None], seg[:, :, 1]], axis=1)
         assert (lens.sum(axis=1) == sizes).all()
+        host = np.array([b.host_ptr for b in blocks], dtype=np.int64)
+        dsts = host[:, None] + dst
+        fbase = slot.fixed.data_ptr() + np.arange(n, dtype=np.int64) * slot.fixed_stride
+        srcs = np.where(src < 0, fbase[:, None], slot.arena.data_ptr() + src)
         resident = [j for j, ptr in enumerate(list(dev_dst or ())[:n]) if ptr is not None]
         if resident:
-            dptr = np.array([dev_dst[j] for j in resident], dtype=np.uint64)
-            ddst = np.concatenate([dptr[:, None], dptr[:, None] + planes[resident, :-1].astype(np.uint64)], axis=1)
-            dsts = np.concatenate([dsts, ddst])
+            dptr = np.array([dev_dst[j] for j in resident], dtype=np.int64)
+            dsts = np.concatenate([dsts, dptr[:, None] + dst[resident]])
             srcs = np.concatenate([srcs, srcs[resident]])
             lens = np.concatenate([lens, lens[resident]])
         dev = slot.arena.device
         cs = _d2h_stream(dev)
         with torch.cuda.device(dev):
             try:
-                _batch_copy(np.ascontiguousarray(dsts.ravel()), np.ascontiguousarray(srcs.ravel()),
-                            np.ascontiguousarray(lens.ravel()), cs)
+                _batch_copy(np.ascontiguousarray(dsts.ravel().astype(np.uint64)),
+                            np.ascontiguousarray(srcs.ravel().astype(np.uint64)), np.ascontiguousarray(lens.ravel()), cs)
             finally:
                 cs.synchronize()             # no block leaves this function while a copy may still write it
-        return [HostContainer(blk, blk.nbytes, parse_header(blk.view()), planes[j].copy()) for j, blk in enumerate(blocks)]
+        return [HostContainer(blk, blk.nbytes, codec.parse_header(blk.view()), planes[j].copy())
+                for j, blk in enumerate(blocks)]
     except BaseException:
         for blk in blocks:
             blk.free()

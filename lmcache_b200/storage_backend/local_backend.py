@@ -580,8 +580,14 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         return self.out_dtype() or dtype_of_code(rec.max_dtype)
 
     @property
+    def layerwise_store_blocking(self) -> bool:
+        """Does a layer-wise store's finish() return only once its containers have landed?  Not on a host tier: nothing
+        outside the tier sees an entry before it lands, and a retrieve of its keys waits for it."""
+        return False
+
+    @property
     def layerwise_max_tokens(self) -> int:
-        """the largest chunk a layer-major retrieve takes: one group per container"""
+        """the largest chunk a layer-major retrieve or a layer-wise store takes: one group per container"""
         return self.codec.layerwise_max_tokens
 
     # ------------------------------------------------------------------ retrieve
@@ -613,11 +619,12 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
 
     def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int):
         """A pipeline.LayerwiseEncode of tokens [tok_begin, T) of `view` (whose KV may not be written yet), or None
-        when this tier's containers for `chunk_size` are not version 3, or version 4 for a latent KV (the layer-wise
-        encode writes no other)."""
+        when this tier's containers for `chunk_size` are not ones a layer-wise encode writes: versions 3 and 4 (CacheGen,
+        chunks of at most 256 tokens), versions 5 and 6 (lossless, at most 4096)."""
         from lmcache_b200.pipeline import LayerwiseEncode, SegmentPool
         try:
-            if self.codec.coder_for(chunk_size, view.latent) not in (N.CODER_RANS_COMPACT, N.CODER_LATENT):
+            if self.codec.coder_for(chunk_size, view.latent) not in (N.CODER_RANS_COMPACT, N.CODER_LATENT,
+                                                                     N.CODER_LOSSLESS, N.CODER_LOSSLESS_LATENT):
                 return None
         except ValueError:
             return None
@@ -865,6 +872,14 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
         while self.capacity is not None and self._disk_bytes > self.capacity and self._evict_one(None):
             pass
         return len(self.dict)
+
+    @property
+    def layerwise_store_blocking(self) -> bool:
+        """On a lossless disk tier, yes: its layer-wise store replaced a blocking store() at finish(), and the directory
+        is read by other engines and by a restarted tier, so finish() keeps returning with the files in place (the
+        encode still runs layer by layer on the side stream).  A CacheGen disk tier's layer-wise store lands in the
+        background, as it always has."""
+        return self.lossless
 
     # the dict is keyed by file path: CacheEngineKey -> path is many-to-one ("/" and "-"), exactly as in the reference
     @property
