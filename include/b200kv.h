@@ -43,6 +43,7 @@ extern "C" {
                                     *    b200kv_lossless_decode (container versions 5 and 6), b200kv_lossless_plane_offsets /
                                     *    b200kv_lossless_plane_offsets_device / b200kv_lossless_decode_plan /
                                     *    b200kv_lossless_decode_layers (b200kv_lossless_decode_plan_t),
+                                    *    b200kv_lossless_decode_plan_heads,
                                     *    b200kv_lossless_encode_layers_workspace_bytes /
                                     *    b200kv_lossless_encode_layers_plan / b200kv_lossless_encode_layers /
                                     *    b200kv_lossless_encode_layers_finish (b200kv_lossless_encode_plan_t).
@@ -420,6 +421,30 @@ int b200kv_lossless_decode_plan(const void* containers, int64_t containers_bytes
                                 void* stream);
 int b200kv_lossless_decode_layers(const b200kv_lossless_decode_plan_t* plan, int32_t layer_begin, int32_t layer_end,
                                   void* stream);
+
+/*
+ * b200kv_lossless_decode_plan for a window of each container's KV heads, as b200kv_decode_plan_heads is for
+ * b200kv_decode_plan: decoding the lossless containers of another tensor-parallel layout into this rank's heads.
+ * Container j holds src_H heads (its header's L and D are dst's, its H is src_H; the workspace is
+ * b200kv_lossless_workspace_bytes(L, src_H, D, ..., decode = 1)).  Its heads [src_head0[j], src_head0[j] + n_heads[j])
+ * are decoded into destination heads [dst_head0[j], dst_head0[j] + n_heads[j]) at token dst_tok[j]; every other
+ * destination byte is left as it was.  The three arrays are HOST int32[n_chunks].  Containers may share a dst_tok when
+ * their destination head ranges do not overlap.  The result is an ordinary plan: b200kv_lossless_decode_layers runs it.
+ * The values are the bits the source layout stored: every (plane, channel) stream is independent, and the stream offsets
+ * come from the lengths section, which the plan sums whole.  Only the tiles of 128 streams that meet a window are
+ * launched; a thread whose channel lies outside its window reads its length only and writes nothing.  Status bits come
+ * from the header, the frequency rows of the planes decoded and the streams decoded: a damaged stream outside the window
+ * sets none (a damaged length before the window moves the window's offsets, and its streams then fail).  Refused,
+ * writing nothing and leaving status_out alone: n_heads[j] < 1, a window outside [0, src_H), a destination range outside
+ * [0, dst->H), overlapping destination ranges at one dst_tok, and a latent destination (version 6 has no heads).  As for
+ * the whole decode, dst's dtype must be the stored one.
+ */
+int b200kv_lossless_decode_plan_heads(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                                      const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok,
+                                      int32_t n_chunks, int32_t max_dtype, const b200kv_kv_desc* dst,
+                                      uint32_t* status_out, void* workspace, int64_t workspace_bytes,
+                                      b200kv_lossless_decode_plan_t* plan, void* stream, int32_t src_H,
+                                      const int32_t* src_head0, const int32_t* dst_head0, const int32_t* n_heads);
 
 /*
  * The lossless encode in three steps, as b200kv_encode_layers_plan / _layers / _finish for the CacheGen containers: a

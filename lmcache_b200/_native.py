@@ -137,6 +137,9 @@ SIGNATURES = {
     "b200kv_lossless_decode_plan": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, ctypes.POINTER(KvDesc),
                                              c_vp, c_vp, c_i64, ctypes.POINTER(LosslessDecodePlan), c_vp]),
     "b200kv_lossless_decode_layers": (c_i32, [ctypes.POINTER(LosslessDecodePlan), c_i32, c_i32, c_vp]),
+    "b200kv_lossless_decode_plan_heads": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32,
+                                                   ctypes.POINTER(KvDesc), c_vp, c_vp, c_i64,
+                                                   ctypes.POINTER(LosslessDecodePlan), c_vp, c_i32, c_vp, c_vp, c_vp]),
     "b200kv_lossless_encode_layers_workspace_bytes": (c_i64, [c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
     "b200kv_lossless_encode_layers_plan": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp,
                                                    c_i64, c_vp, c_vp, c_i32, c_vp, c_i64,

@@ -1127,25 +1127,51 @@ class LosslessCodec(_ContainerIO):
         """Decode containers that already sit in device memory at base_ptr + offsets[j] (asynchronous), as
         CacheGenCodec.decode_raw.  max_dtype is the stored element dtype, which must be dst's; coder names the version
         (N.CODER_LOSSLESS_LATENT: 6), which must match dst's latent-ness."""
+        self._decode_raw(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, stream, _locked)
+
+    def decode_raw_heads(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
+                         ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
+                         src_H: int, src_head0: Sequence[int], dst_head0: Sequence[int], n_heads: Sequence[int],
+                         stream: Optional[torch.cuda.Stream] = None) -> None:
+        """decode_raw for a window of each container's heads (b200kv_lossless_decode_plan_heads): every container holds
+        src_H heads, and its heads [src_head0[j], src_head0[j] + n_heads[j]) land in dst's heads from dst_head0[j] on, at
+        token dst_tok[j], bit for bit as the source layout stored them.  The rest of dst is left as it was."""
+        self._decode_raw(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, stream, False,
+                         (src_H, src_head0, dst_head0, n_heads))
+
+    @staticmethod
+    def _check_coder(coder: int, dst: KvView) -> None:
+        if coder not in (N.CODER_LOSSLESS, N.CODER_LOSSLESS_LATENT) or bool(coder & N.KV_LATENT) != dst.latent:
+            raise ValueError(f"coder {coder} does not name the lossless container of this destination")
+
+    def _decode_raw(self, base_ptr, buf_bytes, offsets, totals, ntokens, dst: KvView, dst_tok, max_dtype, coder, stream,
+                    _locked: bool, heads=None) -> None:
         n = len(offsets)
         if n == 0:
             return
-        if coder not in (N.CODER_LOSSLESS, N.CODER_LOSSLESS_LATENT) or bool(coder & N.KV_LATENT) != dst.latent:
-            raise ValueError(f"coder {coder} does not name the lossless container of this destination")
+        self._check_coder(coder, dst)
         lib = N.lib()
 
         def run():
             tstream = stream if stream is not None else torch.cuda.current_stream()
-            ws_bytes = max(lib.b200kv_lossless_workspace_bytes(dst.L, dst.H, dst.D, max(ntokens), n, int(dst.latent), 1),
+            ws_bytes = max(lib.b200kv_lossless_workspace_bytes(dst.L, int(heads[0]) if heads else dst.H, dst.D,
+                                                               max(ntokens), n, int(dst.latent), 1),
                            0)          # < 0: a shape the decode call refuses, with its reason
             if not _locked:
                 self._order_decode(tstream, 0, ws_bytes)
             self._dec_ws = self._grow(self._dec_ws, max(ws_bytes, 16), dst.device)
-            N.check(lib.b200kv_lossless_decode(base_ptr, int(buf_bytes), N.i64_array(list(offsets)),
-                                               N.i64_array(list(totals)), N.i32_array(list(ntokens)),
-                                               N.i64_array(list(dst_tok)), n, int(max_dtype), ctypes.byref(dst.desc),
-                                               self._status_buffer(n).dev_ptr, self._dec_ws.data_ptr(),
-                                               self._dec_ws.numel(), tstream.cuda_stream), "lossless_decode")
+            args = (base_ptr, int(buf_bytes), N.i64_array(list(offsets)), N.i64_array(list(totals)),
+                    N.i32_array(list(ntokens)), N.i64_array(list(dst_tok)), n, int(max_dtype), ctypes.byref(dst.desc),
+                    self._status_buffer(n).dev_ptr, self._dec_ws.data_ptr(), self._dec_ws.numel())
+            if heads is None:
+                N.check(lib.b200kv_lossless_decode(*args, tstream.cuda_stream), "lossless_decode")
+            else:
+                plan = N.LosslessDecodePlan()
+                N.check(lib.b200kv_lossless_decode_plan_heads(*args, ctypes.byref(plan), tstream.cuda_stream,
+                                                              int(heads[0]), N.i32_array(list(heads[1])),
+                                                              N.i32_array(list(heads[2])), N.i32_array(list(heads[3]))),
+                        "lossless_decode_plan_heads")
+                self.decode_layers(plan, 0, dst.L, tstream)
             if self._dec_event is None:
                 self._dec_event = torch.cuda.Event()
             self._dec_event.record(tstream)
@@ -1162,20 +1188,36 @@ class LosslessCodec(_ContainerIO):
         """CacheGenCodec.decode_plan for lossless containers (b200kv_lossless_decode_plan): enqueue on `stream` the
         kernels that read [0, off_raw) of every container and return (plan, workspace); decode_layers decodes a range of
         layers once its raw rows and streams are there.  The workspace is the caller's, recorded on `stream`."""
-        if coder not in (N.CODER_LOSSLESS, N.CODER_LOSSLESS_LATENT) or bool(coder & N.KV_LATENT) != dst.latent:
-            raise ValueError(f"coder {coder} does not name the lossless container of this destination")
+        return self._decode_plan(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, stream,
+                                 status_ptr)
+
+    def decode_plan_heads(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
+                          ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
+                          src_H: int, src_head0: Sequence[int], dst_head0: Sequence[int], n_heads: Sequence[int],
+                          stream: torch.cuda.Stream, status_ptr: int = 0) -> Tuple["N.LosslessDecodePlan", torch.Tensor]:
+        """decode_plan for head windows (see decode_raw_heads); decode_layers runs the plan."""
+        return self._decode_plan(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, stream,
+                                 status_ptr, (src_H, src_head0, dst_head0, n_heads))
+
+    def _decode_plan(self, base_ptr, buf_bytes, offsets, totals, ntokens, dst: KvView, dst_tok, max_dtype, coder, stream,
+                     status_ptr, heads=None) -> Tuple["N.LosslessDecodePlan", torch.Tensor]:
+        self._check_coder(coder, dst)
         n = len(offsets)
         lib = N.lib()
-        ws = torch.empty(max(lib.b200kv_lossless_workspace_bytes(dst.L, dst.H, dst.D, max(ntokens), n, int(dst.latent),
-                                                                 1), 16),
+        ws = torch.empty(max(lib.b200kv_lossless_workspace_bytes(dst.L, int(heads[0]) if heads else dst.H, dst.D,
+                                                                 max(ntokens), n, int(dst.latent), 1), 16),
                          dtype=torch.uint8, device=dst.device)    # < 0: a shape the plan call refuses, with its reason
         ws.record_stream(stream)
         plan = N.LosslessDecodePlan()
-        N.check(lib.b200kv_lossless_decode_plan(base_ptr, int(buf_bytes), N.i64_array(list(offsets)),
-                                                N.i64_array(list(totals)), N.i32_array(list(ntokens)),
-                                                N.i64_array(list(dst_tok)), n, int(max_dtype), ctypes.byref(dst.desc),
-                                                status_ptr or None, ws.data_ptr(), ws.numel(), ctypes.byref(plan),
-                                                stream.cuda_stream), "lossless_decode_plan")
+        args = (base_ptr, int(buf_bytes), N.i64_array(list(offsets)), N.i64_array(list(totals)),
+                N.i32_array(list(ntokens)), N.i64_array(list(dst_tok)), n, int(max_dtype), ctypes.byref(dst.desc),
+                status_ptr or None, ws.data_ptr(), ws.numel(), ctypes.byref(plan), stream.cuda_stream)
+        if heads is None:
+            N.check(lib.b200kv_lossless_decode_plan(*args), "lossless_decode_plan")
+        else:
+            N.check(lib.b200kv_lossless_decode_plan_heads(*args, int(heads[0]), N.i32_array(list(heads[1])),
+                                                          N.i32_array(list(heads[2])), N.i32_array(list(heads[3]))),
+                    "lossless_decode_plan_heads")
         return plan, ws
 
     @staticmethod

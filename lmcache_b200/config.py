@@ -51,13 +51,19 @@ class LMCacheEngineConfig:
     device_cache_bytes: Optional[int] = None
     # not in the reference: other tensor-parallel world sizes whose stored chunks a retrieve may decode into this rank's
     # KV heads once its own layout's prefix ends (lmcache_b200/reshard.py), tried in this order.  None = off.  Needs a
-    # remote tier with the CacheGen serde (CreateStorageBackend); must not hold the engine's own world size (LMCacheEngine).
+    # remote tier with the CacheGen serde, or with the lossless serde and reshard_lossless (CreateStorageBackend).  Must
+    # not hold the engine's own world size (LMCacheEngine).
     reshard_world_sizes: Optional[List[int]] = None
     # not in the reference as a key (it is the reference's nine-field CacheGenConfig): the CacheGen bin layout of a model
     # outside the five-name table of CacheGenConfig.from_model_name, e.g. a 70B model's 80 layers.  A mapping of exactly
     # the nine fields; None = the table.  When set, the engine's CacheGen tiers and serdes use it for any model name, and
     # write and read version-3 containers only -- the one version that records the bins (chunk_size <= 256).
     cachegen_config: Optional[Dict[str, int]] = None
+    # not in the reference: with remote_serde "lossless", let reshard_world_sizes decode other layouts' lossless
+    # containers (b200kv_lossless_decode_plan_heads): this rank's heads come back bit for bit as it would have stored them.
+    # False = a lossless remote tier refuses reshard_world_sizes, as it did before the key existed; True needs
+    # reshard_world_sizes and remote_serde "lossless", and every layout named there must store lossless containers too.
+    reshard_lossless: bool = False
 
     def __post_init__(self):
         if self.local_serde is None:
@@ -79,6 +85,11 @@ class LMCacheEngineConfig:
             self.reshard_world_sizes = list(r)
         if self.cachegen_config is not None:
             self.cachegen_config = check_cachegen_config(self.cachegen_config)
+        if not isinstance(self.reshard_lossless, bool):
+            raise ValueError(f"Invalid reshard_lossless: {self.reshard_lossless!r} (True or False)")
+        if self.reshard_lossless and (self.reshard_world_sizes is None or self.remote_serde != "lossless"):
+            raise ValueError("reshard_lossless needs reshard_world_sizes and remote_serde='lossless', not "
+                             f"reshard_world_sizes={self.reshard_world_sizes!r} with remote_serde={self.remote_serde!r}")
 
     @staticmethod
     def from_defaults(chunk_size: int = 256, local_device: str = "cuda",
@@ -88,10 +99,11 @@ class LMCacheEngineConfig:
                       local_capacity_bytes: Optional[int] = None,
                       device_cache_bytes: Optional[int] = None,
                       reshard_world_sizes: Optional[List[int]] = None,
-                      cachegen_config: Optional[Dict[str, int]] = None) -> "LMCacheEngineConfig":
+                      cachegen_config: Optional[Dict[str, int]] = None,
+                      reshard_lossless: bool = False) -> "LMCacheEngineConfig":
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
                                    save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes,
-                                   reshard_world_sizes, cachegen_config)
+                                   reshard_world_sizes, cachegen_config, reshard_lossless)
 
     @staticmethod
     def from_legacy(chunk_size: int = 256, backend: str = "cuda", persist_path: Optional[str] = None,
@@ -100,7 +112,8 @@ class LMCacheEngineConfig:
                     local_capacity_bytes: Optional[int] = None,
                     device_cache_bytes: Optional[int] = None,
                     reshard_world_sizes: Optional[List[int]] = None,
-                    cachegen_config: Optional[Dict[str, int]] = None) -> "LMCacheEngineConfig":
+                    cachegen_config: Optional[Dict[str, int]] = None,
+                    reshard_lossless: bool = False) -> "LMCacheEngineConfig":
         """backend: "cpu" | "cuda" | "file://<dir>/" | "<scheme>://<host>:<port>" (config.py:51-82)."""
         local_device: Optional[str] = None
         remote_url: Optional[str] = None
@@ -112,7 +125,7 @@ class LMCacheEngineConfig:
             remote_url = backend
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
                                    save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes,
-                                   reshard_world_sizes, cachegen_config)
+                                   reshard_world_sizes, cachegen_config, reshard_lossless)
 
     @staticmethod
     def from_file(file_path: str) -> "LMCacheEngineConfig":
@@ -130,6 +143,7 @@ class LMCacheEngineConfig:
         device_cache_bytes = cfg.get("device_cache_bytes", None)
         reshard_world_sizes = cfg.get("reshard_world_sizes", None)
         cachegen_config = cfg.get("cachegen_config", None)
+        reshard_lossless = cfg.get("reshard_lossless", False)
 
         if local_device in ("cpu", "cuda", None):
             pass
@@ -143,7 +157,7 @@ class LMCacheEngineConfig:
 
         return LMCacheEngineConfig(chunk_size, local_device, remote_url, remote_serde, pipelined_backend,
                                    save_decode_cache, local_serde, local_capacity_bytes, device_cache_bytes,
-                                   reshard_world_sizes, cachegen_config)
+                                   reshard_world_sizes, cachegen_config, reshard_lossless)
 
 
 CACHEGEN_CONFIG_FIELDS = ("key_first_layers", "key_second_layers", "key_third_layers", "key_first_bins",

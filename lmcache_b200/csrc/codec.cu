@@ -2195,44 +2195,17 @@ static int decode_plan_impl(const void* containers, int64_t containers_bytes, co
     B2_REQUIRE(containers && offsets && total_bytes && ntokens && dst_tok && n_chunks > 0, "bad chunk arrays");
     B2_REQUIRE(max_dtype == B200KV_DT_BF16 || max_dtype == B200KV_DT_FP16, "bad max_dtype");
     B2_REQUIRE(dst->sT > 0 && dst->sT < (1ll << 23), "destination token stride out of range");
-    const bool windows = src_head0 != nullptr;
-    B2_REQUIRE(!windows || !latent, "head windows need a (K, V) destination: a latent KV has no heads to split");
-    if (windows) {
-        B2_REQUIRE(dst_head0 != nullptr && n_heads != nullptr, "head window arrays are NULL");
-        B2_REQUIRE(src_H > 0 && (int64_t)src_H * dst->D < (1ll << 24), "src_H out of range");
-    } else {
-        src_H = dst->H;
-    }
+    if (src_head0 == nullptr) src_H = dst->H;
+    std::vector<HeadWindow> win;
+    if (int rc = plan_head_windows(n_chunks, dst_tok, latent, dst->H, dst->D, src_H, src_head0, dst_head0, n_heads, CT,
+                                   &win, &P.wtpp))
+        return rc;
     P.sT = dst->sT; P.sH = dst->sH;
     P.slot_map = dst->slot_map;
     P.L = dst->L; P.H = src_H; P.D = dst->D; P.C = src_H * dst->D;
     P.out_dtype = kv_dtype(dst); P.max_dtype = max_dtype; P.n_chunks = n_chunks;
     P.tpp = tiles_per_plane(P.C);
-    P.wtpp = P.tpp;
     P.lb = 0; P.nlay = P.L;
-    if (windows) {
-        int wt = 1;
-        for (int j = 0; j < n_chunks; ++j) {
-            B2_REQUIRE(n_heads[j] >= 1, "a head window must hold at least one head");
-            B2_REQUIRE(src_head0[j] >= 0 && src_head0[j] <= src_H - n_heads[j], "head window outside the container's heads");
-            B2_REQUIRE(dst_head0[j] >= 0 && dst_head0[j] <= dst->H - n_heads[j],
-                       "head window outside the destination's heads");
-            const int c0 = src_head0[j] * P.D, c1 = (src_head0[j] + n_heads[j]) * P.D;
-            wt = std::max(wt, (c1 - 1) / CT - c0 / CT + 1);
-        }
-        // containers that share a destination token must not share a destination head
-        std::vector<int> ord((size_t)n_chunks);
-        for (int j = 0; j < n_chunks; ++j) ord[(size_t)j] = j;
-        std::sort(ord.begin(), ord.end(), [&](int a, int b) {
-            return dst_tok[a] != dst_tok[b] ? dst_tok[a] < dst_tok[b] : dst_head0[a] < dst_head0[b];
-        });
-        for (size_t k = 1; k < ord.size(); ++k) {
-            const int a = ord[k - 1], b = ord[k];
-            B2_REQUIRE(dst_tok[a] != dst_tok[b] || dst_head0[a] + n_heads[a] <= dst_head0[b],
-                       "head windows overlap at the same destination token");
-        }
-        P.wtpp = wt;
-    }
     int tmax = 0;
     for (int j = 0; j < n_chunks; ++j) {
         B2_REQUIRE(ntokens[j] > 0, "ntokens must be positive");
@@ -2284,11 +2257,12 @@ static int decode_plan_impl(const void* containers, int64_t containers_bytes, co
             hc[j].ngroups = (ntokens[j] + kGroup - 1) / kGroup;
             const Layout lj = make_layout(P.L, P.C, ntokens[j], P.compact, P.ppl);
             hc[j].payload_bytes = (uint32_t)(total_bytes[j] - lj.off_payload);
-            hc[j].cw0 = windows ? src_head0[j] * P.D : 0;
-            hc[j].cw1 = windows ? (src_head0[j] + n_heads[j]) * P.D : P.C;
-            hc[j].dshift = windows ? (dst_head0[j] - src_head0[j]) * P.D : 0;
-            hc[j].ct0 = hc[j].cw0 / CT;
-            hc[j].ntw = (hc[j].cw1 - 1) / CT - hc[j].ct0 + 1;
+            const HeadWindow& w = win[(size_t)j];
+            hc[j].cw0 = w.cw0;
+            hc[j].cw1 = w.cw1;
+            hc[j].dshift = w.dshift;
+            hc[j].ct0 = w.ct0;
+            hc[j].ntw = w.ntw;
         }
         cudaError_t e = cudaMemcpyAsync(ws, hc, sizeof(DecChunk) * (size_t)n_chunks, cudaMemcpyHostToDevice, stream);
         free(hc);

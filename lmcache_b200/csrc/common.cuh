@@ -4,7 +4,9 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <algorithm>
 #include <string>
+#include <vector>
 
 #include "../../include/b200kv.h"
 
@@ -54,6 +56,60 @@ template <bool PAGED>
 __device__ __forceinline__ int64_t tok_row(const int64_t* slot_map, int64_t tok) {
     if constexpr (PAGED) return __ldg(slot_map + tok);
     else return tok;
+}
+
+// The head window of one container in a decode plan (b200kv_decode_plan_heads, b200kv_lossless_decode_plan_heads; the
+// whole container otherwise): container channels [cw0, cw1) are decoded into destination channel c + dshift; they lie in
+// tiles [ct0, ct0 + ntw) of CT channels of every plane.
+struct HeadWindow {
+    int32_t ct0, ntw, cw0, cw1, dshift;
+};
+
+// The head windows of a decode plan's n_chunks containers of src_H heads of D channels, and in *wtpp the largest ntw
+// (the tiles a decode launches per plane).  With src_head0 != NULL, container j's heads [src_head0[j], src_head0[j] +
+// n_heads[j]) land in the destination's heads from dst_head0[j] on.  Refused (nothing written): a latent destination
+// (no heads to split), NULL window arrays, src_H out of range, an empty window, one outside the container's heads or
+// the destination's dst_H heads, and two containers at one destination token that share a destination head.
+// src_head0 == NULL: every container whole, [0, src_H * D) with no shift.  Returns 0, or -2 with the error set.
+inline int plan_head_windows(int32_t n_chunks, const int64_t* dst_tok, bool latent, int32_t dst_H, int32_t D,
+                             int32_t src_H, const int32_t* src_head0, const int32_t* dst_head0, const int32_t* n_heads,
+                             int CT, std::vector<HeadWindow>* win, int32_t* wtpp) {
+    const bool windows = src_head0 != nullptr;
+    B2_REQUIRE(!windows || !latent, "head windows need a (K, V) destination: a latent KV has no heads to split");
+    if (windows) {
+        B2_REQUIRE(dst_head0 != nullptr && n_heads != nullptr, "head window arrays are NULL");
+        B2_REQUIRE(src_H > 0 && (int64_t)src_H * D < (1ll << 24), "src_H out of range");
+        for (int j = 0; j < n_chunks; ++j) {
+            B2_REQUIRE(n_heads[j] >= 1, "a head window must hold at least one head");
+            B2_REQUIRE(src_head0[j] >= 0 && src_head0[j] <= src_H - n_heads[j], "head window outside the container's heads");
+            B2_REQUIRE(dst_head0[j] >= 0 && dst_head0[j] <= dst_H - n_heads[j],
+                       "head window outside the destination's heads");
+        }
+        // containers that share a destination token must not share a destination head
+        std::vector<int> ord((size_t)n_chunks);
+        for (int j = 0; j < n_chunks; ++j) ord[(size_t)j] = j;
+        std::sort(ord.begin(), ord.end(), [&](int a, int b) {
+            return dst_tok[a] != dst_tok[b] ? dst_tok[a] < dst_tok[b] : dst_head0[a] < dst_head0[b];
+        });
+        for (size_t k = 1; k < ord.size(); ++k) {
+            const int a = ord[k - 1], b = ord[k];
+            B2_REQUIRE(dst_tok[a] != dst_tok[b] || dst_head0[a] + n_heads[a] <= dst_head0[b],
+                       "head windows overlap at the same destination token");
+        }
+    }
+    win->resize((size_t)n_chunks);
+    int32_t wt = windows ? 1 : (int32_t)(((int64_t)src_H * D + CT - 1) / CT);
+    for (int j = 0; j < n_chunks; ++j) {
+        HeadWindow& w = (*win)[(size_t)j];
+        w.cw0 = windows ? src_head0[j] * D : 0;
+        w.cw1 = windows ? (src_head0[j] + n_heads[j]) * D : src_H * D;
+        w.dshift = windows ? (dst_head0[j] - src_head0[j]) * D : 0;
+        w.ct0 = w.cw0 / CT;
+        w.ntw = (w.cw1 - 1) / CT - w.ct0 + 1;
+        wt = std::max(wt, w.ntw);
+    }
+    *wtpp = wt;
+    return 0;
 }
 
 // A set of layers [0, B200KV_MAX_PLANES / 2): bit l % 64 of word l / 64.  The layer-wise encode plans (CacheGen and

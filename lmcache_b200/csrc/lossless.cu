@@ -92,14 +92,18 @@ struct LlDecChunk {
     const uint8_t* base;
     int64_t dst_tok;
     int64_t payload_bytes;               // total_bytes - off_payload, from the caller: every stream must lie inside
-    int32_t t, pad;
+    int32_t t;
+    // head window (b200kv_lossless_decode_plan_heads; the whole container otherwise): container channels [cw0, cw1) are
+    // decoded into destination channel c + dshift; they lie in tiles [ct0, ct0 + ntw) of every plane
+    int32_t ct0, ntw, cw0, cw1, dshift;
 };
 
 struct LlDec {
     PlaneTable pt;                       // destination planes (maxq unused)
     int64_t sT, sH;
     const int64_t* slot_map;
-    int32_t L, H, D, C, NP, tpp, ntiles, dtype, version, n_chunks;
+    int32_t L, H, D, C, NP, tpp, ntiles, dtype, version, n_chunks;   // H, C: the containers' (src_H with windows)
+    int32_t wtpp;                        // tiles launched per plane: the largest window's ntw (tpp without windows)
     int32_t lb, nl;                      // the launch decodes layers [lb, lb + nl): blockIdx.y < nl keys, then values
     const LlDecChunk* chunks;
     unsigned long long* tile;            // [n][ntiles]
@@ -490,14 +494,20 @@ __global__ void __launch_bounds__(1024) ll_dec_scan_kernel(LlDec P) {
 // A launch covers the planes of layers [lb, lb + nl) only (b200kv_lossless_decode_layers): it reads the header, those
 // planes' frequency rows, the lengths section (through the tile offsets the plan computed from it), those planes' raw
 // rows and those planes' streams, and nothing else of the container.
+// With a head window (b200kv_lossless_decode_plan_heads) CTA x of a plane is tile ct0 + x of the container, and CTAs
+// past the window's ntw leave.  Every thread of a tile still reads its length and joins the scan, because a stream's
+// offset depends on the lengths before it in the tile, but only the channels [cw0, cw1) decode, into destination
+// channel c + dshift, and only they can set status bits: a damaged stream outside the window is never read.
 template <bool PAGED>
 __global__ void __launch_bounds__(kCT) ll_decode_kernel(LlDec P) {
     __shared__ uint32_t s_ent[kSyms];
     __shared__ uint8_t s_sym[kM];
     __shared__ uint32_t s_w[kCT / 32];
-    const int j = blockIdx.z, tile = blockIdx.x;
+    const int j = blockIdx.z;
     const int p = (int)blockIdx.y < P.nl ? P.lb + (int)blockIdx.y : P.L + P.lb + ((int)blockIdx.y - P.nl);
     const LlDecChunk dc = P.chunks[j];
+    if ((int)blockIdx.x >= dc.ntw) return;
+    const int tile = dc.ct0 + (int)blockIdx.x;
     const int t = dc.t;
     const LlLayout lo = ll_layout(P.NP, P.C, t);
     uint32_t bad = 0u;
@@ -533,7 +543,7 @@ __global__ void __launch_bounds__(kCT) ll_decode_kernel(LlDec P) {
     const uint32_t len = on ? reinterpret_cast<const uint16_t*>(dc.base + lo.off_lens)[(int64_t)p * P.C + c] : 0u;
     uint32_t tot;
     const uint32_t ex = cta_excl_scan<kCT>(len, s_w, &tot);
-    if (on) {
+    if (on && c >= dc.cw0 && c < dc.cw1) {
         const unsigned long long off = P.tile[(int64_t)j * P.ntiles + (int64_t)p * P.tpp + tile] + ex;
         if (off + len > (unsigned long long)dc.payload_bytes) {
             bad |= 2u;
@@ -545,7 +555,8 @@ __global__ void __launch_bounds__(kCT) ll_decode_kernel(LlDec P) {
             const uint16_t* wp = sp + 2;
             const uint32_t nw = (len - 4u) >> 1;
             uint32_t k = 0u;
-            const int h = c / P.D, d = c - h * P.D;
+            const int oc = c + dc.dshift;                // destination channel
+            const int h = oc / P.D, d = oc - h * P.D;
             uint16_t* dst = const_cast<uint16_t*>(P.pt.p[p]) + (int64_t)h * P.sH + d;
             const uint8_t* raw = dc.base + lo.off_raw + (int64_t)p * t * P.C + c;
 #pragma unroll 4
@@ -807,12 +818,14 @@ int b200kv_lossless_plane_offsets_device(const void* containers, int64_t stride,
     return 0;
 }
 
-int b200kv_lossless_decode_plan(const void* containers, int64_t containers_bytes, const int64_t* offsets,
-                                const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok,
-                                int32_t n_chunks, int32_t max_dtype, const b200kv_kv_desc* dst, uint32_t* status_out,
-                                void* workspace, int64_t workspace_bytes, b200kv_lossless_decode_plan_t* plan_out,
-                                void* stream_) {
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+// b200kv_lossless_decode_plan and b200kv_lossless_decode_plan_heads: src_head0 == NULL decodes every container whole
+// (src_H = dst->H)
+static int ll_decode_plan_impl(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                               const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok,
+                               int32_t n_chunks, int32_t max_dtype, const b200kv_kv_desc* dst, uint32_t* status_out,
+                               void* workspace, int64_t workspace_bytes, b200kv_lossless_decode_plan_t* plan_out,
+                               cudaStream_t stream, int32_t src_H, const int32_t* src_head0, const int32_t* dst_head0,
+                               const int32_t* n_heads) {
     B2_REQUIRE(plan_out != nullptr, "plan is NULL");
     LlPlan* plan = reinterpret_cast<LlPlan*>(plan_out);
     plan->magic = 0u;
@@ -824,8 +837,13 @@ int b200kv_lossless_decode_plan(const void* containers, int64_t containers_bytes
     B2_REQUIRE(kv_dtype(dst) == max_dtype,
                "the destination's dtype is not the stored one: a lossless container is decoded into its own dtype only");
     B2_REQUIRE(shape_ok(dst->L, dst->H, dst->D, 1), "bad destination shape");
+    if (src_head0 == nullptr) src_H = dst->H;
+    std::vector<HeadWindow> win;
+    if (int rc = plan_head_windows(n_chunks, dst_tok, kv_ppl(dst) == 1, dst->H, dst->D, src_H, src_head0, dst_head0,
+                                   n_heads, kCT, &win, &P.wtpp))
+        return rc;
     P.NP = kv_ppl(dst) * dst->L;
-    P.L = dst->L; P.H = dst->H; P.D = dst->D; P.C = dst->H * dst->D;
+    P.L = dst->L; P.H = src_H; P.D = dst->D; P.C = src_H * dst->D;
     P.dtype = max_dtype;
     P.version = kv_ppl(dst) == 1 ? 6 : 5;
     P.sT = dst->sT; P.sH = dst->sH;
@@ -853,7 +871,12 @@ int b200kv_lossless_decode_plan(const void* containers, int64_t containers_bytes
             hc[j].dst_tok = dst_tok[j];
             hc[j].payload_bytes = total_bytes[j] - ll_layout(P.NP, P.C, ntokens[j]).off_payload;
             hc[j].t = ntokens[j];
-            hc[j].pad = 0;
+            const HeadWindow& w = win[(size_t)j];
+            hc[j].ct0 = w.ct0;
+            hc[j].ntw = w.ntw;
+            hc[j].cw0 = w.cw0;
+            hc[j].cw1 = w.cw1;
+            hc[j].dshift = w.dshift;
         }
         cudaError_t e = cudaMemcpyAsync(ws, hc, sizeof(LlDecChunk) * (size_t)n_chunks, cudaMemcpyHostToDevice, stream);
         free(hc);
@@ -871,6 +894,29 @@ int b200kv_lossless_decode_plan(const void* containers, int64_t containers_bytes
     return 0;
 }
 
+int b200kv_lossless_decode_plan(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                                const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok,
+                                int32_t n_chunks, int32_t max_dtype, const b200kv_kv_desc* dst, uint32_t* status_out,
+                                void* workspace, int64_t workspace_bytes, b200kv_lossless_decode_plan_t* plan_out,
+                                void* stream) {
+    return ll_decode_plan_impl(containers, containers_bytes, offsets, total_bytes, ntokens, dst_tok, n_chunks, max_dtype,
+                               dst, status_out, workspace, workspace_bytes, plan_out, static_cast<cudaStream_t>(stream), 0,
+                               nullptr, nullptr, nullptr);
+}
+
+int b200kv_lossless_decode_plan_heads(const void* containers, int64_t containers_bytes, const int64_t* offsets,
+                                      const int64_t* total_bytes, const int32_t* ntokens, const int64_t* dst_tok,
+                                      int32_t n_chunks, int32_t max_dtype, const b200kv_kv_desc* dst,
+                                      uint32_t* status_out, void* workspace, int64_t workspace_bytes,
+                                      b200kv_lossless_decode_plan_t* plan_out, void* stream, int32_t src_H,
+                                      const int32_t* src_head0, const int32_t* dst_head0, const int32_t* n_heads) {
+    if (plan_out != nullptr) reinterpret_cast<LlPlan*>(plan_out)->magic = 0u;
+    B2_REQUIRE(src_head0 != nullptr, "head window arrays are NULL");
+    return ll_decode_plan_impl(containers, containers_bytes, offsets, total_bytes, ntokens, dst_tok, n_chunks, max_dtype,
+                               dst, status_out, workspace, workspace_bytes, plan_out, static_cast<cudaStream_t>(stream),
+                               src_H, src_head0, dst_head0, n_heads);
+}
+
 int b200kv_lossless_decode_layers(const b200kv_lossless_decode_plan_t* plan_in, int32_t layer_begin, int32_t layer_end,
                                   void* stream_) {
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -882,7 +928,7 @@ int b200kv_lossless_decode_layers(const b200kv_lossless_decode_plan_t* plan_in, 
     P.lb = layer_begin;
     P.nl = layer_end - layer_begin;
     const int ppl = P.NP / P.L;
-    const dim3 g((unsigned)P.tpp, (unsigned)(ppl * P.nl), (unsigned)P.n_chunks);
+    const dim3 g((unsigned)P.wtpp, (unsigned)(ppl * P.nl), (unsigned)P.n_chunks);
     if (P.slot_map) ll_decode_kernel<true><<<g, kCT, 0, stream>>>(P);
     else ll_decode_kernel<false><<<g, kCT, 0, stream>>>(P);
     B2_CHECK_CUDA(cudaGetLastError());

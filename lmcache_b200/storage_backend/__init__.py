@@ -29,10 +29,12 @@ def CreateStorageBackend(config: LMCacheEngineConfig, metadata: LMCacheEngineMet
         from lmcache_b200.storage_backend.serde.lossless import _check_chunk_size
         _check_chunk_size(config)
     if config.reshard_world_sizes is not None:
-        # another layout's chunks exist only on a shared remote tier, and only CacheGen containers can be decoded a
-        # window of heads at a time
-        if remote is None or config.remote_serde != "cachegen":
-            raise ValueError("reshard_world_sizes needs a remote tier with remote_serde='cachegen', not "
+        # another layout's chunks exist only on a shared remote tier, and only containers can be decoded a window of
+        # heads at a time: CacheGen ones, or lossless ones when the configuration opts in (reshard_lossless)
+        lossless = config.remote_serde == "lossless" and config.reshard_lossless
+        if remote is None or not (config.remote_serde == "cachegen" or lossless):
+            raise ValueError("reshard_world_sizes needs a remote tier with remote_serde='cachegen', or with "
+                             "remote_serde='lossless' and reshard_lossless=True, not "
                              f"remote_url={remote!r} with remote_serde={config.remote_serde!r}")
     if local is None and isinstance(remote, str):
         from lmcache_b200.storage_backend.remote_backend import LMCPipelinedRemoteBackend, LMCRemoteBackend

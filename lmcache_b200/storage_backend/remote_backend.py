@@ -329,7 +329,7 @@ class LMCRemoteBackend(LMCBackendInterface):
         source containers and the window of each that makes up this rank's heads (the same windows for every chunk).
         They are fetched over the striped connections and decoded into `dst` (chunk i at token dst_tok0 + i *
         chunk_size) up to the first chunk that is incomplete.  Returns the number of whole chunks served; with `stats`,
-        stats["bytes"] grows by the container bytes of those chunks.  CacheGen serde only; nothing is kept."""
+        stats["bytes"] grows by the container bytes of those chunks.  CacheGen and lossless serdes; nothing is kept."""
         if not (len(groups) and self._striped()):
             return 0
         return self._get_striped_groups(groups, [w for _, w in groups[0]], dst, dst_tok0, chunk_size, stats)

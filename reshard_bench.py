@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """reshard_bench.py -- what a retrieve across tensor-parallel layouts costs against the ordinary one, on one GPU.
 
-  python reshard_bench.py [--steps K] [--warmup W] [--tokens 8192]
+  python reshard_bench.py [--steps K] [--warmup W] [--tokens 8192] [--serde cachegen|lossless]
 
 Workload: a 32-layer / 8-KV-head / 128-dim model in bf16 (Llama-3-8B-shaped, Mistral-7B's bin table), chunks of 256
 tokens, synthetic KV (SURVEY 8d: log-normal channel scales, 1 % outlier channels).  1, 2, 4 and 8 all divide the 8 KV
@@ -18,6 +18,11 @@ Per leg: the median wall clock of retrieve() (host clock around the call and a d
 fetched, and the decode kernel time (CUDA events, median of repeated calls on device-resident containers) of the leg's
 decode against a whole decode of the same containers.  Every resharded result is checked bit for bit against the
 source layout's own retrieve.  Prints one JSON line with the GPU's name and power limit.  Writes nothing into the tree.
+
+--serde lossless runs the same legs with remote_serde "lossless" and reshard_lossless (container version 5): the
+containers are then the KV's own bits, and every resharded result is also checked bit for bit against the original
+KV's heads of the retrieving rank.  The JSON line then carries "serde": "lossless"; the default (cachegen) prints
+what it always printed.
 """
 import argparse
 import ctypes
@@ -49,6 +54,7 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--tokens", type=int, default=8192)
+    ap.add_argument("--serde", choices=("cachegen", "lossless"), default="cachegen")
     args = ap.parse_args()
     import torch
 
@@ -78,7 +84,8 @@ def main():
         seqs = {W: torch.randint(0, 32000, (T,), device=dev, generator=g) for W in (1, 2, 4)}
 
         def engine(W, r, reshard=None):
-            cfg = LMCacheEngineConfig(CS, None, url, "cachegen", False, False, reshard_world_sizes=reshard)
+            cfg = LMCacheEngineConfig(CS, None, url, args.serde, False, False, reshard_world_sizes=reshard,
+                                      reshard_lossless=reshard is not None and args.serde == "lossless")
             e = LMCacheEngine(cfg, LMCacheEngineMetadata(MODEL, W, r, "vllm", "bfloat16"))
             engines.append(e)
             return e
@@ -134,6 +141,10 @@ def main():
                 for x in range(2):
                     want = torch.cat([p[l][x] for p in parts], dim=1)
                     assert torch.equal(got[l][x].view(torch.int16), want.view(torch.int16)), f"{name} differs"
+                    if args.serde == "lossless":        # and the bits this rank's heads had before any store
+                        a, b = rd * HG // Wd, (rd + 1) * HG // Wd
+                        assert torch.equal(got[l][x].view(torch.int16), kv[l, x, :, a:b].view(torch.int16)), \
+                            f"{name} differs from the original KV"
 
         # decode kernel time of each leg's decode against a whole decode of the same containers
         codec = retr["own1"].engine_.deserializer.codec
@@ -157,7 +168,8 @@ def main():
             raw = b"".join(blobs) + b"\0" * N.READ_SLACK
             buf = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev)
             hd = N.Header.from_buffer_copy(raw[:N.HEADER_BYTES])
-            md, cd = int(hd.max_dtype), int(hd.version) - 1
+            md = int(hd.max_dtype)
+            cd = int(hd.version) - 1 if args.serde == "cachegen" else codec.coder_for(CS)
             win = torch.empty((L, 2, T, HG // Wd, D), dtype=torch.bfloat16, device=dev)
             whole = torch.empty((L, 2, T, hs, D), dtype=torch.bfloat16, device=dev)
             vw, vf = KvView.from_blob(win, "vllm"), KvView.from_blob(whole, "vllm")
@@ -187,6 +199,8 @@ def main():
         result = {"metric": "reshard_retrieve_ms", "tokens": T, "layers": L, "kv_heads": HG, "head_dim": D,
                   "chunk": CS, "steps": args.steps, "warmup": args.warmup, "gpu": torch.cuda.get_device_name(dev),
                   "power_limit": _power_limit(), "legs": {}}
+        if args.serde != "cachegen":
+            result["serde"] = args.serde
         for name, (Wd, rd, W, rs) in legs.items():
             k_win, k_full, fetched = kernel_ms(W, Wd, rd)         # the leg fetches every container it decodes
             leg = {"retrieve_ms_median": round(statistics.median(runs[name]), 3),
