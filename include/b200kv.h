@@ -46,7 +46,9 @@ extern "C" {
                                     *    b200kv_lossless_decode_plan_heads,
                                     *    b200kv_lossless_encode_layers_workspace_bytes /
                                     *    b200kv_lossless_encode_layers_plan / b200kv_lossless_encode_layers /
-                                    *    b200kv_lossless_encode_layers_finish (b200kv_lossless_encode_plan_t).
+                                    *    b200kv_lossless_encode_layers_finish (b200kv_lossless_encode_plan_t),
+                                    *    b200kv_lm_open_begin / b200kv_lm_read_ranges / b200kv_lm_close_handles,
+                                    *    b200kv_lm_server_num_handles.
                                     *    B200KV_MAX_PLANES went from 128 to 256 (models of up to 128 layers): the row
                                     *    width of b200kv_plane_offsets_device, B200KV_MAX_PLANES + 1, and the size of
                                     *    b200kv_encode_plan_t, 256 -> 512 words, changed with it; a caller takes them
@@ -588,6 +590,23 @@ int b200kv_lm_exists(void* conn, const char* key);                              
 int64_t b200kv_lm_get_begin(void* conn, const char* key);
 int64_t b200kv_lm_list_begin(void* conn);                                           /* keys joined by '\n' */
 int b200kv_lm_read(void* conn, void* dst, int64_t len);
+/* Ranged reads of stored values (this project's servers only: send them after b200kv_lm_exists(conn, "b200kv-ranges-v1")
+ * returned 1; the reference server answers 0, and it ignores an unknown command without a reply, so a client that sent
+ * one would wait forever).  A handle holds the
+ * value as it was at OPEN -- a later PUT of the key does not change what READ returns -- and lives until CLOSE or the
+ * end of the connection; a server keeps at most 4096 per connection.
+ *   n = b200kv_lm_open_begin(conn, key, prefix, &handle, &size)   n = min(prefix, size) bytes pending, -1 = miss or
+ *                                                                    the handle cap, < -1 = error; then
+ *   b200kv_lm_read(conn, dst, n)                                   the value's first n bytes into caller memory
+ *   b200kv_lm_read_ranges(conn, m, handles, offsets, sizes, dst)   range i of handle i into dst[i]; sum of sizes < 2^31;
+ *                                                                    0 = done, 1 = refused (unknown handle or a range
+ *                                                                    out of bounds; nothing written), < 0 = error
+ *   b200kv_lm_close_handles(conn, m, handles)                      unknown handles are ignored */
+int64_t b200kv_lm_open_begin(void* conn, const char* key, int64_t prefix, uint32_t* handle, int64_t* size);
+int b200kv_lm_read_ranges(void* conn, int32_t m, const uint32_t* handles, const uint64_t* offsets, const uint64_t* sizes,
+                          void* const* dst);
+int b200kv_lm_close_handles(void* conn, int32_t m, const uint32_t* handles);
+int64_t b200kv_lm_server_num_handles(void* server);                                 /* open handles, all connections */
 
 #ifdef __cplusplus
 }

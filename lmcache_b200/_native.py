@@ -179,6 +179,10 @@ SIGNATURES = {
     "b200kv_lm_get_begin": (c_i64, [c_vp, ctypes.c_char_p]),
     "b200kv_lm_list_begin": (c_i64, [c_vp]),
     "b200kv_lm_read": (c_i32, [c_vp, c_vp, c_i64]),
+    "b200kv_lm_open_begin": (c_i64, [c_vp, ctypes.c_char_p, c_i64, c_vp, c_vp]),
+    "b200kv_lm_read_ranges": (c_i32, [c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
+    "b200kv_lm_close_handles": (c_i32, [c_vp, c_i32, c_vp]),
+    "b200kv_lm_server_num_handles": (c_i64, [c_vp]),
 }
 PROFILE_SLOTS = ("absmax", "cdf", "encode", "compact", "tile_sum", "tile_scan", "decode")
 

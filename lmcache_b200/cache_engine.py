@@ -23,7 +23,7 @@ from lmcache_b200.codec import KvView, PinnedBuffer
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.logging import init_logger
 from lmcache_b200.storage_backend import CreateStorageBackend
-from lmcache_b200.pipeline import HeadWindow, LayerwiseUpload
+from lmcache_b200.pipeline import HeadWindow, LayerwiseUpload, join_uploads
 from lmcache_b200.reshard import first_source_rank, source_shards
 from lmcache_b200.utils import CacheEngineKey, KVCache, _lmcache_nvtx_annotate
 
@@ -660,6 +660,12 @@ class LMCacheEngine:
         if layout is None and not own_miss:
             own = (get_kv or self.engine_.get_kv_into)(self._keys_of(chunk_hashes, fmt), view, tok0, self.chunk_size)
         layout, n = self._reshard_get(chunk_hashes[own:], fmt, view, tok0 + own * self.chunk_size, layout)
+        uploads = getattr(get_kv, "uploads", None)
+        if n and uploads:
+            # chunk-major chunks after a layer-major prefix: every layer's ready event also comes after their decode
+            ev = torch.cuda.Event()
+            ev.record(torch.cuda.current_stream())
+            uploads.append(LayerwiseUpload.completed(n, view.L, ev))
         return layout, own, own + n
 
     def _retrieve_into_blob(self, tokens, full_chain, ret_mask, num_skip_tok, num_skip_chunk, extra, fmt, st, get_kv):
@@ -707,24 +713,27 @@ class LMCacheEngine:
 
     # ------------------------------------------------------------------ layer-wise retrieve
     def _layerwise_get(self):
-        """(get_kv for _retrieve / _retrieve_paged, list that receives the LayerwiseUpload), or None: the backend has no
-        layer-major path (raw, remote and hybrid tiers) or its containers hold several groups (CacheGen containers of
-        more than 256 tokens; a lossless container is always one group)"""
+        """(get_kv for _retrieve / _retrieve_paged, whose `uploads` list receives the LayerwiseUploads), or None: the
+        backend cannot serve this engine's chunks layer-major -- it says so (supports_layerwise_get: raw tiers, a remote
+        tier whose server has no ranged reads, a serde without containers), or its containers hold several groups
+        (CacheGen containers of more than 256 tokens; a lossless container is always one group)"""
         f = getattr(self.engine_, "get_kv_layerwise", None)
-        if f is None or not self._fast_path() or \
-                self.chunk_size > getattr(self.engine_, "layerwise_max_tokens", N.GROUP_TOKENS):
+        ok = getattr(self.engine_, "supports_layerwise_get", None)
+        if f is None or ok is None or not self._fast_path() or \
+                self.chunk_size > getattr(self.engine_, "layerwise_max_tokens", N.GROUP_TOKENS) or not ok():
             return None
         uploads: List[LayerwiseUpload] = []
 
         def get_kv(keys, view, tok0, cs):
             uploads.append(f(keys, view, tok0, cs))
             return uploads[-1].n
+        get_kv.uploads = uploads
         return get_kv, uploads
 
     @staticmethod
     def _layerwise_result(ret_mask, kv, num_layers: int, uploads) -> LayerwiseRetrieval:
         if uploads:
-            return LayerwiseRetrieval(ret_mask, kv, num_layers, uploads[0])
+            return LayerwiseRetrieval(ret_mask, kv, num_layers, join_uploads(uploads, num_layers))
         # nothing went layer-major: everything this call enqueued is before one event
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream())
@@ -734,9 +743,14 @@ class LMCacheEngine:
     def retrieve_layerwise(self, tokens: torch.Tensor, mask: Optional[torch.Tensor] = None) -> LayerwiseRetrieval:
         """retrieve(), with the KV made available one layer at a time: returns once the hit is known; ret_mask and the
         KV after synchronize() are those of retrieve().  On the compressed host and disk tiers the containers are
-        uploaded and decoded layer-major, so layer 0 is ready after about 1/L of the bytes; on every other tier (and
-        for CacheGen chunks of more than 256 tokens) this is retrieve() followed by one event that stands for every
-        layer."""
+        uploaded and decoded layer-major, so layer 0 is ready after about 1/L of the bytes.  On the remote tier, opted in
+        with LMCACHE_B200_REMOTE_LAYERWISE=1 and with a server that has ranged reads (this project's), they are also
+        fetched layer-major: every chunk's layer l before
+        any chunk's layer l + 1.  A hybrid tier does both parts so and joins them.  Chunks served from another
+        tensor-parallel layout after a layer-major prefix are decoded whole, before every layer's event.  On every other
+        tier (and for CacheGen chunks of more than 256 tokens) this is retrieve() followed by one event that stands for
+        every layer.  A remote fetch that fails after the match (a lost server) raises in wait_layer / synchronize for
+        the layers not yet released: ret_mask was already promised."""
         get_kv, uploads = self._layerwise_get() or (None, [])
         kv, ret_mask = self._retrieve(tokens, mask, get_kv)
         geom = self._kv_geometry()
@@ -745,8 +759,9 @@ class LMCacheEngine:
     @torch.no_grad()
     def retrieve_paged_layerwise(self, tokens: torch.Tensor, kv_caches, slot_mapping: torch.Tensor,
                                  mask: Optional[torch.Tensor] = None) -> LayerwiseRetrieval:
-        """retrieve_paged(), with the KV made available one layer at a time (see retrieve_layerwise).  A first chunk
-        that straddles the mask is decoded and scattered whole before layer 0's wait; `kv` is None."""
+        """retrieve_paged(), with the KV made available one layer at a time (see retrieve_layerwise: the same tiers go
+        layer-major, the remote one included).  A first chunk that straddles the mask is decoded and scattered whole
+        before layer 0's wait; `kv` is None."""
         get_kv, uploads = self._layerwise_get() or (None, [])
         ret_mask = self._retrieve_paged(tokens, kv_caches, slot_mapping, mask, get_kv)
         return self._layerwise_result(ret_mask, None, len(kv_caches), uploads)

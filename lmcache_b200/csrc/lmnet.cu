@@ -12,6 +12,18 @@
 //   PUT has no reply (server/__main__.py:46-48); GET miss = FAIL with length 0; EXIST = SUCCESS / FAIL with length 0;
 //   LIST = SUCCESS + keys joined by '\n'.
 //
+// Ranged reads (this project's servers only; the reference server ignores an unknown command -- no reply, and the body
+// is read as the next header -- so a client that sent one would wait forever: a client sends them only after EXIST on
+// kRangesProbe has answered SUCCESS -- the reference answers FAIL):
+//   OPEN  (5)  key, length = prefix bytes wanted -> SUCCESS, 16 + n: u32 handle | u32 0 | u64 value size | the first
+//              n = min(prefix, size) bytes; a miss, or a connection already holding kMaxHandles, is FAIL with length 0
+//   READ  (6)  length = 24 m, body m x {u32 handle | u32 0 | u64 offset | u64 nbytes} -> SUCCESS, sum nbytes, then the
+//              ranges in request order; an unknown handle or a range out of bounds is FAIL with length 0 (the connection
+//              stays in step)
+//   CLOSE (7)  length = 4 m, body m x u32 handle -> SUCCESS, 0 (unknown handles are ignored)
+// A handle holds the value as it was at OPEN (the stored Blob is shared, never mutated: a PUT replaces it), so every
+// byte read through it comes from one stored value.  A connection's handles are dropped when it closes.
+//
 // What is different from the reference, on purpose: payloads go from / into caller memory with one send / recv loop
 // (pinned slabs and Python bytes alike: no intermediate copies), the server keeps values in a hash map behind a
 // reader-writer lock (EXIST and GET are O(1) and concurrent), and a connection serialises whole request / response
@@ -44,7 +56,10 @@ namespace {
 constexpr int kKeyLen = 150;
 constexpr int kClientHdr = 8 + kKeyLen;     // struct "ii150s"
 constexpr int kServerHdr = 8;               // struct "ii"
-enum { kPut = 1, kGet = 2, kExist = 3, kList = 4, kSuccess = 200, kFail = 400 };
+enum { kPut = 1, kGet = 2, kExist = 3, kList = 4, kOpen = 5, kRead = 6, kClose = 7, kSuccess = 200, kFail = 400 };
+constexpr const char* kRangesProbe = "b200kv-ranges-v1";    // EXIST on it: SUCCESS from a server that has OPEN / READ / CLOSE
+constexpr size_t kMaxHandles = 4096;                         // open handles per connection
+constexpr int64_t kMaxReply = INT32_MAX;                    // a reply's length is an int32
 constexpr size_t kIoChunk = 1u << 20;      // bytes per send / recv call
 
 bool send_all(int fd, const void* p, size_t n) {
@@ -78,6 +93,16 @@ bool recv_all(int fd, void* p, size_t n) {
 
 void tune(int) {}     // kernel defaults (as the reference's Python sockets): autotuned buffers, Nagle on -- measured fastest
 
+// An OPEN or READ reply is corked while its pieces are sent and uncorked at the end, which pushes its last partial
+// segment at once: under Nagle alone that tail would wait for the peer's (delayed) ACK of the reply's earlier segments,
+// on every round trip of a layer-by-layer fetch.
+struct Corked {
+    int fd;
+    explicit Corked(int f) : fd(f) { set(1); }
+    ~Corked() { set(0); }
+    void set(int on) { setsockopt(fd, IPPROTO_TCP, TCP_CORK, &on, sizeof on); }
+};
+
 void pack_client(char* hdr, int32_t cmd, int32_t len, const char* key) {
     memcpy(hdr, &cmd, 4);
     memcpy(hdr + 4, &len, 4);
@@ -109,9 +134,19 @@ struct Server {
     std::atomic<int> active{0};             // running worker threads (detached; stop() waits for zero)
     std::shared_mutex mu;
     std::unordered_map<std::string, std::shared_ptr<Blob>> store;
+    std::atomic<int64_t> handles_open{0};   // OPEN handles of every connection (b200kv_lm_server_num_handles)
+
+    std::shared_ptr<Blob> find(const std::string& key) {
+        std::shared_lock<std::shared_mutex> lk(mu);
+        auto it = store.find(key);
+        return it == store.end() ? nullptr : it->second;
+    }
 
     void serve(int fd) {
         tune(fd);
+        std::unordered_map<uint32_t, std::shared_ptr<Blob>> handles;     // this connection's snapshots
+        uint32_t next_handle = 1;
+        std::vector<char> body;
         char hdr[kClientHdr];
         while (!stop.load(std::memory_order_relaxed) && recv_all(fd, hdr, kClientHdr)) {
             int32_t cmd, len;
@@ -145,12 +180,77 @@ struct Server {
                     if (!reply(kSuccess, blob->len) || !send_all(fd, blob->data.get(), (size_t)blob->len)) break;
                 }
             } else if (cmd == kExist) {
-                bool ok;
-                {
+                bool ok = key == kRangesProbe;
+                if (!ok) {
                     std::shared_lock<std::shared_mutex> lk(mu);
                     ok = store.find(key) != store.end();
                 }
                 if (!reply(ok ? kSuccess : kFail, 0)) break;
+            } else if (cmd == kOpen) {
+                std::shared_ptr<Blob> blob = len >= 0 && handles.size() < kMaxHandles ? find(key) : nullptr;
+                if (!blob) {
+                    if (!reply(kFail, 0)) break;
+                    continue;
+                }
+                while (handles.count(next_handle) || next_handle == 0) ++next_handle;
+                const uint32_t h = next_handle++;
+                handles[h] = blob;
+                handles_open.fetch_add(1);
+                const int32_t n = len < blob->len ? len : blob->len;
+                char meta[16];
+                const uint32_t zero = 0;
+                const uint64_t size = (uint64_t)blob->len;
+                memcpy(meta, &h, 4);
+                memcpy(meta + 4, &zero, 4);
+                memcpy(meta + 8, &size, 8);
+                Corked cork(fd);
+                if (!reply(kSuccess, 16 + n) || !send_all(fd, meta, 16) || !send_all(fd, blob->data.get(), (size_t)n)) break;
+            } else if (cmd == kRead || cmd == kClose) {
+                const int unit = cmd == kRead ? 24 : 4;
+                if (len < 0) break;
+                body.resize((size_t)len);
+                if (!recv_all(fd, body.data(), (size_t)len)) break;
+                const size_t m = (size_t)len / unit;
+                if (cmd == kClose) {
+                    for (size_t i = 0; i < m; ++i) {
+                        uint32_t h;
+                        memcpy(&h, body.data() + 4 * i, 4);
+                        if (handles.erase(h)) handles_open.fetch_sub(1);
+                    }
+                    if (!reply(kSuccess, 0)) break;
+                    continue;
+                }
+                // every entry is checked before a byte is sent: a refused READ sends nothing but its header
+                std::vector<const char*> src(m);
+                int64_t total = 0;
+                bool ok = len % unit == 0;
+                for (size_t i = 0; ok && i < m; ++i) {
+                    uint32_t h;
+                    uint64_t off, nb;
+                    memcpy(&h, body.data() + 24 * i, 4);
+                    memcpy(&off, body.data() + 24 * i + 8, 8);
+                    memcpy(&nb, body.data() + 24 * i + 16, 8);
+                    auto it = handles.find(h);
+                    ok = it != handles.end() && off <= (uint64_t)it->second->len &&
+                         nb <= (uint64_t)it->second->len - off && total + (int64_t)nb <= kMaxReply;
+                    if (ok) {
+                        src[i] = it->second->data.get() + off;
+                        total += (int64_t)nb;
+                    }
+                }
+                if (!ok) {
+                    if (!reply(kFail, 0)) break;
+                    continue;
+                }
+                Corked cork(fd);
+                if (!reply(kSuccess, (int32_t)total)) break;
+                bool sent = true;
+                for (size_t i = 0; sent && i < m; ++i) {
+                    uint64_t nb;
+                    memcpy(&nb, body.data() + 24 * i + 16, 8);
+                    sent = send_all(fd, src[i], (size_t)nb);
+                }
+                if (!sent) break;
             } else if (cmd == kList) {
                 std::string all;
                 {
@@ -165,6 +265,7 @@ struct Server {
                 break;      // unknown command: drop the connection, as the reference does by raising
             }
         }
+        handles_open.fetch_sub((int64_t)handles.size());
         {
             std::lock_guard<std::mutex> lk(conn_mu);
             for (size_t i = 0; i < conns.size(); ++i)
@@ -262,6 +363,10 @@ int64_t b200kv_lm_server_num_keys(void* server) {
     Server* s = static_cast<Server*>(server);
     std::shared_lock<std::shared_mutex> lk(s->mu);
     return (int64_t)s->store.size();
+}
+
+int64_t b200kv_lm_server_num_handles(void* server) {
+    return server ? static_cast<Server*>(server)->handles_open.load() : -1;
 }
 
 int b200kv_lm_server_stop(void* server) {
@@ -390,6 +495,101 @@ int b200kv_lm_read(void* conn, void* dst, int64_t len) {
     if (!recv_all(c->fd, dst, (size_t)len)) {
         set_error("lm:// receive failed");
         return -1;
+    }
+    return 0;
+}
+
+// OPEN: n = b200kv_lm_open_begin(conn, key, prefix, &handle, &size) -> prefix bytes pending (min(prefix, size)),
+// -1 = miss (or the server's handle cap), < -1 = error; the prefix then comes through b200kv_lm_read(conn, dst, n)
+int64_t b200kv_lm_open_begin(void* conn, const char* key, int64_t prefix, uint32_t* handle, int64_t* size) {
+    if (!conn || !key || strlen(key) > (size_t)kKeyLen || prefix < 0 || prefix > INT32_MAX - 16 || !handle || !size) {
+        set_error("invalid argument: bad key / connection / prefix");
+        return -2;
+    }
+    Conn* c = static_cast<Conn*>(conn);
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (c->pending != 0) {
+        set_error("invalid argument: a GET payload is still pending on this connection");
+        return -2;
+    }
+    char hdr[kClientHdr], rep[kServerHdr], meta[16];
+    pack_client(hdr, kOpen, (int32_t)prefix, key);
+    if (!send_all(c->fd, hdr, kClientHdr) || !recv_all(c->fd, rep, kServerHdr)) {
+        set_error("lm:// exchange failed");
+        return -3;
+    }
+    int32_t code, len;
+    memcpy(&code, rep, 4);
+    memcpy(&len, rep + 4, 4);
+    if (code != kSuccess) return -1;
+    if (len < 16 || !recv_all(c->fd, meta, 16)) {
+        set_error("lm:// OPEN reply malformed or cut short");
+        return -3;
+    }
+    memcpy(handle, meta, 4);
+    memcpy(size, meta + 8, 8);
+    c->pending = len - 16;
+    return len - 16;
+}
+
+// READ: the m ranges (handles[i], offsets[i], sizes[i]) straight into dst[i] (caller memory, e.g. slab blocks).
+// 0 = done, 1 = refused by the server (unknown handle / out of bounds: nothing was written), < 0 = error.
+int b200kv_lm_read_ranges(void* conn, int32_t m, const uint32_t* handles, const uint64_t* offsets, const uint64_t* sizes,
+                          void* const* dst) {
+    B2_REQUIRE(conn != nullptr && m >= 0 && (int64_t)m * 24 <= INT32_MAX &&
+               (m == 0 || (handles && offsets && sizes && dst)), "bad READ arguments");
+    int64_t total = 0;
+    for (int32_t i = 0; i < m; ++i) {
+        B2_REQUIRE(sizes[i] <= (uint64_t)kMaxReply && (sizes[i] == 0 || dst[i] != nullptr), "bad READ range");
+        total += (int64_t)sizes[i];
+    }
+    B2_REQUIRE(total <= kMaxReply, "a READ reply must stay below 2^31 bytes: split the request");
+    Conn* c = static_cast<Conn*>(conn);
+    std::lock_guard<std::mutex> lk(c->mu);
+    B2_REQUIRE(c->pending == 0, "a GET payload is still pending on this connection");
+    std::vector<char> req(kClientHdr + 24 * (size_t)m);
+    pack_client(req.data(), kRead, 24 * m, "");
+    for (int32_t i = 0; i < m; ++i) {
+        char* e = req.data() + kClientHdr + 24 * (size_t)i;
+        const uint32_t zero = 0;
+        memcpy(e, &handles[i], 4);
+        memcpy(e + 4, &zero, 4);
+        memcpy(e + 8, &offsets[i], 8);
+        memcpy(e + 16, &sizes[i], 8);
+    }
+    char rep[kServerHdr];
+    if (!send_all(c->fd, req.data(), req.size()) || !recv_all(c->fd, rep, kServerHdr)) {
+        set_error("lm:// exchange failed");
+        return -3;
+    }
+    int32_t code, len;
+    memcpy(&code, rep, 4);
+    memcpy(&len, rep + 4, 4);
+    if (code != kSuccess) return 1;
+    if (len != total) {
+        set_error("lm:// READ reply length does not match the request");
+        return -3;
+    }
+    for (int32_t i = 0; i < m; ++i)
+        if (!recv_all(c->fd, dst[i], (size_t)sizes[i])) {
+            set_error("lm:// receive failed");
+            return -3;
+        }
+    return 0;
+}
+
+int b200kv_lm_close_handles(void* conn, int32_t m, const uint32_t* handles) {
+    B2_REQUIRE(conn != nullptr && m >= 0 && (int64_t)m * 4 <= INT32_MAX && (m == 0 || handles), "bad CLOSE arguments");
+    Conn* c = static_cast<Conn*>(conn);
+    std::lock_guard<std::mutex> lk(c->mu);
+    B2_REQUIRE(c->pending == 0, "a GET payload is still pending on this connection");
+    std::vector<char> req(kClientHdr + 4 * (size_t)m);
+    pack_client(req.data(), kClose, 4 * m, "");
+    if (m) memcpy(req.data() + kClientHdr, handles, 4 * (size_t)m);
+    char rep[kServerHdr];
+    if (!send_all(c->fd, req.data(), req.size()) || !recv_all(c->fd, rep, kServerHdr)) {
+        set_error("lm:// exchange failed");
+        return -3;
     }
     return 0;
 }

@@ -584,15 +584,26 @@ def land_segments(slab, slot: SegmentSlot, batch, blocks: Optional[list] = None,
         raise
 
 
-def read_container(codec: CacheGenCodec, blk, nbytes: int, latent: bool = False) -> Optional[HostContainer]:
+def read_container(codec: CacheGenCodec, blk, nbytes: int, latent: bool = False,
+                   prefix: Optional[int] = None) -> Optional[HostContainer]:
     """The record of a container a disk read or a GET put into the first `nbytes` of `blk`, or None -- with the block
     freed -- when it is damaged, was written with another model's bins, or holds the other kind of KV than `latent`
     says (version 4 for a latent engine, versions 1 to 3 otherwise; versions 6 and 5 for a lossless codec): a miss, not an
-    error.  The header is checked by the codec's own parse_header, so a container of the other codec family is a miss."""
+    error.  The header is checked by the codec's own parse_header, so a container of the other codec family is a miss.
+    `prefix`: only the container's first `prefix` bytes are in `blk` yet (a ranged read; the container is `nbytes`
+    long): the header is checked against nbytes, and the plane offsets are read when the prefix holds the fixed sections
+    (None otherwise: the container is then uploaded whole)."""
+    got = nbytes if prefix is None else min(int(prefix), nbytes)
     try:
-        hd = codec.parse_header(blk.view()[:nbytes])
+        hd = codec.parse_header(blk.view()[:got], nbytes)
         if codec.accepts(hd, latent):
-            return HostContainer(blk, nbytes, hd, codec.plane_offsets(blk.view()[:nbytes]))   # on the reader's thread
+            try:
+                planes = codec.plane_offsets(blk.view()[:got])      # on the reader's thread
+            except N.NativeError:
+                if prefix is None:
+                    raise
+                planes = None                                      # the prefix stops inside the fixed sections
+            return HostContainer(blk, nbytes, hd, planes)
     except ValueError:
         pass
     blk.free()
@@ -844,6 +855,7 @@ class LayerwiseUpload:
         self.n = n
         self.num_layers = num_layers
         self.enqueue_s: List[float] = []    # host seconds the worker spent enqueueing: fixed sections + plan, then per layer
+        self.wait_s: List[float] = []       # of which host_ready waits (bytes still on their way), in the same order
         self._ready: List[torch.cuda.Event] = []
         self._error: Optional[BaseException] = None
         self._cv = threading.Condition()
@@ -874,6 +886,43 @@ class LayerwiseUpload:
             if len(self._ready) <= layer:
                 raise self._error
             return self._ready[layer]
+
+
+class JoinedUpload:
+    """Several LayerwiseUploads of one retrieve as one handle (a hybrid tier's local and remote parts, or a layer-major
+    prefix followed by chunk-major chunks): ready(l) is an event after every part's layer l, recorded on a stream of the
+    handle's own that waits for them.  A part's error is raised by ready() as the part raises it."""
+
+    def __init__(self, parts: Sequence[LayerwiseUpload], num_layers: int):
+        self.parts = list(parts)
+        self.n = sum(p.n for p in self.parts)
+        self.num_layers = num_layers
+        self.enqueue_s: List[float] = []
+        self.wait_s: List[float] = []
+        self._ready: dict = {}
+        self._stream: Optional[torch.cuda.Stream] = None
+        self._lock = threading.Lock()
+
+    def ready(self, layer: int) -> torch.cuda.Event:
+        evs = [p.ready(layer) for p in self.parts]
+        if len(evs) == 1:
+            return evs[0]
+        with self._lock:
+            ev = self._ready.get(layer)
+            if ev is None:
+                if self._stream is None:
+                    self._stream = torch.cuda.Stream()
+                for e in evs:
+                    self._stream.wait_event(e)
+                ev = torch.cuda.Event(enable_timing=True)
+                ev.record(self._stream)
+                self._ready[layer] = ev
+            return ev
+
+
+def join_uploads(parts: Sequence, num_layers: int):
+    """one handle for the uploads of one retrieve (the part itself when there is one)"""
+    return parts[0] if len(parts) == 1 else JoinedUpload(parts, num_layers)
 
 
 class LayerwiseUploader:
@@ -950,10 +999,66 @@ def layer_copy_ranges(plane_offs: Sequence[Optional[np.ndarray]], nbytes: Sequen
     return fixed, start, size
 
 
+READ_MAX_BYTES = (1 << 31) - 1      # an lm:// reply's length is an int32 (protocol.MAX_REPLY)
+READ_MAX_RANGES = 1 << 20          # ranges per READ: a request body of 24 MiB at most
+
+
+def ranged_read_plan(fixed: np.ndarray, start: np.ndarray, size: np.ndarray, got: Sequence[int],
+                     conn_of: Sequence[int], k: int, max_bytes: int = READ_MAX_BYTES,
+                     max_ranges: int = READ_MAX_RANGES) -> List[List[List[np.ndarray]]]:
+    """The READs of a layer-major remote fetch (pure host arithmetic).  fixed, start, size: layer_copy_ranges of n
+    containers (column i of start / size belongs to container i % n); got[j]: the first bytes of container j that OPEN
+    already delivered; conn_of[j]: the connection (0 .. k-1) that holds its handle.  Returns reads[c][l], the READs
+    connection c sends for layer l, each an int64 [m, 3] array of (container, offset, nbytes).  Layer 0 also carries
+    bytes [got, fixed) of a container whose prefix stops short of its fixed sections (one uploaded whole).  Ranges are
+    clipped to what the prefix lacks, so the prefix and the READs cover every container exactly once; empty ranges are
+    dropped.  A READ asks for at most max_bytes in at most max_ranges ranges; a longer range is split."""
+    n = len(got)
+    L = start.shape[0]
+    reads: List[List[List[np.ndarray]]] = [[[] for _ in range(L)] for _ in range(k)]
+    if n == 0:
+        return reads
+    got = np.asarray(got, dtype=np.int64)
+    conn_of = np.asarray(conn_of, dtype=np.int64)
+    col = np.arange(start.shape[1]) % n
+    g = got[col][None, :]
+    lo = np.maximum(start, g)
+    ln = np.maximum(start + size, g) - lo
+    rest = np.asarray(fixed, dtype=np.int64) - got
+    for layer in range(L):
+        ent = np.stack([col, lo[layer], ln[layer]], axis=1)
+        if layer == 0 and (rest > 0).any():
+            j = np.nonzero(rest > 0)[0]
+            ent = np.concatenate([np.stack([j, got[j], rest[j]], axis=1), ent])
+        ent = ent[ent[:, 2] > 0]
+        for c in range(k):
+            e = ent[conn_of[ent[:, 0]] == c]
+            if len(e) == 0:
+                continue
+            if len(e) <= max_ranges and int(e[:, 2].sum()) <= max_bytes:
+                reads[c][layer].append(np.ascontiguousarray(e))
+                continue
+            cur, tot = [], 0
+            for j, off, nb in e.tolist():
+                while nb > 0:
+                    if len(cur) == max_ranges or tot == max_bytes:
+                        reads[c][layer].append(np.array(cur, dtype=np.int64))
+                        cur, tot = [], 0
+                    take = min(nb, max_bytes - tot)
+                    cur.append((j, off, take))
+                    tot += take
+                    off += take
+                    nb -= take
+            if cur:
+                reads[c][layer].append(np.array(cur, dtype=np.int64))
+    return reads
+
+
 def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, records: Iterable[Optional[HostContainer]],
                             dst: KvView, dst_tok0: int, chunk_size: int, release: Optional[DeferredFree] = None,
                             on_done: Optional[Callable[[], None]] = None,
-                            level: Optional[DeviceLevel] = None) -> LayerwiseUpload:
+                            level: Optional[DeviceLevel] = None,
+                            host_ready: Optional[Callable[[int], None]] = None) -> LayerwiseUpload:
     """upload_decode in layer-major order, so that layer 0 of every chunk is decoded after ~1/L of the bytes.
 
     The match follows upload_decode's rules and is made on the calling thread, which consumes `records` to its end
@@ -969,7 +1074,11 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
     With a device `level`, resident records take no copies: they get a plan of their own over the level's pool (after
     their fill events), and each layer is decoded by both plans before its ready event.  Their `last_read` is left
     alone and their `dev_read` becomes the last decode's event.  The uploaded records are offered to the level
-    (level.promote) after the last copy."""
+    (level.promote) after the last copy.
+
+    `host_ready(l)`: the records' blocks are still being filled (a ranged remote read, RangedFetch.wait): the worker
+    calls it before it enqueues the fixed sections (l = 0) and before each layer l's copy, and it returns once the bytes
+    those copies read are in host memory, or raises -- which fails the upload."""
     matched: List[HostContainer] = []
     L = dst.L
     submitted = False
@@ -1032,6 +1141,7 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
             try:
                 with torch.cuda.device(uploader.device):
                     t0 = time.perf_counter()
+                    waited = 0.0
                     cs.wait_event(start)
                     ds.wait_event(start)
                     if res:
@@ -1041,6 +1151,10 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
                                                        [r.nbytes for r in res], [r.ntokens for r in res], dst,
                                                        [dst_tok[j] for j in res_j], first.max_dtype, first.coder, ds))
                     if up:
+                        if host_ready is not None:
+                            w0 = time.perf_counter()
+                            host_ready(0)
+                            waited = time.perf_counter() - w0
                         _batch_copy(dev, host, fixed, cs)
                         last = torch.cuda.Event()
                         last.record(cs)
@@ -1049,9 +1163,15 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
                                                        [r.ntokens for r in up], dst, [dst_tok[j] for j in up_j],
                                                        first.max_dtype, first.coder, ds))
                     t1 = time.perf_counter()
-                    upload.enqueue_s.append(t1 - t0)
+                    upload.enqueue_s.append(t1 - t0 - waited)
+                    upload.wait_s.append(waited)
                     for layer in range(L):
+                        waited = 0.0
                         if up:
+                            if host_ready is not None:
+                                w0 = time.perf_counter()
+                                host_ready(layer)
+                                waited = time.perf_counter() - w0
                             _batch_copy(lay_dst[layer], lay_src[layer], sz[layer], cs)
                             last = torch.cuda.Event()
                             last.record(cs)
@@ -1062,7 +1182,8 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
                         ev.record(ds)
                         upload._publish(ev)
                         t0, t1 = t1, time.perf_counter()
-                        upload.enqueue_s.append(t1 - t0)
+                        upload.enqueue_s.append(t1 - t0 - waited)
+                        upload.wait_s.append(waited)
                     if level is not None:             # staging is recorded on the copy stream: freed after these
                         for j, r, off in zip(up_j, up, offs):
                             level.promote(j, r, base + off, cs)

@@ -4,12 +4,17 @@ Default: the native server of libb200kv (csrc/lmnet.cu); `--python` runs the pur
 Speaks the reference wire protocol (lmcache/protocol.py, lmcache/server/__main__.py:29-93): opaque bytes
 in an in-memory dict, thread per client, no ack on PUT.  It never touches KV math; it exists so the
 engine-over-socket configurations can be exercised on a box that does not have the reference tree.
-EXIST is a dict lookup (the reference scans list_keys(), server/__main__.py:78-80)."""
+EXIST is a dict lookup (the reference scans list_keys(), server/__main__.py:78-80).
+
+Ranged reads (OPEN / READ / CLOSE, lmcache_b200/protocol.py) as the native server has them: a handle keeps the
+bytearray the key held at OPEN -- a PUT replaces that object, never mutates it -- so READ serves that snapshot."""
 import socket
+import struct
 import sys
 import threading
 
-from lmcache_b200.protocol import ClientMetaMessage, Constants, ServerMetaMessage
+from lmcache_b200.protocol import (MAX_HANDLES, MAX_REPLY, OPEN_META, RANGES_PROBE_KEY, READ_ENTRY, ClientMetaMessage,
+                                   Constants, ServerMetaMessage)
 
 
 class LMCacheServer:
@@ -21,6 +26,7 @@ class LMCacheServer:
         self.sock.setsockopt(socket.SOL_SOCKET, socket.SO_REUSEADDR, 1)
         self.sock.bind((host, port))
         self.sock.listen()
+        self.handles_open = 0        # OPEN handles of every connection
 
     @staticmethod
     def _recv_exact(conn, n):
@@ -33,7 +39,59 @@ class LMCacheServer:
             got += k
         return buf
 
+    def _count(self, d: int) -> None:
+        with self.lock:
+            self.handles_open += d
+
+    def num_handles(self) -> int:
+        with self.lock:
+            return self.handles_open
+
+    def _ranges(self, conn, meta, handles, nxt):
+        """OPEN / READ / CLOSE; returns the next handle number, or None when the connection is lost"""
+        fail = ServerMetaMessage(Constants.SERVER_FAIL, 0).serialize()
+        if meta.command == Constants.CLIENT_OPEN:
+            with self.lock:
+                data = self.store.get(meta.key)
+            if data is None or meta.length < 0 or len(handles) >= MAX_HANDLES:
+                conn.sendall(fail)
+                return nxt
+            while nxt in handles or nxt == 0:
+                nxt = (nxt + 1) & 0xffffffff
+            handles[nxt] = data
+            self._count(1)
+            n = min(meta.length, len(data))
+            conn.sendall(ServerMetaMessage(Constants.SERVER_SUCCESS, 16 + n).serialize() + OPEN_META.pack(nxt, 0, len(data)) +
+                         bytes(memoryview(data)[:n]))
+            return (nxt + 1) & 0xffffffff
+        if meta.length < 0:
+            return None
+        body = self._recv_exact(conn, meta.length)
+        if body is None:
+            return None
+        if meta.command == Constants.CLIENT_CLOSE:
+            for (h,) in struct.iter_unpack("<I", body[:meta.length // 4 * 4]):
+                if handles.pop(h, None) is not None:
+                    self._count(-1)
+            conn.sendall(ServerMetaMessage(Constants.SERVER_SUCCESS, 0).serialize())
+            return nxt
+        ranges, total = [], 0
+        ok = meta.length % READ_ENTRY.size == 0
+        for h, _, off, nb in (READ_ENTRY.iter_unpack(body) if ok else ()):
+            data = handles.get(h)
+            if data is None or off > len(data) or nb > len(data) - off or total + nb > MAX_REPLY:
+                ok = False
+                break
+            ranges.append(memoryview(data)[off:off + nb])
+            total += nb
+        if not ok:
+            conn.sendall(fail)
+            return nxt
+        conn.sendall(b"".join([ServerMetaMessage(Constants.SERVER_SUCCESS, total).serialize()] + ranges))
+        return nxt
+
     def handle_client(self, conn):
+        handles, nxt = {}, 1                 # this connection's snapshots
         try:
             while True:
                 header = self._recv_exact(conn, ClientMetaMessage.packlength())
@@ -56,7 +114,7 @@ class LMCacheServer:
                         conn.sendall(data)
                 elif meta.command == Constants.CLIENT_EXIST:
                     with self.lock:
-                        ok = meta.key in self.store
+                        ok = meta.key in self.store or meta.key == RANGES_PROBE_KEY
                     conn.sendall(ServerMetaMessage(Constants.SERVER_SUCCESS if ok else Constants.SERVER_FAIL,
                                                    0).serialize())
                 elif meta.command == Constants.CLIENT_LIST:
@@ -64,9 +122,14 @@ class LMCacheServer:
                         data = "\n".join(self.store.keys()).encode()
                     conn.sendall(ServerMetaMessage(Constants.SERVER_SUCCESS, len(data)).serialize())
                     conn.sendall(data)
+                elif meta.command in (Constants.CLIENT_OPEN, Constants.CLIENT_READ, Constants.CLIENT_CLOSE):
+                    nxt = self._ranges(conn, meta, handles, nxt)
+                    if nxt is None:
+                        break
                 else:
                     break
         finally:
+            self._count(-len(handles))
             conn.close()
 
     def run(self):

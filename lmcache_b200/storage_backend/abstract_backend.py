@@ -39,6 +39,11 @@ class LMCBackendInterface(metaclass=abc.ABCMeta):
             else:
                 yield None
 
+    def supports_layerwise_get(self) -> bool:
+        """Can get_kv_layerwise serve this tier's chunks layer-major?  A tier that has the method can; the remote tier
+        also needs a server with ranged reads, and asks it once."""
+        return getattr(self, "get_kv_layerwise", None) is not None
+
     @abc.abstractmethod
     def close(self):
         pass

@@ -3,10 +3,12 @@ from lmcache_b200.protocol.  One lock covers a whole request/response exchange, 
 threads cannot interleave on the socket (the reference locks sends only, see its TODO:1)."""
 import ctypes
 import socket
+import struct
 import threading
-from typing import List, Optional
+from typing import Callable, List, Optional, Sequence, Tuple
 
-from lmcache_b200.protocol import ClientMetaMessage, Constants, ServerMetaMessage
+from lmcache_b200.protocol import (MAX_REPLY, OPEN_META, RANGES_PROBE_KEY, READ_ENTRY, ClientMetaMessage, Constants,
+                                   ServerMetaMessage)
 from lmcache_b200.storage_backend.connector.base_connector import RemoteConnector
 
 
@@ -79,6 +81,71 @@ class LMCServerConnector(RemoteConnector):
                     return None
                 got += k
             return n
+
+    def _recv_to(self, ptr: int, n: int) -> None:
+        if n == 0:
+            return
+        view = memoryview((ctypes.c_char * n).from_address(ptr)).cast("B")
+        got = 0
+        while got < n:
+            k = self.sock.recv_into(view[got:], n - got)
+            if k == 0:
+                raise ConnectionError("lm:// connection closed")
+            got += k
+
+    def _reply(self) -> ServerMetaMessage:
+        hdr = self._recv_exact(ServerMetaMessage.packlength())
+        if hdr is None:
+            raise ConnectionError("lm:// connection closed")
+        return ServerMetaMessage.deserialize(bytes(hdr))
+
+    # ---- ranged reads (lmcache_b200/protocol.py): only after supports_ranges() said the server has them
+    def supports_ranges(self) -> bool:
+        return self.exists(RANGES_PROBE_KEY)
+
+    def open_into(self, key: str, prefix: int, alloc: Callable[[int], Tuple[int, object]]):
+        """LMCNativeConnector.open_into: (handle, size, prefix bytes received, obj) or None on a miss"""
+        with self.lock:
+            self.sock.sendall(ClientMetaMessage(Constants.CLIENT_OPEN, key, int(prefix)).serialize())
+            meta = self._reply()
+            if meta.code != Constants.SERVER_SUCCESS:
+                return None
+            body = self._recv_exact(OPEN_META.size)
+            if body is None or meta.length < OPEN_META.size:
+                raise ConnectionError("lm:// OPEN reply malformed or cut short")
+            handle, _, size = OPEN_META.unpack(bytes(body))
+            n = meta.length - OPEN_META.size
+            try:
+                ptr, obj = alloc(size)
+            except BaseException:
+                self._recv_exact(n)
+                self.sock.sendall(ClientMetaMessage(Constants.CLIENT_CLOSE, "", 4).serialize() + struct.pack("<I", handle))
+                self._reply()
+                raise
+            self._recv_to(ptr, n)
+        return handle, size, n, obj
+
+    def read_ranges(self, handles: Sequence[int], offsets: Sequence[int], sizes: Sequence[int],
+                    dst_ptrs: Sequence[int]) -> bool:
+        sizes = [int(z) for z in sizes]
+        assert sum(sizes) <= MAX_REPLY, "a READ reply must stay below 2^31 bytes: split the request"
+        body = b"".join(READ_ENTRY.pack(int(h), 0, int(o), z) for h, o, z in zip(handles, offsets, sizes))
+        with self.lock:
+            self.sock.sendall(ClientMetaMessage(Constants.CLIENT_READ, "", len(body)).serialize() + body)
+            meta = self._reply()
+            if meta.code != Constants.SERVER_SUCCESS:
+                return False
+            if meta.length != sum(sizes):
+                raise ConnectionError("lm:// READ reply length does not match the request")
+            for p, z in zip(dst_ptrs, sizes):
+                self._recv_to(int(p), z)
+        return True
+
+    def close_handles(self, handles: Sequence[int]) -> None:
+        body = b"".join(struct.pack("<I", int(h)) for h in handles)
+        with self.lock:
+            self.sock.sendall(ClientMetaMessage(Constants.CLIENT_CLOSE, "", len(body)).serialize() + body)
+            self._reply()
 
     def list(self) -> List[str]:
         with self.lock:

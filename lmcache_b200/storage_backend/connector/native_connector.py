@@ -4,10 +4,12 @@ with the GIL released -- payloads are sent straight from the caller's buffer (Py
 received straight into the bytearray handed back to the deserializer."""
 import ctypes
 import threading
-from typing import List, Optional
+from typing import Callable, List, Optional, Sequence, Tuple
+
+import numpy as np
 
 from lmcache_b200 import _native as N
-from lmcache_b200.protocol import MAX_KEY_LENGTH
+from lmcache_b200.protocol import MAX_KEY_LENGTH, RANGES_PROBE_KEY
 from lmcache_b200.storage_backend.connector.base_connector import RemoteConnector
 
 
@@ -85,6 +87,54 @@ class LMCNativeConnector(RemoteConnector):
                 return None
             rc = self._lib.b200kv_lm_read(self._h, ctypes.c_void_p(dst_ptr) if n else None, n)
             return n if rc == 0 else None
+
+    # ---- ranged reads (lmcache_b200/protocol.py): only after supports_ranges() said the server has them
+    def supports_ranges(self) -> bool:
+        return self.exists(RANGES_PROBE_KEY)
+
+    def open_into(self, key: str, prefix: int, alloc: Callable[[int], Tuple[int, object]]):
+        """OPEN `key`: alloc(size) -> (address, obj) gives the memory its first min(prefix, size) bytes go to.  Returns
+        (handle, size, prefix bytes received, obj), or None on a miss.  Raises when the exchange fails (the connection is
+        then out of step) or alloc raises (the handle is closed first)."""
+        handle, size = ctypes.c_uint32(), ctypes.c_int64()
+        with self.lock:
+            if self._h is None:
+                raise N.NativeError("lm:// connection is closed")
+            n = self._lib.b200kv_lm_open_begin(self._h, self._key(key), int(prefix), ctypes.byref(handle),
+                                               ctypes.byref(size))
+            if n == -1:
+                return None
+            N.check(n, "lm_open_begin")
+            try:
+                ptr, obj = alloc(int(size.value))
+            except BaseException:
+                self._read(n)
+                self._lib.b200kv_lm_close_handles(self._h, 1, ctypes.byref(handle))
+                raise
+            N.check(self._lib.b200kv_lm_read(self._h, ctypes.c_void_p(ptr) if n else None, n), "lm_read")
+        return int(handle.value), int(size.value), int(n), obj
+
+    def read_ranges(self, handles: Sequence[int], offsets: Sequence[int], sizes: Sequence[int],
+                    dst_ptrs: Sequence[int]) -> bool:
+        """READ: range i (offset, size) of handles[i] straight into dst_ptrs[i].  The sizes add up to less than 2^31.
+        True when done, False when the server refused it (nothing written); raises when the exchange fails."""
+        h = np.ascontiguousarray(handles, dtype=np.uint32)
+        o = np.ascontiguousarray(offsets, dtype=np.uint64)
+        z = np.ascontiguousarray(sizes, dtype=np.uint64)
+        d = np.ascontiguousarray(dst_ptrs, dtype=np.uint64)
+        with self.lock:
+            if self._h is None:
+                raise N.NativeError("lm:// connection is closed")
+            rc = N.check(self._lib.b200kv_lm_read_ranges(self._h, len(h), h.ctypes.data, o.ctypes.data, z.ctypes.data,
+                                                         d.ctypes.data), "lm_read_ranges")
+        return rc == 0
+
+    def close_handles(self, handles: Sequence[int]) -> None:
+        h = np.ascontiguousarray(handles, dtype=np.uint32)
+        with self.lock:
+            if self._h is None:
+                raise N.NativeError("lm:// connection is closed")
+            N.check(self._lib.b200kv_lm_close_handles(self._h, len(h), h.ctypes.data), "lm_close_handles")
 
     def list(self) -> List[str]:
         with self.lock:

@@ -10,6 +10,7 @@ from typing import Iterable, List, Optional, Tuple
 
 import torch
 
+from lmcache_b200 import _native as N
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.storage_backend.abstract_backend import LMCBackendInterface
 from lmcache_b200.utils import CacheEngineKey
@@ -76,6 +77,37 @@ class LMCHybridBackend(LMCBackendInterface):
         keys only, and the chunks served are not kept in it (they are another layout's quantisation, not this one's)."""
         f = getattr(self.remote_store, "get_kv_shards_into", None)
         return f(groups, dst, dst_tok0, chunk_size, stats) if f is not None else 0
+
+    @property
+    def layerwise_max_tokens(self) -> int:
+        """the smaller of the two tiers' (a tier without a layer-major path counts with one group of 256 tokens)"""
+        return min(getattr(s, "layerwise_max_tokens", N.GROUP_TOKENS) for s in (self.local_store, self.remote_store))
+
+    def supports_layerwise_get(self) -> bool:
+        return any(s.supports_layerwise_get() for s in (self.local_store, self.remote_store))
+
+    def get_kv_layerwise(self, keys, dst, dst_tok0: int, chunk_size: int):
+        """get_kv_into with each part layer-major where its tier can: the local tier's prefix, then the remote tier's
+        rest.  A part whose tier cannot is decoded chunk-major and counts as ready for every layer.  Returns one handle
+        whose ready(l) comes after both parts' layer l (pipeline.join_uploads)."""
+        from lmcache_b200.pipeline import join_uploads
+        parts: list = []
+        n = self._get_part(self.local_store, keys, dst, dst_tok0, chunk_size, parts)
+        if n < len(keys):
+            self._get_part(self.remote_store, keys[n:], dst, dst_tok0 + n * chunk_size, chunk_size, parts)
+        return join_uploads(parts, dst.L)
+
+    @staticmethod
+    def _get_part(store, keys, dst, dst_tok0: int, chunk_size: int, parts: list) -> int:
+        from lmcache_b200.pipeline import LayerwiseUpload
+        if store.supports_layerwise_get() and chunk_size <= getattr(store, "layerwise_max_tokens", N.GROUP_TOKENS):
+            parts.append(store.get_kv_layerwise(keys, dst, dst_tok0, chunk_size))
+        else:
+            n = store.get_kv_into(keys, dst, dst_tok0, chunk_size)
+            ev = torch.cuda.Event()
+            ev.record(torch.cuda.current_stream())
+            parts.append(LayerwiseUpload.completed(n, dst.L, ev))
+        return parts[-1].n
 
     def touch(self, keys) -> None:
         f = getattr(self.local_store, "touch", None)

@@ -9,15 +9,24 @@ Engine fast paths (CacheGen serde + a connector with get_into), both pipelined a
   get   the containers of all requested chunks are fetched by k connections into the slab while the main thread uploads
         and decodes the waves that are already complete (network || H2D || decode: what remote_backend.py:183-275 does
         with a network thread and a deserialize thread, here also on the engine's one-blob path).
-LMCACHE_B200_REMOTE_CONNS sets k (default 4; one TCP stream is slower than the GPU side)."""
+  get, layer-major (get_kv_layerwise, on a server with ranged reads): every matched container is OPENed -- its fixed
+        sections arrive with the OPEN -- and then k network threads READ every chunk's layer l before any chunk's layer
+        l + 1, while the uploader copies and decodes each layer as soon as its bytes are in host memory.
+LMCACHE_B200_REMOTE_CONNS sets k (default 4; one TCP stream is slower than the GPU side).  The layer-major get is opt-in,
+LMCACHE_B200_REMOTE_LAYERWISE=1: over loopback it brings layer 0 sooner but the last layer later than the chunk-major get
+(DESIGN.md section 4), so by default retrieve_layerwise on this tier stays retrieve() plus one event for every layer."""
+import collections
 import os
 import queue
 import threading
-from concurrent.futures import ThreadPoolExecutor
-from typing import Iterable, Iterator, List, Optional, Set, Tuple, Union
+import time
+from concurrent.futures import Future, ThreadPoolExecutor
+from typing import Callable, Iterable, Iterator, List, Optional, Set, Tuple, Union
 
+import numpy as np
 import torch
 
+from lmcache_b200 import _native as N
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.logging import init_logger
 from lmcache_b200.pipeline import DeferredFree
@@ -49,6 +58,102 @@ class LazyFlat:
         for g in self.groups:
             for key, _ in g:
                 yield key
+
+
+READ_BATCH_BYTES = 4 << 20      # a network thread merges the READs of consecutive layers (after layer 0) up to this
+
+
+class RangedFetch:
+    """The network side of a layer-major remote retrieve: for each of the k connections a pool thread sends, layer after
+    layer, that connection's READs of pipeline.ranged_read_plan (small layers merged, see _batch), straight into the
+    containers' blocks, and publishes how many layers it has completed.  wait(l) -- the uploader's host_ready -- returns once every connection has completed
+    layer l, and raises once a READ has failed (a lost connection, or a READ the server refused) and every thread has
+    stopped: no block is released while a thread may still write it.  finish() waits for the threads and CLOSEs the
+    handles."""
+
+    def __init__(self, conns, reads, handles: List[Optional[int]], ptrs: List[int], num_layers: int,
+                 count: Callable[..., None]):
+        self.conns, self.reads, self.handles, self.ptrs = conns, reads, handles, ptrs
+        self.L = num_layers
+        self.count = count                 # count(reads=, bytes=, read_s=, thread_s=): the backend's ranged_stats
+        self._done = [0] * len(conns)
+        self._left = len(conns)            # threads still running
+        self._error: Optional[BaseException] = None
+        self._cv = threading.Condition()
+        self._futs: List[Future] = []
+
+    def start(self, pool: ThreadPoolExecutor) -> None:
+        self._futs = [pool.submit(self._run, c) for c in range(len(self.conns))]
+
+    def _run(self, c: int) -> None:
+        conn, handles = self.conns[c], self.handles
+        ptrs = np.asarray(self.ptrs, dtype=np.int64)
+        t_start = time.perf_counter()
+        try:
+            layer = 0
+            while layer < self.L:
+                batch, end = self._batch(c, layer)
+                for e in batch:
+                    if self._error is not None:
+                        return
+                    j, off, nb = e[:, 0], e[:, 1], e[:, 2]
+                    t0 = time.perf_counter()
+                    if not conn.read_ranges([handles[i] for i in j.tolist()], off, nb, ptrs[j] + off):
+                        raise RuntimeError(f"lm:// READ of layers {layer}..{end - 1} refused by the server")
+                    self.count(reads=1, bytes=int(nb.sum()), read_s=time.perf_counter() - t0)
+                with self._cv:
+                    self._done[c] = end
+                    self._cv.notify_all()
+                layer = end
+        except BaseException as e:          # noqa: BLE001 -- the upload fails in wait()
+            with self._cv:
+                if self._error is None:
+                    self._error = e
+        finally:
+            self.count(thread_s=time.perf_counter() - t_start)
+            with self._cv:
+                self._left -= 1
+                self._cv.notify_all()
+
+    def _batch(self, c: int, layer: int):
+        """(READs, end): connection c's READs for layers [layer, end).  Layer 0 goes alone, so that it is ready as soon
+        as possible; after it, layers whose READ is a single one are merged into one READ until it carries
+        READ_BATCH_BYTES -- each exchange costs a round trip, which dominates when a layer's share is small."""
+        from lmcache_b200.pipeline import READ_MAX_BYTES, READ_MAX_RANGES
+        reads = self.reads[c]
+        batch, end = list(reads[layer]), layer + 1
+        if layer == 0 or len(batch) > 1:
+            return batch, end
+        nbytes = int(batch[0][:, 2].sum()) if batch else 0
+        nrng = len(batch[0]) if batch else 0
+        while end < self.L and len(reads[end]) <= 1 and nbytes < READ_BATCH_BYTES:
+            b = int(reads[end][0][:, 2].sum()) if reads[end] else 0
+            r = len(reads[end][0]) if reads[end] else 0
+            if nbytes + b > READ_MAX_BYTES or nrng + r > READ_MAX_RANGES:
+                break
+            batch += reads[end]
+            nbytes, nrng, end = nbytes + b, nrng + r, end + 1
+        return ([np.concatenate(batch)] if len(batch) > 1 else batch), end
+
+    def wait(self, layer: int) -> None:
+        with self._cv:
+            while min(self._done) <= layer:
+                if self._error is not None and self._left == 0:
+                    raise self._error
+                self._cv.wait()
+
+    def finish(self) -> None:
+        for f in self._futs:
+            f.result()
+        by_conn = collections.defaultdict(list)
+        for j, h in enumerate(self.handles):
+            if h is not None:
+                by_conn[j % len(self.conns)].append(h)
+        for c, hs in by_conn.items():
+            try:
+                self.conns[c].close_handles(hs)
+            except Exception:      # noqa: BLE001 -- a lost connection has dropped its handles
+                pass
 
 
 def _grouped(recs, k: int, sizes: List[int]):
@@ -101,6 +206,21 @@ class LMCRemoteBackend(LMCBackendInterface):
         self._upload = None
         self._release = DeferredFree()   # fetched blocks that uploads may still read
         self._peek = None            # (key, HostContainer): the container peek_geometry fetched, reused by get_kv_into
+        # layer-major retrieve (get_kv_layerwise, opt-in): does the server have ranged reads (None: not asked yet), its
+        # own k connections (chunk j's handle lives on connection j mod k), a pool for the OPENs of the match and one for
+        # the READ threads (a retrieve's match does not wait behind an earlier retrieve's whole fetch), the uploader, and
+        # what it fetched: ranged_stats counts OPENs, READs, bytes, and host seconds spent in them (open_s: in OPEN
+        # exchanges on the pool threads; match_s: the calling thread's match; read_s: inside READ exchanges; thread_s:
+        # the READ threads' whole lives)
+        self._lw_enabled = os.environ.get("LMCACHE_B200_REMOTE_LAYERWISE", "0") == "1"
+        self._ranges: Optional[bool] = None
+        self._lw_conns: List = []
+        self._lw_open_pool: Optional[ThreadPoolExecutor] = None
+        self._lw_pool: Optional[ThreadPoolExecutor] = None
+        self._layerwise = None
+        self._stats_lock = threading.Lock()
+        self.ranged_stats = {"retrieves": 0, "opens": 0, "reads": 0, "bytes": 0, "open_s": 0.0, "match_s": 0.0,
+                             "read_s": 0.0, "thread_s": 0.0}
 
     @_lmcache_nvtx_annotate
     def put_worker(self):
@@ -373,7 +493,198 @@ class LMCRemoteBackend(LMCBackendInterface):
                 stats["bytes"] = stats.get("bytes", 0) + sum(sizes[:n])
             return n
 
+    # ---- layer-major get (ranged reads)
+    @property
+    def layerwise_max_tokens(self) -> int:
+        """the largest chunk a layer-major retrieve takes: one group per container (256 tokens for CacheGen, 4096 for
+        lossless); 0 for a serde without containers"""
+        codec = getattr(self.deserializer, "codec", None)
+        return getattr(codec, "layerwise_max_tokens", 0) if self._striped() else 0
+
+    def _count(self, **kw) -> None:
+        with self._stats_lock:
+            for key, v in kw.items():
+                self.ranged_stats[key] += v
+
+    def supports_layerwise_get(self) -> bool:
+        """Opted in (LMCACHE_B200_REMOTE_LAYERWISE=1), a container serde on the striped path, and a server that answers
+        the ranged-read probe (asked once, on the first layer-wise retrieve: the reference server does not have ranged
+        reads).  Without the opt-in nothing is sent."""
+        if not (self._lw_enabled and self._striped() and hasattr(self.deserializer, "codec") and hasattr(self.connection, "supports_ranges")):
+            return False
+        if self._ranges is None:
+            try:
+                self._ranges = bool(self.connection.supports_ranges())
+            except Exception:       # noqa: BLE001 -- a broken connection: chunk-major, as every get would be
+                self._ranges = False
+        return self._ranges
+
+    def _lw_connections(self):
+        if not self._lw_conns:
+            self._lw_conns = [CreateConnector(self._url) for _ in range(self._nconn)]
+            self._lw_open_pool = ThreadPoolExecutor(max_workers=self._nconn, thread_name_prefix="b200kv-open")
+            self._lw_pool = ThreadPoolExecutor(max_workers=self._nconn, thread_name_prefix="b200kv-ranges")
+        return self._lw_conns
+
+    def _layerwise_uploader(self, device):
+        from lmcache_b200.pipeline import LayerwiseUploader
+        if self._layerwise is None or self._layerwise.device != device:
+            if self._layerwise is not None:
+                self._layerwise.close()
+            self._layerwise = LayerwiseUploader(device)
+        return self._layerwise
+
+    def _open(self, conn, key: CacheEngineKey, prefix: int, bound: int):
+        """OPEN one container into a fresh slab block of its size (on a pool thread): (HostContainer or None, handle or
+        None, prefix bytes received).  A miss, a broken connection, a container larger than `bound` and a damaged or
+        foreign one all give no record; a handle that was opened is still returned, for CLOSE."""
+        from lmcache_b200.pipeline import read_container
+
+        def alloc(size: int):
+            if size > bound or size == 0:
+                raise ValueError("not a container this retrieve can take")
+            blk = self._host_slab().alloc(size)
+            return blk.host_ptr, blk
+        t0 = time.perf_counter()
+        try:
+            r = conn.open_into(self._combine_key(key), prefix, alloc)
+        except Exception:           # noqa: BLE001 -- a miss, as in _fetch
+            return None, None, 0
+        finally:
+            self._count(open_s=time.perf_counter() - t0)
+        if r is None:
+            return None, None, 0
+        handle, size, got, blk = r
+        return read_container(self.deserializer.codec, blk, size, self.latent, prefix=got), handle, got
+
+    def get_kv_layerwise(self, keys, dst, dst_tok0: int, chunk_size: int):
+        """get_kv_into in layer-major order, over ranged reads (supports_layerwise_get must be True).  On the calling
+        thread: the keys are OPENed in chain order, pipelined over the k connections, each container's fixed sections
+        landing in a slab block of its size, and matched as get_kv_into matches them (first miss, damaged or foreign
+        container, change of dtype or coder); the handles past the match are closed.  Then the network threads READ
+        layer 0 of every matched chunk, then layer 1, ... into those blocks, and the uploader copies and decodes layer l
+        once its bytes are there (pipeline.upload_decode_layerwise with host_ready).  Returns the
+        pipeline.LayerwiseUpload: n is known, ready(l) is the event after layer l's decode.  Every matched container
+        sits in page-locked memory until its last copy.  A failed READ fails the upload: ready(l) raises for the layers
+        not yet published (n was promised already), the blocks and handles are released."""
+        from lmcache_b200.codec import lossless_raw_rows
+        from lmcache_b200.pipeline import (LayerwiseUpload, _continues_match, layer_copy_ranges, ranged_read_plan,
+                                           upload_decode_layerwise, wave_chunks_default)
+        self._release.sweep()
+        codec = self.deserializer.codec
+        conns = self._lw_connections()
+        k, pool = len(conns), self._lw_open_pool
+        t_match = time.perf_counter()
+        lo = codec.layout(dst.L, dst.H, dst.D, chunk_size, dst.latent)
+        prefix = int(lo.off_raw if hasattr(lo, "off_raw") else lo.off_payload)     # the fixed sections of a full chunk
+        bound = (self.deserializer.container_bound(dst.L, dst.H, dst.D, chunk_size, dst.latent) + 255) & ~255
+        peek, self._peek = self._peek, None
+        if peek is not None and not (len(keys) and peek[0] == keys[0]):
+            peek[1].blk.free()
+            peek = None
+        window = max(2 * k, 2 * wave_chunks_default())
+        pending: "collections.deque" = collections.deque()
+        keys_it = enumerate(keys)
+        recs, handles, got = [], [], []
+        stale = collections.defaultdict(list)          # handles past the match, per connection
+
+        def fill():
+            while len(pending) < window:
+                try:
+                    j, key = next(keys_it)
+                except StopIteration:
+                    return
+                if j == 0 and peek is not None:
+                    f = Future()
+                    f.set_result((peek[1], None, peek[1].nbytes))    # fetched whole by peek_geometry: used as it is
+                else:
+                    f = pool.submit(self._open, conns[j % k], key, prefix, bound)
+                pending.append((j, f))
+
+        def drop(j, rec, h):
+            if rec is not None:
+                rec.blk.free()
+            if h is not None:
+                stale[j % k].append(h)
+        try:
+            fill()
+            while pending:
+                j, f = pending.popleft()
+                rec, h, g = f.result()
+                if rec is None or not _continues_match(rec, recs[0] if recs else None, dst,
+                                                       dst_tok0 + len(recs) * chunk_size):
+                    drop(j, rec, h)
+                    break
+                recs.append(rec)
+                handles.append(h)
+                got.append(g)
+                fill()
+        except BaseException:
+            for rec, h, j in zip(recs, handles, range(len(recs))):
+                drop(j, rec, h)
+            recs = []
+            raise
+        finally:
+            for j, f in pending:
+                drop(j, *f.result()[:2])
+            for c, hs in stale.items():
+                try:
+                    conns[c].close_handles(hs)
+                except Exception:      # noqa: BLE001 -- a lost connection has dropped its handles
+                    pass
+        n = len(recs)
+        self._count(retrieves=1, opens=sum(h is not None for h in handles), match_s=time.perf_counter() - t_match,
+                    bytes=sum(g for g, h in zip(got, handles) if h is not None))
+        if n == 0:
+            with torch.cuda.device(dst.device):
+                ev = torch.cuda.Event()
+                ev.record(torch.cuda.current_stream())
+            return LayerwiseUpload.completed(0, dst.L, ev)
+        L = dst.L
+        try:
+            raw = None
+            if (recs[0].coder & 0xff) == N.CODER_LOSSLESS:
+                raw = [lossless_raw_rows(r.L, r.H, r.D, r.ntokens, dst.latent) for r in recs]
+            fixed, start, size = layer_copy_ranges([r.planes for r in recs], [r.nbytes for r in recs], L,
+                                                   dst.planes // L, raw)
+            reads = ranged_read_plan(fixed, start, size, got, [j % k for j in range(n)], k)
+            fetch = RangedFetch(conns, reads, handles, [r.blk.host_ptr for r in recs], L, self._count)
+            fetch.start(self._lw_pool)
+        except BaseException:                 # nothing reads the blocks yet: free them, close the handles
+            left = collections.defaultdict(list)
+            for j, (rec, h) in enumerate(zip(recs, handles)):
+                rec.blk.free()
+                if h is not None:
+                    left[j % k].append(h)
+            for c, hs in left.items():
+                try:
+                    conns[c].close_handles(hs)
+                except Exception:      # noqa: BLE001
+                    pass
+            raise
+
+        def done():
+            try:
+                fetch.finish()
+            finally:
+                self._release.add(recs[0].last_read, [r.blk for r in recs])
+        return upload_decode_layerwise(codec, self._layerwise_uploader(dst.device), iter(recs), dst, dst_tok0,
+                                       chunk_size, on_done=done, host_ready=fetch.wait)
+
     def close(self):
+        if getattr(self, "_layerwise", None) is not None:
+            self._layerwise.close()            # every layer-major job has ended (its fetch stopped, its blocks released)
+            self._layerwise = None
+        for attr in ("_lw_open_pool", "_lw_pool"):
+            if getattr(self, attr, None) is not None:
+                getattr(self, attr).shutdown(wait=True)
+                setattr(self, attr, None)
+        for c in getattr(self, "_lw_conns", []):
+            try:
+                c.close()
+            except Exception:       # noqa: BLE001
+                pass
+        self._lw_conns = []
         if self.put_thread is not None and self.put_thread.is_alive():
             self.put_queue.put(RemoteBackendEndSignal())
             self.put_thread.join()
