@@ -1,8 +1,9 @@
 """Host-side driver of the CUDA codec: descriptors, buffers, and batched encode / decode calls.
 
 This is plumbing above the C ABI (include/b200kv.h): PyTorch supplies device memory and streams,
-libb200kv does all the work.  The serde plugins (storage_backend/serde/cachegen_*.py) and the
-engine fast paths are thin layers over `CacheGenCodec`.
+libb200kv does all the work.  The serde plugins (storage_backend/serde/*.py) and the engine fast
+paths are thin layers over `CacheGenCodec` and `LosslessCodec`, which share one host-side flow (`_ContainerIO`) and
+differ only in their native calls and container checks.
 """
 from __future__ import annotations
 
@@ -320,22 +321,43 @@ class KvView:
         return buf, [buf[j * stride: j * stride + per_tok * t].view(shape(t)) for j, t in enumerate(sizes)]
 
 
-def parse_header(buf, total: Optional[int] = None) -> N.Header:
-    """Validate and return the 64-byte header of a B2KV container (bytes / bytearray / memoryview).  `buf` is the whole
-    container, or -- when `total`, the size of the whole container, is given -- a prefix of it that holds the header
-    and, for versions 3 and 4, the nb map after it."""
+def _parse_preamble(buf, total: Optional[int], versions: Tuple[int, ...],
+                    bad_version: str) -> Tuple[memoryview, N.Header]:
+    """The checks every B2KV header parse starts with: the buffer holds a header, the magic, a version of `versions`
+    (else ValueError(bad_version with the version)), total_bytes within the container (`total`: its size, when `buf` is
+    a prefix of it) and no encoder error status.  Returns the buffer's memoryview and the header."""
     mv = memoryview(buf)
     if mv.nbytes < N.HEADER_BYTES:
         raise ValueError("buffer too small for a B2KV container")
     hd = N.Header.from_buffer_copy(bytes(mv[:N.HEADER_BYTES]))
     if hd.magic != N.MAGIC:
         raise ValueError("not a B2KV container (bad magic)")
-    if hd.version not in (1, 2, 3, 4):
-        raise ValueError(f"unsupported B2KV version {hd.version}")
+    if hd.version not in versions:
+        raise ValueError(bad_version.format(hd.version))
     if hd.total_bytes > (mv.nbytes if total is None else total):
         raise ValueError("truncated B2KV container")
     if hd.status != 0:
         raise ValueError(f"B2KV container carries encoder error status {hd.status}")
+    return mv, hd
+
+
+def _plane_offsets(buf, versions: Tuple[int, ...], native, what: str) -> Optional[np.ndarray]:
+    """plane_offsets / lossless_plane_offsets: `native` (b200kv_plane_offsets or b200kv_lossless_plane_offsets) on a
+    container of one of `versions`, None for any other version and for lengths that do not add up."""
+    src = np.frombuffer(buf, dtype=np.uint8)
+    version, L = (int(v) for v in src[4:12].view(np.uint32))
+    if version not in versions:
+        return None
+    o = np.empty(N.planes_of(version, L) + 1, dtype=np.int64)
+    rc = N.check(native(src.ctypes.data, src.size, o.ctypes.data, o.size), what)
+    return o if rc == 0 else None
+
+
+def parse_header(buf, total: Optional[int] = None) -> N.Header:
+    """Validate and return the 64-byte header of a B2KV container (bytes / bytearray / memoryview).  `buf` is the whole
+    container, or -- when `total`, the size of the whole container, is given -- a prefix of it that holds the header
+    and, for versions 3 and 4, the nb map after it."""
+    mv, hd = _parse_preamble(buf, total, (1, 2, 3, 4), "unsupported B2KV version {}")
     nb = None
     if hd.version >= 3:
         P = N.planes_of(hd.version, hd.L)
@@ -352,13 +374,7 @@ def plane_offsets(buf) -> Optional[np.ndarray]:
     planes in version 4), plane p is bytes [o[p], o[p + 1]) of the container; o[0] is the start of the payload and
     o[P] == total_bytes.  None for versions 1 and 2, and when the lengths do not add up to the header's payload (a
     damaged container: it is only ever uploaded whole)."""
-    src = np.frombuffer(buf, dtype=np.uint8)
-    version, L = (int(v) for v in src[4:12].view(np.uint32))
-    if version not in (3, 4):
-        return None
-    o = np.empty(N.planes_of(version, L) + 1, dtype=np.int64)
-    rc = N.check(N.lib().b200kv_plane_offsets(src.ctypes.data, src.size, o.ctypes.data, o.size), "plane_offsets")
-    return o if rc == 0 else None
+    return _plane_offsets(buf, (3, 4), N.lib().b200kv_plane_offsets, "plane_offsets")
 
 
 def container_layout_of(hd: "N.Header") -> "N.Layout":
@@ -418,7 +434,7 @@ class EncodedBatch:
 
 @dataclass
 class EncodeTicket:
-    """An encode in flight (CacheGenCodec.encode_async).  `wait()` blocks the calling host thread -- not the stream --
+    """An encode in flight (encode_async).  `wait()` blocks the calling host thread -- not the stream --
     until the kernels are done and returns the batch with its sizes."""
     buf: torch.Tensor
     stride: int
@@ -445,9 +461,19 @@ class EncodeTicket:
 
 
 class _ContainerIO:
-    """What every codec does the same way around its own encode_async / decode: the blocking and host-copy forms of the
-    encode, the page-locked staging of containers on their way in, and the ordering of decodes that share buffers.  A
-    codec provides encode_async, parse_header (its container check) and the attributes _init_io sets."""
+    """The host-side flow both codecs share around their own native calls: encode_async and its blocking and host-copy
+    forms, decode (header checks, then the upload of host containers through the codec's staging), decode_raw /
+    decode_raw_heads and the decode plan calls, and the ordering of calls that share buffers.  A codec provides its
+    container check (parse_header, accepts), coder_for, layout, out_stride, decode_layers, and these hooks:
+
+    _check_source(view)                     ValueError for a KV the codec cannot encode (default: none)
+    _encode_ws_bytes(view, chunk_size, n_chunks, coder)
+    _encode_launch(view, tok_begin, n_tokens, chunk_size, n_chunks, last, coder, out, stride, sizes, stream)
+                                            enqueue the encode; returns the EncodeTicket fields it sets
+    _decode_ws_bytes(dst, src_H, tmax, n)   a decode plan's workspace bytes (never negative)
+    _plan_native(args, coder, dst, status, ws, stream, window)
+                                            the plan call, whole (window ()) or over head windows; returns the plan
+    _check_container(hd, dst)               decode()'s check of a header beyond its kind and shape"""
 
     def _init_io(self) -> None:
         self._enc_lock = threading.RLock()
@@ -471,6 +497,59 @@ class _ContainerIO:
         if t is None or t.numel() < nbytes or t.device != device:
             t = torch.empty(int(nbytes), dtype=torch.uint8, device=device)
         return t
+
+    def _check_source(self, view: KvView) -> None:
+        """ValueError for a KV this codec cannot encode"""
+
+    # ------------------------------------------------------------------ encode
+    def encode_async(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int,
+                     stream: Optional[torch.cuda.Stream] = None, out: Optional[torch.Tensor] = None,
+                     sizes: Optional[PinnedBuffer] = None) -> EncodeTicket:
+        """Enqueue the encode of tokens [tok_begin, tok_begin + n_tokens) of `view` as ceil(n_tokens / chunk_size)
+        containers on `stream` and return at once: no host synchronisation.  The containers land in `out` (device,
+        `out_stride` apart; the codec's own staging when None) and their sizes in `sizes` (mapped page-locked memory,
+        8 bytes per chunk; the codec's own when None) -- both are valid once the ticket's event has completed.
+        The KV is read in stream order, so the caller may reuse it for later work on the same stream (this is the
+        snapshot a non-blocking store needs; reference cache_engine.py:274-275 materialises chunk copies instead)."""
+        if n_tokens <= 0:
+            raise ValueError("n_tokens must be positive")
+        self._check_source(view)
+        coder = self.coder_for(chunk_size, view.latent)
+        n_chunks = (n_tokens + chunk_size - 1) // chunk_size
+        last = n_tokens - (n_chunks - 1) * chunk_size
+        stride = self.out_stride(view.L, view.H, view.D, chunk_size, view.latent)
+        with self._enc_lock, torch.cuda.device(view.device):
+            tstream = stream if stream is not None else torch.cuda.current_stream()
+            ws_bytes = self._encode_ws_bytes(view, chunk_size, n_chunks, coder)
+            own_out, own_sizes = out is None, sizes is None
+            need_out = stride * n_chunks + N.READ_SLACK if own_out else 0
+            # the workspace (and the codec's own staging) are shared by consecutive calls: order after the previous
+            # encode on whatever stream it ran; never free a buffer a kernel may still be using
+            if self._enc_event is not None:
+                grow = (self._enc_ws is None or self._enc_ws.numel() < ws_bytes or self._enc_ws.device != view.device or
+                        (own_out and (self._enc_out is None or self._enc_out.numel() < need_out)))
+                if grow:
+                    self._enc_event.synchronize()
+                else:
+                    tstream.wait_event(self._enc_event)
+            self._enc_ws = self._grow(self._enc_ws, ws_bytes, view.device)
+            if own_out:
+                self._enc_out = self._grow(self._enc_out, need_out, view.device)
+                out = self._enc_out
+            elif out.numel() < stride * n_chunks:
+                raise ValueError("encode output buffer too small")
+            if own_sizes:
+                if self._sizes is None or self._sizes.nbytes < 8 * n_chunks:
+                    self._sizes = PinnedBuffer(max(4096, 8 * n_chunks))
+                sizes = self._sizes
+            elif sizes.nbytes < 8 * n_chunks:
+                raise ValueError("sizes buffer too small")
+            extra = self._encode_launch(view, tok_begin, n_tokens, chunk_size, n_chunks, last, coder, out, stride, sizes,
+                                        tstream)
+            ev = torch.cuda.Event()
+            ev.record(tstream)
+            self._enc_event = ev
+            return EncodeTicket(out, stride, n_chunks, sizes, ev, view.dtype_code, coder, view, **extra)
 
     def encode(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int,
                stream: Optional[torch.cuda.Stream] = None, out: Optional[torch.Tensor] = None) -> EncodedBatch:
@@ -517,6 +596,7 @@ class _ContainerIO:
             finally:
                 del views
 
+    # ------------------------------------------------------------------ decode
     @contextlib.contextmanager
     def pinned_staging(self, nbytes: int):
         """A page-locked receive slab of at least nbytes (kept across calls): a remote tier reads containers straight
@@ -567,6 +647,149 @@ class _ContainerIO:
             self._dec_event.synchronize()
             return list((ctypes.c_uint32 * self._dec_status_n).from_address(self._dec_status.host_ptr))
 
+    def decode_raw(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
+                   ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
+                   stream: Optional[torch.cuda.Stream] = None, _locked: bool = False) -> None:
+        """Decode containers that already sit in device memory at base_ptr + offsets[j] (asynchronous): decode_plan on
+        the codec's own workspace and status words, then decode_layers over every layer.  `buf_bytes` is the size of the
+        buffer behind base_ptr: it must extend N.READ_SLACK bytes past every container (checked by the library);
+        totals[j] = header.total_bytes.  max_dtype and coder are the headers' (N.coder_of_version); a lossless
+        container's max_dtype is its element dtype, which must be dst's."""
+        self._decode_raw(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, stream, _locked)
+
+    def decode_raw_heads(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
+                         ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
+                         src_H: int, src_head0: Sequence[int], dst_head0: Sequence[int], n_heads: Sequence[int],
+                         stream: Optional[torch.cuda.Stream] = None) -> None:
+        """decode_raw for a window of each container's heads (decode_plan_heads): every container holds src_H heads, and
+        its heads [src_head0[j], src_head0[j] + n_heads[j]) land in dst's heads from dst_head0[j] on, at token
+        dst_tok[j] (a lossless container's bit for bit as the source layout stored them).  The rest of dst is left as it
+        was."""
+        self._decode_raw(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, stream, False,
+                         (src_H, src_head0, dst_head0, n_heads))
+
+    def _decode_raw(self, base_ptr, buf_bytes, offsets, totals, ntokens, dst: KvView, dst_tok, max_dtype, coder, stream,
+                    _locked: bool, heads=None) -> None:
+        n = len(offsets)
+        if n == 0:
+            return
+
+        def run():
+            tstream = stream if stream is not None else torch.cuda.current_stream()
+            ws_bytes = self._decode_ws_bytes(dst, heads[0] if heads else dst.H, max(ntokens), n)
+            if not _locked:
+                self._order_decode(tstream, 0, ws_bytes)
+            self._dec_ws = self._grow(self._dec_ws, ws_bytes, dst.device)
+            plan, _ = self._plan(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, heads,
+                                 self._dec_ws, self._status_buffer(n).dev_ptr, tstream)
+            self.decode_layers(plan, 0, dst.L, tstream)
+            if self._dec_event is None:
+                self._dec_event = torch.cuda.Event()
+            self._dec_event.record(tstream)
+
+        if _locked:
+            run()
+        else:
+            with self._dec_lock, torch.cuda.device(dst.device):
+                run()
+
+    def decode_plan(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
+                    ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
+                    stream: torch.cuda.Stream, status_ptr: int = 0) -> Tuple[ctypes.Structure, torch.Tensor]:
+        """First half of decode_raw (b200kv_decode_plan; b200kv_lossless_decode_plan): enqueue on `stream` the kernels
+        that read what the plan needs of every container -- its fixed sections; [0, off_raw) of a lossless one -- and
+        return (plan, workspace).  The payloads may still be uploading; decode_layers decodes a range of layers once its
+        bytes are there.  The workspace is the caller's (not the codec's shared one), so plans of concurrent retrieves do
+        not order after each other; it must be released only after the plan's last decode_layers (it is recorded on
+        `stream`: run those on the same stream)."""
+        return self._plan(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, None, None,
+                          status_ptr, stream)
+
+    def decode_plan_heads(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
+                          ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
+                          src_H: int, src_head0: Sequence[int], dst_head0: Sequence[int], n_heads: Sequence[int],
+                          stream: torch.cuda.Stream, status_ptr: int = 0) -> Tuple[ctypes.Structure, torch.Tensor]:
+        """decode_plan for head windows (see decode_raw_heads); decode_layers runs the plan."""
+        return self._plan(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder,
+                          (src_H, src_head0, dst_head0, n_heads), None, status_ptr, stream)
+
+    def _plan(self, base_ptr, buf_bytes, offsets, totals, ntokens, dst: KvView, dst_tok, max_dtype, coder, heads, ws,
+              status_ptr, stream) -> Tuple[ctypes.Structure, torch.Tensor]:
+        """the plan call of decode_plan (heads None) or decode_plan_heads (heads: (src_H, src_head0, dst_head0,
+        n_heads)); ws None: a workspace of the caller's own, recorded on `stream`"""
+        n = len(offsets)
+        if ws is None:
+            ws = torch.empty(self._decode_ws_bytes(dst, heads[0] if heads else dst.H, max(ntokens), n),
+                             dtype=torch.uint8, device=dst.device)
+            ws.record_stream(stream)
+        args = (base_ptr, int(buf_bytes), N.i64_array(list(offsets)), N.i64_array(list(totals)),
+                N.i32_array(list(ntokens)), N.i64_array(list(dst_tok)), n, int(max_dtype))
+        window = () if heads is None else (int(heads[0]), *(N.i32_array(list(h)) for h in heads[1:]))
+        return self._plan_native(args, coder, dst, status_ptr or None, ws, stream, window), ws
+
+    def decode(self, containers: Sequence[Union[bytes, bytearray, memoryview, torch.Tensor]], dst: KvView,
+               dst_tok: Sequence[int], stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Decode containers into `dst` at token offsets `dst_tok` (asynchronous on `stream`).  Host containers are
+        uploaded first; a single 16-byte-aligned device tensor is used in place.  ValueError for a container that is not
+        of this codec's family, whose kind (one plane per layer or a (K, V) pair) or shape is not dst's, that the codec
+        refuses (CacheGen: written with other bins; lossless: of another dtype than dst's), or that does not fit dst's
+        tokens; and for containers of one call that differ in max_dtype or version."""
+        n = len(containers)
+        if n == 0:
+            return
+        heads = []
+        for c in containers:
+            if isinstance(c, torch.Tensor):
+                hd = self.parse_header(c[:N.HEADER_BYTES + N.MAX_PLANES].cpu().numpy().tobytes(), c.numel())
+            else:
+                hd = self.parse_header(c)
+            if (hd.version in (4, 6)) != dst.latent:          # versions 4 and 6 hold one plane per layer
+                raise ValueError(f"a version-{hd.version} container does not fit a destination of "
+                                 f"{'one plane' if dst.latent else 'a (K, V) pair'} per layer")
+            self._check_container(hd, dst)
+            if (hd.L, hd.H, hd.D) != (dst.L, dst.H, dst.D):
+                raise ValueError(f"container shape L/H/D={hd.L}/{hd.H}/{hd.D} does not match destination "
+                                 f"{dst.L}/{dst.H}/{dst.D}")
+            heads.append(hd)
+        max_dtype = heads[0].max_dtype
+        if any(h.max_dtype != max_dtype or h.version != heads[0].version for h in heads):
+            raise ValueError("containers of one decode call must share max_dtype and container version")
+        coder = N.coder_of_version(heads[0].version)
+        totals = [int(h.total_bytes) for h in heads]
+        ntoks = [int(h.ntokens) for h in heads]
+        for tok, nt in zip(dst_tok, ntoks):
+            if tok < 0 or tok + nt > dst.ntokens:
+                raise ValueError(f"container of {nt} tokens at offset {tok} does not fit a {dst.ntokens}-token destination")
+        lib = N.lib()
+        with self._dec_lock, torch.cuda.device(dst.device):
+            tstream = stream if stream is not None else torch.cuda.current_stream()
+            sp = tstream.cuda_stream
+            need_in = sum((t + 15) & ~15 for t in totals) + N.READ_SLACK
+            self._order_decode(tstream, need_in, self._decode_ws_bytes(dst, dst.H, max(ntoks), n))
+            if n == 1 and isinstance(containers[0], torch.Tensor) and containers[0].is_cuda \
+                    and containers[0].data_ptr() % 16 == 0 and containers[0].numel() >= totals[0] + N.READ_SLACK:
+                keep_dev = containers[0]
+                self.decode_raw(keep_dev.data_ptr(), keep_dev.numel(), [0], totals, ntoks, dst, dst_tok, max_dtype, coder,
+                                tstream, _locked=True)
+                return
+            self._dec_in = self._grow(self._dec_in, need_in, dst.device)
+            base_ptr = self._dec_in.data_ptr()
+            offsets, o = [], 0
+            for c, nb in zip(containers, totals):
+                if isinstance(c, torch.Tensor):
+                    keep = c
+                    src_ptr = c.data_ptr()
+                else:
+                    keep = np.frombuffer(c, dtype=np.uint8, count=nb)   # zero-copy view of bytes/bytearray/memoryview
+                    src_ptr = keep.ctypes.data
+                # pageable sources are staged by the driver before the call returns
+                N.check(lib.b200kv_copy_async(base_ptr + o, src_ptr, nb, sp), "copy")
+                del keep
+                offsets.append(o)
+                o += (nb + 15) & ~15
+            self.decode_raw(base_ptr, self._dec_in.numel(), offsets, totals, ntoks, dst, dst_tok, max_dtype, coder, tstream,
+                            _locked=True)
+
 
 class CacheGenCodec(_ContainerIO):
     """Batched CacheGen encode / decode on the current CUDA device.
@@ -610,8 +833,23 @@ class CacheGenCodec(_ContainerIO):
     # ------------------------------------------------------------------ helpers
     parse_header = staticmethod(parse_header)    # the CacheGen container check (versions 1 to 4)
     plane_offsets = staticmethod(plane_offsets)  # where a version-3 / version-4 container's planes lie
-    plane_offsets_device = "b200kv_plane_offsets_device"     # the same for containers on the device (pipeline.land)
     layerwise_max_tokens = N.GROUP_TOKENS         # a layer-major retrieve needs one group per container
+
+    @staticmethod
+    def plane_offsets_device(containers: int, stride: int, n: int, out: int, stream) -> None:
+        """plane_offsets for n containers `stride` apart in device memory (b200kv_plane_offsets_device, pipeline.land):
+        int64[N.MAX_PLANES + 1] rows into `out`.  Through N.pylib(): the call keeps the GIL."""
+        N.check(N.pylib().b200kv_plane_offsets_device(ctypes.c_void_p(containers), stride, n, ctypes.c_void_p(out),
+                                                      stream), "b200kv_plane_offsets_device")
+
+    @staticmethod
+    def raw_rows(records, latent: bool = False) -> None:
+        """layer_copy_ranges' `raw` for these containers: None, a plane of a CacheGen container is its streams"""
+        return None
+
+    def plan_prefix(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> int:
+        """bytes [0, n) of a full chunk's container that decode_plan reads: its fixed sections"""
+        return int(self.layout(L, H, D, chunk_tokens, latent).off_payload)
 
     def coder_for(self, chunk_tokens: int, latent: bool = False) -> int:
         """The container this codec writes for chunks of `chunk_tokens`: the compact one holds <= 256 tokens.  A latent
@@ -666,13 +904,14 @@ class CacheGenCodec(_ContainerIO):
             return (lo.fixed_bytes + (1 if latent else 2) * L * H * D * (chunk_tokens + 4 + hdr) + 16 + 15) & ~15
         return lo.max_total_bytes
 
+    def _check_source(self, view: KvView) -> None:
+        if view.L > self.nlayers:
+            raise ValueError(f"KV has {view.L} layers but the bin table of this model has {self.nlayers}")
+
     # ------------------------------------------------------------------ layer-wise encode (pipeline.LayerwiseEncode)
     # b200kv_encode_layers_plan / _layers / _finish, version-3 (version-4) containers; a segment row per (chunk, plane)
     # is (arena offset, bytes) of the plane's streams
     seg_row = 2
-    layer_plan_type = N.EncodePlan
-    encode_layers_fn = "b200kv_encode_layers"
-    encode_layers_finish_fn = "b200kv_encode_layers_finish"
 
     def segment_layout(self, L: int, H: int, D: int, ntokens: int, latent: bool = False) -> SegmentLayout:
         lo = N.container_layout(L, H, D, ntokens, N.CODER_LATENT if latent else N.CODER_RANS_COMPACT)
@@ -688,175 +927,62 @@ class CacheGenCodec(_ContainerIO):
         return N.check(N.lib().b200kv_encode_layers_workspace_bytes(L, H, D, chunk_tokens, n_chunks, 1),
                        "encode_layers_workspace")
 
-    def encode_layers_plan(self, view: KvView, tok_begin: int, n: int, chunk_tokens: int, last: int, slot, plan,
-                           stream: torch.cuda.Stream) -> None:
-        """b200kv_encode_layers_plan into a pipeline.SegmentSlot, one layer per call"""
-        if view.L > self.nlayers:
-            raise ValueError(f"KV has {view.L} layers but the bin table of this model has {self.nlayers}")
+    def encode_layers_plan(self, view: KvView, tok_begin: int, n: int, chunk_tokens: int, last: int, slot,
+                           stream: torch.cuda.Stream) -> "N.EncodePlan":
+        """b200kv_encode_layers_plan into a pipeline.SegmentSlot, one layer per call; returns the plan"""
+        self._check_source(view)
+        plan = N.EncodePlan()
         N.check(N.lib().b200kv_encode_layers_plan(ctypes.byref(view.desc), tok_begin, n, chunk_tokens, last, self._kb,
                                                   self._vb, N.CODER_RANS_COMPACT, slot.arena.data_ptr(), slot.arena_bytes,
                                                   slot.fixed.data_ptr(), slot.fixed_stride, slot.seg.dev_ptr,
                                                   slot.sizes.dev_ptr, 1, slot.ws.data_ptr(), slot.ws.numel(),
                                                   ctypes.byref(plan), stream.cuda_stream), "encode_layers_plan")
+        return plan
 
-    # ------------------------------------------------------------------ encode
-    def encode_async(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int,
-                     stream: Optional[torch.cuda.Stream] = None, out: Optional[torch.Tensor] = None,
-                     sizes: Optional[PinnedBuffer] = None) -> "EncodeTicket":
-        """Enqueue the encode of tokens [tok_begin, tok_begin + n_tokens) of `view` as ceil(n_tokens / chunk_size)
-        containers on `stream` and return at once: no host synchronisation.  The containers land in `out` (device,
-        `out_stride` apart; the codec's own staging when None) and their sizes in `sizes` (mapped page-locked memory,
-        8 bytes per chunk; the codec's own when None) -- both are valid once the ticket's event has completed.
-        The KV is read in stream order, so the caller may reuse it for later work on the same stream (this is the
-        snapshot a non-blocking store needs; reference cache_engine.py:274-275 materialises chunk copies instead)."""
-        if n_tokens <= 0:
-            raise ValueError("n_tokens must be positive")
-        if view.L > self.nlayers:
-            raise ValueError(f"KV has {view.L} layers but the bin table of this model has {self.nlayers}")
-        n_chunks = (n_tokens + chunk_size - 1) // chunk_size
-        last = n_tokens - (n_chunks - 1) * chunk_size
-        stride = self.out_stride(view.L, view.H, view.D, chunk_size, view.latent)
-        lib = N.lib()
-        with self._enc_lock, torch.cuda.device(view.device):
-            tstream = stream if stream is not None else torch.cuda.current_stream()
-            coder = self.coder_for(chunk_size, view.latent)
-            ws_bytes = lib.b200kv_encode_workspace_bytes(view.L, view.H, view.D, chunk_size, n_chunks, coder)
-            own_out, own_sizes = out is None, sizes is None
-            need_out = stride * n_chunks + N.READ_SLACK if own_out else 0
-            # the workspace (and the codec's own staging) are shared by consecutive calls: order after the previous
-            # encode on whatever stream it ran; never free a buffer a kernel may still be using
-            if self._enc_event is not None:
-                grow = (self._enc_ws is None or self._enc_ws.numel() < ws_bytes or self._enc_ws.device != view.device or
-                        (own_out and (self._enc_out is None or self._enc_out.numel() < need_out)))
-                if grow:
-                    self._enc_event.synchronize()
-                else:
-                    tstream.wait_event(self._enc_event)
-            self._enc_ws = self._grow(self._enc_ws, ws_bytes, view.device)
-            if own_out:
-                self._enc_out = self._grow(self._enc_out, need_out, view.device)
-                out = self._enc_out
-            elif out.numel() < stride * n_chunks:
-                raise ValueError("encode output buffer too small")
-            if own_sizes:
-                if self._sizes is None or self._sizes.nbytes < 8 * n_chunks:
-                    self._sizes = PinnedBuffer(max(4096, 8 * n_chunks))
-                sizes = self._sizes
-            elif sizes.nbytes < 8 * n_chunks:
-                raise ValueError("sizes buffer too small")
-            # KV statistics of one model are stable from call to call: the previous call's measured entropy picks the
-            # compaction kernel's shared-memory stage size for this one (byte-identical output either way)
-            # (the threshold is in coder bits per symbol; a version-3 payload also holds ~0.4 bits of stream headers)
-            b = self._last_bits_per_symbol - (0.4 if coder & 0xff == N.CODER_RANS_COMPACT else 0.0)
-            flags = (coder & 0xff) | (N.ENCODE_HINT_MID_ENTROPY if b > 1.2 else 0)   # the descriptor says latent
-            N.check(lib.b200kv_encode_chunks(ctypes.byref(view.desc), tok_begin, n_chunks, chunk_size, last,
-                                             self._kb, self._vb, flags, out.data_ptr(), stride, sizes.dev_ptr,
-                                             self._enc_ws.data_ptr(), self._enc_ws.numel(), tstream.cuda_stream),
-                    "encode_chunks")
-            ev = torch.cuda.Event()
-            ev.record(tstream)
-            self._enc_event = ev
-            fixed = self.layout(view.L, view.H, view.D, chunk_size, view.latent).fixed_bytes
-            return EncodeTicket(out, stride, n_chunks, sizes, ev, view.dtype_code, coder, view, self,
-                                (fixed, float(view.planes) * view.H * view.D * n_tokens))
+    @staticmethod
+    def encode_layers(plan: "N.EncodePlan", layer_begin: int, layer_end: int, stream: torch.cuda.Stream) -> None:
+        """b200kv_encode_layers: enqueue the encode of layers [layer_begin, layer_end)"""
+        N.check(N.lib().b200kv_encode_layers(ctypes.byref(plan), int(layer_begin), int(layer_end), stream.cuda_stream),
+                "encode_layers")
 
-    # ------------------------------------------------------------------ decode
-    def decode_raw(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
-                   ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
-                   stream: Optional[torch.cuda.Stream] = None, _locked: bool = False) -> None:
-        """Decode containers that already sit in device memory at base_ptr + offsets[j] (asynchronous).  `buf_bytes` is
-        the size of the buffer behind base_ptr: it must extend N.READ_SLACK bytes past every container (checked by the
-        library); totals[j] = header.total_bytes."""
-        self._decode_raw(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, stream, _locked)
+    @staticmethod
+    def encode_layers_finish(plan: "N.EncodePlan", stream: torch.cuda.Stream) -> None:
+        """b200kv_encode_layers_finish: enqueue the headers and container sizes"""
+        N.check(N.lib().b200kv_encode_layers_finish(ctypes.byref(plan), stream.cuda_stream), "encode_layers_finish")
 
-    def decode_raw_heads(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
-                         ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
-                         src_H: int, src_head0: Sequence[int], dst_head0: Sequence[int], n_heads: Sequence[int],
-                         stream: Optional[torch.cuda.Stream] = None) -> None:
-        """decode_raw for a window of each container's heads (b200kv_decode_plan_heads): every container holds src_H
-        heads, and its heads [src_head0[j], src_head0[j] + n_heads[j]) land in dst's heads from dst_head0[j] on, at token
-        dst_tok[j].  The rest of dst is left as it was."""
-        self._decode_raw(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, stream, False,
-                         (src_H, src_head0, dst_head0, n_heads))
+    # ------------------------------------------------------------------ encode / decode hooks of _ContainerIO
+    def _encode_ws_bytes(self, view: KvView, chunk_size: int, n_chunks: int, coder: int) -> int:
+        return N.lib().b200kv_encode_workspace_bytes(view.L, view.H, view.D, chunk_size, n_chunks, coder)
 
-    def _decode_raw(self, base_ptr, buf_bytes, offsets, totals, ntokens, dst: KvView, dst_tok, max_dtype, coder, stream,
-                    _locked: bool, heads=None) -> None:
-        n = len(offsets)
-        if n == 0:
-            return
-        lib = N.lib()
-        tmax = max(ntokens)
+    def _encode_launch(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int, n_chunks: int, last: int,
+                       coder: int, out: torch.Tensor, stride: int, sizes: PinnedBuffer, stream) -> dict:
+        # KV statistics of one model are stable from call to call: the previous call's measured entropy picks the
+        # compaction kernel's shared-memory stage size for this one (byte-identical output either way)
+        # (the threshold is in coder bits per symbol; a version-3 payload also holds ~0.4 bits of stream headers)
+        b = self._last_bits_per_symbol - (0.4 if coder & 0xff == N.CODER_RANS_COMPACT else 0.0)
+        flags = (coder & 0xff) | (N.ENCODE_HINT_MID_ENTROPY if b > 1.2 else 0)   # the descriptor says latent
+        N.check(N.lib().b200kv_encode_chunks(ctypes.byref(view.desc), tok_begin, n_chunks, chunk_size, last, self._kb,
+                                             self._vb, flags, out.data_ptr(), stride, sizes.dev_ptr,
+                                             self._enc_ws.data_ptr(), self._enc_ws.numel(), stream.cuda_stream),
+                "encode_chunks")
+        # the ticket measures this call's bits per symbol for the next one
+        fixed = self.layout(view.L, view.H, view.D, chunk_size, view.latent).fixed_bytes
+        return dict(codec=self, stats=(fixed, float(view.planes) * view.H * view.D * n_tokens))
 
-        def run():
-            tstream = stream if stream is not None else torch.cuda.current_stream()
-            # a shape the library refuses has no workspace size (< 0): the decode call below says why
-            ws_bytes = max(lib.b200kv_decode_workspace_bytes(dst.L, heads[0] if heads else dst.H, dst.D, tmax, n), 0)
-            if not _locked:
-                self._order_decode(tstream, 0, ws_bytes)
-            self._dec_ws = self._grow(self._dec_ws, ws_bytes, dst.device)
-            args = (base_ptr, int(buf_bytes), N.i64_array(list(offsets)), N.i64_array(list(totals)),
-                    N.i32_array(list(ntokens)), N.i64_array(list(dst_tok)), n, int(max_dtype), int(coder),
-                    ctypes.byref(dst.desc), self._kb, self._vb, self._status_buffer(n).dev_ptr, self._dec_ws.data_ptr(),
-                    self._dec_ws.numel())
-            if heads is None:
-                N.check(lib.b200kv_decode_chunks(*args, tstream.cuda_stream), "decode_chunks")
-            else:
-                plan = N.DecodePlan()
-                N.check(lib.b200kv_decode_plan_heads(*args, ctypes.byref(plan), tstream.cuda_stream, int(heads[0]),
-                                                     N.i32_array(list(heads[1])), N.i32_array(list(heads[2])),
-                                                     N.i32_array(list(heads[3]))), "decode_plan_heads")
-                self.decode_layers(plan, 0, dst.L, tstream)
-            if self._dec_event is None:
-                self._dec_event = torch.cuda.Event()
-            self._dec_event.record(tstream)
+    def _decode_ws_bytes(self, dst: KvView, src_H: int, tmax: int, n: int) -> int:
+        # < 0: a shape the plan call refuses, with its reason
+        return max(N.lib().b200kv_decode_workspace_bytes(dst.L, int(src_H), dst.D, tmax, n), 0)
 
-        if _locked:
-            run()
+    def _plan_native(self, args: tuple, coder: int, dst: KvView, status, ws: torch.Tensor, stream,
+                     window: tuple) -> "N.DecodePlan":
+        plan = N.DecodePlan()
+        args += (int(coder), ctypes.byref(dst.desc), self._kb, self._vb, status, ws.data_ptr(), ws.numel(),
+                 ctypes.byref(plan), stream.cuda_stream)
+        if window:
+            N.check(N.lib().b200kv_decode_plan_heads(*args, *window), "decode_plan_heads")
         else:
-            with self._dec_lock, torch.cuda.device(dst.device):
-                run()
-
-    def decode_plan(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
-                    ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
-                    stream: torch.cuda.Stream, status_ptr: int = 0) -> Tuple["N.DecodePlan", torch.Tensor]:
-        """First half of decode_raw (b200kv_decode_plan): enqueue on `stream` the kernels that read the containers'
-        fixed sections and return (plan, workspace).  The payloads may still be uploading; decode_layers decodes a range
-        of layers once its bytes are there.  The workspace is the caller's (not the codec's shared one), so plans of
-        concurrent retrieves do not order after each other; it must be released only after the plan's last
-        decode_layers (it is recorded on `stream`: run those on the same stream)."""
-        n = len(offsets)
-        lib = N.lib()
-        ws = torch.empty(lib.b200kv_decode_workspace_bytes(dst.L, dst.H, dst.D, max(ntokens), n), dtype=torch.uint8,
-                         device=dst.device)
-        ws.record_stream(stream)
-        plan = N.DecodePlan()
-        N.check(lib.b200kv_decode_plan(base_ptr, int(buf_bytes), N.i64_array(list(offsets)), N.i64_array(list(totals)),
-                                       N.i32_array(list(ntokens)), N.i64_array(list(dst_tok)), n, int(max_dtype),
-                                       int(coder), ctypes.byref(dst.desc), self._kb, self._vb, status_ptr or None,
-                                       ws.data_ptr(), ws.numel(), ctypes.byref(plan), stream.cuda_stream),
-                "decode_plan")
-        return plan, ws
-
-    def decode_plan_heads(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
-                          ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
-                          src_H: int, src_head0: Sequence[int], dst_head0: Sequence[int], n_heads: Sequence[int],
-                          stream: torch.cuda.Stream, status_ptr: int = 0) -> Tuple["N.DecodePlan", torch.Tensor]:
-        """decode_plan for head windows (see decode_raw_heads); decode_layers runs the plan."""
-        n = len(offsets)
-        lib = N.lib()
-        ws = torch.empty(max(lib.b200kv_decode_workspace_bytes(dst.L, int(src_H), dst.D, max(ntokens), n), 0),
-                         dtype=torch.uint8, device=dst.device)     # < 0: a shape the plan call refuses, with its reason
-        ws.record_stream(stream)
-        plan = N.DecodePlan()
-        N.check(lib.b200kv_decode_plan_heads(base_ptr, int(buf_bytes), N.i64_array(list(offsets)),
-                                             N.i64_array(list(totals)), N.i32_array(list(ntokens)),
-                                             N.i64_array(list(dst_tok)), n, int(max_dtype), int(coder),
-                                             ctypes.byref(dst.desc), self._kb, self._vb, status_ptr or None,
-                                             ws.data_ptr(), ws.numel(), ctypes.byref(plan), stream.cuda_stream,
-                                             int(src_H), N.i32_array(list(src_head0)), N.i32_array(list(dst_head0)),
-                                             N.i32_array(list(n_heads))),
-                "decode_plan_heads")
-        return plan, ws
+            N.check(N.lib().b200kv_decode_plan(*args), "decode_plan")
+        return plan
 
     @staticmethod
     def decode_layers(plan: "N.DecodePlan", layer_begin: int, layer_end: int, stream: torch.cuda.Stream) -> None:
@@ -864,75 +990,16 @@ class CacheGenCodec(_ContainerIO):
         N.check(N.lib().b200kv_decode_layers(ctypes.byref(plan), int(layer_begin), int(layer_end), stream.cuda_stream),
                 "decode_layers")
 
+    def _check_container(self, hd: "N.Header", dst: KvView) -> None:
+        if not self.accepts(hd, dst.latent):
+            raise ValueError("compact container written with another model's bins" if hd.version >= 3 else
+                             f"a codec made from a cachegen_config reads version 3 only, not version {hd.version}")
+
     def decode_device_batch(self, batch: EncodedBatch, ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int],
                             stream: Optional[torch.cuda.Stream] = None) -> None:
         """Decode an EncodedBatch straight from its device staging buffer (no host hop, no header reads)."""
         self.decode_raw(batch.buf.data_ptr(), batch.buf.numel(), [j * batch.stride for j in range(len(batch.sizes))],
                         batch.sizes, ntokens, dst, dst_tok, batch.max_dtype, batch.coder, stream)
-
-    def decode(self, containers: Sequence[Union[bytes, bytearray, memoryview, torch.Tensor]], dst: KvView,
-               dst_tok: Sequence[int], stream: Optional[torch.cuda.Stream] = None) -> None:
-        """Decode containers into `dst` at token offsets `dst_tok` (asynchronous on `stream`).
-        Host containers are uploaded first; a single 16-byte-aligned device tensor is used in place."""
-        n = len(containers)
-        if n == 0:
-            return
-        lib = N.lib()
-        heads = []
-        for c in containers:
-            if isinstance(c, torch.Tensor):
-                hd = parse_header(c[:N.HEADER_BYTES + N.MAX_PLANES].cpu().numpy().tobytes(), c.numel())
-            else:
-                hd = parse_header(c)
-            if (hd.version == 4) != dst.latent:
-                raise ValueError(f"a version-{hd.version} container does not fit a destination of "
-                                 f"{'one plane' if dst.latent else 'a (K, V) pair'} per layer")
-            if not self.accepts(hd, dst.latent):
-                raise ValueError("compact container written with another model's bins" if hd.version >= 3 else
-                                 f"a codec made from a cachegen_config reads version 3 only, not version {hd.version}")
-            if (hd.L, hd.H, hd.D) != (dst.L, dst.H, dst.D):
-                raise ValueError(f"container shape L/H/D={hd.L}/{hd.H}/{hd.D} does not match destination "
-                                 f"{dst.L}/{dst.H}/{dst.D}")
-            heads.append(hd)
-        max_dtype = heads[0].max_dtype
-        if any(h.max_dtype != max_dtype or h.version != heads[0].version for h in heads):
-            raise ValueError("containers of one decode call must share max_dtype and container version")
-        coder = N.coder_of_version(heads[0].version)
-        totals = [int(h.total_bytes) for h in heads]
-        ntoks = [int(h.ntokens) for h in heads]
-        tmax = max(ntoks)
-        for tok, nt in zip(dst_tok, ntoks):
-            if tok < 0 or tok + nt > dst.ntokens:
-                raise ValueError(f"container of {nt} tokens at offset {tok} does not fit a {dst.ntokens}-token destination")
-        with self._dec_lock, torch.cuda.device(dst.device):
-            tstream = stream if stream is not None else torch.cuda.current_stream()
-            sp = tstream.cuda_stream
-            need_in = sum((int(h.total_bytes) + 15) & ~15 for h in heads) + N.READ_SLACK
-            self._order_decode(tstream, need_in, lib.b200kv_decode_workspace_bytes(dst.L, dst.H, dst.D, tmax, n))
-            if n == 1 and isinstance(containers[0], torch.Tensor) and containers[0].is_cuda \
-                    and containers[0].data_ptr() % 16 == 0 and containers[0].numel() >= totals[0] + N.READ_SLACK:
-                keep_dev = containers[0]
-                self.decode_raw(keep_dev.data_ptr(), keep_dev.numel(), [0], totals, ntoks, dst, dst_tok, max_dtype, coder,
-                                tstream, _locked=True)
-                return
-            self._dec_in = self._grow(self._dec_in, need_in, dst.device)
-            base_ptr = self._dec_in.data_ptr()
-            offsets, o = [], 0
-            for c, h in zip(containers, heads):
-                nb = int(h.total_bytes)
-                if isinstance(c, torch.Tensor):
-                    keep = c
-                    src_ptr = c.data_ptr()
-                else:
-                    keep = np.frombuffer(c, dtype=np.uint8, count=nb)   # zero-copy view of bytes/bytearray/memoryview
-                    src_ptr = keep.ctypes.data
-                # pageable sources are staged by the driver before the call returns
-                N.check(lib.b200kv_copy_async(base_ptr + o, src_ptr, nb, sp), "copy")
-                del keep
-                offsets.append(o)
-                o += (nb + 15) & ~15
-            self.decode_raw(base_ptr, self._dec_in.numel(), offsets, totals, ntoks, dst, dst_tok, max_dtype, coder, tstream,
-                            _locked=True)
 
 
 def dtype_of_code(code: int) -> torch.dtype:
@@ -944,18 +1011,7 @@ def parse_lossless_header(buf, total: Optional[int] = None) -> N.Header:
     """Validate and return the 64-byte header of a lossless B2KV container (versions 5 and 6; ValueError for anything
     else, CacheGen containers included).  `buf` is the whole container, or a prefix of at least the header when `total`,
     the size of the whole container, is given."""
-    mv = memoryview(buf)
-    if mv.nbytes < N.HEADER_BYTES:
-        raise ValueError("buffer too small for a B2KV container")
-    hd = N.Header.from_buffer_copy(bytes(mv[:N.HEADER_BYTES]))
-    if hd.magic != N.MAGIC:
-        raise ValueError("not a B2KV container (bad magic)")
-    if hd.version not in (5, 6):
-        raise ValueError(f"not a lossless B2KV container (version {hd.version})")
-    if hd.total_bytes > (mv.nbytes if total is None else total):
-        raise ValueError("truncated B2KV container")
-    if hd.status != 0:
-        raise ValueError(f"B2KV container carries encoder error status {hd.status}")
+    hd = _parse_preamble(buf, total, (5, 6), "not a lossless B2KV container (version {})")[1]
     check_lossless_header(hd)
     return hd
 
@@ -983,21 +1039,8 @@ def lossless_plane_offsets(buf) -> Optional[np.ndarray]:
     lengths), from its lengths section: int64[P + 1] (P = 2L, or L for version 6), the streams of plane p are bytes
     [o[p], o[p + 1]) of the container, o[0] is off_payload and o[P] == total_bytes.  None when the lengths do not add up
     to the header's total (a damaged container: it is only ever uploaded whole).  Plane p's raw rows come from the
-    layout: lossless_raw_rows."""
-    src = np.frombuffer(buf, dtype=np.uint8)
-    version, L = (int(v) for v in src[4:12].view(np.uint32))
-    if version not in (5, 6):
-        return None
-    o = np.empty(N.planes_of(version, L) + 1, dtype=np.int64)
-    rc = N.check(N.lib().b200kv_lossless_plane_offsets(src.ctypes.data, src.size, o.ctypes.data, o.size),
-                 "lossless_plane_offsets")
-    return o if rc == 0 else None
-
-
-def lossless_raw_rows(L: int, H: int, D: int, ntokens: int, latent: bool) -> Tuple[int, int]:
-    """(off_raw, bytes per plane) of a lossless container: plane p's raw rows are bytes
-    [off_raw + p * t * C, off_raw + (p + 1) * t * C)."""
-    return int(N.lossless_layout(L, H, D, ntokens, latent).off_raw), int(ntokens) * H * D
+    layout: LosslessCodec.raw_rows."""
+    return _plane_offsets(buf, (5, 6), N.lib().b200kv_lossless_plane_offsets, "lossless_plane_offsets")
 
 
 class LosslessCodec(_ContainerIO):
@@ -1014,8 +1057,25 @@ class LosslessCodec(_ContainerIO):
 
     parse_header = staticmethod(parse_lossless_header)
     plane_offsets = staticmethod(lossless_plane_offsets)
-    plane_offsets_device = "b200kv_lossless_plane_offsets_device"
     layerwise_max_tokens = N.LOSSLESS_MAX_TOKENS   # a lossless container is always one group
+
+    @staticmethod
+    def plane_offsets_device(containers: int, stride: int, n: int, out: int, stream) -> None:
+        """CacheGenCodec.plane_offsets_device for lossless containers (b200kv_lossless_plane_offsets_device)"""
+        N.check(N.pylib().b200kv_lossless_plane_offsets_device(ctypes.c_void_p(containers), stride, n,
+                                                               ctypes.c_void_p(out), stream),
+                "b200kv_lossless_plane_offsets_device")
+
+    @staticmethod
+    def raw_rows(records, latent: bool = False) -> List[Tuple[int, int]]:
+        """layer_copy_ranges' `raw` for these containers (records with L, H, D and ntokens): per container (off_raw,
+        bytes per plane), plane p's raw rows are bytes [off_raw + p * t * C, off_raw + (p + 1) * t * C)"""
+        return [(int(N.lossless_layout(r.L, r.H, r.D, r.ntokens, latent).off_raw), int(r.ntokens) * r.H * r.D)
+                for r in records]
+
+    def plan_prefix(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> int:
+        """bytes [0, n) of a full chunk's container that decode_plan reads: [0, off_raw)"""
+        return int(self.layout(L, H, D, chunk_tokens, latent).off_raw)
 
     @staticmethod
     def coder_for(chunk_tokens: int, latent: bool = False) -> int:
@@ -1045,9 +1105,6 @@ class LosslessCodec(_ContainerIO):
     # b200kv_lossless_encode_layers_plan / _layers / _finish; a segment row per (chunk, plane) is (arena offset of the
     # plane's raw rows, arena offset of its streams, stream bytes)
     seg_row = 3
-    layer_plan_type = N.LosslessEncodePlan
-    encode_layers_fn = "b200kv_lossless_encode_layers"
-    encode_layers_finish_fn = "b200kv_lossless_encode_layers_finish"
 
     def segment_layout(self, L: int, H: int, D: int, ntokens: int, latent: bool = False) -> SegmentLayout:
         lo = self.layout(L, H, D, ntokens, latent)
@@ -1065,160 +1122,58 @@ class LosslessCodec(_ContainerIO):
                                                                              int(latent), 1),
                        "lossless_encode_layers_workspace")
 
-    def encode_layers_plan(self, view: KvView, tok_begin: int, n: int, chunk_tokens: int, last: int, slot, plan,
-                           stream: torch.cuda.Stream) -> None:
-        """b200kv_lossless_encode_layers_plan into a pipeline.SegmentSlot, one layer per call"""
+    def encode_layers_plan(self, view: KvView, tok_begin: int, n: int, chunk_tokens: int, last: int, slot,
+                           stream: torch.cuda.Stream) -> "N.LosslessEncodePlan":
+        """b200kv_lossless_encode_layers_plan into a pipeline.SegmentSlot, one layer per call; returns the plan"""
+        plan = N.LosslessEncodePlan()
         N.check(N.lib().b200kv_lossless_encode_layers_plan(ctypes.byref(view.desc), tok_begin, n, chunk_tokens, last,
                                                            slot.arena.data_ptr(), slot.arena_bytes, slot.fixed.data_ptr(),
                                                            slot.fixed_stride, slot.seg.dev_ptr, slot.sizes.dev_ptr, 1,
                                                            slot.ws.data_ptr(), slot.ws.numel(), ctypes.byref(plan),
                                                            stream.cuda_stream), "lossless_encode_layers_plan")
-
-    # ------------------------------------------------------------------ encode
-    def encode_async(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int,
-                     stream: Optional[torch.cuda.Stream] = None, out: Optional[torch.Tensor] = None,
-                     sizes: Optional[PinnedBuffer] = None) -> "EncodeTicket":
-        """CacheGenCodec.encode_async for lossless containers: enqueue on `stream`, no host synchronisation; the KV is
-        read in stream order (twice: histogram, then coding)."""
-        if n_tokens <= 0:
-            raise ValueError("n_tokens must be positive")
-        coder = self.coder_for(chunk_size, view.latent)
-        n_chunks = (n_tokens + chunk_size - 1) // chunk_size
-        last = n_tokens - (n_chunks - 1) * chunk_size
-        stride = self.out_stride(view.L, view.H, view.D, chunk_size, view.latent)
-        lib = N.lib()
-        with self._enc_lock, torch.cuda.device(view.device):
-            tstream = stream if stream is not None else torch.cuda.current_stream()
-            ws_bytes = N.check(lib.b200kv_lossless_workspace_bytes(view.L, view.H, view.D, chunk_size, n_chunks,
-                                                                   int(view.latent), 0), "lossless_workspace_bytes")
-            own_out, own_sizes = out is None, sizes is None
-            need_out = stride * n_chunks + N.READ_SLACK if own_out else 0
-            if self._enc_event is not None:
-                grow = (self._enc_ws is None or self._enc_ws.numel() < ws_bytes or self._enc_ws.device != view.device or
-                        (own_out and (self._enc_out is None or self._enc_out.numel() < need_out)))
-                if grow:
-                    self._enc_event.synchronize()
-                else:
-                    tstream.wait_event(self._enc_event)
-            self._enc_ws = self._grow(self._enc_ws, ws_bytes, view.device)
-            if own_out:
-                self._enc_out = self._grow(self._enc_out, need_out, view.device)
-                out = self._enc_out
-            elif out.numel() < stride * n_chunks:
-                raise ValueError("encode output buffer too small")
-            if own_sizes:
-                if self._sizes is None or self._sizes.nbytes < 8 * n_chunks:
-                    self._sizes = PinnedBuffer(max(4096, 8 * n_chunks))
-                sizes = self._sizes
-            elif sizes.nbytes < 8 * n_chunks:
-                raise ValueError("sizes buffer too small")
-            N.check(lib.b200kv_lossless_encode(ctypes.byref(view.desc), tok_begin, n_chunks, chunk_size, last,
-                                               out.data_ptr(), stride, sizes.dev_ptr, self._enc_ws.data_ptr(),
-                                               self._enc_ws.numel(), tstream.cuda_stream), "lossless_encode")
-            ev = torch.cuda.Event()
-            ev.record(tstream)
-            self._enc_event = ev
-            return EncodeTicket(out, stride, n_chunks, sizes, ev, view.dtype_code, coder, view)
-
-    # ------------------------------------------------------------------ decode
-    def decode_raw(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
-                   ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
-                   stream: Optional[torch.cuda.Stream] = None, _locked: bool = False) -> None:
-        """Decode containers that already sit in device memory at base_ptr + offsets[j] (asynchronous), as
-        CacheGenCodec.decode_raw.  max_dtype is the stored element dtype, which must be dst's; coder names the version
-        (N.CODER_LOSSLESS_LATENT: 6), which must match dst's latent-ness."""
-        self._decode_raw(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, stream, _locked)
-
-    def decode_raw_heads(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
-                         ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
-                         src_H: int, src_head0: Sequence[int], dst_head0: Sequence[int], n_heads: Sequence[int],
-                         stream: Optional[torch.cuda.Stream] = None) -> None:
-        """decode_raw for a window of each container's heads (b200kv_lossless_decode_plan_heads): every container holds
-        src_H heads, and its heads [src_head0[j], src_head0[j] + n_heads[j]) land in dst's heads from dst_head0[j] on, at
-        token dst_tok[j], bit for bit as the source layout stored them.  The rest of dst is left as it was."""
-        self._decode_raw(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, stream, False,
-                         (src_H, src_head0, dst_head0, n_heads))
+        return plan
 
     @staticmethod
-    def _check_coder(coder: int, dst: KvView) -> None:
+    def encode_layers(plan: "N.LosslessEncodePlan", layer_begin: int, layer_end: int, stream: torch.cuda.Stream) -> None:
+        """b200kv_lossless_encode_layers: enqueue the encode of layers [layer_begin, layer_end)"""
+        N.check(N.lib().b200kv_lossless_encode_layers(ctypes.byref(plan), int(layer_begin), int(layer_end),
+                                                      stream.cuda_stream), "lossless_encode_layers")
+
+    @staticmethod
+    def encode_layers_finish(plan: "N.LosslessEncodePlan", stream: torch.cuda.Stream) -> None:
+        """b200kv_lossless_encode_layers_finish: enqueue the headers and container sizes"""
+        N.check(N.lib().b200kv_lossless_encode_layers_finish(ctypes.byref(plan), stream.cuda_stream),
+                "lossless_encode_layers_finish")
+
+    # ------------------------------------------------------------------ encode / decode hooks of _ContainerIO
+    def _encode_ws_bytes(self, view: KvView, chunk_size: int, n_chunks: int, coder: int) -> int:
+        return N.check(N.lib().b200kv_lossless_workspace_bytes(view.L, view.H, view.D, chunk_size, n_chunks,
+                                                               int(view.latent), 0), "lossless_workspace_bytes")
+
+    def _encode_launch(self, view: KvView, tok_begin: int, n_tokens: int, chunk_size: int, n_chunks: int, last: int,
+                       coder: int, out: torch.Tensor, stride: int, sizes: PinnedBuffer, stream) -> dict:
+        # the KV is read in stream order twice: histogram, then coding
+        N.check(N.lib().b200kv_lossless_encode(ctypes.byref(view.desc), tok_begin, n_chunks, chunk_size, last,
+                                               out.data_ptr(), stride, sizes.dev_ptr, self._enc_ws.data_ptr(),
+                                               self._enc_ws.numel(), stream.cuda_stream), "lossless_encode")
+        return {}
+
+    def _decode_ws_bytes(self, dst: KvView, src_H: int, tmax: int, n: int) -> int:
+        # < 0: a shape the plan call refuses, with its reason
+        return max(N.lib().b200kv_lossless_workspace_bytes(dst.L, int(src_H), dst.D, tmax, n, int(dst.latent), 1), 16)
+
+    def _plan_native(self, args: tuple, coder: int, dst: KvView, status, ws: torch.Tensor, stream,
+                     window: tuple) -> "N.LosslessDecodePlan":
+        # the library takes no coder: the destination says which version it decodes (6 for a latent one)
         if coder not in (N.CODER_LOSSLESS, N.CODER_LOSSLESS_LATENT) or bool(coder & N.KV_LATENT) != dst.latent:
             raise ValueError(f"coder {coder} does not name the lossless container of this destination")
-
-    def _decode_raw(self, base_ptr, buf_bytes, offsets, totals, ntokens, dst: KvView, dst_tok, max_dtype, coder, stream,
-                    _locked: bool, heads=None) -> None:
-        n = len(offsets)
-        if n == 0:
-            return
-        self._check_coder(coder, dst)
-        lib = N.lib()
-
-        def run():
-            tstream = stream if stream is not None else torch.cuda.current_stream()
-            ws_bytes = max(lib.b200kv_lossless_workspace_bytes(dst.L, int(heads[0]) if heads else dst.H, dst.D,
-                                                               max(ntokens), n, int(dst.latent), 1),
-                           0)          # < 0: a shape the decode call refuses, with its reason
-            if not _locked:
-                self._order_decode(tstream, 0, ws_bytes)
-            self._dec_ws = self._grow(self._dec_ws, max(ws_bytes, 16), dst.device)
-            args = (base_ptr, int(buf_bytes), N.i64_array(list(offsets)), N.i64_array(list(totals)),
-                    N.i32_array(list(ntokens)), N.i64_array(list(dst_tok)), n, int(max_dtype), ctypes.byref(dst.desc),
-                    self._status_buffer(n).dev_ptr, self._dec_ws.data_ptr(), self._dec_ws.numel())
-            if heads is None:
-                N.check(lib.b200kv_lossless_decode(*args, tstream.cuda_stream), "lossless_decode")
-            else:
-                plan = N.LosslessDecodePlan()
-                N.check(lib.b200kv_lossless_decode_plan_heads(*args, ctypes.byref(plan), tstream.cuda_stream,
-                                                              int(heads[0]), N.i32_array(list(heads[1])),
-                                                              N.i32_array(list(heads[2])), N.i32_array(list(heads[3]))),
-                        "lossless_decode_plan_heads")
-                self.decode_layers(plan, 0, dst.L, tstream)
-            if self._dec_event is None:
-                self._dec_event = torch.cuda.Event()
-            self._dec_event.record(tstream)
-
-        if _locked:
-            run()
-        else:
-            with self._dec_lock, torch.cuda.device(dst.device):
-                run()
-
-    def decode_plan(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
-                    ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
-                    stream: torch.cuda.Stream, status_ptr: int = 0) -> Tuple["N.LosslessDecodePlan", torch.Tensor]:
-        """CacheGenCodec.decode_plan for lossless containers (b200kv_lossless_decode_plan): enqueue on `stream` the
-        kernels that read [0, off_raw) of every container and return (plan, workspace); decode_layers decodes a range of
-        layers once its raw rows and streams are there.  The workspace is the caller's, recorded on `stream`."""
-        return self._decode_plan(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, stream,
-                                 status_ptr)
-
-    def decode_plan_heads(self, base_ptr: int, buf_bytes: int, offsets: Sequence[int], totals: Sequence[int],
-                          ntokens: Sequence[int], dst: KvView, dst_tok: Sequence[int], max_dtype: int, coder: int,
-                          src_H: int, src_head0: Sequence[int], dst_head0: Sequence[int], n_heads: Sequence[int],
-                          stream: torch.cuda.Stream, status_ptr: int = 0) -> Tuple["N.LosslessDecodePlan", torch.Tensor]:
-        """decode_plan for head windows (see decode_raw_heads); decode_layers runs the plan."""
-        return self._decode_plan(base_ptr, buf_bytes, offsets, totals, ntokens, dst, dst_tok, max_dtype, coder, stream,
-                                 status_ptr, (src_H, src_head0, dst_head0, n_heads))
-
-    def _decode_plan(self, base_ptr, buf_bytes, offsets, totals, ntokens, dst: KvView, dst_tok, max_dtype, coder, stream,
-                     status_ptr, heads=None) -> Tuple["N.LosslessDecodePlan", torch.Tensor]:
-        self._check_coder(coder, dst)
-        n = len(offsets)
-        lib = N.lib()
-        ws = torch.empty(max(lib.b200kv_lossless_workspace_bytes(dst.L, int(heads[0]) if heads else dst.H, dst.D,
-                                                                 max(ntokens), n, int(dst.latent), 1), 16),
-                         dtype=torch.uint8, device=dst.device)    # < 0: a shape the plan call refuses, with its reason
-        ws.record_stream(stream)
         plan = N.LosslessDecodePlan()
-        args = (base_ptr, int(buf_bytes), N.i64_array(list(offsets)), N.i64_array(list(totals)),
-                N.i32_array(list(ntokens)), N.i64_array(list(dst_tok)), n, int(max_dtype), ctypes.byref(dst.desc),
-                status_ptr or None, ws.data_ptr(), ws.numel(), ctypes.byref(plan), stream.cuda_stream)
-        if heads is None:
-            N.check(lib.b200kv_lossless_decode_plan(*args), "lossless_decode_plan")
+        args += (ctypes.byref(dst.desc), status, ws.data_ptr(), ws.numel(), ctypes.byref(plan), stream.cuda_stream)
+        if window:
+            N.check(N.lib().b200kv_lossless_decode_plan_heads(*args, *window), "lossless_decode_plan_heads")
         else:
-            N.check(lib.b200kv_lossless_decode_plan_heads(*args, int(heads[0]), N.i32_array(list(heads[1])),
-                                                          N.i32_array(list(heads[2])), N.i32_array(list(heads[3]))),
-                    "lossless_decode_plan_heads")
-        return plan, ws
+            N.check(N.lib().b200kv_lossless_decode_plan(*args), "lossless_decode_plan")
+        return plan
 
     @staticmethod
     def decode_layers(plan: "N.LosslessDecodePlan", layer_begin: int, layer_end: int, stream: torch.cuda.Stream) -> None:
@@ -1227,65 +1182,10 @@ class LosslessCodec(_ContainerIO):
         N.check(N.lib().b200kv_lossless_decode_layers(ctypes.byref(plan), int(layer_begin), int(layer_end),
                                                       stream.cuda_stream), "lossless_decode_layers")
 
-    def decode(self, containers: Sequence[Union[bytes, bytearray, memoryview, torch.Tensor]], dst: KvView,
-               dst_tok: Sequence[int], stream: Optional[torch.cuda.Stream] = None) -> None:
-        """Decode lossless containers into `dst` at token offsets `dst_tok` (asynchronous on `stream`).  Host
-        containers are uploaded first; a single 16-byte-aligned device tensor is used in place.  ValueError for a
-        container that is not lossless, whose kind (version 6: latent) or shape is not dst's, or whose dtype is not."""
-        n = len(containers)
-        if n == 0:
-            return
-        heads = []
-        for c in containers:
-            if isinstance(c, torch.Tensor):
-                hd = parse_lossless_header(c[:N.HEADER_BYTES].cpu().numpy().tobytes(), c.numel())
-            else:
-                hd = parse_lossless_header(c)
-            if not self.accepts(hd, dst.latent):
-                raise ValueError(f"a version-{hd.version} container does not fit a destination of "
-                                 f"{'one plane' if dst.latent else 'a (K, V) pair'} per layer")
-            if (hd.L, hd.H, hd.D) != (dst.L, dst.H, dst.D):
-                raise ValueError(f"container shape L/H/D={hd.L}/{hd.H}/{hd.D} does not match destination "
-                                 f"{dst.L}/{dst.H}/{dst.D}")
-            if hd.max_dtype != dst.dtype_code:
-                raise ValueError(f"container holds {dtype_of_code(hd.max_dtype)}, destination is {dst.dtype}: a lossless "
-                                 f"container is decoded into its own dtype")
-            heads.append(hd)
-        totals = [int(h.total_bytes) for h in heads]
-        ntoks = [int(h.ntokens) for h in heads]
-        for tok, nt in zip(dst_tok, ntoks):
-            if tok < 0 or tok + nt > dst.ntokens:
-                raise ValueError(f"container of {nt} tokens at offset {tok} does not fit a {dst.ntokens}-token destination")
-        coder = self.coder_for(max(ntoks), dst.latent)
-        lib = N.lib()
-        with self._dec_lock, torch.cuda.device(dst.device):
-            tstream = stream if stream is not None else torch.cuda.current_stream()
-            sp = tstream.cuda_stream
-            need_in = sum((t + 15) & ~15 for t in totals) + N.READ_SLACK
-            self._order_decode(tstream, need_in, lib.b200kv_lossless_workspace_bytes(dst.L, dst.H, dst.D, max(ntoks), n,
-                                                                                     int(dst.latent), 1))
-            if n == 1 and isinstance(containers[0], torch.Tensor) and containers[0].is_cuda \
-                    and containers[0].data_ptr() % 16 == 0 and containers[0].numel() >= totals[0] + N.READ_SLACK:
-                keep_dev = containers[0]
-                self.decode_raw(keep_dev.data_ptr(), keep_dev.numel(), [0], totals, ntoks, dst, dst_tok,
-                                dst.dtype_code, coder, tstream, _locked=True)
-                return
-            self._dec_in = self._grow(self._dec_in, need_in, dst.device)
-            base_ptr = self._dec_in.data_ptr()
-            offsets, o = [], 0
-            for c, nb in zip(containers, totals):
-                if isinstance(c, torch.Tensor):
-                    keep = c
-                    src_ptr = c.data_ptr()
-                else:
-                    keep = np.frombuffer(c, dtype=np.uint8, count=nb)   # zero-copy view of bytes/bytearray/memoryview
-                    src_ptr = keep.ctypes.data
-                N.check(lib.b200kv_copy_async(base_ptr + o, src_ptr, nb, sp), "copy")
-                del keep
-                offsets.append(o)
-                o += (nb + 15) & ~15
-            self.decode_raw(base_ptr, self._dec_in.numel(), offsets, totals, ntoks, dst, dst_tok, dst.dtype_code, coder,
-                            tstream, _locked=True)
+    def _check_container(self, hd: "N.Header", dst: KvView) -> None:
+        if hd.max_dtype != dst.dtype_code:
+            raise ValueError(f"container holds {dtype_of_code(hd.max_dtype)}, destination is {dst.dtype}: a lossless "
+                             f"container is decoded into its own dtype")
 
 
 def engine_codec(config, model_name: str) -> CacheGenCodec:

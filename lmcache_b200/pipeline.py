@@ -32,8 +32,7 @@ import numpy as np
 import torch
 
 from lmcache_b200 import _native as N
-from lmcache_b200.codec import (CacheGenCodec, EncodedBatch, EncodeTicket, KvView, PinnedBuffer, SegmentLayout,
-                                lossless_raw_rows)
+from lmcache_b200.codec import CacheGenCodec, EncodedBatch, EncodeTicket, KvView, PinnedBuffer, SegmentLayout
 
 
 def wave_chunks_default() -> int:
@@ -294,9 +293,8 @@ def land(slab, slot: WaveSlot, batch, blocks: Optional[list] = None,
             try:
                 # plane offsets of the wave, read on the device before the bytes leave it: no host pass over the
                 # lengths sections (on the store worker such a pass made every e2e store ~2 ms slower, measured)
-                N.check(getattr(N.pylib(), codec.plane_offsets_device)(
-                    ctypes.c_void_p(slot.dev.data_ptr()), batch.stride, len(blocks), ctypes.c_void_p(slot.planes.dev_ptr),
-                    cs.cuda_stream), codec.plane_offsets_device)
+                codec.plane_offsets_device(slot.dev.data_ptr(), batch.stride, len(blocks), slot.planes.dev_ptr,
+                                           cs.cuda_stream)
                 for j, (blk, size) in enumerate(zip(blocks, batch.sizes)):
                     N.check(N.lib().b200kv_copy_async(ctypes.c_void_p(blk.host_ptr),
                                                       ctypes.c_void_p(slot.dev.data_ptr() + j * batch.stride), size,
@@ -464,7 +462,6 @@ class LayerwiseEncode:
                     budget or layerwise_store_budget_default())
         ws_bytes = codec.layerwise_workspace_bytes(L, H, D, chunk_size, n, latent)
         self.codec, self.pool, self.view, self.L, self.n_chunks = codec, pool, view, L, n
-        self.plan = codec.layer_plan_type()
         self.slot = pool.acquire(arena, n * stride, ws_bytes, n, view.planes, codec.seg_row)
         s = self.slot
         s.n_chunks, s.P, s.seg_row, s.fixed_stride, s.coder = n, view.planes, codec.seg_row, stride, coder
@@ -473,7 +470,7 @@ class LayerwiseEncode:
         try:
             with torch.cuda.device(pool.device):
                 view.record_stream(pool.stream)          # the caller's KV outlives the encode's last read of it
-                codec.encode_layers_plan(view, tok_begin, n, chunk_size, last, s, self.plan, pool.stream)
+                self.plan = codec.encode_layers_plan(view, tok_begin, n, chunk_size, last, s, pool.stream)
         except BaseException:
             self.abandon()
             raise
@@ -483,14 +480,11 @@ class LayerwiseEncode:
             ev = torch.cuda.Event()
             ev.record(stream)
             self.pool.stream.wait_event(ev)
-            N.check(getattr(N.lib(), self.codec.encode_layers_fn)(ctypes.byref(self.plan), layer, layer + 1,
-                                                                  self.pool.stream.cuda_stream), "encode_layers")
+            self.codec.encode_layers(self.plan, layer, layer + 1, self.pool.stream)
 
     def finish(self) -> torch.cuda.Event:
         with torch.cuda.device(self.pool.device):
-            N.check(getattr(N.lib(), self.codec.encode_layers_finish_fn)(ctypes.byref(self.plan),
-                                                                         self.pool.stream.cuda_stream),
-                    "encode_layers_finish")
+            self.codec.encode_layers_finish(self.plan, self.pool.stream)
             self.done = torch.cuda.Event()
             self.done.record(self.pool.stream)
         self.slot.ticket = _SegmentTicket(self.slot, self.done, self.view)
@@ -969,7 +963,7 @@ def layer_copy_ranges(plane_offs: Sequence[Optional[np.ndarray]], nbytes: Sequen
     start int64[L, ppl * n], size int64[L, ppl * n]).  Container j's first fixed[j] bytes go first (its fixed sections;
     all of it when it has no plane offsets); row l holds the key ranges (plane l) of containers 0..n-1, then their value
     ranges (plane L + l).  A latent KV (ppl = 1, version 4: plane l is layer l) has one range per container in row l.
-    Lossless containers (versions 5 and 6) pass `raw`, their (off_raw, bytes per plane) (codec.lossless_raw_rows): then
+    Lossless containers (versions 5 and 6) pass `raw`, their (off_raw, bytes per plane) (codec.raw_rows): then
     fixed[j] is off_raw, the part the decode plan reads, and a plane is two ranges, its raw rows and its streams, so the
     rows are [L, 2 * ppl * n]: the raw ranges of every plane of the row, then the stream ranges.  Together they cover
     every container exactly once."""
@@ -1124,10 +1118,8 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
             host = np.array([r.blk.host_ptr for r in up], dtype=np.uint64)
             dev = base + np.array(offs, dtype=np.uint64)
             ppl = dst.planes // L
-            raw = None
-            if (first.coder & 0xff) == N.CODER_LOSSLESS:      # a plane is its raw rows and its streams
-                raw = [lossless_raw_rows(r.L, r.H, r.D, r.ntokens, dst.latent) for r in up]
-            fixed, lo, sz = layer_copy_ranges([r.planes for r in up], [r.nbytes for r in up], L, ppl, raw)
+            fixed, lo, sz = layer_copy_ranges([r.planes for r in up], [r.nbytes for r in up], L, ppl,
+                                              codec.raw_rows(up, dst.latent))
             k = lo.shape[1] // len(up)
             lay_src = np.ascontiguousarray(np.tile(np.concatenate([host] * k), (L, 1)) + lo.astype(np.uint64))
             lay_dst = np.ascontiguousarray(np.tile(np.concatenate([dev] * k), (L, 1)) + lo.astype(np.uint64))

@@ -26,7 +26,6 @@ from typing import Callable, Iterable, Iterator, List, Optional, Set, Tuple, Uni
 import numpy as np
 import torch
 
-from lmcache_b200 import _native as N
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.logging import init_logger
 from lmcache_b200.pipeline import DeferredFree
@@ -567,7 +566,6 @@ class LMCRemoteBackend(LMCBackendInterface):
         pipeline.LayerwiseUpload: n is known, ready(l) is the event after layer l's decode.  Every matched container
         sits in page-locked memory until its last copy.  A failed READ fails the upload: ready(l) raises for the layers
         not yet published (n was promised already), the blocks and handles are released."""
-        from lmcache_b200.codec import lossless_raw_rows
         from lmcache_b200.pipeline import (LayerwiseUpload, _continues_match, layer_copy_ranges, ranged_read_plan,
                                            upload_decode_layerwise, wave_chunks_default)
         self._release.sweep()
@@ -575,8 +573,7 @@ class LMCRemoteBackend(LMCBackendInterface):
         conns = self._lw_connections()
         k, pool = len(conns), self._lw_open_pool
         t_match = time.perf_counter()
-        lo = codec.layout(dst.L, dst.H, dst.D, chunk_size, dst.latent)
-        prefix = int(lo.off_raw if hasattr(lo, "off_raw") else lo.off_payload)     # the fixed sections of a full chunk
+        prefix = codec.plan_prefix(dst.L, dst.H, dst.D, chunk_size, dst.latent)     # the fixed sections of a full chunk
         bound = (self.deserializer.container_bound(dst.L, dst.H, dst.D, chunk_size, dst.latent) + 255) & ~255
         peek, self._peek = self._peek, None
         if peek is not None and not (len(keys) and peek[0] == keys[0]):
@@ -642,11 +639,8 @@ class LMCRemoteBackend(LMCBackendInterface):
             return LayerwiseUpload.completed(0, dst.L, ev)
         L = dst.L
         try:
-            raw = None
-            if (recs[0].coder & 0xff) == N.CODER_LOSSLESS:
-                raw = [lossless_raw_rows(r.L, r.H, r.D, r.ntokens, dst.latent) for r in recs]
             fixed, start, size = layer_copy_ranges([r.planes for r in recs], [r.nbytes for r in recs], L,
-                                                   dst.planes // L, raw)
+                                                   dst.planes // L, codec.raw_rows(recs, dst.latent))
             reads = ranged_read_plan(fixed, start, size, got, [j % k for j in range(n)], k)
             fetch = RangedFetch(conns, reads, handles, [r.blk.host_ptr for r in recs], L, self._count)
             fetch.start(self._lw_pool)

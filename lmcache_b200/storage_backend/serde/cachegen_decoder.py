@@ -1,6 +1,6 @@
 """CacheGenDeserializer -- the decode-side serde plugin (lmcache/storage_backend/serde/cachegen_decoder.py:109-202).
 
-from_bytes = one host->device copy of the container + one b200kv_decode_chunks call that writes the final
+from_bytes = one host->device copy of the container + one decode (b200kv_decode_plan + _layers) that writes the final
 bf16 (vllm) / fp16 (huggingface) blob directly (no uint8 / fp32 intermediates, no stack/permute/cast passes).
 """
 from typing import List, Optional, Sequence
