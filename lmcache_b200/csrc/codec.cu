@@ -352,13 +352,15 @@ __device__ __forceinline__ void for_each_symbol_rev(const uint16_t* cbase, const
 // rows each, over all C channels) and tpp tiles.  Tickets are claimed with one atomicAdd each and come in steps of
 // kAbsItems + tpp: step s holds the absmax items of unit s, then the tiles of unit s - kAbsLead.  A tile waits until its
 // unit's ready counter shows every absmax item done.
-// Measured on the H100 (DESIGN.md 3.2): 8 rows and a lead of 8 units beat 16 rows and leads of 2, 8 or 16 units.
+// Measured on the H100 (DESIGN.md 3.2): 8 rows and a lead of 16 units beat 4 rows and leads of 8, 24 and 32.
 constexpr int kAbsRows = 8;                   // token rows per absmax item: 2 per warp
 constexpr int kAbsItems = kGroup / kAbsRows;  // absmax items per unit (a ragged chunk's unused items only count as done)
-constexpr int kAbsLead = 8;                   // units by which a unit's absmax items run ahead of its tiles
+constexpr int kAbsLead = 16;                  // units by which a unit's absmax items run ahead of its tiles
 
 // The maxima of token rows [item * kAbsRows, +kAbsRows) of one unit, written to the container's maxes section exactly as
-// absmax_kernel writes them; then the unit's ready counter goes up by one.  Uses no shared memory.
+// absmax_kernel writes them; then the unit's ready counter goes up by one.  Uses no shared memory.  An item does not get
+// faster with more bytes in flight: 8 loads per lane measured the same, bulk copies into shared-memory slots slower
+// (DESIGN.md 3.2).
 template <bool PAGED>
 __device__ __forceinline__ void absmax_item(const EncParams& P, int unit, int item) {
     const int nloc = P.ppl * P.nlay;
@@ -453,18 +455,8 @@ __device__ __forceinline__ void encode_tile(const EncParams& P, TileOf tile_of, 
         uint16_t* hist = crow;
 #pragma unroll
         for (int i = 0; i < kLp; ++i) crow[i] = 0;
-        // pull the whole tile (gt token rows x 256 B) into L2 up front: one prefetch per 128-byte line, spread over
-        // the CTA, so pass 1's loads pay L2 latency instead of a DRAM round trip per batch
-        if (!PAGED) {
-            const int lines_per_tok = (ncols * 2 + 127) >> 7;
-            const uint16_t* tile0 = P.pt.p[nl] + (P.tok_begin + (int64_t)j * P.chunk_tokens + id.tok0) * P.sT +
-                                    (int64_t)((ct * CT) / P.D) * P.sH + ((ct * CT) % P.D);
-            if ((ct * CT) / P.D == (ct * CT + ncols - 1) / P.D)    // tile lies within one head row: contiguous per token
-                for (int i = tid; i < gt * lines_per_tok; i += CT) {
-                    const int tok = i / lines_per_tok, ln = i - tok * lines_per_tok;
-                    asm volatile("prefetch.global.L2 [%0];" ::"l"(tile0 + (int64_t)tok * s1 + ln * 64));
-                }
-        }
+        // No L2 prefetch of the tile's rows: its unit's absmax items read them shortly before, and a prefetch burst
+        // per tile made the encode slower (DESIGN.md 3.2).
         __syncthreads();   // fac ready
         if (active) {
             // ---- pass 1: batches of 12 tokens (two packed words), register double-buffered: the loads of batch b+1
