@@ -14,8 +14,9 @@
  *   - there is NO CPU fallback: without a CUDA device every compute entry point fails.
  *
  * KV layout: element (l, kv, tok, h, d) of the chunk/blob lives at
- *       base + (l*sL + kv*sKV + tok*sT + h*sH + d) * 2 bytes            (d is contiguous)
- *   or, when `planes` is non-NULL, at planes[kv*L + l] + (tok*sT + h*sH + d) * 2 bytes.
+ *       base + (l*sL + kv*sKV + tok*sT + h*sH + d) * es bytes           (d is contiguous)
+ *   or, when `planes` is non-NULL, at planes[kv*L + l] + (tok*sT + h*sH + d) * es bytes,
+ *   es = the element size of kv->dtype: 2 for B200KV_DT_BF16 / _FP16, 1 for B200KV_DT_U8 / _FP8_E4M3 / _FP8_E5M2.
  *   vllm blob [L,2,T,H,D]: sL=2*T*H*D sKV=T*H*D sT=H*D sH=D ; huggingface [L,2,H,T,D]: sT=D sH=T*D.
  *   The planes form takes the 2L tensors of the engine's kv tuple as they are
  *   (replaces the stack/stack/stack/permute + split/.contiguous() copies of
@@ -66,7 +67,7 @@ extern "C" {
                                                * 10+ KB).  Output bytes are identical either way. */
 #define B200KV_KV_LATENT 0x100  /* OR into b200kv_kv_desc.dtype: the KV holds ONE plane per layer (multi-head latent attention,
                                  * e.g. DeepSeek-V2/V3's [T, 576] latent vector), not a (K, V) pair.  Plane l of layer l is
-                                 * planes[l], or base + (l*sL + tok*sT + h*sH + d) * 2 (sKV unused); it is coded with layer l's
+                                 * planes[l], or base + (l*sL + tok*sT + h*sH + d) * es (sKV unused); it is coded with layer l's
                                  * KEY bins.  Such a descriptor reads and writes container version 4 = version 3 with L planes
                                  * instead of 2L (rANS-compact coder only; refused with coders 0 and 1).  OR it into `coder`
                                  * wherever a coder names a container: b200kv_container_layout_v, b200kv_encode_workspace_bytes
@@ -79,6 +80,14 @@ extern "C" {
 #define B200KV_MAX_PLANES 256   /* 2 * nlayers upper bound: models of up to 128 layers */
 #define B200KV_DT_BF16 0
 #define B200KV_DT_FP16 1
+/* One-byte elements (FP8 KV caches): torch.uint8 (vLLM 0.6.x allocates its fp8 cache so), torch.float8_e4m3fn,
+ * torch.float8_e5m2.  Added without changing anything that existed (b200kv_version() stays 4).  The mover and the
+ * lossless codec take them; the CacheGen entry points (b200kv_encode_chunks, b200kv_encode_layers_plan,
+ * b200kv_decode_chunks, b200kv_decode_plan, b200kv_decode_plan_heads) refuse them (< 0, nothing enqueued): their
+ * quantiser would round values FP8 has already rounded. */
+#define B200KV_DT_U8 2
+#define B200KV_DT_FP8_E4M3 3
+#define B200KV_DT_FP8_E5M2 4
 
 #define B200KV_READ_SLACK 640   /* bytes that must be readable past the end of every container handed to the decoder */
 #define B200KV_MAGIC 0x564B3242u /* "B2KV" little-endian */
@@ -317,12 +326,16 @@ int b200kv_encode_layers_finish(const b200kv_encode_plan_t* plan, void* stream);
  * and neither b200kv_container_layout_v nor the CacheGen decode calls know these versions.
  *
  * Version 5 holds a (K, V) KV of P = 2L planes (keys of layers 0..L-1, then values), version 6 a latent KV
- * (B200KV_KV_LATENT) of P = L planes.  header.max_dtype is the element dtype (bf16 or fp16), ngroups = 1, reserved = 0,
- * 1 <= ntokens = t <= 4096; C = H * D channels.  Every 16-bit element u is split, for both dtypes alike, as
+ * (B200KV_KV_LATENT) of P = L planes.  header.max_dtype is the element dtype (B200KV_DT_*), ngroups = 1, reserved = 0,
+ * 1 <= ntokens = t <= 4096; C = H * D channels.  Every 16-bit element u (bf16, fp16) is split, for both dtypes alike, as
  *     v = rotl16(u, 1),  sym = v >> 8,  raw = v & 0xff        (bf16: sym = the 8 exponent bits; fp16: the 5 exponent bits
  *                                                              and the 3 top mantissa bits), u = rotr16((sym << 8) | raw, 1)
+ * A one-byte element (B200KV_DT_U8, _FP8_E4M3, _FP8_E5M2) is its own symbol, sym = the byte, and has no raw byte: the
+ * raw section of such a container is empty (0 bytes, so off_payload == off_raw); everything else below is the same.
+ * A build that predates the one-byte dtypes refuses such a container through its max_dtype check, and off_payload
+ * follows from max_dtype, so a one-byte container is never read as a 16-bit one.
  * Sections, each starting 16-byte aligned, little-endian:
- *     header | freq u16[P][256] | lens u16[P][C] | raw u8[P][t][C] | streams
+ *     header | freq u16[P][256] | lens u16[P][C] | raw u8[P][t][C] (16-bit elements only) | streams
  * freq[p]: the symbol histogram n_s of plane p (its t * C elements, N = t * C) normalised to M = 4096:
  *     K = #{s : n_s > 0};  f_s = 0 if n_s = 0, else 1 + floor(n_s * (4096 - K) / N)      (integer arithmetic)
  *     then the symbol with the largest n_s (the smallest symbol among equals) gets 4096 - sum(f) added.
@@ -342,7 +355,8 @@ int b200kv_encode_layers_finish(const b200kv_encode_plan_t* plan, void* stream);
  *   The renormalisation bound is f << 20; it is tested as (x >> 20) >= f because a single-symbol plane has f = 4096 and
  *   4096 << 20 overflows 32 bits (such a plane's streams are the 4 bytes of x = 2^16 and nothing else).  A stream is at
  *   most 4 + 2 * ceil(3t / 4) + 2 bytes (12 bits per symbol), which fits u16 for t <= 4096; an encode whose stream
- *   exceeds it sets header.status bit 0 (sizes_out 0).  tests/lossless_ref.py is the numpy statement of all this.
+ *   exceeds it sets header.status bit 0 (sizes_out 0).  tests/lossless_ref.py is the numpy statement of all this for
+ *   16-bit elements, tests/lossless8_ref.py for one-byte ones.
  */
 typedef struct b200kv_lossless_layout_t {
     int64_t off_freq, off_lens, off_raw, off_payload;
@@ -351,10 +365,17 @@ typedef struct b200kv_lossless_layout_t {
     int64_t max_total_bytes;   /* align16(off_payload + P * C * max_stream_bytes): the out_stride an encode needs */
 } b200kv_lossless_layout_t;
 
-/* Section offsets of a version-5 (latent = 0) or version-6 (latent != 0) container; L <= 128, 1 <= ntokens <= 4096. */
+/* Section offsets of a version-5 (latent = 0) or version-6 (latent != 0) container of 16-bit elements; L <= 128,
+ * 1 <= ntokens <= 4096. */
 int b200kv_lossless_layout(int32_t L, int32_t H, int32_t D, int32_t ntokens, int32_t latent, b200kv_lossless_layout_t* out);
+/* The same for elements of `dtype` (B200KV_DT_*, without the latent flag): for a one-byte dtype off_payload == off_raw
+ * and max_total_bytes has no raw section.  A 16-bit layout bounds the one-byte layout of the same shape field by field. */
+int b200kv_lossless_layout_dt(int32_t L, int32_t H, int32_t D, int32_t ntokens, int32_t latent, int32_t dtype,
+                              b200kv_lossless_layout_t* out);
 /* Bytes of device scratch one b200kv_lossless_encode (decode = 0) or b200kv_lossless_decode (decode != 0) call needs;
- * < 0 for a shape the calls refuse.  The encode's is dominated by a worst-case scratch row per stream. */
+ * < 0 for a shape the calls refuse.  The encode's is dominated by a worst-case scratch row per stream.  The figure is
+ * that of 16-bit elements and bounds the need of one-byte elements too (this and
+ * b200kv_lossless_encode_layers_workspace_bytes take no dtype). */
 int64_t b200kv_lossless_workspace_bytes(int32_t L, int32_t H, int32_t D, int32_t chunk_tokens, int32_t n_chunks,
                                         int32_t latent, int32_t decode);
 /*
@@ -386,8 +407,9 @@ int b200kv_lossless_decode(const void* containers, int64_t containers_bytes, con
 
 /* Host side: where each plane's streams lie in a lossless container in host memory (the header and the lengths section
  * are read, nothing else; nbytes >= off_raw): out[0..P], the streams of plane p (keys of layer p, then values of layer
- * p - L; P = L for version 6) are bytes [out[p], out[p+1]) of the container, out[0] = off_payload.  Plane p's raw rows are
- * bytes [off_raw + p * t * C, off_raw + (p + 1) * t * C): the layout gives them.  Returns 0, 1 when the lengths do not
+ * p - L; P = L for version 6) are bytes [out[p], out[p+1]) of the container, out[0] = off_payload (the header's
+ * max_dtype decides it).  Plane p's raw rows are bytes [off_raw + p * t * C, off_raw + (p + 1) * t * C) for 16-bit
+ * elements, none for one-byte ones: b200kv_lossless_layout_dt gives them.  Returns 0, 1 when the lengths do not
  * add up to header.total_bytes (damaged), <0 for anything that is not a lossless container of a possible shape. */
 int b200kv_lossless_plane_offsets(const void* container, int64_t nbytes, int64_t* out, int32_t n_out);
 /* Same for n containers in DEVICE memory at containers + j*stride, as b200kv_plane_offsets_device: row j of out (DEVICE or
@@ -463,8 +485,9 @@ int b200kv_lossless_decode_plan_heads(const void* containers, int64_t containers
  * layer_begin.., or planes layer_begin.. alone for version 6 -- of every chunk: the histograms and frequency rows
  * (into the fixed image), the coding (lengths into the fixed image), and one segment per chunk in the device arena of
  * arena_bytes bytes:
- *     [the call's planes' raw rows, t * C bytes each, in plane order; in the call that holds the last plane followed by
- *      the container's zero bytes up to off_payload; zeros to a 16-byte boundary] [the call's planes' streams, in order]
+ *     [the call's planes' raw rows, t * C bytes each (none for one-byte elements), in plane order; in the call that
+ *      holds the last plane followed by the container's zero bytes up to off_payload; zeros to a 16-byte boundary]
+ *     [the call's planes' streams, in order]
  * Segments are placed by the rule of b200kv_encode_layers (16-byte aligned at a device-held cursor in (call, chunk)
  * order, with a reserve for the layers still to come; the chunks that fit are always a prefix).  Row (j, p) of
  * seg_sizes_out (DEVICE or mapped-host int64[n_chunks][P][3], P = 2L or L) gets (arena offset of plane p's raw rows,
@@ -477,7 +500,8 @@ int b200kv_lossless_decode_plan_heads(const void* containers, int64_t containers
  * stream outgrew its bound), and fails unless every layer was encoded.
  *
  * For every chunk that did not fail, fixed image [0, off_raw) || for p = 0..P-1 the raw bytes at row (j, p)[0]
- * (t * C of them; for p = P - 1 up to off_payload) || for p = 0..P-1 the row (j, p)[2] stream bytes at row (j, p)[1]
+ * (t * C of them, 0 for one-byte elements; for p = P - 1 up to off_payload) || for p = 0..P-1 the row (j, p)[2] stream
+ * bytes at row (j, p)[1]
  * is byte for byte the container b200kv_lossless_encode writes.  Every refusal returns < 0 and enqueues nothing: a layer
  * range out of bounds or encoded before, finish before every layer was encoded, a plan not made by
  * b200kv_lossless_encode_layers_plan, a misaligned arena or fixed image, a too small fixed stride or workspace, and the
@@ -524,7 +548,8 @@ int b200kv_sha256_chain_ready(const void* tokens, int32_t elem_size, const int64
  * (cache_engine.py:98-161,362-368) with one gather / scatter kernel.
  * `chunks` is DEVICE memory, or pinned host memory mapped into the device address space (then the kernel
  * itself is the GPU->host mover).  Chunk j starts at chunks + j*chunk_stride_bytes.
- * hf_layout != 0 selects the huggingface chunk layout.
+ * hf_layout != 0 selects the huggingface chunk layout.  Elements of every B200KV_DT_* move as they are (16-byte
+ * vectors when D, the strides and the pointers allow it, element by element otherwise).
  */
 int b200kv_pack_chunks(const b200kv_kv_desc* src, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
                        int32_t last_chunk_tokens, int32_t hf_layout, void* chunks, int64_t chunk_stride_bytes,

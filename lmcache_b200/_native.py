@@ -16,6 +16,10 @@ LIB_PATH = os.path.join(_HERE, "libb200kv.so")
 
 DT_BF16 = 0
 DT_FP16 = 1
+DT_U8 = 2           # one-byte elements: torch.uint8 (vLLM 0.6.x's fp8 cache), float8_e4m3fn, float8_e5m2
+DT_FP8_E4M3 = 3
+DT_FP8_E5M2 = 4
+ONE_BYTE_DTYPES = (DT_U8, DT_FP8_E4M3, DT_FP8_E5M2)
 CODER_AC = 0       # container version 1: arithmetic coder
 CODER_RANS = 1     # container version 2: rANS
 CODER_RANS_COMPACT = 2   # container version 3: rANS streams that carry their own histogram (no CDF section), one-byte lengths
@@ -127,6 +131,7 @@ SIGNATURES = {
     "b200kv_encode_layers": (c_i32, [ctypes.POINTER(EncodePlan), c_i32, c_i32, c_vp]),
     "b200kv_encode_layers_finish": (c_i32, [ctypes.POINTER(EncodePlan), c_vp]),
     "b200kv_lossless_layout": (c_i32, [c_i32, c_i32, c_i32, c_i32, c_i32, ctypes.POINTER(LosslessLayout)]),
+    "b200kv_lossless_layout_dt": (c_i32, [c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, ctypes.POINTER(LosslessLayout)]),
     "b200kv_lossless_workspace_bytes": (c_i64, [c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
     "b200kv_lossless_encode": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp, c_vp,
                                         c_i64, c_vp]),
@@ -279,10 +284,12 @@ def planes_of(version: int, L: int) -> int:
     return L if version in (4, 6) else 2 * L
 
 
-def lossless_layout(L: int, H: int, D: int, ntokens: int, latent: bool = False) -> LosslessLayout:
-    """Section offsets of a lossless container (version 5, or 6 for a latent KV)."""
+def lossless_layout(L: int, H: int, D: int, ntokens: int, latent: bool = False, dtype: int = DT_BF16) -> LosslessLayout:
+    """Section offsets of a lossless container (version 5, or 6 for a latent KV) of elements of `dtype` (DT_*): a
+    one-byte dtype has no raw section."""
     lo = LosslessLayout()
-    check(lib().b200kv_lossless_layout(L, H, D, ntokens, int(bool(latent)), ctypes.byref(lo)), "lossless_layout")
+    check(lib().b200kv_lossless_layout_dt(L, H, D, ntokens, int(bool(latent)), int(dtype), ctypes.byref(lo)),
+          "lossless_layout")
     return lo
 
 

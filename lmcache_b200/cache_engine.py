@@ -19,7 +19,7 @@ from typing import Callable, Dict, Iterable, List, Optional, Tuple, Union
 import torch
 
 from lmcache_b200 import _native as N
-from lmcache_b200.codec import KvView, PinnedBuffer
+from lmcache_b200.codec import NATIVE_DTYPES, KvView, PinnedBuffer
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.logging import init_logger
 from lmcache_b200.storage_backend import CreateStorageBackend
@@ -29,6 +29,12 @@ from lmcache_b200.utils import CacheEngineKey, KVCache, _lmcache_nvtx_annotate
 
 logger = init_logger(__name__)
 
+
+
+def _bytes_of(t: torch.Tensor) -> torch.Tensor:
+    """A one-byte (FP8) tensor as its bytes, any other as it is: the paged gathers and scatters index the bytes, as
+    indexed reads and writes do not take every float8 dtype."""
+    return t.view(torch.uint8) if t.element_size() == 1 else t
 
 class LazySeq:
     """A read-only sequence whose items are computed on access: fn(base[i]).  Slices stay lazy.  The engine passes its
@@ -418,9 +424,10 @@ class LMCacheEngine:
 
         def put(keys, tok_begin):
             kv_cuda = self._as_cuda_kv(kv_tensors_raw)
-            if self._first(kv_cuda).dtype not in (torch.bfloat16, torch.float16):
-                # the native pack / codec kernels move 16-bit KV; any other dtype (the reference's local and torch-serde
-                # paths accept every dtype) takes the reference's own blob ops on the GPU (cache_engine.py:98-161)
+            if self._first(kv_cuda).dtype not in NATIVE_DTYPES:
+                # the native pack / codec kernels move 16-bit and one-byte (FP8) KV; any other dtype (the reference's
+                # local and torch-serde paths accept every dtype) takes the reference's own blob ops on the GPU
+                # (cache_engine.py:98-161)
                 chunks = self._pack_chunks_torch(kv_cuda, tok_begin, fmt)
                 return self.engine_.batched_put(zip(keys, chunks), blocking=blocking)
             view = KvView.from_tuple(kv_cuda, fmt)
@@ -502,7 +509,8 @@ class LMCacheEngine:
         if not self._fast_path():
             flat = self._flat_paged(kv_caches)
             idx = slot_mapping.to(self._first(flat).device)
-            kv = tuple(c[idx] for c in flat) if self._mla else tuple((k[idx], v[idx]) for k, v in flat)
+            g = lambda c: _bytes_of(c)[idx].view(c.dtype)  # noqa: E731
+            kv = tuple(g(c) for c in flat) if self._mla else tuple((g(k), g(v)) for k, v in flat)
             return self.store(tokens, kv, skip_existing, blocking)
         chunk_hashes = self._prefix_hash(tokens)
         start = self._skip_scan(chunk_hashes, "vllm") if skip_existing else 0
@@ -535,11 +543,11 @@ class LMCacheEngine:
                 idx = slots[ret_mask.to(dev)]
                 if self._mla:
                     for c, x in zip(flat, kv):
-                        c[idx] = x.to(c.dtype)
+                        _bytes_of(c)[idx] = _bytes_of(x.to(c.dtype))
                 else:
                     for (kc, vc), (k, v) in zip(flat, kv):
-                        kc[idx] = k.to(kc.dtype)
-                        vc[idx] = v.to(vc.dtype)
+                        _bytes_of(kc)[idx] = _bytes_of(k.to(kc.dtype))
+                        _bytes_of(vc)[idx] = _bytes_of(v.to(vc.dtype))
             return ret_mask
         cs = self.chunk_size
         ret_mask, num_skip_tok, num_skip_chunk, extra = self._split_mask(tokens, mask)
@@ -559,11 +567,11 @@ class LMCacheEngine:
                 idx = slots[base + extra: base + t0]
                 if self._mla:
                     for l, c in enumerate(flat):
-                        c[idx] = tmp[l, extra:]
+                        _bytes_of(c)[idx] = _bytes_of(tmp[l, extra:])
                 else:
                     for l, (kc, vc) in enumerate(flat):
-                        kc[idx] = tmp[l, 0, extra:]
-                        vc[idx] = tmp[l, 1, extra:]
+                        _bytes_of(kc)[idx] = _bytes_of(tmp[l, 0, extra:])
+                        _bytes_of(vc)[idx] = _bytes_of(tmp[l, 1, extra:])
         if got_chunks == first and len(chunk_hashes) > first:       # not after a straddling chunk that missed
             layout, own_rest, n = self._fetch(chunk_hashes[first:], "vllm", view, first * cs, get_kv, layout)
             own += own_rest
@@ -768,11 +776,11 @@ class LMCacheEngine:
 
     # ------------------------------------------------------------------ layer-wise store
     def _layerwise_store_ok(self, dtype: torch.dtype) -> bool:
-        """Can this store be encoded layer by layer?  The compressed host and disk tiers can, for 16-bit KV and chunks of
-        at most the tier's layerwise_max_tokens (256 for CacheGen's version-3 containers, 4096 for lossless ones); raw,
-        remote and hybrid tiers cannot."""
+        """Can this store be encoded layer by layer?  The compressed host and disk tiers can, for the KV their codec
+        encodes (CacheGen: 16-bit; lossless: 16-bit and one-byte) and chunks of at most the tier's layerwise_max_tokens
+        (256 for CacheGen's version-3 containers, 4096 for lossless ones); raw, remote and hybrid tiers cannot."""
         return (getattr(self.engine_, "begin_layerwise_store", None) is not None and self._fast_path() and
-                self.chunk_size <= self.engine_.layerwise_max_tokens and dtype in (torch.bfloat16, torch.float16))
+                self.chunk_size <= self.engine_.layerwise_max_tokens and dtype in NATIVE_DTYPES)
 
     def _begin_layerwise(self, tokens, view_fn, fmt: str, num_layers: int, skip_existing: bool,
                          fallback: Callable) -> LayerwiseStore:

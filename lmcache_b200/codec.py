@@ -18,8 +18,13 @@ import torch
 
 from lmcache_b200 import _native as N
 
-_DTYPE_CODE = {torch.bfloat16: N.DT_BF16, torch.float16: N.DT_FP16}
+_DTYPE_CODE = {torch.bfloat16: N.DT_BF16, torch.float16: N.DT_FP16, torch.uint8: N.DT_U8,
+               torch.float8_e4m3fn: N.DT_FP8_E4M3, torch.float8_e5m2: N.DT_FP8_E5M2}
 _CODE_DTYPE = {v: k for k, v in _DTYPE_CODE.items()}
+NATIVE_DTYPES = tuple(_DTYPE_CODE)      # the element dtypes the kernels move and the lossless codec stores
+# CacheGen quantises 16-bit KV only; what a CacheGen serde or tier says to a one-byte (FP8) KV
+_CACHEGEN_FP8 = ("CacheGen codes bfloat16 and float16 KV only, not {}: FP8 KV is stored bit-exact by the lossless codec "
+                 "(local_serde: lossless / remote_serde: lossless), or raw on the cpu / cuda tiers")
 
 
 def _stream_ptr(stream: Optional[torch.cuda.Stream]) -> int:
@@ -108,7 +113,8 @@ class KvView:
     @staticmethod
     def _code(dtype: torch.dtype) -> int:
         if dtype not in _DTYPE_CODE:
-            raise TypeError(f"KV dtype must be bfloat16 or float16, got {dtype}")
+            raise TypeError(f"KV dtype must be bfloat16, float16 or a one-byte type (uint8, float8_e4m3fn, "
+                            f"float8_e5m2), got {dtype}")
         return _DTYPE_CODE[dtype]
 
     # A chunk blob holds t tokens of every layer: [L,2,t,H,D] (vllm) or [L,2,H,t,D] (huggingface); a latent one [L,t,D]
@@ -905,6 +911,8 @@ class CacheGenCodec(_ContainerIO):
         return lo.max_total_bytes
 
     def _check_source(self, view: KvView) -> None:
+        if view.dtype_code in N.ONE_BYTE_DTYPES:
+            raise TypeError(_CACHEGEN_FP8.format(view.dtype))
         if view.L > self.nlayers:
             raise ValueError(f"KV has {view.L} layers but the bin table of this model has {self.nlayers}")
 
@@ -913,7 +921,9 @@ class CacheGenCodec(_ContainerIO):
     # is (arena offset, bytes) of the plane's streams
     seg_row = 2
 
-    def segment_layout(self, L: int, H: int, D: int, ntokens: int, latent: bool = False) -> SegmentLayout:
+    def segment_layout(self, L: int, H: int, D: int, ntokens: int, latent: bool = False,
+                       dtype: int = N.DT_BF16) -> SegmentLayout:
+        """dtype: the KV's N.DT_* (16-bit: the only kind this codec encodes)"""
         lo = N.container_layout(L, H, D, ntokens, N.CODER_LATENT if latent else N.CODER_RANS_COMPACT)
         return SegmentLayout(int(lo.off_payload), int(lo.off_payload))
 
@@ -975,6 +985,8 @@ class CacheGenCodec(_ContainerIO):
 
     def _plan_native(self, args: tuple, coder: int, dst: KvView, status, ws: torch.Tensor, stream,
                      window: tuple) -> "N.DecodePlan":
+        if dst.dtype_code in N.ONE_BYTE_DTYPES:
+            raise TypeError(_CACHEGEN_FP8.format(dst.dtype))
         plan = N.DecodePlan()
         args += (int(coder), ctypes.byref(dst.desc), self._kb, self._vb, status, ws.data_ptr(), ws.numel(),
                  ctypes.byref(plan), stream.cuda_stream)
@@ -991,6 +1003,8 @@ class CacheGenCodec(_ContainerIO):
                 "decode_layers")
 
     def _check_container(self, hd: "N.Header", dst: KvView) -> None:
+        if dst.dtype_code in N.ONE_BYTE_DTYPES:
+            raise TypeError(_CACHEGEN_FP8.format(dst.dtype))
         if not self.accepts(hd, dst.latent):
             raise ValueError("compact container written with another model's bins" if hd.version >= 3 else
                              f"a codec made from a cachegen_config reads version 3 only, not version {hd.version}")
@@ -1017,16 +1031,17 @@ def parse_lossless_header(buf, total: Optional[int] = None) -> N.Header:
 
 
 def check_lossless_header(hd: "N.Header") -> None:
-    """Structural checks of a lossless header: a possible shape (L <= 128 layers, 1..4096 tokens), a 16-bit dtype, one
-    group, and total_bytes = fixed sections + payload_bytes with a payload between 4 bytes per stream and the worst case."""
+    """Structural checks of a lossless header: a possible shape (L <= 128 layers, 1..4096 tokens), a known element dtype
+    (16-bit or one-byte), one group, and total_bytes = fixed sections + payload_bytes with a payload between 4 bytes per
+    stream and the worst case."""
     if not (0 < hd.L <= N.MAX_PLANES // 2 and hd.H > 0 and hd.D > 0 and hd.H * hd.D < (1 << 24) and
             0 < hd.ntokens <= N.LOSSLESS_MAX_TOKENS):
         raise ValueError("B2KV header carries an impossible shape")
-    if hd.max_dtype not in (N.DT_BF16, N.DT_FP16):
+    if hd.max_dtype not in _CODE_DTYPE:
         raise ValueError("B2KV header carries an unknown element dtype")
     if hd.ngroups != 1 or any(hd.reserved):
         raise ValueError("B2KV lossless header: ngroups must be 1 and reserved 0")
-    lo = N.lossless_layout(hd.L, hd.H, hd.D, hd.ntokens, hd.version == 6)
+    lo = N.lossless_layout(hd.L, hd.H, hd.D, hd.ntokens, hd.version == 6, hd.max_dtype)
     if hd.total_bytes != lo.off_payload + hd.payload_bytes:
         raise ValueError("B2KV header: total_bytes != fixed sections + payload_bytes (truncated or corrupt)")
     nstreams = N.planes_of(hd.version, hd.L) * hd.H * hd.D
@@ -1038,15 +1053,18 @@ def lossless_plane_offsets(buf) -> Optional[np.ndarray]:
     """Where the streams of each plane lie in a lossless container (`buf`: at least its header, frequency rows and
     lengths), from its lengths section: int64[P + 1] (P = 2L, or L for version 6), the streams of plane p are bytes
     [o[p], o[p + 1]) of the container, o[0] is off_payload and o[P] == total_bytes.  None when the lengths do not add up
-    to the header's total (a damaged container: it is only ever uploaded whole).  Plane p's raw rows come from the
-    layout: LosslessCodec.raw_rows."""
+    to the header's total (a damaged container: it is only ever uploaded whole).  Plane p's raw rows (none for one-byte
+    elements) come from the layout: LosslessCodec.raw_rows."""
     return _plane_offsets(buf, (5, 6), N.lib().b200kv_lossless_plane_offsets, "lossless_plane_offsets")
 
 
 class LosslessCodec(_ContainerIO):
     """Lossless encode / decode on the current CUDA device (container versions 5 and 6, include/b200kv.h): every
     element's high byte after a one-bit rotation (bf16: the exponent) is rANS-coded per (plane, channel) against one
-    frequency row per plane, the low byte is kept verbatim, and the decode gives back the same bits.  It presents what the
+    frequency row per plane, the low byte is kept verbatim, and the decode gives back the same bits.  A one-byte element
+    (FP8, uint8) is coded whole: its container has no raw section.  Sizes this codec reserves (out_stride,
+    max_container_bytes, layerwise_chunk_bound) are those of 16-bit elements, which bound the one-byte ones; the exact
+    layouts (layout, segment_layout, raw_rows) follow the element dtype.  It presents what the
     remote tier's pipelines take from CacheGenCodec; it needs no model table, and decodes into the stored dtype only.
 
     Thread model as CacheGenCodec: one encoder and one decoder may run concurrently from different threads."""
@@ -1068,10 +1086,11 @@ class LosslessCodec(_ContainerIO):
 
     @staticmethod
     def raw_rows(records, latent: bool = False) -> List[Tuple[int, int]]:
-        """layer_copy_ranges' `raw` for these containers (records with L, H, D and ntokens): per container (off_raw,
-        bytes per plane), plane p's raw rows are bytes [off_raw + p * t * C, off_raw + (p + 1) * t * C)"""
-        return [(int(N.lossless_layout(r.L, r.H, r.D, r.ntokens, latent).off_raw), int(r.ntokens) * r.H * r.D)
-                for r in records]
+        """layer_copy_ranges' `raw` for these containers (records with L, H, D, ntokens and max_dtype): per container
+        (off_raw, bytes per plane), plane p's raw rows are bytes [off_raw + p * t * C, off_raw + (p + 1) * t * C); 0
+        bytes per plane for one-byte elements"""
+        return [(int(N.lossless_layout(r.L, r.H, r.D, r.ntokens, latent, r.max_dtype).off_raw),
+                 0 if r.max_dtype in N.ONE_BYTE_DTYPES else int(r.ntokens) * r.H * r.D) for r in records]
 
     def plan_prefix(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> int:
         """bytes [0, n) of a full chunk's container that decode_plan reads: [0, off_raw)"""
@@ -1089,9 +1108,11 @@ class LosslessCodec(_ContainerIO):
         6) or of (K, V) pairs (version 5)?"""
         return hd.version in (5, 6) and (hd.version == 6) == latent
 
-    def layout(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> "N.LosslessLayout":
+    def layout(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False,
+               dtype: int = N.DT_BF16) -> "N.LosslessLayout":
+        """the container of elements of `dtype` (N.DT_*); the 16-bit one by default, which bounds the one-byte one"""
         self.coder_for(chunk_tokens, latent)
-        return N.lossless_layout(L, H, D, chunk_tokens, latent)
+        return N.lossless_layout(L, H, D, chunk_tokens, latent, dtype)
 
     def out_stride(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> int:
         """Bytes reserved per container: the worst case, every stream at 12 bits per symbol."""
@@ -1106,9 +1127,10 @@ class LosslessCodec(_ContainerIO):
     # plane's raw rows, arena offset of its streams, stream bytes)
     seg_row = 3
 
-    def segment_layout(self, L: int, H: int, D: int, ntokens: int, latent: bool = False) -> SegmentLayout:
-        lo = self.layout(L, H, D, ntokens, latent)
-        return SegmentLayout(int(lo.off_raw), int(lo.off_payload), int(ntokens) * H * D)
+    def segment_layout(self, L: int, H: int, D: int, ntokens: int, latent: bool = False,
+                       dtype: int = N.DT_BF16) -> SegmentLayout:
+        lo = self.layout(L, H, D, ntokens, latent, dtype)
+        return SegmentLayout(int(lo.off_raw), int(lo.off_payload), 0 if dtype in N.ONE_BYTE_DTYPES else int(ntokens) * H * D)
 
     def layerwise_chunk_bound(self, L: int, H: int, D: int, chunk_tokens: int, latent: bool = False) -> int:
         """arena bytes a chunk can take: everything of its worst case after the fixed image, and per layer the alignment

@@ -1635,13 +1635,15 @@ int make_plane_table(const b200kv_kv_desc* kv, const float* key_bins, const floa
     B2_REQUIRE(kv != nullptr, "kv descriptor is NULL");
     B2_REQUIRE(kv->L > 0 && 2 * kv->L <= B200KV_MAX_PLANES, "L out of range");
     B2_REQUIRE(kv->H > 0 && kv->D > 0, "H/D must be positive");
-    B2_REQUIRE(kv_dtype(kv) == B200KV_DT_BF16 || kv_dtype(kv) == B200KV_DT_FP16, "dtype must be bf16 or fp16");
+    const int es = kv_elem_bytes(kv);
+    B2_REQUIRE(es != 0, "dtype must be one of B200KV_DT_*");
     B2_REQUIRE(kv->planes != nullptr || kv->base != nullptr, "no KV pointer");
     for (int kvi = 0; kvi < kv_ppl(kv); ++kvi)
         for (int l = 0; l < kv->L; ++l) {
             const int nl = kvi * kv->L + l;
-            const uint16_t* p = kv->planes ? static_cast<const uint16_t*>(kv->planes[nl])
-                                           : static_cast<const uint16_t*>(kv->base) + l * kv->sL + kvi * kv->sKV;
+            const uint16_t* p = reinterpret_cast<const uint16_t*>(
+                kv->planes ? static_cast<const uint8_t*>(kv->planes[nl])
+                           : static_cast<const uint8_t*>(kv->base) + (l * kv->sL + kvi * kv->sKV) * es);
             B2_REQUIRE(p != nullptr, "NULL plane pointer");
             out->p[nl] = p;
             const float bins = kvi ? value_bins[l] : key_bins[l];
@@ -1652,6 +1654,15 @@ int make_plane_table(const b200kv_kv_desc* kv, const float* key_bins, const floa
 }
 
 static int tiles_per_plane(int C) { return (C + CT - 1) / CT; }
+
+// The CacheGen codec quantises 16-bit elements: a one-byte KV (FP8) is refused here, before anything is enqueued, and
+// stored by the lossless codec instead
+static int cachegen_dtype_ok(const b200kv_kv_desc* kv) {
+    B2_REQUIRE(kv != nullptr, "kv descriptor is NULL");
+    B2_REQUIRE(kv_elem_bytes(kv) == 2,
+               "CacheGen codes bf16 / fp16 KV only; one-byte (FP8) KV is stored by the lossless codec");
+    return 0;
+}
 
 // ---- optional per-kernel timing (bench.py's roofline leg): events around each launch of the last call
 enum { kProfAbsmax = 0, kProfCdf, kProfEncode, kProfFinalize, kProfTileSum, kProfTileScan, kProfDecode, kProfCount };
@@ -1901,6 +1912,7 @@ int b200kv_encode_chunks(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     EncParams P;
     B2_REQUIRE(key_bins && value_bins, "bins are NULL");
+    if (int rc = cachegen_dtype_ok(kv)) return rc;
     const bool hint_mid = (coder & B200KV_ENCODE_HINT_MID_ENTROPY) != 0;
     coder &= 0xff;
     B2_REQUIRE(coder >= CODER_AC && coder <= CODER_RANS_COMPACT, "coder must be one of B200KV_CODER_*");
@@ -2054,6 +2066,7 @@ int b200kv_encode_layers_plan(const b200kv_kv_desc* kv, int64_t tok_begin, int32
     B2_REQUIRE(key_bins && value_bins, "bins are NULL");
     B2_REQUIRE((coder & 0xff) == CODER_RANS_COMPACT,
                "the layer-wise encode writes compact containers only (B200KV_CODER_RANS_COMPACT)");
+    if (int rc = cachegen_dtype_ok(kv)) return rc;
     if (int rc = make_plane_table(kv, key_bins, value_bins, &P.pt)) return rc;
     P.ppl = kv_ppl(kv);
     B2_REQUIRE(n_chunks > 0 && chunk_tokens > 0, "n_chunks / chunk_tokens must be positive");
@@ -2165,6 +2178,7 @@ static int decode_plan_impl(const void* containers, int64_t containers_bytes, co
     DecParams& P = plan->P;
     B2_REQUIRE(key_bins && value_bins, "bins are NULL");
     B2_REQUIRE(dst != nullptr, "destination descriptor is NULL");
+    if (int rc = cachegen_dtype_ok(dst)) return rc;
     const bool latent = (coder & B200KV_KV_LATENT) != 0;
     coder &= ~B200KV_KV_LATENT;
     B2_REQUIRE(coder >= CODER_AC && coder <= CODER_RANS_COMPACT, "coder must be one of B200KV_CODER_*");

@@ -36,7 +36,7 @@ void set_error(const std::string& msg);   // thread-local last error (api.cu)
 // that holds one stays under the classic 4 KB kernel-parameter limit (static_asserts next to each).
 template <int N>
 struct PlaneTableT {
-    const uint16_t* p[N];
+    const uint16_t* p[N];                // first element of the plane; one-byte elements: read it as a uint8_t*
     float maxq[N];                       // bins // 2 - 1
 };
 using PlaneTable = PlaneTableT<B200KV_MAX_PLANES>;
@@ -45,9 +45,15 @@ constexpr size_t kMaxParamBytes = 4096;
 // Planes per layer of a kv_desc (1 for a latent KV, B200KV_KV_LATENT) and its element dtype without the flag.
 inline int kv_ppl(const b200kv_kv_desc* kv) { return (kv->dtype & B200KV_KV_LATENT) ? 1 : 2; }
 inline int kv_dtype(const b200kv_kv_desc* kv) { return kv->dtype & ~B200KV_KV_LATENT; }
+// Bytes per element of a B200KV_DT_* code (without the latent flag), 0 for an unknown code.
+inline int dtype_bytes(int dt) {
+    return dt == B200KV_DT_BF16 || dt == B200KV_DT_FP16 ? 2
+           : dt == B200KV_DT_U8 || dt == B200KV_DT_FP8_E4M3 || dt == B200KV_DT_FP8_E5M2 ? 1 : 0;
+}
+inline int kv_elem_bytes(const b200kv_kv_desc* kv) { return dtype_bytes(kv_dtype(kv)); }
 
 // Fill a PlaneTable from a kv_desc + bins (planes kv * L + l; a latent KV's plane l takes key_bins[l]); returns 0 or <0
-// with error set.
+// with error set.  Takes every dtype of dtype_bytes: the CacheGen entry points refuse the one-byte ones themselves.
 int make_plane_table(const b200kv_kv_desc* kv, const float* key_bins, const float* value_bins, PlaneTable* out);
 
 // Row of a token inside its plane.  PAGED: the caller's slot mapping (vLLM's paged KV cache: row = block * block_size

@@ -3,7 +3,10 @@
 // Every 16-bit element u is split as v = rotl16(u, 1): sym = v >> 8 (bf16: the 8 exponent bits; fp16: the 5 exponent bits
 // and the top 3 mantissa bits), raw = v & 0xff (sign and the rest of the mantissa).  The raw bytes are stored verbatim; the
 // symbols of each (plane, channel) are rANS-coded (32-bit state, 16-bit renormalisation, 12-bit probabilities) against
-// one frequency row per plane.  include/b200kv.h states the format; tests/lossless_ref.py is its numpy statement.
+// one frequency row per plane.  A one-byte element (FP8, uint8) is its own symbol and has no raw byte.  include/b200kv.h
+// states the format; tests/lossless_ref.py (16-bit) and tests/lossless8_ref.py (one-byte) are its numpy statements.
+// The kernels that touch elements take the element size as a template parameter EB (2 or 1); LlEnc / LlDec.rawb is the
+// raw bytes per element, EB - 1.
 //
 // Thread mapping, as in codec.cu: one stream = one (plane, channel) = one thread; a CTA owns CT consecutive channels of
 // one plane of one chunk, so a warp reads 64 contiguous bytes per token and writes 32 contiguous raw bytes.
@@ -23,6 +26,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "ac_core.cuh"
 #include "common.cuh"
@@ -38,18 +42,19 @@ constexpr int kMaxTokens = 4096;         // tokens per container (u16 stream len
 constexpr int kSlice = 128;              // tokens per histogram CTA
 constexpr int kFreqRowBytes = 2 * kSyms;
 
-// fixed sections of a container of P planes of C channels and t tokens; max_stream: the longest stream the encoder can
-// produce (4 state bytes + <= ceil(3t/4) + 1 renormalisation halfwords), max_total: the worst-case container
+// fixed sections of a container of P planes of C channels and t tokens with rawb raw bytes per element (1 for 16-bit
+// elements, 0 for one-byte ones); max_stream: the longest stream the encoder can produce (4 state bytes + <= ceil(3t/4)
+// + 1 renormalisation halfwords), max_total: the worst-case container
 struct LlLayout {
     int64_t off_freq, off_lens, off_raw, off_payload, max_stream, max_total;
 };
 __host__ __device__ __forceinline__ int64_t ll_max_words(int t) { return (3 * (int64_t)t + 3) / 4 + 1; }
-__host__ __device__ __forceinline__ LlLayout ll_layout(int P, int64_t C, int t) {
+__host__ __device__ __forceinline__ LlLayout ll_layout(int P, int64_t C, int t, int rawb) {
     LlLayout lo;
     lo.off_freq = B200KV_HEADER_BYTES;
     lo.off_lens = lo.off_freq + (int64_t)P * kFreqRowBytes;
     lo.off_raw = align16(lo.off_lens + 2 * (int64_t)P * C);
-    lo.off_payload = align16(lo.off_raw + (int64_t)P * t * C);
+    lo.off_payload = align16(lo.off_raw + (int64_t)P * t * C * rawb);
     lo.max_stream = 4 + 2 * ll_max_words(t);
     lo.max_total = align16(lo.off_payload + (int64_t)P * C * lo.max_stream);
     return lo;
@@ -60,6 +65,7 @@ struct LlEnc {
     int64_t sT, sH, tok_begin;
     const int64_t* slot_map;
     int32_t L, H, D, C, NP, dtype;       // NP = planes: 2L, or L for a latent KV
+    int32_t rawb;                        // raw bytes per element: 1 (16-bit elements) or 0 (one-byte elements)
     int32_t n_chunks, chunk_tokens, last_chunk_tokens, tpp, ntiles, rw;   // rw: halfwords per scratch row
     uint8_t* out;                        // containers (the layer-wise encode: fixed images [0, off_raw))
     int64_t out_stride;
@@ -75,6 +81,7 @@ struct LlEnc {
     uint32_t* state;                     // [n][npc][C] final coder states
     uint16_t* scratch;                   // [n][npc][C][rw] renormalisation halfwords, the last one pushed first
     uint8_t* raw;                        // raw rows of (chunk j, local plane pl): raw + j * raw_stride + pl * t * C
+                                         // (16-bit elements only)
     int64_t raw_stride;
     // b200kv_lossless_encode_layers only (arena NULL otherwise): raw rows and streams go to a device arena
     uint8_t* arena;
@@ -103,6 +110,7 @@ struct LlDec {
     int64_t sT, sH;
     const int64_t* slot_map;
     int32_t L, H, D, C, NP, tpp, ntiles, dtype, version, n_chunks;   // H, C: the containers' (src_H with windows)
+    int32_t rawb;                        // raw bytes per element: 1 (16-bit elements) or 0 (one-byte elements)
     int32_t wtpp;                        // tiles launched per plane: the largest window's ntw (tpp without windows)
     int32_t lb, nl;                      // the launch decodes layers [lb, lb + nl): blockIdx.y < nl keys, then values
     const LlDecChunk* chunks;
@@ -143,15 +151,15 @@ __device__ __forceinline__ int ll_plane(const LlEnc& P, int pl) {
 // bytes of the raw part of a chunk's segment in the layer-wise encode: the call's raw rows, and -- in the call that
 // holds the last plane -- the container's zero bytes between the raw section and off_payload, then 16-byte aligned
 __device__ __forceinline__ int64_t ll_seg_raw(const LlEnc& P, int t, const LlLayout& lo) {
-    int64_t r = (int64_t)P.npc * t * P.C;
-    if (P.lb + P.nl == P.L) r += lo.off_payload - lo.off_raw - (int64_t)P.NP * t * P.C;
+    int64_t r = (int64_t)P.npc * t * P.C * P.rawb;
+    if (P.lb + P.nl == P.L) r += lo.off_payload - lo.off_raw - (int64_t)P.NP * t * P.C * P.rawb;
     return align16(r);
 }
 
 // header of chunk j with `payload` stream bytes
 __device__ __forceinline__ void ll_put_header(const LlEnc& P, int j, unsigned long long payload, uint32_t status) {
     const int t = ll_chunk_t(P, j);
-    const LlLayout lo = ll_layout(P.NP, P.C, t);
+    const LlLayout lo = ll_layout(P.NP, P.C, t, P.rawb);
     b200kv_header hd;
     memset(&hd, 0, sizeof(hd));
     hd.magic = B200KV_MAGIC;
@@ -170,6 +178,12 @@ __device__ __forceinline__ void ll_put_header(const LlEnc& P, int j, unsigned lo
 
 __device__ __forceinline__ uint32_t rotl1(uint32_t u) { return ((u << 1) | (u >> 15)) & 0xffffu; }
 __device__ __forceinline__ uint32_t rotr1(uint32_t v) { return ((v >> 1) | (v << 15)) & 0xffffu; }
+
+// element type of EB bytes, and the coded form of an element u: 16-bit v = rotl16(u, 1) (symbol v >> 8, raw byte
+// v & 0xff); a one-byte element is its own symbol (v = u << 8, no raw byte)
+template <int EB> using ll_elem_t = typename std::conditional<EB == 2, uint16_t, uint8_t>::type;
+template <int EB>
+__device__ __forceinline__ uint32_t ll_code(uint32_t u) { return EB == 2 ? rotl1(u) : u << 8; }
 
 // exclusive prefix of v over a CTA of NT threads, and the CTA's total (every thread must call it)
 template <int NT, class T>
@@ -198,7 +212,7 @@ __device__ __forceinline__ T cta_excl_scan(T v, T* s_w, T* total) {
 // ------------------------------------------------------------------------------------------ encode
 // 1) symbol histogram of one (chunk, plane, channel tile, slice of kSlice tokens): warp-private bins in shared memory,
 //    lanes with equal symbols aggregated (__match_any_sync), then one global add per nonzero bin
-template <bool PAGED>
+template <bool PAGED, int EB>
 __global__ void __launch_bounds__(kCT) ll_hist_kernel(LlEnc P) {
     __shared__ uint32_t s_h[kCT / 32][kSyms];
     const int j = blockIdx.z, pl = blockIdx.y, p = ll_plane(P, pl);
@@ -212,7 +226,7 @@ __global__ void __launch_bounds__(kCT) ll_hist_kernel(LlEnc P) {
     const int c = tile * kCT + threadIdx.x;
     const bool on = c < P.C;
     const int h = on ? c / P.D : 0, d = on ? c - h * P.D : 0;
-    const uint16_t* base = P.pt.p[p] + (int64_t)h * P.sH + d;
+    const ll_elem_t<EB>* base = reinterpret_cast<const ll_elem_t<EB>*>(P.pt.p[p]) + (int64_t)h * P.sH + d;
     const int64_t tok0 = P.tok_begin + (int64_t)j * P.chunk_tokens;
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
     for (int i = i0; i < i1; i += 4) {
@@ -222,7 +236,7 @@ __global__ void __launch_bounds__(kCT) ll_hist_kernel(LlEnc P) {
             u[k] = on && i + k < i1 ? __ldg(base + tok_row<PAGED>(P.slot_map, tok0 + i + k) * P.sT) : 0u;
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-            const uint32_t sym = on && i + k < i1 ? rotl1(u[k]) >> 8 : 0x100u;   // 0x100: no symbol
+            const uint32_t sym = on && i + k < i1 ? ll_code<EB>(u[k]) >> 8 : 0x100u;   // 0x100: no symbol
             const uint32_t peers = __match_any_sync(0xffffffffu, sym);
             if (sym < 0x100u && lane == __ffs(peers) - 1) atomicAdd(&s_h[w][sym], (uint32_t)__popc(peers));
         }
@@ -277,7 +291,8 @@ __global__ void __launch_bounds__(kSyms) ll_norm_kernel(LlEnc P) {
 //      if (x >> 20) >= f: push x & 0xffff, x >>= 16;   x = ((x / f) << 12) + (x mod f) + start
 //    The bound is compared as x >> 20 against f, not x against f << 20: a single-symbol plane has f = 4096, and 4096 << 20
 //    does not fit 32 bits.  With f = 4096 the step leaves x unchanged and pushes nothing.  Plain integer division.
-template <bool PAGED>
+//    One-byte elements have no raw bytes.
+template <bool PAGED, int EB>
 __global__ void __launch_bounds__(kCT) ll_encode_kernel(LlEnc P) {
     __shared__ uint32_t s_tab[kSyms];
     __shared__ unsigned long long s_w[kCT / 32];
@@ -288,13 +303,13 @@ __global__ void __launch_bounds__(kCT) ll_encode_kernel(LlEnc P) {
     __syncthreads();
     const int c = tile * kCT + threadIdx.x;
     const bool on = c < P.C;
-    const LlLayout lo = ll_layout(P.NP, P.C, t);
+    const LlLayout lo = ll_layout(P.NP, P.C, t, P.rawb);
     uint8_t* cont = P.out + (int64_t)j * P.out_stride;
     uint32_t x = kRansLow;
     int32_t k = 0;
     if (on) {
         const int h = c / P.D, d = c - h * P.D;
-        const uint16_t* base = P.pt.p[p] + (int64_t)h * P.sH + d;
+        const ll_elem_t<EB>* base = reinterpret_cast<const ll_elem_t<EB>*>(P.pt.p[p]) + (int64_t)h * P.sH + d;
         const int64_t tok0 = P.tok_begin + (int64_t)j * P.chunk_tokens;
         uint8_t* raw = P.raw + (int64_t)j * P.raw_stride + (int64_t)pl * t * P.C + c;
         uint16_t* srow = P.scratch + (row * P.C + c) * P.rw;
@@ -303,8 +318,8 @@ __global__ void __launch_bounds__(kCT) ll_encode_kernel(LlEnc P) {
         for (int i = t - 1; i >= 0; --i) {
             const uint32_t u = nxt;
             if (i > 0) nxt = __ldg(base + tok_row<PAGED>(P.slot_map, tok0 + i - 1) * P.sT);
-            const uint32_t v = rotl1(u);
-            raw[(int64_t)i * P.C] = (uint8_t)v;
+            const uint32_t v = ll_code<EB>(u);
+            if (EB == 2) raw[(int64_t)i * P.C] = (uint8_t)v;
             const uint32_t e = s_tab[v >> 8];
             const uint32_t f = e & 0xffffu;
             if ((x >> 20) >= f) {
@@ -359,7 +374,7 @@ __global__ void __launch_bounds__(1024) ll_enc_scan_kernel(LlEnc P) {
     const unsigned long long payload = ll_scan_tiles(P.tile + (int64_t)j * P.ntiles, P.ntiles);
     if (threadIdx.x != 0) return;
     const int t = ll_chunk_t(P, j);
-    const LlLayout lo = ll_layout(P.NP, P.C, t);
+    const LlLayout lo = ll_layout(P.NP, P.C, t, P.rawb);
     if (P.arena != nullptr) {
         P.totals[j] = (unsigned long long)ll_seg_raw(P, t, lo) + payload;
         return;
@@ -367,7 +382,7 @@ __global__ void __launch_bounds__(1024) ll_enc_scan_kernel(LlEnc P) {
     ll_put_header(P, j, payload, P.err[j]);
     uint8_t* cont = P.out + (int64_t)j * P.out_stride;
     for (int64_t b = lo.off_lens + 2 * (int64_t)P.NP * P.C; b < lo.off_raw; ++b) cont[b] = 0u;
-    for (int64_t b = lo.off_raw + (int64_t)P.NP * t * P.C; b < lo.off_payload; ++b) cont[b] = 0u;
+    for (int64_t b = lo.off_raw + (int64_t)P.NP * t * P.C * P.rawb; b < lo.off_payload; ++b) cont[b] = 0u;
 }
 
 // 4b) streams into the payload (the layer-wise encode: into the chunk's segment, after its raw part), a warp per 32
@@ -377,7 +392,7 @@ __global__ void __launch_bounds__(kCT) ll_compact_kernel(LlEnc P) {
     const int j = blockIdx.z, pl = blockIdx.y, p = ll_plane(P, pl), tile = blockIdx.x;
     if (P.err[j]) return;                                // an overflowed stream, or no room in the arena
     const int t = ll_chunk_t(P, j);
-    const LlLayout lo = ll_layout(P.NP, P.C, t);
+    const LlLayout lo = ll_layout(P.NP, P.C, t, P.rawb);
     uint8_t* cont = P.out + (int64_t)j * P.out_stride;
     uint8_t* base = P.arena != nullptr ? P.arena + P.chunk_base[j] + ll_seg_raw(P, t, lo) : cont + lo.off_payload;
     const int64_t row = (int64_t)j * P.npc + pl;
@@ -413,18 +428,18 @@ __global__ void __launch_bounds__(1024) ll_place_kernel(LlEnc P) {
     for (int j = tid; j < P.n_chunks; j += 1024)
         if (P.chunk_base[j] != ~0ull) {
             const int t = ll_chunk_t(P, j);
-            P.ptotal[j] += P.totals[j] - (unsigned long long)ll_seg_raw(P, t, ll_layout(P.NP, P.C, t));
+            P.ptotal[j] += P.totals[j] - (unsigned long long)ll_seg_raw(P, t, ll_layout(P.NP, P.C, t, P.rawb));
         }
     for (int k = tid; k < P.n_chunks * P.npc; k += 1024) {
         const int j = k / P.npc, pl = k - j * P.npc;
         const int t = ll_chunk_t(P, j);
-        const unsigned long long raw = (unsigned long long)ll_seg_raw(P, t, ll_layout(P.NP, P.C, t));
+        const unsigned long long raw = (unsigned long long)ll_seg_raw(P, t, ll_layout(P.NP, P.C, t, P.rawb));
         const unsigned long long* tb = P.tile + (int64_t)j * P.ntiles;
         const unsigned long long off = tb[pl * P.tpp];
         const unsigned long long end = pl + 1 < P.npc ? tb[(pl + 1) * P.tpp] : P.totals[j] - raw;
         const unsigned long long cb = P.chunk_base[j];
         int64_t* row = P.seg + ((int64_t)j * P.NP + ll_plane(P, pl)) * 3;
-        row[0] = cb == ~0ull ? -1 : (int64_t)(cb + (unsigned long long)pl * t * P.C);
+        row[0] = cb == ~0ull ? -1 : (int64_t)(cb + (unsigned long long)pl * t * P.C * P.rawb);
         row[1] = cb == ~0ull ? -1 : (int64_t)(cb + raw + off);
         row[2] = (int64_t)(end - off);
     }
@@ -436,7 +451,7 @@ __global__ void __launch_bounds__(256) ll_raw_copy_kernel(LlEnc P) {
     const int j = blockIdx.y;
     if (P.err[j]) return;
     const int t = ll_chunk_t(P, j);
-    const int64_t nraw = (int64_t)P.npc * t * P.C, nseg = ll_seg_raw(P, t, ll_layout(P.NP, P.C, t));
+    const int64_t nraw = (int64_t)P.npc * t * P.C * P.rawb, nseg = ll_seg_raw(P, t, ll_layout(P.NP, P.C, t, P.rawb));
     const uint8_t* src = P.raw + (int64_t)j * P.raw_stride;
     uint8_t* dst = P.arena + P.chunk_base[j];
     for (int64_t b = 16 * ((int64_t)blockIdx.x * blockDim.x + threadIdx.x); b < nseg; b += 16 * (int64_t)gridDim.x * blockDim.x) {
@@ -498,7 +513,7 @@ __global__ void __launch_bounds__(1024) ll_dec_scan_kernel(LlDec P) {
 // past the window's ntw leave.  Every thread of a tile still reads its length and joins the scan, because a stream's
 // offset depends on the lengths before it in the tile, but only the channels [cw0, cw1) decode, into destination
 // channel c + dshift, and only they can set status bits: a damaged stream outside the window is never read.
-template <bool PAGED>
+template <bool PAGED, int EB>
 __global__ void __launch_bounds__(kCT) ll_decode_kernel(LlDec P) {
     __shared__ uint32_t s_ent[kSyms];
     __shared__ uint8_t s_sym[kM];
@@ -509,7 +524,7 @@ __global__ void __launch_bounds__(kCT) ll_decode_kernel(LlDec P) {
     if ((int)blockIdx.x >= dc.ntw) return;
     const int tile = dc.ct0 + (int)blockIdx.x;
     const int t = dc.t;
-    const LlLayout lo = ll_layout(P.NP, P.C, t);
+    const LlLayout lo = ll_layout(P.NP, P.C, t, P.rawb);
     uint32_t bad = 0u;
     if (threadIdx.x == 0) {
         const b200kv_header* hd = reinterpret_cast<const b200kv_header*>(dc.base);
@@ -557,11 +572,11 @@ __global__ void __launch_bounds__(kCT) ll_decode_kernel(LlDec P) {
             uint32_t k = 0u;
             const int oc = c + dc.dshift;                // destination channel
             const int h = oc / P.D, d = oc - h * P.D;
-            uint16_t* dst = const_cast<uint16_t*>(P.pt.p[p]) + (int64_t)h * P.sH + d;
+            ll_elem_t<EB>* dst = reinterpret_cast<ll_elem_t<EB>*>(const_cast<uint16_t*>(P.pt.p[p])) + (int64_t)h * P.sH + d;
             const uint8_t* raw = dc.base + lo.off_raw + (int64_t)p * t * P.C + c;
 #pragma unroll 4
             for (int i = 0; i < t; ++i) {
-                const uint32_t rb = raw[(int64_t)i * P.C];
+                const uint32_t rb = EB == 2 ? raw[(int64_t)i * P.C] : 0u;
                 const uint32_t slot = x & (kM - 1u);
                 const uint32_t sym = s_sym[slot];
                 const uint32_t e = s_ent[sym];
@@ -571,7 +586,8 @@ __global__ void __launch_bounds__(kCT) ll_decode_kernel(LlDec P) {
                     ++k;
                     x = (x << 16) | hw;
                 }
-                dst[tok_row<PAGED>(P.slot_map, dc.dst_tok + i) * P.sT] = (uint16_t)rotr1((sym << 8) | rb);
+                dst[tok_row<PAGED>(P.slot_map, dc.dst_tok + i) * P.sT] =
+                    EB == 2 ? (ll_elem_t<EB>)rotr1((sym << 8) | rb) : (ll_elem_t<EB>)sym;
             }
             if (x != kRansLow || k != nw) bad |= 1u;
         }
@@ -587,8 +603,13 @@ __host__ __device__ __forceinline__ bool ll_offsets_header_ok(const b200kv_heade
         hd.L > (uint32_t)(B200KV_MAX_PLANES / 2) || hd.H == 0u || hd.D == 0u ||
         (uint64_t)hd.H * hd.D >= (1ull << 24) || hd.ntokens == 0u || hd.ntokens > (uint32_t)kMaxTokens)
         return false;
+    int rawb;                                           // the element dtype decides the raw section
+    if (hd.max_dtype == B200KV_DT_BF16 || hd.max_dtype == B200KV_DT_FP16) rawb = 1;
+    else if (hd.max_dtype == B200KV_DT_U8 || hd.max_dtype == B200KV_DT_FP8_E4M3 || hd.max_dtype == B200KV_DT_FP8_E5M2)
+        rawb = 0;
+    else return false;
     *NP = hd.version == 6u ? (int)hd.L : 2 * (int)hd.L;
-    *lo = ll_layout(*NP, (int64_t)hd.H * hd.D, (int)hd.ntokens);
+    *lo = ll_layout(*NP, (int64_t)hd.H * hd.D, (int)hd.ntokens, rawb);
     return (uint64_t)lo->off_payload <= hd.total_bytes && lo->off_payload <= limit;
 }
 
@@ -633,6 +654,18 @@ __global__ void __launch_bounds__(1024) ll_plane_offsets_kernel(const uint8_t* b
 }
 
 // ------------------------------------------------------------------------------------------ host side
+// launch KERNEL<paged, element bytes> of an LlEnc / LlDec parameter block P (kCT threads per CTA)
+#define LL_LAUNCH_ELEM(KERNEL, GRID, P, STREAM)                                                                        \
+    do {                                                                                                               \
+        if ((P).slot_map != nullptr) {                                                                                 \
+            if ((P).rawb) KERNEL<true, 2><<<(GRID), kCT, 0, (STREAM)>>>(P);                                            \
+            else KERNEL<true, 1><<<(GRID), kCT, 0, (STREAM)>>>(P);                                                     \
+        } else {                                                                                                       \
+            if ((P).rawb) KERNEL<false, 2><<<(GRID), kCT, 0, (STREAM)>>>(P);                                           \
+            else KERNEL<false, 1><<<(GRID), kCT, 0, (STREAM)>>>(P);                                                    \
+        }                                                                                                              \
+    } while (0)
+
 int fill_planes(const b200kv_kv_desc* kv, PlaneTable* pt) {
     float bins[B200KV_MAX_PLANES];
     for (int i = 0; i < B200KV_MAX_PLANES; ++i) bins[i] = 32.0f;   // no quantiser here; keeps the table valid
@@ -703,9 +736,15 @@ extern "C" {
 
 int b200kv_lossless_layout(int32_t L, int32_t H, int32_t D, int32_t ntokens, int32_t latent,
                            b200kv_lossless_layout_t* out) {
+    return b200kv_lossless_layout_dt(L, H, D, ntokens, latent, B200KV_DT_BF16, out);
+}
+
+int b200kv_lossless_layout_dt(int32_t L, int32_t H, int32_t D, int32_t ntokens, int32_t latent, int32_t dtype,
+                              b200kv_lossless_layout_t* out) {
     B2_REQUIRE(out != nullptr, "out is NULL");
     B2_REQUIRE(shape_ok(L, H, D, ntokens), "bad shape (L <= 128, H * D < 2^24, 1 <= ntokens <= 4096)");
-    const LlLayout lo = ll_layout(latent ? L : 2 * L, (int64_t)H * D, ntokens);
+    B2_REQUIRE(dtype_bytes(dtype) != 0, "dtype must be one of B200KV_DT_*");
+    const LlLayout lo = ll_layout(latent ? L : 2 * L, (int64_t)H * D, ntokens, dtype_bytes(dtype) - 1);
     out->off_freq = lo.off_freq;
     out->off_lens = lo.off_lens;
     out->off_raw = lo.off_raw;
@@ -742,7 +781,8 @@ int b200kv_lossless_encode(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t 
     B2_REQUIRE(tok_begin >= 0, "tok_begin must be >= 0");
     P.NP = kv_ppl(kv) * kv->L;
     P.L = kv->L; P.H = kv->H; P.D = kv->D; P.C = kv->H * kv->D; P.dtype = kv_dtype(kv);
-    const LlLayout lo = ll_layout(P.NP, P.C, chunk_tokens);
+    P.rawb = kv_elem_bytes(kv) - 1;
+    const LlLayout lo = ll_layout(P.NP, P.C, chunk_tokens, P.rawb);
     B2_REQUIRE(out_stride >= lo.max_total, "out_stride smaller than the worst-case container (b200kv_lossless_layout)");
     P.sT = kv->sT; P.sH = kv->sH; P.tok_begin = tok_begin;
     P.slot_map = kv->slot_map;
@@ -769,17 +809,14 @@ int b200kv_lossless_encode(const b200kv_kv_desc* kv, int64_t tok_begin, int32_t 
     P.state = reinterpret_cast<uint32_t*>(ws + w.state);
     P.scratch = reinterpret_cast<uint16_t*>(ws + w.scratch);
     B2_CHECK_CUDA(cudaMemsetAsync(ws, 0, w.tab, stream));        // histograms and error words
-    const bool paged = kv->slot_map != nullptr;
     const unsigned nslices = (unsigned)((chunk_tokens + kSlice - 1) / kSlice);
     const dim3 ghist((unsigned)P.tpp * nslices, (unsigned)P.NP, (unsigned)n_chunks);
     const dim3 gtile((unsigned)P.tpp, (unsigned)P.NP, (unsigned)n_chunks);
-    if (paged) ll_hist_kernel<true><<<ghist, kCT, 0, stream>>>(P);
-    else ll_hist_kernel<false><<<ghist, kCT, 0, stream>>>(P);
+    LL_LAUNCH_ELEM(ll_hist_kernel, ghist, P, stream);
     B2_CHECK_CUDA(cudaGetLastError());
     ll_norm_kernel<<<dim3((unsigned)P.NP, (unsigned)n_chunks), kSyms, 0, stream>>>(P);
     B2_CHECK_CUDA(cudaGetLastError());
-    if (paged) ll_encode_kernel<true><<<gtile, kCT, 0, stream>>>(P);
-    else ll_encode_kernel<false><<<gtile, kCT, 0, stream>>>(P);
+    LL_LAUNCH_ELEM(ll_encode_kernel, gtile, P, stream);
     B2_CHECK_CUDA(cudaGetLastError());
     ll_enc_scan_kernel<<<(unsigned)n_chunks, 1024, 0, stream>>>(P);
     B2_CHECK_CUDA(cudaGetLastError());
@@ -833,7 +870,7 @@ static int ll_decode_plan_impl(const void* containers, int64_t containers_bytes,
     if (int rc = fill_planes(dst, &P.pt)) return rc;
     B2_REQUIRE(containers && offsets && total_bytes && ntokens && dst_tok && n_chunks > 0 && n_chunks <= 65535,
                "bad chunk arrays");
-    B2_REQUIRE(max_dtype == B200KV_DT_BF16 || max_dtype == B200KV_DT_FP16, "bad max_dtype");
+    B2_REQUIRE(dtype_bytes(max_dtype) != 0, "bad max_dtype");
     B2_REQUIRE(kv_dtype(dst) == max_dtype,
                "the destination's dtype is not the stored one: a lossless container is decoded into its own dtype only");
     B2_REQUIRE(shape_ok(dst->L, dst->H, dst->D, 1), "bad destination shape");
@@ -845,6 +882,7 @@ static int ll_decode_plan_impl(const void* containers, int64_t containers_bytes,
     P.NP = kv_ppl(dst) * dst->L;
     P.L = dst->L; P.H = src_H; P.D = dst->D; P.C = src_H * dst->D;
     P.dtype = max_dtype;
+    P.rawb = dtype_bytes(max_dtype) - 1;
     P.version = kv_ppl(dst) == 1 ? 6 : 5;
     P.sT = dst->sT; P.sH = dst->sH;
     P.slot_map = dst->slot_map;
@@ -854,7 +892,7 @@ static int ll_decode_plan_impl(const void* containers, int64_t containers_bytes,
     for (int j = 0; j < n_chunks; ++j) {
         B2_REQUIRE(ntokens[j] > 0 && ntokens[j] <= kMaxTokens, "ntokens must be in [1, 4096]");
         B2_REQUIRE((offsets[j] & 15) == 0, "container offsets must be 16-byte aligned");
-        const LlLayout lj = ll_layout(P.NP, P.C, ntokens[j]);
+        const LlLayout lj = ll_layout(P.NP, P.C, ntokens[j], P.rawb);
         B2_REQUIRE(total_bytes[j] >= lj.off_payload, "container shorter than its fixed sections (truncated or corrupt)");
         B2_REQUIRE(offsets[j] >= 0 && offsets[j] + total_bytes[j] + B200KV_READ_SLACK <= containers_bytes,
                    "containers buffer must extend B200KV_READ_SLACK bytes past the end of every container");
@@ -869,7 +907,7 @@ static int ll_decode_plan_impl(const void* containers, int64_t containers_bytes,
         for (int j = 0; j < n_chunks; ++j) {
             hc[j].base = static_cast<const uint8_t*>(containers) + offsets[j];
             hc[j].dst_tok = dst_tok[j];
-            hc[j].payload_bytes = total_bytes[j] - ll_layout(P.NP, P.C, ntokens[j]).off_payload;
+            hc[j].payload_bytes = total_bytes[j] - ll_layout(P.NP, P.C, ntokens[j], P.rawb).off_payload;
             hc[j].t = ntokens[j];
             const HeadWindow& w = win[(size_t)j];
             hc[j].ct0 = w.ct0;
@@ -929,8 +967,7 @@ int b200kv_lossless_decode_layers(const b200kv_lossless_decode_plan_t* plan_in, 
     P.nl = layer_end - layer_begin;
     const int ppl = P.NP / P.L;
     const dim3 g((unsigned)P.wtpp, (unsigned)(ppl * P.nl), (unsigned)P.n_chunks);
-    if (P.slot_map) ll_decode_kernel<true><<<g, kCT, 0, stream>>>(P);
-    else ll_decode_kernel<false><<<g, kCT, 0, stream>>>(P);
+    LL_LAUNCH_ELEM(ll_decode_kernel, g, P, stream);
     B2_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -977,7 +1014,8 @@ int b200kv_lossless_encode_layers_plan(const b200kv_kv_desc* kv, int64_t tok_beg
                "fixed_out / fixed_stride must be 16-byte aligned");
     P.NP = kv_ppl(kv) * kv->L;
     P.L = kv->L; P.H = kv->H; P.D = kv->D; P.C = kv->H * kv->D; P.dtype = kv_dtype(kv);
-    const LlLayout lo = ll_layout(P.NP, P.C, chunk_tokens);
+    P.rawb = kv_elem_bytes(kv) - 1;
+    const LlLayout lo = ll_layout(P.NP, P.C, chunk_tokens, P.rawb);
     B2_REQUIRE(fixed_stride >= lo.off_raw, "fixed_stride smaller than the fixed image [0, off_raw) (b200kv_lossless_layout)");
     P.sT = kv->sT; P.sH = kv->sH; P.tok_begin = tok_begin;
     P.slot_map = kv->slot_map;
@@ -1036,21 +1074,20 @@ int b200kv_lossless_encode_layers(b200kv_lossless_encode_plan_t* plan_in, int32_
     P.layers_left = P.L - plan->done.count() - bits.count();
     const int n = P.n_chunks;
     B2_CHECK_CUDA(cudaMemsetAsync(P.hist, 0, sizeof(uint32_t) * (size_t)n * P.npc * kSyms, stream));
-    const bool paged = P.slot_map != nullptr;
     const unsigned nslices = (unsigned)((P.chunk_tokens + kSlice - 1) / kSlice);
     const dim3 ghist((unsigned)P.tpp * nslices, (unsigned)P.npc, (unsigned)n);
     const dim3 gtile((unsigned)P.tpp, (unsigned)P.npc, (unsigned)n);
-    if (paged) ll_hist_kernel<true><<<ghist, kCT, 0, stream>>>(P);
-    else ll_hist_kernel<false><<<ghist, kCT, 0, stream>>>(P);
+    LL_LAUNCH_ELEM(ll_hist_kernel, ghist, P, stream);
     ll_norm_kernel<<<dim3((unsigned)P.npc, (unsigned)n), kSyms, 0, stream>>>(P);
-    if (paged) ll_encode_kernel<true><<<gtile, kCT, 0, stream>>>(P);
-    else ll_encode_kernel<false><<<gtile, kCT, 0, stream>>>(P);
+    LL_LAUNCH_ELEM(ll_encode_kernel, gtile, P, stream);
     ll_enc_scan_kernel<<<(unsigned)n, 1024, 0, stream>>>(P);
     ll_place_kernel<<<1, 1024, 0, stream>>>(P);
-    // ~16 KB of raw rows per CTA pass; at most 64 CTAs per chunk
-    const int64_t raw_bytes = align16((int64_t)P.npc * P.chunk_tokens * P.C) + 16;
-    const unsigned rx = (unsigned)std::min<int64_t>(64, (raw_bytes + 16 * 256 * 4 - 1) / (16 * 256 * 4));
-    ll_raw_copy_kernel<<<dim3(rx, (unsigned)n), 256, 0, stream>>>(P);
+    if (P.rawb) {   // one-byte elements have no raw rows, and their segments no raw part
+        // ~16 KB of raw rows per CTA pass; at most 64 CTAs per chunk
+        const int64_t raw_bytes = align16((int64_t)P.npc * P.chunk_tokens * P.C) + 16;
+        const unsigned rx = (unsigned)std::min<int64_t>(64, (raw_bytes + 16 * 256 * 4 - 1) / (16 * 256 * 4));
+        ll_raw_copy_kernel<<<dim3(rx, (unsigned)n), 256, 0, stream>>>(P);
+    }
     ll_compact_kernel<<<gtile, kCT, 0, stream>>>(P);
     B2_CHECK_CUDA(cudaGetLastError());
     plan->done.add(bits);

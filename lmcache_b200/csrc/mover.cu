@@ -31,11 +31,11 @@ struct PackParams {
 };
 static_assert(sizeof(PackParams) < kMaxParamBytes, "PackParams must stay under 4 KB of kernel parameters");
 
-// One grid-stride loop over (chunk, plane, token, vector) units; VEC halfs per unit.
-// vllm chunk layout [L,2,t,H,D]; huggingface [L,2,H,t,D]; a latent KV (ppl = 1) [L,t,H,D].
-template <int VEC, bool PACK>
+// One grid-stride loop over (chunk, plane, token, vector) units; VEC elements of type E per unit (one 16-byte vector,
+// or one element).  vllm chunk layout [L,2,t,H,D]; huggingface [L,2,H,t,D]; a latent KV (ppl = 1) [L,t,H,D].
+template <class E, int VEC, bool PACK>
 __global__ void __launch_bounds__(256) pack_kernel(PackParams P) {
-    using vec_t = typename std::conditional<VEC == 8, uint4, uint16_t>::type;
+    using vec_t = typename std::conditional<VEC * sizeof(E) == 16, uint4, E>::type;
     const int NL = P.ppl * P.L;
     const int vph = P.D / VEC;                 // vectors per head row
     const int64_t vpt = (int64_t)P.H * vph;    // vectors per token
@@ -55,16 +55,28 @@ __global__ void __launch_bounds__(256) pack_kernel(PackParams P) {
         const int h = (int)(r / vph);
         const int v = (int)(r - (int64_t)h * vph);
         const int l = P.ppl == 2 ? lk >> 1 : lk, kv = P.ppl == 2 ? lk & 1 : 0;
-        const uint16_t* plane = P.pt.p[kv * P.L + l];
+        const E* plane = reinterpret_cast<const E*>(P.pt.p[kv * P.L + l]);
         int64_t row = P.tok_begin + j * P.chunk_tokens + tok;
         if (P.slot_map) row = __ldg(P.slot_map + row);       // consecutive threads share the token: broadcast, L1 hit
         const int64_t src_off = row * P.sT + (int64_t)h * P.sH + (int64_t)v * VEC;
-        int64_t dst_off;   // in halfs, inside the chunk
+        int64_t dst_off;   // in elements, inside the chunk
         if (P.hf_layout) dst_off = (((int64_t)lk * P.H + h) * t + tok) * P.D + (int64_t)v * VEC;
         else dst_off = (((int64_t)lk * t + tok) * P.H + h) * P.D + (int64_t)v * VEC;
-        uint16_t* cptr = reinterpret_cast<uint16_t*>(P.chunks + j * P.chunk_stride_bytes) + dst_off;
+        E* cptr = reinterpret_cast<E*>(P.chunks + j * P.chunk_stride_bytes) + dst_off;
         if (PACK) *reinterpret_cast<vec_t*>(cptr) = *reinterpret_cast<const vec_t*>(plane + src_off);
-        else *reinterpret_cast<vec_t*>(const_cast<uint16_t*>(plane) + src_off) = *reinterpret_cast<const vec_t*>(cptr);
+        else *reinterpret_cast<vec_t*>(const_cast<E*>(plane) + src_off) = *reinterpret_cast<const vec_t*>(cptr);
+    }
+}
+
+template <class E>
+static void launch_pack_kernel(bool pack, bool vec, unsigned blocks, const PackParams& P, cudaStream_t stream) {
+    constexpr int V = 16 / sizeof(E);
+    if (pack) {
+        if (vec) pack_kernel<E, V, true><<<blocks, 256, 0, stream>>>(P);
+        else pack_kernel<E, 1, true><<<blocks, 256, 0, stream>>>(P);
+    } else {
+        if (vec) pack_kernel<E, V, false><<<blocks, 256, 0, stream>>>(P);
+        else pack_kernel<E, 1, false><<<blocks, 256, 0, stream>>>(P);
     }
 }
 
@@ -80,7 +92,8 @@ static int launch_pack(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, i
                "bad chunking");
     B2_REQUIRE(chunks != nullptr, "chunks is NULL");
     P.ppl = kv_ppl(kv);
-    const int64_t chunk_bytes = 2ll * kv->L * P.ppl * chunk_tokens * kv->H * kv->D;
+    const int es = kv_elem_bytes(kv);
+    const int64_t chunk_bytes = (int64_t)es * kv->L * P.ppl * chunk_tokens * kv->H * kv->D;
     B2_REQUIRE(chunk_stride_bytes >= chunk_bytes || n_chunks == 1, "chunk_stride_bytes too small");
     P.sT = kv->sT; P.sH = kv->sH; P.tok_begin = tok_begin;
     P.slot_map = kv->slot_map;
@@ -89,10 +102,11 @@ static int launch_pack(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, i
     P.hf_layout = hf_layout;
     P.chunks = static_cast<uint8_t*>(chunks);
     P.chunk_stride_bytes = chunk_stride_bytes;
-    bool vec = (kv->D % 8 == 0) && (kv->sT % 8 == 0) && (kv->sH % 8 == 0) &&
+    const int ev = 16 / es;                    // elements per 16-byte vector
+    bool vec = (kv->D % ev == 0) && (kv->sT % ev == 0) && (kv->sH % ev == 0) &&
                ((reinterpret_cast<uintptr_t>(chunks) & 15) == 0) && (chunk_stride_bytes % 16 == 0);
     for (int nl = 0; nl < P.ppl * P.L && vec; ++nl) vec = (reinterpret_cast<uintptr_t>(P.pt.p[nl]) & 15) == 0;
-    const int V = vec ? 8 : 1;
+    const int V = vec ? ev : 1;
     const int64_t total = ((int64_t)(n_chunks - 1) * chunk_tokens + last_chunk_tokens) * P.ppl * kv->L * kv->H * (kv->D / V);
     int64_t blocks = (total + 255) / 256;
     int dev = 0, sms = 0;
@@ -101,13 +115,8 @@ static int launch_pack(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, i
     const int64_t cap = (int64_t)sms * 8 * 4;   // a few waves of SMs x 8 CTAs; grid-stride covers the rest
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
-    if (pack) {
-        if (vec) pack_kernel<8, true><<<(unsigned)blocks, 256, 0, stream>>>(P);
-        else pack_kernel<1, true><<<(unsigned)blocks, 256, 0, stream>>>(P);
-    } else {
-        if (vec) pack_kernel<8, false><<<(unsigned)blocks, 256, 0, stream>>>(P);
-        else pack_kernel<1, false><<<(unsigned)blocks, 256, 0, stream>>>(P);
-    }
+    if (es == 2) launch_pack_kernel<uint16_t>(pack, vec, (unsigned)blocks, P, stream);
+    else launch_pack_kernel<uint8_t>(pack, vec, (unsigned)blocks, P, stream);
     B2_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -456,7 +456,8 @@ class LayerwiseEncode:
         last = n_tok - (n - 1) * chunk_size
         L, H, D, latent = view.L, view.H, view.D, view.latent
         coder = codec.coder_for(chunk_size, latent)
-        layouts = (codec.segment_layout(L, H, D, chunk_size, latent), codec.segment_layout(L, H, D, last, latent))
+        dt = view.dtype_code
+        layouts = (codec.segment_layout(L, H, D, chunk_size, latent, dt), codec.segment_layout(L, H, D, last, latent, dt))
         stride = (layouts[0].head + 15) & ~15
         arena = min(n * codec.layerwise_chunk_bound(L, H, D, chunk_size, latent),
                     budget or layerwise_store_budget_default())

@@ -1,6 +1,6 @@
 """LosslessSerializer / LosslessDeserializer -- the `lossless` serde: KV chunks in lossless B2KV containers (versions 5
 and 6, include/b200kv.h), coded and decoded on the GPU by LosslessCodec.  A decode gives back the stored bits exactly, in
-the stored dtype (bf16 or fp16); a KV of another dtype is refused.
+the stored dtype (bf16, fp16, or one-byte: uint8, float8_e4m3fn, float8_e5m2); a KV of another dtype is refused.
 
 The plugins carry the same engine fast-path methods as the CacheGen serde (view_to_bytes_batch, view_to_pinned_batch,
 decode_into, container_bound, .codec), so the remote tier runs its striped pipelines with them: k connections,
@@ -10,7 +10,7 @@ from typing import List, Optional, Sequence
 import torch
 
 from lmcache_b200 import _native as N
-from lmcache_b200.codec import KvView, LosslessCodec, dtype_of_code, parse_lossless_header
+from lmcache_b200.codec import NATIVE_DTYPES, KvView, LosslessCodec, dtype_of_code, parse_lossless_header
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.storage_backend.serde.serde import Deserializer, Serializer
 
@@ -32,8 +32,9 @@ class LosslessSerializer(Serializer):
         self.codec = LosslessCodec()
 
     def _view(self, tensor: torch.Tensor) -> KvView:
-        if tensor.dtype not in (torch.bfloat16, torch.float16):
-            raise TypeError(f"the lossless serde codes bfloat16 and float16 KV only, not {tensor.dtype}")
+        if tensor.dtype not in NATIVE_DTYPES:
+            raise TypeError(f"the lossless serde codes bfloat16 and float16 KV and one-byte KV (uint8, float8_e4m3fn, "
+                            f"float8_e5m2) only, not {tensor.dtype}")
         if not tensor.is_cuda:
             tensor = tensor.cuda()
         return KvView.from_blob(tensor, self.fmt)
