@@ -49,7 +49,8 @@ extern "C" {
                                     *    b200kv_lossless_encode_layers_plan / b200kv_lossless_encode_layers /
                                     *    b200kv_lossless_encode_layers_finish (b200kv_lossless_encode_plan_t),
                                     *    b200kv_lm_open_begin / b200kv_lm_read_ranges / b200kv_lm_close_handles,
-                                    *    b200kv_lm_server_num_handles.
+                                    *    b200kv_lm_server_num_handles, b200kv_pack_chunks_layers /
+                                    *    b200kv_unpack_chunks_layers.
                                     *    B200KV_MAX_PLANES went from 128 to 256 (models of up to 128 layers): the row
                                     *    width of b200kv_plane_offsets_device, B200KV_MAX_PLANES + 1, and the size of
                                     *    b200kv_encode_plan_t, 256 -> 512 words, changed with it; a caller takes them
@@ -557,6 +558,20 @@ int b200kv_pack_chunks(const b200kv_kv_desc* src, int64_t tok_begin, int32_t n_c
 int b200kv_unpack_chunks(const void* chunks, int64_t chunk_stride_bytes, int32_t n_chunks, int32_t chunk_tokens,
                          int32_t last_chunk_tokens, int32_t hf_layout, const b200kv_kv_desc* dst, int64_t tok_begin,
                          void* stream);
+/* The same for the layers [layer_begin, layer_end) of every chunk, in one launch, wherever each chunk lives.
+ * chunk_ptrs is a DEVICE array of n_chunks pointers (device or mapped pinned memory): chunk j's layer l lies at
+ * chunk_ptrs[j] + (l - layer_begin) * slice_bytes(t_j), where a layer slice is [2,t,H,D] (vllm) / [2,H,t,D]
+ * (huggingface) / [t,D] (latent KV) and t_j is chunk_tokens, or last_chunk_tokens for the last chunk.  One pointer thus
+ * names the range inside a full chunk blob (blob_j + layer_begin * slice) or a staging area that holds only the range.
+ * Planes of other layers are neither read nor written.  16-byte vectors where D, the strides, the planes and each
+ * chunk pointer allow it (a chunk pointer that is not 16-byte aligned moves element by element).  < 0, with nothing
+ * enqueued, for a NULL table, a range outside 0 <= layer_begin < layer_end <= L, or a bad chunking. */
+int b200kv_pack_chunks_layers(const b200kv_kv_desc* src, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
+                              int32_t last_chunk_tokens, int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
+                              void* const* chunk_ptrs, void* stream);
+int b200kv_unpack_chunks_layers(const void* const* chunk_ptrs, int32_t n_chunks, int32_t chunk_tokens,
+                                int32_t last_chunk_tokens, int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
+                                const b200kv_kv_desc* dst, int64_t tok_begin, void* stream);
 
 /*
  * GPU <-> pinned-host mover.  Replaces LMCLocalBackend.put_blocking/put_nonblocking/get

@@ -2,6 +2,7 @@
 """layerwise_bench.py -- what a layer-by-layer retrieve buys on the compressed host tier, on one GPU.
 
   python layerwise_bench.py [--steps K] [--warmup W] [--tokens 8192,65536] [--chunk C] [--cold N]
+                            [--raw cpu|cuda] [--dtype bf16|e4m3]
 
 Workload: bench.py's e2e shape (32 layers / 32 heads / 128 dims, bf16 KV, chunk 256, synthetic SURVEY 8d data), stored
 once through LMCacheEngine.store into the compressed host tier, then retrieved again and again, alternating
@@ -17,7 +18,10 @@ Per leg, from CUDA events (the start event is recorded on the caller's stream ri
 The layer-wise leg runs warm (the same sequence again and again) and cold (`--cold` sequences stored before the timed
 loop and retrieved once each).  The last warm step's KV of the two legs is compared through per-layer digests of the bit
 patterns.  Sequences longer than 8192 tokens repeat bench.py's 8192-token KV.  A token count that does not fit on the card
-is reported as skipped.  Prints one JSON line.  Writes nothing into the tree.
+is reported as skipped.  --raw cpu / --raw cuda measure the raw tiers instead (local_device "cpu" / "cuda" without a
+serde: chunk blobs copied and unpacked one layer at a time); they keep 8 of the 32 KV heads (a GQA shape, so that 65536
+tokens of raw blobs and the retrieved KV fit the card), and --dtype e4m3 stores an FP8 E4M3 KV.  Prints one JSON line.
+Writes nothing into the tree.
 """
 import argparse
 import json
@@ -54,7 +58,7 @@ def _digest(kv, w_cache={}):
     return torch.stack(out).cpu()
 
 
-def run(T, cs, steps, warmup, cold_steps):
+def run(T, cs, steps, warmup, cold_steps, raw=None, dt="bf16"):
     import torch
 
     import bench
@@ -63,7 +67,11 @@ def run(T, cs, steps, warmup, cold_steps):
 
     dev = torch.device("cuda", 0)
     meta = LMCacheEngineMetadata(bench.MODEL, 1, 0, "vllm", "bfloat16")
-    engine = LMCacheEngine(LMCacheEngineConfig.from_legacy(chunk_size=cs, backend="cpu", local_serde="cachegen"), meta)
+    if raw is None:
+        cfg = LMCacheEngineConfig.from_legacy(chunk_size=cs, backend="cpu", local_serde="cachegen")
+    else:
+        cfg = LMCacheEngineConfig(cs, raw, None, None, False, False, None)
+    engine = LMCacheEngine(cfg, meta)
     g = torch.Generator(device=dev).manual_seed(3)
     try:
         tokens = torch.randint(0, 32000, (T,), device=dev, generator=g)
@@ -71,6 +79,10 @@ def run(T, cs, steps, warmup, cold_steps):
         # more memory than the card has): same statistics, same bytes per chunk
         base_T = min(T, 8192)
         kv = bench.synth_kv_torch(base_T, dev, 1236, "kv8d")                # [L,2,t,H,D]
+        if raw is not None:
+            kv = kv[:, :, :, :8].contiguous()
+            if dt == "e4m3":
+                kv = kv.to(torch.float8_e4m3fn)
         if T > base_T:
             kv = torch.cat([kv] * (T // base_T), dim=2)
         L = kv.shape[0]
@@ -85,7 +97,7 @@ def run(T, cs, steps, warmup, cold_steps):
         torch.cuda.synchronize()
         torch.cuda.empty_cache()
         cur = torch.cuda.current_stream()
-        host_bytes = engine.engine_.host_bytes() // (1 + cold_steps)
+        host_bytes = engine.engine_.host_bytes() // (1 + cold_steps) if raw is None else None
 
         def plain():
             s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -157,7 +169,11 @@ def main():
     ap.add_argument("--tokens", type=str, default="8192,65536")
     ap.add_argument("--chunk", type=int, default=256)
     ap.add_argument("--cold", type=int, default=3)
+    ap.add_argument("--raw", choices=("cpu", "cuda"), default=None)
+    ap.add_argument("--dtype", choices=("bf16", "e4m3"), default="bf16")
     args = ap.parse_args()
+    if args.dtype != "bf16" and args.raw is None:
+        raise SystemExit("--dtype e4m3 needs --raw: CacheGen codes 16-bit KV only")
     import torch
 
     import __graft_entry__ as ge
@@ -166,12 +182,16 @@ def main():
     results = []
     for T in (int(x) for x in args.tokens.split(",")):
         try:
-            results.append(run(T, args.chunk, args.steps, args.warmup, args.cold))
+            results.append(run(T, args.chunk, args.steps, args.warmup, args.cold, args.raw, args.dtype))
         except torch.cuda.OutOfMemoryError:
             results.append({"tokens": T, "skipped": "does not fit on the card"})
         torch.cuda.empty_cache()
-    print(json.dumps({"metric": "layerwise_retrieve_ms", "chunk": args.chunk, "steps": args.steps, "warmup": args.warmup,
-                      "gpu": torch.cuda.get_device_name(0), "power_limit": _power_limit(), "results": results}))
+    out = {"metric": "layerwise_retrieve_ms", "chunk": args.chunk, "steps": args.steps, "warmup": args.warmup,
+           "gpu": torch.cuda.get_device_name(0), "power_limit": _power_limit()}
+    if args.raw is not None:
+        out.update(raw=args.raw, dtype=args.dtype, kv_heads=8)
+    out["results"] = results
+    print(json.dumps(out))
 
 
 if __name__ == "__main__":

@@ -2,7 +2,7 @@
 """layerwise_store_bench.py -- what a layer-by-layer store costs and hides during a prefill step, on one GPU.
 
   python layerwise_store_bench.py [--steps K] [--warmup W] [--tokens 8192,65536] [--ffn F]
-                                  [--local-serde cachegen|lossless] [--dtype bf16|fp16]
+                                  [--local-serde cachegen|lossless] [--dtype bf16|fp16|e4m3] [--raw cpu|cuda]
 
 Model of a prefill step: L = 32 layers, 32 KV heads x 128 dims, bf16, chunk 256, a paged KV cache (block 16, scrambled
 slot mapping).  Per layer the forward stream runs a stand-in for the layer's compute -- one [T, 4096] x [4096, F] bf16
@@ -22,7 +22,11 @@ Containers of both legs are compared through digests of their bytes after the ti
 the chunks both legs hold; chunks_landed says how many each leg holds (a layer-wise store keeps the prefix of chunks that
 fit its device arena, LMCACHE_B200_LAYERWISE_STORE_MB).  --local-serde lossless stores lossless containers (versions 5
 and 6) instead of CacheGen ones, --dtype fp16 keeps an fp16 KV cache; the JSON line names them when they are not the
-defaults.  Prints one JSON line.  Writes nothing into the tree.
+defaults.  --raw cpu / --raw cuda store into a raw tier instead (local_device "cpu" / "cuda" without a serde: chunk
+blobs packed one layer at a time), with 8 of the 32 KV heads (a GQA shape: 65536 tokens of raw blobs fit the card) and
+--dtype e4m3 for an FP8 E4M3 cache; a raw tier is unbounded, so each step's blobs are dropped after it, and
+peak_hbm_mb is the step's peak of allocated device memory above what was allocated at its start.  Prints one JSON line.
+Writes nothing into the tree.
 """
 import argparse
 import hashlib
@@ -56,16 +60,31 @@ def _container_digests(engine, keys):
     return out
 
 
-def run(T, steps, warmup, ffn, serde="cachegen", dt="bf16"):
+def _raw_digests(engine, keys):
+    """sha256 of every chunk's raw blob, None for a chunk the tier does not hold"""
+    import torch
+
+    from lmcache_b200.storage_backend.local_backend import _HostEntry
+    out = []
+    for k in keys:
+        v = engine.engine_.dict.get(k)
+        if isinstance(v, _HostEntry):
+            v.wait()
+            v = v.host
+        out.append(None if v is None else hashlib.sha256(v.contiguous().view(-1).view(torch.uint8).cpu().numpy()).hexdigest())
+    return out
+
+
+def run(T, steps, warmup, ffn, serde="cachegen", dt="bf16", raw=None):
     import torch
 
     import bench
     from lmcache_b200.cache_engine import LMCacheEngine
     from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
-    L, H, D, cs, bs = 32, 32, 128, 256, 16
+    L, H, D, cs, bs = 32, 32 if raw is None else 8, 128, 256, 16
     dev = torch.device("cuda", 0)
-    dtype = torch.float16 if dt == "fp16" else torch.bfloat16
-    base = bench.synth_kv_torch(min(T, 8192), dev, seed=0).to(dtype)  # SURVEY 8d data, as bench.py's headline
+    dtype = {"fp16": torch.float16, "bf16": torch.bfloat16, "e4m3": torch.float8_e4m3fn}[dt]
+    base = bench.synth_kv_torch(min(T, 8192), dev, seed=0)[:, :, :, :H].to(dtype)  # SURVEY 8d data, as bench.py's headline
     reps = -(-T // base.shape[2])
     nblk = T // bs + 8
     try:
@@ -78,8 +97,12 @@ def run(T, steps, warmup, ffn, serde="cachegen", dt="bf16"):
     slots = torch.randperm(nblk * bs, device=dev)[:T]
     meta = LMCacheEngineMetadata("lmsys/longchat-7b-16k", 1, 0, "vllm", "float16" if dt == "fp16" else "bfloat16")
     # a fresh sequence per step: the tier is bounded (8 GiB), so older sequences are evicted
-    eng = LMCacheEngine(LMCacheEngineConfig.from_legacy(chunk_size=cs, backend="cpu", local_serde=serde,
-                                                        local_capacity_bytes=8 << 30), meta)
+    def new_engine(capacity=None):
+        if raw is not None:
+            return LMCacheEngine(LMCacheEngineConfig(cs, raw, None, None, False, False, None), meta)
+        return LMCacheEngine(LMCacheEngineConfig.from_legacy(chunk_size=cs, backend="cpu", local_serde=serde,
+                                                             local_capacity_bytes=capacity), meta)
+    eng = new_engine(8 << 30)
     fwd = torch.cuda.current_stream()
 
     def layer(l):
@@ -92,6 +115,8 @@ def run(T, steps, warmup, ffn, serde="cachegen", dt="bf16"):
         tokens = torch.arange(T, device=dev) + seq * T
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
         torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        mem0 = torch.cuda.memory_allocated()
         t0 = time.perf_counter()
         ev[0].record(fwd)
         call = 0.0
@@ -113,7 +138,14 @@ def run(T, steps, warmup, ffn, serde="cachegen", dt="bf16"):
             h.finish()
         ev[2].record(fwd)
         held = 0
-        if mode != "bare":
+        if mode != "bare" and raw is not None:
+            for k in [eng._make_key(d, "vllm") for d in eng._prefix_hash(tokens)]:
+                e = eng.engine_.dict.get(k)
+                if e is not None and hasattr(e, "wait"):
+                    e.wait()                         # the entry's last device->host copy
+                held += e is not None
+            torch.cuda.current_stream().synchronize()
+        elif mode != "bare":
             eng.retrieve(tokens[:1])                 # waits for the landing of chunk 0 ...
             for k in [eng._make_key(d, "vllm") for d in eng._prefix_hash(tokens)]:
                 e = eng.engine_.dict[k]
@@ -121,9 +153,12 @@ def run(T, steps, warmup, ffn, serde="cachegen", dt="bf16"):
                 held += e.error is None and e.rec is not None
         landed = time.perf_counter() - t0
         torch.cuda.synchronize()
+        peak = (torch.cuda.max_memory_allocated() - mem0) / 2 ** 20
+        if raw is not None:
+            eng.engine_.dict.clear()                 # unbounded tier: the next step's sequence is a fresh one
         return {"step_ms": ev[0].elapsed_time(ev[2]), "fwd_ms": ev[0].elapsed_time(ev[1]),
                 "store_tail_ms": ev[1].elapsed_time(ev[2]), "landed_ms": landed * 1e3, "call_ms": call * 1e3,
-                "chunks_held": held}, tokens
+                "chunks_held": held, "peak_hbm_mb": round(peak, 1)}, tokens
 
     res = {m: [] for m in ("bare", "store_paged", "layerwise")}
     seq = 1
@@ -136,7 +171,7 @@ def run(T, steps, warmup, ffn, serde="cachegen", dt="bf16"):
     # equality of the legs: the same tokens and KV stored by both, compared by container digests
     digests = []
     for m in ("store_paged", "layerwise"):
-        e2 = LMCacheEngine(LMCacheEngineConfig.from_legacy(chunk_size=cs, backend="cpu", local_serde=serde), meta)
+        e2 = new_engine()
         eng, keep = e2, eng
         tokens = torch.arange(T, device=dev) + 10 ** 7
         if m == "store_paged":
@@ -149,7 +184,8 @@ def run(T, steps, warmup, ffn, serde="cachegen", dt="bf16"):
                 layer(l)
                 h.save_layer(l)
             h.finish()
-        digests.append(_container_digests(eng, [eng._make_key(d, "vllm") for d in eng._prefix_hash(tokens)]))
+        keys = [eng._make_key(d, "vllm") for d in eng._prefix_hash(tokens)]
+        digests.append(_container_digests(eng, keys) if raw is None else _raw_digests(eng, keys))
         e2.close()
         eng = keep
     eng.close()
@@ -170,15 +206,20 @@ def main():
     ap.add_argument("--tokens", default="8192,65536")
     ap.add_argument("--ffn", type=int, default=14336)
     ap.add_argument("--local-serde", choices=("cachegen", "lossless"), default="cachegen")
-    ap.add_argument("--dtype", choices=("bf16", "fp16"), default="bf16")
+    ap.add_argument("--dtype", choices=("bf16", "fp16", "e4m3"), default="bf16")
+    ap.add_argument("--raw", choices=("cpu", "cuda"), default=None)
     a = ap.parse_args()
+    if a.dtype == "e4m3" and a.raw is None and a.local_serde == "cachegen":
+        raise SystemExit("--dtype e4m3 needs --raw or --local-serde lossless: CacheGen codes 16-bit KV only")
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("layerwise_store_bench.py needs a CUDA device")
     torch.cuda.set_device(0)
-    results = [run(int(t), a.steps, a.warmup, a.ffn, a.local_serde, a.dtype) for t in a.tokens.split(",")]
+    results = [run(int(t), a.steps, a.warmup, a.ffn, a.local_serde, a.dtype, a.raw) for t in a.tokens.split(",")]
     out = {"bench": "layerwise_store", "gpu": _gpu_info(), "ffn": a.ffn}
-    if a.local_serde != "cachegen" or a.dtype != "bf16":
+    if a.raw is not None:
+        out.update(raw=a.raw, dtype=a.dtype, kv_heads=8)
+    elif a.local_serde != "cachegen" or a.dtype != "bf16":
         out.update(local_serde=a.local_serde, dtype=a.dtype)
     out.update(arena_budget_mb=int(os.environ.get("LMCACHE_B200_LAYERWISE_STORE_MB", "1024")), results=results)
     print(json.dumps(out))

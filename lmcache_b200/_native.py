@@ -155,6 +155,10 @@ SIGNATURES = {
     "b200kv_sha256_chain_ready": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, ctypes.c_uint32, c_vp]),
     "b200kv_pack_chunks": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp]),
     "b200kv_unpack_chunks": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_i32, c_i32, ctypes.POINTER(KvDesc), c_i64, c_vp]),
+    "b200kv_pack_chunks_layers": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp,
+                                          c_vp]),
+    "b200kv_unpack_chunks_layers": (c_i32, [c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, ctypes.POINTER(KvDesc),
+                                            c_i64, c_vp]),
     "b200kv_pinned_alloc": (c_i32, [ctypes.POINTER(c_vp), c_i64]),
     "b200kv_pinned_free": (c_i32, [c_vp]),
     "b200kv_host_device_ptr": (c_i32, [c_vp, ctypes.POINTER(c_vp)]),

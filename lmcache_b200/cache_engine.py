@@ -197,8 +197,9 @@ class LayerwiseStore:
     pass.  save_layer(l, stream) says that layer l is written in `stream` order; finish(stream) completes the store.
     Neither waits on the host, except finish() on a lossless disk tier, which returns once the files are written, as
     the store() it replaced did (the tier's layerwise_store_blocking).  On the compressed host and disk tiers each layer
-    is encoded on a side stream as soon as it is saved (pipeline.LayerwiseEncode); elsewhere save_layer only records the
-    layer and finish() runs the ordinary store.  A handle dropped without finish() stores nothing and gives its device scratch back."""
+    is encoded on a side stream as soon as it is saved (pipeline.LayerwiseEncode), and on the raw cpu and cuda tiers
+    packed into its chunk blobs (local_backend.RawLayerwiseStore); elsewhere save_layer only records the layer and
+    finish() runs the ordinary store.  A handle dropped without finish() stores nothing and gives its device scratch back."""
 
     def __init__(self, num_layers: int, enc, on_finish: Callable):
         self.num_layers = num_layers
@@ -722,8 +723,8 @@ class LMCacheEngine:
     # ------------------------------------------------------------------ layer-wise retrieve
     def _layerwise_get(self):
         """(get_kv for _retrieve / _retrieve_paged, whose `uploads` list receives the LayerwiseUploads), or None: the
-        backend cannot serve this engine's chunks layer-major -- it says so (supports_layerwise_get: raw tiers, a remote
-        tier whose server has no ranged reads, a serde without containers), or its containers hold several groups
+        backend cannot serve this engine's chunks layer-major -- it says so (supports_layerwise_get: a remote tier whose
+        server has no ranged reads, a serde without containers), or its containers hold several groups
         (CacheGen containers of more than 256 tokens; a lossless container is always one group)"""
         f = getattr(self.engine_, "get_kv_layerwise", None)
         ok = getattr(self.engine_, "supports_layerwise_get", None)
@@ -751,7 +752,8 @@ class LMCacheEngine:
     def retrieve_layerwise(self, tokens: torch.Tensor, mask: Optional[torch.Tensor] = None) -> LayerwiseRetrieval:
         """retrieve(), with the KV made available one layer at a time: returns once the hit is known; ret_mask and the
         KV after synchronize() are those of retrieve().  On the compressed host and disk tiers the containers are
-        uploaded and decoded layer-major, so layer 0 is ready after about 1/L of the bytes.  On the remote tier, opted in
+        uploaded and decoded layer-major, so layer 0 is ready after about 1/L of the bytes; on the raw cpu and cuda tiers
+        each layer of every chunk blob is copied and unpacked in one launch per layer.  On the remote tier, opted in
         with LMCACHE_B200_REMOTE_LAYERWISE=1 and with a server that has ranged reads (this project's), they are also
         fetched layer-major: every chunk's layer l before
         any chunk's layer l + 1.  A hybrid tier does both parts so and joins them.  Chunks served from another
@@ -778,7 +780,8 @@ class LMCacheEngine:
     def _layerwise_store_ok(self, dtype: torch.dtype) -> bool:
         """Can this store be encoded layer by layer?  The compressed host and disk tiers can, for the KV their codec
         encodes (CacheGen: 16-bit; lossless: 16-bit and one-byte) and chunks of at most the tier's layerwise_max_tokens
-        (256 for CacheGen's version-3 containers, 4096 for lossless ones); raw, remote and hybrid tiers cannot."""
+        (256 for CacheGen's version-3 containers, 4096 for lossless ones); the raw cpu and cuda tiers can for every
+        chunk size and every KV the mover moves; remote and hybrid tiers cannot."""
         return (getattr(self.engine_, "begin_layerwise_store", None) is not None and self._fast_path() and
                 self.chunk_size <= self.engine_.layerwise_max_tokens and dtype in NATIVE_DTYPES)
 

@@ -26,17 +26,23 @@ struct PackParams {
     const int64_t* slot_map;       // paged KV: token i lives in row slot_map[i]; NULL = row i
     int32_t L, H, D, n_chunks, chunk_tokens, last_chunk_tokens, hf_layout;
     int32_t ppl;                   // planes per layer: 2 (K, V) or 1 (latent KV: chunk blob [L, t, H*D])
+    int32_t l0, nl;                // layers [l0, l0 + nl) move; a chunk holds only those, layer l0 first
     uint8_t* chunks;
     int64_t chunk_stride_bytes;
+    uint8_t* const* table;         // TABLE: chunk j starts at table[j] (a device array) instead of chunks + j * stride
 };
 static_assert(sizeof(PackParams) < kMaxParamBytes, "PackParams must stay under 4 KB of kernel parameters");
 
 // One grid-stride loop over (chunk, plane, token, vector) units; VEC elements of type E per unit (one 16-byte vector,
-// or one element).  vllm chunk layout [L,2,t,H,D]; huggingface [L,2,H,t,D]; a latent KV (ppl = 1) [L,t,H,D].
-template <class E, int VEC, bool PACK>
+// or one element).  vllm chunk layout [L,2,t,H,D]; huggingface [L,2,H,t,D]; a latent KV (ppl = 1) [L,t,H,D] -- of the
+// nl layers of the range, whose local layer i is the KV's layer l0 + i.
+// TABLE: the chunk pointers come from a device table the host never reads, so a vector instance checks each chunk's
+// alignment itself and moves a misaligned chunk's vectors element by element (a layer slice is a multiple of 16 bytes
+// whenever the vector path is taken, so the chunk pointer decides for all of its layers).
+template <class E, int VEC, bool PACK, bool TABLE>
 __global__ void __launch_bounds__(256) pack_kernel(PackParams P) {
     using vec_t = typename std::conditional<VEC * sizeof(E) == 16, uint4, E>::type;
-    const int NL = P.ppl * P.L;
+    const int NL = P.ppl * P.nl;
     const int vph = P.D / VEC;                 // vectors per head row
     const int64_t vpt = (int64_t)P.H * vph;    // vectors per token
     const int64_t per_chunk_full = (int64_t)NL * P.chunk_tokens * vpt;
@@ -46,15 +52,15 @@ __global__ void __launch_bounds__(256) pack_kernel(PackParams P) {
         if (j >= P.n_chunks) j = P.n_chunks - 1;
         int64_t r = u - j * per_chunk_full;
         const int t = (j == P.n_chunks - 1) ? P.last_chunk_tokens : P.chunk_tokens;
-        // r indexes [l][kv][tok][h][v] of the chunk (vllm order) -- map to plane nl = kv*L + l
+        // r indexes [l][kv][tok][h][v] of the chunk (vllm order) -- map to plane kv*L + l0 + l
         const int64_t per_plane = (int64_t)t * vpt;
-        const int lk = (int)(r / per_plane);       // l*ppl + kv
+        const int lk = (int)(r / per_plane);       // l*ppl + kv, l local to the range
         r -= (int64_t)lk * per_plane;
         const int tok = (int)(r / vpt);
         r -= (int64_t)tok * vpt;
         const int h = (int)(r / vph);
         const int v = (int)(r - (int64_t)h * vph);
-        const int l = P.ppl == 2 ? lk >> 1 : lk, kv = P.ppl == 2 ? lk & 1 : 0;
+        const int l = P.l0 + (P.ppl == 2 ? lk >> 1 : lk), kv = P.ppl == 2 ? lk & 1 : 0;
         const E* plane = reinterpret_cast<const E*>(P.pt.p[kv * P.L + l]);
         int64_t row = P.tok_begin + j * P.chunk_tokens + tok;
         if (P.slot_map) row = __ldg(P.slot_map + row);       // consecutive threads share the token: broadcast, L1 hit
@@ -62,39 +68,56 @@ __global__ void __launch_bounds__(256) pack_kernel(PackParams P) {
         int64_t dst_off;   // in elements, inside the chunk
         if (P.hf_layout) dst_off = (((int64_t)lk * P.H + h) * t + tok) * P.D + (int64_t)v * VEC;
         else dst_off = (((int64_t)lk * t + tok) * P.H + h) * P.D + (int64_t)v * VEC;
-        E* cptr = reinterpret_cast<E*>(P.chunks + j * P.chunk_stride_bytes) + dst_off;
+        uint8_t* base;
+        if (TABLE) base = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(P.table) + j));
+        else base = P.chunks + j * P.chunk_stride_bytes;
+        E* cptr = reinterpret_cast<E*>(base) + dst_off;
+        if (TABLE && VEC > 1 && (reinterpret_cast<uintptr_t>(base) & 15) != 0) {
+            E* kptr = const_cast<E*>(plane) + src_off;
+#pragma unroll
+            for (int e = 0; e < VEC; ++e) {
+                if (PACK) cptr[e] = kptr[e];
+                else kptr[e] = cptr[e];
+            }
+            continue;
+        }
         if (PACK) *reinterpret_cast<vec_t*>(cptr) = *reinterpret_cast<const vec_t*>(plane + src_off);
         else *reinterpret_cast<vec_t*>(const_cast<E*>(plane) + src_off) = *reinterpret_cast<const vec_t*>(cptr);
     }
 }
 
-template <class E>
+template <class E, bool TABLE>
 static void launch_pack_kernel(bool pack, bool vec, unsigned blocks, const PackParams& P, cudaStream_t stream) {
     constexpr int V = 16 / sizeof(E);
     if (pack) {
-        if (vec) pack_kernel<E, V, true><<<blocks, 256, 0, stream>>>(P);
-        else pack_kernel<E, 1, true><<<blocks, 256, 0, stream>>>(P);
+        if (vec) pack_kernel<E, V, true, TABLE><<<blocks, 256, 0, stream>>>(P);
+        else pack_kernel<E, 1, true, TABLE><<<blocks, 256, 0, stream>>>(P);
     } else {
-        if (vec) pack_kernel<E, V, false><<<blocks, 256, 0, stream>>>(P);
-        else pack_kernel<E, 1, false><<<blocks, 256, 0, stream>>>(P);
+        if (vec) pack_kernel<E, V, false, TABLE><<<blocks, 256, 0, stream>>>(P);
+        else pack_kernel<E, 1, false, TABLE><<<blocks, 256, 0, stream>>>(P);
     }
 }
 
+// layer_end < 0: every layer.  table != NULL: chunk j starts at table[j] (chunks and chunk_stride_bytes unused).
 static int launch_pack(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
-                       int32_t last_chunk_tokens, int32_t hf_layout, void* chunks, int64_t chunk_stride_bytes,
-                       cudaStream_t stream) {
+                       int32_t last_chunk_tokens, int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
+                       void* chunks, int64_t chunk_stride_bytes, void* const* table, cudaStream_t stream) {
     PackParams P;
     B2_REQUIRE(kv != nullptr && kv->L > 0 && 2 * kv->L <= B200KV_MAX_PLANES, "bad kv descriptor");
+    if (layer_end < 0) layer_end = kv->L;
+    B2_REQUIRE(0 <= layer_begin && layer_begin < layer_end && layer_end <= kv->L, "bad layer range");
     float bins[B200KV_MAX_PLANES];
     for (int i = 0; i < B200KV_MAX_PLANES; ++i) bins[i] = 32.0f;   // unused by pack/unpack; keeps the table valid
     if (int rc = make_plane_table(kv, bins, bins, &P.pt)) return rc;
     B2_REQUIRE(n_chunks > 0 && chunk_tokens > 0 && last_chunk_tokens > 0 && last_chunk_tokens <= chunk_tokens,
                "bad chunking");
-    B2_REQUIRE(chunks != nullptr, "chunks is NULL");
+    B2_REQUIRE(table != nullptr || chunks != nullptr, "chunks is NULL");
     P.ppl = kv_ppl(kv);
+    P.l0 = layer_begin;
+    P.nl = layer_end - layer_begin;
     const int es = kv_elem_bytes(kv);
-    const int64_t chunk_bytes = (int64_t)es * kv->L * P.ppl * chunk_tokens * kv->H * kv->D;
-    B2_REQUIRE(chunk_stride_bytes >= chunk_bytes || n_chunks == 1, "chunk_stride_bytes too small");
+    const int64_t chunk_bytes = (int64_t)es * P.nl * P.ppl * chunk_tokens * kv->H * kv->D;
+    B2_REQUIRE(table != nullptr || chunk_stride_bytes >= chunk_bytes || n_chunks == 1, "chunk_stride_bytes too small");
     P.sT = kv->sT; P.sH = kv->sH; P.tok_begin = tok_begin;
     P.slot_map = kv->slot_map;
     P.L = kv->L; P.H = kv->H; P.D = kv->D;
@@ -102,12 +125,16 @@ static int launch_pack(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, i
     P.hf_layout = hf_layout;
     P.chunks = static_cast<uint8_t*>(chunks);
     P.chunk_stride_bytes = chunk_stride_bytes;
+    P.table = reinterpret_cast<uint8_t* const*>(table);
     const int ev = 16 / es;                    // elements per 16-byte vector
+    // a table's entries are checked by the kernel (they are in device memory)
     bool vec = (kv->D % ev == 0) && (kv->sT % ev == 0) && (kv->sH % ev == 0) &&
-               ((reinterpret_cast<uintptr_t>(chunks) & 15) == 0) && (chunk_stride_bytes % 16 == 0);
-    for (int nl = 0; nl < P.ppl * P.L && vec; ++nl) vec = (reinterpret_cast<uintptr_t>(P.pt.p[nl]) & 15) == 0;
+               (table != nullptr || (((reinterpret_cast<uintptr_t>(chunks) & 15) == 0) && (chunk_stride_bytes % 16 == 0)));
+    for (int kvi = 0; kvi < P.ppl && vec; ++kvi)
+        for (int l = layer_begin; l < layer_end && vec; ++l)
+            vec = (reinterpret_cast<uintptr_t>(P.pt.p[kvi * P.L + l]) & 15) == 0;
     const int V = vec ? ev : 1;
-    const int64_t total = ((int64_t)(n_chunks - 1) * chunk_tokens + last_chunk_tokens) * P.ppl * kv->L * kv->H * (kv->D / V);
+    const int64_t total = ((int64_t)(n_chunks - 1) * chunk_tokens + last_chunk_tokens) * P.ppl * P.nl * kv->H * (kv->D / V);
     int64_t blocks = (total + 255) / 256;
     int dev = 0, sms = 0;
     B2_CHECK_CUDA(cudaGetDevice(&dev));
@@ -115,8 +142,13 @@ static int launch_pack(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, i
     const int64_t cap = (int64_t)sms * 8 * 4;   // a few waves of SMs x 8 CTAs; grid-stride covers the rest
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
-    if (es == 2) launch_pack_kernel<uint16_t>(pack, vec, (unsigned)blocks, P, stream);
-    else launch_pack_kernel<uint8_t>(pack, vec, (unsigned)blocks, P, stream);
+    if (table != nullptr) {
+        if (es == 2) launch_pack_kernel<uint16_t, true>(pack, vec, (unsigned)blocks, P, stream);
+        else launch_pack_kernel<uint8_t, true>(pack, vec, (unsigned)blocks, P, stream);
+    } else {
+        if (es == 2) launch_pack_kernel<uint16_t, false>(pack, vec, (unsigned)blocks, P, stream);
+        else launch_pack_kernel<uint8_t, false>(pack, vec, (unsigned)blocks, P, stream);
+    }
     B2_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -130,15 +162,33 @@ extern "C" {
 int b200kv_pack_chunks(const b200kv_kv_desc* src, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
                        int32_t last_chunk_tokens, int32_t hf_layout, void* chunks, int64_t chunk_stride_bytes,
                        void* stream) {
-    return launch_pack(true, src, tok_begin, n_chunks, chunk_tokens, last_chunk_tokens, hf_layout, chunks,
-                       chunk_stride_bytes, static_cast<cudaStream_t>(stream));
+    return launch_pack(true, src, tok_begin, n_chunks, chunk_tokens, last_chunk_tokens, hf_layout, 0, -1, chunks,
+                       chunk_stride_bytes, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 int b200kv_unpack_chunks(const void* chunks, int64_t chunk_stride_bytes, int32_t n_chunks, int32_t chunk_tokens,
                          int32_t last_chunk_tokens, int32_t hf_layout, const b200kv_kv_desc* dst, int64_t tok_begin,
                          void* stream) {
-    return launch_pack(false, dst, tok_begin, n_chunks, chunk_tokens, last_chunk_tokens, hf_layout,
-                       const_cast<void*>(chunks), chunk_stride_bytes, static_cast<cudaStream_t>(stream));
+    return launch_pack(false, dst, tok_begin, n_chunks, chunk_tokens, last_chunk_tokens, hf_layout, 0, -1,
+                       const_cast<void*>(chunks), chunk_stride_bytes, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+int b200kv_pack_chunks_layers(const b200kv_kv_desc* src, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
+                              int32_t last_chunk_tokens, int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
+                              void* const* chunk_ptrs, void* stream) {
+    B2_REQUIRE(chunk_ptrs != nullptr, "chunk_ptrs is NULL");
+    B2_REQUIRE(layer_end >= 0, "bad layer range");
+    return launch_pack(true, src, tok_begin, n_chunks, chunk_tokens, last_chunk_tokens, hf_layout, layer_begin,
+                       layer_end, nullptr, 0, chunk_ptrs, static_cast<cudaStream_t>(stream));
+}
+
+int b200kv_unpack_chunks_layers(const void* const* chunk_ptrs, int32_t n_chunks, int32_t chunk_tokens,
+                                int32_t last_chunk_tokens, int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
+                                const b200kv_kv_desc* dst, int64_t tok_begin, void* stream) {
+    B2_REQUIRE(chunk_ptrs != nullptr, "chunk_ptrs is NULL");
+    B2_REQUIRE(layer_end >= 0, "bad layer range");
+    return launch_pack(false, dst, tok_begin, n_chunks, chunk_tokens, last_chunk_tokens, hf_layout, layer_begin,
+                       layer_end, nullptr, 0, const_cast<void* const*>(chunk_ptrs), static_cast<cudaStream_t>(stream));
 }
 
 int b200kv_pinned_alloc(void** host_ptr, int64_t bytes) {

@@ -10,9 +10,12 @@ a "non-blocking put" is simply a put whose event has not been waited on yet), an
 ordered on the caller's stream.
 """
 import ctypes
+import sys
 import threading
-from typing import Dict, Optional
+import time
+from typing import Dict, List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from lmcache_b200 import _native as N
@@ -45,6 +48,166 @@ def _copy_async(dst: torch.Tensor, src: torch.Tensor, stream: torch.cuda.Stream)
                                       src.numel() * src.element_size(), stream.cuda_stream), "copy_async")
 
 
+# ---------------------------------------------------------------------------------------------- layer slices of raw blobs
+# A raw chunk blob of t tokens holds its layers back to back: layer l is one contiguous slice of t * row bytes at
+# l * t * row, where row = ppl * H * D * element bytes (ppl = 2 for [L,2,t,H,D] / [L,2,H,t,D], 1 for a latent [L,t,D]).
+LAYER_SLOTS = 3          # staging ring of the raw cpu tier's layer-wise paths: a layer's copy overlaps the previous unpack
+
+
+def layer_row_bytes(H: int, D: int, elem_bytes: int, latent: bool) -> int:
+    """bytes per token of one layer slice of a raw chunk blob (H = 1 for a latent KV)"""
+    return (1 if latent else 2) * H * D * elem_bytes
+
+
+def layer_table(bases: Sequence[int], tokens: Sequence[int], row_bytes: int, layer: int) -> np.ndarray:
+    """uint64 [n]: where layer `layer` of chunk j starts, for chunk blobs at bases[j] of tokens[j] tokens each -- the
+    chunk_ptrs of b200kv_pack_chunks_layers / b200kv_unpack_chunks_layers for the range [layer, layer + 1).  A staging
+    area that holds one layer of every chunk back to back is layer_table(area + packed_offsets(tokens, row), ..., 0)."""
+    return np.asarray(bases, dtype=np.uint64) + np.uint64(layer * row_bytes) * np.asarray(tokens, dtype=np.uint64)
+
+
+def packed_offsets(tokens: Sequence[int], row_bytes: int) -> np.ndarray:
+    """uint64 [n]: offset of chunk j's slice in an area that holds one layer slice of each chunk back to back"""
+    sl = np.asarray(tokens, dtype=np.uint64) * np.uint64(row_bytes)
+    return np.concatenate([np.zeros(1, np.uint64), np.cumsum(sl, dtype=np.uint64)[:-1]]) if len(sl) else sl
+
+
+def chunk_runs(tokens: Sequence[int], chunk_size: int) -> List[tuple]:
+    """The chunk ranges [a, b) one mover launch takes: every chunk but the range's last has chunk_size tokens, and its
+    last at most that many; a chunk of any other size moves alone.  Returns (a, b, chunk_tokens, last_chunk_tokens)."""
+    runs, a = [], 0
+    for j, t in enumerate(tokens):
+        if t > chunk_size and a < j:                 # a longer chunk is never the tail of a run
+            runs.append((a, j, chunk_size, tokens[j - 1]))
+            a = j
+        if t != chunk_size or j == len(tokens) - 1:
+            runs.append((a, j + 1, chunk_size if j > a else t, t))
+            a = j + 1
+    return runs
+
+
+def _device_table(rows: np.ndarray, device, stream: torch.cuda.Stream) -> torch.Tensor:
+    """a pointer table in device memory, uploaded on `stream` (which is also the stream the allocator ties it to)"""
+    with torch.cuda.stream(stream):
+        return torch.from_numpy(np.ascontiguousarray(rows).view(np.int64)).pin_memory().to(device, non_blocking=True)
+
+
+def _mover_layers(pack: bool, view, table_ptr: int, tok_begin: int, run: tuple, layer: int, stream) -> None:
+    a, b, ct, lt = run
+    hf = int(getattr(view, "fmt", "vllm") == "huggingface")
+    if pack:
+        rc = N.lib().b200kv_pack_chunks_layers(ctypes.byref(view.desc), tok_begin, b - a, ct, lt, hf, layer, layer + 1,
+                                               ctypes.c_void_p(table_ptr + 8 * a), stream.cuda_stream)
+    else:
+        rc = N.lib().b200kv_unpack_chunks_layers(ctypes.c_void_p(table_ptr + 8 * a), b - a, ct, lt, hf, layer, layer + 1,
+                                                 ctypes.byref(view.desc), tok_begin, stream.cuda_stream)
+    N.check(rc, "pack_chunks_layers" if pack else "unpack_chunks_layers")
+
+
+class RawLayerwiseStore:
+    """One layer-wise store into a raw tier (LMCLocalBackend.begin_layerwise_store): what LayerwiseStore uses of a
+    pipeline.LayerwiseEncode.  encode_layer(l, stream) packs layer l of every chunk (b200kv_pack_chunks_layers) on the
+    tier's pack stream behind an event on `stream`.  The cuda tier packs straight into the final blobs; the cpu tier
+    packs into a device ring of LAYER_SLOTS layer slots and moves each layer into the store's page-locked buffer with one
+    strided copy on the copy stream, so that the store holds a few layers of HBM, not the whole store.  The blobs are
+    byte for byte those of KvView.pack_chunks (store / store_paged)."""
+
+    def __init__(self, tier: "LMCLocalBackend", view, tok_begin: int, chunk_size: int):
+        n_tok = view.ntokens - tok_begin
+        n = (n_tok + chunk_size - 1) // chunk_size
+        self.tier, self.view, self.tok_begin, self.cs = tier, view, tok_begin, chunk_size
+        self.L, self.H, self.D, self.latent, self.fmt = view.L, view.H, view.D, view.latent, view.fmt
+        self.sizes = [min(chunk_size, n_tok - j * chunk_size) for j in range(n)]
+        self.run = (0, n, chunk_size, self.sizes[-1])
+        es = view.dtype.itemsize
+        self.row = layer_row_bytes(view.H, view.D, es, view.latent)
+        self.stride = view.L * self.row * chunk_size             # bytes between chunk blobs, as in pack_chunks
+        self.ps, self.cs_stream = tier._layer_streams(view.device)
+        self.saves = 0
+        self.copied: List[torch.cuda.Event] = []                 # cpu tier: the copy event of each save, in save order
+        self.done: Optional[torch.cuda.Event] = None
+        self.host = None
+        with torch.cuda.device(view.device):
+            view.record_stream(self.ps)                          # the caller's KV outlives the last pack that reads it
+            if tier.device == "cuda":
+                # allocated on the caller's stream like pack_chunks' buffer: the entries are read there afterwards
+                self.buf = torch.empty(n * self.stride // es, dtype=view.dtype, device=view.device)
+                self.buf.record_stream(self.ps)
+                rows = np.stack([layer_table(self.buf.data_ptr() + self.stride * np.arange(n, dtype=np.uint64),
+                                             self.sizes, self.row, l) for l in range(view.L)])
+            else:
+                self.host = torch.empty(n * self.stride // es, dtype=view.dtype, pin_memory=True)
+                self.slot_bytes = n_tok * self.row
+                with torch.cuda.stream(self.ps):
+                    self.buf = torch.empty(LAYER_SLOTS * self.slot_bytes, dtype=torch.uint8, device=view.device)
+                self.buf.record_stream(self.cs_stream)
+                offs = packed_offsets(self.sizes, self.row)
+                rows = np.stack([np.uint64(self.buf.data_ptr() + r * self.slot_bytes) + offs for r in range(LAYER_SLOTS)])
+            self.table = _device_table(rows, view.device, self.ps)
+
+    def encode_layer(self, layer: int, stream: torch.cuda.Stream) -> None:
+        with torch.cuda.device(self.view.device):
+            ev = torch.cuda.Event()
+            ev.record(stream)
+            self.ps.wait_event(ev)
+            k, self.saves = self.saves, self.saves + 1
+            if self.host is None:
+                _mover_layers(True, self.view, self.table[layer].data_ptr(), self.tok_begin, self.run, layer, self.ps)
+                return
+            slot = k % LAYER_SLOTS
+            if k >= LAYER_SLOTS:
+                self.ps.wait_event(self.copied[k - LAYER_SLOTS])      # the slot's previous layer has left it
+            _mover_layers(True, self.view, self.table[slot].data_ptr(), self.tok_begin, self.run, layer, self.ps)
+            packed = torch.cuda.Event()
+            packed.record(self.ps)
+            self.cs_stream.wait_event(packed)
+            src = self.buf.data_ptr() + slot * self.slot_bytes
+            dst = self.host.data_ptr() + layer * self.cs * self.row
+            full = len(self.sizes) if self.sizes[-1] == self.cs else len(self.sizes) - 1
+            sl = self.cs * self.row
+            N.check(N.lib().b200kv_copy2d_async(ctypes.c_void_p(dst), self.stride, ctypes.c_void_p(src), sl, sl, full,
+                                                self.cs_stream.cuda_stream), "copy2d")
+            if full < len(self.sizes):                              # the ragged last chunk's slice
+                t = self.sizes[-1]
+                N.check(N.lib().b200kv_copy_async(ctypes.c_void_p(self.host.data_ptr() + full * self.stride +
+                                                                  layer * t * self.row),
+                                                  ctypes.c_void_p(src + full * sl), t * self.row,
+                                                  self.cs_stream.cuda_stream), "copy_async")
+            copied = torch.cuda.Event()
+            copied.record(self.cs_stream)
+            self.copied.append(copied)
+
+    def finish(self) -> torch.cuda.Event:
+        """the event after the last pack: the caller's KV is no longer read.  self.done: the blobs are complete"""
+        with torch.cuda.device(self.view.device):
+            last = torch.cuda.Event()
+            last.record(self.ps)
+            if self.host is None:
+                self.done = last
+            else:
+                self.done = torch.cuda.Event()
+                self.done.record(self.cs_stream)
+        self.view = None
+        return last
+
+    def blobs(self) -> list:
+        """the chunk blobs (device tensors, or page-locked views for the cpu tier), after finish()"""
+        out = []
+        base = self.buf if self.host is None else self.host
+        es = base.element_size()
+        for j, t in enumerate(self.sizes):
+            shape = (self.L, t, self.D) if self.latent else KvView.blob_shape(self.fmt, self.L, self.H, self.D, t)
+            off = j * self.stride // es
+            out.append(base[off: off + t * self.L * self.row // es].view(shape))
+        return out
+
+    def abandon(self) -> None:
+        """drop the store; copies still queued keep the page-locked buffer alive until they have run"""
+        if self.host is not None and self.copied:
+            self.tier._keep_until(self.copied[-1], self.host)
+        self.view, self.host, self.buf = None, None, None
+
+
 class LMCLocalBackend(LMCBackendInterface):
 
     def __init__(self, config: LMCacheEngineConfig, metadata=None):
@@ -59,12 +222,25 @@ class LMCLocalBackend(LMCBackendInterface):
         self.dict: Dict[CacheEngineKey, object] = {}
         self.update_lock = threading.Lock()
         self._side: Optional[torch.cuda.Stream] = None
+        self._layer: Optional[tuple] = None   # (mover stream, copy stream) of the layer-wise paths
         self._inflight = []   # (event, pinned tensor) of uploads still reading host memory
 
     def _side_stream(self, device) -> torch.cuda.Stream:
         if self._side is None or self._side.device != device:
             self._side = torch.cuda.Stream(device=device)
         return self._side
+
+    def _layer_streams(self, device) -> tuple:
+        """the streams of the layer-wise store and retrieve: one for the pack / unpack kernels, one for the copies"""
+        device = torch.device(device)
+        if self._layer is None or self._layer[0].device != device:
+            self._layer = (torch.cuda.Stream(device=device), torch.cuda.Stream(device=device))
+        return self._layer
+
+    def _keep_until(self, event: torch.cuda.Event, host) -> None:
+        """the page-locked block(s) `host` outlive the copies before `event` even if nothing else holds them"""
+        self._inflight = [(e, h) for e, h in self._inflight if not e.query()]
+        self._inflight.append((event, host))
 
     def contains(self, key: CacheEngineKey) -> bool:
         return key in self.dict
@@ -125,9 +301,35 @@ class LMCLocalBackend(LMCBackendInterface):
         t = val.host if isinstance(val, _HostEntry) else val
         return KvView.blob_geometry(t, fmt) if t.dim() == (3 if self.latent else 5) else None
 
-    def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True) -> int:
+    @property
+    def layerwise_max_tokens(self) -> int:
+        """the largest chunk a layer-major retrieve or a layer-wise store takes: raw blobs have no group limit"""
+        return sys.maxsize
+
+    def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int) -> RawLayerwiseStore:
+        """A layer-wise store of tokens [tok_begin, T) of `view`, whose KV may not be written yet (RawLayerwiseStore);
+        put_kv_chunks(..., encoded=it) publishes its blobs after finish()."""
+        return RawLayerwiseStore(self, view, tok_begin, chunk_size)
+
+    def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True,
+                      encoded: Optional[RawLayerwiseStore] = None) -> int:
         """Store tokens [tok_begin, T) of `view` as len(keys) chunk blobs: ONE gather kernel (b200kv_pack_chunks)
-        builds every chunk blob; for the host tier ONE device->host DMA moves them all into a page-locked slab."""
+        builds every chunk blob; for the host tier ONE device->host DMA moves them all into a page-locked slab.
+        encoded: a finished layer-wise store of these chunks (store_layerwise), whose blobs are published instead: the
+        host tier's entries complete with its last copy, which nothing waits for here unless `blocking`."""
+        if encoded is not None:
+            vals = encoded.blobs()
+            assert len(vals) == len(keys)
+            if encoded.host is not None:
+                vals = [_HostEntry(v, encoded.done, None) for v in vals]
+                if blocking:
+                    encoded.done.synchronize()
+                    for v in vals:
+                        v.event = None
+            with self.update_lock:
+                for key, v in zip(keys, vals):
+                    self.dict[key] = v
+            return len(vals)
         with torch.cuda.device(view.device):
             dev, vals = view.pack_chunks(tok_begin, chunk_size)
             assert len(vals) == len(keys)
@@ -227,6 +429,101 @@ class LMCLocalBackend(LMCBackendInterface):
                 src.record_stream(stream)
                 n += 1
         return n
+
+    def get_kv_layerwise(self, keys, dst, dst_tok0: int, chunk_size: int):
+        """get_kv_into in layer-major order: the hits (the rules of _get_kv_scatter) are known when this returns, with a
+        pipeline.LayerwiseUpload whose ready(l) is the event after layer l of every hit chunk is in `dst`.  Per layer,
+        one b200kv_unpack_chunks_layers over every hit chunk on the tier's mover stream: from the stored device blobs
+        (cuda tier), or (cpu tier) from a device slot of a LAYER_SLOTS ring that one batched copy on the copy stream
+        has filled with the layer's slice of every chunk, so that layer l + 1's copy runs while layer l is unpacked.
+        Everything is enqueued before this returns; the host never waits."""
+        from lmcache_b200.pipeline import LayerwiseUpload, _batch_copy
+        t0 = time.perf_counter()
+        L = dst.L
+        hits = []                                            # (stored value, source blob, tokens)
+        for i, key in enumerate(keys):
+            val = self.dict.get(key, None)
+            if val is None:
+                break
+            src = val.host if isinstance(val, _HostEntry) else val
+            if src.dim() != (3 if dst.latent else 5):
+                break                                       # a chunk of the other kind (latent / (K, V)): a miss
+            t = src.shape[KvView.token_dim(dst.fmt, dst.latent)]
+            tok = dst_tok0 + i * chunk_size
+            if tok + t > dst.ntokens or src.dtype != dst.dtype:
+                break
+            if src.numel() != dst.planes * dst.H * dst.D * t:
+                break                                       # another geometry: its slices are not this KV's layers
+            hits.append((val, src, t))
+        n = len(hits)
+        with torch.cuda.device(dst.device):
+            srcs = []
+            for val, src, _ in hits:
+                if isinstance(val, _HostEntry):
+                    if not src.is_contiguous():
+                        src = src.contiguous().pin_memory()
+                elif not src.is_cuda or not src.is_contiguous():
+                    src = src.contiguous().to(dst.device)        # on the current stream, before `start`
+                srcs.append(src)
+            start = torch.cuda.Event()
+            start.record(torch.cuda.current_stream())
+            if n == 0:
+                return LayerwiseUpload.completed(0, L, start)
+            ms, cs = self._layer_streams(dst.device)
+            ms.wait_event(start)
+            cs.wait_event(start)
+            for val, _, _ in hits:
+                if isinstance(val, _HostEntry) and val.event is not None:
+                    cs.wait_event(val.event)                # a store's copy into the block is still queued
+            dst.record_stream(ms)
+            tokens = [t for _, _, t in hits]
+            row = layer_row_bytes(dst.H, dst.D, dst.dtype.itemsize, dst.latent)
+            runs = chunk_runs(tokens, chunk_size)
+            bases = np.array([s.data_ptr() for s in srcs], dtype=np.uint64)
+            host = self.device != "cuda"
+            if host:
+                slot_bytes = sum(tokens) * row
+                with torch.cuda.stream(ms):
+                    staging = torch.empty(LAYER_SLOTS * slot_bytes, dtype=torch.uint8, device=dst.device)
+                staging.record_stream(cs)
+                offs = packed_offsets(tokens, row)
+                rows = np.stack([np.uint64(staging.data_ptr() + r * slot_bytes) + offs for r in range(LAYER_SLOTS)])
+                sizes = np.ascontiguousarray(np.asarray(tokens, dtype=np.int64) * row)
+            else:
+                for s in srcs:
+                    s.record_stream(ms)
+                rows = np.stack([layer_table(bases, tokens, row, l) for l in range(L)])
+            table = _device_table(rows, dst.device, ms)
+            upload = LayerwiseUpload(n, L)
+            copied = None
+            t1 = time.perf_counter()
+            upload.enqueue_s.append(t1 - t0)
+            upload.wait_s.append(0.0)
+            for layer in range(L):
+                if host:
+                    slot = layer % LAYER_SLOTS
+                    if layer >= LAYER_SLOTS:
+                        cs.wait_event(upload._ready[layer - LAYER_SLOTS])   # the slot's previous layer is unpacked
+                    dsts = np.ascontiguousarray(rows[slot])
+                    hsrc = layer_table(bases, tokens, row, layer)
+                    _batch_copy(dsts, hsrc, sizes, cs)
+                    copied = torch.cuda.Event()
+                    copied.record(cs)
+                    ms.wait_event(copied)
+                    tp = table[slot].data_ptr()
+                else:
+                    tp = table[layer].data_ptr()
+                for run in runs:
+                    _mover_layers(False, dst, tp, dst_tok0 + run[0] * chunk_size, run, layer, ms)
+                ev = torch.cuda.Event(enable_timing=True)     # a caller may time the layers against each other
+                ev.record(ms)
+                upload._publish(ev)
+                t0, t1 = t1, time.perf_counter()
+                upload.enqueue_s.append(t1 - t0)
+                upload.wait_s.append(0.0)
+            if host:
+                self._keep_until(copied, srcs)
+        return upload
 
     def close(self):
         for val in list(self.dict.values()):
