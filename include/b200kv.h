@@ -76,6 +76,19 @@ extern "C" {
                                  * decode whose coder and destination disagree on the flag is refused).  Added without
                                  * changing anything that existed: every entry point below that names "2L" means L for a latent
                                  * descriptor, and b200kv_decode_plan_heads refuses a latent destination. */
+#define B200KV_KV_PAGED_SPLIT 0x400  /* OR into b200kv_kv_desc.dtype: a paged (K, V) cache in the split layout of vLLM's
+                                      * PagedAttention / xFormers backend (PagedAttention.split_kv_cache), where a token's
+                                      * row is not contiguous.  Added without changing anything that existed
+                                      * (b200kv_version() stays 4).  planes[kv*L + l] are layer l's key and value block
+                                      * tensors, slot_map is required (slot s: block b = s / bs, offset o = s % bs), sT
+                                      * carries bs (block_size), sL / sKV / sH are unused.  With x = 16 / es (8 for 16-bit
+                                      * elements, 16 for one-byte ones), element (h, d) of slot s is, in elements,
+                                      *   key   [nb, H, D/x, bs, x]: planes[l]     + ((b*H + h)*(D/x) + d/x)*bs*x + o*x + d%x
+                                      *   value [nb, H, D, bs]:      planes[L + l] + ((b*H + h)*D + d)*bs + o
+                                      * Only the mover takes it: b200kv_pack_chunks / _unpack_chunks / _pack_chunks_layers /
+                                      * _unpack_chunks_layers, vllm chunk layout (hf_layout 0), D % x == 0.  Every CacheGen and
+                                      * lossless entry point refuses it (< 0, nothing enqueued): stage the KV into a blob with
+                                      * b200kv_pack_chunks first.  Not combined with B200KV_KV_LATENT. */
 #define B200KV_LP 33            /* CDF entries per stream (cachegen_encoder.py:287-289: int(bins.max()) + 1) */
 #define B200KV_GROUP_TOKENS 256 /* CACHEGEN_GPU_MAX_TOKENS_PER_CHUNK (cachegen_basics.py:13) */
 #define B200KV_MAX_PLANES 256   /* 2 * nlayers upper bound: models of up to 128 layers */

@@ -25,6 +25,7 @@ CODER_RANS = 1     # container version 2: rANS
 CODER_RANS_COMPACT = 2   # container version 3: rANS streams that carry their own histogram (no CDF section), one-byte lengths
 ENCODE_HINT_MID_ENTROPY = 0x200    # B200KV_ENCODE_HINT_MID_ENTROPY
 KV_LATENT = 0x100        # B200KV_KV_LATENT: OR-ed into KvDesc.dtype (one plane per layer) and into a coder (container version 4)
+KV_PAGED_SPLIT = 0x400   # B200KV_KV_PAGED_SPLIT: OR-ed into KvDesc.dtype (vLLM's PagedAttention split cache; mover only)
 CODER_LATENT = CODER_RANS_COMPACT | KV_LATENT   # the coder argument that names container version 4
 CODER_LOSSLESS = 4       # names container version 5: lossless, (K, V) planes (not a b200kv_encode_chunks coder)
 CODER_LOSSLESS_LATENT = CODER_LOSSLESS | KV_LATENT   # container version 6: lossless, one plane per layer

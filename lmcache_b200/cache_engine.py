@@ -19,7 +19,7 @@ from typing import Callable, Dict, Iterable, List, Optional, Tuple, Union
 import torch
 
 from lmcache_b200 import _native as N
-from lmcache_b200.codec import NATIVE_DTYPES, KvView, PinnedBuffer
+from lmcache_b200.codec import NATIVE_DTYPES, KvView, PinnedBuffer, paged_layout
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.logging import init_logger
 from lmcache_b200.storage_backend import CreateStorageBackend
@@ -351,6 +351,23 @@ class LMCacheEngine:
             return tuple(torch.unbind(blob, dim=0))                        # L views [T, D] of the [L, T, D] blob
         return tuple((layer[0], layer[1]) for layer in torch.unbind(blob, dim=0))
 
+    def _mover_paged(self, kv_caches) -> Optional[str]:
+        """The layout of a paged (K, V) cache whose rows torch indexing cannot reach in place ("strided", "split"): its
+        gathers and scatters go through the mover with a KvView.  None for the FlashAttention layout and latent caches."""
+        if self._mla:
+            return None
+        kind = paged_layout(*kv_caches[0]).kind
+        return None if kind == "flash" else kind
+
+    def _stages_split(self, kv_caches) -> bool:
+        """A split cache on a tier that reads KV views through the codec kernels (every container tier): its stores and
+        retrieves go through one device blob of the raw bytes of the tokens moved (KvView.staged / unpack_blob).  The raw
+        cpu and cuda tiers move a split view themselves (supports_split_view)."""
+        if self._mover_paged(kv_caches) != "split":
+            return False
+        f = getattr(self.engine_, "supports_split_view", None)
+        return not (f and f())
+
     def _flat_paged(self, kv_caches) -> list:
         """the paged caches as [num_slots, ...] views: per layer a latent cache, or a (key, value) pair"""
         if self._mla:
@@ -508,6 +525,11 @@ class LMCacheEngine:
         An MLA engine takes one latent cache [num_blocks, block_size, D] (or [num_slots, D]) per layer."""
         self._check_paged_args(tokens, slot_mapping, kv_caches)
         if not self._fast_path():
+            if self._mover_paged(kv_caches):
+                # the mover gathers the rows a torch index cannot reach in place
+                blob = KvView.from_paged(kv_caches, slot_mapping.cuda()).staged(0).blob
+                return self.store(tokens, tuple((blob[l, 0], blob[l, 1]) for l in range(blob.shape[0])), skip_existing,
+                                  blocking)
             flat = self._flat_paged(kv_caches)
             idx = slot_mapping.to(self._first(flat).device)
             g = lambda c: _bytes_of(c)[idx].view(c.dtype)  # noqa: E731
@@ -519,6 +541,9 @@ class LMCacheEngine:
         def put(keys, tok_begin):
             view = KvView.from_paged(kv_caches, slot_mapping.cuda())
             self._geom = (view.L, view.H, view.D, view.dtype)
+            if self._stages_split(kv_caches):
+                # one blob of the stored range for every part of the tier; the view keeps it alive for the tier's kernels
+                view, tok_begin = view.staged(tok_begin), 0
             return self.engine_.put_kv_chunks(keys, view, tok_begin, self.chunk_size, blocking=blocking)
         self._store_put(chunk_hashes, start, "vllm", put)
 
@@ -535,12 +560,18 @@ class LMCacheEngine:
         """retrieve_paged; get_kv as in _retrieve, for every chunk but a first one that straddles the mask"""
         self._check_paged_args(tokens, slot_mapping)
         self._check_kind(kv_caches, "kv_caches")
-        flat = self._flat_paged(kv_caches)
-        dev = self._first(flat).device
+        mover = self._mover_paged(kv_caches)
+        flat = None if mover else self._flat_paged(kv_caches)      # a strided cache's reshape would be a copy
+        dev = self._first(kv_caches).device
         slots = slot_mapping.to(dev)
         if not self._fast_path():
             kv, ret_mask = self.retrieve(tokens, mask)
-            if len(kv) > 0:
+            if len(kv) > 0 and self._mover_paged(kv_caches):
+                # the retrieved tokens are one run after the masked-off prefix: the mover scatters them
+                a = 0 if mask is None else int(len(mask) - torch.sum(mask))
+                blob = torch.stack([torch.stack(p) for p in kv]).to(self._first(kv_caches).dtype)
+                KvView.from_paged(kv_caches, slots[a:]).unpack_blob(blob, 0)
+            elif len(kv) > 0:
                 idx = slots[ret_mask.to(dev)]
                 if self._mla:
                     for c, x in zip(flat, kv):
@@ -564,7 +595,9 @@ class LMCacheEngine:
             tmp = torch.empty(KvView.blob_shape("vllm", view.L, view.H, view.D, t0, self._mla), dtype=view.dtype,
                               device=dev)
             layout, own, got_chunks = self._fetch(chunk_hashes[:1], "vllm", KvView.from_blob(tmp, "vllm"), 0)
-            if got_chunks:
+            if got_chunks and mover:
+                view.unpack_blob(tmp[:, :, extra:], extra)
+            elif got_chunks:
                 idx = slots[base + extra: base + t0]
                 if self._mla:
                     for l, c in enumerate(flat):
@@ -574,7 +607,16 @@ class LMCacheEngine:
                         _bytes_of(kc)[idx] = _bytes_of(tmp[l, 0, extra:])
                         _bytes_of(vc)[idx] = _bytes_of(tmp[l, 1, extra:])
         if got_chunks == first and len(chunk_hashes) > first:       # not after a straddling chunk that missed
-            layout, own_rest, n = self._fetch(chunk_hashes[first:], "vllm", view, first * cs, get_kv, layout)
+            dst, tok0 = view, first * cs
+            if self._stages_split(kv_caches):
+                # decoded into a blob of the tokens asked for, then only the retrieved ones unpacked into the cache
+                n_stage = view.ntokens - tok0
+                dst = KvView.from_blob(torch.empty(KvView.blob_shape("vllm", view.L, view.H, view.D, n_stage),
+                                                   dtype=view.dtype, device=dev), "vllm")
+                tok0 = 0
+            layout, own_rest, n = self._fetch(chunk_hashes[first:], "vllm", dst, tok0, get_kv, layout)
+            if dst is not view and n:
+                view.unpack_blob(dst.blob.narrow(2, 0, min(n * cs, n_stage)), first * cs)
             own += own_rest
             got_chunks += n
         self._touch(full_chain[:num_skip_chunk + own], "vllm")
@@ -772,7 +814,9 @@ class LMCacheEngine:
         """retrieve_paged(), with the KV made available one layer at a time (see retrieve_layerwise: the same tiers go
         layer-major, the remote one included).  A first chunk that straddles the mask is decoded and scattered whole
         before layer 0's wait; `kv` is None."""
-        get_kv, uploads = self._layerwise_get() or (None, [])
+        self._check_kind(kv_caches, "kv_caches")
+        # a split cache on a container tier is retrieved whole through its staging blob: one event for every layer
+        get_kv, uploads = (None if self._stages_split(kv_caches) else self._layerwise_get()) or (None, [])
         ret_mask = self._retrieve_paged(tokens, kv_caches, slot_mapping, mask, get_kv)
         return self._layerwise_result(ret_mask, None, len(kv_caches), uploads)
 
@@ -822,7 +866,8 @@ class LMCacheEngine:
         def fallback(stream, enc):
             with torch.cuda.stream(stream):
                 self.store_paged(tokens, kv_caches, slot_mapping, skip_existing)
-        if not self._layerwise_store_ok(self._first(kv_caches).dtype):
+        if not self._layerwise_store_ok(self._first(kv_caches).dtype) or self._stages_split(kv_caches):
+            # a split cache on a container tier is staged whole: the store runs at finish()
             return LayerwiseStore(len(kv_caches), None, fallback)
         return self._begin_layerwise(tokens, lambda: KvView.from_paged(kv_caches, slot_mapping.cuda()), "vllm",
                                      len(kv_caches), skip_existing, fallback)

@@ -63,6 +63,71 @@ class PinnedBuffer:
             pass
 
 
+class PagedLayout(NamedTuple):
+    """A paged (key, value) cache pair as paged_layout recognises it.  kind: "flash" (FlashAttention: contiguous
+    [nb, bs, H, D] or [num_slots, H, D] rows), "strided" (FlashInfer's kv[:, 0] / kv[:, 1] of a [nb, 2, bs, H, D] cache:
+    [nb, bs, H, D] rows whose blocks start rows_per_block rows apart) or "split" (PagedAttention / xFormers: key
+    [nb, H, D/x, bs, x], value [nb, H, D, bs], x elements per 16-byte key vector)."""
+    kind: str
+    nb: int
+    bs: int
+    H: int
+    D: int
+    rows_per_block: int      # "strided": block stride in rows; "flash": bs ([num_slots, H, D]: 1); "split": bs
+    x: int                   # "split": elements per 16-byte key vector; 0 otherwise
+
+
+def paged_layout(key: torch.Tensor, value: torch.Tensor) -> PagedLayout:
+    """The layout of one layer's (key_cache, value_cache) pair, from shapes, strides and dtype alone (no data is read,
+    any device).  ValueError for a pair no rule matches: key and value that disagree on nb, bs, H or D, D % x != 0, a
+    split or strided pair in a dtype the mover does not move, or strides of no known layout."""
+    if key.dtype != value.dtype:
+        raise ValueError(f"key and value caches differ in dtype ({key.dtype}, {value.dtype})")
+    native = key.dtype in _DTYPE_CODE
+    if key.dim() == 5:
+        if not native:
+            raise ValueError(f"a split paged cache must hold a dtype the mover moves ({NATIVE_DTYPES}), not {key.dtype}")
+        x = 16 // key.element_size()
+        nb, H, dx, bs, kx = key.shape
+        if value.dim() != 4:
+            raise ValueError(f"a split key cache [nb, H, D/x, bs, x] needs a value cache [nb, H, D, bs], got "
+                             f"{tuple(value.shape)}")
+        vnb, vH, D, vbs = value.shape
+        if (vnb, vH, vbs) != (nb, H, bs) or dx * kx != D:
+            raise ValueError(f"split key {tuple(key.shape)} and value {tuple(value.shape)} caches disagree on nb, bs, H "
+                             f"or D")
+        if kx != x or D % x != 0:
+            raise ValueError(f"a split paged cache of {key.dtype} needs x = {x} (16 bytes) and D % x == 0, got x = {kx}, "
+                             f"D = {D}")
+        if not (key.is_contiguous() and value.is_contiguous()):
+            raise ValueError("split paged caches must be contiguous (they are written in place)")
+        return PagedLayout("split", nb, bs, H, D, bs, x)
+    if key.dim() not in (3, 4) or key.shape != value.shape:
+        raise ValueError(f"paged key {tuple(key.shape)} and value {tuple(value.shape)} caches disagree on nb, bs, H or D "
+                         f"(or are of no known layout)")
+    if key.stride() != value.stride():
+        raise ValueError("paged key and value caches must share strides")
+    if key.dim() == 3:
+        nb, bs, (H, D) = key.shape[0], 1, key.shape[1:]
+    else:
+        nb, bs, H, D = key.shape
+    if key.is_contiguous():
+        return PagedLayout("flash", nb, bs, H, D, bs, 0)
+    HD = H * D
+    if key.dim() == 4 and key.stride()[1:] == (HD, D, 1) and key.stride(0) % HD == 0 and key.stride(0) >= bs * HD:
+        if not native:
+            raise ValueError(f"a block-strided paged cache must hold a dtype the mover moves ({NATIVE_DTYPES}), not "
+                             f"{key.dtype}")
+        return PagedLayout("strided", nb, bs, H, D, key.stride(0) // HD, 0)
+    raise ValueError("paged K/V caches must be contiguous [nb, bs, H, D] rows, block-strided rows (FlashInfer's kv[:, 0] "
+                     "and kv[:, 1]) or PagedAttention's split pair (they are written in place)")
+
+
+def strided_slots(slot_mapping: torch.Tensor, bs: int, rows_per_block: int) -> torch.Tensor:
+    """The row of each slot in a block-strided cache, on the slot map's device: (s // bs) * rows_per_block + s % bs."""
+    return torch.div(slot_mapping, bs, rounding_mode="floor") * rows_per_block + torch.remainder(slot_mapping, bs)
+
+
 class KvView:
     """A KV source / destination for the native library: either one strided blob tensor or the engine's
     tuple of 2L per-layer tensors (no stack / permute / contiguous copies).  Keeps the tensors alive.
@@ -81,6 +146,7 @@ class KvView:
         self.dtype = dtype
         self.fmt = fmt
         self.blob = blob      # the single blob tensor behind this view, when there is one
+        self.layout: Optional[str] = None    # a paged (K, V) view: "flash", "strided" or "split" (see paged_layout)
 
     @property
     def L(self): return self.desc.L
@@ -96,8 +162,12 @@ class KvView:
         return self.L if self.latent else 2 * self.L
     @property
     def dtype_code(self) -> int:
-        """N.DT_* of the elements (the descriptor's dtype without the latent flag)."""
-        return int(self.desc.dtype) & ~N.KV_LATENT
+        """N.DT_* of the elements (the descriptor's dtype without the latent and split flags)."""
+        return int(self.desc.dtype) & ~(N.KV_LATENT | N.KV_PAGED_SPLIT)
+    @property
+    def split(self) -> bool:
+        """a paged cache in PagedAttention's split layout: only the mover (pack / unpack) reads and writes it"""
+        return bool(self.desc.dtype & N.KV_PAGED_SPLIT)
 
     def record_stream(self, stream: torch.cuda.Stream) -> None:
         """Mark every tensor behind the view as used by work on `stream`: the caching allocator reuses none of them
@@ -287,17 +357,16 @@ class KvView:
         ref = kv_caches[0][0]
         if not ref.is_cuda:
             raise RuntimeError("KV caches must live on a CUDA device (no CPU fallback)")
+        lay = paged_layout(*kv_caches[0])
         keep = [slot_mapping]
         ptrs = (ctypes.c_void_p * (2 * L))()
         for l, (k, v) in enumerate(kv_caches):
+            if paged_layout(k, v) != lay or k.dtype != ref.dtype or k.device != ref.device or v.device != ref.device:
+                raise ValueError("all K/V caches must share layout, shape, strides, dtype and device")
             for kvi, t in ((0, k), (1, v)):
-                if t.shape != ref.shape or t.dtype != ref.dtype or t.device != ref.device or t.stride() != ref.stride():
-                    raise ValueError("all K/V caches must share shape, strides, dtype and device")
-                if not t.is_contiguous():
-                    raise ValueError("paged K/V caches must be contiguous (they are written in place)")
                 keep.append(t)
                 ptrs[kvi * L + l] = t.data_ptr()
-        H, D = ref.shape[-2], ref.shape[-1]
+        H, D = lay.H, lay.D
         d = N.KvDesc()
         d.base = None
         d.planes = ctypes.cast(ptrs, ctypes.POINTER(ctypes.c_void_p))
@@ -305,8 +374,37 @@ class KvView:
         d.sT, d.sH = H * D, D
         d.L, d.H, d.D = L, H, D
         d.dtype = KvView._code(ref.dtype)
+        if lay.kind == "strided":
+            # block b's rows start rows_per_block rows apart: every kernel reads the cache as rows through this slot map
+            slot_mapping = strided_slots(slot_mapping, lay.bs, lay.rows_per_block)
+            keep[0] = slot_mapping
+        elif lay.kind == "split":
+            d.sT, d.sH = lay.bs, 0                  # B200KV_KV_PAGED_SPLIT: sT carries the block size
+            d.dtype |= N.KV_PAGED_SPLIT
         d.slot_map = slot_mapping.data_ptr()
-        return KvView(d, (keep, ptrs), slot_mapping.numel(), ref.device, ref.dtype, "vllm")
+        view = KvView(d, (keep, ptrs), slot_mapping.numel(), ref.device, ref.dtype, "vllm")
+        view.layout = lay.kind
+        return view
+
+    def staged(self, tok_begin: int) -> "KvView":
+        """Tokens [tok_begin, T) of this view packed into one device blob [L, 2, T - tok_begin, H, D] by one mover launch
+        on the current stream, as a blob view (the view keeps the blob alive).  What the container tiers encode from when
+        the cache is split: its HBM cost is the raw bytes of those tokens."""
+        n = self.ntokens - tok_begin
+        buf, (blob,) = self.pack_chunks(tok_begin, n)
+        return KvView.from_blob(blob, "vllm")
+
+    def unpack_blob(self, blob: torch.Tensor, tok_begin: int) -> None:
+        """Write the t tokens of a vllm blob [L, 2, t, H, D] to tokens [tok_begin, tok_begin + t) of this view with one
+        b200kv_unpack_chunks launch on the current stream (the mover: any layout the view has)."""
+        t = blob.shape[2]
+        if t == 0:
+            return
+        blob = blob.contiguous()
+        with torch.cuda.device(self.device):
+            N.check(N.lib().b200kv_unpack_chunks(ctypes.c_void_p(blob.data_ptr()), blob.numel() * blob.element_size(),
+                                                 1, t, t, 0, ctypes.byref(self.desc), tok_begin, _stream_ptr(None)),
+                    "unpack_chunks")
 
     def pack_chunks(self, tok_begin: int, chunk_size: int) -> Tuple[torch.Tensor, List[torch.Tensor]]:
         """Gather tokens [tok_begin, T), at least one, into blobs of chunk_size tokens (the last may be shorter) with one

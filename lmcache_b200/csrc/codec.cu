@@ -1633,6 +1633,7 @@ __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
 // ------------------------------------------------------------------------------------------ host side
 int make_plane_table(const b200kv_kv_desc* kv, const float* key_bins, const float* value_bins, PlaneTable* out) {
     B2_REQUIRE(kv != nullptr, "kv descriptor is NULL");
+    B2_REQUIRE(!kv_split(kv), B2_SPLIT_REFUSED);
     B2_REQUIRE(kv->L > 0 && 2 * kv->L <= B200KV_MAX_PLANES, "L out of range");
     B2_REQUIRE(kv->H > 0 && kv->D > 0, "H/D must be positive");
     const int es = kv_elem_bytes(kv);
@@ -1659,6 +1660,7 @@ static int tiles_per_plane(int C) { return (C + CT - 1) / CT; }
 // stored by the lossless codec instead
 static int cachegen_dtype_ok(const b200kv_kv_desc* kv) {
     B2_REQUIRE(kv != nullptr, "kv descriptor is NULL");
+    B2_REQUIRE(!kv_split(kv), B2_SPLIT_REFUSED);
     B2_REQUIRE(kv_elem_bytes(kv) == 2,
                "CacheGen codes bf16 / fp16 KV only; one-byte (FP8) KV is stored by the lossless codec");
     return 0;

@@ -42,9 +42,16 @@ struct PlaneTableT {
 using PlaneTable = PlaneTableT<B200KV_MAX_PLANES>;
 constexpr size_t kMaxParamBytes = 4096;
 
-// Planes per layer of a kv_desc (1 for a latent KV, B200KV_KV_LATENT) and its element dtype without the flag.
+// Planes per layer of a kv_desc (1 for a latent KV, B200KV_KV_LATENT) and its element dtype without the latent flag.
+// The split flag (B200KV_KV_PAGED_SPLIT) is kept in kv_dtype on purpose: dtype_bytes of it is 0, so no entry point can
+// read a split descriptor as rows; the mover, the only one that takes it, clears it with kv_split_dtype.
 inline int kv_ppl(const b200kv_kv_desc* kv) { return (kv->dtype & B200KV_KV_LATENT) ? 1 : 2; }
 inline int kv_dtype(const b200kv_kv_desc* kv) { return kv->dtype & ~B200KV_KV_LATENT; }
+inline bool kv_split(const b200kv_kv_desc* kv) { return (kv->dtype & B200KV_KV_PAGED_SPLIT) != 0; }
+inline int kv_split_dtype(const b200kv_kv_desc* kv) { return kv->dtype & ~B200KV_KV_PAGED_SPLIT; }
+#define B2_SPLIT_REFUSED                                                                                             \
+    "a split paged descriptor (B200KV_KV_PAGED_SPLIT) is taken by the pack / unpack calls only: stage it into a "  \
+    "blob with b200kv_pack_chunks first"
 // Bytes per element of a B200KV_DT_* code (without the latent flag), 0 for an unknown code.
 inline int dtype_bytes(int dt) {
     return dt == B200KV_DT_BF16 || dt == B200KV_DT_FP16 ? 2

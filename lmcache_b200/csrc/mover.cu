@@ -98,12 +98,251 @@ static void launch_pack_kernel(bool pack, bool vec, unsigned blocks, const PackP
     }
 }
 
+// ---------------------------------------------------------------------------------------- split paged caches
+// B200KV_KV_PAGED_SPLIT (vLLM's PagedAttention / xFormers layout): per layer a key block tensor [nb, H, D/x, bs, x] and a
+// value block tensor [nb, H, D, bs] (x = 16 / es).  The chunk side is the vllm blob [nl, 2, t, H, D], as for rows.
+//
+// Work unit: one group of bs consecutive call tokens (slot-map indices [k*bs, k*bs + bs)) x one plane x hb heads.  A
+// group whose tokens all lie in the moved range and in one chunk, and whose slots are b*bs + 0 .. bs-1, is a tile: the
+// CTA moves it through shared memory (rows [hh][o][D] of `pitch` bytes), with coalesced accesses on both sides:
+//   key:   the cache holds 16-byte vectors (x channels of one token) in [D/x][bs] order per head: a permutation of
+//          vectors, read in cache order and written in chunk-row order;
+//   value: the cache holds [D][bs] per head, a real transpose: vw-byte vectors along the tokens of one channel are
+//          scattered into the rows, the rows leave as 16-byte vectors.
+// Every other group (a call that starts mid-block, a scrambled slot map, ragged ends, a misaligned chunk) moves element
+// by element in the same launch.
+struct SplitParams {
+    PlaneTable pt;                 // planes kv*L + l: layer l's key (kv 0) and value (kv 1) block tensors
+    const int64_t* slot_map;
+    uint8_t* chunks;
+    int64_t chunk_stride_bytes;
+    uint8_t* const* table;         // TABLE: chunk j starts at table[j]
+    int64_t tok_begin, k0;         // first call token; first group
+    int32_t n_groups, hb, nhb;     // groups; heads per unit; head blocks per group (H / hb)
+    int32_t L, H, D, bs, n_chunks, chunk_tokens, last_chunk_tokens, l0, nl;
+    int32_t vw;                    // bytes per value-side vector of the tile path (16 or 8); 0: element-wise only
+    int32_t pitch;                 // shared-memory bytes per token row of one head: D * es + 16
+};
+static_assert(sizeof(SplitParams) < kMaxParamBytes, "SplitParams must stay under 4 KB of kernel parameters");
+
+template <int W>
+struct VecOf;
+template <>
+struct VecOf<16> { using T = uint4; };
+template <>
+struct VecOf<8> { using T = uint2; };
+
+// value tile, cache side: W-byte vectors along the tokens of one channel <-> elements of the shared-memory rows
+template <class E, int W, bool PACK>
+__device__ __forceinline__ void split_value_tile(const SplitParams& P, E* cache, uint8_t* s) {
+    using V = typename VecOf<W>::T;
+    constexpr int VO = W / (int)sizeof(E);         // tokens per vector
+    const int noc = P.bs / VO;                     // vectors per channel row of the cache
+    const int nv = P.hb * P.D * noc;
+    for (int i = threadIdx.x; i < nv; i += blockDim.x) {
+        const int hh = i / (P.D * noc), r = i - hh * (P.D * noc);
+        const int d = r / noc, oc = r - d * noc;
+        E* srow = reinterpret_cast<E*>(s + (int64_t)(hh * P.bs + oc * VO) * P.pitch) + d;
+        union { V v; E e[VO]; } u;
+        if (PACK) {
+            u.v = *reinterpret_cast<const V*>(cache + (int64_t)i * VO);
+#pragma unroll
+            for (int e = 0; e < VO; ++e) srow[(int64_t)e * P.pitch / (int)sizeof(E)] = u.e[e];
+        } else {
+#pragma unroll
+            for (int e = 0; e < VO; ++e) u.e[e] = srow[(int64_t)e * P.pitch / (int)sizeof(E)];
+            *reinterpret_cast<V*>(cache + (int64_t)i * VO) = u.v;
+        }
+    }
+}
+
+template <class E, bool PACK, bool TABLE>
+__global__ void __launch_bounds__(256) split_kernel(SplitParams P) {
+    extern __shared__ __align__(16) uint8_t s_tile[];
+    constexpr int X = 16 / (int)sizeof(E);         // elements per 16-byte vector: the key's x
+    const int DX = P.D / X;
+    const int64_t g_end = P.tok_begin + (int64_t)(P.n_chunks - 1) * P.chunk_tokens + P.last_chunk_tokens;
+    const int64_t units = (int64_t)P.n_groups * 2 * P.nl * P.nhb;
+    for (int64_t u = blockIdx.x; u < units; u += gridDim.x) {
+        const int hbi = (int)(u % P.nhb);
+        const int64_t r = u / P.nhb;
+        const int64_t g0 = (P.k0 + r % P.n_groups) * P.bs;
+        const int lk = (int)(r / P.n_groups);      // local layer * 2 + kv
+        const int kv = lk & 1, h0 = hbi * P.hb;
+        E* plane = const_cast<E*>(reinterpret_cast<const E*>(P.pt.p[kv * P.L + P.l0 + (lk >> 1)]));
+        // tile test (uniform over the CTA until the slot check)
+        bool tile = P.vw != 0 && g0 >= P.tok_begin && g0 + P.bs <= g_end;
+        int64_t j = 0, blk = 0;
+        int tok0 = 0, t = 0;
+        uint8_t* base = nullptr;
+        if (tile) {
+            j = (g0 - P.tok_begin) / P.chunk_tokens;
+            tok0 = (int)(g0 - P.tok_begin - j * P.chunk_tokens);
+            t = j == P.n_chunks - 1 ? P.last_chunk_tokens : P.chunk_tokens;
+            base = TABLE ? reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(P.table) + j))
+                         : P.chunks + j * P.chunk_stride_bytes;
+            tile = tok0 + P.bs <= t && (!TABLE || (reinterpret_cast<uintptr_t>(base) & 15) == 0);
+        }
+        if (tile) {
+            const int64_t s0 = __ldg(P.slot_map + g0);
+            blk = s0 / P.bs;
+            bool ok = s0 % P.bs == 0;
+            for (int o = threadIdx.x; o < P.bs; o += blockDim.x) ok = ok && __ldg(P.slot_map + g0 + o) == s0 + o;
+            tile = __syncthreads_and(ok) != 0;
+        }
+        if (tile) {
+            E* cache = plane + (blk * P.H + h0) * (int64_t)P.D * P.bs;     // heads h0 .. h0 + hb - 1: contiguous
+            E* crow = reinterpret_cast<E*>(base) + (((int64_t)lk * t + tok0) * P.H + h0) * P.D;
+            const int nv = P.hb * P.bs * DX;       // 16-byte vectors of the tile
+            const int64_t HD = (int64_t)P.H * P.D;
+            if (!PACK) {                           // chunk rows -> shared memory
+                for (int i = threadIdx.x; i < nv; i += blockDim.x) {
+                    const int o = i / (P.hb * DX), q = i - o * (P.hb * DX), hh = q / DX, dx = q - hh * DX;
+                    *reinterpret_cast<uint4*>(s_tile + (int64_t)(hh * P.bs + o) * P.pitch + dx * 16) =
+                        *reinterpret_cast<const uint4*>(crow + o * HD + (int64_t)hh * P.D + dx * X);
+                }
+                __syncthreads();
+            }
+            if (kv == 0) {                         // key: vector i of the cache = (hh, dx, o)
+                for (int i = threadIdx.x; i < nv; i += blockDim.x) {
+                    const int hh = i / (P.bs * DX), q = i - hh * (P.bs * DX), dx = q / P.bs, o = q - dx * P.bs;
+                    uint4* sv = reinterpret_cast<uint4*>(s_tile + (int64_t)(hh * P.bs + o) * P.pitch + dx * 16);
+                    uint4* cv = reinterpret_cast<uint4*>(cache + (int64_t)i * X);
+                    if (PACK) *sv = *cv;
+                    else *cv = *sv;
+                }
+            } else if (P.vw == 16) {
+                split_value_tile<E, 16, PACK>(P, cache, s_tile);
+            } else {
+                split_value_tile<E, 8, PACK>(P, cache, s_tile);
+            }
+            if (PACK) {                            // shared memory -> chunk rows
+                __syncthreads();
+                for (int i = threadIdx.x; i < nv; i += blockDim.x) {
+                    const int o = i / (P.hb * DX), q = i - o * (P.hb * DX), hh = q / DX, dx = q - hh * DX;
+                    *reinterpret_cast<uint4*>(crow + o * HD + (int64_t)hh * P.D + dx * X) =
+                        *reinterpret_cast<const uint4*>(s_tile + (int64_t)(hh * P.bs + o) * P.pitch + dx * 16);
+                }
+            }
+            __syncthreads();                       // the next unit reuses the shared rows
+            continue;
+        }
+        // element-wise: every token of the group that the call moves, wherever its slot is
+        const int ne = P.bs * P.hb * P.D;
+        for (int i = threadIdx.x; i < ne; i += blockDim.x) {
+            const int o = i / (P.hb * P.D), q = i - o * (P.hb * P.D), hh = q / P.D, d = q - hh * P.D;
+            const int64_t g = g0 + o;
+            if (g < P.tok_begin || g >= g_end) continue;
+            const int64_t jj = (g - P.tok_begin) / P.chunk_tokens;
+            const int tok = (int)(g - P.tok_begin - jj * P.chunk_tokens);
+            const int tt = jj == P.n_chunks - 1 ? P.last_chunk_tokens : P.chunk_tokens;
+            uint8_t* cb = TABLE ? reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(P.table) + jj))
+                                : P.chunks + jj * P.chunk_stride_bytes;
+            const int64_t s = __ldg(P.slot_map + g), b = s / P.bs, so = s - b * P.bs;
+            const int h = h0 + hh;
+            const int64_t coff = kv == 0 ? (((b * P.H + h) * DX + d / X) * P.bs + so) * X + d % X
+                                         : ((b * P.H + h) * (int64_t)P.D + d) * P.bs + so;
+            E* ce = reinterpret_cast<E*>(cb) + (((int64_t)lk * tt + tok) * P.H + h) * P.D + d;
+            if (PACK) *ce = plane[coff];
+            else plane[coff] = *ce;
+        }
+    }
+}
+
+template <class E, bool TABLE>
+static int launch_split_kernel(bool pack, unsigned blocks, size_t smem, const SplitParams& P, cudaStream_t stream) {
+    auto k = pack ? split_kernel<E, true, TABLE> : split_kernel<E, false, TABLE>;
+    if (smem > 48 * 1024) B2_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k<<<blocks, 256, smem, stream>>>(P);
+    return 0;
+}
+
+static int launch_split(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
+                        int32_t last_chunk_tokens, int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
+                        void* chunks, int64_t chunk_stride_bytes, void* const* table, cudaStream_t stream) {
+    B2_REQUIRE(kv->L > 0 && 2 * kv->L <= B200KV_MAX_PLANES, "bad kv descriptor");
+    B2_REQUIRE(!(kv->dtype & B200KV_KV_LATENT), "a latent KV has no split layout (B200KV_KV_PAGED_SPLIT)");
+    B2_REQUIRE(hf_layout == 0, "a split paged KV (B200KV_KV_PAGED_SPLIT) moves to and from vllm chunks only (hf_layout 0)");
+    B2_REQUIRE(kv->slot_map != nullptr, "a split paged KV (B200KV_KV_PAGED_SPLIT) needs a slot_map");
+    const int es = dtype_bytes(kv_split_dtype(kv));
+    B2_REQUIRE(es != 0, "dtype must be one of B200KV_DT_*");
+    B2_REQUIRE(kv->H > 0 && kv->D > 0 && kv->sT > 0, "H, D and the block size (sT) must be positive");
+    B2_REQUIRE(kv->D % (16 / es) == 0, "a split paged KV needs D % x == 0 (x = 16 / element size)");
+    B2_REQUIRE(tok_begin >= 0, "tok_begin must be >= 0");
+    if (layer_end < 0) layer_end = kv->L;
+    B2_REQUIRE(0 <= layer_begin && layer_begin < layer_end && layer_end <= kv->L, "bad layer range");
+    B2_REQUIRE(n_chunks > 0 && chunk_tokens > 0 && last_chunk_tokens > 0 && last_chunk_tokens <= chunk_tokens,
+               "bad chunking");
+    B2_REQUIRE(table != nullptr || chunks != nullptr, "chunks is NULL");
+    SplitParams P;
+    b200kv_kv_desc rows = *kv;                 // the planes' pointers, read through the rows' table builder
+    rows.dtype = kv_split_dtype(kv);
+    float bins[B200KV_MAX_PLANES];
+    for (int i = 0; i < B200KV_MAX_PLANES; ++i) bins[i] = 32.0f;
+    if (int rc = make_plane_table(&rows, bins, bins, &P.pt)) return rc;
+    P.l0 = layer_begin;
+    P.nl = layer_end - layer_begin;
+    const int64_t chunk_bytes = (int64_t)es * P.nl * 2 * chunk_tokens * kv->H * kv->D;
+    B2_REQUIRE(table != nullptr || chunk_stride_bytes >= chunk_bytes || n_chunks == 1, "chunk_stride_bytes too small");
+    P.slot_map = kv->slot_map;
+    P.chunks = static_cast<uint8_t*>(chunks);
+    P.chunk_stride_bytes = chunk_stride_bytes;
+    P.table = reinterpret_cast<uint8_t* const*>(table);
+    P.tok_begin = tok_begin;
+    P.L = kv->L; P.H = kv->H; P.D = kv->D;
+    B2_REQUIRE(kv->sT <= (1 << 20), "block size out of range");
+    P.bs = (int32_t)kv->sT;
+    P.n_chunks = n_chunks; P.chunk_tokens = chunk_tokens; P.last_chunk_tokens = last_chunk_tokens;
+    const int64_t g_end = tok_begin + (int64_t)(n_chunks - 1) * chunk_tokens + last_chunk_tokens;
+    P.k0 = tok_begin / P.bs;
+    const int64_t n_groups = (g_end - 1) / P.bs - P.k0 + 1;
+    B2_REQUIRE(n_groups < (1ll << 31), "too many tokens");
+    P.n_groups = (int32_t)n_groups;
+    // heads per unit: the most that keep a tile within 16 KB (at least one)
+    const int64_t head_bytes = (int64_t)P.bs * P.D * es;
+    P.hb = 1;
+    for (int h = kv->H; h >= 1; --h)
+        if (kv->H % h == 0 && h * head_bytes <= 16384) { P.hb = h; break; }
+    P.nhb = kv->H / P.hb;
+    P.pitch = P.D * es + 16;
+    // the tile path: 16-byte aligned planes and chunks (a table's entries are checked by the kernel), a whole number of
+    // 8- or 16-byte vectors per cache channel row, and a tile that fits in shared memory
+    P.vw = (P.bs * es) % 16 == 0 ? 16 : (P.bs * es) % 8 == 0 ? 8 : 0;
+    if (table == nullptr && (((reinterpret_cast<uintptr_t>(chunks) & 15) != 0) || chunk_stride_bytes % 16 != 0)) P.vw = 0;
+    for (int kvi = 0; kvi < 2 && P.vw; ++kvi)
+        for (int l = layer_begin; l < layer_end && P.vw; ++l)
+            if ((reinterpret_cast<uintptr_t>(P.pt.p[kvi * P.L + l]) & 15) != 0) P.vw = 0;
+    size_t smem = (size_t)P.hb * P.bs * P.pitch;
+    if (smem > 200 * 1024) P.vw = 0;
+    if (P.vw == 0) smem = 0;
+    const int64_t units = n_groups * 2 * P.nl * P.nhb;
+    int dev = 0, sms = 0;
+    B2_CHECK_CUDA(cudaGetDevice(&dev));
+    B2_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    int64_t blocks = std::min<int64_t>(units, (int64_t)sms * 8 * 4);
+    if (blocks < 1) blocks = 1;
+    int rc;
+    if (table != nullptr) {
+        if (es == 2) rc = launch_split_kernel<uint16_t, true>(pack, (unsigned)blocks, smem, P, stream);
+        else rc = launch_split_kernel<uint8_t, true>(pack, (unsigned)blocks, smem, P, stream);
+    } else {
+        if (es == 2) rc = launch_split_kernel<uint16_t, false>(pack, (unsigned)blocks, smem, P, stream);
+        else rc = launch_split_kernel<uint8_t, false>(pack, (unsigned)blocks, smem, P, stream);
+    }
+    if (rc) return rc;
+    B2_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
 // layer_end < 0: every layer.  table != NULL: chunk j starts at table[j] (chunks and chunk_stride_bytes unused).
 static int launch_pack(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
                        int32_t last_chunk_tokens, int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
                        void* chunks, int64_t chunk_stride_bytes, void* const* table, cudaStream_t stream) {
     PackParams P;
     B2_REQUIRE(kv != nullptr && kv->L > 0 && 2 * kv->L <= B200KV_MAX_PLANES, "bad kv descriptor");
+    if (kv_split(kv))
+        return launch_split(pack, kv, tok_begin, n_chunks, chunk_tokens, last_chunk_tokens, hf_layout, layer_begin,
+                            layer_end, chunks, chunk_stride_bytes, table, stream);
     if (layer_end < 0) layer_end = kv->L;
     B2_REQUIRE(0 <= layer_begin && layer_begin < layer_end && layer_end <= kv->L, "bad layer range");
     float bins[B200KV_MAX_PLANES];

@@ -61,6 +61,11 @@ class LMCHybridBackend(LMCBackendInterface):
         f, g = getattr(self.local_store, "supports_kv_view", None), getattr(self.remote_store, "supports_kv_view", None)
         return bool(f and f() and g and g())
 
+    def supports_split_view(self) -> bool:
+        """both parts take a split paged view as it is; otherwise the engine stages it once for both"""
+        f, g = getattr(self.local_store, "supports_split_view", None), getattr(self.remote_store, "supports_split_view", None)
+        return bool(f and f() and g and g())
+
     def put_kv_chunks(self, keys: List[CacheEngineKey], view, tok_begin: int, chunk_size: int, blocking: bool = True) -> int:
         n = self.local_store.put_kv_chunks(keys, view, tok_begin, chunk_size, blocking=True)
         self.remote_store.put_kv_chunks(keys, view, tok_begin, chunk_size, blocking=blocking)

@@ -292,6 +292,10 @@ class LMCLocalBackend(LMCBackendInterface):
     def supports_kv_view(self) -> bool:
         return True
 
+    def supports_split_view(self) -> bool:
+        """a split paged view (PagedAttention's layout) is read and written by the mover alone: taken as it is"""
+        return True
+
     def peek_geometry(self, key, fmt: str = "vllm"):
         """(L, H, D, dtype) of a stored chunk blob, from its shape (no copy): [L,2,t,H,D] (vllm) / [L,2,H,t,D] (hf); for
         a latent engine [L,t,D] (H = 1).  None for a blob of the other kind."""
