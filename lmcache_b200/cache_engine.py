@@ -82,6 +82,9 @@ class _HashRun:
         with _HashRun._pool_lock:
             _HashRun._epoch = (_HashRun._epoch % 0x7fffffff) + 1
             self.epoch = _HashRun._epoch
+            # a pooled buffer whose own finaliser ran after it was pooled (both were garbage of one reference cycle,
+            # such as an error's traceback that reaches this run) is closed: drop it, never hand it out
+            _HashRun._pool = [b for b in _HashRun._pool if b.host_ptr]
             fit = [b for b in _HashRun._pool if b.nbytes >= need]
             if fit:
                 self.buf = min(fit, key=lambda b: b.nbytes)
@@ -195,11 +198,12 @@ class LayerwiseStore:
     """What store_layerwise / store_paged_layerwise return: a store whose KV is handed over one layer at a time, as
     vLLM's KV connector does with save_kv_layer after each attention layer and wait_for_save at the end of the forward
     pass.  save_layer(l, stream) says that layer l is written in `stream` order; finish(stream) completes the store.
-    Neither waits on the host, except finish() on a lossless disk tier, which returns once the files are written, as
-    the store() it replaced did (the tier's layerwise_store_blocking).  On the compressed host and disk tiers each layer
-    is encoded on a side stream as soon as it is saved (pipeline.LayerwiseEncode), and on the raw cpu and cuda tiers
-    packed into its chunk blobs (local_backend.RawLayerwiseStore); elsewhere save_layer only records the layer and
-    finish() runs the ordinary store.  A handle dropped without finish() stores nothing and gives its device scratch back."""
+    Neither waits on the host, except finish() on a lossless disk tier, which returns once the files are written, and on
+    the remote and hybrid tiers, which returns once the server holds the containers, as the store() it replaced did (the
+    tier's layerwise_store_blocking).  On the compressed host and disk tiers and the remote tier each layer is encoded
+    on a side stream as soon as it is saved (pipeline.LayerwiseEncode), and on the raw cpu and cuda tiers packed into
+    its chunk blobs (local_backend.RawLayerwiseStore); a hybrid tier does both parts so (once, when they keep the same
+    containers); elsewhere save_layer only records the layer and finish() runs the ordinary store.  A handle dropped without finish() stores nothing and gives its device scratch back."""
 
     def __init__(self, num_layers: int, enc, on_finish: Callable):
         self.num_layers = num_layers
@@ -822,10 +826,11 @@ class LMCacheEngine:
 
     # ------------------------------------------------------------------ layer-wise store
     def _layerwise_store_ok(self, dtype: torch.dtype) -> bool:
-        """Can this store be encoded layer by layer?  The compressed host and disk tiers can, for the KV their codec
-        encodes (CacheGen: 16-bit; lossless: 16-bit and one-byte) and chunks of at most the tier's layerwise_max_tokens
-        (256 for CacheGen's version-3 containers, 4096 for lossless ones); the raw cpu and cuda tiers can for every
-        chunk size and every KV the mover moves; remote and hybrid tiers cannot."""
+        """Can this store be encoded layer by layer?  The compressed host and disk tiers and the lm:// remote tier with
+        the cachegen or lossless serde can, for the KV their codec encodes (CacheGen: 16-bit; lossless: 16-bit and
+        one-byte) and chunks of at most the tier's layerwise_max_tokens (256 for CacheGen's version-3 containers, 4096
+        for lossless ones); the raw cpu and cuda tiers can for every chunk size and every KV the mover moves; a hybrid
+        tier can when both its parts can.  A remote tier with the torch serde cannot (layerwise_max_tokens 0)."""
         return (getattr(self.engine_, "begin_layerwise_store", None) is not None and self._fast_path() and
                 self.chunk_size <= self.engine_.layerwise_max_tokens and dtype in NATIVE_DTYPES)
 
@@ -860,7 +865,10 @@ class LMCacheEngine:
         """store_paged(), with the KV handed over one layer at a time: the caches may still be unwritten when this is
         called; call save_layer(l) once layer l is written and finish() after the last layer (LayerwiseStore).  The keys
         stored, the containers and the eviction touches are those of store_paged(tokens, kv_caches, slot_mapping,
-        skip_existing)."""
+        skip_existing).  Layer by layer on the compressed host and disk tiers, the raw cpu and cuda tiers, the lm://
+        remote tier with the cachegen or lossless serde, and hybrids of these (one encode for both parts when they keep
+        the same containers); on the remote and hybrid tiers finish() returns once the server holds every chunk.  Every
+        other case, and a split (PagedAttention) cache on a container tier, runs store_paged() at finish()."""
         self._check_paged_args(tokens, slot_mapping, kv_caches)
 
         def fallback(stream, enc):

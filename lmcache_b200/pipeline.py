@@ -51,6 +51,7 @@ class WaveSlot:
         self.sizes = PinnedBuffer(max(64, 8 * wave))
         self.planes = PinnedBuffer(8 * (N.MAX_PLANES + 1) * wave)      # b200kv_plane_offsets_device rows, one per chunk
         self.ticket: Optional[EncodeTicket] = None
+        self.refs = 1                       # sinks that still land this wave (EncodeRing.hold / release)
 
     def close(self):
         self.sizes.close()
@@ -70,6 +71,7 @@ class EncodeRing:
         self.stride = codec.out_stride(L, H, D, chunk_size, latent)
         n = slots or wave_slots_default()
         self._free: "queue.Queue[WaveSlot]" = queue.Queue()
+        self._lock = threading.Lock()
         self._all: List[WaveSlot] = []
         for _ in range(n):
             s = WaveSlot(self.stride * self.wave, self.wave, device)
@@ -83,9 +85,20 @@ class EncodeRing:
         return sum(s.dev.numel() for s in self._all)
 
     def acquire(self) -> WaveSlot:
-        return self._free.get()
+        slot = self._free.get()
+        slot.refs = 1
+        return slot
+
+    def hold(self, slot: WaveSlot) -> None:
+        """one more release() is needed before `slot` is free again (a wave that two sinks land)"""
+        with self._lock:
+            slot.refs += 1
 
     def release(self, slot: WaveSlot) -> None:
+        with self._lock:
+            slot.refs -= 1
+            if slot.refs > 0:
+                return
         slot.ticket = None
         self._free.put(slot)
 
@@ -126,6 +139,18 @@ class StoreJob:
             raise self.error
 
 
+class SharedWaves:
+    """The second sink of an encode that two tiers land (EncodePipeline.submit's `shared`): `pipe`, the other tier's
+    EncodePipeline, whose worker hands every wave to its own sink; `items`, that sink's per-chunk payload; `job`, set by
+    submit, which completes when that sink has taken every wave.  The first pipeline's worker passes each wave on to
+    `pipe` once its own sink is done with it, so the first tier holds a wave's chunks before the second one does, and
+    the two sinks never use the slot at the same time."""
+
+    def __init__(self, pipe: "EncodePipeline", items: Sequence):
+        self.pipe, self.items = pipe, items
+        self.job: Optional[StoreJob] = None
+
+
 class EncodePipeline:
     """encode waves on the caller's stream; a worker thread hands every finished wave to `sink`.
 
@@ -155,19 +180,24 @@ class EncodePipeline:
         """Hand a finished layer-wise encode (LayerwiseEncode.finish has been called) to the worker: it lands the
         containers that fit the arena, as one wave, in submission order with the other stores."""
         job = StoreJob(1)
-        self._q.put((enc.pool, enc.slot, 0, list(items), job))
+        self._q.put((enc.pool, enc.slot, 0, list(items), job, None))
         return job
 
     def submit(self, view: KvView, tok_begin: int, chunk_size: int, items: Sequence,
-               stream: Optional[torch.cuda.Stream] = None) -> StoreJob:
+               stream: Optional[torch.cuda.Stream] = None, shared: Optional["SharedWaves"] = None) -> StoreJob:
         """Enqueue the encode of tokens [tok_begin, T) of `view`, len(items) chunks, in waves.  Returns once every wave
-        is enqueued on `stream` (default: the current stream); the job completes when the sink has taken them all."""
+        is enqueued on `stream` (default: the current stream); the job completes when the sink has taken them all.
+        shared: another pipeline whose sink lands every wave too, from the same slot, with its own items, after this
+        pipeline's sink (a hybrid tier whose parts keep the same containers); shared.job completes when that sink has
+        taken them all, and a slot is free again only after both sinks."""
         n_tok = view.ntokens - tok_begin
         n_chunks = len(items)
         assert n_chunks == (n_tok + chunk_size - 1) // chunk_size and n_chunks > 0
         ring = self._ring_for(view, chunk_size)
         W = ring.wave
         job = StoreJob((n_chunks + W - 1) // W)
+        if shared is not None:
+            shared.job = StoreJob((n_chunks + W - 1) // W)
         with torch.cuda.device(view.device):
             for c0 in range(0, n_chunks, W):
                 k = min(W, n_chunks - c0)
@@ -179,8 +209,14 @@ class EncodePipeline:
                 except BaseException as e:       # noqa: BLE001 -- give the slot back, fail the job, re-raise
                     ring.release(slot)
                     job.wave_done(e)
+                    if shared is not None:
+                        shared.job.wave_done(e)
                     raise
-                self._q.put((ring, slot, c0, list(items[c0:c0 + k]), job))
+                then = None
+                if shared is not None:
+                    ring.hold(slot)             # the second sink's reference, taken before this worker can release it
+                    then = (shared.pipe, list(shared.items[c0:c0 + k]), shared.job)
+                self._q.put((ring, slot, c0, list(items[c0:c0 + k]), job, then))
         return job
 
     # ------------------------------------------------------------------ worker side
@@ -190,7 +226,7 @@ class EncodePipeline:
             item = self._q.get()
             if item is None:
                 return
-            ring, slot, c0, items, job = item
+            ring, slot, c0, items, job, then = item
             err = None
             try:
                 batch = slot.ticket.wait()          # host wait on this wave's kernels -- on the worker thread only
@@ -198,6 +234,9 @@ class EncodePipeline:
             except BaseException as e:              # noqa: BLE001 -- a failed background store is a miss later
                 err = e
             finally:
+                if then is not None:                # SharedWaves: the second sink lands the wave after this one
+                    pipe, items2, job2 = then
+                    pipe._q.put((ring, slot, c0, items2, job2, None))
                 ring.release(slot)
                 job.wave_done(err)
 
@@ -371,6 +410,7 @@ class SegmentSlot:
         self.seg = PinnedBuffer(max(64, 8 * row * P * n_chunks))
         self.arena_bytes = arena_bytes
         self.ticket = None
+        self.refs = 1                       # sinks that still land this slot (SegmentPool.hold / release)
         self.layouts: tuple = ()            # (SegmentLayout of a full chunk, of the last chunk)
         self.fixed_stride = 0
         self.coder = N.CODER_RANS_COMPACT   # the coder that names the containers' version (N.CODER_LATENT: 4)
@@ -390,7 +430,8 @@ class SegmentPool:
     """Reusable SegmentSlots for the layer-wise stores of one tier and device, and the stream they encode on.  A slot
     is reused by the next store that fits it; at most `keep` idle slots are kept.  Every kernel that touches a slot runs
     on `stream` and its tensors are allocated there, so reuse and release are ordered by the stream; the worker hands a
-    slot back only after its device->host copies have completed."""
+    slot back only after its device->host copies have completed.  A slot that several sinks land (a hybrid tier whose two
+    parts keep the same containers) takes one hold() per extra sink and goes back with the last release()."""
 
     def __init__(self, device, keep: int = 2):
         self.device = torch.device(device)
@@ -405,13 +446,22 @@ class SegmentPool:
             for s in self._free:
                 if s.holds(arena_bytes, fixed_bytes, ws_bytes, n_chunks, P, row):
                     self._free.remove(s)
+                    s.refs = 1
                     return s
         with torch.cuda.device(self.device), torch.cuda.stream(self.stream):
             return SegmentSlot(arena_bytes, fixed_bytes, ws_bytes, n_chunks, P, self.device, row)
 
-    def release(self, slot: SegmentSlot) -> None:
-        slot.ticket = None
+    def hold(self, slot: SegmentSlot) -> None:
+        """one more release() is needed before `slot` goes back to the pool"""
         with self._lock:
+            slot.refs += 1
+
+    def release(self, slot: SegmentSlot) -> None:
+        with self._lock:
+            slot.refs -= 1
+            if slot.refs > 0:
+                return
+            slot.ticket = None
             self._free.append(slot)
             drop = self._free[:-self.keep] if len(self._free) > self.keep else []
             self._free = self._free[len(drop):]
@@ -476,11 +526,10 @@ class LayerwiseEncode:
             self.abandon()
             raise
 
-    def encode_layer(self, layer: int, stream: torch.cuda.Stream) -> None:
+    def encode_layer(self, layer: int, stream: torch.cuda.Stream, ready: Optional[torch.cuda.Event] = None) -> None:
+        """`ready`: an event already recorded on `stream` after layer `layer` was written (FanOutEncode's)"""
         with torch.cuda.device(self.pool.device):
-            ev = torch.cuda.Event()
-            ev.record(stream)
-            self.pool.stream.wait_event(ev)
+            self.pool.stream.wait_event(ready or _recorded(stream))
             self.codec.encode_layers(self.plan, layer, layer + 1, self.pool.stream)
 
     def finish(self) -> torch.cuda.Event:
@@ -498,6 +547,94 @@ class LayerwiseEncode:
         if self.slot is not None:
             slot, self.slot, self.view = self.slot, None, None
             self.pool.release(slot)
+
+
+def _recorded(stream: torch.cuda.Stream) -> torch.cuda.Event:
+    ev = torch.cuda.Event()
+    ev.record(stream)
+    return ev
+
+
+# the containers a layer-wise encode writes: versions 3 and 4 (CacheGen), 5 and 6 (lossless)
+LAYERWISE_CODERS = (N.CODER_RANS_COMPACT, N.CODER_LATENT, N.CODER_LOSSLESS, N.CODER_LOSSLESS_LATENT)
+
+
+def layerwise_encodes(codec, chunk_size: int, latent: bool) -> bool:
+    """Does a layer-wise encode write `codec`'s containers for chunks of `chunk_size`?  Not for CacheGen chunks of more
+    than 256 tokens, the 'rans' and 'ac' coders, or lossless chunks of more than 4096 tokens."""
+    try:
+        return codec.coder_for(chunk_size, latent) in LAYERWISE_CODERS
+    except ValueError:
+        return False
+
+
+def same_containers(a, b, chunk_size: int, latent: bool) -> bool:
+    """Do codecs `a` and `b` write byte-identical containers for chunks of `chunk_size` (a latent KV if `latent`)?  Yes
+    when both are of one family and write the same coder for this chunk size, and CacheGen codecs code with the same key
+    and value bins (the same cachegen_config, or the same model row).  None (a tier without containers) is never the
+    same."""
+    if a is None or b is None or type(a) is not type(b):
+        return False
+    try:
+        if a.coder_for(chunk_size, latent) != b.coder_for(chunk_size, latent):
+            return False
+    except ValueError:
+        return False
+    ca, cb = getattr(a, "config", None), getattr(b, "config", None)
+    if ca is None or cb is None:
+        return ca is cb
+    return ca.key_bins_list() == cb.key_bins_list() and ca.value_bins_list() == cb.value_bins_list()
+
+
+def segment_pool_for(pool: Optional[SegmentPool], device) -> SegmentPool:
+    """`pool` when it serves `device`; otherwise `pool` is closed and a new one made"""
+    if pool is None or pool.device != torch.device(device):
+        if pool is not None:
+            pool.close()
+        pool = SegmentPool(device)
+    return pool
+
+
+class NoEncode:
+    """A layer-wise store that encodes and stores nothing: the handle of a tier that takes no stores from this engine
+    (an MLA engine's remote tier on ranks other than 0).  No GPU work is enqueued."""
+
+    def encode_layer(self, layer: int, stream: torch.cuda.Stream, ready: Optional[torch.cuda.Event] = None) -> None:
+        pass
+
+    def finish(self) -> torch.cuda.Event:
+        """an event that was never recorded: waiting on it waits for nothing"""
+        return torch.cuda.Event()
+
+    def abandon(self) -> None:
+        pass
+
+
+class FanOutEncode:
+    """One layer-wise store into two tiers that do not keep the same containers (a hybrid tier): `parts` are the
+    tiers' own handles (LayerwiseEncode, local_backend.RawLayerwiseStore, NoEncode), in the hybrid's order (local,
+    remote).  encode_layer records one event on the caller's stream and every part enqueues its own launches behind
+    it; finish() returns an event after every part's; abandon() drops every part."""
+
+    def __init__(self, parts: Sequence, stream: torch.cuda.Stream):
+        self.parts = list(parts)
+        self._stream = stream           # where the join of the parts' finish events is recorded
+
+    def encode_layer(self, layer: int, stream: torch.cuda.Stream, ready: Optional[torch.cuda.Event] = None) -> None:
+        ready = ready or _recorded(stream)
+        for p in self.parts:
+            p.encode_layer(layer, stream, ready=ready)
+
+    def finish(self) -> torch.cuda.Event:
+        evs = [p.finish() for p in self.parts]
+        with torch.cuda.device(self._stream.device):
+            for ev in evs:
+                self._stream.wait_event(ev)
+            return _recorded(self._stream)
+
+    def abandon(self) -> None:
+        for p in self.parts:
+            p.abandon()
 
 
 def segment_copy_ranges(seg: np.ndarray, layouts: Sequence[SegmentLayout]):

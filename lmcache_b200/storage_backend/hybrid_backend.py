@@ -3,9 +3,10 @@ both, reads are served locally when possible and fall through to the remote tier
 The reference prefetches the whole remote store into the local tier at start-up (hybrid_backend.py:26-62: list() + one
 get/put per key -- a full deserialise of everything the server holds); here the local tier fills on demand.
 
-Both tiers keep their engine fast paths: a store hands the caller's KV view to each tier once, a retrieve asks the local
-tier for the longest prefix it holds and the remote tier for the rest, all decoded / copied straight into the one
-destination blob."""
+Both tiers keep their engine fast paths: a store hands the caller's KV view to each tier once -- or, when both keep the
+same containers (pipeline.same_containers), encodes it once and lands every container in both -- and a retrieve asks
+the local tier for the longest prefix it holds and the remote tier for the rest, all decoded / copied straight into the
+one destination blob."""
 from typing import Iterable, List, Optional, Tuple
 
 import torch
@@ -33,6 +34,7 @@ class LMCHybridBackend(LMCBackendInterface):
         # process's own, takes every rank's
         self.local_store = CreateStorageBackend(local_cfg, metadata)
         self.remote_store = CreateStorageBackend(remote_cfg, metadata)
+        self._join: Optional[torch.cuda.Stream] = None     # where a FanOutEncode joins its parts' finish events
 
     def contains(self, key: CacheEngineKey) -> bool:
         return self.local_store.contains(key) or self.remote_store.contains(key)
@@ -66,10 +68,88 @@ class LMCHybridBackend(LMCBackendInterface):
         f, g = getattr(self.local_store, "supports_split_view", None), getattr(self.remote_store, "supports_split_view", None)
         return bool(f and f() and g and g())
 
-    def put_kv_chunks(self, keys: List[CacheEngineKey], view, tok_begin: int, chunk_size: int, blocking: bool = True) -> int:
-        n = self.local_store.put_kv_chunks(keys, view, tok_begin, chunk_size, blocking=True)
-        self.remote_store.put_kv_chunks(keys, view, tok_begin, chunk_size, blocking=blocking)
+    def _shares_containers(self, chunk_size: int, view) -> bool:
+        """Do both parts keep the same containers for chunks of `chunk_size` of `view`'s kind (pipeline.same_containers
+        of the local tier's codec and the remote serializer's), so that one encode serves both?  The remote part must be on its
+        striped path: that path lands containers from a device slot."""
+        from lmcache_b200.pipeline import same_containers
+        remote = self.remote_store
+        striped = getattr(remote, "_striped", None)
+        if striped is None or not striped():
+            return False
+        return same_containers(getattr(self.local_store, "codec", None), getattr(remote.serializer, "codec", None),
+                               chunk_size, view.latent)
+
+    def put_kv_chunks(self, keys: List[CacheEngineKey], view, tok_begin: int, chunk_size: int, blocking: bool = True,
+                      encoded=None) -> int:
+        """The local tier's put (blocking), then the remote tier's.  When both keep the same containers, the chunks are
+        encoded once: on the caller's stream, wave by wave, each wave landed by both tiers' workers from the same device
+        slot (pipeline.SharedWaves); or, with `encoded`, one layer-wise encode whose slot both land.  `encoded` of two
+        tiers that do not (a pipeline.FanOutEncode) gives each tier its own part."""
+        from lmcache_b200.pipeline import FanOutEncode, SharedWaves
+        local, remote = self.local_store, self.remote_store
+        if isinstance(encoded, FanOutEncode):
+            try:
+                n = local.put_kv_chunks(keys, None, tok_begin, chunk_size, blocking=True, encoded=encoded.parts[0])
+            except BaseException:
+                encoded.parts[1].abandon()
+                raise
+            remote.put_kv_chunks(keys, None, tok_begin, chunk_size, blocking=blocking, encoded=encoded.parts[1])
+            return n
+        if encoded is not None:
+            # one slot, two sinks: the remote part's reference is taken before the local worker can release the slot
+            if not remote.puts:
+                return local.put_kv_chunks(keys, None, tok_begin, chunk_size, blocking=True, encoded=encoded)
+            encoded.pool.hold(encoded.slot)
+            try:
+                n = local.put_kv_chunks(keys, None, tok_begin, chunk_size, blocking=True, encoded=encoded)
+            except BaseException:
+                encoded.pool.release(encoded.slot)
+                raise
+            remote.put_kv_chunks(keys, None, tok_begin, chunk_size, blocking=blocking, encoded=encoded)
+            return n
+        if not (getattr(remote, "puts", False) and self._shares_containers(chunk_size, view)):
+            n = local.put_kv_chunks(keys, view, tok_begin, chunk_size, blocking=True)
+            remote.put_kv_chunks(keys, view, tok_begin, chunk_size, blocking=blocking)
+            return n
+        shared = SharedWaves(remote._pipeline(), keys)
+        n = local.put_kv_chunks(keys, view, tok_begin, chunk_size, blocking=True, shared=shared)
+        if blocking:
+            shared.job.wait()
+            remote.flush()
         return n
+
+    @property
+    def layerwise_store_blocking(self) -> bool:
+        """Yes: finish() returns once the server holds the containers (the remote part's guarantee), after the local
+        part has landed them."""
+        return True
+
+    def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int):
+        """A layer-wise store into both parts, or None when either part cannot take one (a torch-serde remote tier, a
+        chunk size over a part's limit): the engine then stores both at finish().  When both parts keep the same
+        containers it is one pipeline.LayerwiseEncode on the local tier's pool, whose slot put_kv_chunks lands into
+        both; otherwise a pipeline.FanOutEncode of the two parts' own handles."""
+        from lmcache_b200.pipeline import FanOutEncode
+        begins = [getattr(s, "begin_layerwise_store", None) for s in (self.local_store, self.remote_store)]
+        if None in begins:
+            return None
+        if self._shares_containers(chunk_size, view):
+            return begins[0](view, tok_begin, chunk_size)
+        local = begins[0](view, tok_begin, chunk_size)
+        if local is None:
+            return None
+        try:
+            remote = begins[1](view, tok_begin, chunk_size)
+        except BaseException:
+            local.abandon()
+            raise
+        if remote is None:
+            local.abandon()
+            return None
+        if self._join is None or self._join.device != view.device:
+            self._join = torch.cuda.Stream(device=view.device)
+        return FanOutEncode([local, remote], self._join)
 
     def get_kv_into(self, keys: List[CacheEngineKey], dst, dst_tok0: int, chunk_size: int) -> int:
         n = self.local_store.get_kv_into(keys, dst, dst_tok0, chunk_size)

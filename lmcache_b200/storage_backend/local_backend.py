@@ -145,10 +145,13 @@ class RawLayerwiseStore:
                 rows = np.stack([np.uint64(self.buf.data_ptr() + r * self.slot_bytes) + offs for r in range(LAYER_SLOTS)])
             self.table = _device_table(rows, view.device, self.ps)
 
-    def encode_layer(self, layer: int, stream: torch.cuda.Stream) -> None:
+    def encode_layer(self, layer: int, stream: torch.cuda.Stream, ready: Optional[torch.cuda.Event] = None) -> None:
+        """`ready`: an event already recorded on `stream` after layer `layer` was written (pipeline.FanOutEncode's)"""
         with torch.cuda.device(self.view.device):
-            ev = torch.cuda.Event()
-            ev.record(stream)
+            ev = ready
+            if ev is None:
+                ev = torch.cuda.Event()
+                ev.record(stream)
             self.ps.wait_event(ev)
             k, self.saves = self.saves, self.saves + 1
             if self.host is None:
@@ -808,17 +811,19 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
     def _new_store(self) -> _Store:
         return _Store(getattr(self._touched, "tick", None) if self.capacity is not None else None)
 
-    def _submit(self, view, tok_begin: int, chunk_size: int, entries, encoded):
-        return self._pipe.submit(view, tok_begin, chunk_size, entries) if encoded is None else \
+    def _submit(self, view, tok_begin: int, chunk_size: int, entries, encoded, shared=None):
+        return self._pipe.submit(view, tok_begin, chunk_size, entries, shared=shared) if encoded is None else \
             self._pipe.submit_encoded(encoded, entries)
 
-    def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True, encoded=None) -> int:
+    def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True, encoded=None,
+                      shared=None) -> int:
         # `keys` may be lazy (the engine's hash chain produces key i after keys 0..i-1): the encode waves
         # need no keys, so they are enqueued first; the entries are published as their keys arrive.  Readers wait on `ready`.
         # encoded: a finished pipeline.LayerwiseEncode of these chunks (store_layerwise), landed instead of encoding `view`
+        # shared: a pipeline.SharedWaves whose pipeline lands every encoded wave as well (LMCHybridBackend)
         store = self._new_store()
         entries = [_CEntry(store) for _ in range(len(keys))]
-        job = self._submit(view, tok_begin, chunk_size, entries, encoded)
+        job = self._submit(view, tok_begin, chunk_size, entries, encoded, shared)
         old = []
         for k, e in zip(keys, entries):
             with self.update_lock:
@@ -922,17 +927,10 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         """A pipeline.LayerwiseEncode of tokens [tok_begin, T) of `view` (whose KV may not be written yet), or None
         when this tier's containers for `chunk_size` are not ones a layer-wise encode writes: versions 3 and 4 (CacheGen,
         chunks of at most 256 tokens), versions 5 and 6 (lossless, at most 4096)."""
-        from lmcache_b200.pipeline import LayerwiseEncode, SegmentPool
-        try:
-            if self.codec.coder_for(chunk_size, view.latent) not in (N.CODER_RANS_COMPACT, N.CODER_LATENT,
-                                                                     N.CODER_LOSSLESS, N.CODER_LOSSLESS_LATENT):
-                return None
-        except ValueError:
+        from lmcache_b200.pipeline import LayerwiseEncode, layerwise_encodes, segment_pool_for
+        if not layerwise_encodes(self.codec, chunk_size, view.latent):
             return None
-        if self._segments is None or self._segments.device != view.device:
-            if self._segments is not None:
-                self._segments.close()
-            self._segments = SegmentPool(view.device)
+        self._segments = segment_pool_for(self._segments, view.device)
         return LayerwiseEncode(self.codec, self._segments, view, tok_begin, chunk_size)
 
     def _layerwise_uploader(self, device):
@@ -1267,7 +1265,8 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
             for e in entries:
                 e.ready.set()                             # readers see the entry only once its file is in place
 
-    def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True, encoded=None) -> int:
+    def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True, encoded=None,
+                      shared=None) -> int:
         store = self._new_store()
         entries = [_CEntry(store) for _ in keys]
         for k, e in zip(keys, entries):
@@ -1280,7 +1279,7 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
                     old.append(self.dict[e.path])
                 self.dict[e.path] = e                     # an overwritten chunk's file is replaced atomically by the rename
         # the parent's sink sets `ready` before the file exists: keep readers out until the file is written
-        job = self._submit(view, tok_begin, chunk_size, entries, encoded)
+        job = self._submit(view, tok_begin, chunk_size, entries, encoded, shared)
         self.touch(keys)
         for prev in old:      # an overwritten chunk's device copy is never served again (its sink checks `retired`)
             self._retire(prev)

@@ -202,6 +202,7 @@ class LMCRemoteBackend(LMCBackendInterface):
         self._conns_lock = threading.Lock()
         self._slab = None
         self._pipe = None
+        self._segments = None            # pipeline.SegmentPool, made by the first layer-wise store
         self._upload = None
         self._release = DeferredFree()   # fetched blocks that uploads may still read
         self._peek = None            # (key, HostContainer): the container peek_geometry fetched, reused by get_kv_into
@@ -345,20 +346,28 @@ class LMCRemoteBackend(LMCBackendInterface):
             self.connection.set(self._combine_key(key), bs)
             self.existing_keys.add(key)
 
+    def _pipeline(self):
+        if self._pipe is None:
+            from lmcache_b200.pipeline import EncodePipeline
+            self._pipe = EncodePipeline(self.serializer.codec, self._sink, name="b200kv-remote-store")
+        return self._pipe
+
     def put_kv_chunks(self, keys: List[CacheEngineKey], view, tok_begin: int, chunk_size: int,
-                      blocking: bool = True) -> int:
+                      blocking: bool = True, encoded=None) -> int:
         """Store tokens [tok_begin, T) of `view` as len(keys) chunks.  Striped path: every wave is encoded on the caller's
         stream before this returns (so a non-blocking store has consumed the caller's KV in stream order -- paged caches
         included -- like the reference's materialised chunk list, cache_engine.py:274-275); D2H and the sends happen on
-        the pipeline's worker.  Other serdes: one batched encode, then one set() per chunk.  A latent KV's rank other
-        than 0 stores nothing (returns 0)."""
+        the pipeline's worker.  encoded: a finished pipeline.LayerwiseEncode of these chunks (begin_layerwise_store),
+        whose containers are landed and sent instead of encoding `view`.  Other serdes: one batched encode, then one
+        set() per chunk.  A latent KV's rank other than 0 stores nothing (returns 0)."""
         if not self.puts:
             return 0
         if self._striped():
-            if self._pipe is None:
-                from lmcache_b200.pipeline import EncodePipeline
-                self._pipe = EncodePipeline(self.serializer.codec, self._sink, name="b200kv-remote-store")
-            job = self._pipe.submit(view, tok_begin, chunk_size, keys)      # keys may be lazy: a wave's are read when it is queued
+            pipe = self._pipeline()
+            if encoded is None:
+                job = pipe.submit(view, tok_begin, chunk_size, keys)   # keys may be lazy: a wave's are read when it is queued
+            else:
+                job = pipe.submit_encoded(encoded, keys)
             if blocking:
                 job.wait()
                 self.flush()
@@ -499,6 +508,28 @@ class LMCRemoteBackend(LMCBackendInterface):
         lossless); 0 for a serde without containers"""
         codec = getattr(self.deserializer, "codec", None)
         return getattr(codec, "layerwise_max_tokens", 0) if self._striped() else 0
+
+    # ---- layer-wise store
+    @property
+    def layerwise_store_blocking(self) -> bool:
+        """Yes: a layer-wise store's finish() returns only once the server holds every container (the pipeline's job,
+        then flush()), as the blocking store() it replaced did, so that another engine's retrieve that starts after
+        finish() finds the chunks."""
+        return True
+
+    def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int):
+        """A pipeline.LayerwiseEncode of tokens [tok_begin, T) of `view` (whose KV may not be written yet) on this tier's
+        own SegmentPool; put_kv_chunks(..., encoded=it) lands and sends its containers.  None off the striped path (a
+        serde without containers) and when the containers for `chunk_size` are not ones a layer-wise encode writes
+        (pipeline.layerwise_encodes).  A latent KV's rank other than 0 gets a pipeline.NoEncode: it stores nothing, so
+        nothing is encoded."""
+        from lmcache_b200.pipeline import LayerwiseEncode, NoEncode, layerwise_encodes, segment_pool_for
+        if not (self._striped() and layerwise_encodes(self.serializer.codec, chunk_size, view.latent)):
+            return None
+        if not self.puts:
+            return NoEncode()
+        self._segments = segment_pool_for(self._segments, view.device)
+        return LayerwiseEncode(self.serializer.codec, self._segments, view, tok_begin, chunk_size)
 
     def _count(self, **kw) -> None:
         with self._stats_lock:
@@ -685,6 +716,9 @@ class LMCRemoteBackend(LMCBackendInterface):
         if getattr(self, "_pipe", None) is not None:
             self._pipe.close()
             self._pipe = None
+        if getattr(self, "_segments", None) is not None:
+            self._segments.close()
+            self._segments = None
         if getattr(self, "_pool", None) is not None:
             self._pool.shutdown(wait=True)
             self._pool = None
