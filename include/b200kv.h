@@ -50,7 +50,7 @@ extern "C" {
                                     *    b200kv_lossless_encode_layers_finish (b200kv_lossless_encode_plan_t),
                                     *    b200kv_lm_open_begin / b200kv_lm_read_ranges / b200kv_lm_close_handles,
                                     *    b200kv_lm_server_num_handles, b200kv_pack_chunks_layers /
-                                    *    b200kv_unpack_chunks_layers.
+                                    *    b200kv_unpack_chunks_layers, b200kv_rope_table / b200kv_rope_shift.
                                     *    B200KV_MAX_PLANES went from 128 to 256 (models of up to 128 layers): the row
                                     *    width of b200kv_plane_offsets_device, B200KV_MAX_PLANES + 1, and the size of
                                     *    b200kv_encode_plan_t, 256 -> 512 words, changed with it; a caller takes them
@@ -585,6 +585,33 @@ int b200kv_pack_chunks_layers(const b200kv_kv_desc* src, int64_t tok_begin, int3
 int b200kv_unpack_chunks_layers(const void* const* chunk_ptrs, int32_t n_chunks, int32_t chunk_tokens,
                                 int32_t last_chunk_tokens, int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
                                 const b200kv_kv_desc* dst, int64_t tok_begin, void* stream);
+
+/*
+ * Rotary position shift of stored keys (non-prefix reuse: a segment cached at positions 0..n-1 served at positions
+ * s..s+n-1).  vLLM caches K after the rotary embedding, R(i)·k_i; at offset s attention needs R(s + i)·k_i =
+ * R(s)·(R(i)·k_i).  Added without changing anything that existed (b200kv_version() stays 4).
+ *
+ * b200kv_rope_table fills cos_sin (DEVICE float [n_seg][rotary_dim/2][2]) with (cos, sin) of shifts[s] * inv_freq[j]:
+ * shifts is a DEVICE int64 [n_seg], inv_freq a DEVICE float32 [rotary_dim/2] (any frequency-only rope scaling: plain
+ * theta, Llama-3's, YaRN's frequencies).  The angle is computed in fp64 and range-reduced before sincos, then rounded
+ * once to fp32.  < 0, nothing enqueued: NULL pointers, n_seg <= 0, an odd or non-positive rotary_dim.
+ *
+ * b200kv_rope_shift rotates in place, in one launch, channels [offset, offset + rotary_dim) of every head of the KEY
+ * planes (kv = 0; the one plane of a B200KV_KV_LATENT descriptor) of tokens [tok_begin, tok_begin + ntok) of the view,
+ * every layer.  Token tok_begin + i is rotated by table row seg_of_tok[i] (DEVICE int32 [ntok]); -1 leaves the row
+ * alone, neither read nor written.  style 0 (neox) pairs channels (d, d + rotary_dim/2), style 1 (gptj) (2d, 2d + 1);
+ * pair j turns by row (cos, sin)[j]: (a, b) <- (a cos - b sin, b cos + a sin), each element loaded, converted to fp32,
+ * rotated and rounded once back to its dtype.  V planes, channels outside the rotary range and other tokens are not
+ * touched.  Every layout a kv_desc carries: blobs (vllm, huggingface), tuples, latent views, slot-mapped rows and
+ * B200KV_KV_PAGED_SPLIT key blocks.  16-byte vectors where offset, rotary_dim, the strides and the planes allow it.
+ * < 0, nothing enqueued: a one-byte dtype (FP8 / U8: rotating would round values FP8 already rounded), an odd or
+ * non-positive rotary_dim, offset < 0 or offset + rotary_dim > D, a NULL cos_sin, a NULL seg_of_tok with ntok > 0, a
+ * style other than 0 and 1.  Table rows are not bounds-checked: seg_of_tok holds -1 or rows of cos_sin.
+ */
+int b200kv_rope_table(const int64_t* shifts, int32_t n_seg, const float* inv_freq, int32_t rotary_dim, float* cos_sin,
+                      void* stream);
+int b200kv_rope_shift(const b200kv_kv_desc* kv, int64_t tok_begin, int64_t ntok, const int32_t* seg_of_tok,
+                      const float* cos_sin, int32_t rotary_dim, int32_t offset, int32_t style, void* stream);
 
 /*
  * GPU <-> pinned-host mover.  Replaces LMCLocalBackend.put_blocking/put_nonblocking/get

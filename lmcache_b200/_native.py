@@ -160,6 +160,8 @@ SIGNATURES = {
                                           c_vp]),
     "b200kv_unpack_chunks_layers": (c_i32, [c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, ctypes.POINTER(KvDesc),
                                             c_i64, c_vp]),
+    "b200kv_rope_table": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_vp, c_vp]),
+    "b200kv_rope_shift": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i64, c_vp, c_vp, c_i32, c_i32, c_i32, c_vp]),
     "b200kv_pinned_alloc": (c_i32, [ctypes.POINTER(c_vp), c_i64]),
     "b200kv_pinned_free": (c_i32, [c_vp]),
     "b200kv_host_device_ptr": (c_i32, [c_vp, ctypes.POINTER(c_vp)]),

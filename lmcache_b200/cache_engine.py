@@ -25,6 +25,7 @@ from lmcache_b200.logging import init_logger
 from lmcache_b200.storage_backend import CreateStorageBackend
 from lmcache_b200.pipeline import HeadWindow, LayerwiseUpload, join_uploads
 from lmcache_b200.reshard import first_source_rank, source_shards
+from lmcache_b200.rope import RopeSpec, hash_input, plan_segments, rope_shift, seg_of_tok
 from lmcache_b200.utils import CacheEngineKey, KVCache, _lmcache_nvtx_annotate
 
 logger = init_logger(__name__)
@@ -898,6 +899,182 @@ class LMCacheEngine:
             return LayerwiseStore(len(kv_tensors_raw), None, fallback)
         return self._begin_layerwise(tokens, lambda: KvView.from_tuple(kv_tensors_raw, fmt), fmt, len(kv_tensors_raw),
                                      skip_existing, fallback)
+
+    # ------------------------------------------------------------------ non-prefix segments
+    @staticmethod
+    def _check_rope_dtype(dtype: torch.dtype) -> None:
+        if dtype not in (torch.bfloat16, torch.float16):
+            raise TypeError(f"segment retrieve rotates 16-bit keys only, not {dtype}: rotating an FP8 key would round it "
+                            f"a third time")
+
+    def _segment_hashes(self, tokens: torch.Tensor, plans) -> list:
+        """every segment's chunk digests, its tokens hashed as their own sequence: one hash-chain launch for all"""
+        toks, offs = hash_input(tokens, plans)
+        chain = sha256_prefix_chain_lazy(toks, self.chunk_size, offs)
+        return [chain[p.chunk_begin:p.chunk_begin + p.n_chunks] for p in plans]
+
+    def _segments_prologue(self, tokens: torch.Tensor, segments, rope: RopeSpec):
+        """the plan and the refusals every segment retrieve makes before it fetches anything"""
+        assert len(tokens.shape) == 1, f"Invalid shape of tokens: {tokens.shape}"
+        if not isinstance(rope, RopeSpec):
+            raise TypeError(f"rope must be a RopeSpec, got {type(rope).__name__}")
+        plans = plan_segments(len(tokens), segments, self.chunk_size)
+        md = str(self.metadata.dtype).lower()
+        if any(s in md for s in ("fp8", "float8", "uint8")):
+            raise TypeError(f"segment retrieve rotates 16-bit keys only; this engine's KV dtype is {self.metadata.dtype}")
+        return plans
+
+    def _rotate(self, view: KvView, written, rope: RopeSpec) -> None:
+        """one rope shift of the written key rows of every segment that does not start at token 0"""
+        sot, lo, hi, shifts = seg_of_tok(view.ntokens, written)
+        if hi > lo:
+            seg = torch.tensor(sot, dtype=torch.int32).to(view.device)
+            sh = torch.tensor(shifts, dtype=torch.int64).to(view.device)
+            rope_shift(view, lo, seg, sh, rope)
+
+    def _segments_blob(self, tokens, plans, hashes, fmt: str, rope: Optional[RopeSpec] = None):
+        """Every segment's longest stored prefix of chunks in one zeroed blob of the request's T tokens, each at its
+        start (unrotated).  Returns (blob or None when nothing was found, [(plan, tokens written)]).  With `rope`, the
+        geometry's dtype and D are checked against it once known, before any chunk is written."""
+        T, cs = len(tokens), self.chunk_size
+        tdim = KvView.token_dim(fmt, self._mla)
+        dev = torch.device("cuda", torch.cuda.current_device())
+        written, blob = [], None
+        fast = self._fast_path()
+        if fast:
+            geom = self._kv_geometry()
+            peek = getattr(self.engine_, "peek_geometry", None)
+            for hs in hashes:
+                if geom is not None:
+                    break
+                key0 = self._make_key(hs[0], fmt)
+                if peek is not None:
+                    geom = peek(key0, fmt)
+                else:
+                    first = self.engine_.get(key0)
+                    if first is not None and first.dim() == (3 if self._mla else 5):
+                        geom = KvView.blob_geometry(first, fmt)
+            if geom is not None:
+                self._geom = geom
+                L, H, D, dtype = geom
+                od = getattr(self.engine_, "out_dtype", None) or \
+                    getattr(getattr(self.engine_, "deserializer", None), "out_dtype", None)
+                if od is not None and od() is not None:
+                    dtype = od()
+                self._check_rope_dtype(dtype)
+                if rope is not None:
+                    rope.check(D)
+                blob = torch.zeros(KvView.blob_shape(fmt, L, H, D, T, self._mla), dtype=dtype, device=dev)
+        dst = None if blob is None else KvView.from_blob(blob, fmt)
+        for p, hs in zip(plans, hashes):
+            n_tok = 0
+            if fast and blob is not None:
+                own = self.engine_.get_kv_into(self._keys_of(hs, fmt), dst, p.start, cs)
+                self._touch(hs[:own], fmt)
+                n_tok = min(own * cs, p.end - p.start)
+            elif not fast:
+                chunks = []
+                for c in self.engine_.batched_get(self._make_key(h, fmt) for h in hs):
+                    if c is None or c.dim() != (3 if self._mla else 5):    # the other kind's blob is a miss
+                        break
+                    chunks.append(c)
+                self._touch(hs[:len(chunks)], fmt)
+                if chunks and blob is None:
+                    L, H, D, dtype = KvView.blob_geometry(chunks[0], fmt)
+                    self._check_rope_dtype(dtype)
+                    if rope is not None:
+                        rope.check(D)
+                    blob = torch.zeros(KvView.blob_shape(fmt, L, H, D, T, self._mla), dtype=dtype, device=dev)
+                for k, c in enumerate(chunks):
+                    t = c.shape[tdim]
+                    blob.narrow(tdim, p.start + k * cs, t).copy_(c)
+                    n_tok += t
+            written.append((p, n_tok))
+        return blob, written
+
+    @_lmcache_nvtx_annotate
+    @torch.no_grad()
+    def retrieve_segments(self, tokens: torch.Tensor, segments, rope: RopeSpec) -> Tuple[KVCache, torch.Tensor]:
+        """Non-prefix retrieve (a RAG prompt's documents, seen before as prompts of their own, at new positions).
+        segments: (start, end) token ranges of `tokens`, non-overlapping, in any order.  Each segment gets its longest
+        stored prefix of chunks, keyed by the hash chain of its own tokens (what a store of tokens[start:end] alone
+        stored), at tokens start... of the result, its keys turned by `start` positions (rope).  Returns (kv, ret_mask):
+        kv is retrieve()'s per-layer views of one [L, 2, T, H, D] blob (an MLA engine: [L, T, D]) in which every token
+        not retrieved is zero, or () when no segment hits; ret_mask marks exactly the tokens written.  One segment
+        (0, T) gives retrieve(tokens)'s rows and ret_mask.  TypeError for FP8 KV, ValueError for empty, overlapping or
+        out-of-range segments and for a rotary range that does not fit a key head, all before anything is fetched.
+        reshard_world_sizes is not consulted."""
+        fmt = self.metadata.fmt
+        if fmt not in ("vllm", "huggingface"):
+            raise ValueError(f"Invalid format: {fmt}")
+        plans = self._segments_prologue(tokens, segments, rope)
+        geom = self._kv_geometry()
+        if geom is not None:
+            self._check_rope_dtype(geom[3])
+            rope.check(geom[2])
+        blob, written = self._segments_blob(tokens, plans, self._segment_hashes(tokens, plans), fmt, rope)
+        ret_mask = torch.zeros(len(tokens), dtype=torch.bool)
+        if blob is None:
+            return (), ret_mask
+        for p, n in written:
+            ret_mask[p.start:p.start + n] = True
+        self._rotate(KvView.from_blob(blob, fmt), written, rope)
+        return self._blob_to_tuple_kv(blob), ret_mask
+
+    @_lmcache_nvtx_annotate
+    @torch.no_grad()
+    def retrieve_paged_segments(self, tokens: torch.Tensor, kv_caches, slot_mapping: torch.Tensor, segments,
+                                rope: RopeSpec) -> torch.Tensor:
+        """retrieve_segments straight into a paged KV cache (any layout retrieve_paged takes): each segment's stored
+        chunks are written to rows slot_mapping[start...], through the fetch step of retrieve_paged on every tier, then
+        one rope shift turns the written key rows of every segment by its start (a segment at 0 is not rotated).
+        Returns ret_mask, marking exactly the tokens written; every other row is untouched.  One segment (0, T) gives
+        retrieve_paged(tokens, kv_caches, slot_mapping)'s ret_mask and rows bit for bit.  An MLA engine takes
+        RopeSpec(64, inv_freq, "gptj", offset=512): only the decoupled RoPE channels of its latent turn."""
+        self._check_paged_args(tokens, slot_mapping)
+        self._check_kind(kv_caches, "kv_caches")
+        plans = self._segments_prologue(tokens, segments, rope)
+        first = self._first(kv_caches)
+        self._check_rope_dtype(first.dtype)
+        rope.check(first.shape[-1] if self._mla else paged_layout(*kv_caches[0]).D)
+        dev, cs = first.device, self.chunk_size
+        slots = slot_mapping.to(dev)
+        hashes = self._segment_hashes(tokens, plans)
+        if not self._fast_path():
+            # the tier hands out chunk blobs: assemble them, then scatter each segment's run as retrieve_paged does
+            blob, written = self._segments_blob(tokens, plans, hashes, "vllm")
+            for p, n in written:
+                if n == 0:
+                    continue
+                if self._mla:
+                    idx = slots[p.start:p.start + n]
+                    for l, c in enumerate(self._flat_paged(kv_caches)):
+                        c[idx] = blob[l, p.start:p.start + n].to(c.dtype)
+                else:
+                    KvView.from_paged(kv_caches, slots[p.start:p.start + n]).unpack_blob(
+                        blob[:, :, p.start:p.start + n].to(first.dtype), 0)
+        else:
+            stage = self._stages_split(kv_caches)
+            view = KvView.from_paged(kv_caches, slots)
+            written = []
+            for p, hs in zip(plans, hashes):
+                dst, tok0 = view, p.start
+                if stage:
+                    # decoded into a blob of the segment, then only the retrieved tokens unpacked into the cache
+                    dst = KvView.from_blob(torch.empty(KvView.blob_shape("vllm", view.L, view.H, view.D, p.end - p.start),
+                                                       dtype=view.dtype, device=dev), "vllm")
+                    tok0 = 0
+                own = self.engine_.get_kv_into(self._keys_of(hs, "vllm"), dst, tok0, cs)
+                self._touch(hs[:own], "vllm")
+                n = min(own * cs, p.end - p.start)
+                if dst is not view and n:
+                    view.unpack_blob(dst.blob.narrow(2, 0, n), p.start)
+                written.append((p, n))
+        ret_mask = torch.zeros(len(tokens), dtype=torch.bool)
+        for p, n in written:
+            ret_mask[p.start:p.start + n] = True
+        self._rotate(KvView.from_paged(kv_caches, slots), written, rope)
+        return ret_mask
 
     def close(self):
         self.engine_.close()
