@@ -612,6 +612,20 @@ int b200kv_rope_table(const int64_t* shifts, int32_t n_seg, const float* inv_fre
                       void* stream);
 int b200kv_rope_shift(const b200kv_kv_desc* kv, int64_t tok_begin, int64_t ntok, const int32_t* seg_of_tok,
                       const float* cos_sin, int32_t rotary_dim, int32_t offset, int32_t style, void* stream);
+/* b200kv_pack_chunks with the keys turned on the way (a segment of a longer prompt stored as if prefilled alone: its
+ * keys turned by -start): the same descriptors (blobs, tuples, latent views, slot-mapped and block-strided rows,
+ * B200KV_KV_PAGED_SPLIT), chunk layouts and destinations (device or mapped pinned memory) as b200kv_pack_chunks, in one
+ * launch.  Call token tok_begin + i has channels [offset, offset + rotary_dim) of its key planes (kv = 0; the plane of a
+ * B200KV_KV_LATENT descriptor) turned by row seg_of_tok[i] (DEVICE int32, one per token packed) of cos_sin, with
+ * b200kv_rope_shift's pairing and arithmetic; -1, V planes and every other channel are copied bit for bit.  The result
+ * is bit-identical to b200kv_pack_chunks followed by b200kv_rope_shift of the packed rows; the source is only read.
+ * < 0, nothing enqueued: what b200kv_rope_shift refuses (one-byte dtypes, an odd or non-positive rotary_dim, offset < 0
+ * or offset + rotary_dim > D, NULL cos_sin or seg_of_tok, a style other than 0 and 1) and what b200kv_pack_chunks
+ * refuses.  Added without changing anything that existed (b200kv_version() stays 4). */
+int b200kv_pack_chunks_rope(const b200kv_kv_desc* src, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
+                            int32_t last_chunk_tokens, int32_t hf_layout, void* chunks, int64_t chunk_stride_bytes,
+                            const int32_t* seg_of_tok, const float* cos_sin, int32_t rotary_dim, int32_t offset,
+                            int32_t style, void* stream);
 
 /*
  * GPU <-> pinned-host mover.  Replaces LMCLocalBackend.put_blocking/put_nonblocking/get

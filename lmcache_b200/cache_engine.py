@@ -25,7 +25,8 @@ from lmcache_b200.logging import init_logger
 from lmcache_b200.storage_backend import CreateStorageBackend
 from lmcache_b200.pipeline import HeadWindow, LayerwiseUpload, join_uploads
 from lmcache_b200.reshard import first_source_rank, source_shards
-from lmcache_b200.rope import RopeSpec, hash_input, plan_segments, rope_shift, seg_of_tok
+from lmcache_b200.rope import (RopeSpec, derived_digest, hash_input, pack_rope, plan_segment_store, plan_segments,
+                                rope_shift, rope_table, seg_of_tok, skip_chunks)
 from lmcache_b200.utils import CacheEngineKey, KVCache, _lmcache_nvtx_annotate
 
 logger = init_logger(__name__)
@@ -924,6 +925,33 @@ class LMCacheEngine:
             raise TypeError(f"segment retrieve rotates 16-bit keys only; this engine's KV dtype is {self.metadata.dtype}")
         return plans
 
+    def _derived_key(self, chunk_hash: str, fmt: str) -> CacheEngineKey:
+        """the key of a chunk of a segment stored from inside a longer prompt (rope.derived_digest)"""
+        return self._make_key(derived_digest(chunk_hash), fmt)
+
+    def _derived_keys(self, chunk_hashes, fmt: str) -> LazySeq:
+        return LazySeq(lambda h: self._derived_key(h, fmt), chunk_hashes)
+
+    def _chain_keys(self, chunk_hashes, p: int, n: int, fmt: str) -> list:
+        """the keys of a segment's chunks [0, n): prefix keys for [0, p), derived keys after"""
+        return [self._make_key(h, fmt) for h in chunk_hashes[:p]] + \
+            [self._derived_key(h, fmt) for h in chunk_hashes[p:n]]
+
+    def _touch_chain(self, chunk_hashes, p: int, n: int, fmt: str) -> None:
+        """_touch of a segment's chunks [0, n) as one chain, chunk 0 first, under the keys they hit"""
+        f = getattr(self.engine_, "touch", None)
+        if f is not None:
+            f(self._chain_keys(chunk_hashes, p, n, fmt))
+
+    def _get_chunks(self, keys) -> List[torch.Tensor]:
+        """batched_get of `keys` up to the first miss (a blob of the other kind is one)"""
+        chunks = []
+        for c in self.engine_.batched_get(iter(keys)):
+            if c is None or c.dim() != (3 if self._mla else 5):
+                break
+            chunks.append(c)
+        return chunks
+
     def _rotate(self, view: KvView, written, rope: RopeSpec) -> None:
         """one rope shift of the written key rows of every segment that does not start at token 0"""
         sot, lo, hi, shifts = seg_of_tok(view.ntokens, written)
@@ -944,16 +972,17 @@ class LMCacheEngine:
         if fast:
             geom = self._kv_geometry()
             peek = getattr(self.engine_, "peek_geometry", None)
-            for hs in hashes:
-                if geom is not None:
-                    break
-                key0 = self._make_key(hs[0], fmt)
-                if peek is not None:
-                    geom = peek(key0, fmt)
-                else:
-                    first = self.engine_.get(key0)
-                    if first is not None and first.dim() == (3 if self._mla else 5):
-                        geom = KvView.blob_geometry(first, fmt)
+            for p, hs in zip(plans, hashes):
+                # a segment inside the prompt may be stored under its derived keys only
+                for key0 in [self._make_key(hs[0], fmt)] + ([self._derived_key(hs[0], fmt)] if p.start > 0 else []):
+                    if geom is not None:
+                        break
+                    if peek is not None:
+                        geom = peek(key0, fmt)
+                    else:
+                        first = self.engine_.get(key0)
+                        if first is not None and first.dim() == (3 if self._mla else 5):
+                            geom = KvView.blob_geometry(first, fmt)
             if geom is not None:
                 self._geom = geom
                 L, H, D, dtype = geom
@@ -970,15 +999,17 @@ class LMCacheEngine:
             n_tok = 0
             if fast and blob is not None:
                 own = self.engine_.get_kv_into(self._keys_of(hs, fmt), dst, p.start, cs)
-                self._touch(hs[:own], fmt)
-                n_tok = min(own * cs, p.end - p.start)
+                more = 0
+                if p.start > 0 and own < len(hs):
+                    more = self.engine_.get_kv_into(self._derived_keys(hs[own:], fmt), dst, p.start + own * cs, cs)
+                self._touch_chain(hs, own, own + more, fmt)
+                n_tok = min((own + more) * cs, p.end - p.start)
             elif not fast:
-                chunks = []
-                for c in self.engine_.batched_get(self._make_key(h, fmt) for h in hs):
-                    if c is None or c.dim() != (3 if self._mla else 5):    # the other kind's blob is a miss
-                        break
-                    chunks.append(c)
-                self._touch(hs[:len(chunks)], fmt)
+                chunks = self._get_chunks(self._keys_of(hs, fmt))
+                own = len(chunks)
+                if p.start > 0 and own < len(hs):
+                    chunks += self._get_chunks(self._derived_keys(hs[own:], fmt))
+                self._touch_chain(hs, own, len(chunks), fmt)
                 if chunks and blob is None:
                     L, H, D, dtype = KvView.blob_geometry(chunks[0], fmt)
                     self._check_rope_dtype(dtype)
@@ -1065,8 +1096,12 @@ class LMCacheEngine:
                                                        dtype=view.dtype, device=dev), "vllm")
                     tok0 = 0
                 own = self.engine_.get_kv_into(self._keys_of(hs, "vllm"), dst, tok0, cs)
-                self._touch(hs[:own], "vllm")
-                n = min(own * cs, p.end - p.start)
+                more = 0
+                if p.start > 0 and own < len(hs):
+                    # continued in the namespace of segments stored from inside a longer prompt
+                    more = self.engine_.get_kv_into(self._derived_keys(hs[own:], "vllm"), dst, tok0 + own * cs, cs)
+                self._touch_chain(hs, own, own + more, "vllm")
+                n = min((own + more) * cs, p.end - p.start)
                 if dst is not view and n:
                     view.unpack_blob(dst.blob.narrow(2, 0, n), p.start)
                 written.append((p, n))
@@ -1075,6 +1110,105 @@ class LMCacheEngine:
             ret_mask[p.start:p.start + n] = True
         self._rotate(KvView.from_paged(kv_caches, slots), written, rope)
         return ret_mask
+
+    # ------------------------------------------------------------------ segment store
+    def _store_segments(self, tokens: torch.Tensor, segments, rope: RopeSpec, fmt: str, first: torch.Tensor, D: int,
+                        view_fn: Callable[[], KvView], prefix_store: Callable[[int], None], skip_existing: bool,
+                        blocking: bool) -> None:
+        """Every segment store: the refusals, then a segment at 0 through prefix_store(end), then every other segment's
+        skip scan, one table and one b200kv_pack_chunks_rope launch into one staging blob, and one put per segment
+        under its derived keys."""
+        plans = self._segments_prologue(tokens, segments, rope)
+        self._check_rope_dtype(first.dtype)
+        rope.check(D)
+        cs = self.chunk_size
+        # the segments inside the prompt, planned again: their hash input and chain offsets leave out a segment at 0
+        inner = plan_segments(len(tokens), [(p.start, p.end) for p in plans if p.start > 0], cs)
+        for p in plans:
+            if p.start == 0:
+                # exactly a prefill of tokens[:end]: its ordinary prefix keys, unrotated
+                prefix_store(p.end)
+        if not inner:
+            return
+        hashes = self._segment_hashes(tokens, inner)
+        hits = []
+        for p, hs in zip(inner, hashes):
+            if not skip_existing:
+                hits.append((0, 0))
+                continue
+            has = lambda k: lambda i: self.engine_.contains(k(hs[i], fmt))   # noqa: E731
+            ph, dh = skip_chunks(p.n_chunks, has(self._make_key), has(self._derived_key))
+            self._touch_chain(hs, ph, ph + dh, fmt)
+            hits.append((ph, dh))
+        runs, rows, sot, shifts = plan_segment_store(inner, hits, cs)
+        if not runs:
+            return
+        view = view_fn()
+        self._geom = (view.L, view.H, view.D, view.dtype)
+        dev = view.device
+        with torch.cuda.device(dev):
+            src = view.rows(torch.tensor(rows, dtype=torch.int64).to(dev))
+            blob = torch.empty(KvView.blob_shape(fmt, view.L, view.H, view.D, len(rows), self._mla), dtype=view.dtype,
+                               device=dev)
+            pack_rope(src, blob, torch.tensor(sot, dtype=torch.int32).to(dev),
+                      rope_table(torch.tensor(shifts, dtype=torch.int64).to(dev), rope), rope)
+        tdim = KvView.token_dim(fmt, self._mla)
+        fast = self._fast_path()
+        for r in runs:
+            hs = hashes[r.plan.index]
+            part = KvView.from_blob(blob.narrow(tdim, r.stage_begin, r.n_tok), fmt)
+            keys = self._derived_keys(hs[r.first:], fmt)
+            if fast:
+                self.engine_.put_kv_chunks(keys, part, 0, cs, blocking=blocking)
+            else:
+                _, chunks = part.pack_chunks(0, cs)
+                self.engine_.batched_put(zip(keys, chunks), blocking=blocking)
+            self._touch_chain(hs, r.prefix_hits, len(hs), fmt)
+        logger.info(f"Stored {len(rows)} tokens of {len(runs)} segments under derived keys")
+
+    @_lmcache_nvtx_annotate
+    @torch.no_grad()
+    def store_paged_segments(self, tokens: torch.Tensor, kv_caches, slot_mapping: torch.Tensor, segments,
+                             rope: RopeSpec, skip_existing=True, blocking=True) -> None:
+        """Store documents from inside a longer prompt, for retrieve_paged_segments / retrieve_segments at any later
+        position.  segments: (start, end) token ranges of `tokens`, non-overlapping, in any order (plan_segments).  A
+        segment at start > 0 is stored as a prefill of tokens[start:end] alone would have laid it out: chunks aligned to
+        its start, its keys turned by -start (rope) on the way into one staging blob (one b200kv_pack_chunks_rope launch
+        for all segments), keyed by the derived digests of its own hash chain (rope.derived_digest) -- a namespace that
+        retrieve() / retrieve_paged() never look up, since that KV attended to the tokens before it.  A segment at 0 is
+        store_paged(tokens[:end], kv_caches, slot_mapping[:end]).  skip_existing: chunks held under the segment's prefix
+        keys (stored alone), then under its derived keys, are skipped.  Any layout store_paged takes, every tier; the
+        staging costs the raw bytes of the tokens stored.  TypeError for FP8 KV, ValueError for bad segments or a
+        rotary range that does not fit, all before anything is hashed or written.  reshard_world_sizes is not
+        consulted."""
+        self._check_paged_args(tokens, slot_mapping, kv_caches)
+        first = self._first(kv_caches)
+        D = first.shape[-1] if self._mla else paged_layout(*kv_caches[0]).D
+        slots = slot_mapping.to(first.device)
+        self._store_segments(
+            tokens, segments, rope, "vllm", first, D, lambda: KvView.from_paged(kv_caches, slots),
+            lambda end: self.store_paged(tokens[:end], kv_caches, slot_mapping[:end], skip_existing, blocking),
+            skip_existing, blocking)
+
+    @_lmcache_nvtx_annotate
+    @torch.no_grad()
+    def store_segments(self, tokens: torch.Tensor, kv_tensors_raw: KVCache, segments, rope: RopeSpec,
+                       skip_existing=True, blocking=True) -> None:
+        """store_paged_segments for store()'s KV (per-layer (K, V) in the engine's vllm or huggingface format, or an MLA
+        engine's latent per layer): a segment at 0 is store(tokens[:end], the KV's first end tokens)."""
+        fmt = self.metadata.fmt
+        self._check_store_args(tokens, kv_tensors_raw, fmt)
+        first = self._first(kv_tensors_raw)
+        tdim = KvView.token_dim(fmt) - 2         # a layer's token dimension (a latent's: 0)
+
+        def head(end):
+            if self._mla:
+                return tuple(t[:end] for t in kv_tensors_raw)
+            return tuple((k.narrow(tdim, 0, end), v.narrow(tdim, 0, end)) for k, v in kv_tensors_raw)
+        self._store_segments(
+            tokens, segments, rope, fmt, first, first.shape[-1],
+            lambda: KvView.from_tuple(self._as_cuda_kv(kv_tensors_raw), fmt),
+            lambda end: self.store(tokens[:end], head(end), skip_existing, blocking), skip_existing, blocking)
 
     def close(self):
         self.engine_.close()

@@ -147,6 +147,7 @@ class KvView:
         self.fmt = fmt
         self.blob = blob      # the single blob tensor behind this view, when there is one
         self.layout: Optional[str] = None    # a paged (K, V) view: "flash", "strided" or "split" (see paged_layout)
+        self.slots: Optional[torch.Tensor] = None   # a paged view: the slot map its descriptor reads (rows if strided)
 
     @property
     def L(self): return self.desc.L
@@ -335,7 +336,9 @@ class KvView:
         d.sL = 0
         d.sT, d.sH = D, D
         d.slot_map = slot_mapping.data_ptr()
-        return KvView(d, ([slot_mapping] + list(kv_caches), ptrs), slot_mapping.numel(), ref.device, ref.dtype, "vllm")
+        view = KvView(d, ([slot_mapping] + list(kv_caches), ptrs), slot_mapping.numel(), ref.device, ref.dtype, "vllm")
+        view.slots = slot_mapping
+        return view
 
     @staticmethod
     def from_paged(kv_caches: Sequence[Tuple[torch.Tensor, torch.Tensor]], slot_mapping: torch.Tensor) -> "KvView":
@@ -384,6 +387,22 @@ class KvView:
         d.slot_map = slot_mapping.data_ptr()
         view = KvView(d, (keep, ptrs), slot_mapping.numel(), ref.device, ref.dtype, "vllm")
         view.layout = lay.kind
+        view.slots = slot_mapping
+        return view
+
+    def rows(self, tokens: torch.Tensor) -> "KvView":
+        """The same planes with token i of the new view at token tokens[i] of this one (int64 CUDA): a paged view reads
+        through its slot map composed with `tokens`, a tuple view (no slot map) through `tokens` as rows.  Not for blob
+        views, whose descriptor has no slot map to compose."""
+        if self.blob is not None:
+            raise ValueError("a blob view has no rows to compose")
+        d = N.KvDesc.from_buffer_copy(self.desc)
+        slots = tokens if self.slots is None else self.slots[tokens]
+        slots = slots.contiguous()
+        d.slot_map = slots.data_ptr()
+        view = KvView(d, (self._keep, slots), slots.numel(), self.device, self.dtype, self.fmt)
+        view.layout = self.layout
+        view.slots = slots
         return view
 
     def staged(self, tok_begin: int) -> "KvView":

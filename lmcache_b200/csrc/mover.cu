@@ -17,6 +17,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "rope.cuh"
 
 namespace b200kv {
 
@@ -30,6 +31,11 @@ struct PackParams {
     uint8_t* chunks;
     int64_t chunk_stride_bytes;
     uint8_t* const* table;         // TABLE: chunk j starts at table[j] (a device array) instead of chunks + j * stride
+    // ROPE (b200kv_pack_chunks_rope): channels [rot_offset, rot_offset + 2 half) of the key planes of call token i turn
+    // by table row seg_of_tok[i] of cs (-1: copied as they are); neox pairs (d, d + half), gptj (2d, 2d + 1)
+    const int32_t* seg_of_tok;
+    const float2* cs;
+    int32_t half, rot_offset, neox;
 };
 static_assert(sizeof(PackParams) < kMaxParamBytes, "PackParams must stay under 4 KB of kernel parameters");
 
@@ -39,7 +45,10 @@ static_assert(sizeof(PackParams) < kMaxParamBytes, "PackParams must stay under 4
 // TABLE: the chunk pointers come from a device table the host never reads, so a vector instance checks each chunk's
 // alignment itself and moves a misaligned chunk's vectors element by element (a layer slice is a multiple of 16 bytes
 // whenever the vector path is taken, so the chunk pointer decides for all of its layers).
-template <class E, int VEC, bool PACK, bool TABLE>
+// ROPE (pack only, E a 16-bit float type, TABLE false): a key unit of a turned token turns its own VEC channels on the
+// way, reading a neox partner vector from the same source row (rope_turn_vec); the launch rule takes the vector path
+// only when no vector straddles the rotary range or its halves.
+template <class E, int VEC, bool PACK, bool TABLE, bool ROPE = false>
 __global__ void __launch_bounds__(256) pack_kernel(PackParams P) {
     using vec_t = typename std::conditional<VEC * sizeof(E) == 16, uint4, E>::type;
     const int NL = P.ppl * P.nl;
@@ -81,8 +90,19 @@ __global__ void __launch_bounds__(256) pack_kernel(PackParams P) {
             }
             continue;
         }
-        if (PACK) *reinterpret_cast<vec_t*>(cptr) = *reinterpret_cast<const vec_t*>(plane + src_off);
-        else *reinterpret_cast<vec_t*>(const_cast<E*>(plane) + src_off) = *reinterpret_cast<const vec_t*>(cptr);
+        if (ROPE && PACK) {
+            union { vec_t q; E e[VEC]; } w;
+            w.q = *reinterpret_cast<const vec_t*>(plane + src_off);
+            const int seg = kv == 0 ? __ldg(P.seg_of_tok + j * P.chunk_tokens + tok) : -1;
+            if (seg >= 0)
+                rope_turn_vec<E, VEC>(w.e, plane + (src_off - (int64_t)v * VEC), v * VEC, P.cs + (int64_t)seg * P.half,
+                                      P.half, P.rot_offset, P.neox != 0);
+            *reinterpret_cast<vec_t*>(cptr) = w.q;
+        } else if (PACK) {
+            *reinterpret_cast<vec_t*>(cptr) = *reinterpret_cast<const vec_t*>(plane + src_off);
+        } else {
+            *reinterpret_cast<vec_t*>(const_cast<E*>(plane) + src_off) = *reinterpret_cast<const vec_t*>(cptr);
+        }
     }
 }
 
@@ -96,6 +116,12 @@ static void launch_pack_kernel(bool pack, bool vec, unsigned blocks, const PackP
         if (vec) pack_kernel<E, V, false, TABLE><<<blocks, 256, 0, stream>>>(P);
         else pack_kernel<E, 1, false, TABLE><<<blocks, 256, 0, stream>>>(P);
     }
+}
+
+template <class E>
+static void launch_pack_rope_kernel(bool vec, unsigned blocks, const PackParams& P, cudaStream_t stream) {
+    if (vec) pack_kernel<E, 16 / sizeof(E), true, false, true><<<blocks, 256, 0, stream>>>(P);
+    else pack_kernel<E, 1, true, false, true><<<blocks, 256, 0, stream>>>(P);
 }
 
 // ---------------------------------------------------------------------------------------- split paged caches
@@ -122,6 +148,9 @@ struct SplitParams {
     int32_t L, H, D, bs, n_chunks, chunk_tokens, last_chunk_tokens, l0, nl;
     int32_t vw;                    // bytes per value-side vector of the tile path (16 or 8); 0: element-wise only
     int32_t pitch;                 // shared-memory bytes per token row of one head: D * es + 16
+    const int32_t* seg_of_tok;     // ROPE: as in PackParams, indexed by call token - tok_begin
+    const float2* cs;
+    int32_t half, rot_offset, neox;
 };
 static_assert(sizeof(SplitParams) < kMaxParamBytes, "SplitParams must stay under 4 KB of kernel parameters");
 
@@ -156,7 +185,11 @@ __device__ __forceinline__ void split_value_tile(const SplitParams& P, E* cache,
     }
 }
 
-template <class E, bool PACK, bool TABLE>
+// ROPE (pack only, E a 16-bit float type, TABLE false): the tile path turns each key vector as it leaves the permuted
+// shared-memory rows for the chunk (a neox partner is read from the same shared row), which takes a rotary range
+// aligned to 16-byte vectors (the launch rule sends any other to the element-wise path); the element-wise path turns
+// each key element it moves, reading its partner from the cache (a pack never writes the cache).
+template <class E, bool PACK, bool TABLE, bool ROPE = false>
 __global__ void __launch_bounds__(256) split_kernel(SplitParams P) {
     extern __shared__ __align__(16) uint8_t s_tile[];
     constexpr int X = 16 / (int)sizeof(E);         // elements per 16-byte vector: the key's x
@@ -220,6 +253,17 @@ __global__ void __launch_bounds__(256) split_kernel(SplitParams P) {
                 __syncthreads();
                 for (int i = threadIdx.x; i < nv; i += blockDim.x) {
                     const int o = i / (P.hb * DX), q = i - o * (P.hb * DX), hh = q / DX, dx = q - hh * DX;
+                    if (ROPE) {
+                        const E* srow = reinterpret_cast<const E*>(s_tile + (int64_t)(hh * P.bs + o) * P.pitch);
+                        union { uint4 q; E e[X]; } w;
+                        w.q = *reinterpret_cast<const uint4*>(srow + dx * X);
+                        const int seg = kv == 0 ? __ldg(P.seg_of_tok + (g0 + o - P.tok_begin)) : -1;
+                        if (seg >= 0)
+                            rope_turn_vec<E, X>(w.e, srow, dx * X, P.cs + (int64_t)seg * P.half, P.half, P.rot_offset,
+                                                P.neox != 0);
+                        *reinterpret_cast<uint4*>(crow + o * HD + (int64_t)hh * P.D + dx * X) = w.q;
+                        continue;
+                    }
                     *reinterpret_cast<uint4*>(crow + o * HD + (int64_t)hh * P.D + dx * X) =
                         *reinterpret_cast<const uint4*>(s_tile + (int64_t)(hh * P.bs + o) * P.pitch + dx * 16);
                 }
@@ -243,10 +287,49 @@ __global__ void __launch_bounds__(256) split_kernel(SplitParams P) {
             const int64_t coff = kv == 0 ? (((b * P.H + h) * DX + d / X) * P.bs + so) * X + d % X
                                          : ((b * P.H + h) * (int64_t)P.D + d) * P.bs + so;
             E* ce = reinterpret_cast<E*>(cb) + (((int64_t)lk * tt + tok) * P.H + h) * P.D + d;
-            if (PACK) *ce = plane[coff];
-            else plane[coff] = *ce;
+            if (ROPE && PACK) {
+                E e = plane[coff];
+                const int c = d - P.rot_offset;
+                const int seg = kv == 0 && c >= 0 && c < 2 * P.half ? __ldg(P.seg_of_tok + (g - P.tok_begin)) : -1;
+                if (seg >= 0) {
+                    const int pd = P.rot_offset + rope_partner(c, P.half, P.neox != 0);
+                    const E p = plane[(((b * P.H + h) * DX + pd / X) * P.bs + so) * X + pd % X];
+                    e = rope_turn_one(e, p, c, P.cs + (int64_t)seg * P.half, P.half, P.neox != 0);
+                }
+                *ce = e;
+            } else if (PACK) {
+                *ce = plane[coff];
+            } else {
+                plane[coff] = *ce;
+            }
         }
     }
+}
+
+// b200kv_pack_chunks_rope's rotation: seg_of_tok per call token, the (cos, sin) table, the rotary channels and pairing
+struct RopeArgs {
+    const int32_t* seg_of_tok;
+    const float* cos_sin;
+    int32_t rotary_dim, offset, style;
+    // 16-byte vectors can turn: no vector straddles the rotary range or (neox) its halves
+    bool vec_ok(int ev) const { return offset % ev == 0 && (style == 0 ? (rotary_dim / 2) % ev : rotary_dim % ev) == 0; }
+};
+
+template <class P_t>
+static void set_rope(P_t& P, const RopeArgs* rope) {
+    P.seg_of_tok = rope ? rope->seg_of_tok : nullptr;
+    P.cs = rope ? reinterpret_cast<const float2*>(rope->cos_sin) : nullptr;
+    P.half = rope ? rope->rotary_dim / 2 : 0;
+    P.rot_offset = rope ? rope->offset : 0;
+    P.neox = rope ? rope->style == 0 : 0;
+}
+
+template <class E>
+static int launch_split_rope_kernel(unsigned blocks, size_t smem, const SplitParams& P, cudaStream_t stream) {
+    auto k = split_kernel<E, true, false, true>;
+    if (smem > 48 * 1024) B2_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k<<<blocks, 256, smem, stream>>>(P);
+    return 0;
 }
 
 template <class E, bool TABLE>
@@ -259,7 +342,8 @@ static int launch_split_kernel(bool pack, unsigned blocks, size_t smem, const Sp
 
 static int launch_split(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
                         int32_t last_chunk_tokens, int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
-                        void* chunks, int64_t chunk_stride_bytes, void* const* table, cudaStream_t stream) {
+                        void* chunks, int64_t chunk_stride_bytes, void* const* table, cudaStream_t stream,
+                        const RopeArgs* rope = nullptr) {
     B2_REQUIRE(kv->L > 0 && 2 * kv->L <= B200KV_MAX_PLANES, "bad kv descriptor");
     B2_REQUIRE(!(kv->dtype & B200KV_KV_LATENT), "a latent KV has no split layout (B200KV_KV_PAGED_SPLIT)");
     B2_REQUIRE(hf_layout == 0, "a split paged KV (B200KV_KV_PAGED_SPLIT) moves to and from vllm chunks only (hf_layout 0)");
@@ -312,6 +396,8 @@ static int launch_split(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, 
     for (int kvi = 0; kvi < 2 && P.vw; ++kvi)
         for (int l = layer_begin; l < layer_end && P.vw; ++l)
             if ((reinterpret_cast<uintptr_t>(P.pt.p[kvi * P.L + l]) & 15) != 0) P.vw = 0;
+    if (rope && !rope->vec_ok(16 / es)) P.vw = 0;     // the tile turns whole 16-byte vectors
+    set_rope(P, rope);
     size_t smem = (size_t)P.hb * P.bs * P.pitch;
     if (smem > 200 * 1024) P.vw = 0;
     if (P.vw == 0) smem = 0;
@@ -322,7 +408,10 @@ static int launch_split(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, 
     int64_t blocks = std::min<int64_t>(units, (int64_t)sms * 8 * 4);
     if (blocks < 1) blocks = 1;
     int rc;
-    if (table != nullptr) {
+    if (rope) {
+        if (kv_split_dtype(kv) == B200KV_DT_BF16) rc = launch_split_rope_kernel<__nv_bfloat16_raw>((unsigned)blocks, smem, P, stream);
+        else rc = launch_split_rope_kernel<__half_raw>((unsigned)blocks, smem, P, stream);
+    } else if (table != nullptr) {
         if (es == 2) rc = launch_split_kernel<uint16_t, true>(pack, (unsigned)blocks, smem, P, stream);
         else rc = launch_split_kernel<uint8_t, true>(pack, (unsigned)blocks, smem, P, stream);
     } else {
@@ -335,14 +424,16 @@ static int launch_split(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, 
 }
 
 // layer_end < 0: every layer.  table != NULL: chunk j starts at table[j] (chunks and chunk_stride_bytes unused).
+// rope != NULL (pack, no table): b200kv_pack_chunks_rope, which has checked the rotation's arguments
 static int launch_pack(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
                        int32_t last_chunk_tokens, int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
-                       void* chunks, int64_t chunk_stride_bytes, void* const* table, cudaStream_t stream) {
+                       void* chunks, int64_t chunk_stride_bytes, void* const* table, cudaStream_t stream,
+                       const RopeArgs* rope = nullptr) {
     PackParams P;
     B2_REQUIRE(kv != nullptr && kv->L > 0 && 2 * kv->L <= B200KV_MAX_PLANES, "bad kv descriptor");
     if (kv_split(kv))
         return launch_split(pack, kv, tok_begin, n_chunks, chunk_tokens, last_chunk_tokens, hf_layout, layer_begin,
-                            layer_end, chunks, chunk_stride_bytes, table, stream);
+                            layer_end, chunks, chunk_stride_bytes, table, stream, rope);
     if (layer_end < 0) layer_end = kv->L;
     B2_REQUIRE(0 <= layer_begin && layer_begin < layer_end && layer_end <= kv->L, "bad layer range");
     float bins[B200KV_MAX_PLANES];
@@ -372,6 +463,8 @@ static int launch_pack(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, i
     for (int kvi = 0; kvi < P.ppl && vec; ++kvi)
         for (int l = layer_begin; l < layer_end && vec; ++l)
             vec = (reinterpret_cast<uintptr_t>(P.pt.p[kvi * P.L + l]) & 15) == 0;
+    if (rope) vec = vec && rope->vec_ok(ev);
+    set_rope(P, rope);
     const int V = vec ? ev : 1;
     const int64_t total = ((int64_t)(n_chunks - 1) * chunk_tokens + last_chunk_tokens) * P.ppl * P.nl * kv->H * (kv->D / V);
     int64_t blocks = (total + 255) / 256;
@@ -381,7 +474,10 @@ static int launch_pack(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, i
     const int64_t cap = (int64_t)sms * 8 * 4;   // a few waves of SMs x 8 CTAs; grid-stride covers the rest
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
-    if (table != nullptr) {
+    if (rope) {
+        if (kv_dtype(kv) == B200KV_DT_BF16) launch_pack_rope_kernel<__nv_bfloat16_raw>(vec, (unsigned)blocks, P, stream);
+        else launch_pack_rope_kernel<__half_raw>(vec, (unsigned)blocks, P, stream);
+    } else if (table != nullptr) {
         if (es == 2) launch_pack_kernel<uint16_t, true>(pack, vec, (unsigned)blocks, P, stream);
         else launch_pack_kernel<uint8_t, true>(pack, vec, (unsigned)blocks, P, stream);
     } else {
@@ -403,6 +499,25 @@ int b200kv_pack_chunks(const b200kv_kv_desc* src, int64_t tok_begin, int32_t n_c
                        void* stream) {
     return launch_pack(true, src, tok_begin, n_chunks, chunk_tokens, last_chunk_tokens, hf_layout, 0, -1, chunks,
                        chunk_stride_bytes, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+int b200kv_pack_chunks_rope(const b200kv_kv_desc* src, int64_t tok_begin, int32_t n_chunks, int32_t chunk_tokens,
+                            int32_t last_chunk_tokens, int32_t hf_layout, void* chunks, int64_t chunk_stride_bytes,
+                            const int32_t* seg_of_tok, const float* cos_sin, int32_t rotary_dim, int32_t offset,
+                            int32_t style, void* stream) {
+    // b200kv_rope_shift's refusals; launch_pack makes b200kv_pack_chunks' own
+    B2_REQUIRE(src != nullptr, "kv descriptor is NULL");
+    B2_REQUIRE(cos_sin != nullptr, "cos_sin table is NULL");
+    B2_REQUIRE(seg_of_tok != nullptr, "seg_of_tok is NULL");
+    B2_REQUIRE(style == 0 || style == 1, "style must be 0 (neox) or 1 (gptj)");
+    const int dt = kv_split(src) ? kv_split_dtype(src) : kv_dtype(src);
+    B2_REQUIRE(dt == B200KV_DT_BF16 || dt == B200KV_DT_FP16,
+               "the rope pack takes 16-bit keys only: rotating a one-byte (FP8) key would round it again");
+    B2_REQUIRE(rotary_dim > 0 && rotary_dim % 2 == 0, "rotary_dim must be even and positive");
+    B2_REQUIRE(offset >= 0 && (int64_t)offset + rotary_dim <= src->D, "offset + rotary_dim exceeds the head size D");
+    const RopeArgs rope{seg_of_tok, cos_sin, rotary_dim, offset, style};
+    return launch_pack(true, src, tok_begin, n_chunks, chunk_tokens, last_chunk_tokens, hf_layout, 0, -1, chunks,
+                       chunk_stride_bytes, nullptr, static_cast<cudaStream_t>(stream), &rope);
 }
 
 int b200kv_unpack_chunks(const void* chunks, int64_t chunk_stride_bytes, int32_t n_chunks, int32_t chunk_tokens,

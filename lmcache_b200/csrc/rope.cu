@@ -15,6 +15,7 @@
 #include <stdint.h>
 
 #include "common.cuh"
+#include "rope.cuh"     // to_f / from_f / rotate: the same arithmetic as the mover's b200kv_pack_chunks_rope
 
 namespace b200kv {
 
@@ -37,25 +38,6 @@ __device__ __forceinline__ int64_t key_off(const RopeParams& P, int64_t row, int
         return (((b * P.H + h) * (P.D / X) + c / X) * P.bs + o) * X + c % X;
     }
     return row * P.sT + (int64_t)h * P.sH + c;
-}
-
-template <class E> __device__ __forceinline__ float to_f(E v);
-template <> __device__ __forceinline__ float to_f<__nv_bfloat16_raw>(__nv_bfloat16_raw v) {
-    return __uint_as_float((uint32_t)v.x << 16);
-}
-template <> __device__ __forceinline__ float to_f<__half_raw>(__half_raw v) { return __half2float(__half(v)); }
-template <class E> __device__ __forceinline__ E from_f(float f);
-template <> __device__ __forceinline__ __nv_bfloat16_raw from_f<__nv_bfloat16_raw>(float f) {
-    return __nv_bfloat16_raw(__float2bfloat16_rn(f));
-}
-template <> __device__ __forceinline__ __half_raw from_f<__half_raw>(float f) { return __half_raw(__float2half_rn(f)); }
-
-// (a, b) <- (a cos - b sin, b cos + a sin), in fp32, rounded once to E
-template <class E>
-__device__ __forceinline__ void rotate(E& a, E& b, float2 t) {
-    const float x = to_f(a), y = to_f(b);
-    a = from_f<E>(fmaf(x, t.x, -y * t.y));
-    b = from_f<E>(fmaf(y, t.x, x * t.y));
 }
 
 // One unit = NP rotation pairs of one (token, layer, head).  NEOX: pairs (j, j + half), a unit reads NP channels from

@@ -1,14 +1,20 @@
-"""Non-prefix KV reuse: the rotation a retrieved segment's keys need, and the plan of a segment retrieve.
+"""Non-prefix KV reuse: the rotation a retrieved segment's keys need, and the plans of a segment retrieve and store.
 
 vLLM caches K after the rotary embedding.  A document prefilled alone at positions 0..n-1 holds R(i)·k_i; served at
 positions s..s+n-1 its keys must be R(s + i)·k_i = R(s)·(R(i)·k_i), so each retrieved key row is rotated by s·θ_j
 (b200kv_rope_shift).  V carries no position.  A document stored as its own prompt is keyed by the hash chain of its own
 tokens, which is exactly what a segment lookup recomputes from those tokens inside a longer request: existing caches
-serve as segments without being stored again."""
+serve as segments without being stored again.
+
+A document stored from position s > 0 of a longer prompt is turned back by -s (b200kv_pack_chunks_rope), so its keys
+are those of position 0 on.  Its KV still attended to the tokens before s, which a prefill of the document alone did
+not: it is keyed in a namespace of its own (derived_digest), which retrieve() never looks up.  A segment lookup
+continues there from the first chunk the prefix keys miss."""
 from __future__ import annotations
 
 import ctypes
-from typing import List, NamedTuple, Sequence, Tuple
+import hashlib
+from typing import Callable, List, NamedTuple, Sequence, Tuple
 
 import torch
 
@@ -127,6 +133,20 @@ def seg_of_tok(n_tokens: int, written: Sequence[Tuple[SegmentPlan, int]]) -> Tup
     return sot, lo, hi, shifts
 
 
+def rope_table(shifts: torch.Tensor, rope: RopeSpec) -> torch.Tensor:
+    """(cos, sin) of every shift (int64 CUDA) times every frequency, float32 [n, rotary_dim/2, 2]: one
+    b200kv_rope_table launch on the current stream of the shifts' device"""
+    dev = shifts.device
+    with torch.cuda.device(dev):
+        inv = rope.inv_freq.to(dev, non_blocking=True)
+        table = torch.empty(shifts.numel(), rope.rotary_dim // 2, 2, dtype=torch.float32, device=dev)
+        N.check(N.lib().b200kv_rope_table(ctypes.c_void_p(shifts.data_ptr()), shifts.numel(),
+                                          ctypes.c_void_p(inv.data_ptr()), rope.rotary_dim,
+                                          ctypes.c_void_p(table.data_ptr()), torch.cuda.current_stream().cuda_stream),
+                "rope_table")
+    return table
+
+
 def rope_shift(view, tok_begin: int, seg: torch.Tensor, shifts: torch.Tensor, rope: RopeSpec) -> None:
     """Rotate the keys of tokens [tok_begin, tok_begin + len(seg)) of a KvView on the current stream: one table launch
     (b200kv_rope_table) and one shift launch (b200kv_rope_shift).  seg: int32 CUDA, a row of the table per token or -1;
@@ -134,11 +154,82 @@ def rope_shift(view, tok_begin: int, seg: torch.Tensor, shifts: torch.Tensor, ro
     dev = view.device
     with torch.cuda.device(dev):
         st = torch.cuda.current_stream().cuda_stream
-        inv = rope.inv_freq.to(dev, non_blocking=True)
-        table = torch.empty(shifts.numel(), rope.rotary_dim // 2, 2, dtype=torch.float32, device=dev)
-        N.check(N.lib().b200kv_rope_table(ctypes.c_void_p(shifts.data_ptr()), shifts.numel(),
-                                          ctypes.c_void_p(inv.data_ptr()), rope.rotary_dim,
-                                          ctypes.c_void_p(table.data_ptr()), st), "rope_table")
+        table = rope_table(shifts, rope)
         N.check(N.lib().b200kv_rope_shift(ctypes.byref(view.desc), tok_begin, seg.numel(),
                                           ctypes.c_void_p(seg.data_ptr()), ctypes.c_void_p(table.data_ptr()),
                                           rope.rotary_dim, rope.offset, STYLES[rope.style], st), "rope_shift")
+
+
+def pack_rope(view, blob: torch.Tensor, seg: torch.Tensor, table: torch.Tensor, rope: RopeSpec) -> None:
+    """Tokens [0, T) of a KvView packed into `blob`, one chunk of T tokens in the view's chunk layout, with the keys of
+    token i turned by table row seg[i] (-1: copied) on the way: one b200kv_pack_chunks_rope launch on the current
+    stream.  seg: int32 CUDA [T]; table: rope_table's."""
+    t = view.ntokens
+    with torch.cuda.device(view.device):
+        N.check(N.lib().b200kv_pack_chunks_rope(ctypes.byref(view.desc), 0, 1, t, t, int(view.fmt == "huggingface"),
+                                                ctypes.c_void_p(blob.data_ptr()), blob.numel() * blob.element_size(),
+                                                ctypes.c_void_p(seg.data_ptr()), ctypes.c_void_p(table.data_ptr()),
+                                                rope.rotary_dim, rope.offset, STYLES[rope.style],
+                                                torch.cuda.current_stream().cuda_stream), "pack_chunks_rope")
+
+
+# ---------------------------------------------------------------------------------------------- segment store
+DERIVED_TAG = b"lmcache-b200 contextual kv v1\0"
+
+
+def derived_digest(chunk_hash: str) -> str:
+    """The key digest of a chunk of a segment stored from inside a longer prompt: sha256(DERIVED_TAG || raw chain
+    digest) as 64 hex characters.  A key string keeps its shape and length, and no prefix digest equals one unless
+    SHA-256 collides."""
+    return hashlib.sha256(DERIVED_TAG + bytes.fromhex(chunk_hash)).hexdigest()
+
+
+def skip_chunks(n_chunks: int, prefix_has: Callable[[int], bool], derived_has: Callable[[int], bool]) -> Tuple[int, int]:
+    """A segment store's skip scan: (p, d) -- chunks [0, p) hit under their prefix keys (the document was stored alone),
+    chunks [p, p + d) under their derived keys; the chunks from p + d on are stored.  Each lookup runs only while the
+    walk is still hitting."""
+    p = 0
+    while p < n_chunks and prefix_has(p):
+        p += 1
+    d = 0
+    while p + d < n_chunks and derived_has(p + d):
+        d += 1
+    return p, d
+
+
+class StoreRun(NamedTuple):
+    """The part of one segment (start > 0) that a segment store stores: chunks [first, n_chunks) of its plan, request
+    tokens [begin, plan.end), staged at tokens [stage_begin, stage_begin + n_tok) of the staging blob, turned by table row
+    `row` (shift -start)."""
+    plan: SegmentPlan
+    prefix_hits: int
+    first: int
+    begin: int
+    stage_begin: int
+    n_tok: int
+    row: int
+
+
+def plan_segment_store(plans: Sequence[SegmentPlan], hits: Sequence[Tuple[int, int]],
+                       chunk_size: int) -> Tuple[List[StoreRun], List[int], List[int], List[int]]:
+    """The staging of a segment store, from the plans of segments at start > 0 and their skip scans (p, d):
+    (runs of the segments with chunks to store, the request token of every staged token, seg_of_tok of every staged
+    token, the shift of every table row).  A run's tokens are staged back to back in plan order and each segment with
+    something to store has one table row, shift -start; every staged token is stored, so seg_of_tok holds no -1."""
+    runs: List[StoreRun] = []
+    rows: List[int] = []
+    sot: List[int] = []
+    shifts: List[int] = []
+    for p, (ph, dh) in zip(plans, hits):
+        if p.start <= 0:
+            raise ValueError(f"segment ({p.start}, {p.end}) starts at token 0: it is stored under its prefix keys")
+        first = min(ph + dh, p.n_chunks)
+        begin = p.start + first * chunk_size
+        if begin >= p.end:
+            continue
+        n = p.end - begin
+        runs.append(StoreRun(p, min(ph, first), first, begin, len(rows), n, len(shifts)))
+        rows.extend(range(begin, p.end))
+        sot.extend([len(shifts)] * n)
+        shifts.append(-p.start)
+    return runs, rows, sot, shifts
