@@ -612,6 +612,32 @@ int b200kv_rope_table(const int64_t* shifts, int32_t n_seg, const float* inv_fre
                       void* stream);
 int b200kv_rope_shift(const b200kv_kv_desc* kv, int64_t tok_begin, int64_t ntok, const int32_t* seg_of_tok,
                       const float* cos_sin, int32_t rotary_dim, int32_t offset, int32_t style, void* stream);
+/* b200kv_rope_shift restricted to the key planes of layers [layer_begin, layer_end): a layer-wise retrieve turns each
+ * layer's keys as soon as that layer has landed.  b200kv_rope_shift is the range [0, L), and calls whose ranges cover
+ * each layer once give its result bit for bit.  Plane pointers of other layers are never dereferenced, and the vector
+ * path's alignment test looks at the range's planes only.  < 0, nothing enqueued: what b200kv_rope_shift refuses, and a
+ * layer range that is empty or outside [0, L).  Added without changing anything that existed (b200kv_version() stays
+ * 4). */
+/* The unpack direction of b200kv_pack_chunks_rope, for a layer range: chunk j (chunk_ptrs[j], DEVICE, the chunk's
+ * layer range as in b200kv_unpack_chunks_layers) holds chunk_ntok[j] tokens (DEVICE int32, 1 .. chunk_tokens) and
+ * lands at view token dst_tok[j] (DEVICE int64); the rotary channels of its key planes turn by table row chunk_seg[j]
+ * (DEVICE int32; -1: copied).  Chunks need not be contiguous in the view nor of one size: a layer-wise segment retrieve
+ * writes one layer of every hit chunk of every segment in one launch.  Every destination b200kv_unpack_chunks_layers
+ * takes (blobs, tuples, latent views, slot-mapped and block-strided rows, B200KV_KV_PAGED_SPLIT).  Each key element
+ * reads its rotation partner from the chunk, with b200kv_rope_shift's arithmetic: the result is bit-identical to
+ * b200kv_unpack_chunks_layers of each chunk followed by b200kv_rope_shift_layers.  A misaligned chunk pointer moves
+ * element by element.  < 0, nothing enqueued: NULL arrays, what b200kv_rope_shift_layers refuses (one-byte dtypes, an
+ * odd or non-positive rotary_dim, offset < 0 or offset + rotary_dim > D, a NULL cos_sin, a bad style or layer range)
+ * and what b200kv_unpack_chunks_layers refuses.  The device arrays are not bounds-checked.  Added without changing
+ * anything that existed (b200kv_version() stays 4). */
+int b200kv_unpack_chunks_layers_rope(const void* const* chunk_ptrs, int32_t n_chunks, int32_t chunk_tokens,
+                                     const int32_t* chunk_ntok, const int64_t* dst_tok, const int32_t* chunk_seg,
+                                     int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
+                                     const b200kv_kv_desc* dst, const float* cos_sin, int32_t rotary_dim, int32_t offset,
+                                     int32_t style, void* stream);
+int b200kv_rope_shift_layers(const b200kv_kv_desc* kv, int32_t layer_begin, int32_t layer_end, int64_t tok_begin,
+                             int64_t ntok, const int32_t* seg_of_tok, const float* cos_sin, int32_t rotary_dim,
+                             int32_t offset, int32_t style, void* stream);
 /* b200kv_pack_chunks with the keys turned on the way (a segment of a longer prompt stored as if prefilled alone: its
  * keys turned by -start): the same descriptors (blobs, tuples, latent views, slot-mapped and block-strided rows,
  * B200KV_KV_PAGED_SPLIT), chunk layouts and destinations (device or mapped pinned memory) as b200kv_pack_chunks, in one

@@ -25,8 +25,8 @@ from lmcache_b200.logging import init_logger
 from lmcache_b200.storage_backend import CreateStorageBackend
 from lmcache_b200.pipeline import HeadWindow, LayerwiseUpload, join_uploads
 from lmcache_b200.reshard import first_source_rank, source_shards
-from lmcache_b200.rope import (RopeSpec, derived_digest, hash_input, pack_rope, plan_segment_store, plan_segments,
-                                rope_shift, rope_table, seg_of_tok, skip_chunks)
+from lmcache_b200.rope import (RopeSpec, Rotation, derived_digest, hash_input, pack_rope, plan_segment_store,
+                                plan_segments, rope_shift, rope_table, seg_of_tok, skip_chunks)
 from lmcache_b200.utils import CacheEngineKey, KVCache, _lmcache_nvtx_annotate
 
 logger = init_logger(__name__)
@@ -960,6 +960,35 @@ class LMCacheEngine:
             sh = torch.tensor(shifts, dtype=torch.int64).to(view.device)
             rope_shift(view, lo, seg, sh, rope)
 
+    def _segments_geometry(self, plans, hashes, fmt: str, rope: Optional[RopeSpec]):
+        """(L, H, D, dtype of the result) of a segment retrieve on a native-path tier: the engine's, or read from the
+        first chunk any segment has stored; None when neither tells.  The dtype, and D against `rope`, are checked."""
+        geom = self._kv_geometry()
+        peek = getattr(self.engine_, "peek_geometry", None)
+        for p, hs in zip(plans, hashes):
+            # a segment inside the prompt may be stored under its derived keys only
+            for key0 in [self._make_key(hs[0], fmt)] + ([self._derived_key(hs[0], fmt)] if p.start > 0 else []):
+                if geom is not None:
+                    break
+                if peek is not None:
+                    geom = peek(key0, fmt)
+                else:
+                    first = self.engine_.get(key0)
+                    if first is not None and first.dim() == (3 if self._mla else 5):
+                        geom = KvView.blob_geometry(first, fmt)
+        if geom is None:
+            return None
+        self._geom = geom
+        L, H, D, dtype = geom
+        od = getattr(self.engine_, "out_dtype", None) or \
+            getattr(getattr(self.engine_, "deserializer", None), "out_dtype", None)
+        if od is not None and od() is not None:
+            dtype = od()
+        self._check_rope_dtype(dtype)
+        if rope is not None:
+            rope.check(D)
+        return L, H, D, dtype
+
     def _segments_blob(self, tokens, plans, hashes, fmt: str, rope: Optional[RopeSpec] = None):
         """Every segment's longest stored prefix of chunks in one zeroed blob of the request's T tokens, each at its
         start (unrotated).  Returns (blob or None when nothing was found, [(plan, tokens written)]).  With `rope`, the
@@ -970,29 +999,9 @@ class LMCacheEngine:
         written, blob = [], None
         fast = self._fast_path()
         if fast:
-            geom = self._kv_geometry()
-            peek = getattr(self.engine_, "peek_geometry", None)
-            for p, hs in zip(plans, hashes):
-                # a segment inside the prompt may be stored under its derived keys only
-                for key0 in [self._make_key(hs[0], fmt)] + ([self._derived_key(hs[0], fmt)] if p.start > 0 else []):
-                    if geom is not None:
-                        break
-                    if peek is not None:
-                        geom = peek(key0, fmt)
-                    else:
-                        first = self.engine_.get(key0)
-                        if first is not None and first.dim() == (3 if self._mla else 5):
-                            geom = KvView.blob_geometry(first, fmt)
+            geom = self._segments_geometry(plans, hashes, fmt, rope)
             if geom is not None:
-                self._geom = geom
                 L, H, D, dtype = geom
-                od = getattr(self.engine_, "out_dtype", None) or \
-                    getattr(getattr(self.engine_, "deserializer", None), "out_dtype", None)
-                if od is not None and od() is not None:
-                    dtype = od()
-                self._check_rope_dtype(dtype)
-                if rope is not None:
-                    rope.check(D)
                 blob = torch.zeros(KvView.blob_shape(fmt, L, H, D, T, self._mla), dtype=dtype, device=dev)
         dst = None if blob is None else KvView.from_blob(blob, fmt)
         for p, hs in zip(plans, hashes):
@@ -1110,6 +1119,93 @@ class LMCacheEngine:
             ret_mask[p.start:p.start + n] = True
         self._rotate(KvView.from_paged(kv_caches, slots), written, rope)
         return ret_mask
+
+    # ------------------------------------------------------------------ layer-wise segment retrieve
+    def _segments_runs_get(self, kv_caches=None):
+        """The tier's multi-run layer-major get (get_kv_layerwise_runs) when it can serve this engine's chunks so
+        (retrieve_layerwise's conditions, and no split cache staged through a blob), else None"""
+        f = getattr(self.engine_, "get_kv_layerwise_runs", None)
+        if f is None or self._layerwise_get() is None or (kv_caches is not None and self._stages_split(kv_caches)):
+            return None
+        return f
+
+    def _segments_layerwise(self, get, plans, hashes, fmt: str, view: KvView, rope: RopeSpec, n_tokens: int):
+        """Every segment's stored chunks fetched into `view` by ONE layer-major get, each at its start: its prefix keys,
+        then (start > 0) its derived keys from their first miss on; the keys of every segment at start > 0 turned by its
+        start, layer by layer, inside the upload.  Touches each segment's chain.  Returns (ret_mask, LayerwiseUpload)."""
+        shifted = [p for p in plans if p.shift != 0]
+        rotation = None
+        if shifted:
+            with torch.cuda.device(view.device):
+                table = rope_table(torch.tensor([p.shift for p in shifted], dtype=torch.int64).to(view.device), rope)
+            rows = {p.index: k for k, p in enumerate(shifted)}
+            rotation = Rotation(rope, table, [rows.get(p.index, -1) for p in plans], [p.end for p in plans])
+        runs = [(self._keys_of(hs, fmt), self._derived_keys(hs, fmt) if p.start > 0 else None, p.start)
+                for p, hs in zip(plans, hashes)]
+        with torch.cuda.device(view.device):
+            hits, upload = get(runs, view, self.chunk_size, rotation)
+        ret_mask = torch.zeros(n_tokens, dtype=torch.bool)
+        for p, hs, (own, more) in zip(plans, hashes, hits):
+            self._touch_chain(hs, own, own + more, fmt)
+            ret_mask[p.start:p.start + min((own + more) * self.chunk_size, p.end - p.start)] = True
+        return ret_mask, upload
+
+    @torch.no_grad()
+    def retrieve_paged_segments_layerwise(self, tokens: torch.Tensor, kv_caches, slot_mapping: torch.Tensor, segments,
+                                          rope: RopeSpec) -> LayerwiseRetrieval:
+        """retrieve_paged_segments, with the KV made available one layer at a time (`kv` is None): returns once every
+        segment's hit is known; after wait_layer(l, stream) layer l's rows are written and turned by each segment's
+        start; after synchronize() ret_mask and every row are retrieve_paged_segments'.  On every tier with a
+        layer-major get (raw, CacheGen and lossless host and disk, lm:// with ranged reads, hybrid), every segment's
+        chunks go through one layer-major upload (the tier's get_kv_layerwise_runs), each layer's keys turned as that
+        layer lands.  Every other case -- the remote tier without the opt-in or ranged reads, the torch serde, CacheGen
+        chunks of more than 256 tokens, a split (PagedAttention) cache on a container tier -- runs
+        retrieve_paged_segments with one event for every layer.  The refusals are
+        retrieve_paged_segments', raised before anything is hashed or fetched."""
+        self._check_paged_args(tokens, slot_mapping)
+        self._check_kind(kv_caches, "kv_caches")
+        plans = self._segments_prologue(tokens, segments, rope)
+        first = self._first(kv_caches)
+        self._check_rope_dtype(first.dtype)
+        rope.check(first.shape[-1] if self._mla else paged_layout(*kv_caches[0]).D)
+        get = self._segments_runs_get(kv_caches)
+        if get is None:
+            ret_mask = self.retrieve_paged_segments(tokens, kv_caches, slot_mapping, segments, rope)
+            return self._layerwise_result(ret_mask, None, len(kv_caches), [])
+        view = KvView.from_paged(kv_caches, slot_mapping.to(first.device))
+        ret_mask, upload = self._segments_layerwise(get, plans, self._segment_hashes(tokens, plans), "vllm", view, rope,
+                                                    len(tokens))
+        return LayerwiseRetrieval(ret_mask, None, len(kv_caches), upload)
+
+    @torch.no_grad()
+    def retrieve_segments_layerwise(self, tokens: torch.Tensor, segments, rope: RopeSpec) -> LayerwiseRetrieval:
+        """retrieve_segments, with the KV made available one layer at a time: `kv` holds retrieve_segments' per-layer
+        views of one blob (rows not retrieved are zero), whose layer l may be read once wait_layer(l, stream) was called.
+        The same tiers go layer-major as for retrieve_paged_segments_layerwise.  On a total miss before the geometry is
+        known, kv is () and num_layers 0."""
+        fmt = self.metadata.fmt
+        if fmt not in ("vllm", "huggingface"):
+            raise ValueError(f"Invalid format: {fmt}")
+        plans = self._segments_prologue(tokens, segments, rope)
+        geom = self._kv_geometry()
+        if geom is not None:
+            self._check_rope_dtype(geom[3])
+            rope.check(geom[2])
+        get = self._segments_runs_get()
+        if get is None:
+            kv, ret_mask = self.retrieve_segments(tokens, segments, rope)
+            geom = self._kv_geometry()
+            return self._layerwise_result(ret_mask, kv, len(kv) or (geom[0] if geom else 0), [])
+        hashes = self._segment_hashes(tokens, plans)
+        geom = self._segments_geometry(plans, hashes, fmt, rope)
+        if geom is None:
+            return self._layerwise_result(torch.zeros(len(tokens), dtype=torch.bool), (), 0, [])
+        L, H, D, dtype = geom
+        blob = torch.zeros(KvView.blob_shape(fmt, L, H, D, len(tokens), self._mla), dtype=dtype,
+                           device=torch.device("cuda", torch.cuda.current_device()))
+        ret_mask, upload = self._segments_layerwise(get, plans, hashes, fmt, KvView.from_blob(blob, fmt), rope,
+                                                    len(tokens))
+        return LayerwiseRetrieval(ret_mask, self._blob_to_tuple_kv(blob), L, upload)
 
     # ------------------------------------------------------------------ segment store
     def _store_segments(self, tokens: torch.Tensor, segments, rope: RopeSpec, fmt: str, first: torch.Tensor, D: int,

@@ -488,6 +488,105 @@ static int launch_pack(bool pack, const b200kv_kv_desc* kv, int64_t tok_begin, i
     return 0;
 }
 
+// ---------------------------------------------------------------------------------------- unpack with the keys turned
+// b200kv_unpack_chunks_layers_rope: one layer range of chunks of any sizes, each landing at its own destination token,
+// with the rotary channels of its key planes turned by its own table row on the way (a layer-wise segment retrieve:
+// the chunks of several segments, each segment's tail chunk short).  Units are laid out over chunk_tokens per chunk and
+// skip the tokens past chunk_ntok[j].  A key unit turns its own VEC channels, reading a neox partner from the CHUNK row
+// (the source, never written), with rope_turn_vec: the result is the bits of b200kv_unpack_chunks_layers of each chunk
+// followed by b200kv_rope_shift_layers.  SPLIT (B200KV_KV_PAGED_SPLIT, VEC = x): a key vector is x channels of one
+// token, stored whole; a value vector is scattered element by element along the block's channel rows.
+struct UnpackRopeParams {
+    PlaneTable pt;
+    int64_t sT, sH;
+    const int64_t* slot_map;
+    const void* const* chunk_ptrs;     // chunk j's layer range, [nl][ppl][t][H][D] (vllm) or [nl][ppl][H][t][D] (hf)
+    const int32_t* chunk_ntok;         // t of chunk j
+    const int64_t* dst_tok;            // view token of chunk j's first token
+    const int32_t* chunk_seg;          // table row of chunk j, -1: copied
+    const float2* cs;
+    int32_t L, H, D, n_chunks, chunk_tokens, hf_layout, ppl, l0, nl, bs, half, rot_offset, neox;
+};
+static_assert(sizeof(UnpackRopeParams) < kMaxParamBytes, "UnpackRopeParams must stay under 4 KB of kernel parameters");
+
+template <class E, int VEC, bool SPLIT>
+__global__ void __launch_bounds__(256) unpack_rope_kernel(UnpackRopeParams P) {
+    using vec_t = typename std::conditional<VEC * sizeof(E) == 16, uint4, E>::type;
+    constexpr int X = 16 / (int)sizeof(E);
+    const int NL = P.ppl * P.nl;
+    const int vph = P.D / VEC;
+    const int64_t vpt = (int64_t)P.H * vph;
+    const int64_t per_plane = (int64_t)P.chunk_tokens * vpt;
+    const int64_t per_chunk = (int64_t)NL * per_plane;
+    const int64_t total = (int64_t)P.n_chunks * per_chunk;
+    for (int64_t u = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; u < total; u += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t j = u / per_chunk;
+        int64_t r = u - j * per_chunk;
+        const int lk = (int)(r / per_plane);
+        r -= (int64_t)lk * per_plane;
+        const int tok = (int)(r / vpt);
+        const int t = __ldg(P.chunk_ntok + j);
+        if (tok >= t) continue;
+        r -= (int64_t)tok * vpt;
+        const int h = (int)(r / vph);
+        const int v = (int)(r - (int64_t)h * vph);
+        const int l = P.l0 + (P.ppl == 2 ? lk >> 1 : lk), kv = P.ppl == 2 ? lk & 1 : 0;
+        E* plane = const_cast<E*>(reinterpret_cast<const E*>(P.pt.p[kv * P.L + l]));
+        int64_t row = __ldg(P.dst_tok + j) + tok;
+        if (P.slot_map) row = __ldg(P.slot_map + row);
+        const uint8_t* base = reinterpret_cast<const uint8_t*>(
+            __ldg(reinterpret_cast<const unsigned long long*>(P.chunk_ptrs) + j));
+        const int64_t head_row = P.hf_layout ? (((int64_t)lk * P.H + h) * t + tok) * P.D
+                                             : (((int64_t)lk * t + tok) * P.H + h) * P.D;
+        const E* crow = reinterpret_cast<const E*>(base) + head_row;     // the chunk's row of this (token, head)
+        const int seg = kv == 0 ? __ldg(P.chunk_seg + j) : -1;
+        const float2* tab = P.cs + (int64_t)(seg < 0 ? 0 : seg) * P.half;
+        union { vec_t q; E e[VEC]; } w;
+        const bool aligned = VEC == 1 || (reinterpret_cast<uintptr_t>(base) & 15) == 0;
+        if (aligned) {
+            w.q = *reinterpret_cast<const vec_t*>(crow + v * VEC);
+            if (seg >= 0) rope_turn_vec<E, VEC>(w.e, crow, v * VEC, tab, P.half, P.rot_offset, P.neox != 0);
+        } else {                                   // a misaligned chunk: element by element, partners the same way
+#pragma unroll
+            for (int e = 0; e < VEC; ++e) {
+                w.e[e] = crow[v * VEC + e];
+                if (seg >= 0) rope_turn_vec<E, 1>(&w.e[e], crow, v * VEC + e, tab, P.half, P.rot_offset, P.neox != 0);
+            }
+        }
+        const int d0 = v * VEC;
+        if (SPLIT) {
+            const int64_t b = row / P.bs, so = row - b * P.bs;
+            if (kv == 0) {
+                E* dst = plane + (((b * P.H + h) * (P.D / X) + d0 / X) * P.bs + so) * X + d0 % X;
+                if (VEC == X) {
+                    *reinterpret_cast<vec_t*>(dst) = w.q;
+                } else {
+#pragma unroll
+                    for (int e = 0; e < VEC; ++e) plane[(((b * P.H + h) * (P.D / X) + (d0 + e) / X) * P.bs + so) * X +
+                                                        (d0 + e) % X] = w.e[e];
+                }
+            } else {
+#pragma unroll
+                for (int e = 0; e < VEC; ++e) plane[((b * P.H + h) * (int64_t)P.D + d0 + e) * P.bs + so] = w.e[e];
+            }
+        } else {
+            *reinterpret_cast<vec_t*>(plane + row * P.sT + (int64_t)h * P.sH + d0) = w.q;
+        }
+    }
+}
+
+template <class E>
+static void launch_unpack_rope(bool vec, bool split, unsigned blocks, const UnpackRopeParams& P, cudaStream_t st) {
+    constexpr int V = 16 / sizeof(E);
+    if (split) {
+        if (vec) unpack_rope_kernel<E, V, true><<<blocks, 256, 0, st>>>(P);
+        else unpack_rope_kernel<E, 1, true><<<blocks, 256, 0, st>>>(P);
+    } else {
+        if (vec) unpack_rope_kernel<E, V, false><<<blocks, 256, 0, st>>>(P);
+        else unpack_rope_kernel<E, 1, false><<<blocks, 256, 0, st>>>(P);
+    }
+}
+
 }  // namespace b200kv
 
 using namespace b200kv;
@@ -543,6 +642,71 @@ int b200kv_unpack_chunks_layers(const void* const* chunk_ptrs, int32_t n_chunks,
     B2_REQUIRE(layer_end >= 0, "bad layer range");
     return launch_pack(false, dst, tok_begin, n_chunks, chunk_tokens, last_chunk_tokens, hf_layout, layer_begin,
                        layer_end, nullptr, 0, const_cast<void* const*>(chunk_ptrs), static_cast<cudaStream_t>(stream));
+}
+
+int b200kv_unpack_chunks_layers_rope(const void* const* chunk_ptrs, int32_t n_chunks, int32_t chunk_tokens,
+                                     const int32_t* chunk_ntok, const int64_t* dst_tok, const int32_t* chunk_seg,
+                                     int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
+                                     const b200kv_kv_desc* dst, const float* cos_sin, int32_t rotary_dim, int32_t offset,
+                                     int32_t style, void* stream) {
+    B2_REQUIRE(dst != nullptr, "kv descriptor is NULL");
+    B2_REQUIRE(chunk_ptrs != nullptr && chunk_ntok != nullptr && dst_tok != nullptr && chunk_seg != nullptr,
+               "chunk_ptrs, chunk_ntok, dst_tok or chunk_seg is NULL");
+    B2_REQUIRE(cos_sin != nullptr, "cos_sin table is NULL");
+    B2_REQUIRE(style == 0 || style == 1, "style must be 0 (neox) or 1 (gptj)");
+    B2_REQUIRE(dst->L > 0 && 2 * dst->L <= B200KV_MAX_PLANES, "bad kv descriptor");
+    B2_REQUIRE(dst->H > 0 && dst->D > 0, "H/D must be positive");
+    B2_REQUIRE(0 <= layer_begin && layer_begin < layer_end && layer_end <= dst->L, "bad layer range");
+    B2_REQUIRE(n_chunks > 0 && chunk_tokens > 0, "bad chunking");
+    B2_REQUIRE(hf_layout == 0 || hf_layout == 1, "hf_layout must be 0 or 1");
+    const bool split = kv_split(dst);
+    const int dt = split ? kv_split_dtype(dst) : kv_dtype(dst);
+    B2_REQUIRE(dt == B200KV_DT_BF16 || dt == B200KV_DT_FP16,
+               "the rope unpack takes 16-bit keys only: rotating a one-byte (FP8) key would round it again");
+    B2_REQUIRE(rotary_dim > 0 && rotary_dim % 2 == 0, "rotary_dim must be even and positive");
+    B2_REQUIRE(offset >= 0 && (int64_t)offset + rotary_dim <= dst->D, "offset + rotary_dim exceeds the head size D");
+    if (split) {
+        B2_REQUIRE(!(dst->dtype & B200KV_KV_LATENT), "a latent KV has no split layout (B200KV_KV_PAGED_SPLIT)");
+        B2_REQUIRE(hf_layout == 0, "a split paged KV (B200KV_KV_PAGED_SPLIT) moves to and from vllm chunks only (hf_layout 0)");
+        B2_REQUIRE(dst->slot_map != nullptr, "a split paged KV (B200KV_KV_PAGED_SPLIT) needs a slot_map");
+        B2_REQUIRE(dst->D % 8 == 0, "a split paged KV needs D % x == 0 (x = 16 / element size)");
+        B2_REQUIRE(dst->sT > 0 && dst->sT <= (1 << 20), "block size out of range");
+    }
+    UnpackRopeParams P;
+    b200kv_kv_desc rows = *dst;                // the planes' pointers, read through the rows' table builder
+    rows.dtype = dt | (dst->dtype & B200KV_KV_LATENT);
+    float bins[B200KV_MAX_PLANES];
+    for (int i = 0; i < B200KV_MAX_PLANES; ++i) bins[i] = 32.0f;
+    if (int rc = make_plane_table(&rows, bins, bins, &P.pt)) return rc;
+    P.sT = dst->sT; P.sH = dst->sH;
+    P.slot_map = dst->slot_map;
+    P.chunk_ptrs = chunk_ptrs; P.chunk_ntok = chunk_ntok; P.dst_tok = dst_tok; P.chunk_seg = chunk_seg;
+    P.cs = reinterpret_cast<const float2*>(cos_sin);
+    P.L = dst->L; P.H = dst->H; P.D = dst->D;
+    P.n_chunks = n_chunks; P.chunk_tokens = chunk_tokens; P.hf_layout = hf_layout;
+    P.ppl = split ? 2 : kv_ppl(dst);
+    P.l0 = layer_begin; P.nl = layer_end - layer_begin;
+    P.bs = split ? (int32_t)dst->sT : 0;
+    P.half = rotary_dim / 2; P.rot_offset = offset; P.neox = style == 0;
+    constexpr int ev = 8;                      // 16-bit elements per 16-byte vector
+    const RopeArgs rope{nullptr, cos_sin, rotary_dim, offset, style};
+    // chunk pointers are device data: the kernel checks each one's alignment itself
+    bool vec = dst->D % ev == 0 && rope.vec_ok(ev) && (split || (dst->sT % ev == 0 && dst->sH % ev == 0));
+    for (int kvi = 0; kvi < P.ppl && vec; ++kvi)
+        for (int l = layer_begin; l < layer_end && vec; ++l)
+            vec = (reinterpret_cast<uintptr_t>(P.pt.p[kvi * P.L + l]) & 15) == 0;
+    const int V = vec ? ev : 1;
+    const int64_t total = (int64_t)n_chunks * P.ppl * P.nl * chunk_tokens * dst->H * (dst->D / V);
+    int dev = 0, sms = 0;
+    B2_CHECK_CUDA(cudaGetDevice(&dev));
+    B2_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    int64_t blocks = std::min<int64_t>((total + 255) / 256, (int64_t)sms * 8 * 4);
+    if (blocks < 1) blocks = 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (dt == B200KV_DT_BF16) launch_unpack_rope<__nv_bfloat16_raw>(vec, split, (unsigned)blocks, P, st);
+    else launch_unpack_rope<__half_raw>(vec, split, (unsigned)blocks, P, st);
+    B2_CHECK_CUDA(cudaGetLastError());
+    return 0;
 }
 
 int b200kv_pinned_alloc(void** host_ptr, int64_t bytes) {

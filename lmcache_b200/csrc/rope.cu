@@ -9,6 +9,8 @@
 //                      ~4e-3 rad off, far more than one bf16 ulp of the result).
 //   b200kv_rope_shift: one launch rotates channels [offset, offset + rotary_dim) of the key rows of a token range, every
 //                      layer and head, in any layout a kv_desc carries (rows, slot-mapped rows, the split key blocks).
+//   b200kv_rope_shift_layers: the same for the key planes of a layer range only (a layer-wise retrieve turns each
+//                      layer as it lands); b200kv_rope_shift is its range [0, L).
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -25,7 +27,8 @@ struct RopeParams {
     const int32_t* seg_of_tok;     // [ntok]: table row of token tok_begin + i, or -1
     const float2* cs;              // [n_seg][half]: (cos, sin)
     int64_t sT, sH, tok_begin, ntok;
-    int32_t L, H, D, half, offset, bs;   // bs: the split layout's block size
+    int32_t L, H, D, half, offset, bs;   // L: layers turned, l0 .. l0 + L - 1; bs: the split layout's block size
+    int32_t l0;
 };
 static_assert(sizeof(RopeParams) < kMaxParamBytes, "RopeParams must stay under 4 KB of kernel parameters");
 
@@ -66,7 +69,7 @@ __global__ void __launch_bounds__(256) rope_shift_kernel(RopeParams P) {
         const int h = (int)(lh % P.H), l = (int)(lh / P.H);
         const int64_t tok = P.tok_begin + i;
         const int64_t row = P.slot_map ? __ldg(P.slot_map + tok) : tok;
-        E* plane = const_cast<E*>(reinterpret_cast<const E*>(P.pt.p[l]));
+        E* plane = const_cast<E*>(reinterpret_cast<const E*>(P.pt.p[P.l0 + l]));
         const int j0 = v * NP;
         const float2* t = P.cs + (int64_t)seg * P.half + j0;
         if (NEOX) {
@@ -154,8 +157,9 @@ int b200kv_rope_table(const int64_t* shifts, int32_t n_seg, const float* inv_fre
     return 0;
 }
 
-int b200kv_rope_shift(const b200kv_kv_desc* kv, int64_t tok_begin, int64_t ntok, const int32_t* seg_of_tok,
-                      const float* cos_sin, int32_t rotary_dim, int32_t offset, int32_t style, void* stream) {
+int b200kv_rope_shift_layers(const b200kv_kv_desc* kv, int32_t layer_begin, int32_t layer_end, int64_t tok_begin,
+                             int64_t ntok, const int32_t* seg_of_tok, const float* cos_sin, int32_t rotary_dim,
+                             int32_t offset, int32_t style, void* stream) {
     B2_REQUIRE(kv != nullptr, "kv descriptor is NULL");
     B2_REQUIRE(cos_sin != nullptr, "cos_sin table is NULL");
     B2_REQUIRE(ntok >= 0 && tok_begin >= 0, "bad token range");
@@ -163,6 +167,7 @@ int b200kv_rope_shift(const b200kv_kv_desc* kv, int64_t tok_begin, int64_t ntok,
     B2_REQUIRE(style == 0 || style == 1, "style must be 0 (neox) or 1 (gptj)");
     B2_REQUIRE(kv->L > 0 && 2 * kv->L <= B200KV_MAX_PLANES, "L out of range");
     B2_REQUIRE(kv->H > 0 && kv->D > 0, "H/D must be positive");
+    B2_REQUIRE(0 <= layer_begin && layer_begin < layer_end && layer_end <= kv->L, "bad layer range");
     const bool split = kv_split(kv);
     const int dt = split ? kv_split_dtype(kv) : kv_dtype(kv);
     B2_REQUIRE(dt == B200KV_DT_BF16 || dt == B200KV_DT_FP16,
@@ -186,7 +191,8 @@ int b200kv_rope_shift(const b200kv_kv_desc* kv, int64_t tok_begin, int64_t ntok,
     P.seg_of_tok = seg_of_tok;
     P.cs = reinterpret_cast<const float2*>(cos_sin);
     P.sT = kv->sT; P.sH = kv->sH; P.tok_begin = tok_begin; P.ntok = ntok;
-    P.L = kv->L; P.H = kv->H; P.D = kv->D;
+    P.L = layer_end - layer_begin; P.H = kv->H; P.D = kv->D;
+    P.l0 = layer_begin;
     P.half = rotary_dim / 2;
     P.offset = offset;
     P.bs = split ? (int32_t)kv->sT : 0;
@@ -195,9 +201,9 @@ int b200kv_rope_shift(const b200kv_kv_desc* kv, int64_t tok_begin, int64_t ntok,
     // 16-byte aligned (the split layout keeps X = 8 channels of one token together: its strides are always aligned)
     bool vec = offset % 8 == 0 && (neox ? P.half % 8 == 0 : rotary_dim % 8 == 0) &&
                (split || (kv->sT % 8 == 0 && kv->sH % 8 == 0));
-    for (int l = 0; l < kv->L && vec; ++l) vec = (reinterpret_cast<uintptr_t>(P.pt.p[l]) & 15) == 0;
+    for (int l = layer_begin; l < layer_end && vec; ++l) vec = (reinterpret_cast<uintptr_t>(P.pt.p[l]) & 15) == 0;
     const int np = vec ? (neox ? 8 : 4) : 1;
-    const int64_t total = ntok * kv->L * kv->H * (P.half / np);
+    const int64_t total = ntok * P.L * kv->H * (P.half / np);
     int dev = 0, sms = 0;
     B2_CHECK_CUDA(cudaGetDevice(&dev));
     B2_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -208,6 +214,13 @@ int b200kv_rope_shift(const b200kv_kv_desc* kv, int64_t tok_begin, int64_t ntok,
     else launch_rope_e<__half_raw>(vec, neox, split, (unsigned)blocks, P, st);
     B2_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+int b200kv_rope_shift(const b200kv_kv_desc* kv, int64_t tok_begin, int64_t ntok, const int32_t* seg_of_tok,
+                      const float* cos_sin, int32_t rotary_dim, int32_t offset, int32_t style, void* stream) {
+    B2_REQUIRE(kv != nullptr, "kv descriptor is NULL");
+    return b200kv_rope_shift_layers(kv, 0, kv->L, tok_begin, ntok, seg_of_tok, cos_sin, rotary_dim, offset, style,
+                                    stream);
 }
 
 }  // extern "C"

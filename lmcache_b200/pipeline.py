@@ -26,7 +26,7 @@ import queue
 import threading
 import time
 from concurrent.futures import Future
-from typing import Callable, Iterable, Iterator, List, NamedTuple, Optional, Sequence
+from typing import Callable, Iterable, Iterator, List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -1186,6 +1186,38 @@ def ranged_read_plan(fixed: np.ndarray, start: np.ndarray, size: np.ndarray, got
     return reads
 
 
+def match_runs(runs: Sequence[Tuple[Iterable, Optional[Callable[[int], Iterable]], int]], chunk_size: int,
+               fits: Callable[[object, int], bool]) -> List[Tuple[List[Tuple[object, int]], int]]:
+    """The match of a multi-run fetch (get_kv_layerwise_runs), on the calling thread.  Each run is (primary items,
+    fallback(i) -> the items that continue it from its chunk i (None: no continuation), destination token of its chunk
+    0).  A run takes its primary items up to the first miss -- None, or an item that fits(item, destination token)
+    refuses -- then fallback(k) from that index k on, up to their first miss.  A miss ends only its own run.  Returns
+    per run ([(item, destination token)], number of primary items among them)."""
+    out = []
+    for primary, fallback, tok0 in runs:
+        got: List[Tuple[object, int]] = []
+        own = None
+        for src in (primary, None):
+            if src is None:
+                own = len(got)
+                if fallback is None:
+                    break
+                src = fallback(own)
+            for it in src:
+                tok = tok0 + len(got) * chunk_size
+                if it is None or not fits(it, tok):
+                    break
+                got.append((it, tok))
+        out.append((got, len(got) if own is None else own))
+    return out
+
+
+def rest_runs(runs: Sequence[Tuple[Sequence, int]], hits: Sequence[int], chunk_size: int) -> List[Tuple[Sequence, int]]:
+    """What another tier is asked for after one served `hits[i]` chunks of each run (keys, destination token of its
+    chunk 0): the keys after them, at the token after them.  Each chunk of a run is served by one tier only."""
+    return [(keys[h:], tok0 + h * chunk_size) for (keys, tok0), h in zip(runs, hits)]
+
+
 def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, records: Iterable[Optional[HostContainer]],
                             dst: KvView, dst_tok0: int, chunk_size: int, release: Optional[DeferredFree] = None,
                             on_done: Optional[Callable[[], None]] = None,
@@ -1211,20 +1243,41 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
     `host_ready(l)`: the records' blocks are still being filled (a ranged remote read, RangedFetch.wait): the worker
     calls it before it enqueues the fixed sections (l = 0) and before each layer l's copy, and it returns once the bytes
     those copies read are in host memory, or raises -- which fails the upload."""
+    return upload_decode_layerwise_runs(codec, uploader, [(records, None, dst_tok0)], dst, chunk_size, release, on_done,
+                                        level, host_ready)[1]
+
+
+def upload_decode_layerwise_runs(codec: CacheGenCodec, uploader: LayerwiseUploader,
+                                 runs: Sequence[Tuple[Iterable[Optional[HostContainer]],
+                                                      Optional[Callable[[int], Iterable[Optional[HostContainer]]]], int]],
+                                 dst: KvView, chunk_size: int, release: Optional[DeferredFree] = None,
+                                 on_done: Optional[Callable[[], None]] = None, level: Optional[DeviceLevel] = None,
+                                 host_ready: Optional[Callable[[int], None]] = None, rotation=None):
+    """upload_decode_layerwise of several runs of chunks, each at its own destination (match_runs: a run is its
+    records, a callable that continues it from chunk i with other records or None, and its destination token), in one
+    upload: each layer is copied and decoded for every chunk of every run before the next layer.  Every record matches
+    against the first one of the call.  `rotation` (rope.Rotation, whose rows are per run): the keys of layer l of the
+    chunks written are turned on the decode stream after layer l's decode, before its ready event.  Returns ([(primary
+    hits, fallback hits)] per run, LayerwiseUpload)."""
     matched: List[HostContainer] = []
     L = dst.L
     submitted = False
     try:
         first = None
-        for r in records:
-            if r is None:
-                break
-            if not _continues_match(r, first, dst, dst_tok0 + len(matched) * chunk_size):
+
+        def fits(r: HostContainer, tok: int) -> bool:
+            nonlocal first
+            if not _continues_match(r, first, dst, tok):
                 if release is not None and r.blk is not None:
                     r.blk.free()
-                break
+                return False
             first = first or r
-            matched.append(r)
+            matched.append(r)                  # runs match one after another: matched is in run order
+            return True
+        per_run = match_runs(runs, chunk_size, fits)
+        hits = [(own, len(got) - own) for got, own in per_run]
+        placed = [(k, tok, r.ntokens) for k, (got, _) in enumerate(per_run) for r, tok in got]
+        dst_tok = [tok for got, _ in per_run for _, tok in got]
         n = len(matched)
         res_j = [j for j, r in enumerate(matched) if level is not None and level.resident(r)]
         up_j = [j for j in range(n) if j not in res_j] if res_j else list(range(n))
@@ -1239,7 +1292,7 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
                 submitted = True
                 if on_done is not None:
                     on_done()
-                return LayerwiseUpload.completed(0, L, start)
+                return hits, LayerwiseUpload.completed(0, L, start)
             offs, o = [], 0
             for r in up:
                 offs.append(o)
@@ -1250,6 +1303,10 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
                 staging.record_stream(uploader.copy_stream)
                 staging.record_stream(uploader.decode_stream)
             dst.record_stream(uploader.decode_stream)
+            rot = None if rotation is None else rotation.prepare(placed, dst.device)
+            if rot is not None:
+                rot.record_stream(uploader.decode_stream)
+                start.record(torch.cuda.current_stream())       # after the upload of its seg_of_tok
 
         if up:
             base = staging.data_ptr()
@@ -1262,7 +1319,6 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
             lay_src = np.ascontiguousarray(np.tile(np.concatenate([host] * k), (L, 1)) + lo.astype(np.uint64))
             lay_dst = np.ascontiguousarray(np.tile(np.concatenate([dev] * k), (L, 1)) + lo.astype(np.uint64))
         upload = LayerwiseUpload(n, L)
-        dst_tok = [dst_tok0 + j * chunk_size for j in range(n)]
 
         def job():
             cs, ds = uploader.copy_stream, uploader.decode_stream
@@ -1308,6 +1364,8 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
                             ds.wait_event(last)
                         for plan, _ in plans:
                             codec.decode_layers(plan, layer, layer + 1, ds)
+                        if rot is not None:
+                            rot.shift_layer(dst, layer, ds)
                         ev = torch.cuda.Event(enable_timing=True)     # a caller may time the layers against each other
                         ev.record(ds)
                         upload._publish(ev)
@@ -1334,7 +1392,7 @@ def upload_decode_layerwise(codec: CacheGenCodec, uploader: LayerwiseUploader, r
 
         uploader.submit(job)
         submitted = True
-        return upload
+        return hits, upload
     finally:
         if not submitted:                             # failed before the worker took over: nothing was enqueued
             if release is not None:

@@ -14,8 +14,9 @@ from __future__ import annotations
 
 import ctypes
 import hashlib
-from typing import Callable, List, NamedTuple, Sequence, Tuple
+from typing import Callable, List, NamedTuple, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from lmcache_b200 import _native as N
@@ -158,6 +159,87 @@ def rope_shift(view, tok_begin: int, seg: torch.Tensor, shifts: torch.Tensor, ro
         N.check(N.lib().b200kv_rope_shift(ctypes.byref(view.desc), tok_begin, seg.numel(),
                                           ctypes.c_void_p(seg.data_ptr()), ctypes.c_void_p(table.data_ptr()),
                                           rope.rotary_dim, rope.offset, STYLES[rope.style], st), "rope_shift")
+
+
+def rope_shift_layers(view, layer_begin: int, layer_end: int, tok_begin: int, seg: torch.Tensor, table: torch.Tensor,
+                      rope: RopeSpec, stream: torch.cuda.Stream) -> None:
+    """rope_shift of the key planes of layers [layer_begin, layer_end) only, by a prepared table (rope_table's), on
+    `stream`: one b200kv_rope_shift_layers launch"""
+    N.check(N.lib().b200kv_rope_shift_layers(ctypes.byref(view.desc), layer_begin, layer_end, tok_begin, seg.numel(),
+                                             ctypes.c_void_p(seg.data_ptr()), ctypes.c_void_p(table.data_ptr()),
+                                             rope.rotary_dim, rope.offset, STYLES[rope.style], stream.cuda_stream),
+            "rope_shift_layers")
+
+
+def written_seg_of_tok(chunks: Sequence[Tuple[int, int, int]], run_rows: Sequence[int],
+                       run_ends: Sequence[int]) -> Tuple[int, np.ndarray]:
+    """The shift's arguments for the chunks a multi-run fetch wrote, (run, destination token, tokens) each:
+    (lo, int32 seg_of_tok of tokens [lo, lo + len)).  A chunk of run r turns by table row run_rows[r], its tokens
+    clipped to the run's end run_ends[r]; -1 (a segment at token 0) leaves it alone, like every token no chunk wrote.
+    Empty when nothing turns.  The runs are segments of one plan, which never overlap (plan_segments)."""
+    turned = [(tok, min(tok + n, run_ends[r]), run_rows[r]) for r, tok, n in chunks if run_rows[r] >= 0]
+    turned = [t for t in turned if t[1] > t[0]]
+    if not turned:
+        return 0, np.zeros(0, np.int32)
+    lo, hi = min(a for a, _, _ in turned), max(b for _, b, _ in turned)
+    sot = np.full(hi - lo, -1, dtype=np.int32)
+    for a, b, k in turned:
+        sot[a - lo:b - lo] = k
+    return lo, sot
+
+
+def chunk_arrays(chunks: Sequence[Tuple[int, int, int]], run_rows: Sequence[int]):
+    """The per-chunk arguments of b200kv_unpack_chunks_layers_rope for the chunks a multi-run fetch wrote, (run,
+    destination token, tokens) each: (chunk_ntok int32, dst_tok int64, chunk_seg int32), chunk_seg the run's table row
+    (-1: a segment at token 0, copied)."""
+    return (np.array([n for _, _, n in chunks], dtype=np.int32), np.array([t for _, t, _ in chunks], dtype=np.int64),
+            np.array([run_rows[r] for r, _, _ in chunks], dtype=np.int32))
+
+
+def unpack_rope_layers(view, table_ptr: int, arrays, chunk_tokens: int, layer_begin: int, layer_end: int,
+                       rot: "Rotation", stream: torch.cuda.Stream) -> None:
+    """one b200kv_unpack_chunks_layers_rope launch on `stream`: chunk j's layer range starts at the device pointer
+    table_ptr[j]; arrays: device (chunk_ntok, dst_tok, chunk_seg) of chunk_arrays"""
+    ntok, dst_tok, seg = arrays
+    N.check(N.lib().b200kv_unpack_chunks_layers_rope(
+        ctypes.c_void_p(table_ptr), ntok.numel(), chunk_tokens, ctypes.c_void_p(ntok.data_ptr()),
+        ctypes.c_void_p(dst_tok.data_ptr()), ctypes.c_void_p(seg.data_ptr()), int(view.fmt == "huggingface"),
+        layer_begin, layer_end, ctypes.byref(view.desc), ctypes.c_void_p(rot.table.data_ptr()), rot.rope.rotary_dim,
+        rot.rope.offset, STYLES[rot.rope.style], stream.cuda_stream), "unpack_chunks_layers_rope")
+
+
+class Rotation:
+    """The turn a layer-major multi-run fetch (a tier's get_kv_layerwise_runs) gives the keys it writes: the chunks of
+    run r turn by row run_rows[r] of `table` (rope_table's: one row per segment that does not start at token 0; -1 for
+    one that does), up to the run's segment end run_ends[r].  The tier turns each layer on the stream that wrote it,
+    before that layer's ready event."""
+
+    def __init__(self, rope: RopeSpec, table: torch.Tensor, run_rows: Sequence[int], run_ends: Sequence[int]):
+        self.rope, self.table, self.run_rows, self.run_ends = rope, table, list(run_rows), list(run_ends)
+
+    def prepare(self, chunks: Sequence[Tuple[int, int, int]], device) -> Optional["PreparedRotation"]:
+        """The rotation of the chunks a fetch matched, (run, destination token, tokens) each, or None when none of them
+        turns.  Its seg_of_tok is uploaded on the current stream: call it before the fetch's start event."""
+        lo, sot = written_seg_of_tok(chunks, self.run_rows, self.run_ends)
+        if not len(sot):
+            return None
+        return PreparedRotation(self, lo, torch.from_numpy(sot).to(device, non_blocking=True))
+
+
+class PreparedRotation:
+    def __init__(self, rot: Rotation, lo: int, seg: torch.Tensor):
+        self.rot, self.lo, self.seg = rot, lo, seg
+
+    def shift_layers(self, view, layer_begin: int, layer_end: int, stream: torch.cuda.Stream) -> None:
+        """turn the written keys of layers [layer_begin, layer_end) on `stream` (the stream that wrote them)"""
+        rope_shift_layers(view, layer_begin, layer_end, self.lo, self.seg, self.rot.table, self.rot.rope, stream)
+
+    def shift_layer(self, view, layer: int, stream: torch.cuda.Stream) -> None:
+        self.shift_layers(view, layer, layer + 1, stream)
+
+    def record_stream(self, stream: torch.cuda.Stream) -> None:
+        self.seg.record_stream(stream)
+        self.rot.table.record_stream(stream)
 
 
 def pack_rope(view, blob: torch.Tensor, seg: torch.Tensor, table: torch.Tensor, rope: RopeSpec) -> None:

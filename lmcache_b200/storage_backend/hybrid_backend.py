@@ -182,6 +182,54 @@ class LMCHybridBackend(LMCBackendInterface):
             self._get_part(self.remote_store, keys[n:], dst, dst_tok0 + n * chunk_size, chunk_size, parts)
         return join_uploads(parts, dst.L)
 
+    def get_kv_layerwise_runs(self, runs, dst, chunk_size: int, rotation=None):
+        """get_kv_layerwise_runs as get_kv_into would serve each run: its keys from the local tier, then from the remote
+        tier where the local one missed; then (when the keys missed) its fallback keys the same way.  Each part is one
+        multi-run get of one tier (a tier that cannot go layer-major decodes its part chunk-major), each chunk is in
+        exactly one part, and each part turns only the rows it wrote (`rotation`).  Returns ([(key hits, fallback
+        hits)] per run, one handle whose ready(l) comes after every part's layer l)."""
+        from lmcache_b200.pipeline import join_uploads
+        parts: list = []
+        own = self._runs_parts([(keys, tok0) for keys, _, tok0 in runs], dst, chunk_size, rotation, parts)
+        fb = [(f[h:] if f is not None and h < len(f) else [], tok0 + h * chunk_size)
+              for (_, f, tok0), h in zip(runs, own)]
+        more = self._runs_parts(fb, dst, chunk_size, rotation, parts)
+        return list(zip(own, more)), join_uploads(parts, dst.L)
+
+    def _runs_parts(self, runs, dst, chunk_size: int, rotation, parts: list) -> list:
+        """runs of (keys, destination token) from the local tier, then their rest (rest_runs) from the remote tier;
+        returns the hits per run"""
+        from lmcache_b200.pipeline import rest_runs
+        hits = [0] * len(runs)
+        for store in (self.local_store, self.remote_store):
+            if any(len(keys) for keys, _ in runs):
+                n = self._runs_part(store, runs, dst, chunk_size, rotation, parts)
+                hits = [h + m for h, m in zip(hits, n)]
+                runs = rest_runs(runs, n, chunk_size)
+        return hits
+
+    @staticmethod
+    def _runs_part(store, runs, dst, chunk_size: int, rotation, parts: list) -> list:
+        from lmcache_b200.pipeline import LayerwiseUpload
+        f = getattr(store, "get_kv_layerwise_runs", None)
+        if f is not None and store.supports_layerwise_get() and \
+                chunk_size <= getattr(store, "layerwise_max_tokens", N.GROUP_TOKENS):
+            hits, up = f([(keys, None, tok0) for keys, tok0 in runs], dst, chunk_size, rotation)
+            parts.append(up)
+            return [h for h, _ in hits]
+        # chunk-major: every run through get_kv_into, then the rows written turned for every layer at once
+        n = [store.get_kv_into(keys, dst, tok0, chunk_size) if len(keys) else 0 for keys, tok0 in runs]
+        stream = torch.cuda.current_stream()
+        rot = None if rotation is None else rotation.prepare(
+            [(r, tok0 + j * chunk_size, min(chunk_size, dst.ntokens - tok0 - j * chunk_size))
+             for r, ((_, tok0), m) in enumerate(zip(runs, n)) for j in range(m)], dst.device)
+        if rot is not None:
+            rot.shift_layers(dst, 0, dst.L, stream)
+        ev = torch.cuda.Event()
+        ev.record(stream)
+        parts.append(LayerwiseUpload.completed(sum(n), dst.L, ev))
+        return n
+
     @staticmethod
     def _get_part(store, keys, dst, dst_tok0: int, chunk_size: int, parts: list) -> int:
         from lmcache_b200.pipeline import LayerwiseUpload

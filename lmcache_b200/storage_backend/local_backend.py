@@ -444,24 +444,44 @@ class LMCLocalBackend(LMCBackendInterface):
         (cuda tier), or (cpu tier) from a device slot of a LAYER_SLOTS ring that one batched copy on the copy stream
         has filled with the layer's slice of every chunk, so that layer l + 1's copy runs while layer l is unpacked.
         Everything is enqueued before this returns; the host never waits."""
-        from lmcache_b200.pipeline import LayerwiseUpload, _batch_copy
+        return self.get_kv_layerwise_runs([(keys, None, dst_tok0)], dst, chunk_size)[1]
+
+    def get_kv_layerwise_runs(self, runs, dst, chunk_size: int, rotation=None):
+        """get_kv_layerwise of several runs in one upload: each run is (keys, fallback keys or None, destination token
+        of its chunk 0), and takes its keys up to the first miss, then its fallback keys from that index on
+        (pipeline.match_runs).  Each layer is unpacked for every hit chunk of every run before the next layer.
+        `rotation` (rope.Rotation): each layer of every chunk is unpacked with its keys turned by its run's table row in
+        one b200kv_unpack_chunks_layers_rope launch, on the mover stream, before layer l's ready event.  Returns ([(key hits, fallback hits)] per
+        run, LayerwiseUpload)."""
+        from lmcache_b200.pipeline import LayerwiseUpload, _batch_copy, match_runs
         t0 = time.perf_counter()
         L = dst.L
-        hits = []                                            # (stored value, source blob, tokens)
-        for i, key in enumerate(keys):
-            val = self.dict.get(key, None)
-            if val is None:
-                break
+
+        def fits(val, tok: int) -> bool:
             src = val.host if isinstance(val, _HostEntry) else val
             if src.dim() != (3 if dst.latent else 5):
-                break                                       # a chunk of the other kind (latent / (K, V)): a miss
+                return False                                # a chunk of the other kind (latent / (K, V)): a miss
             t = src.shape[KvView.token_dim(dst.fmt, dst.latent)]
-            tok = dst_tok0 + i * chunk_size
             if tok + t > dst.ntokens or src.dtype != dst.dtype:
-                break
-            if src.numel() != dst.planes * dst.H * dst.D * t:
-                break                                       # another geometry: its slices are not this KV's layers
-            hits.append((val, src, t))
+                return False
+            # another geometry: its slices are not this KV's layers
+            return src.numel() == dst.planes * dst.H * dst.D * t
+        per_run = match_runs([(map(self.dict.get, keys), None if fb is None else (lambda i, fb=fb: map(self.dict.get, fb[i:])),
+                               tok0) for keys, fb, tok0 in runs], chunk_size, fits)
+        hit_counts = [(own, len(got) - own) for got, own in per_run]
+        hits = []                                            # (stored value, source blob, tokens)
+        placed = []                                          # (run, destination token, tokens)
+        mover_runs = []                                      # (chunk_runs entry over the call's chunks, token of its first)
+        for k, (got, _) in enumerate(per_run):
+            base = len(hits)
+            for val, tok in got:
+                src = val.host if isinstance(val, _HostEntry) else val
+                t = src.shape[KvView.token_dim(dst.fmt, dst.latent)]
+                hits.append((val, src, t))
+                placed.append((k, tok, t))
+            if got:
+                for a, b, ct, lt in chunk_runs([h[2] for h in hits[base:]], chunk_size):
+                    mover_runs.append(((base + a, base + b, ct, lt), got[a][1]))
         n = len(hits)
         with torch.cuda.device(dst.device):
             srcs = []
@@ -472,11 +492,20 @@ class LMCLocalBackend(LMCBackendInterface):
                 elif not src.is_cuda or not src.is_contiguous():
                     src = src.contiguous().to(dst.device)        # on the current stream, before `start`
                 srcs.append(src)
+            fused = None            # with a rotation: one fused unpack-and-turn launch per layer over every chunk
+            if rotation is not None and n:
+                from lmcache_b200.rope import chunk_arrays
+                fused = tuple(torch.from_numpy(a).to(dst.device, non_blocking=True)
+                              for a in chunk_arrays(placed, rotation.run_rows))
             start = torch.cuda.Event()
             start.record(torch.cuda.current_stream())
             if n == 0:
-                return LayerwiseUpload.completed(0, L, start)
+                return hit_counts, LayerwiseUpload.completed(0, L, start)
             ms, cs = self._layer_streams(dst.device)
+            if fused is not None:
+                for a in fused:
+                    a.record_stream(ms)
+                rotation.table.record_stream(ms)
             ms.wait_event(start)
             cs.wait_event(start)
             for val, _, _ in hits:
@@ -485,7 +514,6 @@ class LMCLocalBackend(LMCBackendInterface):
             dst.record_stream(ms)
             tokens = [t for _, _, t in hits]
             row = layer_row_bytes(dst.H, dst.D, dst.dtype.itemsize, dst.latent)
-            runs = chunk_runs(tokens, chunk_size)
             bases = np.array([s.data_ptr() for s in srcs], dtype=np.uint64)
             host = self.device != "cuda"
             if host:
@@ -520,8 +548,12 @@ class LMCLocalBackend(LMCBackendInterface):
                     tp = table[slot].data_ptr()
                 else:
                     tp = table[layer].data_ptr()
-                for run in runs:
-                    _mover_layers(False, dst, tp, dst_tok0 + run[0] * chunk_size, run, layer, ms)
+                if fused is not None:
+                    from lmcache_b200.rope import unpack_rope_layers
+                    unpack_rope_layers(dst, tp, fused, max(tokens), layer, layer + 1, rotation, ms)
+                else:
+                    for run, tok in mover_runs:
+                        _mover_layers(False, dst, tp, tok, run, layer, ms)
                 ev = torch.cuda.Event(enable_timing=True)     # a caller may time the layers against each other
                 ev.record(ms)
                 upload._publish(ev)
@@ -530,7 +562,7 @@ class LMCLocalBackend(LMCBackendInterface):
                 upload.wait_s.append(0.0)
             if host:
                 self._keep_until(copied, srcs)
-        return upload
+        return hit_counts, upload
 
     def close(self):
         for val in list(self.dict.values()):
@@ -922,6 +954,20 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         return upload_decode_layerwise(self.codec, self._layerwise_uploader(dst.device), self._pinned_records(keys, pinned),
                                        dst, dst_tok0, chunk_size, on_done=lambda: self._unpin(pinned),
                                        level=self._level(dst.device, pinned))
+
+    def get_kv_layerwise_runs(self, runs, dst, chunk_size: int, rotation=None):
+        """get_kv_layerwise of several runs in one upload (pipeline.upload_decode_layerwise_runs): each run is (keys,
+        fallback keys or None, destination token of its chunk 0); a run takes its keys up to the first miss, then its
+        fallback keys from that index on.  `rotation` (rope.Rotation) turns the keys of the chunks written, layer by
+        layer.  Returns ([(key hits, fallback hits)] per run, LayerwiseUpload).  The device level is neither read nor
+        filled here (its chunks are decoded from their host copies, which an inclusive level keeps)."""
+        from lmcache_b200.pipeline import upload_decode_layerwise_runs
+        pinned = []
+        recs = [(self._pinned_records(keys, pinned),
+                 None if fb is None else (lambda i, fb=fb: self._pinned_records(fb[i:], pinned)), tok0)
+                for keys, fb, tok0 in runs]
+        return upload_decode_layerwise_runs(self.codec, self._layerwise_uploader(dst.device), recs, dst, chunk_size,
+                                            on_done=lambda: self._unpin(pinned), rotation=rotation)
 
     def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int):
         """A pipeline.LayerwiseEncode of tokens [tok_begin, T) of `view` (whose KV may not be written yet), or None
@@ -1361,6 +1407,20 @@ class LMCLocalDiskBackend(LMCLocalCompressedBackend):
                                            chunk_size, self._release,
                                            on_done=None if level is None else (lambda: self._unpin(level.entries)),
                                            level=level)
+
+    def get_kv_layerwise_runs(self, runs, dst, chunk_size: int, rotation=None):
+        """LMCLocalCompressedBackend.get_kv_layerwise_runs over container files: every run's files are read on the
+        reader pool (a fallback's once its run has missed), and the device level is not used."""
+        import contextlib
+
+        from lmcache_b200.pipeline import fetched_in_order, upload_decode_layerwise_runs
+        self._release.sweep()
+        with contextlib.ExitStack() as opened:
+            def recs(keys):
+                return opened.enter_context(contextlib.closing(fetched_in_order(self._reads(keys, None))))
+            srcs = [(recs(keys), None if fb is None else (lambda i, fb=fb: recs(fb[i:])), tok0) for keys, fb, tok0 in runs]
+            return upload_decode_layerwise_runs(self.codec, self._layerwise_uploader(dst.device), srcs, dst, chunk_size,
+                                                self._release, rotation=rotation)
 
     def host_bytes(self) -> int:
         return sum(e.rec.nbytes for e in self.dict.values() if e.rec is not None)

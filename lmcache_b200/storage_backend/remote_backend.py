@@ -597,8 +597,16 @@ class LMCRemoteBackend(LMCBackendInterface):
         pipeline.LayerwiseUpload: n is known, ready(l) is the event after layer l's decode.  Every matched container
         sits in page-locked memory until its last copy.  A failed READ fails the upload: ready(l) raises for the layers
         not yet published (n was promised already), the blocks and handles are released."""
+        return self.get_kv_layerwise_runs([(keys, None, dst_tok0)], dst, chunk_size)[1]
+
+    def get_kv_layerwise_runs(self, runs, dst, chunk_size: int, rotation=None):
+        """get_kv_layerwise of several runs in one ranged fetch and one upload: each run is (keys, fallback keys or None,
+        destination token of its chunk 0).  A run's keys are OPENed and matched as get_kv_layerwise matches them, then
+        (when it missed) its fallback keys from that index on; every container matches against the call's first one.
+        `rotation` (rope.Rotation) turns the keys of the chunks written, layer by layer, after each layer's decode
+        (pipeline.upload_decode_layerwise_runs).  Returns ([(key hits, fallback hits)] per run, LayerwiseUpload)."""
         from lmcache_b200.pipeline import (LayerwiseUpload, _continues_match, layer_copy_ranges, ranged_read_plan,
-                                           upload_decode_layerwise, wave_chunks_default)
+                                           upload_decode_layerwise_runs, wave_chunks_default)
         self._release.sweep()
         codec = self.deserializer.codec
         conns = self._lw_connections()
@@ -607,80 +615,98 @@ class LMCRemoteBackend(LMCBackendInterface):
         prefix = codec.plan_prefix(dst.L, dst.H, dst.D, chunk_size, dst.latent)     # the fixed sections of a full chunk
         bound = (self.deserializer.container_bound(dst.L, dst.H, dst.D, chunk_size, dst.latent) + 255) & ~255
         peek, self._peek = self._peek, None
-        if peek is not None and not (len(keys) and peek[0] == keys[0]):
+        keys0 = runs[0][0] if runs else []
+        if peek is not None and not (len(keys0) and peek[0] == keys0[0]):
             peek[1].blk.free()
             peek = None
         window = max(2 * k, 2 * wave_chunks_default())
-        pending: "collections.deque" = collections.deque()
-        keys_it = enumerate(keys)
-        recs, handles, got = [], [], []
+        recs, handles, got, conn_of = [], [], [], []
         stale = collections.defaultdict(list)          # handles past the match, per connection
 
-        def fill():
-            while len(pending) < window:
-                try:
-                    j, key = next(keys_it)
-                except StopIteration:
-                    return
-                if j == 0 and peek is not None:
-                    f = Future()
-                    f.set_result((peek[1], None, peek[1].nbytes))    # fetched whole by peek_geometry: used as it is
-                else:
-                    f = pool.submit(self._open, conns[j % k], key, prefix, bound)
-                pending.append((j, f))
-
-        def drop(j, rec, h):
+        def drop(c, rec, h):
             if rec is not None:
                 rec.blk.free()
             if h is not None:
-                stale[j % k].append(h)
-        try:
-            fill()
-            while pending:
-                j, f = pending.popleft()
-                rec, h, g = f.result()
-                if rec is None or not _continues_match(rec, recs[0] if recs else None, dst,
-                                                       dst_tok0 + len(recs) * chunk_size):
-                    drop(j, rec, h)
-                    break
-                recs.append(rec)
-                handles.append(h)
-                got.append(g)
+                stale[c].append(h)
+
+        def match(keys, tok0: int, use_peek: bool) -> int:
+            """OPEN `keys` in chain order over the k connections and append their records up to the first miss"""
+            pending: "collections.deque" = collections.deque()
+            keys_it = enumerate(keys)
+            n0 = len(recs)
+
+            def fill():
+                while len(pending) < window:
+                    try:
+                        j, key = next(keys_it)
+                    except StopIteration:
+                        return
+                    if j == 0 and use_peek and peek is not None:
+                        f = Future()
+                        f.set_result((peek[1], None, peek[1].nbytes))    # fetched whole by peek_geometry: used as it is
+                    else:
+                        f = pool.submit(self._open, conns[j % k], key, prefix, bound)
+                    pending.append((j, f))
+            try:
                 fill()
+                while pending:
+                    j, f = pending.popleft()
+                    rec, h, g = f.result()
+                    if rec is None or not _continues_match(rec, recs[0] if recs else None, dst,
+                                                           tok0 + (len(recs) - n0) * chunk_size):
+                        drop(j % k, rec, h)
+                        break
+                    recs.append(rec)
+                    handles.append(h)
+                    got.append(g)
+                    conn_of.append(j % k)
+                    fill()
+            finally:
+                for j, f in pending:
+                    drop(j % k, *f.result()[:2])
+            return len(recs) - n0
+
+        bounds = []                                    # per run: its records are recs[a:b] (keys), recs[b:c] (fallback)
+        try:
+            for i, (keys, fb, tok0) in enumerate(runs):
+                a = len(recs)
+                own = match(keys, tok0, i == 0)
+                if fb is not None and own < len(fb):
+                    match(fb[own:], tok0 + own * chunk_size, False)
+                bounds.append((a, a + own, len(recs)))
         except BaseException:
-            for rec, h, j in zip(recs, handles, range(len(recs))):
-                drop(j, rec, h)
+            for c, rec, h in zip(conn_of, recs, handles):
+                drop(c, rec, h)
             recs = []
             raise
         finally:
-            for j, f in pending:
-                drop(j, *f.result()[:2])
             for c, hs in stale.items():
                 try:
                     conns[c].close_handles(hs)
                 except Exception:      # noqa: BLE001 -- a lost connection has dropped its handles
                     pass
         n = len(recs)
+        hits = [(b - a, c - b) for a, b, c in bounds]
         self._count(retrieves=1, opens=sum(h is not None for h in handles), match_s=time.perf_counter() - t_match,
                     bytes=sum(g for g, h in zip(got, handles) if h is not None))
         if n == 0:
             with torch.cuda.device(dst.device):
                 ev = torch.cuda.Event()
                 ev.record(torch.cuda.current_stream())
-            return LayerwiseUpload.completed(0, dst.L, ev)
+            return hits, LayerwiseUpload.completed(0, dst.L, ev)
         L = dst.L
         try:
             fixed, start, size = layer_copy_ranges([r.planes for r in recs], [r.nbytes for r in recs], L,
                                                    dst.planes // L, codec.raw_rows(recs, dst.latent))
-            reads = ranged_read_plan(fixed, start, size, got, [j % k for j in range(n)], k)
+            reads = ranged_read_plan(fixed, start, size, got, conn_of, k)
             fetch = RangedFetch(conns, reads, handles, [r.blk.host_ptr for r in recs], L, self._count)
             fetch.start(self._lw_pool)
         except BaseException:                 # nothing reads the blocks yet: free them, close the handles
             left = collections.defaultdict(list)
-            for j, (rec, h) in enumerate(zip(recs, handles)):
+            for c, rec, h in zip(conn_of, recs, handles):
                 rec.blk.free()
                 if h is not None:
-                    left[j % k].append(h)
+                    left[c].append(h)
             for c, hs in left.items():
                 try:
                     conns[c].close_handles(hs)
@@ -693,8 +719,10 @@ class LMCRemoteBackend(LMCBackendInterface):
                 fetch.finish()
             finally:
                 self._release.add(recs[0].last_read, [r.blk for r in recs])
-        return upload_decode_layerwise(codec, self._layerwise_uploader(dst.device), iter(recs), dst, dst_tok0,
-                                       chunk_size, on_done=done, host_ready=fetch.wait)
+        matched = [(iter(recs[a:b]), (lambda i, rest=recs[b:c]: iter(rest)) if c > b else None, run[2])
+                   for (a, b, c), run in zip(bounds, runs)]
+        return upload_decode_layerwise_runs(codec, self._layerwise_uploader(dst.device), matched, dst, chunk_size,
+                                            on_done=done, host_ready=fetch.wait, rotation=rotation)
 
     def close(self):
         if getattr(self, "_layerwise", None) is not None:
