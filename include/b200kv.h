@@ -638,6 +638,25 @@ int b200kv_unpack_chunks_layers_rope(const void* const* chunk_ptrs, int32_t n_ch
 int b200kv_rope_shift_layers(const b200kv_kv_desc* kv, int32_t layer_begin, int32_t layer_end, int64_t tok_begin,
                              int64_t ntok, const int32_t* seg_of_tok, const float* cos_sin, int32_t rotary_dim,
                              int32_t offset, int32_t style, void* stream);
+/* The pack direction of b200kv_unpack_chunks_layers_rope: chunk j takes chunk_ntok[j] tokens (DEVICE int32, 1 ..
+ * chunk_tokens) from view token src_tok[j] (DEVICE int64) and writes layers [layer_begin, layer_end) of them to
+ * chunk_ptrs[j] (DEVICE array; device or mapped pinned memory) in b200kv_pack_chunks_layers' chunk layout ([2,t,H,D],
+ * [2,H,t,D] with hf_layout, [t,D] for a latent KV, per layer, t = chunk_ntok[j]); the rotary channels of its key
+ * planes turn by table row chunk_seg[j] (DEVICE int32; -1: copied).  A layer-wise segment store stages one layer of
+ * every segment in one launch, each turned back by -start.  Every source b200kv_pack_chunks_rope takes (blobs, tuples,
+ * latent views, slot-mapped and block-strided rows, B200KV_KV_PAGED_SPLIT).  Each key element reads its rotation
+ * partner from the source, which is never written, with b200kv_rope_shift's arithmetic: the result is bit-identical to
+ * b200kv_pack_chunks_rope of the same tokens restricted to the range, and to b200kv_pack_chunks_layers followed by
+ * b200kv_rope_shift_layers of the packed chunk.  V planes, other channels and other layers' planes are neither read
+ * nor written.  A misaligned chunk pointer is written element by element.  < 0, nothing enqueued: NULL arrays, what
+ * b200kv_rope_shift_layers refuses (one-byte dtypes, an odd or non-positive rotary_dim, offset < 0 or offset +
+ * rotary_dim > D, a NULL cos_sin, a bad style or layer range) and what b200kv_pack_chunks_layers refuses.  The device
+ * arrays are not bounds-checked.  Added without changing anything that existed (b200kv_version() stays 4). */
+int b200kv_pack_chunks_layers_rope(const b200kv_kv_desc* src, int32_t n_chunks, int32_t chunk_tokens,
+                                   const int32_t* chunk_ntok, const int64_t* src_tok, const int32_t* chunk_seg,
+                                   int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
+                                   void* const* chunk_ptrs, const float* cos_sin, int32_t rotary_dim,
+                                   int32_t offset, int32_t style, void* stream);
 /* b200kv_pack_chunks with the keys turned on the way (a segment of a longer prompt stored as if prefilled alone: its
  * keys turned by -start): the same descriptors (blobs, tuples, latent views, slot-mapped and block-strided rows,
  * B200KV_KV_PAGED_SPLIT), chunk layouts and destinations (device or mapped pinned memory) as b200kv_pack_chunks, in one

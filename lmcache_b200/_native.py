@@ -164,6 +164,8 @@ SIGNATURES = {
     "b200kv_rope_shift": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i64, c_vp, c_vp, c_i32, c_i32, c_i32, c_vp]),
     "b200kv_unpack_chunks_layers_rope": (c_i32, [c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32,
                                                  ctypes.POINTER(KvDesc), c_vp, c_i32, c_i32, c_i32, c_vp]),
+    "b200kv_pack_chunks_layers_rope": (c_i32, [ctypes.POINTER(KvDesc), c_i32, c_i32, c_vp, c_vp, c_vp, c_i32, c_i32,
+                                               c_i32, c_vp, c_vp, c_i32, c_i32, c_i32, c_vp]),
     "b200kv_rope_shift_layers": (c_i32, [ctypes.POINTER(KvDesc), c_i32, c_i32, c_i64, c_i64, c_vp, c_vp, c_i32, c_i32,
                                          c_i32, c_vp]),
     "b200kv_pack_chunks_rope": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp,

@@ -14,7 +14,7 @@ from __future__ import annotations
 import ctypes
 import threading
 import time
-from typing import Callable, Dict, Iterable, List, Optional, Tuple, Union
+from typing import Any, Callable, Dict, Iterable, List, Optional, Tuple, Union
 
 import torch
 
@@ -23,10 +23,11 @@ from lmcache_b200.codec import NATIVE_DTYPES, KvView, PinnedBuffer, paged_layout
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.logging import init_logger
 from lmcache_b200.storage_backend import CreateStorageBackend
-from lmcache_b200.pipeline import HeadWindow, LayerwiseUpload, join_uploads
+from lmcache_b200.pipeline import (HeadWindow, LayerwiseUpload, SegmentsEncode, arena_of, begin_runs, join_uploads,
+                                   layerwise_store_budget_default)
 from lmcache_b200.reshard import first_source_rank, source_shards
-from lmcache_b200.rope import (RopeSpec, Rotation, derived_digest, hash_input, pack_rope, plan_segment_store,
-                                plan_segments, rope_shift, rope_table, seg_of_tok, skip_chunks)
+from lmcache_b200.rope import (RopeSpec, Rotation, StagedGather, derived_digest, hash_input, pack_rope,
+                                plan_segment_store, plan_segments, rope_shift, rope_table, seg_of_tok, skip_chunks)
 from lmcache_b200.utils import CacheEngineKey, KVCache, _lmcache_nvtx_annotate
 
 logger = init_logger(__name__)
@@ -273,6 +274,7 @@ class LMCacheEngine:
             self._check_mla_config(config, metadata)
         self.engine_ = CreateStorageBackend(config, metadata)
         self._reshard_counts: Dict[int, Dict[str, int]] = {}
+        self._seg_stream: Optional[torch.cuda.Stream] = None    # the layer-wise segment store's gathers
         logger.debug(f"Current storage backend type {type(self.engine_)}")
 
     @staticmethod
@@ -882,6 +884,12 @@ class LMCacheEngine:
         return self._begin_layerwise(tokens, lambda: KvView.from_paged(kv_caches, slot_mapping.cuda()), "vllm",
                                      len(kv_caches), skip_existing, fallback)
 
+    def _in_place(self, kv_tensors_raw: KVCache) -> bool:
+        """do all of store()'s tensors share layer 0's strides, with a contiguous last dimension (KvView.from_tuple
+        reads them in place)?"""
+        k0 = self._first(kv_tensors_raw)
+        return all(t.stride() == k0.stride() and t.stride(-1) == 1 for t in self._tensors(kv_tensors_raw))
+
     @torch.no_grad()
     def store_layerwise(self, tokens: torch.Tensor, kv_tensors_raw: KVCache, skip_existing=True) -> LayerwiseStore:
         """store(), with the KV handed over one layer at a time (see store_paged_layerwise): kv_tensors_raw is store()'s
@@ -895,8 +903,7 @@ class LMCacheEngine:
         k0 = self._first(kv_tensors_raw)
         # the kernels must read the caller's tensors in place (KvView.from_tuple would copy tensors of other strides
         # now, before they are written): anything else takes the ordinary store at finish()
-        in_place = all(t.stride() == k0.stride() and t.stride(-1) == 1 for t in self._tensors(kv_tensors_raw))
-        if not k0.is_cuda or not in_place or not self._layerwise_store_ok(k0.dtype):
+        if not k0.is_cuda or not self._in_place(kv_tensors_raw) or not self._layerwise_store_ok(k0.dtype):
             return LayerwiseStore(len(kv_tensors_raw), None, fallback)
         return self._begin_layerwise(tokens, lambda: KvView.from_tuple(kv_tensors_raw, fmt), fmt, len(kv_tensors_raw),
                                      skip_existing, fallback)
@@ -1208,24 +1215,29 @@ class LMCacheEngine:
         return LayerwiseRetrieval(ret_mask, self._blob_to_tuple_kv(blob), L, upload)
 
     # ------------------------------------------------------------------ segment store
-    def _store_segments(self, tokens: torch.Tensor, segments, rope: RopeSpec, fmt: str, first: torch.Tensor, D: int,
-                        view_fn: Callable[[], KvView], prefix_store: Callable[[int], None], skip_existing: bool,
-                        blocking: bool) -> None:
-        """Every segment store: the refusals, then a segment at 0 through prefix_store(end), then every other segment's
-        skip scan, one table and one b200kv_pack_chunks_rope launch into one staging blob, and one put per segment
-        under its derived keys."""
+    def _segment_store_check(self, tokens: torch.Tensor, segments, rope: RopeSpec, first: torch.Tensor, D: int):
+        """the plan and the refusals every segment store makes before it hashes or stores anything"""
         plans = self._segments_prologue(tokens, segments, rope)
         self._check_rope_dtype(first.dtype)
         rope.check(D)
+        return plans
+
+    def _segment_store_plan(self, tokens: torch.Tensor, plans, fmt: str, prefix_store: Callable[[int], Any],
+                            skip_existing: bool):
+        """Every segment store after its refusals: a segment at 0 through prefix_store(end), then every other segment's
+        hash chain, skip scan (with the touches of the chains it hit) and staging plan (plan_segment_store).  Returns
+        (prefix_store's result, or None without a segment at 0; the digests of the segments inside the prompt; runs,
+        rows, seg_of_tok and shifts of plan_segment_store)."""
         cs = self.chunk_size
         # the segments inside the prompt, planned again: their hash input and chain offsets leave out a segment at 0
         inner = plan_segments(len(tokens), [(p.start, p.end) for p in plans if p.start > 0], cs)
+        head = None
         for p in plans:
             if p.start == 0:
                 # exactly a prefill of tokens[:end]: its ordinary prefix keys, unrotated
-                prefix_store(p.end)
+                head = prefix_store(p.end)
         if not inner:
-            return
+            return head, [], [], [], [], []
         hashes = self._segment_hashes(tokens, inner)
         hits = []
         for p, hs in zip(inner, hashes):
@@ -1236,9 +1248,19 @@ class LMCacheEngine:
             ph, dh = skip_chunks(p.n_chunks, has(self._make_key), has(self._derived_key))
             self._touch_chain(hs, ph, ph + dh, fmt)
             hits.append((ph, dh))
-        runs, rows, sot, shifts = plan_segment_store(inner, hits, cs)
+        return (head, hashes) + tuple(plan_segment_store(inner, hits, cs))
+
+    def _store_segments(self, tokens: torch.Tensor, segments, rope: RopeSpec, fmt: str, first: torch.Tensor, D: int,
+                        view_fn: Callable[[], KvView], prefix_store: Callable[[int], None], skip_existing: bool,
+                        blocking: bool) -> None:
+        """Every segment store: the refusals, then a segment at 0 through prefix_store(end), then every other segment's
+        skip scan, one table and one b200kv_pack_chunks_rope launch into one staging blob, and one put per segment
+        under its derived keys."""
+        plans = self._segment_store_check(tokens, segments, rope, first, D)
+        _, hashes, runs, rows, sot, shifts = self._segment_store_plan(tokens, plans, fmt, prefix_store, skip_existing)
         if not runs:
             return
+        cs = self.chunk_size
         view = view_fn()
         self._geom = (view.L, view.H, view.D, view.dtype)
         dev = view.device
@@ -1295,16 +1317,124 @@ class LMCacheEngine:
         fmt = self.metadata.fmt
         self._check_store_args(tokens, kv_tensors_raw, fmt)
         first = self._first(kv_tensors_raw)
-        tdim = KvView.token_dim(fmt) - 2         # a layer's token dimension (a latent's: 0)
-
-        def head(end):
-            if self._mla:
-                return tuple(t[:end] for t in kv_tensors_raw)
-            return tuple((k.narrow(tdim, 0, end), v.narrow(tdim, 0, end)) for k, v in kv_tensors_raw)
         self._store_segments(
             tokens, segments, rope, fmt, first, first.shape[-1],
             lambda: KvView.from_tuple(self._as_cuda_kv(kv_tensors_raw), fmt),
-            lambda end: self.store(tokens[:end], head(end), skip_existing, blocking), skip_existing, blocking)
+            lambda end: self.store(tokens[:end], self._kv_head(kv_tensors_raw, end, fmt), skip_existing, blocking),
+            skip_existing, blocking)
+
+    def _kv_head(self, kv_tensors_raw: KVCache, end: int, fmt: str) -> KVCache:
+        """the first `end` tokens of store()'s KV, as views"""
+        if self._mla:
+            return tuple(t[:end] for t in kv_tensors_raw)
+        tdim = KvView.token_dim(fmt) - 2         # a layer's token dimension
+        return tuple((k.narrow(tdim, 0, end), v.narrow(tdim, 0, end)) for k, v in kv_tensors_raw)
+
+    # ------------------------------------------------------------------ layer-wise segment store
+    def _seg_side_stream(self, device) -> torch.cuda.Stream:
+        """the engine's side stream of the layer-wise segment store's gathers on `device`"""
+        s = self._seg_stream
+        if s is None or s.device != torch.device(device):
+            s = self._seg_stream = torch.cuda.Stream(device=device)
+        return s
+
+    def _store_segments_layerwise(self, tokens: torch.Tensor, segments, rope: RopeSpec, fmt: str, first: torch.Tensor,
+                                  D: int, num_layers: int, ok: bool, view_fn: Callable[[], KvView],
+                                  prefix_store: Callable[[int], LayerwiseStore], fallback: Callable,
+                                  skip_existing: bool) -> LayerwiseStore:
+        """Every layer-wise segment store.  At the call: the whole form's refusals; where the store cannot go layer by
+        layer (not `ok`), a handle that runs the whole form at finish(); otherwise the whole form's plan, with the
+        segment at 0 through prefix_store(end) (a layer-wise store handle), the staging (rope.StagedGather) and one
+        tier handle per run (pipeline.begin_runs).  finish() then finishes the segment at 0 (its touches and put) and
+        makes one put and one chain touch per run, in the whole form's order."""
+        plans = self._segment_store_check(tokens, segments, rope, first, D)
+        if not ok:
+            return LayerwiseStore(num_layers, None, fallback)
+        head, hashes, runs, _, _, shifts = self._segment_store_plan(tokens, plans, fmt, prefix_store, skip_existing)
+        cs = self.chunk_size
+        handles, gather = [], None
+        if runs:
+            try:
+                view = view_fn()
+                self._geom = (view.L, view.H, view.D, view.dtype)
+                gather = StagedGather(view, runs, shifts, fmt, self._mla, rope, self._seg_side_stream(view.device),
+                                      KvView.blob_shape)
+                # one budget for the whole store: the segment at 0's encode takes its arena first
+                budget = layerwise_store_budget_default() - (0 if head is None else arena_of(head._enc))
+                handles = begin_runs(self.engine_.begin_layerwise_store,
+                                     [KvView.from_blob(b, fmt) for b in gather.blobs], cs, budget)
+            except BaseException:
+                if head is not None:
+                    head.close()
+                raise
+            if handles is None:
+                # the tier writes no layer-wise containers for these chunks: the whole form runs at finish()
+                if head is not None:
+                    head.close()
+                return LayerwiseStore(num_layers, None, fallback)
+
+        def publish(stream, enc):
+            if enc is None:                     # closed before finish(): nothing is stored
+                return
+            if enc.head is not None:
+                enc.head.finish(stream)
+            blocking = bool(getattr(self.engine_, "layerwise_store_blocking", False))
+            for r, h in zip(runs, enc.handles):
+                hs = hashes[r.plan.index]
+                self.engine_.put_kv_chunks(self._derived_keys(hs[r.first:], fmt), None, 0, cs, blocking=blocking,
+                                           encoded=h)
+                self._touch_chain(hs, r.prefix_hits, len(hs), fmt)
+        return LayerwiseStore(num_layers, SegmentsEncode(head, handles, gather), publish)
+
+    @torch.no_grad()
+    def store_paged_segments_layerwise(self, tokens: torch.Tensor, kv_caches, slot_mapping: torch.Tensor, segments,
+                                       rope: RopeSpec, skip_existing=True) -> LayerwiseStore:
+        """store_paged_segments(), with the KV handed over one layer at a time (LayerwiseStore: save_layer(l, stream)
+        once layer l is written, finish(stream) after the last): the caches may still be unwritten when this is called.
+        The refusals, the hash chain, the skip scan with its touches and the staging plan are made here; a segment at 0
+        is store_paged_layerwise(tokens[:end], kv_caches, slot_mapping[:end], skip_existing).  Each save_layer(l)
+        gathers layer l of every other segment, its keys turned by -start, into its own staged chunk blob with one
+        b200kv_pack_chunks_layers_rope launch on the engine's side stream, and each segment's tier handle encodes (or,
+        on the raw tiers, packs) it behind that launch.  LMCACHE_B200_LAYERWISE_STORE_MB bounds the encode arenas of the
+        whole store (pipeline.begin_runs).  After finish() the tier holds the keys and bytes store_paged_segments
+        stores.  Where store_paged_layerwise cannot go layer by layer (a torch-serde remote tier, a chunk size over the
+        tier's layerwise_max_tokens) finish() runs store_paged_segments; a split (PagedAttention) cache needs no such
+        fallback, since the encoders read the staged blobs."""
+        self._check_paged_args(tokens, slot_mapping, kv_caches)
+        first = self._first(kv_caches)
+        D = first.shape[-1] if self._mla else paged_layout(*kv_caches[0]).D
+
+        def fallback(stream, enc):
+            with torch.cuda.stream(stream):
+                self.store_paged_segments(tokens, kv_caches, slot_mapping, segments, rope, skip_existing)
+        slots = slot_mapping.to(first.device)
+        return self._store_segments_layerwise(
+            tokens, segments, rope, "vllm", first, D, len(kv_caches), self._layerwise_store_ok(first.dtype),
+            lambda: KvView.from_paged(kv_caches, slots),
+            lambda end: self.store_paged_layerwise(tokens[:end], kv_caches, slot_mapping[:end], skip_existing),
+            fallback, skip_existing)
+
+    @torch.no_grad()
+    def store_segments_layerwise(self, tokens: torch.Tensor, kv_tensors_raw: KVCache, segments, rope: RopeSpec,
+                                 skip_existing=True) -> LayerwiseStore:
+        """store_segments(), with the KV handed over one layer at a time (see store_paged_segments_layerwise):
+        kv_tensors_raw is store()'s per-layer (K, V) tuple (or an MLA engine's latent per layer) on the GPU, possibly not
+        yet written.  A segment at 0 is store_layerwise(tokens[:end], the KV's first end tokens).  KV that is not on the
+        GPU or not laid out for the kernels to read in place (store_layerwise's rule) is stored by store_segments at
+        finish()."""
+        fmt = self.metadata.fmt
+        self._check_store_args(tokens, kv_tensors_raw, fmt)
+        first = self._first(kv_tensors_raw)
+
+        def fallback(stream, enc):
+            with torch.cuda.stream(stream):
+                self.store_segments(tokens, kv_tensors_raw, segments, rope, skip_existing)
+        ok = first.is_cuda and self._in_place(kv_tensors_raw) and self._layerwise_store_ok(first.dtype)
+        return self._store_segments_layerwise(
+            tokens, segments, rope, fmt, first, first.shape[-1], len(kv_tensors_raw), ok,
+            lambda: KvView.from_tuple(kv_tensors_raw, fmt),
+            lambda end: self.store_layerwise(tokens[:end], self._kv_head(kv_tensors_raw, end, fmt), skip_existing),
+            fallback, skip_existing)
 
     def close(self):
         self.engine_.close()

@@ -587,6 +587,175 @@ static void launch_unpack_rope(bool vec, bool split, unsigned blocks, const Unpa
     }
 }
 
+// b200kv_pack_chunks_layers_rope: the pack direction of unpack_rope_kernel, with its parameters (dst_tok is the view
+// token of chunk j's first token, here the source).  Chunk j's tokens [view_tok, view_tok + chunk_ntok[j]) of layers
+// [l0, l0 + nl) land in chunk_ptrs[j] in b200kv_pack_chunks_layers' layout; a key unit turns its own VEC channels by
+// row chunk_seg[j], reading its partner from the SOURCE (never written) with rope_turn_one, as rope_turn_vec does: the
+// bits of b200kv_pack_chunks_layers followed by b200kv_rope_shift_layers of the packed chunk.  Rows: the source row of
+// (token, head) is contiguous, so rope_turn_vec reads the partner itself.  SPLIT (B200KV_KV_PAGED_SPLIT, VEC = x): a
+// key vector is x channels of one token, read whole, and its neox partner is the vector of the partner channels of
+// that token; a value vector is gathered element by element along the block's channel rows.  No shared-memory tile.
+// A misaligned chunk pointer takes the vector from the source and stores it element by element.
+template <class E, int VEC, bool SPLIT>
+__global__ void __launch_bounds__(256) pack_rope_kernel(UnpackRopeParams P) {
+    using vec_t = typename std::conditional<VEC * sizeof(E) == 16, uint4, E>::type;
+    constexpr int X = 16 / (int)sizeof(E);
+    const int NL = P.ppl * P.nl;
+    const int vph = P.D / VEC;
+    const int64_t vpt = (int64_t)P.H * vph;
+    const int64_t per_plane = (int64_t)P.chunk_tokens * vpt;
+    const int64_t per_chunk = (int64_t)NL * per_plane;
+    const int64_t total = (int64_t)P.n_chunks * per_chunk;
+    for (int64_t u = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; u < total; u += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t j = u / per_chunk;
+        int64_t r = u - j * per_chunk;
+        const int lk = (int)(r / per_plane);
+        r -= (int64_t)lk * per_plane;
+        const int tok = (int)(r / vpt);
+        const int t = __ldg(P.chunk_ntok + j);
+        if (tok >= t) continue;
+        r -= (int64_t)tok * vpt;
+        const int h = (int)(r / vph);
+        const int v = (int)(r - (int64_t)h * vph);
+        const int l = P.l0 + (P.ppl == 2 ? lk >> 1 : lk), kv = P.ppl == 2 ? lk & 1 : 0;
+        const E* plane = reinterpret_cast<const E*>(P.pt.p[kv * P.L + l]);
+        int64_t row = __ldg(P.dst_tok + j) + tok;
+        if (P.slot_map) row = __ldg(P.slot_map + row);
+        uint8_t* base = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(P.chunk_ptrs) + j));
+        const int64_t head_row = P.hf_layout ? (((int64_t)lk * P.H + h) * t + tok) * P.D
+                                             : (((int64_t)lk * t + tok) * P.H + h) * P.D;
+        const int seg = kv == 0 ? __ldg(P.chunk_seg + j) : -1;
+        const float2* tab = P.cs + (int64_t)(seg < 0 ? 0 : seg) * P.half;
+        const int d0 = v * VEC;
+        union { vec_t q; E e[VEC]; } w;
+        if (SPLIT) {
+            const int64_t b = row / P.bs, so = row - b * P.bs;
+            // element d of this token's key head: [nb, H, D/x, bs, x]
+            const E* key = plane + (b * P.H + h) * (int64_t)P.D * P.bs + so * X;
+            if (kv == 0) {
+                if (VEC == X) w.q = *reinterpret_cast<const vec_t*>(key + (int64_t)(d0 / X) * P.bs * X);
+                else w.e[0] = key[(int64_t)(d0 / X) * P.bs * X + d0 % X];
+                const int c = d0 - P.rot_offset;
+                if (seg >= 0 && c >= 0 && c < 2 * P.half) {
+                    E p[VEC];
+                    if (VEC > 1 && !P.neox) {
+#pragma unroll
+                        for (int k = 0; k < VEC; ++k) p[k] = w.e[k ^ 1];
+                    } else {
+                        const int pd = P.rot_offset + rope_partner(c, P.half, P.neox != 0);
+                        union { vec_t q; E e[VEC]; } pu;
+                        if (VEC == X) pu.q = *reinterpret_cast<const vec_t*>(key + (int64_t)(pd / X) * P.bs * X);
+                        else pu.e[0] = key[(int64_t)(pd / X) * P.bs * X + pd % X];
+#pragma unroll
+                        for (int k = 0; k < VEC; ++k) p[k] = pu.e[k];
+                    }
+#pragma unroll
+                    for (int k = 0; k < VEC; ++k) w.e[k] = rope_turn_one(w.e[k], p[k], c + k, tab, P.half, P.neox != 0);
+                }
+            } else {
+#pragma unroll
+                for (int e = 0; e < VEC; ++e) w.e[e] = plane[((b * P.H + h) * (int64_t)P.D + d0 + e) * P.bs + so];
+            }
+        } else {
+            const E* srow = plane + row * P.sT + (int64_t)h * P.sH;     // the source row of this (token, head)
+            w.q = *reinterpret_cast<const vec_t*>(srow + d0);
+            if (seg >= 0) rope_turn_vec<E, VEC>(w.e, srow, d0, tab, P.half, P.rot_offset, P.neox != 0);
+        }
+        E* cdst = reinterpret_cast<E*>(base) + head_row + d0;
+        if (VEC == 1 || (reinterpret_cast<uintptr_t>(base) & 15) == 0) {
+            *reinterpret_cast<vec_t*>(cdst) = w.q;
+        } else {                                   // a misaligned chunk: element by element
+#pragma unroll
+            for (int e = 0; e < VEC; ++e) cdst[e] = w.e[e];
+        }
+    }
+}
+
+template <class E>
+static void launch_pack_rope_layers(bool vec, bool split, unsigned blocks, const UnpackRopeParams& P, cudaStream_t st) {
+    constexpr int V = 16 / sizeof(E);
+    if (split) {
+        if (vec) pack_rope_kernel<E, V, true><<<blocks, 256, 0, st>>>(P);
+        else pack_rope_kernel<E, 1, true><<<blocks, 256, 0, st>>>(P);
+    } else {
+        if (vec) pack_rope_kernel<E, V, false><<<blocks, 256, 0, st>>>(P);
+        else pack_rope_kernel<E, 1, false><<<blocks, 256, 0, st>>>(P);
+    }
+}
+
+// b200kv_unpack_chunks_layers_rope (pack false) and b200kv_pack_chunks_layers_rope (pack true): the refusals, the
+// parameters and the launch rule, which are the same in both directions (kv: the destination, or the source)
+static int launch_chunks_rope(bool pack, const void* const* chunk_ptrs, int32_t n_chunks, int32_t chunk_tokens,
+                              const int32_t* chunk_ntok, const int64_t* view_tok, const int32_t* chunk_seg,
+                              int32_t hf_layout, int32_t layer_begin, int32_t layer_end, const b200kv_kv_desc* dst,
+                              const float* cos_sin, int32_t rotary_dim, int32_t offset, int32_t style, void* stream) {
+    B2_REQUIRE(dst != nullptr, "kv descriptor is NULL");
+    B2_REQUIRE(chunk_ptrs != nullptr && chunk_ntok != nullptr && view_tok != nullptr && chunk_seg != nullptr,
+               pack ? "chunk_ptrs, chunk_ntok, src_tok or chunk_seg is NULL"
+                    : "chunk_ptrs, chunk_ntok, dst_tok or chunk_seg is NULL");
+    B2_REQUIRE(cos_sin != nullptr, "cos_sin table is NULL");
+    B2_REQUIRE(style == 0 || style == 1, "style must be 0 (neox) or 1 (gptj)");
+    B2_REQUIRE(dst->L > 0 && 2 * dst->L <= B200KV_MAX_PLANES, "bad kv descriptor");
+    B2_REQUIRE(dst->H > 0 && dst->D > 0, "H/D must be positive");
+    B2_REQUIRE(0 <= layer_begin && layer_begin < layer_end && layer_end <= dst->L, "bad layer range");
+    B2_REQUIRE(n_chunks > 0 && chunk_tokens > 0, "bad chunking");
+    B2_REQUIRE(hf_layout == 0 || hf_layout == 1, "hf_layout must be 0 or 1");
+    const bool split = kv_split(dst);
+    const int dt = split ? kv_split_dtype(dst) : kv_dtype(dst);
+    B2_REQUIRE(dt == B200KV_DT_BF16 || dt == B200KV_DT_FP16,
+               pack ? "the rope pack takes 16-bit keys only: rotating a one-byte (FP8) key would round it again"
+                    : "the rope unpack takes 16-bit keys only: rotating a one-byte (FP8) key would round it again");
+    B2_REQUIRE(rotary_dim > 0 && rotary_dim % 2 == 0, "rotary_dim must be even and positive");
+    B2_REQUIRE(offset >= 0 && (int64_t)offset + rotary_dim <= dst->D, "offset + rotary_dim exceeds the head size D");
+    if (split) {
+        B2_REQUIRE(!(dst->dtype & B200KV_KV_LATENT), "a latent KV has no split layout (B200KV_KV_PAGED_SPLIT)");
+        B2_REQUIRE(hf_layout == 0, "a split paged KV (B200KV_KV_PAGED_SPLIT) moves to and from vllm chunks only (hf_layout 0)");
+        B2_REQUIRE(dst->slot_map != nullptr, "a split paged KV (B200KV_KV_PAGED_SPLIT) needs a slot_map");
+        B2_REQUIRE(dst->D % 8 == 0, "a split paged KV needs D % x == 0 (x = 16 / element size)");
+        B2_REQUIRE(dst->sT > 0 && dst->sT <= (1 << 20), "block size out of range");
+    }
+    UnpackRopeParams P;
+    b200kv_kv_desc rows = *dst;                // the planes' pointers, read through the rows' table builder
+    rows.dtype = dt | (dst->dtype & B200KV_KV_LATENT);
+    float bins[B200KV_MAX_PLANES];
+    for (int i = 0; i < B200KV_MAX_PLANES; ++i) bins[i] = 32.0f;
+    if (int rc = make_plane_table(&rows, bins, bins, &P.pt)) return rc;
+    P.sT = dst->sT; P.sH = dst->sH;
+    P.slot_map = dst->slot_map;
+    P.chunk_ptrs = chunk_ptrs; P.chunk_ntok = chunk_ntok; P.dst_tok = view_tok; P.chunk_seg = chunk_seg;
+    P.cs = reinterpret_cast<const float2*>(cos_sin);
+    P.L = dst->L; P.H = dst->H; P.D = dst->D;
+    P.n_chunks = n_chunks; P.chunk_tokens = chunk_tokens; P.hf_layout = hf_layout;
+    P.ppl = split ? 2 : kv_ppl(dst);
+    P.l0 = layer_begin; P.nl = layer_end - layer_begin;
+    P.bs = split ? (int32_t)dst->sT : 0;
+    P.half = rotary_dim / 2; P.rot_offset = offset; P.neox = style == 0;
+    constexpr int ev = 8;                      // 16-bit elements per 16-byte vector
+    const RopeArgs rope{nullptr, cos_sin, rotary_dim, offset, style};
+    // chunk pointers are device data: the kernel checks each one's alignment itself
+    bool vec = dst->D % ev == 0 && rope.vec_ok(ev) && (split || (dst->sT % ev == 0 && dst->sH % ev == 0));
+    for (int kvi = 0; kvi < P.ppl && vec; ++kvi)
+        for (int l = layer_begin; l < layer_end && vec; ++l)
+            vec = (reinterpret_cast<uintptr_t>(P.pt.p[kvi * P.L + l]) & 15) == 0;
+    const int V = vec ? ev : 1;
+    const int64_t total = (int64_t)n_chunks * P.ppl * P.nl * chunk_tokens * dst->H * (dst->D / V);
+    int dev = 0, sms = 0;
+    B2_CHECK_CUDA(cudaGetDevice(&dev));
+    B2_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    int64_t blocks = std::min<int64_t>((total + 255) / 256, (int64_t)sms * 8 * 4);
+    if (blocks < 1) blocks = 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (pack) {
+        if (dt == B200KV_DT_BF16) launch_pack_rope_layers<__nv_bfloat16_raw>(vec, split, (unsigned)blocks, P, st);
+        else launch_pack_rope_layers<__half_raw>(vec, split, (unsigned)blocks, P, st);
+    } else {
+        if (dt == B200KV_DT_BF16) launch_unpack_rope<__nv_bfloat16_raw>(vec, split, (unsigned)blocks, P, st);
+        else launch_unpack_rope<__half_raw>(vec, split, (unsigned)blocks, P, st);
+    }
+    B2_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace b200kv
 
 using namespace b200kv;
@@ -649,64 +818,18 @@ int b200kv_unpack_chunks_layers_rope(const void* const* chunk_ptrs, int32_t n_ch
                                      int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
                                      const b200kv_kv_desc* dst, const float* cos_sin, int32_t rotary_dim, int32_t offset,
                                      int32_t style, void* stream) {
-    B2_REQUIRE(dst != nullptr, "kv descriptor is NULL");
-    B2_REQUIRE(chunk_ptrs != nullptr && chunk_ntok != nullptr && dst_tok != nullptr && chunk_seg != nullptr,
-               "chunk_ptrs, chunk_ntok, dst_tok or chunk_seg is NULL");
-    B2_REQUIRE(cos_sin != nullptr, "cos_sin table is NULL");
-    B2_REQUIRE(style == 0 || style == 1, "style must be 0 (neox) or 1 (gptj)");
-    B2_REQUIRE(dst->L > 0 && 2 * dst->L <= B200KV_MAX_PLANES, "bad kv descriptor");
-    B2_REQUIRE(dst->H > 0 && dst->D > 0, "H/D must be positive");
-    B2_REQUIRE(0 <= layer_begin && layer_begin < layer_end && layer_end <= dst->L, "bad layer range");
-    B2_REQUIRE(n_chunks > 0 && chunk_tokens > 0, "bad chunking");
-    B2_REQUIRE(hf_layout == 0 || hf_layout == 1, "hf_layout must be 0 or 1");
-    const bool split = kv_split(dst);
-    const int dt = split ? kv_split_dtype(dst) : kv_dtype(dst);
-    B2_REQUIRE(dt == B200KV_DT_BF16 || dt == B200KV_DT_FP16,
-               "the rope unpack takes 16-bit keys only: rotating a one-byte (FP8) key would round it again");
-    B2_REQUIRE(rotary_dim > 0 && rotary_dim % 2 == 0, "rotary_dim must be even and positive");
-    B2_REQUIRE(offset >= 0 && (int64_t)offset + rotary_dim <= dst->D, "offset + rotary_dim exceeds the head size D");
-    if (split) {
-        B2_REQUIRE(!(dst->dtype & B200KV_KV_LATENT), "a latent KV has no split layout (B200KV_KV_PAGED_SPLIT)");
-        B2_REQUIRE(hf_layout == 0, "a split paged KV (B200KV_KV_PAGED_SPLIT) moves to and from vllm chunks only (hf_layout 0)");
-        B2_REQUIRE(dst->slot_map != nullptr, "a split paged KV (B200KV_KV_PAGED_SPLIT) needs a slot_map");
-        B2_REQUIRE(dst->D % 8 == 0, "a split paged KV needs D % x == 0 (x = 16 / element size)");
-        B2_REQUIRE(dst->sT > 0 && dst->sT <= (1 << 20), "block size out of range");
-    }
-    UnpackRopeParams P;
-    b200kv_kv_desc rows = *dst;                // the planes' pointers, read through the rows' table builder
-    rows.dtype = dt | (dst->dtype & B200KV_KV_LATENT);
-    float bins[B200KV_MAX_PLANES];
-    for (int i = 0; i < B200KV_MAX_PLANES; ++i) bins[i] = 32.0f;
-    if (int rc = make_plane_table(&rows, bins, bins, &P.pt)) return rc;
-    P.sT = dst->sT; P.sH = dst->sH;
-    P.slot_map = dst->slot_map;
-    P.chunk_ptrs = chunk_ptrs; P.chunk_ntok = chunk_ntok; P.dst_tok = dst_tok; P.chunk_seg = chunk_seg;
-    P.cs = reinterpret_cast<const float2*>(cos_sin);
-    P.L = dst->L; P.H = dst->H; P.D = dst->D;
-    P.n_chunks = n_chunks; P.chunk_tokens = chunk_tokens; P.hf_layout = hf_layout;
-    P.ppl = split ? 2 : kv_ppl(dst);
-    P.l0 = layer_begin; P.nl = layer_end - layer_begin;
-    P.bs = split ? (int32_t)dst->sT : 0;
-    P.half = rotary_dim / 2; P.rot_offset = offset; P.neox = style == 0;
-    constexpr int ev = 8;                      // 16-bit elements per 16-byte vector
-    const RopeArgs rope{nullptr, cos_sin, rotary_dim, offset, style};
-    // chunk pointers are device data: the kernel checks each one's alignment itself
-    bool vec = dst->D % ev == 0 && rope.vec_ok(ev) && (split || (dst->sT % ev == 0 && dst->sH % ev == 0));
-    for (int kvi = 0; kvi < P.ppl && vec; ++kvi)
-        for (int l = layer_begin; l < layer_end && vec; ++l)
-            vec = (reinterpret_cast<uintptr_t>(P.pt.p[kvi * P.L + l]) & 15) == 0;
-    const int V = vec ? ev : 1;
-    const int64_t total = (int64_t)n_chunks * P.ppl * P.nl * chunk_tokens * dst->H * (dst->D / V);
-    int dev = 0, sms = 0;
-    B2_CHECK_CUDA(cudaGetDevice(&dev));
-    B2_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    int64_t blocks = std::min<int64_t>((total + 255) / 256, (int64_t)sms * 8 * 4);
-    if (blocks < 1) blocks = 1;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (dt == B200KV_DT_BF16) launch_unpack_rope<__nv_bfloat16_raw>(vec, split, (unsigned)blocks, P, st);
-    else launch_unpack_rope<__half_raw>(vec, split, (unsigned)blocks, P, st);
-    B2_CHECK_CUDA(cudaGetLastError());
-    return 0;
+    return launch_chunks_rope(false, chunk_ptrs, n_chunks, chunk_tokens, chunk_ntok, dst_tok, chunk_seg, hf_layout,
+                              layer_begin, layer_end, dst, cos_sin, rotary_dim, offset, style, stream);
+}
+
+int b200kv_pack_chunks_layers_rope(const b200kv_kv_desc* src, int32_t n_chunks, int32_t chunk_tokens,
+                                   const int32_t* chunk_ntok, const int64_t* src_tok, const int32_t* chunk_seg,
+                                   int32_t hf_layout, int32_t layer_begin, int32_t layer_end,
+                                   void* const* chunk_ptrs, const float* cos_sin, int32_t rotary_dim,
+                                   int32_t offset, int32_t style, void* stream) {
+    return launch_chunks_rope(true, const_cast<const void* const*>(chunk_ptrs), n_chunks, chunk_tokens, chunk_ntok,
+                              src_tok, chunk_seg, hf_layout, layer_begin, layer_end, src, cos_sin, rotary_dim, offset,
+                              style, stream);
 }
 
 int b200kv_pinned_alloc(void** host_ptr, int64_t bytes) {

@@ -513,6 +513,7 @@ class LayerwiseEncode:
                     budget or layerwise_store_budget_default())
         ws_bytes = codec.layerwise_workspace_bytes(L, H, D, chunk_size, n, latent)
         self.codec, self.pool, self.view, self.L, self.n_chunks = codec, pool, view, L, n
+        self.arena_bytes = arena            # the arena this store takes of its budget (begin_runs)
         self.slot = pool.acquire(arena, n * stride, ws_bytes, n, view.planes, codec.seg_row)
         s = self.slot
         s.n_chunks, s.P, s.seg_row, s.fixed_stride, s.coder = n, view.planes, codec.seg_row, stride, coder
@@ -635,6 +636,74 @@ class FanOutEncode:
     def abandon(self) -> None:
         for p in self.parts:
             p.abandon()
+
+    @property
+    def arena_bytes(self) -> int:
+        """each part got the same budget: the larger of the parts' arenas is what the store took of it"""
+        return max(arena_of(p) for p in self.parts)
+
+
+def arena_of(handle) -> int:
+    """the device arena a tier's layer-wise store handle took of its budget (0: a raw tier's, or NoEncode)"""
+    return int(getattr(handle, "arena_bytes", 0))
+
+
+def begin_runs(begin: Callable, views: Sequence, chunk_size: int, budget: int) -> Optional[list]:
+    """One layer-wise store handle per run of a layer-wise segment store: begin(view, 0, chunk_size, budget=...) (a
+    tier's begin_layerwise_store) of each run's staged blob, in plan order.  `budget` (LMCACHE_B200_LAYERWISE_STORE_MB)
+    bounds the store as a whole: each run gets what the runs before it left, so the arenas do not grow with the number
+    of segments, and a run that finds too little keeps the prefix of its chunks that fits (the others become misses, as
+    past the budget of one layer-wise store).  None, with every handle made so far abandoned, when the tier takes no
+    layer-wise store for these views."""
+    handles = []
+    left = budget
+    try:
+        for v in views:
+            h = begin(v, 0, chunk_size, budget=max(1, left))
+            if h is None:
+                for x in handles:
+                    x.abandon()
+                return None
+            handles.append(h)
+            left -= arena_of(h)
+    except BaseException:
+        for x in handles:
+            x.abandon()
+        raise
+    return handles
+
+
+class SegmentsEncode:
+    """The encode a layer-wise segment store's LayerwiseStore drives: `head`, the LayerwiseStore of a segment at token
+    0 (store_paged_layerwise / store_layerwise of tokens[:end]) or None; `handles`, one tier handle per run (begin_runs),
+    fed from `gather` (rope.StagedGather; None without runs).  encode_layer(l, stream) forwards save_layer to the head,
+    then gathers layer l of every run on the gather's side stream and enqueues each run's encode of it behind that
+    gather; finish() finishes every run's handle and returns an event after them and every gather (the head is
+    finished by the engine's publish step, which also puts it); abandon() drops every part."""
+
+    def __init__(self, head, handles: Sequence, gather):
+        self.head, self.handles, self.gather = head, list(handles), gather
+
+    def encode_layer(self, layer: int, stream, ready=None) -> None:
+        if self.head is not None:
+            self.head.save_layer(layer, stream)
+        if self.handles:
+            done = self.gather.layer(layer, stream)
+            for h in self.handles:
+                h.encode_layer(layer, self.gather.side, ready=done)
+
+    def finish(self):
+        if not self.handles:
+            return torch.cuda.Event()           # never recorded: waiting on it waits for nothing
+        return self.gather.join([h.finish() for h in self.handles])
+
+    def abandon(self) -> None:
+        head, self.head = self.head, None
+        handles, self.handles = self.handles, []
+        if head is not None:
+            head.close()
+        for h in handles:
+            h.abandon()
 
 
 def segment_copy_ranges(seg: np.ndarray, layouts: Sequence[SegmentLayout]):

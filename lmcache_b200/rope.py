@@ -315,3 +315,89 @@ def plan_segment_store(plans: Sequence[SegmentPlan], hits: Sequence[Tuple[int, i
         sot.extend([len(shifts)] * n)
         shifts.append(-p.start)
     return runs, rows, sot, shifts
+
+
+# ---------------------------------------------------------------------------------------------- layer-wise segment store
+def store_run_arrays(runs: Sequence[StoreRun]) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """The per-chunk arguments of b200kv_pack_chunks_layers_rope for a layer-wise segment store, in which each run of
+    plan_segment_store is one chunk of its n_tok tokens from request token `begin`, turned by its table row:
+    (chunk_ntok int32, src_tok int64, chunk_seg int32)."""
+    return (np.array([r.n_tok for r in runs], dtype=np.int32), np.array([r.begin for r in runs], dtype=np.int64),
+            np.array([r.row for r in runs], dtype=np.int32))
+
+
+def staging_layout(runs: Sequence[StoreRun], shape_of: Callable[[int], Tuple[int, ...]],
+                   layer_elems: Callable[[int], int], L: int) -> Tuple[List[Tuple[int, ...]], List[int], np.ndarray]:
+    """Where a layer-wise segment store stages its runs: each run's own chunk blob (shape_of(n_tok)) back to back in
+    one allocation.  Returns (the blob shapes, each blob's element offset, int64 [L, runs] the element offset of layer l
+    of each run's blob -- the chunk_ptrs of layer l, in elements).  layer_elems(t): elements of one layer of a blob of
+    t tokens."""
+    shapes = [tuple(shape_of(r.n_tok)) for r in runs]
+    sizes = [int(np.prod(s)) for s in shapes]
+    offs = [int(x) for x in np.concatenate([[0], np.cumsum(sizes, dtype=np.int64)[:-1]])] if runs else []
+    per = np.array([layer_elems(r.n_tok) for r in runs], dtype=np.int64)
+    layer_offs = np.array(offs, dtype=np.int64)[None, :] + np.arange(L, dtype=np.int64)[:, None] * per[None, :]
+    return shapes, offs, layer_offs
+
+
+def pack_rope_layers(view, ptrs_ptr: int, arrays, chunk_tokens: int, layer_begin: int, layer_end: int,
+                     table: torch.Tensor, rope: RopeSpec, stream: torch.cuda.Stream) -> None:
+    """one b200kv_pack_chunks_layers_rope launch on `stream`: chunk j's layer range goes to the device pointer
+    ptrs_ptr[j]; arrays: device (chunk_ntok, src_tok, chunk_seg) of store_run_arrays; table: rope_table's"""
+    ntok, src_tok, seg = arrays
+    N.check(N.lib().b200kv_pack_chunks_layers_rope(
+        ctypes.byref(view.desc), ntok.numel(), chunk_tokens, ctypes.c_void_p(ntok.data_ptr()),
+        ctypes.c_void_p(src_tok.data_ptr()), ctypes.c_void_p(seg.data_ptr()), int(view.fmt == "huggingface"),
+        layer_begin, layer_end, ctypes.c_void_p(ptrs_ptr), ctypes.c_void_p(table.data_ptr()), rope.rotary_dim,
+        rope.offset, STYLES[rope.style], stream.cuda_stream), "pack_chunks_layers_rope")
+
+
+class StagedGather:
+    """The staging of a layer-wise segment store.  One device allocation holds each run's own chunk blob
+    (KvView.blob_shape of its n_tok tokens) back to back -- the raw bytes of the tokens stored, as the whole form's one
+    staging blob.  layer(l, stream) makes the side stream wait for `stream` and fills layer l of every run's blob with
+    one b200kv_pack_chunks_layers_rope launch there, keys turned by -start; it returns the event after it.  Everything
+    the launches read is made on the current stream at construction, which the side stream waits for."""
+
+    def __init__(self, view, runs: Sequence[StoreRun], shifts: Sequence[int], fmt: str, latent: bool, rope: RopeSpec,
+                 side: torch.cuda.Stream, blob_shape: Callable):
+        dev = view.device
+        self.view, self.rope, self.side, self.R = view, rope, side, len(runs)
+        self.chunk_tokens = max(r.n_tok for r in runs)
+        L, H, D = view.L, view.H, view.D
+        per_tok = (1 if latent else 2) * H * D                # elements of one token of one layer
+        shapes, offs, layer_offs = staging_layout(runs, lambda t: blob_shape(fmt, L, H, D, t, latent),
+                                                  lambda t: per_tok * t, L)
+        es = view.dtype.itemsize
+        with torch.cuda.device(dev):
+            self.staging = torch.empty(offs[-1] + int(np.prod(shapes[-1])), dtype=view.dtype, device=dev)
+            self.blobs = [self.staging.narrow(0, o, int(np.prod(s))).view(s) for o, s in zip(offs, shapes)]
+            self.ptrs = torch.from_numpy(self.staging.data_ptr() + es * layer_offs).to(dev)
+            self.arrays = tuple(torch.from_numpy(a).to(dev) for a in store_run_arrays(runs))
+            self.table = rope_table(torch.tensor(list(shifts), dtype=torch.int64).to(dev), rope)
+            ready = torch.cuda.Event()
+            ready.record(torch.cuda.current_stream())
+        side.wait_event(ready)
+        view.record_stream(side)                             # the caller's KV outlives the last gather that reads it
+        for t in (self.staging, self.ptrs, self.table) + self.arrays:
+            t.record_stream(side)
+
+    def layer(self, layer: int, stream: torch.cuda.Stream) -> torch.cuda.Event:
+        with torch.cuda.device(self.view.device):
+            written = torch.cuda.Event()
+            written.record(stream)
+            self.side.wait_event(written)
+            pack_rope_layers(self.view, self.ptrs.data_ptr() + 8 * self.R * layer, self.arrays, self.chunk_tokens,
+                             layer, layer + 1, self.table, self.rope, self.side)
+            done = torch.cuda.Event()
+            done.record(self.side)
+        return done
+
+    def join(self, events: Sequence[torch.cuda.Event]) -> torch.cuda.Event:
+        """an event after `events` and every gather"""
+        with torch.cuda.device(self.view.device):
+            for ev in events:
+                self.side.wait_event(ev)
+            done = torch.cuda.Event()
+            done.record(self.side)
+        return done

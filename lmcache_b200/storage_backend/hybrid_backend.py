@@ -125,22 +125,23 @@ class LMCHybridBackend(LMCBackendInterface):
         part has landed them."""
         return True
 
-    def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int):
+    def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int, budget: Optional[int] = None):
         """A layer-wise store into both parts, or None when either part cannot take one (a torch-serde remote tier, a
         chunk size over a part's limit): the engine then stores both at finish().  When both parts keep the same
         containers it is one pipeline.LayerwiseEncode on the local tier's pool, whose slot put_kv_chunks lands into
-        both; otherwise a pipeline.FanOutEncode of the two parts' own handles."""
+        both; otherwise a pipeline.FanOutEncode of the two parts' own handles.  `budget` goes to both parts."""
         from lmcache_b200.pipeline import FanOutEncode
         begins = [getattr(s, "begin_layerwise_store", None) for s in (self.local_store, self.remote_store)]
         if None in begins:
             return None
+        kw = {} if budget is None else {"budget": budget}
         if self._shares_containers(chunk_size, view):
-            return begins[0](view, tok_begin, chunk_size)
-        local = begins[0](view, tok_begin, chunk_size)
+            return begins[0](view, tok_begin, chunk_size, **kw)
+        local = begins[0](view, tok_begin, chunk_size, **kw)
         if local is None:
             return None
         try:
-            remote = begins[1](view, tok_begin, chunk_size)
+            remote = begins[1](view, tok_begin, chunk_size, **kw)
         except BaseException:
             local.abandon()
             raise

@@ -313,9 +313,11 @@ class LMCLocalBackend(LMCBackendInterface):
         """the largest chunk a layer-major retrieve or a layer-wise store takes: raw blobs have no group limit"""
         return sys.maxsize
 
-    def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int) -> RawLayerwiseStore:
+    def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int,
+                              budget: Optional[int] = None) -> RawLayerwiseStore:
         """A layer-wise store of tokens [tok_begin, T) of `view`, whose KV may not be written yet (RawLayerwiseStore);
-        put_kv_chunks(..., encoded=it) publishes its blobs after finish()."""
+        put_kv_chunks(..., encoded=it) publishes its blobs after finish().  `budget` is ignored: raw blobs need no
+        encode arena."""
         return RawLayerwiseStore(self, view, tok_begin, chunk_size)
 
     def put_kv_chunks(self, keys, view, tok_begin: int, chunk_size: int, blocking: bool = True,
@@ -969,15 +971,16 @@ class LMCLocalCompressedBackend(LMCBackendInterface):
         return upload_decode_layerwise_runs(self.codec, self._layerwise_uploader(dst.device), recs, dst, chunk_size,
                                             on_done=lambda: self._unpin(pinned), rotation=rotation)
 
-    def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int):
+    def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int, budget: Optional[int] = None):
         """A pipeline.LayerwiseEncode of tokens [tok_begin, T) of `view` (whose KV may not be written yet), or None
         when this tier's containers for `chunk_size` are not ones a layer-wise encode writes: versions 3 and 4 (CacheGen,
-        chunks of at most 256 tokens), versions 5 and 6 (lossless, at most 4096)."""
+        chunks of at most 256 tokens), versions 5 and 6 (lossless, at most 4096).  `budget`: the cap of its arena
+        (default LMCACHE_B200_LAYERWISE_STORE_MB)."""
         from lmcache_b200.pipeline import LayerwiseEncode, layerwise_encodes, segment_pool_for
         if not layerwise_encodes(self.codec, chunk_size, view.latent):
             return None
         self._segments = segment_pool_for(self._segments, view.device)
-        return LayerwiseEncode(self.codec, self._segments, view, tok_begin, chunk_size)
+        return LayerwiseEncode(self.codec, self._segments, view, tok_begin, chunk_size, budget)
 
     def _layerwise_uploader(self, device):
         from lmcache_b200.pipeline import LayerwiseUploader

@@ -517,19 +517,19 @@ class LMCRemoteBackend(LMCBackendInterface):
         finish() finds the chunks."""
         return True
 
-    def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int):
+    def begin_layerwise_store(self, view, tok_begin: int, chunk_size: int, budget: Optional[int] = None):
         """A pipeline.LayerwiseEncode of tokens [tok_begin, T) of `view` (whose KV may not be written yet) on this tier's
         own SegmentPool; put_kv_chunks(..., encoded=it) lands and sends its containers.  None off the striped path (a
         serde without containers) and when the containers for `chunk_size` are not ones a layer-wise encode writes
         (pipeline.layerwise_encodes).  A latent KV's rank other than 0 gets a pipeline.NoEncode: it stores nothing, so
-        nothing is encoded."""
+        nothing is encoded.  `budget`: the cap of its arena (default LMCACHE_B200_LAYERWISE_STORE_MB)."""
         from lmcache_b200.pipeline import LayerwiseEncode, NoEncode, layerwise_encodes, segment_pool_for
         if not (self._striped() and layerwise_encodes(self.serializer.codec, chunk_size, view.latent)):
             return None
         if not self.puts:
             return NoEncode()
         self._segments = segment_pool_for(self._segments, view.device)
-        return LayerwiseEncode(self.serializer.codec, self._segments, view, tok_begin, chunk_size)
+        return LayerwiseEncode(self.serializer.codec, self._segments, view, tok_begin, chunk_size, budget)
 
     def _count(self, **kw) -> None:
         with self._stats_lock:
