@@ -1325,9 +1325,14 @@ __device__ __forceinline__ uint32_t rans_decode_stream(const uint8_t* cont, uint
     // `pk` points at this stream's entry 0.  Two table layouts (decode_kernel builds either):
     //   TR = false  rows of 33 words per stream (odd pitch: lanes that read the SAME entry never collide; lanes that read
     //               different entries sometimes do -- 2.7 extra wavefronts per warp-symbol at 0.6 bits/symbol, 7.4 at 4.1)
-    //   TR = true   transposed, entry i of every stream in one 512-byte row: a lane never leaves its own bank, at the
-    //               price of two more instructions per symbol for the LUT address and a two-step table build
-    // The host picks by the containers' measured bits per symbol (b200kv_decode_chunks).
+    //   TR = true   transposed, entry i of every stream in one 512-byte row: a lane never leaves its own bank.  A 16-symbol
+    //               table (NSTEPS = 4) fills rows 0..15 only, and rows 16..31 hold the LUT replicated down the columns
+    //               (row 16 + s = lut[s] in every column): the LUT value sits a constant 16 rows past the winning entry,
+    //               so it costs no address arithmetic.  A 32-symbol table computes lut_a + 4 * symbol from the
+    //               entry's address: two more instructions per symbol.
+    // 16-symbol planes always take the transposed table with the LUT replica (decode_kernel); for 32-symbol planes the
+    // host picks by the containers' measured bits per symbol (b200kv_decode_chunks).
+    constexpr bool kRep = TR && NSTEPS == 4;
     constexpr uint32_t kPitch = TR ? CT * 4u : 4u;
     constexpr uint32_t kIdx = TR ? CT : 1u;
     const uint32_t a0 = (uint32_t)__cvta_generic_to_shared(pk);
@@ -1336,14 +1341,16 @@ __device__ __forceinline__ uint32_t rans_decode_stream(const uint8_t* cont, uint
     const uint32_t lut_a = (uint32_t)__cvta_generic_to_shared(lut);            // TR: lut[s] = lut_a + ((a - a0) >> 7)
     const uint32_t lut_rel = lut_a - a0;                                       // !TR: lut[s] = a + lut_rel
     uint32_t off = 0u;                                                         // element offset of the current token row
-    // The integer ALU pipe (ISETP / SEL / PRMT / LOP3, one warp instruction per 2 cycles) is what bounds this loop, the
-    // FMA pipe idles: additions and shifts are therefore written as IMADs whose multiplier ptxas cannot fold (`one` is
-    // 1 but comes from a kernel parameter), which pins them to the FMA pipe.
-    const uint32_t c64k = one << 16, mone = 0u - one, two = one + one, c25 = one << 25;
+    // Two integer pipes share this loop's work: IMAD (FMA pipe) and ISETP / SEL / PRMT / LOP3 (ALU pipe), each one warp
+    // instruction per 2 cycles.  Some additions are written as IMADs whose multiplier ptxas cannot fold (`one` is 1 but
+    // comes from a kernel parameter), which pins them to the FMA pipe; the 16-bit shifts are PRMTs (ALU pipe) and the
+    // warp-uniform token offset a plain add (uniform datapath).  That split measured fastest on the H100 (DESIGN.md 3.4):
+    // with the shifts as IMADs too, the FMA pipe ran 66 of a 4-symbol trip's 151 instructions and bound the loop.
+    const uint32_t mone = 0u - one, two = one + one, c25 = one << 25;
     auto step = [&](float row_max, int i) {
         uint32_t key, xh;
-        asm("mad.lo.u32 %0, %1, %2, 65535;" : "=r"(key) : "r"(st.x), "r"(c64k));      // (x << 16) | 0xffff
-        asm("mul.hi.u32 %0, %1, %2;" : "=r"(xh) : "r"(st.x), "r"(c64k));             // x >> 16
+        asm("prmt.b32 %0, %1, %2, 0x1054;" : "=r"(key) : "r"(st.x), "r"(mone));         // (x << 16) | 0xffff
+        asm("prmt.b32 %0, %1, 0, 0x4432;" : "=r"(xh) : "r"(st.x));                      // x >> 16
         const bool p1 = r_mid <= key;
         uint32_t a = p1 ? a0h : a0;
         const uint32_t m = p1 ? r_hi : r_lo;
@@ -1355,12 +1362,16 @@ __device__ __forceinline__ uint32_t rans_decode_stream(const uint8_t* cont, uint
         uint32_t e, la;
         float lv;
         asm volatile("ld.shared.u32 %0, [%1];" : "=r"(e) : "r"(a));
-        if constexpr (TR) asm("mad.hi.u32 %0, %1, %2, %3;" : "=r"(la) : "r"(a - a0), "r"(c25), "r"(lut_a));   // lut_a + 4 * symbol
-        else la = a + lut_rel;
-        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(lv) : "r"(la));
+        if constexpr (kRep) {
+            asm volatile("ld.shared.f32 %0, [%1+%2];" : "=f"(lv) : "r"(a), "n"(16u * CT * 4u));   // the LUT replica
+        } else {
+            if constexpr (TR) asm("mad.hi.u32 %0, %1, %2, %3;" : "=r"(la) : "r"(a - a0), "r"(c25), "r"(lut_a));   // lut_a + 4 * symbol
+            else la = a + lut_rel;
+            asm volatile("ld.shared.f32 %0, [%1];" : "=f"(lv) : "r"(la));
+        }
         // x = freq * (x >> 16) + slot - start
         uint32_t dl;
-        asm("mul.hi.u32 %0, %1, %2;" : "=r"(dl) : "r"(key - e), "r"(c64k));
+        asm("prmt.b32 %0, %1, 0, 0x4432;" : "=r"(dl) : "r"(key - e));                 // (key - e) >> 16
         st.x = (e & 0xffffu) * xh + dl;
         // renormalisation, branch-free (a warp takes this path on most symbols, so a branch would run for all lanes
         // anyway): p = x < 2^16 -> pull the next halfword out of the window; q = p and the window's upper half was
@@ -1382,7 +1393,7 @@ __device__ __forceinline__ uint32_t rans_decode_stream(const uint8_t* cont, uint
             store_dequant<OUT_DT>(dst + __ldg(slots + i) * (int64_t)sT, 0u, lv, row_max, two);
         } else {
             store_dequant<OUT_DT>(dst, off, lv, row_max, two);
-            asm("mad.lo.u32 %0, %1, %2, %0;" : "+r"(off) : "r"(one), "r"(sT));
+            off += sT;
         }
     };
     int i = 0;
@@ -1448,6 +1459,9 @@ __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
     const uint16_t* cdf_src = reinterpret_cast<const uint16_t*>(dc.base + lo.off_cdf) + ((int64_t)nl * P.C + ct * CT) * kLp;
     const uint16_t* maxes = reinterpret_cast<const uint16_t*>(dc.base + lo.off_maxes) + (int64_t)nl * dc.t + tok0;
     const float cq = dec_maxq<GT>(P, nl);
+    // the rANS table layout of this plane (rans_decode_stream): 16-symbol planes always transposed, 32-symbol ones as
+    // the host chose
+    const bool trl = CODER == CODER_RANS && (TR || cq <= 7.0f);
     bool built = false;
     uint32_t hl = 0u;                        // version 3: bytes of stream header in front of the rANS state
     if constexpr (CODER == CODER_RANS) {
@@ -1543,7 +1557,7 @@ __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
                         uint32_t c1 = acc.value((uint32_t)i + 1u);
                         if (i == 31) c1 = 0x10000u;                              // cdf[32] wraps to 0 in 16 bits and means 65536
                         const uint32_t e = rans_table_entry(c0, c1);
-                        if (TR) tab[i * CT + tid] = e;
+                        if (trl) tab[i * CT + tid] = e;
                         else tab[tid * kLp + i] = e;
                         c0 = c1;
                     }
@@ -1556,7 +1570,7 @@ __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
         }
     }
     if (!built) {
-        if constexpr (CODER == CODER_RANS && TR) {
+        if (trl) {
             // TRANSPOSED table: entry i of stream tid at tab[i * CT + tid], entry = (cdf[i] << 16) | freq(i).  Built in two
             // steps through a staging copy of the raw CDF rows that lives in the table's own upper half (bytes 8448..16895):
             // coalesced global -> staging; every thread turns ITS row (33 halfwords, stride 33: conflict-free) into column
@@ -1619,9 +1633,16 @@ __global__ void __launch_bounds__(CT, 12) decode_kernel(DecParams P) {
     if constexpr (CODER == CODER_RANS) {
         uint32_t xf;
         const uint32_t one = min((uint32_t)P.n_chunks, 1u);      // 1, but opaque to the compiler (see rans_decode_stream)
-        const uint32_t* pk = TR ? tab + tid : tab + tid * kLp;
-        if (cq <= 7.0f) xf = rans_decode_stream<OUT_DT, 4, PAGED, TR>(dc.base, my_off + hl, pk, lut, mx, dst, (uint32_t)P.sT, gt, slots, one);
-        else xf = rans_decode_stream<OUT_DT, 5, PAGED, TR>(dc.base, my_off + hl, pk, lut, mx, dst, (uint32_t)P.sT, gt, slots, one);
+        const uint32_t* pk = trl ? tab + tid : tab + tid * kLp;
+        if (cq <= 7.0f) {
+            // the LUT replica in rows 16..31 of this thread's column, which only this thread reads (whatever the table
+            // build staged there is dead after the barrier above)
+#pragma unroll
+            for (int s = 0; s < 16; ++s) tab[(16 + s) * CT + tid] = __float_as_uint(lut[s]);
+            xf = rans_decode_stream<OUT_DT, 4, PAGED, true>(dc.base, my_off + hl, pk, lut, mx, dst, (uint32_t)P.sT, gt, slots, one);
+        } else {
+            xf = rans_decode_stream<OUT_DT, 5, PAGED, TR>(dc.base, my_off + hl, pk, lut, mx, dst, (uint32_t)P.sT, gt, slots, one);
+        }
         bad |= xf != kRansLow ? 1u : 0u;
     } else {
         if (cq <= 7.0f) decode_stream<OUT_DT, 4, PAGED>(dc.base, my_off, erow, lut, mx, dst, (uint32_t)P.sT, gt, slots);   // <= 16 bins: symbols 0..14
@@ -2230,7 +2251,8 @@ static int decode_plan_impl(const void* containers, int64_t containers_bytes, co
     const int64_t Gmax = (tmax + kGroup - 1) / kGroup;
     const int64_t tiles_max = Gmax * NP * P.tpp;
     B2_REQUIRE(tiles_max < (1ll << 31) && n_chunks <= 65535, "too many tiles / chunks in one call");
-    // table layout of the rANS decoder: the conflict-free (transposed) one pays off above ~3.6 payload bits per symbol
+    // table layout of the rANS decoder's 32-symbol planes (16-symbol planes always take the transposed table with its
+    // LUT replica, decode_kernel): the conflict-free (transposed) one pays off above ~3.6 payload bits per symbol
     // (measured: row-major is faster at 0.6 bits, transposed at 4.1 bits); the containers say how
     // many bits they hold.  B200KV_DECODE_TABLE=rows|transposed overrides (measurement knob).
     bool transposed = false;
