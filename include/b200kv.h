@@ -673,6 +673,39 @@ int b200kv_pack_chunks_rope(const b200kv_kv_desc* src, int64_t tok_begin, int32_
                             int32_t style, void* stream);
 
 /*
+ * CacheBlend's selective recomputation, the cache's side (lmcache_b200/csrc/blend.cu).  A reused document's KV at layers
+ * >= 1 was computed without attending to the tokens now in front of it; the model recomputes the reused tokens whose
+ * cached keys deviate most from fresh ones.  These calls measure the deviation and choose the tokens, identically on
+ * every tensor-parallel rank.  Added without changing anything that existed (b200kv_version() stays 4).
+ *
+ * b200kv_blend_deviation: fresh (DEVICE, n rows of fresh_row_stride elements, the first H*D of each used) holds the
+ * model's keys of one layer after the rotary embedding, in the cache's dtype; row i belongs to view token tok[i]
+ * (DEVICE int64 [n], through slot_map as in every other entry point).  dev[i] (DEVICE float [n]) gets
+ *     sum over h < H, d < D of (fresh[i][h*D + d] - key(layer, tok[i], h, d))^2
+ * in fp32, over the key plane of `layer` only (kv = 0; the one plane of a B200KV_KV_LATENT descriptor, all D channels).
+ * The summation order depends on (H, D) alone: channel c = h*D + d belongs to lane (c / 8) % 32, each lane accumulates
+ * its channels in ascending c with one fma per element, and the 32 lane sums are folded by an xor butterfly (16, 8, 4,
+ * 2, 1).  The same rows therefore give the same bits in every layout, at every n, row index, alignment and launch:
+ * ranks that sum their heads' dev get one total.  Every descriptor b200kv_rope_shift takes: blobs (vllm, huggingface),
+ * tuples, latent views, slot-mapped and block-strided rows, B200KV_KV_PAGED_SPLIT key blocks.  16-byte vectors when D,
+ * the strides, fresh_row_stride and the pointers allow it, element by element otherwise.  < 0, nothing enqueued: a
+ * one-byte dtype, NULL pointers with n > 0, a layer outside [0, L), fresh_row_stride < H*D.
+ *
+ * b200kv_blend_select: rows (DEVICE int64) gets every row i < n with cand[i] == 0 (DEVICE uint8 [n]) in ascending order,
+ * then, in ascending order, the min(k, n_cand) candidate rows (cand != 0) of largest dev (DEVICE float [n]): n_forced +
+ * min(k, n_cand) entries, a count the caller knows from cand.  Ties go to the lower row; NaN ranks as +inf (and -0 as
+ * +0), so a damaged row is recomputed.  Seven operations on `stream` whatever n (a 4 KB memset, four radix-histogram
+ * passes over the keys' bit patterns, a count pass and the compaction), no host sync, and no atomic whose order shows
+ * in the result.  workspace: DEVICE, 4-byte aligned, b200kv_blend_select_workspace_bytes(n) bytes; n < 2^31.  < 0,
+ * nothing enqueued: n or k negative, NULL pointers with n > 0, a small workspace.
+ */
+int b200kv_blend_deviation(const b200kv_kv_desc* kv, int32_t layer, int64_t n, const int64_t* tok, const void* fresh,
+                           int64_t fresh_row_stride, float* dev, void* stream);
+int64_t b200kv_blend_select_workspace_bytes(int64_t n);
+int b200kv_blend_select(const float* dev, const uint8_t* cand, int64_t n, int64_t k, int64_t* rows, void* workspace,
+                        int64_t workspace_bytes, void* stream);
+
+/*
  * GPU <-> pinned-host mover.  Replaces LMCLocalBackend.put_blocking/put_nonblocking/get
  * (local_backend.py:82-100,128-144: pageable tensor.to("cpu") / .to("cuda") + torch.cuda.synchronize()).
  */

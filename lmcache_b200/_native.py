@@ -170,7 +170,10 @@ SIGNATURES = {
                                          c_i32, c_vp]),
     "b200kv_pack_chunks_rope": (c_i32, [ctypes.POINTER(KvDesc), c_i64, c_i32, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp,
                                         c_vp, c_i32, c_i32, c_i32, c_vp]),
-    "b200kv_pinned_alloc": (c_i32, [ctypes.POINTER(c_vp), c_i64]),
+    "b200kv_blend_deviation": (c_i32, [ctypes.POINTER(KvDesc), c_i32, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp]),
+    "b200kv_blend_select_workspace_bytes": (c_i64, [c_i64]),
+    "b200kv_blend_select": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_i64, c_vp]),
+    "b200kv_pinned_alloc":(c_i32, [ctypes.POINTER(c_vp), c_i64]),
     "b200kv_pinned_free": (c_i32, [c_vp]),
     "b200kv_host_device_ptr": (c_i32, [c_vp, ctypes.POINTER(c_vp)]),
     "b200kv_copy_async": (c_i32, [c_vp, c_vp, c_i64, c_vp]),

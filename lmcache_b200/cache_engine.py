@@ -19,6 +19,7 @@ from typing import Any, Callable, Dict, Iterable, List, Optional, Tuple, Union
 import torch
 
 from lmcache_b200 import _native as N
+from lmcache_b200.blend import BlendPlan, BlendSpec, check_blend_args, check_blend_dtype
 from lmcache_b200.codec import NATIVE_DTYPES, KvView, PinnedBuffer, paged_layout
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.logging import init_logger
@@ -1435,6 +1436,38 @@ class LMCacheEngine:
             lambda: KvView.from_tuple(kv_tensors_raw, fmt),
             lambda end: self.store_layerwise(tokens[:end], self._kv_head(kv_tensors_raw, end, fmt), skip_existing),
             fallback, skip_existing)
+
+    # ------------------------------------------------------------------ CacheBlend's selective recomputation
+    def blend_paged(self, kv_caches, slot_mapping: torch.Tensor, ret_mask: torch.Tensor, spec: BlendSpec) -> BlendPlan:
+        """The plan of a blended prefill over the paged caches a (layer-wise) retrieve_paged_segments filled, in any
+        layout it takes (an MLA engine: its latent caches): which tokens the model recomputes at each layer and, at each
+        check layer of `spec`, the deviation of its fresh keys from the cached ones and the choice that follows
+        (BlendPlan.check).  ret_mask: the retrieve's.  TypeError for an FP8 cache; ValueError for a spec that is not a
+        BlendSpec or names a layer the caches do not have, and for a ret_mask of another length than slot_mapping.
+        Nothing is enqueued but the mask's upload."""
+        if self.metadata.fmt != "vllm":
+            raise ValueError(f"paged KV caches use the vllm layout, engine fmt is {self.metadata.fmt}")
+        self._check_kind(kv_caches, "kv_caches")
+        first = self._first(kv_caches)
+        check_blend_dtype(first.dtype)
+        check_blend_args(spec, len(kv_caches), slot_mapping.numel(), ret_mask)
+        slots = slot_mapping.to(first.device)
+        return BlendPlan(KvView.from_paged(kv_caches, slots), ret_mask, spec, slots)
+
+    def blend(self, kv: KVCache, ret_mask: torch.Tensor, spec: BlendSpec) -> BlendPlan:
+        """blend_paged for the dense per-layer views retrieve_segments / retrieve_segments_layerwise return (an MLA
+        engine: its [T, D] latents).  A dense caller writes the fresh K / V of rows_at(layer) into the views itself
+        (index_copy_ along the token dimension); BlendStep.slots is None.  The refusals are blend_paged's, and a kv of
+        no layers (a total miss) is a ValueError: there is nothing to blend."""
+        fmt = self.metadata.fmt
+        if not len(kv):
+            raise ValueError("blend needs the KV of a retrieve that hit: kv holds no layers")
+        self._check_kind(kv, "kv")
+        first = self._first(kv)
+        check_blend_dtype(first.dtype)
+        view = KvView.from_tuple(kv, fmt)
+        check_blend_args(spec, view.L, view.ntokens, ret_mask)
+        return BlendPlan(view, ret_mask, spec)
 
     def close(self):
         self.engine_.close()
