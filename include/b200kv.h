@@ -698,12 +698,30 @@ int b200kv_pack_chunks_rope(const b200kv_kv_desc* src, int64_t tok_begin, int32_
  * passes over the keys' bit patterns, a count pass and the compaction), no host sync, and no atomic whose order shows
  * in the result.  workspace: DEVICE, 4-byte aligned, b200kv_blend_select_workspace_bytes(n) bytes; n < 2^31.  < 0,
  * nothing enqueued: n or k negative, NULL pointers with n > 0, a small workspace.
+ *
+ * b200kv_blend_select_batch: b200kv_blend_select per segment of one array, for a prefill batch of B requests whose rows
+ * are concatenated.  Segment s covers rows [seg[s], seg[s+1]) (DEVICE int64 [B+1]; seg[0] = 0, seg[B] = n, not
+ * decreasing; empty segments are allowed) and selects k[s] (DEVICE int64 [B], >= 0) candidates.  rows gets one block
+ * per segment, in segment order: the segment's forced rows in ascending order, then its min(k[s], candidates of s)
+ * candidates of largest dev in ascending order, as global row indices.  Restricted to one segment the block is exactly
+ * b200kv_blend_select of that slice plus seg[s]: ties to the lower row, NaN as +inf, -0 as +0.  The same seven
+ * operations on `stream` whatever n, B and the spread of the rows over the segments (a memset of the histograms, four
+ * radix passes, a count pass and the compaction), no host sync, and no atomic whose order shows in the result.  seg
+ * and k are device data: their preconditions are the caller's, not checked.  workspace: DEVICE, 4-byte aligned,
+ * b200kv_blend_select_batch_workspace_bytes(n, B) bytes = 4176 bytes per segment (four 256-bin histograms and the
+ * radix state of each pass, the block's start and the segment's first-row counts) + 16 bytes per CTA of the row
+ * split (at most 1024 CTAs).  < 0, nothing enqueued: n outside [0, 2^31), B outside [1, 2^31), NULL pointers with
+ * n > 0, a small or misaligned workspace.
  */
 int b200kv_blend_deviation(const b200kv_kv_desc* kv, int32_t layer, int64_t n, const int64_t* tok, const void* fresh,
                            int64_t fresh_row_stride, float* dev, void* stream);
 int64_t b200kv_blend_select_workspace_bytes(int64_t n);
 int b200kv_blend_select(const float* dev, const uint8_t* cand, int64_t n, int64_t k, int64_t* rows, void* workspace,
                         int64_t workspace_bytes, void* stream);
+int64_t b200kv_blend_select_batch_workspace_bytes(int64_t n, int64_t B);
+int b200kv_blend_select_batch(const float* dev, const uint8_t* cand, int64_t n, int64_t B, const int64_t* seg,
+                              const int64_t* k, int64_t* rows, void* workspace, int64_t workspace_bytes,
+                              void* stream);
 
 /*
  * GPU <-> pinned-host mover.  Replaces LMCLocalBackend.put_blocking/put_nonblocking/get

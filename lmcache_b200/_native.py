@@ -173,6 +173,8 @@ SIGNATURES = {
     "b200kv_blend_deviation": (c_i32, [ctypes.POINTER(KvDesc), c_i32, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp]),
     "b200kv_blend_select_workspace_bytes": (c_i64, [c_i64]),
     "b200kv_blend_select": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_i64, c_vp]),
+    "b200kv_blend_select_batch_workspace_bytes": (c_i64, [c_i64, c_i64]),
+    "b200kv_blend_select_batch": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "b200kv_pinned_alloc":(c_i32, [ctypes.POINTER(c_vp), c_i64]),
     "b200kv_pinned_free": (c_i32, [c_vp]),
     "b200kv_host_device_ptr": (c_i32, [c_vp, ctypes.POINTER(c_vp)]),

@@ -14,12 +14,13 @@ from __future__ import annotations
 import ctypes
 import threading
 import time
-from typing import Any, Callable, Dict, Iterable, List, Optional, Tuple, Union
+from typing import Any, Callable, Dict, Iterable, List, Optional, Sequence, Tuple, Union
 
 import torch
 
 from lmcache_b200 import _native as N
-from lmcache_b200.blend import BlendPlan, BlendSpec, check_blend_args, check_blend_dtype
+from lmcache_b200.blend import (BatchBlendPlan, BlendPlan, BlendSpec, check_blend_args, check_blend_batch_args,
+                                 check_blend_dtype)
 from lmcache_b200.codec import NATIVE_DTYPES, KvView, PinnedBuffer, paged_layout
 from lmcache_b200.config import LMCacheEngineConfig, LMCacheEngineMetadata
 from lmcache_b200.logging import init_logger
@@ -1453,6 +1454,24 @@ class LMCacheEngine:
         check_blend_args(spec, len(kv_caches), slot_mapping.numel(), ret_mask)
         slots = slot_mapping.to(first.device)
         return BlendPlan(KvView.from_paged(kv_caches, slots), ret_mask, spec, slots)
+
+    def blend_paged_batch(self, kv_caches, slot_mapping: torch.Tensor, ret_masks: Sequence[torch.Tensor],
+                          spec: BlendSpec) -> BatchBlendPlan:
+        """blend_paged for a whole prefill batch: slot_mapping is the flattened batch's (as vLLM hands it to attention)
+        and ret_masks holds one mask per request, in batch order -- the ret_mask of its (layer-wise)
+        retrieve_paged_segments; a request that retrieved nothing (a decode step, a prompt whose documents all
+        missed) is all False and all its rows are computed.  Each request keeps its own budgets; every check is one
+        launch sequence for the whole batch (BatchBlendPlan.check).  The layouts and the refusals are blend_paged's,
+        and ret_masks that is not a non-empty list of 1-D bool CPU tensors whose lengths add up to slot_mapping's is
+        a ValueError.  Nothing is enqueued but the masks' upload."""
+        if self.metadata.fmt != "vllm":
+            raise ValueError(f"paged KV caches use the vllm layout, engine fmt is {self.metadata.fmt}")
+        self._check_kind(kv_caches, "kv_caches")
+        first = self._first(kv_caches)
+        check_blend_dtype(first.dtype)
+        check_blend_batch_args(spec, len(kv_caches), slot_mapping.numel(), ret_masks)
+        slots = slot_mapping.to(first.device)
+        return BatchBlendPlan(KvView.from_paged(kv_caches, slots), ret_masks, spec, slots)
 
     def blend(self, kv: KVCache, ret_mask: torch.Tensor, spec: BlendSpec) -> BlendPlan:
         """blend_paged for the dense per-layer views retrieve_segments / retrieve_segments_layerwise return (an MLA
